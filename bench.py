@@ -17,12 +17,13 @@ value : scans/s, queries already resident in HBM (device pointers), `--lanes` ha
         asynchronous submissions (consecutive batches overlap on the GPU).
 e2e   : scans/s through the same C-ABI call with pinned HOST buffers: poses + queries H2D and the folded keep
         mask of the map D2H inside the timed region, every step.
-roofline : the kernel with the largest CUDA-event time per step against the measured HBM peak, plus every kernel's own
+roofline : the kernel with the largest CUDA-event time per step against the HBM peak, plus every kernel's own
         line (`by_kernel`; K1 is the one that moves the path's bytes, R-GPF the latency-bound one).
 cpu_baseline : the oracle port (oracle/, restated reference path: fetch_VoI + ERASOR) on one host core, bounded sample.
 --impl reference : the same oracle port over all host cores (independent nodes in a process pool).
---config NAME : other BASELINE.json configs (dense twin, 50 M-point VoI, 40x360 x 256 k-point scans); their lines are
-        committed under profiles/r02/.  The driver's default stays on seq 05.
+--config NAME : other BASELINE.json configs (dense twin, 40x360 x 256 k-point scans).  The driver's default stays on seq 05.
+--dump-outputs DIR : after the timed steps, what the last step of the `value` path returned to its caller, as float32 .npy
+        files: the resident map's folded keep mask and the per-node counters (VoI points, flagged bins, rejected points).
 """
 import argparse
 import gc
@@ -39,7 +40,7 @@ if ROOT not in sys.path:
 import numpy as np  # noqa: E402
 
 FRAMES_PER_PASS = 20          # 161 nodes / removal_interval 8 (config/seq_05.yaml)
-N_QUERY_COPIES = 20           # resident arm: rotating query copies, 20 x 6.6 MB > 126 MB L2
+N_QUERY_COPIES = 20           # resident arm: rotating query copies, 20 x 6.6 MB > 50 MB L2
 CACHE_DIR = os.environ.get("ERASOR_B200_CACHE", "/tmp/erasor_b200_cache")
 
 CONFIGS = {
@@ -200,26 +201,6 @@ def offline_pass_block(p, map_world, device_index):
                       "every processed node's scan is handed to erasor_updater_prefetch_scan one node ahead (upload + voxelisation under the previous node's path)"}
 
 
-def ncu_dram_traffic():
-    """DRAM bytes per launch (read + write) of the node-mode step's kernels from the committed ncu capture of this workload."""
-    import csv
-    path = os.path.join(ROOT, "profiles", "r02", "ncu_nodes_raw.csv")
-    out = {}
-    try:
-        rows = list(csv.reader(open(path)))
-        hdr, units = rows[0], rows[1]
-        ik, ir, iw = hdr.index("Kernel Name"), hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-        scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        names = (("k1_rpod_bin", "k1_rpod_bin"), ("k2_srt_scatter", "k2_scatter"), ("k4_rgpf", "k4_rgpf_all_classes"))
-        for r in rows[2:]:
-            for pat, key in names:
-                if pat in r[ik]:
-                    out[key] = out.get(key, 0.0) + float(r[ir]) * scale.get(units[ir], 1.0) + float(r[iw]) * scale.get(units[iw], 1.0)
-    except Exception:
-        return {}
-    return {k: float(round(v)) for k, v in out.items()}
-
-
 def clocks_sampler_start(gpu_index: int):
     q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -359,7 +340,7 @@ def workload_config(config, p, n_map, n_voi, qs, world):
             "map_points": int(n_map), "mean_map_voi_points": int(np.mean(n_voi)) if len(n_voi) else 0,
             "mean_query_points": int(np.mean([len(q) for q in qs])),
             "in_bin_voxelize": "skipped on both arms (skip_voxelize=1): v3's per-bin VoxelGrid only changes the cloud outputs, not the masks",
-            "l2": f"resident arm: {N_QUERY_COPIES} rotating query copies (> 126 MB L2); the map is resident by design (uploaded once); "
+            "l2": f"resident arm: {N_QUERY_COPIES} rotating query copies (> 50 MB L2); the map is resident by design (uploaded once); "
                   "e2e arm: inputs come from host memory every step",
             "parallelism": f"frames sharded x{world} (strided: rank r takes nodes r, r + {world}, ...)"}
 
@@ -506,6 +487,10 @@ def run_ours(args):
 
     ms_res_1, launches_1, _ = timed_median("resident_one_lane", submit_resident, 1)
     ms_res, launches, per_rank_res = timed_median("resident", submit_resident, L)
+    if args.dump_outputs and rank == 0:
+        # what the value path's last timed step returned: the map's folded keep mask and that batch's per-node counters
+        last = lanes[(args.steps - 1) % L]
+        dumped = {"keep_mask": gmap.get_keep(), **dict(zip(("node_voi_points", "node_flagged_bins", "node_rejected_points"), last.node_stats()))}
     # --- e2e: host buffers through the same call ---
     ms_e2e_1, _, _ = timed_median("e2e_one_lane", submit_host, 1)
     ms_e2e, _, per_rank_e2e = timed_median("e2e", submit_host, L)
@@ -560,7 +545,7 @@ def run_ours(args):
         if os.path.exists(peaks_path):
             peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (burst copy)"
         else:
-            peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "fallback: H100 SXM data sheet, 3.35 TB/s HBM3"
         NV, n_f = int(n_voi.sum()), int(npts_flagged.sum())
         scans = F * world
         value = scans * args.steps / (ms_res * 1e-3)
@@ -577,12 +562,11 @@ def run_ours(args):
                          "share_of_event_timed_step": round(kernel_ms[k] / (ms_ev / args.steps), 3)} for k in kernel_ms}
         by_kernel["k1_rpod_bin"]["frac_voi_bytes"] = round(16.0 * (NV + NQ) / (kernel_ms["k1_rpod_bin"] * 1e-3) / 1e9 / peak, 4) if kernel_ms["k1_rpod_bin"] > 0 else 0.0
         by_kernel["k1_rpod_bin"]["note"] = ("fused fetch_VoI + R-POD: 16 B per map point scanned per frame (SURVEY 8d fused rule) + 16 B per query point; the resident map "
-                                            "(16 N_map bytes) stays in the 126 MB L2 across the frames of a step, so DRAM traffic is far BELOW these bytes and the kernel is issue-bound")
+                                            "(16 N_map bytes) stays in the 50 MB L2 across the frames of a step, so DRAM traffic is far BELOW these bytes and the kernel is issue-bound")
         dom = max(kernel_ms, key=lambda k: kernel_ms[k])
         step_bytes = 16.0 * (NV + NQ) + NV + 16.0 * n_f
         step_ms = ms_res / args.steps
         step_gbs = step_bytes / (step_ms * 1e-3) / 1e9
-        ncu_traffic = ncu_dram_traffic() if (args.config == "seq05" and F == FRAMES_PER_PASS) else {}
         line = {
             "metric": "LiDAR scans/sec through R-POD+SRT+R-GPF on KITTI-05 (synthetic twin)",
             "value": value, "unit": "scans/s", "n_gpus": world, "steps": args.steps, "warmup": W,
@@ -603,16 +587,13 @@ def run_ours(args):
                             f"the map itself was uploaded once before the steps ({map_upload_ms:.1f} ms for {16 * NG} bytes, load_global_map)"},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": dom, "achieved": by_kernel[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s",
-                         "frac": by_kernel[dom]["frac"], "traffic": ncu_traffic.get(dom),
+                         "frac": by_kernel[dom]["frac"],
                          "peak_source": peak_src, "algorithmic_bytes_per_launch": kbytes[dom], "avg_launch_ms": kernel_ms[dom],
                          "launches_timed": int(kt[dom][1]),
                          "why": "the dominant kernel by CUDA-event time (one lane, plain launches); by_kernel lists all of them: K1 moves the path's bytes "
                                 "and is issue-bound, R-GPF is bound by a serial float dependency chain per bin (exact-order covariance sums + Jacobi SVD, "
                                 "DESIGN.md section 5) and runs under the other kernels of overlapped submissions",
                          "hbm_kernel": "k1_rpod_bin", "by_kernel": by_kernel,
-                         "traffic_by_kernel": ncu_traffic,
-                         "traffic_source": "profiles/r02/ncu_nodes_raw.csv: dram__bytes_read.sum + dram__bytes_write.sum of one launch of each kernel on this "
-                                           "workload (ncu --set full; the 5.4 MB map is L2-resident, so K1's DRAM traffic is far below the bytes it scans)",
                          "ms_per_step_with_event_timing": ms_ev / args.steps},
             "pipeline": {"bytes_per_step": step_bytes, "flagged_bin_points_per_step": n_f, "flagged_bins_per_step": int(len(npts_flagged)),
                          "achieved": step_gbs, "unit": "GB/s", "frac_of_hbm_peak": step_gbs / peak,
@@ -639,10 +620,14 @@ def run_ours(args):
         if world == 1 and args.config == "seq05" and not args.no_sweep:
             try:
                 line["configs"] = {"3_seqs_00_01_02_07": sweep_presets(map_world, poses, qs, qo, dQ[0], gmap, local, args.steps),
-                                   "4_large_scale_50M_voi": "profiles/r02/config4_largescale.json (scripts/config4_largescale.py)",
-                                   "5_synthetic_40x360": "profiles/r02/config5_n*.json (bench.py --config synthetic40x360 --frames 32)"}
+                                   "4_large_scale_50M_voi": "scripts/config4_largescale.py",
+                                   "5_synthetic_40x360": "bench.py --config synthetic40x360 --frames 32"}
             except Exception as e:
                 line["configs"] = {"error": repr(e)}
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, a in dumped.items():
+                np.save(os.path.join(args.dump_outputs, f"{name}.npy"), a.astype(np.float32))
         print(json.dumps(line))
     for h in lanes:
         h.close()
@@ -697,6 +682,7 @@ def main():
     ap.add_argument("--config", default="seq05", choices=sorted(CONFIGS))
     ap.add_argument("--no-offline-pass", action="store_true", help="skip the informational sequential-pass block")
     ap.add_argument("--no-sweep", action="store_true", help="skip the config-3 preset sweep block")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)

@@ -1,12 +1,12 @@
 #!/bin/bash
-# build.sh -- compiles the product library for sm_100a (nvcc cross-compiles without a GPU).
+# build.sh -- compiles the product library for sm_90a (nvcc cross-compiles without a GPU).
 #   erasor_b200/_lib/liberasor_b200.so            the C-ABI library (include/erasor_b200.h)
 #   erasor_b200/_lib/liberasor_b200_hostcheck.so  host-only build of binning.h for the CPU test-suite
 set -euo pipefail
 cd "$(dirname "$0")"
 mkdir -p ../_lib ../_build
 NVCC=${NVCC:-nvcc}
-ARCH="-gencode arch=compute_100a,code=sm_100a"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
 # host float math (pose / inverse matrices) must not be FMA-contracted: the oracle restates it without (aarch64 g++ contracts by default)
 CXXF="-O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -ffp-contract=off"
 $NVCC $ARCH $CXXF -Xptxas -v -c kernels.cu -o ../_build/kernels.o 2> ../_build/kernels.ptxas.log || { cat ../_build/kernels.ptxas.log; exit 1; }
@@ -22,5 +22,5 @@ echo "built: $(ls ../_lib)"
 # C++ host-class demo (include/erasor/erasor.hpp over the C ABI)
 g++ -std=c++17 -O2 -o ../_lib/erasor_cpp_demo ../../examples/erasor_cpp_demo.cpp -L../_lib -lerasor_b200 -Wl,-rpath,'$ORIGIN' \
     -L/usr/local/cuda/lib64 -Wl,-rpath,/usr/local/cuda/lib64
-# micro-benchmark behind profiles/r01/microbench_match_any.txt
+# micro-benchmark of __match_any_sync latency and throughput (the voxelisation kernel groups equal keys with it)
 $NVCC $ARCH -O3 -o ../_lib/mb_match ../../scripts/mb_match.cu

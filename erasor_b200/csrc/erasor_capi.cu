@@ -1,5 +1,5 @@
 // erasor_capi.cu -- the extern "C" boundary (include/erasor_b200.h): context, HBM buffers, launch order.
-// There is no host compute path in this file: every entry point either launches the sm_100a kernels of
+// There is no host compute path in this file: every entry point either launches the sm_90a kernels of
 // kernels.cu or fails with an error code.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -94,7 +94,7 @@ struct erasor_ctx {
     int             device = 0;
     cudaStream_t    stream = nullptr, stream_a = nullptr, stream_b = nullptr, stream_c = nullptr;   // a/b/c: concurrent R-GPF size classes (high priority)
     cudaEvent_t     ev_fork = nullptr, ev_join_a = nullptr, ev_join_b = nullptr, ev_join_c = nullptr;
-    int             sm_count = 148;
+    int             sm_count = 132;
     std::string     err;
     HostBinTables   tables;
     DevBuf          d_ring, d_pos, d_neg, d_guard;

@@ -1,4 +1,4 @@
-// kernels.cu -- the sm_100a kernels of the R-POD -> Scan Ratio Test -> R-GPF path.
+// kernels.cu -- the sm_90a kernels of the R-POD -> Scan Ratio Test -> R-GPF path.
 //
 //   K1  k1_rpod_bin     polar index + per-bin min/max z and count, query and map in one launch
 //                       (ERASOR::voi2r_pod x2 + pt2r_pod, reference erasor.cpp:87-144)
@@ -79,7 +79,7 @@ __device__ __forceinline__ void k1_aggregate(int key, uint32_t zenc, int lane, u
     // Mixed warp (in node mode a third of the lanes of a typical row lie outside the VoI, so runs of equal bins are short):
     // per-lane shared-memory atomics, but only where they can change something -- a bin's min / max settle after its
     // first few points, and a plain (possibly stale) read is a safe filter because the values only move one way.
-    // (A segmented shuffle scan over the runs was measured at 68 instructions per row here, ncu r02; this is ~14.)
+    // (A segmented shuffle scan over the runs takes several times the instructions per row.)
     if (key >= 0) {
         if (key < B) {
             if (zenc < s_mn[key]) atomicMin(&s_mn[key], zenc);
@@ -310,7 +310,7 @@ cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map
     const size_t smem = k1_smem_bytes(T.R, B);
     cudaError_t e;
     // Bin tables beyond ~56 KB (40 x 360 bins: 173 KB) leave one CTA per SM: give that CTA 32 warps instead of 8, the
-    // kernel needs ~32 resident warps per SM to cover its latencies (measured: 1 / 2 / 4 CTAs of 8 warps -> 128 / 75 / 62 us).
+    // kernel needs ~32 resident warps per SM to cover its latencies.
     if (k1_big_tables(T.R, B)) {
         constexpr int THREADS = 1024;
         if (poses) {
@@ -1241,7 +1241,7 @@ __device__ __forceinline__ void group_excl_scan8(uint32_t* CNT, uint32_t* s_part
 // segment (match_any dedups equal digits inside a 32-element step, so no atomics), and after the group-wide scan
 // re-walks the segment in order handing out destinations -- which is what makes the sort stable.  Returns the
 // buffer (A or Bf) that holds the result.  ~35 warp instructions per 32 elements per pass: about 8x fewer than
-// the shared-memory bitonic network this replaced (profiles/README.md, R-GPF section).
+// the shared-memory bitonic network this replaced.
 template <int G, class KeyF>
 __device__ __forceinline__ uint32_t* group_radix_sort(uint32_t* A, uint32_t* Bf, uint32_t n, uint32_t* CNT, uint32_t* s_part,
                                                       int key_bits, KeyF key) {
@@ -2018,7 +2018,7 @@ k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32
             }
             __syncthreads();
             // stable LSD radix sort of the point order by voxel key (ties keep cloud order, like the index-tie-broken network it
-            // replaces -- measured at 57 k cycles for 512 points, r02): 8-bit digits, as many passes as the bin's cell count needs;
+            // replaces): 8-bit digits, as many passes as the bin's cell count needs;
             // every warp ranks a contiguous run of points with match.any, a column scan over the warps' rows makes the ranks global
             {
                 constexpr int NW = K4B_THREADS / 32;
@@ -2366,14 +2366,14 @@ __global__ void __launch_bounds__(256) k_and_unpack_keep(const uint32_t* __restr
 cudaError_t launch_pack_keep_bits(cudaStream_t st, const uint8_t* keep, size_t n, uint32_t* words) {
     const size_t n_words = (n + 31) / 32;
     if (n_words == 0) return cudaSuccess;
-    const unsigned blocks = (unsigned)std::min<size_t>((n_words + 7) / 8, 148 * 8);
+    const unsigned blocks = (unsigned)std::min<size_t>((n_words + 7) / 8, 132 * 8);
     k_pack_keep_bits<<<blocks, 256, 0, st>>>(keep, n, words, n_words);
     return cudaGetLastError();
 }
 cudaError_t launch_and_unpack_keep(cudaStream_t st, const uint32_t* gathered, int n_ranks, size_t n, uint8_t* keep) {
     const size_t n_words = (n + 31) / 32;
     if (n_words == 0) return cudaSuccess;
-    const unsigned blocks = (unsigned)std::min<size_t>((n_words + 7) / 8, 148 * 8);
+    const unsigned blocks = (unsigned)std::min<size_t>((n_words + 7) / 8, 132 * 8);
     k_and_unpack_keep<<<blocks, 256, 0, st>>>(gathered, n_ranks, n_words, n, keep);
     return cudaGetLastError();
 }
@@ -2383,7 +2383,7 @@ __global__ void __launch_bounds__(256) k_fill_u8(uint8_t* __restrict__ p, size_t
 }
 cudaError_t launch_fill_u8(cudaStream_t st, uint8_t* p, size_t n, uint8_t v) {
     if (n == 0) return cudaSuccess;
-    const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 148 * 8);
+    const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 132 * 8);
     k_fill_u8<<<blocks, 256, 0, st>>>(p, n, v);
     return cudaGetLastError();
 }

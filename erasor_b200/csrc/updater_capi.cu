@@ -67,7 +67,7 @@ struct erasor_updater_ctx {
     uint64_t la_ticket = 0;
     uint32_t* h_words = nullptr;                     // pinned read-back of the two device counters (a copy into pageable memory would
                                                      // block until the stream has drained and then some)
-    int sm_count = 148;
+    int sm_count = 132;
     uint64_t map_version = 0;                       // bumped whenever the map changes (processed node, reset)
     uint64_t save_version = ~0ull; float save_leaf = 0.0f; size_t save_n = 0;   // what save_out currently holds
 };

@@ -6,7 +6,7 @@
 // with two substitutions only:
 //     pcl::PointCloud<pcl::PointXYZI>   ->  erasor_b200::PointCloud   (x, y, z, intensity; 16 bytes)
 //     ERASOR(ros::NodeHandle*)          ->  ERASOR(const erasor_params_t&)   (the same /erasor/* keys)
-// Everything the methods compute runs in the sm_100a kernels behind the C ABI; this header holds no
+// Everything the methods compute runs in the sm_90a kernels behind the C ABI; this header holds no
 // arithmetic.  The rviz / debug publishers of the reference (erasor.h:67-77) are not mirrored.
 #pragma once
 #include <algorithm>

@@ -1,5 +1,5 @@
 /* ============================================================================
- * erasor_b200.h -- C ABI of the B200-native R-POD -> Scan Ratio Test -> R-GPF path
+ * erasor_b200.h -- C ABI of the H100-native R-POD -> Scan Ratio Test -> R-GPF path
  *
  * This is the drop-in boundary for the reference's `class ERASOR`
  * (reference include/erasor/erasor.h:43-147, src/offline_map_updater/src/erasor.cpp)

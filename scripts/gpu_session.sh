@@ -16,8 +16,3 @@ for k in k_node_fused k4b_voxelize; do
       python scripts/updater_profile.py > gpurun_out/ncu_updater_$k.log 2>&1
   tail -1 gpurun_out/ncu_updater_$k.log
 done
-# Afterwards, where the reports landed (gpurun_out/ of the build container; ncu reads reports without a GPU):
-#   for f in gpurun_out/prof_*.ncu-rep; do ncu -i $f --page raw --csv --print-units base > ${f%.ncu-rep}.raw.csv; done
-#   python scripts/merge_ncu_csv.py profiles/r02/ncu_nodes_raw.csv   gpurun_out/prof_seq05_k1_rpod_bin.raw.csv gpurun_out/prof_seq05_k2_srt_scatter.raw.csv \
-#                                   gpurun_out/prof_seq05_k4_rgpfint256int32.raw.csv gpurun_out/prof_seq05_k4_rgpfint128int128.raw.csv
-#   python scripts/merge_ncu_csv.py profiles/r02/ncu_updater_raw.csv gpurun_out/prof_updater_k_node_fused.raw.csv gpurun_out/prof_updater_k4b_voxelize.raw.csv

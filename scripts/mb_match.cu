@@ -31,7 +31,7 @@ int main() {
     const char* names[] = {"32 distinct keys", "4 distinct keys", "1 key", "4 lanes, 4 keys"};
     for (int m = 0; m < 4; ++m) printf("match_any %-18s : %.1f cycles/op\n", names[m], h[m * 2] / 1000.0);
     for (int w : {1, 4, 8, 16, 32}) {
-        k_thr<<<148, w * 32>>>(w, d); cudaMemcpy(h, d, 16, cudaMemcpyDeviceToHost);
+        k_thr<<<132, w * 32>>>(w, d); cudaMemcpy(h, d, 16, cudaMemcpyDeviceToHost);
         printf("match_any 32 distinct, %2d warps/SM: %.1f cycles/op per warp\n", w, h[0] / 1000.0);
     }
     return 0;

@@ -1,5 +1,5 @@
 #!/bin/bash
-# scripts/run_config4.sh -- BASELINE config 4 on ONE B200 (gpurun): large_scale_05.yaml geometry, ~50 M-point VoI per frame:
+# scripts/run_config4.sh -- BASELINE config 4 on one GPU: large_scale_05.yaml geometry, ~50 M-point VoI per frame:
 # per-kernel CUDA-event times, then one `ncu --set full` capture of K1, K2 and R-GPF class C on it (dram__bytes vs algorithmic bytes)
 mkdir -p gpurun_out
 python scripts/config4_largescale.py 50000000 5 > gpurun_out/config4_largescale.json 2> gpurun_out/config4.err; tail -c 600 gpurun_out/config4_largescale.json; echo

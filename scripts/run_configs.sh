@@ -1,5 +1,5 @@
 #!/bin/bash
-# scripts/run_configs.sh -- the BASELINE.json configs that are not the driver's default workload, on ONE B200 (gpurun):
+# scripts/run_configs.sh -- the BASELINE.json configs that are not the driver's default workload, on one GPU:
 #   config 4  large_scale_05.yaml geometry, ~50 M-point VoI: per-kernel CUDA-event times + ncu --set full (dram__bytes vs algorithmic bytes)
 #   config 5  40 x 360 bins, 262144-point scans, 2 M-point resident map (per-rank share of the frame-sharded job)
 #   dense     the seq-05 twin at the size SURVEY 8 estimates for the real sequence

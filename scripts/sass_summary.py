@@ -1,5 +1,5 @@
 """Register / spill / shared-memory / SASS summary of every kernel in the product library (CPU only: ptxas -v logs of
-erasor_b200/csrc/build.sh + cuobjdump -sass of the objects).  Writes a markdown table to stdout (profiles/r02/ptxas_sass_summary.md)."""
+erasor_b200/csrc/build.sh + cuobjdump -sass of the objects).  Writes a markdown table to stdout."""
 import os
 import re
 import subprocess

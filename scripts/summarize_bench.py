@@ -1,4 +1,4 @@
-"""Key numbers of a bench.py JSON line (for the tables in BASELINE.md / profiles/README.md).  usage: summarize_bench.py file.json [...]"""
+"""Key numbers of a bench.py JSON line (for the tables in BASELINE.md).  usage: summarize_bench.py file.json [...]"""
 import json
 import sys
 
