@@ -41,6 +41,12 @@ struct NodePose {
     float  lim_lo, lim_hi; // float guard band around limit: d2f < lim_lo => inside for sure, d2f > lim_hi => outside for sure
 };
 
+// pcl::VoxelGrid's cell grid of one filter call (device_common.cuh: voxel_grid_setup)
+struct VoxelGridDims {
+    float leaf, inv;           // leaf size and 1 / leaf
+    int   min_b[3], div[3];    // first cell and number of cells per axis
+};
+
 struct SrtParams {
     double scan_ratio_threshold;
     double th_bin_max_h;

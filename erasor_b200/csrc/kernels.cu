@@ -18,6 +18,7 @@
 #include <cfloat>
 #include <cstdint>
 
+#include "device_common.cuh"
 #include "device_types.h"
 #include "kernels.h"
 
@@ -26,8 +27,6 @@
 #include <unordered_map>
 
 namespace erasor {
-
-#define FULL_MASK 0xFFFFFFFFu
 
 // cudaFuncSetAttribute costs a few microseconds per call; the dynamic shared-memory ceiling of a kernel only ever has
 // to grow, so remember the largest value set per kernel and skip the call otherwise.
@@ -127,16 +126,6 @@ __device__ __forceinline__ int bin_fast(float x, float y, float z, float z_lo, f
     return min(k, S - 1) * R + g;
 }
 
-// pcl::transformPointCloud, PCL 1.8 scalar path: ((m0*x + m1*y) + m2*z) + m3 in float, no contraction -- the same
-// association as updater_kernels.cu::affine and oracle transform_point_cloud (OfflineMapUpdater.cpp:436)
-__device__ __forceinline__ float4 affine12(const float* __restrict__ T, float4 p) {
-    float4 o;
-    o.x = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], p.x), __fmul_rn(T[1], p.y)), __fmul_rn(T[2], p.z)), T[3]);
-    o.y = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4], p.x), __fmul_rn(T[5], p.y)), __fmul_rn(T[6], p.z)), T[7]);
-    o.z = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[8], p.x), __fmul_rn(T[9], p.y)), __fmul_rn(T[10], p.z)), T[11]);
-    o.w = p.w;
-    return o;
-}
 // OfflineMapUpdater::fetch_VoI's cut (OfflineMapUpdater.cpp:394-396): pow(pt.x - x, 2) + pow(pt.y - y, 2) < max_dist_square in
 // double on float differences.  A float evaluation decides every point outside a 1e-6 band around the limit (its error is
 // below 2.4e-7 relative); points inside the band get the reference's double expression.
@@ -201,7 +190,7 @@ k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* _
         auto dense_row = [&](uint32_t n) {             // the first n (<= 32) entries of the ring
             const bool ok = (uint32_t)lane < n;
             const float4 e = q[(qh + lane) & 63u];
-            const float4 pp = affine12(s_pose.T, e);
+            const float4 pp = pcl_affine(s_pose.T, e);
             int b = bin_fast(pp.x, pp.y, pp.z, z_lo, z_hi, smax_lo, smax_hi, inv_ring, inv_ss, eps_q, R, S, s_ring);
             if (__any_sync(FULL_MASK, ok && b == -3)) {
                 if (ok && b == -3) b = bin_exact(T, pp.x, pp.y, pp.z, &fc);   // exact path (rare)
@@ -340,45 +329,6 @@ cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map
 // ============================================================================================
 // K3
 // ============================================================================================
-// exclusive scan of in[0..n) into out[0..n) (may alias); every thread returns the total.
-__device__ uint32_t block_excl_scan(const uint32_t* in, uint32_t* out, int n, uint32_t* s_part /*[34]*/) {
-    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
-    const int seg = (n + nt - 1) / nt;
-    const int b0 = min(n, tid * seg), b1 = min(n, b0 + seg);
-    uint32_t sum = 0;
-    for (int i = b0; i < b1; ++i) sum += in[i];
-    uint32_t incl = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t v = __shfl_up_sync(FULL_MASK, incl, o);
-        if (lane >= o) incl += v;
-    }
-    __syncthreads();                     // s_part may still be read from a previous call
-    if (lane == 31) s_part[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-        const uint32_t w = lane < nw ? s_part[lane] : 0u;
-        uint32_t wi = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t v = __shfl_up_sync(FULL_MASK, wi, o);
-            if (lane >= o) wi += v;
-        }
-        if (lane < nw) s_part[lane] = wi - w;
-        if (lane == 31) s_part[33] = wi;
-    }
-    __syncthreads();
-    uint32_t run = s_part[warp] + incl - sum;
-    const uint32_t total = s_part[33];
-    for (int i = b0; i < b1; ++i) {
-        const uint32_t v = in[i];
-        out[i] = run;
-        run += v;
-    }
-    __syncthreads();
-    return total;
-}
-
 __device__ __forceinline__ double std_min_d(double a, double b) { return (b < a) ? b : a; }   // std::min, NaN-faithful (App. B-4)
 
 // Does the Scan Ratio Test hand this bin to R-GPF?  The same decisions as k3_srt's status passes, reduced to the one bit
@@ -703,7 +653,7 @@ __device__ __forceinline__ void k2_scatter_pass(const uint16_t* __restrict__ ids
             for (int u = 0; u < 4; ++u) {
                 if (dst[g + u] != kSkip) {
                     const size_t o = (size_t)out_base + dst[g + u];
-                    out_pts[o] = NODE ? affine12(s_T, pv[u]) : pv[u];
+                    out_pts[o] = NODE ? pcl_affine(s_T, pv[u]) : pv[u];
                     out_src[o] = si[u];
                 }
             }
@@ -1030,13 +980,8 @@ cudaError_t launch_k2_both(cudaStream_t st, const ChunkDesc* chunks, uint32_t n_
 // ============================================================================================
 // K4  R-GPF
 // ============================================================================================
-// All float arithmetic below is spelled with round-to-nearest intrinsics so that nvcc cannot contract
-// a*b+c into an FMA: the reference's x86-64 build (no -march, CMakeLists.txt:3-4) has none, and the
+// All float arithmetic below is spelled with round-to-nearest intrinsics (FM/FA/FS/FD, device_common.cuh; FSQ): the
 // unshifted covariance of PCL<=1.10 is so ill-conditioned that a single different rounding moves the plane.
-#define FM(a, b) __fmul_rn((a), (b))
-#define FA(a, b) __fadd_rn((a), (b))
-#define FS(a, b) __fsub_rn((a), (b))
-#define FD(a, b) __fdiv_rn((a), (b))
 #define FSQ(a)   __fsqrt_rn((a))
 
 struct Rot { float c, s; };
@@ -1915,13 +1860,10 @@ cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, con
 // ============================================================================================
 constexpr int K4B_THREADS = 512;      // one CTA per flagged bin; the per-bin chain (sort, heads, centroids, 1-NN) is what a launch lasts
 
-// conservative distance along one axis from x to the voxel cell `cell` lying `off` cells away from x's own (see
-// updater_kernels.cu::cell_gap): never more than the true gap, so a cell is only skipped when it cannot hold the nearest point
-__device__ __forceinline__ float k4b_cell_gap(float x, int cell, int off, float leaf, float slack) {
-    if (off == 0) return 0.0f;
-    const float g = (off > 0) ? ((float)cell * leaf - x) : (x - (float)(cell + 1) * leaf);
-    return fmaxf(g - slack, 0.0f);
-}
+struct XyziPts {                      // a bin's points as K4b holds them: separate x, y, z and intensity arrays
+    const float *x, *y, *z, *w;
+    __device__ __forceinline__ float4 operator[](uint32_t i) const { return make_float4(x[i], y[i], z[i], w[i]); }
+};
 
 __global__ void __launch_bounds__(K4B_THREADS)
 k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32_t* __restrict__ n_recs, uint32_t rec_capacity,
@@ -1937,7 +1879,6 @@ k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32
     __shared__ uint32_t s_tot[256];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t nrec = min(*n_recs, rec_capacity);
-    const float inv = FD(1.0f, leaf_f);
     const uint32_t* cq  = cnt + (B + 1);
     const uint32_t* dsm = dst_start;
     const uint32_t* dsq = dst_start + (B + 2);
@@ -1989,41 +1930,27 @@ k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32
             }
             __syncthreads();
         }
-        const float mnx = s_minmax[0], mny = s_minmax[1], mnz = s_minmax[2];
-        const float mxx = s_minmax[3], mxy = s_minmax[4], mxz = s_minmax[5];
-        const long long dx = (long long)FM(FS(mxx, mnx), inv) + 1;
-        const long long dy = (long long)FM(FS(mxy, mny), inv) + 1;
-        const long long dz = (long long)FM(FS(mxz, mnz), inv) + 1;
-        const bool overflow = (dx * dy * dz) > 2147483647LL;
+        bool overflow;
+        unsigned long long cells;
+        const VoxelGridDims vg = voxel_grid_setup(s_minmax, s_minmax + 3, leaf_f, overflow, cells);
+        const XyziPts pts{X, Y, Z, I};
         uint32_t nv;
         float4* out = vox_pts + region;
-        // pcl::VoxelGrid's cell grid of this bin (meaningful when !overflow)
-        const int g_mb0 = (int)floorf(FM(mnx, inv)), g_mb1 = (int)floorf(FM(mny, inv)), g_mb2 = (int)floorf(FM(mnz, inv));
-        const int g_div0 = (int)floorf(FM(mxx, inv)) - g_mb0 + 1, g_div1 = (int)floorf(FM(mxy, inv)) - g_mb1 + 1, g_div2 = (int)floorf(FM(mxz, inv)) - g_mb2 + 1;
         if (overflow) {
             // "Leaf size is too small for the input dataset": output = input
             nv = n;
             for (uint32_t i = tid; i < n; i += K4B_THREADS) out[i] = make_float4(X[i], Y[i], Z[i], I[i]);
             __syncthreads();
         } else {
-            const int mb0 = (int)floorf(FM(mnx, inv)), mb1 = (int)floorf(FM(mny, inv)), mb2 = (int)floorf(FM(mnz, inv));
-            const int Mb0 = (int)floorf(FM(mxx, inv)), Mb1 = (int)floorf(FM(mxy, inv));
-            const int div0 = Mb0 - mb0 + 1, div1 = Mb1 - mb1 + 1;
-            const int mul1 = div0, mul2 = div0 * div1;
-            for (uint32_t i = tid; i < n; i += K4B_THREADS) {
-                const int ijk0 = (int)FS(floorf(FM(X[i], inv)), (float)mb0);
-                const int ijk1 = (int)FS(floorf(FM(Y[i], inv)), (float)mb1);
-                const int ijk2 = (int)FS(floorf(FM(Z[i], inv)), (float)mb2);
-                KEY[i] = (uint32_t)(ijk0 + ijk1 * mul1 + ijk2 * mul2);
-            }
+            for (uint32_t i = tid; i < n; i += K4B_THREADS) KEY[i] = voxel_key_of(vg, X[i], Y[i], Z[i]);
             __syncthreads();
-            // stable LSD radix sort of the point order by voxel key (ties keep cloud order, like the index-tie-broken network it
-            // replaces): 8-bit digits, as many passes as the bin's cell count needs;
-            // every warp ranks a contiguous run of points with match.any, a column scan over the warps' rows makes the ranks global
+            // stable LSD radix sort of the point order by voxel key (ties keep cloud order): 8-bit digits, as many passes as the
+            // bin's cell count needs; every warp ranks a contiguous run of points with match.any, a column scan over the warps' rows
+            // makes the ranks global.  Not group_radix_sort: its [digit][warp] counters put a warp's distinct digits on two
+            // shared-memory banks at 16 warps, and this kernel measured ~6% slower with it (H100 80GB HBM3 SXM, 700 W).
             {
                 constexpr int NW = K4B_THREADS / 32;
-                const uint32_t cells = (uint32_t)((long long)g_div0 * g_div1 * g_div2);       // < 2^31: the overflow case went the other way
-                int bits = 1; while (bits < 31 && (1u << bits) < cells) ++bits;
+                int bits = 1; while (bits < 31 && (1u << bits) < (uint32_t)cells) ++bits;
                 const int npass = (bits + 7) / 8;
                 const uint32_t chunk = ((n + NW * 32u - 1u) / (NW * 32u)) * 32u;
                 const uint32_t w0 = min(n, (uint32_t)warp * chunk), w1 = min(n, w0 + chunk);
@@ -2088,74 +2015,20 @@ k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32
             nv = k4_compact<K4B_THREADS>(n, VST, s_warp, [&](uint32_t i) { return i == 0 || KEY[ORD[i]] != KEY[ORD[i - 1]]; });
             if (tid == 0) VST[nv] = n;
             __syncthreads();
-            // centroids: float sums in member order, divided by float(count)  (pcl::CentroidPoint)
             for (uint32_t v = tid; v < nv; v += K4B_THREADS) {
-                const uint32_t a = VST[v], e = VST[v + 1];
-                float sx = 0.0f, sy = 0.0f, sz = 0.0f, si = 0.0f;
-                for (uint32_t li = a; li < e; ++li) {
-                    const uint32_t q = ORD[li];
-                    sx = FA(sx, X[q]); sy = FA(sy, Y[q]); sz = FA(sz, Z[q]); si = FA(si, I[q]);
-                }
-                const float cn = (float)(e - a);
-                out[v] = make_float4(FD(sx, cn), FD(sy, cn), FD(sz, cn), FD(si, cn));
+                out[v] = voxel_centroid(pts, ORD, VST[v], VST[v + 1]);
+                VK[v] = KEY[ORD[VST[v]]];
             }
             __syncthreads();
         }
         // exact 1-NN of every centroid into the bin's points (ties to the lowest index); copy that point's intensity.
-        // Through the voxel grid itself: the centroid's own cell first, then the 26 around it -- each skipped when even its
-        // nearest corner is provably farther than the best so far -- and further shells only while something unseen could
-        // still be closer.  Same result as comparing against every point (the fallback for the overflow case and for
-        // non-finite centroids), at a few cells per centroid instead of n distance evaluations.
-        if (!overflow) {
-            for (uint32_t v = tid; v < nv; v += K4B_THREADS) VK[v] = KEY[ORD[VST[v]]];
-            __syncthreads();
-        }
+        // Through the voxel grid; comparing against every point in the overflow case and for non-finite centroids.
         for (uint32_t v = tid; v < nv; v += K4B_THREADS) {
             const float4 c = out[v];
-            float best = __int_as_float(0x7f800000);
-            uint32_t bi = 0xFFFFFFFFu;
             const bool finite = (fabsf(c.x) < 3.0e38f) && (fabsf(c.y) < 3.0e38f) && (fabsf(c.z) < 3.0e38f);
-            if (!overflow && finite) {
-                const int ci = (int)FS(floorf(FM(c.x, inv)), (float)g_mb0), cj = (int)FS(floorf(FM(c.y, inv)), (float)g_mb1), ck = (int)FS(floorf(FM(c.z, inv)), (float)g_mb2);
-                const float slack = 1.0e-3f * leaf_f + 4.0e-6f * fmaxf(fabsf(c.x), fmaxf(fabsf(c.y), fabsf(c.z)));
-                int rad = 0;
-                while (true) {
-                    for (int a = -rad; a <= rad; ++a) {
-                        const int ii = ci + a;
-                        if (ii < 0 || ii >= g_div0) continue;
-                        for (int bb = -rad; bb <= rad; ++bb) {
-                            const int jj = cj + bb;
-                            if (jj < 0 || jj >= g_div1) continue;
-                            for (int cc = -rad; cc <= rad; ++cc) {
-                                if (max(abs(a), max(abs(bb), abs(cc))) != rad) continue;
-                                const int kk = ck + cc;
-                                if (kk < 0 || kk >= g_div2) continue;
-                                if (rad > 0) {
-                                    const float gx = k4b_cell_gap(c.x, ii + g_mb0, a, leaf_f, slack);
-                                    const float gy = k4b_cell_gap(c.y, jj + g_mb1, bb, leaf_f, slack);
-                                    const float gz = k4b_cell_gap(c.z, kk + g_mb2, cc, leaf_f, slack);
-                                    if (0.999f * (gx * gx + gy * gy + gz * gz) > best) continue;
-                                }
-                                const uint32_t key = (uint32_t)(ii + jj * g_div0 + kk * g_div0 * g_div1);
-                                uint32_t lo = 0, hi = nv;                 // first voxel with key >= `key`
-                                while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (VK[mid] < key) lo = mid + 1; else hi = mid; }
-                                if (lo >= nv || VK[lo] != key) continue;
-                                for (uint32_t li = VST[lo]; li < VST[lo + 1]; ++li) {
-                                    const uint32_t q = ORD[li];
-                                    const float ddx = FS(c.x, X[q]), ddy = FS(c.y, Y[q]), ddz = FS(c.z, Z[q]);
-                                    const float d = FA(FA(FM(ddx, ddx), FM(ddy, ddy)), FM(ddz, ddz));
-                                    if (d < best || (d == best && q < bi)) { best = d; bi = q; }
-                                }
-                            }
-                        }
-                    }
-                    const float reach = FM(FM((float)rad, leaf_f), 0.9999f);
-                    if (bi != 0xFFFFFFFFu && best < FM(reach, reach)) break;
-                    ++rad;
-                    if (rad > 4096) break;
-                }
-            }
-            if (bi == 0xFFFFFFFFu) {
+            uint32_t bi = (!overflow && finite) ? voxel_grid_nn(pts, ORD, VST, VK, nv, vg, c) : kNoPoint;
+            if (bi == kNoPoint) {
+                float best = __int_as_float(0x7f800000);
                 bi = 0;
                 for (uint32_t i = 0; i < n; ++i) {
                     const float ddx = FS(c.x, X[i]), ddy = FS(c.y, Y[i]), ddz = FS(c.z, Z[i]);

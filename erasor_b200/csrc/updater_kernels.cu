@@ -18,25 +18,10 @@
 #include <cfloat>
 #include <cstdint>
 
+#include "device_common.cuh"
 #include "updater_kernels.h"
 
 namespace erasor {
-
-#define FULL_MASK 0xFFFFFFFFu
-#define FM(a, b) __fmul_rn((a), (b))
-#define FA(a, b) __fadd_rn((a), (b))
-#define FS(a, b) __fsub_rn((a), (b))
-#define FD(a, b) __fdiv_rn((a), (b))
-
-// pcl::transformPointCloud, PCL 1.8 scalar path: ((m0*x + m1*y) + m2*z) + m3, float, no contraction
-__device__ __forceinline__ float4 affine(const Mat4& T, float4 p) {
-    float4 o;
-    o.x = FA(FA(FA(FM(T.m[0], p.x), FM(T.m[1], p.y)), FM(T.m[2], p.z)), T.m[3]);
-    o.y = FA(FA(FA(FM(T.m[4], p.x), FM(T.m[5], p.y)), FM(T.m[6], p.z)), T.m[7]);
-    o.z = FA(FA(FA(FM(T.m[8], p.x), FM(T.m[9], p.y)), FM(T.m[10], p.z)), T.m[11]);
-    o.w = p.w;
-    return o;
-}
 
 __device__ __forceinline__ bool part_pred(const PartPred& P, float4 p) {
     if (P.kind == PART_RADIUS) {
@@ -61,7 +46,7 @@ constexpr int PART_CHUNK = 4096;          // points per partition / head-count c
 
 __global__ void k_affine_copy(Mat4 T, int do_transform, const float4* in, float4* out, uint32_t n) {   // in may alias out
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = do_transform ? affine(T, in[i]) : in[i];
+    if (i < n) out[i] = do_transform ? pcl_affine(T.m, in[i]) : in[i];
 }
 __global__ void __launch_bounds__(256) k_copy_segments(Mat4 T, CopySeg s0, CopySeg s1, CopySeg s2, CopySeg s3) {
     const CopySeg segs[4] = {s0, s1, s2, s3};
@@ -70,7 +55,7 @@ __global__ void __launch_bounds__(256) k_copy_segments(Mat4 T, CopySeg s0, CopyS
     for (int k = 0; k < 4; ++k) {
         const uint32_t blocks = (segs[k].n + 255u) / 256u * 256u;     // segments start on block boundaries: no divergence inside a warp
         if (i < blocks) {
-            if (i < segs[k].n) { const float4 p = segs[k].src[i]; segs[k].dst[i] = segs[k].xform ? affine(T, p) : p; }
+            if (i < segs[k].n) { const float4 p = segs[k].src[i]; segs[k].dst[i] = segs[k].xform ? pcl_affine(T.m, p) : p; }
             return;
         }
         i -= blocks;
@@ -93,9 +78,6 @@ cudaError_t launch_affine_copy(cudaStream_t st, const Mat4& T, bool do_transform
 // ============================================================================================
 // U3  voxelize_preserving_labels
 // ============================================================================================
-__device__ __forceinline__ uint32_t f2ord(float f) { const uint32_t u = __float_as_uint(f); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
-__device__ __forceinline__ float ord2f(uint32_t o) { return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o); }
-
 // Radix-sort segment = the run of points one warp ranks (stably, match.any) in a pass.  The walk is a serial chain of rows, so
 // segments are as short as the counter matrices allow: 8 rows of 32 up to 2 M points, longer beyond (<= 8192 segments).
 constexpr uint32_t RS_ROWS_MIN = 8, RS_MAX_SEGS = 8192;
@@ -105,86 +87,6 @@ __host__ __device__ inline uint32_t rs_seg_len(uint32_t n) {
     uint32_t rows = (uint32_t)(((unsigned long long)n + 32ull * RS_MAX_SEGS - 1ull) / (32ull * RS_MAX_SEGS));
     rows = (rows + RS_ROWS_MIN - 1u) / RS_ROWS_MIN * RS_ROWS_MIN;
     return 32u * (rows < RS_ROWS_MIN ? RS_ROWS_MIN : rows);
-}
-
-// pcl::CentroidPoint: float sums over the voxel's members in cloud order, divided by float(count)
-__device__ __forceinline__ float4 vox_centroid_of(const float4* __restrict__ in, const uint32_t* __restrict__ sidx, const uint32_t* __restrict__ vox_start, uint32_t v) {
-    const uint32_t a = vox_start[v], e = vox_start[v + 1];
-    float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
-    for (uint32_t k = a; k < e; ++k) {
-        const float4 p = in[sidx[k]];
-        sx = FA(sx, p.x); sy = FA(sy, p.y); sz = FA(sz, p.z); si = FA(si, p.w);
-    }
-    const float cn = (float)(e - a);
-    return make_float4(FD(sx, cn), FD(sy, cn), FD(sz, cn), FD(si, cn));
-}
-
-// Conservative distance along one axis from coordinate x to the voxel cell with (absolute) index `cell`, which lies `off` cells
-// away from x's own cell (off < 0: below, > 0: above, 0: the same slab).  A point is assigned to `cell` when
-// floorf(x * (1 / leaf)) == cell in float arithmetic, so the cell's faces sit within a few ulp of cell * leaf and (cell + 1) * leaf;
-// `slack` covers that and the rounding of this expression, so the returned gap never exceeds the true one.
-__device__ __forceinline__ float cell_gap(float x, int cell, int off, float leaf, float slack) {
-    if (off == 0) return 0.0f;
-    const float g = (off > 0) ? ((float)cell * leaf - x) : (x - (float)(cell + 1) * leaf);
-    return fmaxf(g - slack, 0.0f);
-}
-
-// exact 1-NN of a centroid into the source cloud through the voxel grid itself (cells = voxels): grow the Chebyshev shell
-// until nothing unseen can be closer; ties go to the lowest cloud index.  Mirrors oracle/ line by line.
-__device__ __noinline__ float4 vox_label_of(const float4* __restrict__ in, const uint32_t* __restrict__ sidx, const uint32_t* __restrict__ vox_start,
-                                            const uint32_t* __restrict__ vox_key, const VoxGrid* __restrict__ g, uint32_t nv, float4 c) {
-    if (g->overflow) return c;         // every point is its own voxel: the nearest point is itself (or an identical earlier one)
-    const float inv = g->inv, leaf = g->leaf;
-    const int d0 = g->div[0], d1 = g->div[1], d2 = g->div[2];
-    const int ci = (int)FS(floorf(FM(c.x, inv)), (float)g->min_b[0]);
-    const int cj = (int)FS(floorf(FM(c.y, inv)), (float)g->min_b[1]);
-    const int ck = (int)FS(floorf(FM(c.z, inv)), (float)g->min_b[2]);
-    float best_d = __int_as_float(0x7f800000);
-    uint32_t best_i = 0xFFFFFFFFu;
-    const float slack = 1.0e-3f * leaf + 4.0e-6f * fmaxf(fabsf(c.x), fmaxf(fabsf(c.y), fabsf(c.z)));
-    int rad = 0;
-    while (true) {
-        // scan the shell of Chebyshev radius `rad`
-        for (int a = -rad; a <= rad; ++a) {
-            const int ii = ci + a;
-            if (ii < 0 || ii >= d0) continue;
-            for (int b = -rad; b <= rad; ++b) {
-                const int jj = cj + b;
-                if (jj < 0 || jj >= d1) continue;
-                for (int cc = -rad; cc <= rad; ++cc) {
-                    if (max(abs(a), max(abs(b), abs(cc))) != rad) continue;
-                    const int kk = ck + cc;
-                    if (kk < 0 || kk >= d2) continue;
-                    // Skip the cell when even its nearest corner is provably farther than the best so far (strictly: no tie can hide
-                    // there).  The gaps are shortened by more than the float error of the cell assignment, so this only drops work.
-                    if (rad > 0) {
-                        const float gx = cell_gap(c.x, ci + a + g->min_b[0], a, leaf, slack);
-                        const float gy = cell_gap(c.y, cj + b + g->min_b[1], b, leaf, slack);
-                        const float gz = cell_gap(c.z, ck + cc + g->min_b[2], cc, leaf, slack);
-                        if (0.999f * (gx * gx + gy * gy + gz * gz) > best_d) continue;
-                    }
-                    const uint32_t key = (uint32_t)(ii + jj * d0 + kk * d0 * d1);
-                    uint32_t lo = 0, hi = nv;                 // first voxel with vox_key >= key
-                    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (vox_key[mid] < key) lo = mid + 1; else hi = mid; }
-                    if (lo >= nv || vox_key[lo] != key) continue;
-                    for (uint32_t k = vox_start[lo]; k < vox_start[lo + 1]; ++k) {
-                        const uint32_t i = sidx[k];
-                        const float4 p = in[i];
-                        const float dx = FS(c.x, p.x), dy = FS(c.y, p.y), dz = FS(c.z, p.z);
-                        const float d = FA(FA(FM(dx, dx), FM(dy, dy)), FM(dz, dz));
-                        if (d < best_d || (d == best_d && i < best_i)) { best_d = d; best_i = i; }
-                    }
-                }
-            }
-        }
-        const float reach = FM(FM((float)rad, leaf), 0.9999f);
-        if (best_i != 0xFFFFFFFFu && best_d < FM(reach, reach)) break;
-        ++rad;
-        if (rad > 64 && best_i != 0xFFFFFFFFu) break;
-        if (rad > 4096) break;
-    }
-    if (best_i != 0xFFFFFFFFu) c.w = in[best_i].w;
-    return c;
 }
 
 // ============================================================================================
@@ -199,32 +101,6 @@ __device__ __noinline__ float4 vox_label_of(const float4* __restrict__ in, const
 namespace cg = cooperative_groups;
 constexpr int FT = 1024;                 // threads per CTA
 constexpr int FW = FT / 32;
-
-// exclusive scan of v[0..n) in place by one CTA of FT threads; *total (nullable) receives the sum
-__device__ void cta_scan_u32(uint32_t* __restrict__ v, uint32_t n, uint32_t* __restrict__ total, uint32_t* s_part /*[34]*/) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t seg = (n + FT - 1u) / FT;
-    const uint32_t b0 = min(n, tid * seg), b1 = min(n, b0 + seg);
-    uint32_t sum = 0;
-    for (uint32_t i = b0; i < b1; ++i) sum += v[i];
-    uint32_t incl = sum;
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(FULL_MASK, incl, o); if (lane >= o) incl += t; }
-    __syncthreads();
-    if (lane == 31) s_part[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-        const uint32_t w = s_part[lane];
-        uint32_t wi = w;
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(FULL_MASK, wi, o); if (lane >= o) wi += t; }
-        s_part[lane] = wi - w;
-        if (lane == 31) s_part[33] = wi;
-    }
-    __syncthreads();
-    uint32_t run = s_part[warp] + incl - sum;
-    for (uint32_t i = b0; i < b1; ++i) { const uint32_t t = v[i]; v[i] = run; run += t; }
-    if (tid == 0 && total) *total = s_part[33];
-    __syncthreads();
-}
 
 // rank of the flagged threads of one FT-wide row in thread order: `before` = flagged threads in front of this one, `round` = all
 __device__ __forceinline__ void cta_rank(bool flag, uint32_t* s_w /*[FW]*/, uint32_t& before, uint32_t& round) {
@@ -248,6 +124,12 @@ __device__ __forceinline__ uint32_t cta_sum(uint32_t c, uint32_t* s_w /*[FW]*/) 
     for (int w = 0; w < FW; ++w) t += s_w[w];
     __syncthreads();
     return t;
+}
+
+// U3's 1-NN, out of line: k_node_fused runs at __launch_bounds__(1024, 1), which allows at most 64 registers per thread
+__device__ __noinline__ uint32_t u3_nearest(const float4* __restrict__ pts, const uint32_t* __restrict__ order, const uint32_t* __restrict__ vox_start,
+                                            const uint32_t* __restrict__ vox_key, uint32_t nv, VoxelGridDims g, float4 c) {
+    return voxel_grid_nn(pts, order, vox_start, vox_key, nv, g, c);
 }
 
 struct VoxPlan {                          // carve-up of the voxeliser's scratch (host and device agree through this one function)
@@ -293,7 +175,7 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
         uint32_t mn[3] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu}, mx[3] = {0u, 0u, 0u};
         for (uint32_t i = bid * FT + tid; i < n; i += G * FT) {
             const float4 p = J.vin[i];
-            const uint32_t a = f2ord(p.x + 0.0f), b = f2ord(p.y + 0.0f), c = f2ord(p.z + 0.0f);
+            const uint32_t a = float_to_ordered(p.x + 0.0f), b = float_to_ordered(p.y + 0.0f), c = float_to_ordered(p.z + 0.0f);
             mn[0] = min(mn[0], a); mx[0] = max(mx[0], a);
             mn[1] = min(mn[1], b); mx[1] = max(mx[1], b);
             mn[2] = min(mn[2], c); mx[2] = max(mx[2], c);
@@ -334,29 +216,15 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
         __syncthreads();
         if (tid == 0) {
             g->n_vox = 0; g->overflow = 0; g->npass = 0;
-            const float inv = FD(1.0f, J.leaf);
-            g->leaf = J.leaf; g->inv = inv;
             if (n == 0) {
-                for (int k = 0; k < 3; ++k) { g->mn[k] = 0xFFFFFFFFu; g->mx[k] = 0u; g->div[k] = 1; g->min_b[k] = 0; }
                 *J.d_n_out = 0u;
             } else {
-                float mnf[3], mxf[3];
-                for (int k = 0; k < 3; ++k) {
-                    g->mn[k] = s_w[k]; g->mx[k] = s_w[3 + k];
-                    mnf[k] = ord2f(s_w[k]); mxf[k] = ord2f(s_w[3 + k]);
-                }
-                const long long dx = (long long)FM(FS(mxf[0], mnf[0]), inv) + 1;
-                const long long dy = (long long)FM(FS(mxf[1], mnf[1]), inv) + 1;
-                const long long dz = (long long)FM(FS(mxf[2], mnf[2]), inv) + 1;
-                const int ovf = (dx * dy * dz) > 2147483647LL ? 1 : 0;
+                float mm[6];                    // min x, y, z, max x, y, z
+                for (int k = 0; k < 6; ++k) mm[k] = ordered_to_float(s_w[k]);
+                bool ovf;
+                unsigned long long cells;
+                g->dims = voxel_grid_setup(mm, mm + 3, J.leaf, ovf, cells);
                 g->overflow = ovf;
-                unsigned long long cells = 1ull;
-                for (int k = 0; k < 3; ++k) {
-                    g->min_b[k] = (int)floorf(FM(mnf[k], inv));
-                    const int max_b = (int)floorf(FM(mxf[k], inv));
-                    g->div[k] = max_b - g->min_b[k] + 1;
-                    cells *= (unsigned long long)(unsigned)g->div[k];
-                }
                 // radix passes the keys need: keys are < cells (int32 arithmetic as in PCL), or < n in the overflow case
                 unsigned long long lim = ovf ? (unsigned long long)n : cells;
                 int bits = 32;
@@ -366,7 +234,10 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
         }
         __syncthreads();
     }
-    if (J.has_part && bid == G - 1) cta_scan_u32(J.chunk_tmp, pchunks, J.d_total_sel, s_part);
+    if (J.has_part && bid == G - 1) {
+        const uint32_t t = block_excl_scan(J.chunk_tmp, J.chunk_tmp, (int)pchunks, s_part);
+        if (tid == 0) *J.d_total_sel = t;
+    }
     grid.sync();
     PH(2);
 
@@ -375,20 +246,10 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
     uint32_t* const my_c = s_c + warp * RD;
     if (n) {
         const int ovf = g->overflow;
-        const float inv = g->inv;
-        const float mb0 = (float)g->min_b[0], mb1 = (float)g->min_b[1], mb2 = (float)g->min_b[2];
-        const int d0 = g->div[0], d01 = g->div[0] * g->div[1];
+        const VoxelGridDims vg = g->dims;
         for (uint32_t e = bid * FT + tid; e < n; e += G * FT) {
             const float4 p = J.vin[e];
-            uint32_t k;
-            if (ovf) {
-                k = e;      // "Leaf size is too small": output = input, one point per voxel in cloud order
-            } else {
-                const int ijk0 = (int)FS(floorf(FM(p.x, inv)), mb0);
-                const int ijk1 = (int)FS(floorf(FM(p.y, inv)), mb1);
-                const int ijk2 = (int)FS(floorf(FM(p.z, inv)), mb2);
-                k = (uint32_t)(ijk0 + ijk1 * d0 + ijk2 * d01);
-            }
+            const uint32_t k = ovf ? e : voxel_key_of(vg, p.x, p.y, p.z);   // overflow ("Leaf size is too small"): one voxel per point
             vp.key_a[e] = k; vp.idx_a[e] = e;
             atomicAdd(&vp.cnt_x[(size_t)(k & (RD - 1u)) * nseg + e / SEG], 1u);      // pass 0's histogram (counts: order-free)
         }
@@ -406,7 +267,7 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
                 uint32_t rank_sel, round;
                 cta_rank(s, s_w, rank_sel, round);
                 if (ok) {
-                    if (s) J.out_sel[sel_base + rank_sel] = J.xform_sel ? affine(J.T_sel, p) : p;
+                    if (s) J.out_sel[sel_base + rank_sel] = J.xform_sel ? pcl_affine(J.T_sel.m, p) : p;
                     else   J.out_rest[rest_base + (i - r0) - rank_sel] = p;
                 }
                 const uint32_t valid = min((uint32_t)FT, b1 - r0);
@@ -530,7 +391,10 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
         if (tid == 0) vp.chunk[vb] = t;
     }
     grid.sync();
-    if (bid == 0) cta_scan_u32(vp.chunk, hchunks, J.d_n_out, s_part);
+    if (bid == 0) {
+        const uint32_t t = block_excl_scan(vp.chunk, vp.chunk, (int)hchunks, s_part);
+        if (tid == 0) *J.d_n_out = t;
+    }
     grid.sync();
     PH(13);
     const uint32_t n_vox = *J.d_n_out;
@@ -554,9 +418,12 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
     for (uint32_t v0 = ((uint32_t)warp * G + bid) * 32u; v0 < n_vox; v0 += G * FT) {     // 32 consecutive voxels per warp, warps dealt round-robin over the SMs
         const uint32_t v = v0 + lane;
         if (v >= n_vox) continue;
-        float4 c = vox_centroid_of(J.vin, sidx, vp.vstart, v);
-        c = vox_label_of(J.vin, sidx, vp.vstart, vp.vkey, g, n_vox, c);
-        J.vout[v] = J.xform_out ? affine(J.T_out, c) : c;
+        float4 c = voxel_centroid(J.vin, sidx, vp.vstart[v], vp.vstart[v + 1]);
+        if (!g->overflow) {        // else every point is its own voxel: the nearest point is itself (or an identical earlier one)
+            const uint32_t i = u3_nearest(J.vin, sidx, vp.vstart, vp.vkey, n_vox, g->dims, c);
+            if (i != kNoPoint) c.w = J.vin[i].w;
+        }
+        J.vout[v] = J.xform_out ? pcl_affine(J.T_out.m, c) : c;
     }
     PH(15);
 #undef PH

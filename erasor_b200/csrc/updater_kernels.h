@@ -5,6 +5,8 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "device_types.h"
+
 namespace erasor {
 
 struct Mat4 { float m[16]; };            // row-major 4x4, like Eigen::Matrix4f(r, c) = m[4 r + c]
@@ -18,9 +20,7 @@ struct PartPred {
 };
 
 struct VoxGrid {                         // pcl::VoxelGrid state of one filter call, kept on the device
-    uint32_t mn[3], mx[3];               // order-preserving encodings of the cloud's min / max
-    float    leaf, inv;
-    int      min_b[3], div[3];
+    VoxelGridDims dims;
     uint32_t n_vox;
     int      overflow;
     int      npass;                      // 8-bit radix passes the key width needs

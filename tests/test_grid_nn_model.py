@@ -1,5 +1,5 @@
 """CPU model (numpy float32, no FMA -- like the kernels' _rn intrinsics) of the grid-pruned exact 1-NN that labels voxel centroids
-(erasor_b200/csrc/updater_kernels.cu vox_label_of + cell_gap, kernels.cu k4b_voxelize): own cell first, then the 26 around it --
+(erasor_b200/csrc/device_common.cuh voxel_grid_nn + cell_gap, used by k4b_voxelize and k_node_fused): own cell first, then the 26 around it --
 each skipped when 0.999 * (conservative gap)^2 > best -- and further shells while something unseen could still be closer.
 The claim is EXACTNESS: the same (distance, lowest index) as comparing against every point.  The pruning is where that could
 break (a float cell assignment puts the faces a few ulp off k * leaf), so the model is driven with adversarial layouts: points
