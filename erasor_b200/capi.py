@@ -35,7 +35,14 @@ EXPORTS = [
     "erasor_updater_create", "erasor_updater_destroy", "erasor_updater_reset", "erasor_updater_last_error", "erasor_updater_process_node", "erasor_updater_prefetch_scan",
     "erasor_updater_map_size", "erasor_updater_get_cloud", "erasor_updater_save_static_map", "erasor_updater_voxelize", "erasor_updater_mapgen_node",
     "erasor_updater_erasor", "erasor_updater_kernel_launch_count", "erasor_updater_get_fused_profile",
+    "erasor_eval_create", "erasor_eval_destroy", "erasor_eval_last_error", "erasor_evaluate",
 ]
+NO_MATCH = 0xFFFFFFFF        # erasor_evaluate's match entry of a GT point without an inlier
+
+
+class EvalCountsC(ctypes.Structure):
+    """erasor_eval_counts_t"""
+    _fields_ = [(name, c_uint64) for name in ("gt_static", "gt_dynamic", "preserved_static", "preserved_dynamic", "inliers", "ambiguous_ties")]
 
 
 class UpdaterParamsC(ctypes.Structure):
@@ -136,6 +143,12 @@ def _load():
     L.erasor_updater_kernel_launch_count.restype = c_uint64
     L.erasor_updater_kernel_launch_count.argtypes = [c_void_p]
     L.erasor_updater_get_fused_profile.argtypes = [c_void_p, c_void_p]
+    L.erasor_eval_create.argtypes = [c_int, POINTER(c_void_p)]
+    L.erasor_eval_destroy.restype = None
+    L.erasor_eval_destroy.argtypes = [c_void_p]
+    L.erasor_eval_last_error.restype = c_char_p
+    L.erasor_eval_last_error.argtypes = [c_void_p]
+    L.erasor_evaluate.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_double, c_int, c_void_p, POINTER(EvalCountsC)]
     return L
 
 
@@ -468,6 +481,10 @@ class Map:
     def keep_ptr(self) -> int:
         return self.L.erasor_map_keep_device(self.h) or 0
 
+    @property
+    def points_ptr(self) -> int:
+        return self.L.erasor_map_points_device(self.h) or 0
+
     def reset_keep(self):
         rc = self.L.erasor_map_reset_keep(self.h)
         if rc != OK:
@@ -596,3 +613,80 @@ class Updater:
         t = np.zeros(16, dtype=np.uint64)
         self._ck(self.L.erasor_updater_get_fused_profile(self.h, t.ctypes.data))
         return [int(x) - int(t[0]) if x else None for x in t]
+
+
+class Evaluator:
+    """One ``erasor_eval_t``: PR / RR on the device, the counts of ``evaluate.evaluate`` by an exact grid-indexed 1-NN
+    (DESIGN.md section 11).  ``evaluate`` and ``evaluate_map`` return exactly ``evaluate.evaluate``'s dict; ``last_counts()``
+    adds ``inliers``, ``ambiguous_ties`` (inliers whose equally-nearest estimate points hold both classes -- the counts equal
+    sklearn's whenever it is 0) and, when asked for, ``match``.  Unlike sklearn, an empty estimate is no error: no GT point
+    is an inlier."""
+
+    def __init__(self, device: int = 0):
+        self.L = lib()
+        h = c_void_p()
+        rc = self.L.erasor_eval_create(device, ctypes.byref(h))
+        if rc != OK:
+            raise ErasorError(rc, (self.L.erasor_eval_last_error(None) or b"").decode())
+        self.h = h
+        self._last = None
+
+    def _ck(self, rc: int):
+        if rc != OK:
+            raise ErasorError(rc, (self.L.erasor_eval_last_error(self.h) or b"").decode())
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.erasor_eval_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def _finish(self, c: EvalCountsC, match) -> dict:
+        from . import evaluate
+        self._last = {name: int(getattr(c, name)) for name, _ in EvalCountsC._fields_}
+        if match is not None:
+            self._last["match"] = match
+        return evaluate.rates(c.gt_static, c.gt_dynamic, c.preserved_static, c.preserved_dynamic)
+
+    def evaluate(self, gt, est, keep=None, voxelsize: float = 0.2, want_match: bool = False) -> dict:
+        """Host clouds (float32 [n,4] x y z intensity); keep: optional uint8 mask over est (nonzero = part of the estimate)."""
+        g, e = _cloud(gt), _cloud(est)
+        k = None
+        if keep is not None:
+            k = np.ascontiguousarray(keep, dtype=np.uint8).reshape(-1)
+            if len(k) != len(e):
+                raise ValueError("keep must have one entry per estimate point")
+        match = np.empty(len(g), dtype=np.uint32) if want_match else None
+        c = EvalCountsC()
+        self._ck(self.L.erasor_evaluate(self.h, g.ctypes.data, len(g), e.ctypes.data, len(e), k.ctypes.data if k is not None else None,
+                                        float(voxelsize), PTR_HOST, match.ctypes.data if match is not None else None, ctypes.byref(c)))
+        return self._finish(c, match)
+
+    def evaluate_ptr(self, gt_ptr: int, n_gt: int, est_ptr: int, n_est: int, keep_ptr: int = 0, voxelsize: float = 0.2,
+                     ptr_kind: int = PTR_DEVICE, match_ptr: int = 0) -> dict:
+        """Raw pointers (device memory with PTR_DEVICE, float4-aligned clouds); match_ptr: optional uint32 [n_gt] output."""
+        c = EvalCountsC()
+        self._ck(self.L.erasor_evaluate(self.h, c_void_p(gt_ptr), n_gt, c_void_p(est_ptr), n_est, c_void_p(keep_ptr) if keep_ptr else None,
+                                        float(voxelsize), ptr_kind, c_void_p(match_ptr) if match_ptr else None, ctypes.byref(c)))
+        return self._finish(c, None)
+
+    def evaluate_map(self, m: "Map", voxelsize: float = 0.2) -> dict:
+        """Score a resident map in place: GT = the initial map, estimate = its points with keep != 0 (what bench.py's
+        final_map_quality builds on the host).  The handles that write the mask must have finished."""
+        n = m.size
+        return self.evaluate_ptr(m.points_ptr, n, m.points_ptr, n, m.keep_ptr, voxelsize, PTR_DEVICE)
+
+    def last_counts(self) -> dict:
+        """All six counts of the last call, plus ``match`` (uint32 per GT point, NO_MATCH without an inlier) when requested."""
+        return dict(self._last) if self._last is not None else None

@@ -4,7 +4,7 @@
 PR = GT-static inliers whose match is static / GT static; RR = (GT dynamic - GT-dynamic inliers whose match is
 dynamic) / GT dynamic; dynamic = SemanticKITTI classes 252..259 carried numerically in `intensity`.
 Host-side quality judge, not part of the path.  tests/test_evaluate.py checks it against the reference's own script
-when /root/reference is present.
+when /root/reference is present.  capi.Evaluator computes the same counts on the device (DESIGN.md section 11).
 """
 from __future__ import annotations
 
@@ -31,6 +31,13 @@ def evaluate(gt_xyzi: np.ndarray, est_xyzi: np.ndarray, voxelsize: float = 0.2) 
     est_is_dyn = np.isin(est_sem[idx[is_in]], DYNAMIC_CLASSES)
     preserved_static = int(np.sum((~gt_is_dyn) & (~est_is_dyn)))
     preserved_dynamic = int(np.sum(gt_is_dyn & est_is_dyn))
+    return rates(ns_gt, nd_gt, preserved_static, preserved_dynamic)
+
+
+def rates(ns_gt: int, nd_gt: int, preserved_static: int, preserved_dynamic: int) -> dict:
+    """The four counts -> evaluate()'s dict with PR, RR and F1.  The device evaluator (capi.Evaluator) calls this too, so equal
+    counts give identical floats."""
+    ns_gt, nd_gt, preserved_static, preserved_dynamic = int(ns_gt), int(nd_gt), int(preserved_static), int(preserved_dynamic)
     pr = preserved_static / ns_gt * 100.0 if ns_gt else 0.0
     rr = (nd_gt - preserved_dynamic) / nd_gt * 100.0 if nd_gt else 0.0
     f1 = 2 * (pr / 100) * (rr / 100) / ((pr / 100) + (rr / 100)) if (pr + rr) > 0 else 0.0

@@ -5,10 +5,12 @@ scripts/analysis_runner.py):
       -> naive map            erasor_b200.mapgen           (src/mapgen)
       -> static map           capi.Updater, one erasor_updater_process_node per node + save_static_map
                               (OfflineMapUpdater::callback_node / save_static_map, OfflineMapUpdater.cpp:174-330)
-      -> PR / RR              erasor_b200.evaluate         (scripts/analysis_runner.py)
+      -> PR / RR              capi.Evaluator (device), or erasor_b200.evaluate when the updater is injected
+                              (scripts/analysis_runner.py)
 
 Everything heavy runs on the device behind the C ABI; this module only sequences the calls.  The updater and the voxeliser are
-injectable so that tests/test_pipeline.py can drive the same code with the oracle's objects on a machine without a GPU.
+injectable so that tests/test_pipeline.py can drive the same code with the oracle's objects on a machine without a GPU; with an
+injected updater the evaluation stays on the host as well.
 """
 from __future__ import annotations
 
@@ -49,7 +51,12 @@ def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, mak
     original, naive = mapgen.build_map(nodes, leafsize=leaf, is_large_scale=bool(up.is_large_scale), voxelize=voxelize)
     res = run_offline(nodes, naive, up, ep, make_updater=make_updater)
     res["naive_map"] = naive
-    res["quality"] = evaluate.evaluate(naive, res["static_map"], voxelsize=0.2)
+    if make_updater is None:            # the device updater ran: score on the device too (same counts, same dict)
+        from . import capi
+        with capi.Evaluator() as ev:
+            res["quality"] = ev.evaluate(naive, res["static_map"], voxelsize=0.2)
+    else:
+        res["quality"] = evaluate.evaluate(naive, res["static_map"], voxelsize=0.2)
     if out_dir:
         os.makedirs(out_dir, exist_ok=True)
         name = getattr(up, "data_name", "seq")

@@ -300,6 +300,35 @@ uint64_t erasor_updater_kernel_launch_count(erasor_updater_t u);
  * scattered, [15] centroids + labels written. */
 int erasor_updater_get_fused_profile(erasor_updater_t u, uint64_t* ns16);
 
+/* ============================================================================================
+ * PR / RR on the device: the reference's scripts/analysis_runner.py metric (erasor_b200/evaluate.py) by an exact
+ * grid-indexed 1-NN from every ground-truth point into the estimate.  A handle of its own: one CUDA device + one stream,
+ * scratch (16 B per estimate point plus the cell table) kept and grown on demand; not thread-safe.
+ * ========================================================================================== */
+typedef struct erasor_eval_ctx* erasor_eval_t;
+
+typedef struct {
+    uint64_t gt_static;          /* GT points whose class is not dynamic (252..259) */
+    uint64_t gt_dynamic;
+    uint64_t preserved_static;   /* static GT inliers whose nearest estimate point is static */
+    uint64_t preserved_dynamic;  /* dynamic GT inliers whose nearest estimate point is dynamic */
+    uint64_t inliers;            /* GT points with an estimate point at distance < voxelsize * sqrt(3) / 2 */
+    uint64_t ambiguous_ties;     /* inliers whose equally-nearest estimate points hold both classes: only these may differ from sklearn */
+} erasor_eval_counts_t;
+
+int  erasor_eval_create(int device, erasor_eval_t* out);
+void erasor_eval_destroy(erasor_eval_t e);
+const char* erasor_eval_last_error(erasor_eval_t e);   /* e may be NULL: error of the last failed erasor_eval_create */
+/* gt_xyzi: n_gt points; est_xyzi: n_est points, of which est_keep (nullable, n_est bytes) selects those with keep != 0.
+ * The nearest estimate point is the one with the smallest double distance sqrt((dx*dx + dy*dy) + dz*dz); ties go to the lowest
+ * estimate index (original index, also under a keep mask).  match (nullable, n_gt entries): that index for inliers, 0xFFFFFFFF
+ * otherwise.  All buffers host or device (ptr_kind); device clouds 16-byte aligned.  With ERASOR_PTR_DEVICE a resident map is
+ * scored in place: gt = est = erasor_map_points_device(m), est_keep = erasor_map_keep_device(m) (wait for its handles first).
+ * Synchronous.  ERASOR_E_INVALID: a non-finite x, y or z in gt or in a selected estimate point, n_gt or n_est >= 2^32 - 1,
+ * voxelsize <= 0.  An empty (or fully deselected) estimate gives no inliers, where sklearn would raise; an empty gt all-zero counts. */
+int  erasor_evaluate(erasor_eval_t e, const float* gt_xyzi, size_t n_gt, const float* est_xyzi, size_t n_est,
+                     const uint8_t* est_keep, double voxelsize, int ptr_kind, uint32_t* match, erasor_eval_counts_t* out);
+
 #ifdef __cplusplus
 }
 #endif
