@@ -35,7 +35,8 @@ EXPORTS = [
     "erasor_updater_create", "erasor_updater_destroy", "erasor_updater_reset", "erasor_updater_last_error", "erasor_updater_process_node", "erasor_updater_prefetch_scan",
     "erasor_updater_map_size", "erasor_updater_get_cloud", "erasor_updater_save_static_map", "erasor_updater_voxelize", "erasor_updater_mapgen_node",
     "erasor_updater_erasor", "erasor_updater_kernel_launch_count", "erasor_updater_get_fused_profile",
-    "erasor_eval_create", "erasor_eval_destroy", "erasor_eval_last_error", "erasor_evaluate",
+    "erasor_eval_create", "erasor_eval_destroy", "erasor_eval_last_error", "erasor_evaluate", "erasor_eval_overlap",
+    "erasor_eval_count_selected",
 ]
 NO_MATCH = 0xFFFFFFFF        # erasor_evaluate's match entry of a GT point without an inlier
 
@@ -43,6 +44,11 @@ NO_MATCH = 0xFFFFFFFF        # erasor_evaluate's match entry of a GT point witho
 class EvalCountsC(ctypes.Structure):
     """erasor_eval_counts_t"""
     _fields_ = [(name, c_uint64) for name in ("gt_static", "gt_dynamic", "preserved_static", "preserved_dynamic", "inliers", "ambiguous_ties")]
+
+
+class EvalOverlapC(ctypes.Structure):
+    """erasor_eval_overlap_t"""
+    _fields_ = [(name, c_uint64) for name in ("n", "est_static", "est_dynamic", "below_half", "below_one", "below_two", "far_points")] + [("max", c_double)]
 
 
 class UpdaterParamsC(ctypes.Structure):
@@ -149,6 +155,9 @@ def _load():
     L.erasor_eval_last_error.restype = c_char_p
     L.erasor_eval_last_error.argtypes = [c_void_p]
     L.erasor_evaluate.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_double, c_int, c_void_p, POINTER(EvalCountsC)]
+    L.erasor_eval_overlap.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_double, c_int, c_void_p, c_size_t, c_void_p,
+                                      c_void_p, POINTER(EvalOverlapC)]
+    L.erasor_eval_count_selected.argtypes = [c_void_p, c_void_p, c_size_t, c_int, POINTER(c_uint64)]
     return L
 
 
@@ -690,3 +699,75 @@ class Evaluator:
     def last_counts(self) -> dict:
         """All six counts of the last call, plus ``match`` (uint32 per GT point, NO_MATCH without an inlier) when requested."""
         return dict(self._last) if self._last is not None else None
+
+    # -- the overlap report (erasor_eval_overlap) ------------------------------------------------------------------------------
+    def _overlap(self, gt_ptr, n_gt, est_ptr, n_est, keep_ptr, voxelsize, ptr_kind, dist_ptr, n_sel) -> dict:
+        from . import evaluate
+        ranks = np.asarray(evaluate.overlap_ranks(n_sel) if n_sel else [], dtype=np.uint64)
+        vals = np.empty(len(ranks), dtype=np.float64)
+        o = EvalOverlapC()
+        self._ck(self.L.erasor_eval_overlap(self.h, gt_ptr, n_gt, est_ptr, n_est, keep_ptr, float(voxelsize), ptr_kind,
+                                            ranks.ctypes.data if len(ranks) else None, len(ranks), vals.ctypes.data if len(ranks) else None,
+                                            dist_ptr, ctypes.byref(o)))
+        self._last_overlap = {name: (float(getattr(o, name)) if name == "max" else int(getattr(o, name))) for name, _ in EvalOverlapC._fields_}
+        if o.n != n_sel:
+            raise ErasorError(E_STATE, f"the keep mask selects {o.n} points, not the {n_sel} the ranks were computed for")
+        if not n_sel:
+            return None
+        return evaluate.overlap_from_ranks(n_sel, vals, o.max, (o.below_half, o.below_one, o.below_two), voxelsize)
+
+    def overlap(self, gt, est, keep=None, voxelsize: float = 0.2, want_dist: bool = False):
+        """evaluate.overlap's dict, bit for bit, for host clouds (keep: optional uint8 mask over est).  With want_dist, returns
+        (dict, float64 distance per estimate point, NaN where keep drops it).  The dict is None when nothing is selected; an empty
+        GT gives +inf distances.  last_overlap() has the counts, including est_static / est_dynamic and far_points."""
+        g, e = _cloud(gt), _cloud(est)
+        k = None
+        if keep is not None:
+            k = np.ascontiguousarray(keep, dtype=np.uint8).reshape(-1)
+            if len(k) != len(e):
+                raise ValueError("keep must have one entry per estimate point")
+        n_sel = len(e) if k is None else int(np.count_nonzero(k))
+        dist = np.empty(len(e), dtype=np.float64) if want_dist else None
+        r = self._overlap(g.ctypes.data, len(g), e.ctypes.data, len(e), k.ctypes.data if k is not None else None, voxelsize, PTR_HOST,
+                          dist.ctypes.data if dist is not None and len(dist) else None, n_sel)
+        return (r, dist) if want_dist else r
+
+    def overlap_ptr(self, gt_ptr: int, n_gt: int, est_ptr: int, n_est: int, keep_ptr: int = 0, voxelsize: float = 0.2,
+                    ptr_kind: int = PTR_DEVICE, dist_ptr: int = 0, n_sel: int | None = None):
+        """Raw pointers (device memory with PTR_DEVICE); dist_ptr: optional float64 [n_est] output.  n_sel: how many points keep
+        selects -- without it and with a keep mask, erasor_eval_count_selected counts them first (one pass over the mask)."""
+        if n_sel is None:
+            n_sel = self.count_selected(keep_ptr, n_est, ptr_kind) if keep_ptr else n_est
+        return self._overlap(c_void_p(gt_ptr), n_gt, c_void_p(est_ptr), n_est, c_void_p(keep_ptr) if keep_ptr else None, voxelsize, ptr_kind,
+                             c_void_p(dist_ptr) if dist_ptr else None, n_sel)
+
+    def count_selected(self, keep_ptr: int, n: int, ptr_kind: int = PTR_DEVICE) -> int:
+        """how many of the n keep bytes at keep_ptr are nonzero"""
+        c = c_uint64()
+        self._ck(self.L.erasor_eval_count_selected(self.h, c_void_p(keep_ptr), n, ptr_kind, ctypes.byref(c)))
+        return int(c.value)
+
+    def overlap_map(self, m: "Map", voxelsize: float = 0.2, dist_ptr: int = 0):
+        """The overlap report of a resident map scored in place (GT = the initial map, estimate = its points with keep != 0)."""
+        n = m.size
+        return self.overlap_ptr(m.points_ptr, n, m.points_ptr, n, m.keep_ptr, voxelsize, PTR_DEVICE, dist_ptr)
+
+    def last_overlap(self) -> dict:
+        """The counts of the last overlap call: n, est_static, est_dynamic, below_half / one / two, far_points, max."""
+        return dict(self._last_overlap) if getattr(self, "_last_overlap", None) is not None else None
+
+    def _report(self, d: dict, ov) -> dict:
+        c = self._last_overlap
+        d = dict(d)
+        d["est_static"], d["est_dynamic"] = c["est_static"], c["est_dynamic"]
+        d["overlap"] = ov
+        return d
+
+    def report(self, gt, est, keep=None, voxelsize: float = 0.2) -> dict:
+        """evaluate.report's dict: every column of the runner's table and its overlap dict, from both device calls."""
+        d = self.evaluate(gt, est, keep, voxelsize)
+        return self._report(d, self.overlap(gt, est, keep, voxelsize))
+
+    def report_map(self, m: "Map", voxelsize: float = 0.2) -> dict:
+        d = self.evaluate_map(m, voxelsize)
+        return self._report(d, self.overlap_map(m, voxelsize))

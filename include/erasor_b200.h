@@ -329,6 +329,31 @@ const char* erasor_eval_last_error(erasor_eval_t e);   /* e may be NULL: error o
 int  erasor_evaluate(erasor_eval_t e, const float* gt_xyzi, size_t n_gt, const float* est_xyzi, size_t n_est,
                      const uint8_t* est_keep, double voxelsize, int ptr_kind, uint32_t* match, erasor_eval_counts_t* out);
 
+/* The overlap report of analysis_runner.py (its overlap_report and est_S / est_D): the exact distance d from every selected
+ * estimate point to its nearest GT point, at any range, as sklearn computes it (sqrt((dx*dx + dy*dy) + dz*dz) in double from the
+ * float coordinates), with no bound on d.  Counts are over the selected estimate points. */
+typedef struct {
+    uint64_t n;                  /* selected estimate points */
+    uint64_t est_static;         /* of them, not dynamic (252..259) */
+    uint64_t est_dynamic;
+    uint64_t below_half;         /* d < 0.5 * voxelsize (double comparisons, as numpy makes them) */
+    uint64_t below_one;          /* d < voxelsize */
+    uint64_t below_two;          /* d < 2 * voxelsize */
+    uint64_t far_points;         /* points the far path settled (more than a few cells from every GT point) */
+    double   max;                /* the largest d; NaN when n = 0 */
+} erasor_eval_overlap_t;
+/* Same inputs, pointer kinds and errors as erasor_evaluate (a resident map is scored in place the same way).  ranks / rank_values:
+ * HOST arrays of n_ranks entries; rank_values[r] is the value at 0-based position ranks[r] of the selected points' distances
+ * sorted ascending (ERASOR_E_INVALID when a rank is >= n).  est_dist (nullable, n_est doubles, host or device per ptr_kind): d per
+ * estimate point, NaN where the keep mask drops it.  An empty selection gives n = 0 and no ranks; an empty GT gives d = +inf for
+ * every selected point (sklearn raises on both).  Synchronous. */
+int  erasor_eval_overlap(erasor_eval_t e, const float* gt_xyzi, size_t n_gt, const float* est_xyzi, size_t n_est,
+                         const uint8_t* est_keep, double voxelsize, int ptr_kind, const uint64_t* ranks, size_t n_ranks,
+                         double* rank_values, double* est_dist, erasor_eval_overlap_t* out);
+/* *count = how many of the n keep bytes are nonzero (host or device per ptr_kind; synchronous): the n of erasor_eval_overlap for a
+ * keep mask, so that a caller can compute its ranks before the call. */
+int  erasor_eval_count_selected(erasor_eval_t e, const uint8_t* keep, size_t n, int ptr_kind, uint64_t* count);
+
 #ifdef __cplusplus
 }
 #endif
