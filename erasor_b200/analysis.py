@@ -1,6 +1,7 @@
 """The reference's scripts/analysis_runner.py on the device: prints exactly what it prints for two ASCII PCDs -- the estimate -> GT
-distance report, then the PR / RR table -- computed by capi.Evaluator (erasor_evaluate + erasor_eval_overlap).
---host computes it with sklearn instead (erasor_b200.evaluate), for machines without a GPU.
+distance report, then the PR / RR table -- computed by capi.Evaluator (erasor_evaluate + erasor_eval_overlap) on clouds read by
+capi.PcdCodec (erasor_pcd_parse_ascii, bit-identical to read_pcd_ascii).
+--host reads with read_pcd_ascii and computes with sklearn instead (erasor_b200.evaluate), for machines without a GPU.
 
     python -m erasor_b200.analysis --gt gt.pcd --est est.pcd [--voxelsize 0.2] [--host] [--device N]
 """
@@ -24,11 +25,13 @@ def main(argv=None) -> int:
     for path in (args.gt, args.est):
         if not os.path.isfile(path):
             p.error(f"no such file: {path}")
-    gt, est = E.read_pcd_ascii(args.gt), E.read_pcd_ascii(args.est)
     if args.host:
+        gt, est = E.read_pcd_ascii(args.gt), E.read_pcd_ascii(args.est)
         r = E.report(gt, est, args.voxelsize)
     else:
         from . import capi
+        with capi.PcdCodec(device=args.device) as codec:
+            gt, est = codec.read(args.gt), codec.read(args.est)
         with capi.Evaluator(device=args.device) as ev:
             r = ev.report(gt, est, voxelsize=args.voxelsize)
     sys.stdout.write(E.format_report(r, args.voxelsize, args.gt, args.est))

@@ -37,6 +37,7 @@ EXPORTS = [
     "erasor_updater_erasor", "erasor_updater_kernel_launch_count", "erasor_updater_get_fused_profile",
     "erasor_eval_create", "erasor_eval_destroy", "erasor_eval_last_error", "erasor_evaluate", "erasor_eval_overlap",
     "erasor_eval_count_selected",
+    "erasor_pcd_create", "erasor_pcd_destroy", "erasor_pcd_last_error", "erasor_pcd_parse_ascii", "erasor_pcd_format_ascii",
 ]
 NO_MATCH = 0xFFFFFFFF        # erasor_evaluate's match entry of a GT point without an inlier
 
@@ -49,6 +50,12 @@ class EvalCountsC(ctypes.Structure):
 class EvalOverlapC(ctypes.Structure):
     """erasor_eval_overlap_t"""
     _fields_ = [(name, c_uint64) for name in ("n", "est_static", "est_dynamic", "below_half", "below_one", "below_two", "far_points")] + [("max", c_double)]
+
+
+class PcdInfoC(ctypes.Structure):
+    """erasor_pcd_info_t"""
+    _fields_ = [(name, c_uint64) for name in ("points", "rows", "slow_tokens", "error_line", "header_lines")] + [("fields", c_uint32),
+                                                                                                              ("has_intensity", c_uint32)]
 
 
 class UpdaterParamsC(ctypes.Structure):
@@ -158,6 +165,13 @@ def _load():
     L.erasor_eval_overlap.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_double, c_int, c_void_p, c_size_t, c_void_p,
                                       c_void_p, POINTER(EvalOverlapC)]
     L.erasor_eval_count_selected.argtypes = [c_void_p, c_void_p, c_size_t, c_int, POINTER(c_uint64)]
+    L.erasor_pcd_create.argtypes = [c_int, POINTER(c_void_p)]
+    L.erasor_pcd_destroy.restype = None
+    L.erasor_pcd_destroy.argtypes = [c_void_p]
+    L.erasor_pcd_last_error.restype = c_char_p
+    L.erasor_pcd_last_error.argtypes = [c_void_p]
+    L.erasor_pcd_parse_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdInfoC)]
+    L.erasor_pcd_format_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t)]
     return L
 
 
@@ -771,3 +785,104 @@ class Evaluator:
     def report_map(self, m: "Map", voxelsize: float = 0.2) -> dict:
         d = self.evaluate_map(m, voxelsize)
         return self._report(d, self.overlap_map(m, voxelsize))
+
+
+class PcdCodec:
+    """One ``erasor_pcd_t``: ASCII PCD files read and written on the device (DESIGN.md section 12).  ``parse`` / ``read`` give what
+    ``evaluate.read_pcd_ascii`` gives, bit for bit (including its KeyError for a file without x, y, z or intensity); ``format`` /
+    ``write`` give the bytes ``evaluate.write_pcd_ascii`` writes, except that NaN is written "nan" whatever its sign.  Files are read
+    and written as raw bytes."""
+
+    def __init__(self, device: int = 0):
+        self.L = lib()
+        self.device = device
+        h = c_void_p()
+        rc = self.L.erasor_pcd_create(device, ctypes.byref(h))
+        if rc != OK:
+            raise ErasorError(rc, (self.L.erasor_pcd_last_error(None) or b"").decode())
+        self.h = h
+        self._info = None
+
+    def _ck(self, rc: int):
+        if rc != OK:
+            raise ErasorError(rc, (self.L.erasor_pcd_last_error(self.h) or b"").decode())
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.erasor_pcd_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def _call_parse(self, ptr, n_bytes, kind, out_ptr, cap, out_kind, require_intensity):
+        n, info = c_size_t(0), PcdInfoC()
+        rc = self.L.erasor_pcd_parse_ascii(self.h, ptr, n_bytes, kind, out_ptr, cap, out_kind, ctypes.byref(n), ctypes.byref(info))
+        self._info = {name: int(getattr(info, name)) for name, _ in PcdInfoC._fields_}
+        for bit, name in enumerate(("x", "y", "z", "intensity")):
+            if info.header_lines and not (info.fields >> bit) & 1 and (bit < 3 or require_intensity):
+                raise KeyError(name)                  # read_pcd_ascii's error for a missing column of a header it could read
+        self._ck(rc)
+        return n.value
+
+    def parse(self, data, device_out: bool = False, require_intensity: bool = True):
+        """data: the whole file -- bytes-like (host) or a CUDA uint8 tensor.  Returns float32 [rows, 4] x y z intensity: a numpy
+        array, or a CUDA tensor with device_out.  require_intensity=False reads a file without intensity as the C++ reader does
+        (intensity 0) instead of raising KeyError."""
+        if hasattr(data, "is_cuda") and data.is_cuda:
+            ptr, nb, kind, keep = c_void_p(data.data_ptr()), data.numel() * data.element_size(), PTR_DEVICE, data
+        else:
+            keep = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data).view(np.uint8)
+            ptr, nb, kind = c_void_p(keep.ctypes.data if keep.size else 0), keep.size, PTR_HOST
+        pts = self._call_parse(ptr, nb, kind, None, 0, PTR_HOST, require_intensity)
+        if device_out:
+            import torch
+            out = torch.empty((max(pts, 1), 4), dtype=torch.float32, device=f"cuda:{self.device}")
+            rows = self._call_parse(ptr, nb, kind, c_void_p(out.data_ptr()), pts, PTR_DEVICE, require_intensity)
+        else:
+            out = np.empty((max(pts, 1), 4), dtype=np.float32)
+            rows = self._call_parse(ptr, nb, kind, c_void_p(out.ctypes.data), pts, PTR_HOST, require_intensity)
+        del keep
+        return out[:rows]
+
+    def read(self, path: str, device_out: bool = False, require_intensity: bool = True):
+        with open(path, "rb") as f:
+            data = f.read()
+        return self.parse(data, device_out, require_intensity)
+
+    def last_info(self) -> dict:
+        """points, rows, slow_tokens, error_line, header_lines, fields and has_intensity of the last parse"""
+        return dict(self._info) if self._info is not None else None
+
+    def _format(self, xyzi) -> np.ndarray:
+        if hasattr(xyzi, "is_cuda") and xyzi.is_cuda:
+            if str(xyzi.dtype) != "torch.float32" or xyzi.dim() != 2 or xyzi.shape[1] != 4 or not xyzi.is_contiguous():
+                raise ValueError("device clouds are contiguous float32 [n,4] tensors")
+            ptr, n, kind, keep = c_void_p(xyzi.data_ptr()), xyzi.shape[0], PTR_DEVICE, xyzi
+        else:
+            keep = _cloud(xyzi)
+            ptr, n, kind = c_void_p(keep.ctypes.data if len(keep) else 0), len(keep), PTR_HOST
+        size = c_size_t(0)
+        self._ck(self.L.erasor_pcd_format_ascii(self.h, ptr, n, kind, None, 0, PTR_HOST, ctypes.byref(size)))
+        out = np.empty(size.value, dtype=np.uint8)
+        self._ck(self.L.erasor_pcd_format_ascii(self.h, ptr, n, kind, c_void_p(out.ctypes.data), size.value, PTR_HOST, ctypes.byref(size)))
+        del keep
+        return out
+
+    def format(self, xyzi) -> bytes:
+        """the whole file for a float32 [n, 4] cloud (numpy, or a CUDA tensor)"""
+        return self._format(xyzi).tobytes()
+
+    def write(self, path: str, xyzi):
+        out = self._format(xyzi)
+        with open(path, "wb") as f:
+            f.write(memoryview(out))

@@ -1,11 +1,13 @@
-// host_selftest.cpp -- compiles binning.h for the HOST so that the CPU test-suite (-m "not gpu")
-// can check the exact-threshold bin arithmetic against the oracle without a GPU.
+// host_selftest.cpp -- compiles binning.h and pcd_codec.h for the HOST so that the CPU test-suite (-m "not gpu")
+// can check the exact-threshold bin arithmetic against the oracle, and the ASCII PCD codec's per-token arithmetic against
+// numpy and Python, without a GPU.
 // This library is loaded by tests only; the product API (erasor_capi.cu) has no host compute path.
 #include <cstdint>
 #include <cstring>
 #include <string>
 
 #include "binning_tables.h"
+#include "pcd_codec.h"
 #include "pose_math.h"
 
 extern "C" {
@@ -73,6 +75,33 @@ int erasor_hostcheck_guards(const erasor_params_t* p, float* ring_guard, float* 
     if (erasor::build_bin_tables(*p, T, err) != 0) return -1;
     std::memcpy(ring_guard, T.ring_guard.data(), sizeof(float) * T.ring_guard.size());
     smax_lo_hi[0] = T.smax_lo; smax_lo_hi[1] = T.smax_hi;
+    return 0;
+}
+
+// pcd_codec.h's parse on n tokens, token k = text[offs[k] .. offs[k + 1]): bits[k] = the float's bit pattern (0 when invalid),
+// kind[k] = 0 fast path, 1 big-integer path, 2 invalid.  want_value = 0 runs the check alone, as the kernel does for a column it
+// does not keep (kind 0 or 2, bits 0).
+int erasor_hostcheck_pcd_parse(const uint8_t* text, const uint64_t* offs, size_t n, int want_value, uint32_t* bits, int32_t* kind) {
+    pcd::Big D, A, B;
+    for (size_t k = 0; k < n; ++k) {
+        const uint8_t* s = text + offs[k];
+        const uint64_t len = offs[k + 1] - offs[k];
+        const pcd::TokenScan r = pcd::scan_token(s, len, want_value != 0);
+        kind[k] = r.kind;
+        float f = 0.0f;
+        if (r.kind == pcd::TOK_OK && want_value) f = (float)r.value;
+        else if (r.kind == pcd::TOK_SLOW) {
+            const double v = pcd::parse_slow_abs(s, len, D, A, B);
+            f = (float)(r.neg ? -v : v);
+        }
+        bits[k] = pcd::float_to_bits(f);
+    }
+    return 0;
+}
+
+// pcd_codec.h's "%.8g" on n floats: value k's text at out[16 k ..], its length in lens[k]
+int erasor_hostcheck_pcd_format(const float* vals, size_t n, char* out, int32_t* lens) {
+    for (size_t k = 0; k < n; ++k) lens[k] = pcd::format_g8(vals[k], out + 16 * k);
     return 0;
 }
 }

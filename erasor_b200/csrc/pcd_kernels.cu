@@ -1,0 +1,618 @@
+// pcd_kernels.cu -- the ASCII PCD codec on the device (DESIGN.md section 12): erasor_pcd_parse_ascii turns the text of a PCD file
+// into float4 x y z intensity, erasor_pcd_format_ascii turns a cloud into the text write_pcd_ascii / save_pcd_ascii write.  The
+// per-token arithmetic is pcd_codec.h, which the CPU test-suite also runs on the host.
+//
+// Parse: the header (a few hundred bytes) is read on the host.  On the device, over the data bytes:
+//   1. k_pcd_nl_count     line ends per 64 KB chunk (16-byte loads; '\n' or a lone '\r', as Python's universal newlines read
+//                         them), then an exclusive scan of the chunk counts;
+//   2. k_pcd_nl_scatter   the start of every line, in order (a CTA-wide scan per 4 KB tile);
+//   3. k_pcd_classify     1 for a data line (anything but blanks before the end or a '#'), then an exclusive scan: the row of a line;
+//   4. k_pcd_parse        one thread per line: split on blanks, check every token against numpy's loadtxt grammar and the token count
+//                         against FIELDS, parse the kept columns on the fast path; the first bad line wins an atomicMin;
+//   5. k_pcd_parse_slow   one thread per row holding a token the fast path left (limbs in local memory), only when there is one.
+// Format: k_pcd_fmt_len gives every line's length, an exclusive scan its offset, k_pcd_fmt_write writes it after the header.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdio>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/erasor_b200.h"
+#include "pcd_codec.h"
+
+namespace {
+constexpr int kThreads = 256;
+constexpr uint64_t kTile = 16ull * kThreads;          // bytes per CTA iteration of the newline passes
+constexpr uint64_t kChunk = 16ull * kTile;            // bytes per CTA of the newline passes
+constexpr int kScanItems = 4;
+constexpr uint64_t kScanTile = (uint64_t)kScanItems * kThreads;
+constexpr int kMaxFields = 64;
+constexpr int kSlowThreads = 64;
+constexpr int kMaxLine = 4 * 15 + 4;                  // "-1.2345678e-45" is the longest value: 4 values, 3 blanks and '\n'
+
+struct Fields {
+    int n;
+    int8_t slot[kMaxFields];                          // field k -> 0..3 (x, y, z, intensity) or -1 (validated, not kept)
+};
+
+struct PcdStats {
+    unsigned long long err;                           // (0-based data line << 1) | (1: wrong token count), ~0 when none
+    unsigned long long slow_tokens;
+    unsigned long long slow_rows;
+    unsigned long long total;                         // scan totals read back by the host
+};
+
+// the data bytes in a 16-byte aligned frame: byte j of the data is base[j + o], o = the data pointer's misalignment
+struct Text {
+    const uint8_t* base;
+    uint64_t o, len;
+    __device__ __forceinline__ uint8_t at(uint64_t j) const { return base[j + o]; }
+};
+
+// CTA-wide exclusive scan of one value per thread; *total gets the sum.  s: 32 + 1 entries.
+__device__ __forceinline__ uint64_t cta_excl_scan(uint64_t v, uint64_t* s, uint64_t& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    uint64_t x = v;
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, x, d);
+        if (lane >= d) x += y;
+    }
+    if (lane == 31) s[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        uint64_t w = lane < nw ? s[lane] : 0;
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, w, d);
+            if (lane >= d) w += y;
+        }
+        if (lane < nw) s[lane] = w;
+        if (lane == 31) s[32] = w;
+    }
+    __syncthreads();
+    const uint64_t r = x - v + (warp ? s[warp - 1] : 0);
+    total = s[32];
+    __syncthreads();
+    return r;
+}
+
+// the 16 bytes of the frame at f (f % 16 == 0); bytes outside the data read as 0
+__device__ __forceinline__ void load16(const Text& t, uint64_t f, uint8_t b[16]) {
+    if (f >= t.o && f + 16 <= t.o + t.len) {
+        const uint4 v = *reinterpret_cast<const uint4*>(t.base + f);
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+        for (int k = 0; k < 16; ++k) b[k] = (uint8_t)(w[k >> 2] >> (8 * (k & 3)));
+    } else {
+        for (int k = 0; k < 16; ++k) b[k] = (f + k >= t.o && f + k < t.o + t.len) ? t.base[f + k] : 0;
+    }
+}
+
+__device__ __forceinline__ uint8_t byte_at(const Text& t, uint64_t f) { return (f >= t.o && f < t.o + t.len) ? t.base[f] : 0; }
+
+// Line ends as Python's universal newlines read them (read_pcd_ascii opens the file in text mode): '\n', and a '\r' that no '\n'
+// follows.  The '\r' of "\r\n" stays in its line as a blank.  after: the byte following the 16.
+__device__ __forceinline__ bool ends_line(const uint8_t b[16], int k, uint8_t after) {
+    return b[k] == '\n' || (b[k] == '\r' && (k < 15 ? b[k + 1] : after) != '\n');
+}
+
+__global__ void __launch_bounds__(kThreads) k_pcd_nl_count(Text t, uint32_t* cnt) {
+    __shared__ uint32_t s;
+    if (threadIdx.x == 0) s = 0;
+    __syncthreads();
+    const uint64_t end = t.o + t.len;
+    uint32_t c = 0;
+    for (uint64_t f = (uint64_t)blockIdx.x * kChunk + 16ull * threadIdx.x; f < (uint64_t)(blockIdx.x + 1) * kChunk && f < end; f += kTile) {
+        uint8_t b[16];
+        load16(t, f, b);
+        const uint8_t after = byte_at(t, f + 16);
+        for (int k = 0; k < 16; ++k) c += ends_line(b, k, after);
+    }
+    atomicAdd(&s, c);
+    __syncthreads();
+    if (threadIdx.x == 0) cnt[blockIdx.x] = s;
+}
+
+// line_start[1 + k] = the data offset after the k-th line end
+__global__ void __launch_bounds__(kThreads) k_pcd_nl_scatter(Text t, const uint64_t* chunk_off, uint64_t* line_start) {
+    __shared__ uint64_t s[33];
+    const uint64_t end = t.o + t.len;
+    uint64_t run = chunk_off[blockIdx.x];
+    for (uint64_t tile = (uint64_t)blockIdx.x * kChunk; tile < (uint64_t)(blockIdx.x + 1) * kChunk && tile < end; tile += kTile) {
+        const uint64_t f = tile + 16ull * threadIdx.x;
+        uint8_t b[16];
+        if (f < end) load16(t, f, b); else for (int k = 0; k < 16; ++k) b[k] = 0;
+        const uint8_t after = f < end ? byte_at(t, f + 16) : 0;
+        uint32_t c = 0;
+        for (int k = 0; k < 16; ++k) c += ends_line(b, k, after);
+        uint64_t tot;
+        uint64_t at = run + cta_excl_scan(c, s, tot);
+        for (int k = 0; k < 16; ++k)
+            if (ends_line(b, k, after)) line_start[1 + at++] = f + k - t.o + 1;
+        run += tot;
+    }
+}
+
+__device__ __forceinline__ uint64_t line_end(const Text& t, const uint64_t* line_start, uint64_t nlines, uint64_t i) {
+    return i + 1 < nlines ? line_start[i + 1] - 1 : t.len;
+}
+
+__global__ void __launch_bounds__(kThreads) k_pcd_classify(Text t, const uint64_t* line_start, uint64_t nlines, uint32_t* flag) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nlines; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint64_t p = line_start[i];
+        const uint64_t e = line_end(t, line_start, nlines, i);
+        while (p < e && pcd::is_ws(t.at(p))) ++p;
+        flag[i] = (p < e && t.at(p) != '#') ? 1u : 0u;
+    }
+}
+
+// exclusive scan of n uint32 into uint64: per-tile sums, one CTA over the tile sums (sums[ntiles] = total), per-tile apply
+__global__ void __launch_bounds__(kThreads) k_pcd_scan_tiles(const uint32_t* in, uint64_t n, uint64_t* sums) {
+    __shared__ uint64_t s[33];
+    const uint64_t i0 = (uint64_t)blockIdx.x * kScanTile + (uint64_t)threadIdx.x * kScanItems;
+    uint64_t v = 0;
+    for (int k = 0; k < kScanItems; ++k) if (i0 + k < n) v += in[i0 + k];
+    uint64_t tot;
+    cta_excl_scan(v, s, tot);
+    if (threadIdx.x == 0) sums[blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(kThreads) k_pcd_scan_top(uint64_t* sums, uint64_t ntiles) {
+    __shared__ uint64_t s[33];
+    uint64_t run = 0;
+    for (uint64_t b = 0; b < ntiles; b += kThreads) {
+        const uint64_t i = b + threadIdx.x;
+        const uint64_t v = i < ntiles ? sums[i] : 0;
+        uint64_t tot;
+        const uint64_t x = cta_excl_scan(v, s, tot);
+        if (i < ntiles) sums[i] = run + x;
+        run += tot;
+    }
+    if (threadIdx.x == 0) sums[ntiles] = run;
+}
+
+__global__ void __launch_bounds__(kThreads) k_pcd_scan_apply(const uint32_t* in, uint64_t n, const uint64_t* sums, uint64_t* out) {
+    __shared__ uint64_t s[33];
+    const uint64_t i0 = (uint64_t)blockIdx.x * kScanTile + (uint64_t)threadIdx.x * kScanItems;
+    uint32_t v[kScanItems];
+    uint64_t sum = 0;
+    for (int k = 0; k < kScanItems; ++k) { v[k] = i0 + k < n ? in[i0 + k] : 0u; sum += v[k]; }
+    uint64_t tot;
+    uint64_t at = sums[blockIdx.x] + cta_excl_scan(sum, s, tot);
+    for (int k = 0; k < kScanItems; ++k) {
+        if (i0 + k < n) out[i0 + k] = at;
+        at += v[k];
+    }
+}
+
+// One data line: its tokens through scan_token.  Returns false when the line is invalid (*wrong_count: the token count is not
+// f.n); vals gets the kept columns that the fast path settled, *n_slow the kept tokens it left to the slow path.
+__device__ __forceinline__ bool parse_line(const Text& t, uint64_t p, uint64_t e, const Fields& f, float vals[4], int* n_slow,
+                                           bool* wrong_count) {
+    int k = 0;
+    *n_slow = 0;
+    *wrong_count = false;
+    uint8_t tok[32];
+    while (true) {
+        while (p < e && pcd::is_ws(t.at(p))) ++p;
+        if (p >= e || t.at(p) == '#') break;
+        const uint64_t a = p;
+        while (p < e && !pcd::is_ws(t.at(p)) && t.at(p) != '#') ++p;
+        if (k >= f.n) { *wrong_count = true; return false; }
+        const int slot = f.slot[k];
+        const uint64_t len = p - a;
+        pcd::TokenScan r;
+        if (len <= sizeof(tok)) {
+            for (uint64_t j = 0; j < len; ++j) tok[j] = t.at(a + j);
+            r = pcd::scan_token(tok, len, slot >= 0);
+        } else {
+            r = pcd::scan_token(t.base + t.o + a, len, slot >= 0);
+        }
+        if (r.kind == pcd::TOK_INVALID) return false;
+        if (slot >= 0) {
+            if (r.kind == pcd::TOK_SLOW) ++*n_slow;
+            else vals[slot] = (float)r.value;
+        }
+        ++k;
+    }
+    if (k != f.n) { *wrong_count = true; return false; }
+    return true;
+}
+
+__global__ void __launch_bounds__(kThreads) k_pcd_parse(Text t, const uint64_t* line_start, uint64_t nlines, uint32_t* flag,
+                                                        const uint64_t* row_of_line, uint64_t points, Fields f, float4* out, PcdStats* st) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nlines; i += (uint64_t)gridDim.x * blockDim.x) {
+        if (!flag[i]) continue;
+        const uint64_t row = row_of_line[i];
+        if (row >= points) continue;                  // np.loadtxt(max_rows = POINTS) neither reads nor checks the rest
+        float v[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+        int n_slow;
+        bool wrong;
+        if (!parse_line(t, line_start[i], line_end(t, line_start, nlines, i), f, v, &n_slow, &wrong)) {
+            atomicMin(&st->err, (unsigned long long)((i << 1) | (wrong ? 1u : 0u)));
+            continue;
+        }
+        out[row] = make_float4(v[0], v[1], v[2], v[3]);
+        if (n_slow) {
+            flag[i] = 2;
+            atomicAdd(&st->slow_tokens, (unsigned long long)n_slow);
+            atomicAdd(&st->slow_rows, 1ull);
+        }
+    }
+}
+
+// the rows k_pcd_parse flagged 2: their kept tokens that the fast path left, by exact big-integer arithmetic
+__global__ void __launch_bounds__(kSlowThreads) k_pcd_parse_slow(Text t, const uint64_t* line_start, uint64_t nlines, const uint32_t* flag,
+                                                                 const uint64_t* row_of_line, Fields f, float4* out) {
+    pcd::Big D, A, B;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nlines; i += (uint64_t)gridDim.x * blockDim.x) {
+        if (flag[i] != 2) continue;
+        float* o = reinterpret_cast<float*>(out + row_of_line[i]);
+        uint64_t p = line_start[i];
+        const uint64_t e = line_end(t, line_start, nlines, i);
+        for (int k = 0; k < f.n; ++k) {
+            while (p < e && pcd::is_ws(t.at(p))) ++p;
+            const uint64_t a = p;
+            while (p < e && !pcd::is_ws(t.at(p)) && t.at(p) != '#') ++p;
+            const int slot = f.slot[k];
+            if (slot < 0) continue;
+            const uint8_t* s = t.base + t.o + a;
+            const pcd::TokenScan r = pcd::scan_token(s, p - a, true);
+            if (r.kind != pcd::TOK_SLOW) continue;
+            const double v = pcd::parse_slow_abs(s, p - a, D, A, B);
+            o[slot] = (float)(r.neg ? -v : v);
+        }
+    }
+}
+
+__device__ __forceinline__ int format_point(float4 q, char* buf) {
+    int n = pcd::format_g8(q.x, buf);
+    buf[n++] = ' ';
+    n += pcd::format_g8(q.y, buf + n);
+    buf[n++] = ' ';
+    n += pcd::format_g8(q.z, buf + n);
+    buf[n++] = ' ';
+    n += pcd::format_g8(q.w, buf + n);
+    buf[n++] = '\n';
+    return n;
+}
+
+__global__ void __launch_bounds__(kThreads) k_pcd_fmt_len(const float4* pts, uint64_t n, uint32_t* len) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        char buf[kMaxLine];
+        len[i] = (uint32_t)format_point(pts[i], buf);
+    }
+}
+
+__global__ void __launch_bounds__(kThreads) k_pcd_fmt_write(const float4* pts, uint64_t n, const uint64_t* off, uint8_t* text) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        char buf[kMaxLine];
+        const int m = format_point(pts[i], buf);
+        uint8_t* d = text + off[i];
+        for (int k = 0; k < m; ++k) d[k] = (uint8_t)buf[k];
+    }
+}
+
+struct DevBuf {
+    void* p = nullptr; size_t cap = 0;
+    cudaError_t ensure(size_t bytes) {
+        if (bytes <= cap) return cudaSuccess;
+        if (p) { cudaFree(p); p = nullptr; cap = 0; }
+        const size_t want = bytes + bytes / 8 + 4096;
+        const cudaError_t e = cudaMalloc(&p, want);
+        if (e == cudaSuccess) cap = want;
+        return e;
+    }
+    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+thread_local std::string g_pcd_err;
+
+// what the host reads of the header
+struct Header {
+    std::vector<std::string> fields;
+    std::vector<std::string> counts;
+    unsigned long long points = 0;
+    bool have_points = false, have_data = false;
+    std::string data;
+    uint64_t data_off = 0;       // first byte after the DATA line
+    uint64_t lines = 0;          // lines before data_off
+};
+
+bool blank(char c) { return pcd::is_ws((uint8_t)c); }
+
+// header lines up to and including DATA; false when the text ends before a DATA line
+bool parse_header(const char* s, uint64_t n, Header& h) {
+    uint64_t p = 0;
+    while (p < n) {
+        uint64_t e = p;                              // the line ends at '\n', "\r\n" or a lone '\r' (universal newlines)
+        while (e < n && s[e] != '\n' && s[e] != '\r') ++e;
+        std::vector<std::string> tok;
+        for (uint64_t q = p; q < e;) {
+            while (q < e && blank(s[q])) ++q;
+            const uint64_t a = q;
+            while (q < e && !blank(s[q])) ++q;
+            if (q > a) tok.emplace_back(s + a, q - a);
+        }
+        ++h.lines;
+        const uint64_t next = e >= n ? n : (s[e] == '\r' && e + 1 < n && s[e + 1] == '\n') ? e + 2 : e + 1;
+        if (!tok.empty()) {
+            if (tok[0] == "FIELDS") h.fields.assign(tok.begin() + 1, tok.end());
+            else if (tok[0] == "COUNT") h.counts.assign(tok.begin() + 1, tok.end());
+            else if (tok[0] == "POINTS" && tok.size() > 1) {
+                char* end = nullptr;
+                h.points = std::strtoull(tok[1].c_str(), &end, 10);
+                h.have_points = end && *end == 0 && tok[1][0] != '-';
+            } else if (tok[0] == "DATA") {
+                h.have_data = true;
+                h.data = tok.size() > 1 ? tok[1] : std::string();
+                h.data_off = next;
+                return true;
+            }
+        }
+        p = next;
+    }
+    return false;
+}
+
+uint32_t blocks_for(uint64_t n, int per, int cap) { return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + per - 1) / per, (uint64_t)cap)); }
+}  // namespace
+
+struct erasor_pcd_ctx {
+    int device = 0;
+    cudaStream_t st = nullptr;
+    std::string err;
+    DevBuf text, chunk_cnt, chunk_off, lines, flags, rows, sums, out, stats;   // parse
+    DevBuf pts, lens, offs, ftext;                                              // format
+    PcdStats* h_stats = nullptr;                                                // pinned
+    int sm_count = 132;
+    // erasor_pcd_format_ascii's text of its last call, kept for a following call with the same input
+    bool cached = false;
+    const float* c_ptr = nullptr;
+    size_t c_n = 0;
+    int c_kind = -1;
+    uint64_t c_len = 0;
+};
+
+namespace {
+#define PCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { p->err = std::string(#call) + ": " + cudaGetErrorString(e__); return ERASOR_E_CUDA; } } while (0)
+
+int fail(erasor_pcd_t p, int rc, const std::string& msg) { p->err = msg; return rc; }
+
+// exclusive scan of n uint32 at in into out (n uint64); *total = the sum (synchronous read-back when total != nullptr)
+int scan_u32(erasor_pcd_t p, const uint32_t* in, uint64_t n, uint64_t* out, uint64_t* total) {
+    const uint64_t ntiles = (n + kScanTile - 1) / kScanTile;
+    PCK(p->sums.ensure(sizeof(uint64_t) * (ntiles + 1)));
+    uint64_t* sums = p->sums.as<uint64_t>();
+    k_pcd_scan_tiles<<<(unsigned)ntiles, kThreads, 0, p->st>>>(in, n, sums);
+    k_pcd_scan_top<<<1, kThreads, 0, p->st>>>(sums, ntiles);
+    k_pcd_scan_apply<<<(unsigned)ntiles, kThreads, 0, p->st>>>(in, n, sums, out);
+    PCK(cudaGetLastError());
+    if (total) {
+        PCK(cudaMemcpyAsync(total, sums + ntiles, sizeof(uint64_t), cudaMemcpyDeviceToHost, p->st));
+        PCK(cudaStreamSynchronize(p->st));
+    }
+    return ERASOR_OK;
+}
+
+const char* kHeadFmt = "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z intensity\nSIZE 4 4 4 4\nTYPE F F F F\n"
+                       "COUNT 1 1 1 1\nWIDTH %zu\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS %zu\nDATA ascii\n";
+}  // namespace
+
+extern "C" {
+
+int erasor_pcd_create(int device, erasor_pcd_t* out) {
+    if (!out) { g_pcd_err = "null argument"; return ERASOR_E_INVALID; }
+    *out = nullptr;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); g_pcd_err = "no CUDA device"; return ERASOR_E_CUDA; }
+    if (device < 0 || device >= ndev) { g_pcd_err = "device index out of range"; return ERASOR_E_INVALID; }
+    erasor_pcd_ctx* p = new erasor_pcd_ctx();
+    p->device = device;
+    cudaError_t c = cudaSetDevice(device);
+    if (c == cudaSuccess) c = cudaStreamCreateWithFlags(&p->st, cudaStreamNonBlocking);
+    if (c == cudaSuccess) c = cudaMallocHost(&p->h_stats, sizeof(PcdStats));
+    if (c == cudaSuccess) c = p->stats.ensure(sizeof(PcdStats));
+    if (c == cudaSuccess) c = cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, device);
+    if (c != cudaSuccess) {
+        g_pcd_err = std::string("erasor_pcd_create: ") + cudaGetErrorString(c);
+        erasor_pcd_destroy(p);
+        return ERASOR_E_CUDA;
+    }
+    *out = p;
+    return ERASOR_OK;
+}
+
+void erasor_pcd_destroy(erasor_pcd_t p) {
+    if (!p) return;
+    cudaSetDevice(p->device);
+    if (p->st) cudaStreamSynchronize(p->st);
+    for (DevBuf* b : {&p->text, &p->chunk_cnt, &p->chunk_off, &p->lines, &p->flags, &p->rows, &p->sums, &p->out, &p->stats, &p->pts,
+                      &p->lens, &p->offs, &p->ftext}) b->release();
+    if (p->h_stats) cudaFreeHost(p->h_stats);
+    if (p->st) cudaStreamDestroy(p->st);
+    delete p;
+}
+
+const char* erasor_pcd_last_error(erasor_pcd_t p) { return p ? p->err.c_str() : g_pcd_err.c_str(); }
+
+int erasor_pcd_parse_ascii(erasor_pcd_t p, const char* text, size_t len, int text_kind, float* out_xyzi, size_t cap, int out_kind,
+                           size_t* n, erasor_pcd_info_t* info) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    p->cached = false;
+    if (info) *info = erasor_pcd_info_t{};
+    if (!n || (len && !text)) return fail(p, ERASOR_E_INVALID, "null argument");
+    if ((text_kind != ERASOR_PTR_HOST && text_kind != ERASOR_PTR_DEVICE) || (out_kind != ERASOR_PTR_HOST && out_kind != ERASOR_PTR_DEVICE))
+        return fail(p, ERASOR_E_INVALID, "text_kind and out_kind must be ERASOR_PTR_HOST or ERASOR_PTR_DEVICE");
+    PCK(cudaSetDevice(p->device));
+    *n = 0;
+    erasor_pcd_info_t inf{};
+    // 1. the header, on the host (from a device text, growing prefixes until the DATA line is in)
+    Header h;
+    bool found = false;
+    if (text_kind == ERASOR_PTR_HOST) {
+        found = parse_header(text, len, h);
+    } else {
+        std::vector<char> pre;
+        for (uint64_t m = std::min<uint64_t>(len, 1 << 16);; m = std::min<uint64_t>(len, 4 * m)) {
+            pre.resize(m);
+            PCK(cudaMemcpy(pre.data(), text, m, cudaMemcpyDeviceToHost));
+            h = Header();
+            found = parse_header(pre.data(), m, h) && (h.data_off < m || m == len);   // the DATA line's end lies inside the prefix
+            if (found || m == len) break;
+        }
+    }
+    if (!found) return fail(p, ERASOR_E_INVALID, "no DATA line in the PCD header");
+    for (size_t k = 0; k < h.fields.size(); ++k) {
+        const std::string& f = h.fields[k];
+        if (f == "x") inf.fields |= 1u; else if (f == "y") inf.fields |= 2u; else if (f == "z") inf.fields |= 4u; else if (f == "intensity") inf.fields |= 8u;
+    }
+    inf.has_intensity = (inf.fields & 8u) ? 1u : 0u;
+    inf.points = h.points;
+    inf.header_lines = h.lines;
+    if (info) *info = inf;
+    if (h.data != "ascii") return fail(p, ERASOR_E_UNSUPPORTED, "DATA " + h.data + ": only ASCII PCDs are parsed on the device");
+    for (const std::string& c : h.counts)
+        if (c != "1") return fail(p, ERASOR_E_UNSUPPORTED, "COUNT " + c + ": only fields with COUNT 1 are supported");
+    if ((inf.fields & 7u) != 7u) return fail(p, ERASOR_E_INVALID, "the PCD's FIELDS lack x, y or z");
+    if (h.fields.size() > (size_t)kMaxFields) return fail(p, ERASOR_E_UNSUPPORTED, "more than 64 FIELDS");
+    if (!h.have_points) return fail(p, ERASOR_E_INVALID, "no valid POINTS line in the PCD header");
+    if (!out_xyzi) { *n = (size_t)h.points; return ERASOR_OK; }
+    if (cap < h.points) return fail(p, ERASOR_E_CAPACITY, "out_xyzi holds fewer points than the header's POINTS");
+    if (out_kind == ERASOR_PTR_DEVICE && (reinterpret_cast<uintptr_t>(out_xyzi) & 15u))
+        return fail(p, ERASOR_E_INVALID, "device clouds must be 16-byte aligned (one float4 per point)");
+    Fields f{};
+    f.n = (int)h.fields.size();
+    for (int k = 0; k < f.n; ++k) {
+        const std::string& s = h.fields[k];
+        f.slot[k] = s == "x" ? 0 : s == "y" ? 1 : s == "z" ? 2 : s == "intensity" ? 3 : -1;
+    }
+    const uint64_t dlen = len - h.data_off;
+    if (!dlen || !h.points) { if (info) *info = inf; return ERASOR_OK; }
+
+    // 2. the data bytes on the device, in a 16-byte aligned frame
+    Text t{};
+    if (text_kind == ERASOR_PTR_HOST) {
+        PCK(p->text.ensure(dlen));
+        PCK(cudaMemcpyAsync(p->text.p, text + h.data_off, dlen, cudaMemcpyHostToDevice, p->st));
+        t.base = p->text.as<uint8_t>();
+        t.o = 0;
+    } else {
+        const uintptr_t a = reinterpret_cast<uintptr_t>(text) + h.data_off;
+        t.base = reinterpret_cast<const uint8_t*>(a & ~uintptr_t(15));
+        t.o = a & 15u;
+    }
+    t.len = dlen;
+
+    // 3. line structure
+    const uint64_t nchunks = (t.o + dlen + kChunk - 1) / kChunk;
+    PCK(p->chunk_cnt.ensure(sizeof(uint32_t) * nchunks));
+    PCK(p->chunk_off.ensure(sizeof(uint64_t) * nchunks));
+    k_pcd_nl_count<<<(unsigned)nchunks, kThreads, 0, p->st>>>(t, p->chunk_cnt.as<uint32_t>());
+    PCK(cudaGetLastError());
+    uint64_t nl = 0;
+    int rc = scan_u32(p, p->chunk_cnt.as<uint32_t>(), nchunks, p->chunk_off.as<uint64_t>(), &nl);
+    if (rc != ERASOR_OK) return rc;
+    const uint64_t nlines = nl + 1;
+    if (nlines >= 0xFFFFFFFFull) return fail(p, ERASOR_E_UNSUPPORTED, "2^32 or more lines");
+    PCK(p->lines.ensure(sizeof(uint64_t) * nlines));
+    PCK(p->flags.ensure(sizeof(uint32_t) * nlines));
+    PCK(p->rows.ensure(sizeof(uint64_t) * nlines));
+    uint64_t* line_start = p->lines.as<uint64_t>();
+    PCK(cudaMemsetAsync(line_start, 0, sizeof(uint64_t), p->st));
+    k_pcd_nl_scatter<<<(unsigned)nchunks, kThreads, 0, p->st>>>(t, p->chunk_off.as<uint64_t>(), line_start);
+    const uint32_t g_lines = blocks_for(nlines, kThreads, p->sm_count * 16);
+    k_pcd_classify<<<g_lines, kThreads, 0, p->st>>>(t, line_start, nlines, p->flags.as<uint32_t>());
+    PCK(cudaGetLastError());
+    uint64_t data_rows = 0;
+    rc = scan_u32(p, p->flags.as<uint32_t>(), nlines, p->rows.as<uint64_t>(), &data_rows);
+    if (rc != ERASOR_OK) return rc;
+
+    // 4. rows
+    const uint64_t rows = std::min<uint64_t>(data_rows, h.points);
+    float4* d_out = reinterpret_cast<float4*>(out_xyzi);
+    if (out_kind == ERASOR_PTR_HOST) { PCK(p->out.ensure(sizeof(float4) * std::max<uint64_t>(rows, 1))); d_out = p->out.as<float4>(); }
+    PcdStats* d_st = p->stats.as<PcdStats>();
+    PcdStats* hs = p->h_stats;
+    std::memset(hs, 0, sizeof(PcdStats));
+    hs->err = ~0ull;
+    PCK(cudaMemcpyAsync(d_st, hs, sizeof(PcdStats), cudaMemcpyHostToDevice, p->st));
+    k_pcd_parse<<<g_lines, kThreads, 0, p->st>>>(t, line_start, nlines, p->flags.as<uint32_t>(), p->rows.as<uint64_t>(), h.points, f, d_out, d_st);
+    PCK(cudaGetLastError());
+    PCK(cudaMemcpyAsync(hs, d_st, sizeof(PcdStats), cudaMemcpyDeviceToHost, p->st));
+    PCK(cudaStreamSynchronize(p->st));
+    if (hs->err != ~0ull) {
+        const unsigned long long line = h.lines + (hs->err >> 1) + 1;
+        char msg[160];
+        if (hs->err & 1u) std::snprintf(msg, sizeof(msg), "line %llu: the row does not hold exactly %d values (one per FIELDS entry)", line, f.n);
+        else std::snprintf(msg, sizeof(msg), "line %llu: a value that is not a number", line);
+        inf.error_line = line;
+        if (info) *info = inf;
+        return fail(p, ERASOR_E_INVALID, msg);
+    }
+    if (hs->slow_rows) {
+        k_pcd_parse_slow<<<blocks_for(nlines, kSlowThreads, p->sm_count * 16), kSlowThreads, 0, p->st>>>(t, line_start, nlines, p->flags.as<uint32_t>(),
+                                                                                                         p->rows.as<uint64_t>(), f, d_out);
+        PCK(cudaGetLastError());
+    }
+    if (out_kind == ERASOR_PTR_HOST && rows) PCK(cudaMemcpyAsync(out_xyzi, d_out, sizeof(float4) * rows, cudaMemcpyDeviceToHost, p->st));
+    PCK(cudaStreamSynchronize(p->st));
+    inf.rows = rows;
+    inf.slow_tokens = hs->slow_tokens;
+    if (info) *info = inf;
+    *n = (size_t)rows;
+    return ERASOR_OK;
+}
+
+int erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_kind, char* out, size_t cap, int out_kind, size_t* len) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    if (!len || (n && !xyzi)) return fail(p, ERASOR_E_INVALID, "null argument");
+    if ((in_kind != ERASOR_PTR_HOST && in_kind != ERASOR_PTR_DEVICE) || (out_kind != ERASOR_PTR_HOST && out_kind != ERASOR_PTR_DEVICE))
+        return fail(p, ERASOR_E_INVALID, "in_kind and out_kind must be ERASOR_PTR_HOST or ERASOR_PTR_DEVICE");
+    if (in_kind == ERASOR_PTR_DEVICE && (reinterpret_cast<uintptr_t>(xyzi) & 15u))
+        return fail(p, ERASOR_E_INVALID, "device clouds must be 16-byte aligned (one float4 per point)");
+    PCK(cudaSetDevice(p->device));
+    const bool hit = p->cached && p->c_ptr == xyzi && p->c_n == n && p->c_kind == in_kind;
+    p->cached = false;
+    if (!hit) {
+        char head[512];
+        const int hl = std::snprintf(head, sizeof(head), kHeadFmt, n, n);
+        const float4* d_pts = reinterpret_cast<const float4*>(xyzi);
+        if (in_kind == ERASOR_PTR_HOST && n) {
+            PCK(p->pts.ensure(sizeof(float4) * n));
+            PCK(cudaMemcpyAsync(p->pts.p, xyzi, sizeof(float4) * n, cudaMemcpyHostToDevice, p->st));
+            d_pts = p->pts.as<float4>();
+        }
+        uint64_t body = 0;
+        if (n) {
+            PCK(p->lens.ensure(sizeof(uint32_t) * n));
+            PCK(p->offs.ensure(sizeof(uint64_t) * n));
+            const uint32_t g = blocks_for(n, kThreads, p->sm_count * 16);
+            k_pcd_fmt_len<<<g, kThreads, 0, p->st>>>(d_pts, n, p->lens.as<uint32_t>());
+            PCK(cudaGetLastError());
+            const int rc = scan_u32(p, p->lens.as<uint32_t>(), n, p->offs.as<uint64_t>(), &body);
+            if (rc != ERASOR_OK) return rc;
+        }
+        const uint64_t total = (uint64_t)hl + body;
+        PCK(p->ftext.ensure(total));
+        PCK(cudaMemcpyAsync(p->ftext.p, head, hl, cudaMemcpyHostToDevice, p->st));
+        if (n) {
+            k_pcd_fmt_write<<<blocks_for(n, kThreads, p->sm_count * 16), kThreads, 0, p->st>>>(d_pts, n, p->offs.as<uint64_t>(), p->ftext.as<uint8_t>() + hl);
+            PCK(cudaGetLastError());
+        }
+        PCK(cudaStreamSynchronize(p->st));
+        p->c_ptr = xyzi; p->c_n = n; p->c_kind = in_kind; p->c_len = total;
+    }
+    *len = (size_t)p->c_len;
+    if (!out || cap < p->c_len) {
+        p->cached = true;                             // the following call with the same input fetches this text
+        return out ? fail(p, ERASOR_E_CAPACITY, "out holds fewer bytes than the formatted text") : ERASOR_OK;
+    }
+    PCK(cudaMemcpyAsync(out, p->ftext.p, p->c_len, out_kind == ERASOR_PTR_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, p->st));
+    PCK(cudaStreamSynchronize(p->st));
+    return ERASOR_OK;
+}
+
+}  // extern "C"

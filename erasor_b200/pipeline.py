@@ -7,6 +7,7 @@ scripts/analysis_runner.py):
                               (OfflineMapUpdater::callback_node / save_static_map, OfflineMapUpdater.cpp:174-330)
       -> PR / RR              capi.Evaluator (device), or erasor_b200.evaluate when the updater is injected
                               (scripts/analysis_runner.py)
+      -> <name>_naive_map.pcd, <name>_result.pcd (out_dir): capi.PcdCodec (device), or write_pcd_ascii when the updater is injected
 
 Everything heavy runs on the device behind the C ABI; this module only sequences the calls.  The updater and the voxeliser are
 injectable so that tests/test_pipeline.py can drive the same code with the oracle's objects on a machine without a GPU; with an
@@ -60,8 +61,15 @@ def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, mak
     if out_dir:
         os.makedirs(out_dir, exist_ok=True)
         name = getattr(up, "data_name", "seq")
-        evaluate.write_pcd_ascii(os.path.join(out_dir, f"{name}_naive_map.pcd"), naive)
-        evaluate.write_pcd_ascii(os.path.join(out_dir, f"{name}_result.pcd"), res["static_map"])      # save_static_map's file name (:193)
+        paths = (os.path.join(out_dir, f"{name}_naive_map.pcd"), os.path.join(out_dir, f"{name}_result.pcd"))   # save_static_map's name (:193)
+        if make_updater is None:        # the device updater ran: format the files on the device too (the same bytes)
+            from . import capi
+            with capi.PcdCodec() as codec:
+                codec.write(paths[0], naive)
+                codec.write(paths[1], res["static_map"])
+        else:
+            evaluate.write_pcd_ascii(paths[0], naive)
+            evaluate.write_pcd_ascii(paths[1], res["static_map"])
     return res
 
 

@@ -1,8 +1,9 @@
 // examples/offline_map_updater_main.cpp -- ROS-free counterpart of the reference's file-based driver
 // src/offline_map_updater/main_in_your_env.cpp:60-127: reads <data_dir>/dense_global_map.pcd,
 // <data_dir>/poses_lidar2body.csv (header line, then  idx,time,x,y,z,qx,qy,qz,qw ; columns 2..8 are used, :46-49)
-// and <data_dir>/pcds/%06d.pcd, feeds every node to the device-resident OfflineMapUpdater and writes
-// <save_path>/<data_name>_result.pcd with save_static_map(0.2) (:123).
+// and <data_dir>/pcds/%06d.pcd (ASCII files parsed on the device by PcdCodec, binary ones read by load_pcd and uploaded), feeds
+// every node to the device-resident OfflineMapUpdater and writes <save_path>/<data_name>_result.pcd with save_static_map(0.2)
+// (:123), formatted on the device.  The reference reads either kind with pcl::io::loadPCDFile.
 //   usage: offline_map_updater_main <config.yaml> <data_dir> [init_idx]
 #include <cstdio>
 #include <cstdlib>
@@ -10,9 +11,50 @@
 #include <iostream>
 #include <sstream>
 
+#include <cuda_runtime.h>
+
 #include "../include/erasor/offline_map_updater.hpp"
 
 using namespace erasor_b200;
+
+// A scan in device memory (one float4 per point, 16-byte aligned), grown on demand and reused.
+class DeviceCloud {
+public:
+    DeviceCloud() = default;
+    ~DeviceCloud() { if (p_) cudaFree(p_); }
+    DeviceCloud(const DeviceCloud&) = delete;
+    DeviceCloud& operator=(const DeviceCloud&) = delete;
+    float* reserve(size_t n) {
+        if (n > cap_ || !p_) {
+            if (p_) cudaFree(p_);
+            p_ = nullptr; cap_ = 0;
+            if (cudaMalloc(reinterpret_cast<void**>(&p_), sizeof(float) * 4 * (n ? n : 1)) != cudaSuccess) throw std::runtime_error("DeviceCloud: cudaMalloc failed");
+            cap_ = n;
+        }
+        return p_;
+    }
+    const float* data() const { return p_; }
+    size_t size() const { return n_; }
+    void set_size(size_t n) { n_ = n; }
+    void swap(DeviceCloud& o) { std::swap(p_, o.p_); std::swap(n_, o.n_); std::swap(cap_, o.cap_); }
+private:
+    float* p_ = nullptr;
+    size_t n_ = 0, cap_ = 0;
+};
+
+// An ASCII scan is parsed on the device straight into `out`; a binary one (which the codec leaves to load_pcd) is read on the host
+// and copied up.  Either way the scan is complete in device memory on return.
+static void read_scan(PcdCodec& codec, const std::string& path, DeviceCloud& out) {
+    try {
+        out.set_size(codec.read_device(path, [&](size_t n) { return out.reserve(n); }));
+    } catch (const UnsupportedPcd&) {
+        const PointCloud c = load_pcd(path);
+        float* d = out.reserve(c.size());
+        if (!c.empty() && cudaMemcpy(d, c.data(), sizeof(float) * 4 * c.size(), cudaMemcpyHostToDevice) != cudaSuccess)
+            throw std::runtime_error("cannot upload " + path);
+        out.set_size(c.size());
+    }
+}
 
 static std::vector<std::array<double, 7>> load_all_poses(const std::string& txt) {
     std::vector<std::array<double, 7>> poses;
@@ -39,22 +81,27 @@ int main(int argc, char** argv) {
         const std::string data_dir = argv[2];
         const int init_idx = argc > 3 ? std::atoi(argv[3]) : 0;
         cfg.initial_map_path = data_dir + "/dense_global_map.pcd";
-        OfflineMapUpdater updater(cfg);
+        // ASCII PCDs (what the reference writes) are parsed on the device; a binary map is read by load_pcd
+        PcdCodec codec;
+        PointCloud map;
+        try { map = codec.read(cfg.initial_map_path); } catch (const UnsupportedPcd&) { map = load_pcd(cfg.initial_map_path); }
+        OfflineMapUpdater updater(cfg, map);
+        PointCloud().swap(map);
         const auto poses = load_all_poses(data_dir + "/poses_lidar2body.csv");
-        // Scans come from files, so the next one is known: it is loaded before the current node is processed and, when that next
-        // call will process its node (removal_interval), handed to the updater's look-ahead -- its upload and voxelisation
-        // then run under the current node's path.
+        // Scans come from files, so the next one is known: it is parsed on the device (into device memory, complete when
+        // read_device returns) before the current node is processed and, when that next call will process its node
+        // (removal_interval), handed to the updater's look-ahead -- its voxelisation then runs under the current node's path.
         auto scan_path = [&](int i) { char name[64]; std::snprintf(name, sizeof(name), "/pcds/%06d.pcd", i); return data_dir + name; };
         const int n_nodes = (int)poses.size();
-        PointCloud cur, nxt;
-        if (init_idx < n_nodes) cur = load_pcd(scan_path(init_idx));
+        DeviceCloud cur, nxt;
+        if (init_idx < n_nodes) read_scan(codec, scan_path(init_idx), cur);
         for (int i = init_idx; i < n_nodes; ++i) {
             if (i + 1 < n_nodes) {
-                nxt = load_pcd(scan_path(i + 1));
-                if (updater.processes_call(2)) updater.prefetch(nxt);
+                read_scan(codec, scan_path(i + 1), nxt);
+                if (updater.processes_call(2)) updater.prefetch_device(nxt.data(), nxt.size());
             }
-            updater.callback_node(i, poses[i].data(), cur);
-            std::swap(cur, nxt);
+            updater.callback_node_device(i, poses[i].data(), cur.data(), cur.size());
+            cur.swap(nxt);
         }
         updater.save_static_map(0.2f);
         std::cout << "Static map building complete!" << std::endl;

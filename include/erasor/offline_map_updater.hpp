@@ -2,7 +2,8 @@
 // (reference include/erasor/OfflineMapUpdater.h, src/offline_map_updater/src/OfflineMapUpdater.cpp) on top of the
 // C ABI in include/erasor_b200.h.  The global map lives on the GPU; `callback_node` takes what an `erasor/node`
 // message carries (header.seq, odom, lidar) as plain arguments; `save_static_map` writes the same ASCII PCD the
-// reference writes with pcl::io::savePCDFileASCII, which scripts/analysis_runner.py reads.
+// reference writes with pcl::io::savePCDFileASCII, which scripts/analysis_runner.py reads, formatted on the device (PcdCodec).
+// Everything here goes through the C ABI: no CUDA header or runtime library is needed to use it.
 //
 // Config: the reference's rosparam tree (config/*.yaml: /erasor/*, /MapUpdater/*, /large_scale/*, /tf/lidar2body,
 // /verbose) is read by load_config(); no yaml-cpp is needed for the two-level key: value files the reference ships.
@@ -149,10 +150,73 @@ inline void save_pcd_ascii(const std::string& path, const PointCloud& c) {
     for (const auto& p : c) f << p.x << ' ' << p.y << ' ' << p.z << ' ' << p.intensity << '\n';
 }
 
+// ASCII PCD files through the device codec (erasor_pcd_*): the reader gives what load_pcd gives bit for bit (intensity 0 when the
+// file has none), the writer the bytes save_pcd_ascii writes (NaN spelled "nan").  Binary files are not parsed here
+// (UnsupportedPcd): load_pcd reads them.
+struct UnsupportedPcd : std::runtime_error { using std::runtime_error::runtime_error; };
+
+class PcdCodec {
+public:
+    explicit PcdCodec(int device = 0) {
+        if (erasor_pcd_create(device, &p_) != ERASOR_OK) throw std::runtime_error(std::string("PcdCodec: ") + erasor_pcd_last_error(nullptr));
+    }
+    ~PcdCodec() { erasor_pcd_destroy(p_); }
+    PcdCodec(const PcdCodec&) = delete;
+    PcdCodec& operator=(const PcdCodec&) = delete;
+
+    // The file at path into device memory.  device_buffer(n) must return a 16-byte aligned device pointer with room for n points
+    // (the caller owns the memory); returns the points parsed.  Synchronous: the cloud is complete on return.
+    template <class DeviceBuffer>
+    size_t read_device(const std::string& path, DeviceBuffer&& device_buffer) {
+        slurp(path);
+        size_t n = 0;
+        check(erasor_pcd_parse_ascii(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, nullptr, 0, ERASOR_PTR_DEVICE, &n, nullptr), path);
+        float* out = device_buffer(n);
+        check(erasor_pcd_parse_ascii(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, out, n, ERASOR_PTR_DEVICE, &n, nullptr), path);
+        return n;
+    }
+    PointCloud read(const std::string& path) {
+        slurp(path);
+        size_t n = 0;
+        check(erasor_pcd_parse_ascii(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, nullptr, 0, ERASOR_PTR_HOST, &n, nullptr), path);
+        PointCloud c(n);
+        check(erasor_pcd_parse_ascii(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, reinterpret_cast<float*>(c.data()), n, ERASOR_PTR_HOST, &n, nullptr), path);
+        c.resize(n);
+        return c;
+    }
+    void write(const std::string& path, const PointCloud& c) {
+        const float* src = reinterpret_cast<const float*>(c.data());
+        size_t len = 0;
+        check(erasor_pcd_format_ascii(p_, src, c.size(), ERASOR_PTR_HOST, nullptr, 0, ERASOR_PTR_HOST, &len), path);
+        text_.resize(len);
+        check(erasor_pcd_format_ascii(p_, src, c.size(), ERASOR_PTR_HOST, text_.data(), len, ERASOR_PTR_HOST, &len), path);
+        std::ofstream f(path, std::ios::binary);
+        if (!f || !f.write(text_.data(), (std::streamsize)len)) throw std::runtime_error("cannot write " + path);
+    }
+
+private:
+    void slurp(const std::string& path) {
+        std::ifstream f(path, std::ios::binary | std::ios::ate);
+        if (!f) throw std::invalid_argument("cannot open " + path);
+        text_.resize((size_t)f.tellg());
+        f.seekg(0);
+        if (!text_.empty() && !f.read(text_.data(), (std::streamsize)text_.size())) throw std::runtime_error("cannot read " + path);
+    }
+    void check(int rc, const std::string& path) const {
+        if (rc == ERASOR_OK) return;
+        const std::string msg = path + ": " + erasor_pcd_last_error(p_);
+        if (rc == ERASOR_E_UNSUPPORTED) throw UnsupportedPcd(msg);
+        if (rc == ERASOR_E_INVALID) throw std::invalid_argument(msg);
+        throw std::runtime_error(msg);
+    }
+    erasor_pcd_t p_ = nullptr;
+    std::vector<char> text_;
+};
+
 class OfflineMapUpdater {
 public:
     // replaces OfflineMapUpdater::OfflineMapUpdater(): set_params + load_global_map + new ERASOR (OfflineMapUpdater.cpp:5-32)
-    OfflineMapUpdater(const Config& cfg, const PointCloud& initial_map, int device = 0) : cfg_(cfg) {
+    OfflineMapUpdater(const Config& cfg, const PointCloud& initial_map, int device = 0) : cfg_(cfg), device_(device) {
         if (cfg.env != "outdoor") throw std::invalid_argument("This `indoor` mode is not perfect!");   // :149
         const int rc = erasor_updater_create(&cfg_.updater, &cfg_.erasor, reinterpret_cast<const float*>(initial_map.data()),
                                              initial_map.size(), device, &u_);
@@ -177,6 +241,16 @@ public:
     // callback_node call so that its upload and voxelisation (:237-241) run under the current node's path.  `lidar` must stay
     // alive and unchanged until that call; results are identical with and without.
     void prefetch(const PointCloud& lidar) { check(erasor_updater_prefetch_scan(u_, reinterpret_cast<const float*>(lidar.data()), lidar.size(), ERASOR_PTR_HOST)); }
+    // the same two calls with a scan of n points already in device memory (e.g. parsed there by PcdCodec::read_device); the scan
+    // must be complete before prefetch_device, and stay unchanged until its callback_node_device call
+    bool callback_node_device(int seq, const double odom[7], const float* lidar_xyzi, size_t n) {
+        ++calls_;
+        int processed = 0;
+        check(erasor_updater_process_node(u_, seq, odom, lidar_xyzi, n, ERASOR_PTR_DEVICE, &processed));
+        if (cfg_.verbose) std::printf(processed ? "\033[01;32m%dth frame\033[0m is comming\n" : "\033[1;32m PASS! \033[0m\n", seq);
+        return processed != 0;
+    }
+    void prefetch_device(const float* lidar_xyzi, size_t n) { check(erasor_updater_prefetch_scan(u_, lidar_xyzi, n, ERASOR_PTR_DEVICE)); }
     // will the k-th callback_node call from now (k = 1: the next one) process its node, or "PASS!" (removal_interval, :328)?
     bool processes_call(int k) const { return (calls_ + k) % cfg_.updater.removal_interval == 0; }
     // replaces save_static_map(float voxel_size) (:174-196)
@@ -184,7 +258,7 @@ public:
         PointCloud map_to_be_saved = static_map(voxel_size);
         const std::string target = cfg_.save_path + "/" + cfg_.data_name + "_result.pcd";
         std::printf("\033[1;32mTARGET: %s\033[0m\nVoxelization operated with %g voxel size\n", target.c_str(), voxel_size);
-        save_pcd_ascii(target, map_to_be_saved);
+        PcdCodec(device_).write(target, map_to_be_saved);            // the bytes save_pcd_ascii writes, formatted on the device
         std::printf("\033[1;32mComplete to save the final static map\033[0m\n");
     }
     PointCloud static_map(float voxel_size) {
@@ -212,6 +286,7 @@ private:
     }
     Config cfg_;
     erasor_updater_t u_ = nullptr;
+    int device_ = 0;
     long long calls_ = 0;          // callback_node calls so far (the updater's stack_count, :206)
 };
 

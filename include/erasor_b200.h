@@ -354,6 +354,43 @@ int  erasor_eval_overlap(erasor_eval_t e, const float* gt_xyzi, size_t n_gt, con
  * keep mask, so that a caller can compute its ranks before the call. */
 int  erasor_eval_count_selected(erasor_eval_t e, const uint8_t* keep, size_t n, int ptr_kind, uint64_t* count);
 
+/* ============================================================================================
+ * ASCII PCD files on the device: the text of a whole file -> float[n][4] x y z intensity, and a cloud -> the text that
+ * erasor_b200/evaluate.py's write_pcd_ascii and include/erasor/offline_map_updater.hpp's save_pcd_ascii write (the layout of
+ * pcl::io::savePCDFileASCII).  Bit-identical to the host readers (np.loadtxt + astype(float32); istream >> double + (float)) and
+ * byte-identical to the host writers ("%.8g"), except that NaN is written "nan" whatever its sign.  A handle of its own: one CUDA
+ * device + one stream, scratch kept and grown on demand; not thread-safe.  Every call is synchronous.
+ * ========================================================================================== */
+typedef struct erasor_pcd_ctx* erasor_pcd_t;
+
+typedef struct {
+    uint64_t points;             /* POINTS of the header */
+    uint64_t rows;               /* rows parsed: POINTS, or fewer when the file holds fewer data rows */
+    uint64_t slow_tokens;        /* kept values the fast path could not decide, settled by exact big-integer arithmetic */
+    uint64_t error_line;         /* 1-based line of the file that made the call fail with ERASOR_E_INVALID, else 0 */
+    uint64_t header_lines;       /* lines up to and including DATA; 0 when the text holds no DATA line (the rest is then 0 too) */
+    uint32_t fields;             /* bit 0 x, 1 y, 2 z, 3 intensity: which of them FIELDS names */
+    uint32_t has_intensity;      /* 1 when FIELDS names intensity (otherwise the intensity column is 0) */
+} erasor_pcd_info_t;
+
+int  erasor_pcd_create(int device, erasor_pcd_t* out);
+void erasor_pcd_destroy(erasor_pcd_t p);
+const char* erasor_pcd_last_error(erasor_pcd_t p);    /* p may be NULL: error of the last failed erasor_pcd_create */
+/* text: the whole file, len bytes, host or device (text_kind).  The header is read on the host: FIELDS (any order, extras allowed;
+ * x, y, z required), COUNT (all 1), POINTS and DATA (ascii); otherwise ERASOR_E_UNSUPPORTED (binary files, COUNT > 1) or
+ * ERASOR_E_INVALID.  Lines end at '\n', "\r\n" or a lone '\r' (Python's universal newlines, as read_pcd_ascii opens the file).
+ * Rows follow np.loadtxt: '#' starts a comment, blank lines are skipped, blanks are ' ' \t \r \v \f, every row
+ * holds one value per field (each one checked, kept or not), and reading stops after POINTS rows.  A bad row gives ERASOR_E_INVALID,
+ * with its line in info->error_line and erasor_pcd_last_error.  out_xyzi (host or device per out_kind; a device cloud 16-byte
+ * aligned) needs room for POINTS points; NULL only asks for *n = POINTS.  *n = rows parsed.  info (nullable) is written on every
+ * return, as far as the header was read. */
+int  erasor_pcd_parse_ascii(erasor_pcd_t p, const char* text, size_t len, int text_kind, float* out_xyzi, size_t cap, int out_kind,
+                            size_t* n, erasor_pcd_info_t* info);
+/* The whole file for n points (host or device per in_kind): the header, then "x y z intensity\n" per point, each value as
+ * printf("%.8g", (double)v).  out == NULL (or cap too small: ERASOR_E_CAPACITY) returns the exact size in *len and keeps the text
+ * for the following call with the same (xyzi, n, in_kind), which then only copies it out.  out: host or device per out_kind. */
+int  erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_kind, char* out, size_t cap, int out_kind, size_t* len);
+
 #ifdef __cplusplus
 }
 #endif
