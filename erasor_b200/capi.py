@@ -31,7 +31,7 @@ EXPORTS = [
     "erasor_map_create", "erasor_map_destroy", "erasor_map_size", "erasor_map_reset_keep", "erasor_map_get_keep", "erasor_map_keep_device",
     "erasor_map_points_device", "erasor_attach_map", "erasor_process_nodes", "erasor_process_nodes_async", "erasor_get_node_stats",
     "erasor_comm_unique_id", "erasor_comm_init", "erasor_comm_destroy", "erasor_allgather_and_keep", "erasor_and_keep_masks",
-    "erasor_get_kernel_time_ms", "erasor_reset_kernel_times", "erasor_get_rgpf_profile", "erasor_get_srt_profile",
+    "erasor_get_kernel_time_ms", "erasor_reset_kernel_times", "erasor_get_rgpf_profile", "erasor_get_srt_profile", "erasor_profile_k1",
     "erasor_updater_create", "erasor_updater_destroy", "erasor_updater_reset", "erasor_updater_last_error", "erasor_updater_process_node", "erasor_updater_prefetch_scan",
     "erasor_updater_map_size", "erasor_updater_get_cloud", "erasor_updater_save_static_map", "erasor_updater_voxelize", "erasor_updater_mapgen_node",
     "erasor_updater_erasor", "erasor_updater_kernel_launch_count", "erasor_updater_get_fused_profile",
@@ -138,6 +138,7 @@ def _load():
     L.erasor_reset_kernel_times.argtypes = [c_void_p, c_int]
     L.erasor_get_rgpf_profile.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32), POINTER(c_size_t)]
     L.erasor_get_srt_profile.argtypes = [c_void_p, POINTER(c_uint32)]
+    L.erasor_profile_k1.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_size_t), POINTER(c_int)]
     L.erasor_updater_create.argtypes = [POINTER(UpdaterParamsC), POINTER(ErasorParamsC), c_void_p, c_size_t, c_int, POINTER(c_void_p)]
     L.erasor_updater_destroy.restype = None
     L.erasor_updater_destroy.argtypes = [c_void_p]
@@ -286,14 +287,16 @@ class Handle:
         return self.L.erasor_get_max_range(self.h)
 
     # -- parity taps ---------------------------------------------------------------------------
-    def get_bins(self, which: int):
+    def get_bins(self, which: int, per_point: bool = True):
+        """per_point=False: tables only (the form a one-node process_nodes supports); bin_of_point comes back as None."""
         B = self.params.num_bins
         n = self.n_map if which == CLOUD_MAP else self.n_query
-        bop = np.empty(n, dtype=np.int32)
+        bop = np.empty(n, dtype=np.int32) if per_point else None
         mn, mx = np.empty(B, dtype=np.float32), np.empty(B, dtype=np.float32)
         cnt = np.empty(B, dtype=np.uint32)
-        self._ck(self.L.erasor_get_bins(self.h, which, bop.ctypes.data_as(POINTER(c_int32)), mn.ctypes.data_as(POINTER(c_float)),
-                                        mx.ctypes.data_as(POINTER(c_float)), cnt.ctypes.data_as(POINTER(c_uint32))))
+        self._ck(self.L.erasor_get_bins(self.h, which, bop.ctypes.data_as(POINTER(c_int32)) if per_point else None,
+                                        mn.ctypes.data_as(POINTER(c_float)), mx.ctypes.data_as(POINTER(c_float)),
+                                        cnt.ctypes.data_as(POINTER(c_uint32))))
         return bop, mn, mx, cnt
 
     def get_status(self) -> np.ndarray:
@@ -465,6 +468,15 @@ class Handle:
         if k:
             self._ck(self.L.erasor_get_rgpf_profile(self.h, npts.ctypes.data_as(POINTER(c_uint32)), prof.ctypes.data_as(POINTER(c_uint32)), ctypes.byref(cap)))
         return npts, prof
+
+    def k1_profile(self):
+        """K1 of the last node-mode batch as its profiling build: uint32 [chunk, warp, 8] -- SM cycles of scan, compaction,
+        transform + bin, table update, list stores, barrier + flush, then the warp's total and dense rows (all ones: query chunk)."""
+        n, nw = c_size_t(0), c_int(0)
+        self._ck(self.L.erasor_profile_k1(self.h, None, ctypes.byref(n), ctypes.byref(nw)))
+        out = np.zeros(n.value, dtype=np.uint32)
+        self._ck(self.L.erasor_profile_k1(self.h, out.ctypes.data_as(POINTER(c_uint32)), ctypes.byref(n), ctypes.byref(nw)))
+        return out.reshape(-1, nw.value, 8)
 
     def kernel_time_ms(self, kernel_id: int):
         t, n = c_double(), c_uint64()

@@ -13,6 +13,10 @@ constexpr uint32_t kMapPad    = 256;           // slack points behind the reside
 constexpr int      kListWarps = 32;            // node mode: per-chunk stride of the per-warp VoI list counters (K1 runs 8 or 32 warps)
 constexpr int      kMaxIter   = 8;             // gf_iter upper bound for the tap arrays
 
+// K1's profiling build (erasor_profile_k1): per warp, SM cycles spent in each phase of the node-mode map path, the warp's
+// total from the end of the table set-up to the end of the flush, and its dense-row count
+enum : int { kK1ProfScan = 0, kK1ProfCompact, kK1ProfBin, kK1ProfTable, kK1ProfLists, kK1ProfFlush, kK1ProfTotal, kK1ProfRows, kK1ProfSlots };
+
 // status codes held on the device (values published through erasor_get_status)
 enum : uint8_t { ST_LITTLE = 0, ST_MERGE = 1, ST_MAP_HIGH = 2, ST_BLOCKED = 3, ST_CURR_HIGH = 4 };
 // what the selected bin is made of (erasor.cpp:493-563 / 346-427)

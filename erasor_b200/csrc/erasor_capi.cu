@@ -115,6 +115,7 @@ struct erasor_ctx {
     DevBuf d_fence;                            // 4 x u64: negzero, empty fits, ambiguous, slow-path points
     DevBuf d_poses;                            // node mode: NodePose per frame
     DevBuf d_list_idx, d_list_cnt;             // node mode: per chunk, the map index of every VoI point (dense, map order) and their number
+    DevBuf d_k1prof;                           // erasor_profile_k1: per-warp cycle counters of K1's profiling build
     DevBuf d_pack, d_gather;                   // exchange step: packed keep bits of this rank / of every rank
     PinnedBuf h_stage, h_pose, h_words;        // h_words: small device -> host read-backs of a submission (pinned: an asynchronous copy into
                                                // pageable memory blocks the launching thread until the whole stream has drained, which
@@ -124,7 +125,7 @@ struct erasor_ctx {
                 &d_zmax, &d_cnt, &d_dst_start, &d_status, &d_action, &d_flag_slot, &d_nflag, &d_recs, &d_nrecs, &d_queue, &d_bucket, &d_frame_rej,
                 &d_map_sorted, &d_map_src, &d_qry_sorted, &d_qry_src, &d_part, &d_scratch, &d_keep, &d_ground, &d_arranged, &d_map_rej, &d_curr_rej,
                 &d_jobs, &d_out_sizes, &d_k5tmp, &d_fence, &d_vox, &d_vox_cnt, &d_vox_start, &d_vox_scratch, &d_frame_rec_base, &d_poses, &d_list_idx, &d_list_cnt, &d_pack,
-                &d_gather};
+                &d_gather, &d_k1prof};
     }
 
     // batch geometry of the last run
@@ -135,6 +136,7 @@ struct erasor_ctx {
     const float4* cur_map = nullptr;
     const float4* cur_qry = nullptr;
     bool     qry_xyz = false;                  // the staged query cloud is packed x y z (ERASOR_PTR_QUERY_XYZ, mask modes)
+    uint32_t* k1_prof = nullptr;               // set only inside erasor_profile_k1: run_k1 launches K1's profiling build
     std::vector<uint64_t> map_off, qry_off;
     int      desc_mode = -1;                   // mode the uploaded chunk descriptors were built for (-1: none; 0 cloud, 1 batch masks, 2 node masks)
     uint64_t desc_epoch = 0;                   // bumped whenever the descriptors are rebuilt (invalidates cached graphs)
@@ -386,7 +388,7 @@ int run_k1(erasor_ctx* h, int mode) {
                      h->d_bin_map.as<uint16_t>(), h->d_bin_qry.as<uint16_t>(), h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(),
                      h->d_zmax.as<uint32_t>(), h->d_cnt.as<uint32_t>(), B, F, h->d_fence.as<unsigned long long>(),
                      mode == 2 ? h->d_poses.as<NodePose>() : nullptr, mode == 2 ? h->d_list_idx.as<uint32_t>() : nullptr,
-                     mode == 2 ? h->d_list_cnt.as<uint32_t>() : nullptr, mode != 0 && h->qry_xyz));
+                     mode == 2 ? h->d_list_cnt.as<uint32_t>() : nullptr, mode != 0 && h->qry_xyz, mode == 2 ? h->k1_prof : nullptr));
     }
     return ERASOR_OK;
 }
@@ -756,7 +758,9 @@ int erasor_get_ground_viz(erasor_handle_t h, float* ground_xyzi, size_t cap, siz
 
 int erasor_get_bins(erasor_handle_t h, int which_cloud, int32_t* bin_of_point, float* min_h, float* max_h, uint32_t* count) {
     if (!h) return ERASOR_E_INVALID;
-    if (h->stage < 1 || h->F != 1) { h->err = "erasor_get_bins needs a single-frame erasor_set_inputs"; return ERASOR_E_STATE; }
+    const bool node = h->desc_mode == 2 && h->F == 1 && h->stage < 1;      // one node of erasor_process_nodes: tables only
+    if ((h->stage < 1 && !node) || h->F != 1) { h->err = "erasor_get_bins needs a single-frame erasor_set_inputs or a one-node erasor_process_nodes"; return ERASOR_E_STATE; }
+    if (node && bin_of_point) { h->err = "node mode keeps no per-point bins of the map"; return ERASOR_E_STATE; }
     if (which_cloud != 0 && which_cloud != 1) { h->err = "which_cloud"; return ERASOR_E_INVALID; }
     CK(cudaSetDevice(h->device));
     const int B = h->B;
@@ -1351,6 +1355,31 @@ int erasor_get_rgpf_profile(erasor_handle_t h, uint32_t* n_points, uint32_t* pro
         if (n_points) n_points[i] = recs[i].n_points;
         if (prof8) for (int k = 0; k < 8; ++k) prof8[i * 8 + k] = recs[i].prof[k];
     }
+    return ERASOR_OK;
+}
+
+// instrumentation: K1 of the last node-mode batch again, as its profiling build.  It rebuilds the per-frame tables and lists that
+// batch's K1 built (with the same values); the outputs of the later kernels are left as they are.
+int erasor_profile_k1(erasor_handle_t h, uint32_t* out, size_t* n, int* warps_per_cta) {
+    if (!h || !n) return ERASOR_E_INVALID;
+    if (h->desc_mode != 2 || !h->cur_map) { h->err = "no node-mode batch has run"; return ERASOR_E_STATE; }
+    CK(cudaSetDevice(h->device));
+    int rc;
+    if (h->pending && (rc = erasor_wait(h))) return rc;
+    const int nw = k1_big_tables(h->p.num_rings, h->B) ? 32 : 8;
+    const size_t words = (size_t)(h->n_chunks_map + h->n_chunks_qry) * nw * kK1ProfSlots;
+    const size_t cap = *n;
+    *n = words;
+    if (warps_per_cta) *warps_per_cta = nw;
+    if (!out) return ERASOR_OK;
+    if (cap < words) { h->err = "profile buffer too small"; return ERASOR_E_CAPACITY; }
+    CK(h->d_k1prof.ensure(sizeof(uint32_t) * std::max<size_t>(words, 1)));
+    h->k1_prof = h->d_k1prof.as<uint32_t>();
+    rc = run_k1(h, 2);
+    h->k1_prof = nullptr;
+    if (rc) return rc;
+    CK(cudaStreamSynchronize(h->stream));
+    CK(cudaMemcpy(out, h->d_k1prof.p, sizeof(uint32_t) * words, cudaMemcpyDeviceToHost));
     return ERASOR_OK;
 }
 

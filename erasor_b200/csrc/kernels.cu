@@ -75,10 +75,11 @@ __device__ __forceinline__ void k1_aggregate(int key, uint32_t zenc, int lane, u
         }
         return;
     }
-    // Mixed warp (in node mode a third of the lanes of a typical row lie outside the VoI, so runs of equal bins are short):
-    // per-lane shared-memory atomics, but only where they can change something -- a bin's min / max settle after its
-    // first few points, and a plain (possibly stale) read is a safe filter because the values only move one way.
-    // (A segmented shuffle scan over the runs takes several times the instructions per row.)
+    // Mixed warp (in node mode every lane of a dense row lies inside the VoI, but the bins change along the row: 96 % of the
+    // rows are mixed, ~5 keys each, scripts/k1_row_stats.py): per-lane shared-memory atomics, but only where they can
+    // change something -- a bin's min / max settle after its first few points, and a plain (possibly stale) read is a safe
+    // filter because the values only move one way.  One update per distinct key measured slower on an H100 (DESIGN section 5):
+    // match.any + REDUX over each key's lanes (the REDUX runs once per key group) and a segmented shuffle reduction over runs.
     if (key >= 0) {
         if (key < B) {
             if (zenc < s_mn[key]) atomicMin(&s_mn[key], zenc);
@@ -141,13 +142,16 @@ __device__ __forceinline__ bool in_voi_radius(const NodePose& P, float x, float 
 // NODE: the map cloud is the resident global map in the origin frame; every frame's chunks scan it, keep the points
 // inside the frame's radius (fetch_VoI) and bin their origin -> body transforms.  Points outside the VoI get no bin id
 // and are not counted anywhere (they are the reference's map_outskirts_, which never reach ERASOR).
-template <int THREADS, int UNROLL, bool ROWS, bool NODE>
+// PROF: the profiling build behind erasor_profile_k1 -- lane 0 of every warp adds the SM cycles between consecutive phase
+// boundaries of the node-mode map path to its warp's slots (kK1Prof*); with PROF false none of it is compiled.
+template <int THREADS, int UNROLL, bool ROWS, bool NODE, bool PROF = false>
 __global__ void __launch_bounds__(THREADS, THREADS == 256 ? 4 : 1)      // four 8-warp CTAs per SM (64 registers) or one 32-warp CTA
 k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* __restrict__ qry_pts,
             const ChunkDesc* __restrict__ chunks, uint16_t* __restrict__ bin_map, uint16_t* __restrict__ bin_qry,
             uint32_t* __restrict__ ch_cnt, uint32_t* __restrict__ zmin, uint32_t* __restrict__ zmax, uint32_t* __restrict__ cnt_tab,
             int B, int F, unsigned long long* __restrict__ fence, const NodePose* __restrict__ poses,
-            uint32_t* __restrict__ list_idx, uint32_t* __restrict__ list_cnt, int qry_xyz /*query cloud packed x y z (12 bytes per point)*/) {
+            uint32_t* __restrict__ list_idx, uint32_t* __restrict__ list_cnt, int qry_xyz /*query cloud packed x y z (12 bytes per point)*/,
+            uint32_t* __restrict__ prof /*PROF: kK1ProfSlots words per warp*/) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float2*   s_ring = reinterpret_cast<float2*>(smem_raw);               // {up, dn} guard thresholds of r^2 per ring boundary
     uint32_t* s_cnt  = reinterpret_cast<uint32_t*>(s_ring + ((T.R + 2) & ~1));
@@ -160,11 +164,26 @@ k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* _
     __shared__ NodePose s_pose;
     const bool node_map = NODE && cd.cloud == 0;          // CTA-uniform
 
+    __shared__ uint32_t s_prof[PROF ? NW * kK1ProfSlots : 1];
+    long long t_prev = 0, t_start = 0;
+    uint32_t n_rows = 0;
+    auto tick = [&](int phase) {
+        if constexpr (PROF) {
+            const long long t = clock64();
+            if (lane == 0) s_prof[warp * kK1ProfSlots + phase] += (uint32_t)(t - t_prev);
+            t_prev = t;
+        }
+    };
+    if constexpr (PROF) {
+        if (lane == 0) for (int k = 0; k < kK1ProfSlots; ++k) s_prof[warp * kK1ProfSlots + k] = 0u;
+    }
+
     for (int i = tid; i <= T.R; i += THREADS) s_ring[i] = make_float2(T.ring_guard[2 * i], T.ring_guard[2 * i + 1]);
     for (int i = tid; i <= B; i += THREADS) s_cnt[i] = 0u;
     for (int i = tid; i < B; i += THREADS) { s_mn[i] = 0xFFFFFFFFu; s_mx[i] = 0u; }
     if (NODE && tid == 0) s_pose = poses[cd.frame];
     __syncthreads();
+    if constexpr (PROF) { t_start = clock64(); t_prev = t_start; }
 
     const float4* __restrict__ src = (cd.cloud == 0 ? map_pts : qry_pts) + cd.begin;
     uint16_t* __restrict__     dst = (cd.cloud == 0 ? bin_map : bin_qry) + cd.bin_begin;
@@ -177,9 +196,8 @@ k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* _
         // ---- node mode, map cloud: fetch_VoI fused in.  Every warp streams its own contiguous sub-range of the chunk (four
         // float4 loads in flight per lane, no block-wide barrier) and compacts the points inside the VoI, in order, into a
         // 64-entry ring in shared memory; whenever the ring holds a full row the warp runs the expensive part on it --
-        // origin -> body transform, polar bin, table update -- with all 32 lanes busy (in map order a third of the lanes of a
-        // mixed row lie outside the radius, ncu r02), and appends (bin id, map index) to its dense list.  K2 walks those
-        // lists, warp by warp in the same split, instead of every map point.
+        // origin -> body transform, polar bin, table update -- with all 32 lanes busy, and appends (bin id, map index) to its
+        // dense list.  K2 walks those lists, warp by warp in the same split, instead of every map point.
         __shared__ float4 s_ring_q[NODE ? NW * 64 : 1];
         float4* __restrict__ q = s_ring_q + warp * 64;
         const uint32_t sub = (((cd.len + NW - 1) / NW) + 31u) & ~31u;
@@ -195,30 +213,44 @@ k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* _
             if (__any_sync(FULL_MASK, ok && b == -3)) {
                 if (ok && b == -3) b = bin_exact(T, pp.x, pp.y, pp.z, &fc);   // exact path (rare)
             }
+            tick(kK1ProfBin);
             int key = -2;
             if (ok) {
                 lbin[qh + lane] = (b < 0) ? kNoBin16 : (uint16_t)b;
                 lidx[qh + lane] = cd.begin + __float_as_uint(e.w);              // index in the resident map
                 key = (b < 0) ? B : b;
             }
+            tick(kK1ProfLists);
             k1_aggregate(key, float_to_ordered(pp.z), lane, s_cnt, s_mn, s_mx, B);
             qh += n;
             __syncwarp();                              // the row's ring slots may be overwritten from here on
+            tick(kK1ProfTable);
+            ++n_rows;
         };
+        // in_voi_radius's float decision with its constants in registers (read from the shared NodePose, every radius test
+        // waited on shared-memory loads that the compiler re-issues after each ring store); the band goes to in_voi_radius
+        const float pxf = s_pose.pxf, pyf = s_pose.pyf, lim_lo = s_pose.lim_lo, lim_hi = s_pose.lim_hi;
         // (the resident map carries kMapPad points of slack, so the loads need no bounds checks: positions >= w1 are masked below)
+        // The map loads may allocate in L1, unlike the streaming loads of the other modes: every frame of a batch scans the
+        // same resident map, so chunks of different frames over the same map range read the same lines at about the same
+        // time; measured faster than L1::no_allocate on the bench workload (DESIGN section 5).
         for (uint32_t base = w0; base < w1; base += 32u * UNROLL) {
             float4 p[UNROLL];
 #pragma unroll
-            for (int u = 0; u < UNROLL; ++u) p[u] = ld_stream_f4(src + (base + u * 32u + lane));
+            for (int u = 0; u < UNROLL; ++u) p[u] = __ldg(src + (base + u * 32u + lane));
 #pragma unroll
             for (int u = 0; u < UNROLL; ++u) {
                 const uint32_t i = base + u * 32u + lane;
-                const bool in = (i < w1) && in_voi_radius(s_pose, p[u].x, p[u].y);
+                const float dxf = p[u].x - pxf, dyf = p[u].y - pyf;
+                const float d2f = fmaf(dyf, dyf, dxf * dxf);
+                const bool in = (i < w1) && (d2f < lim_lo || (!(d2f > lim_hi) && in_voi_radius(s_pose, p[u].x, p[u].y)));
                 const unsigned bal = __ballot_sync(FULL_MASK, in);
+                tick(kK1ProfScan);
                 if (bal == 0u) continue;                                         // warp-uniform
                 if (in) q[(qt + __popc(bal & ((1u << lane) - 1u))) & 63u] = make_float4(p[u].x, p[u].y, p[u].z, __uint_as_float(i));
                 qt += __popc(bal);
                 __syncwarp();
+                tick(kK1ProfCompact);
                 if (qt - qh >= 32u) dense_row(32u);
             }
         }
@@ -281,6 +313,15 @@ k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* _
     if (fc.negzero) atomicAdd(&fence[0], (unsigned long long)fc.negzero);
     if (fc.ambiguous) atomicAdd(&fence[2], (unsigned long long)fc.ambiguous);
     if (fc.slow) atomicAdd(&fence[3], (unsigned long long)fc.slow);
+    if constexpr (PROF) {
+        tick(kK1ProfFlush);
+        if (lane == 0) {
+            uint32_t* o = prof + ((size_t)blockIdx.x * NW + warp) * kK1ProfSlots;
+            for (int k = 0; k < kK1ProfTotal; ++k) o[k] = s_prof[warp * kK1ProfSlots + k];
+            o[kK1ProfTotal] = (uint32_t)(t_prev - t_start);
+            o[kK1ProfRows]  = node_map ? n_rows : 0xFFFFFFFFu;      // all ones: a query chunk (no node-mode phases)
+        }
+    }
 }
 
 bool k1_big_tables(int R, int B) { return k1_smem_bytes(R, B) > 56 * 1024; }
@@ -292,36 +333,45 @@ size_t k1_smem_bytes(int R, int B) {
 cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map_pts, const float4* qry_pts,
                       const ChunkDesc* chunks, int n_chunks, uint16_t* bin_map, uint16_t* bin_qry, uint32_t* ch_cnt,
                       uint32_t* zmin, uint32_t* zmax, uint32_t* cnt_tab, int B, int F, unsigned long long* fence, const NodePose* poses,
-                      uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz) {
+                      uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz, uint32_t* prof) {
     if (n_chunks == 0) return cudaSuccess;
     const int qx = qry_xyz ? 1 : 0;
     constexpr int UNROLL = 4;
     const size_t smem = k1_smem_bytes(T.R, B);
     cudaError_t e;
+    if (prof && !poses) return cudaErrorInvalidValue;      // the profiling build covers node mode only
     // Bin tables beyond ~56 KB (40 x 360 bins: 173 KB) leave one CTA per SM: give that CTA 32 warps instead of 8, the
     // kernel needs ~32 resident warps per SM to cover its latencies.
     if (k1_big_tables(T.R, B)) {
         constexpr int THREADS = 1024;
-        if (poses) {
+        if (prof) {
+            auto kern = k1_rpod_bin<THREADS, UNROLL, true, true, true>;
+            if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
+            kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx, prof);
+        } else if (poses) {
             auto kern = k1_rpod_bin<THREADS, UNROLL, true, true>;
             if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-            kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx);
+            kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx, nullptr);
         } else {
             auto kern = k1_rpod_bin<THREADS, UNROLL, true, false>;
             if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-            kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, nullptr, nullptr, nullptr, qx);
+            kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, nullptr, nullptr, nullptr, qx, nullptr);
         }
         return cudaGetLastError();
     }
     constexpr int THREADS = 256;
-    if (poses) {
+    if (prof) {
+        auto kern = k1_rpod_bin<THREADS, UNROLL, true, true, true>;
+        if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
+        kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx, prof);
+    } else if (poses) {
         auto kern = k1_rpod_bin<THREADS, UNROLL, true, true>;
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx);
+        kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx, nullptr);
     } else {
         auto kern = k1_rpod_bin<THREADS, UNROLL, true, false>;
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, nullptr, nullptr, nullptr, qx);
+        kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, nullptr, nullptr, nullptr, qx, nullptr);
     }
     return cudaGetLastError();
 }

@@ -28,7 +28,8 @@ cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map
                       const ChunkDesc* chunks, int n_chunks, uint16_t* bin_map, uint16_t* bin_qry, uint32_t* ch_cnt,
                       uint32_t* zmin, uint32_t* zmax, uint32_t* cnt_tab, int B, int F, unsigned long long* fence, const NodePose* poses,
                       uint32_t* list_idx /*node mode: map index of every VoI point, per chunk*/, uint32_t* list_cnt /*node mode: VoI points per chunk*/,
-                      bool qry_xyz = false /*the query cloud is packed x y z, 12 bytes per point (mask modes)*/);
+                      bool qry_xyz = false /*the query cloud is packed x y z, 12 bytes per point (mask modes)*/,
+                      uint32_t* prof = nullptr /*node mode only: run the profiling build, kK1ProfSlots cycle counters per warp*/);
 
 cudaError_t launch_k3(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt,
                       const uint32_t* zmin, const uint32_t* zmax, const uint32_t* frame_off, const uint32_t* cnt, uint32_t* dst_start,

@@ -125,7 +125,8 @@ double erasor_get_max_range(erasor_handle_t h);
 
 /* ---- parity taps (the reference exposes these only as public members / rviz topics) --------- */
 /* r_pod_map / r_pod_curr (erasor.h:143-144): bin of every input point (-1: complement / dropped),
- * per-bin min z, max z (NaN where the bin is empty) and count.  Any pointer may be NULL. Host buffers. */
+ * per-bin min z, max z (NaN where the bin is empty) and count.  Any pointer may be NULL. Host buffers.
+ * After a one-node erasor_process_nodes: the tables of that node's VoI and query (bin_of_point must be NULL there). */
 int erasor_get_bins(erasor_handle_t h, int which_cloud, int32_t* bin_of_point, float* min_h, float* max_h, uint32_t* count);
 /* per-bin status of the last compare as published on /SCDR/debug/polygons_marker (erasor.cpp:439-441,570) */
 int erasor_get_status(erasor_handle_t h, float* status);
@@ -233,6 +234,11 @@ int erasor_get_rgpf_profile(erasor_handle_t h, uint32_t* n_points, uint32_t* pro
 /* SM cycles per phase of the SRT kernel (K3), frame 0 of the last run: status passes, chunk-row prefixes, flagged-bin scan +
  * record base, map scatter offsets, records + R-GPF queue, query scatter offsets; slots 6-7 reserved (host array of 8). */
 int erasor_get_srt_profile(erasor_handle_t h, uint32_t* cycles8);
+/* K1 of the last node-mode batch again, as a profiling build: per warp of every chunk ([chunk][warp][8] words), the SM cycles
+ * of the map path's phases -- scan (loads + radius test), ring compaction, transform + bin, list stores, table update,
+ * barrier + flush -- then the warp's total and its dense-row count (all ones for a query chunk).  Rebuilds that batch's K1
+ * tables with the same values.  *n in: capacity in words, out: words; out == null only queries the size. */
+int erasor_profile_k1(erasor_handle_t h, uint32_t* out, size_t* n, int* warps_per_cta);
 /* number of kernels this library launched on the handle since creation */
 uint64_t erasor_kernel_launch_count(erasor_handle_t h);
 /* CUDA-event time (ms) spent in the binning kernel (K1) since the last reset, and its launch count */
