@@ -1,7 +1,8 @@
 """The reference's scripts/analysis_runner.py on the device: prints exactly what it prints for two ASCII PCDs -- the estimate -> GT
 distance report, then the PR / RR table -- computed by capi.Evaluator (erasor_evaluate + erasor_eval_overlap) on clouds read by
-capi.PcdCodec (erasor_pcd_parse_ascii, bit-identical to read_pcd_ascii).
---host reads with read_pcd_ascii and computes with sklearn instead (erasor_b200.evaluate), for machines without a GPU.
+capi.PcdCodec.load (erasor_pcd_load: ASCII files bit-identical to read_pcd_ascii, and binary and binary_compressed files as PCL
+reads them).
+--host reads ASCII files only, with read_pcd_ascii and computes with sklearn instead (erasor_b200.evaluate), for machines without a GPU.
 
     python -m erasor_b200.analysis --gt gt.pcd --est est.pcd [--voxelsize 0.2] [--host] [--device N]
 """
@@ -31,7 +32,7 @@ def main(argv=None) -> int:
     else:
         from . import capi
         with capi.PcdCodec(device=args.device) as codec:
-            gt, est = codec.read(args.gt), codec.read(args.est)
+            gt, est = codec.load(args.gt), codec.load(args.est)
         with capi.Evaluator(device=args.device) as ev:
             r = ev.report(gt, est, voxelsize=args.voxelsize)
     sys.stdout.write(E.format_report(r, args.voxelsize, args.gt, args.est))

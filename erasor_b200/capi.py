@@ -38,6 +38,7 @@ EXPORTS = [
     "erasor_eval_create", "erasor_eval_destroy", "erasor_eval_last_error", "erasor_evaluate", "erasor_eval_overlap",
     "erasor_eval_count_selected",
     "erasor_pcd_create", "erasor_pcd_destroy", "erasor_pcd_last_error", "erasor_pcd_parse_ascii", "erasor_pcd_format_ascii",
+    "erasor_pcd_load",
 ]
 NO_MATCH = 0xFFFFFFFF        # erasor_evaluate's match entry of a GT point without an inlier
 
@@ -56,6 +57,13 @@ class PcdInfoC(ctypes.Structure):
     """erasor_pcd_info_t"""
     _fields_ = [(name, c_uint64) for name in ("points", "rows", "slow_tokens", "error_line", "header_lines")] + [("fields", c_uint32),
                                                                                                               ("has_intensity", c_uint32)]
+
+
+class PcdLoadInfoC(ctypes.Structure):
+    """erasor_pcd_load_info_t"""
+    _fields_ = [(name, c_uint32) for name in ("data_mode", "fields", "intensity_zero_filled", "point_step")] + \
+               [(name, c_uint64) for name in ("width", "height", "points", "data_offset", "compressed_size", "uncompressed_size", "lzf_tokens")] + \
+               [("ascii", PcdInfoC)]
 
 
 class UpdaterParamsC(ctypes.Structure):
@@ -173,6 +181,7 @@ def _load():
     L.erasor_pcd_last_error.argtypes = [c_void_p]
     L.erasor_pcd_parse_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdInfoC)]
     L.erasor_pcd_format_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t)]
+    L.erasor_pcd_load.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdLoadInfoC)]
     return L
 
 
@@ -800,10 +809,11 @@ class Evaluator:
 
 
 class PcdCodec:
-    """One ``erasor_pcd_t``: ASCII PCD files read and written on the device (DESIGN.md section 12).  ``parse`` / ``read`` give what
-    ``evaluate.read_pcd_ascii`` gives, bit for bit (including its KeyError for a file without x, y, z or intensity); ``format`` /
-    ``write`` give the bytes ``evaluate.write_pcd_ascii`` writes, except that NaN is written "nan" whatever its sign.  Files are read
-    and written as raw bytes."""
+    """One ``erasor_pcd_t``: PCD files read and written on the device (DESIGN.md section 12).  ``parse`` / ``read`` give what
+    ``evaluate.read_pcd_ascii`` gives, bit for bit (including its KeyError for a file without x, y, z or intensity); ``load`` /
+    ``load_bytes`` read any DATA mode (ascii, binary, binary_compressed) as PCL does (section 12.1); ``format`` / ``write`` give the
+    bytes ``evaluate.write_pcd_ascii`` writes, except that NaN is written "nan" whatever its sign.  Files are read and written as raw
+    bytes."""
 
     def __init__(self, device: int = 0):
         self.L = lib()
@@ -874,6 +884,47 @@ class PcdCodec:
     def last_info(self) -> dict:
         """points, rows, slow_tokens, error_line, header_lines, fields and has_intensity of the last parse"""
         return dict(self._info) if self._info is not None else None
+
+    def _call_load(self, ptr, n_bytes, kind, out_ptr, cap, out_kind):
+        n, info = c_size_t(0), PcdLoadInfoC()
+        rc = self.L.erasor_pcd_load(self.h, ptr, n_bytes, kind, out_ptr, cap, out_kind, ctypes.byref(n), ctypes.byref(info))
+        d = {name: int(getattr(info, name)) for name, _ in PcdLoadInfoC._fields_ if name != "ascii"}
+        d["ascii"] = {name: int(getattr(info.ascii, name)) for name, _ in PcdInfoC._fields_}
+        self._load_info = d
+        self._ck(rc)
+        return n.value
+
+    def load_bytes(self, data, device_out: bool = False):
+        """A PCD file in any DATA mode (ascii, binary, binary_compressed) with PCL's field rules (erasor_pcd_load): data is the
+        whole file -- bytes-like (host) or a CUDA uint8 tensor.  A missing intensity, or one that is not F 4 COUNT 1, reads as 0.
+        Returns float32 [n, 4] x y z intensity: a numpy array, or a CUDA tensor with device_out."""
+        if hasattr(data, "is_cuda") and data.is_cuda:
+            ptr, nb, kind, keep = c_void_p(data.data_ptr()), data.numel() * data.element_size(), PTR_DEVICE, data
+        else:
+            keep = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data).view(np.uint8)
+            ptr, nb, kind = c_void_p(keep.ctypes.data if keep.size else 0), keep.size, PTR_HOST
+        pts = self._call_load(ptr, nb, kind, None, 0, PTR_HOST)
+        if device_out:
+            import torch
+            out = torch.empty((max(pts, 1), 4), dtype=torch.float32, device=f"cuda:{self.device}")
+            rows = self._call_load(ptr, nb, kind, c_void_p(out.data_ptr()), pts, PTR_DEVICE)
+        else:
+            out = np.empty((max(pts, 1), 4), dtype=np.float32)
+            rows = self._call_load(ptr, nb, kind, c_void_p(out.ctypes.data), pts, PTR_HOST)
+        del keep
+        return out[:rows]
+
+    def load(self, path: str, device_out: bool = False):
+        """load_bytes of the file at path"""
+        with open(path, "rb") as f:
+            data = f.read()
+        return self.load_bytes(data, device_out)
+
+    def last_load_info(self) -> dict:
+        """erasor_pcd_load_info_t of the last load: data_mode, fields, intensity_zero_filled, point_step, width, height, points,
+        data_offset, compressed_size, uncompressed_size, lzf_tokens, and the ascii branch's info as a dict under "ascii" """
+        info = getattr(self, "_load_info", None)
+        return dict(info) if info is not None else None
 
     def _format(self, xyzi) -> np.ndarray:
         if hasattr(xyzi, "is_cuda") and xyzi.is_cuda:

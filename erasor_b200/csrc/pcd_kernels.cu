@@ -11,6 +11,9 @@
 //                         against FIELDS, parse the kept columns on the fast path; the first bad line wins an atomicMin;
 //   5. k_pcd_parse_slow   one thread per row holding a token the fast path left (limbs in local memory), only when there is one.
 // Format: k_pcd_fmt_len gives every line's length, an exclusive scan its offset, k_pcd_fmt_write writes it after the header.
+// Load (erasor_pcd_load, DESIGN.md section 12.1): ascii goes to the parse above; binary is one pass of k_pcd_gather_tile; a
+// binary_compressed stream is decoded by k_lzf_walk (speculative token discovery), k_lzf_compose (scan of the chunks' entry maps),
+// k_lzf_records, k_lzf_expand / k_lzf_jump / k_lzf_fill (pointer jumping over back-references), then gathered by k_pcd_gather.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -20,6 +23,7 @@
 #include <vector>
 
 #include "../../include/erasor_b200.h"
+#include "pcd_binary.h"
 #include "pcd_codec.h"
 
 namespace {
@@ -308,51 +312,117 @@ struct DevBuf {
 };
 thread_local std::string g_pcd_err;
 
-// what the host reads of the header
-struct Header {
-    std::vector<std::string> fields;
-    std::vector<std::string> counts;
-    unsigned long long points = 0;
-    bool have_points = false, have_data = false;
-    std::string data;
-    uint64_t data_off = 0;       // first byte after the DATA line
-    uint64_t lines = 0;          // lines before data_off
-};
+using pcd::Header;
+using pcd::parse_header;
 
-bool blank(char c) { return pcd::is_ws((uint8_t)c); }
+// ---- binary and binary_compressed (DESIGN.md section 12.1; the per-item logic is pcd_binary.h) ----------------------------
+constexpr int kGatherThreads = 256;
+constexpr uint32_t kGatherTile = 16384;              // file bytes a CTA stages in shared memory per iteration
+constexpr uint64_t kLzfChunk = 4096;                  // compressed bytes per chunk of the token discovery
 
-// header lines up to and including DATA; false when the text ends before a DATA line
-bool parse_header(const char* s, uint64_t n, Header& h) {
-    uint64_t p = 0;
-    while (p < n) {
-        uint64_t e = p;                              // the line ends at '\n', "\r\n" or a lone '\r' (universal newlines)
-        while (e < n && s[e] != '\n' && s[e] != '\r') ++e;
-        std::vector<std::string> tok;
-        for (uint64_t q = p; q < e;) {
-            while (q < e && blank(s[q])) ++q;
-            const uint64_t a = q;
-            while (q < e && !blank(s[q])) ++q;
-            if (q > a) tok.emplace_back(s + a, q - a);
-        }
-        ++h.lines;
-        const uint64_t next = e >= n ? n : (s[e] == '\r' && e + 1 < n && s[e + 1] == '\n') ? e + 2 : e + 1;
-        if (!tok.empty()) {
-            if (tok[0] == "FIELDS") h.fields.assign(tok.begin() + 1, tok.end());
-            else if (tok[0] == "COUNT") h.counts.assign(tok.begin() + 1, tok.end());
-            else if (tok[0] == "POINTS" && tok.size() > 1) {
-                char* end = nullptr;
-                h.points = std::strtoull(tok[1].c_str(), &end, 10);
-                h.have_points = end && *end == 0 && tok[1][0] != '-';
-            } else if (tok[0] == "DATA") {
-                h.have_data = true;
-                h.data = tok.size() > 1 ? tok[1] : std::string();
-                h.data_off = next;
-                return true;
+// binary: a tile of points is staged with 16-byte aligned loads (bytes of a 16-byte block that lie outside the body are read one by
+// one, so nothing outside [body, body + points * stride) is touched), then every thread extracts its points' four fields at any
+// offset and stride and writes one 16-byte value per point
+__global__ void __launch_bounds__(kGatherThreads) k_pcd_gather_tile(const uint8_t* body, uint64_t points, pcd::Gather g, uint32_t per_tile,
+                                                                      uint4* out) {
+    __shared__ __align__(16) uint8_t tile[kGatherTile + 32];
+    const uintptr_t b = reinterpret_cast<uintptr_t>(body);
+    for (uint64_t p0 = (uint64_t)blockIdx.x * per_tile; p0 < points; p0 += (uint64_t)gridDim.x * per_tile) {
+        const uint64_t np = min((uint64_t)per_tile, points - p0);
+        const uintptr_t lo = b + p0 * g.stride, hi = b + (p0 + np) * g.stride;
+        const uintptr_t a0 = lo & ~uintptr_t(15), a1 = (hi + 15) & ~uintptr_t(15);
+        for (uintptr_t a = a0 + 16u * threadIdx.x; a < a1; a += 16u * blockDim.x) {
+            uint8_t* d = tile + (a - a0);
+            if (a >= lo && a + 16 <= hi) {
+                *reinterpret_cast<uint4*>(d) = *reinterpret_cast<const uint4*>(a);
+            } else {
+                for (int k = 0; k < 16; ++k) d[k] = (a + k >= lo && a + k < hi) ? *reinterpret_cast<const uint8_t*>(a + k) : 0;
             }
         }
-        p = next;
+        __syncthreads();
+        const uint8_t* t = tile + (lo - a0);
+        for (uint32_t i = threadIdx.x; i < np; i += blockDim.x) {
+            uint32_t v[4];
+            pcd::gather_point(t, g, i, v);
+            out[p0 + i] = make_uint4(v[0], v[1], v[2], v[3]);
+        }
+        __syncthreads();
     }
-    return false;
+}
+
+// one thread per point, straight from global memory: the decompressed SoA blocks, and binary points wider than a tile
+__global__ void __launch_bounds__(kGatherThreads) k_pcd_gather(const uint8_t* base, uint64_t points, pcd::Gather g, uint4* out) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < points; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint32_t v[4];
+        pcd::gather_point(base, g, i, v);
+        out[i] = make_uint4(v[0], v[1], v[2], v[3]);
+    }
+}
+
+// Stage A: one thread per (chunk, entry)
+__global__ void __launch_bounds__(kThreads) k_lzf_walk(const uint8_t* s, uint64_t csize, uint64_t nchunks, uint8_t* map, uint32_t* tokens,
+                                                       uint32_t* bytes) {
+    const uint64_t total = nchunks * pcd::kLzfEntries;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t k = i / pcd::kLzfEntries;
+        const uint64_t begin = k * kLzfChunk, end = min(begin + kLzfChunk, csize);
+        const pcd::LzfWalk w = pcd::lzf_walk(s, csize, begin, end, (uint32_t)(i - k * pcd::kLzfEntries));
+        map[i] = (uint8_t)w.exit;
+        tokens[i] = w.tokens;
+        bytes[i] = w.bytes;
+    }
+}
+
+// one round of the inclusive scan of the chunks' entry maps under composition: out_k = in_k o in_(k-d) (k >= d)
+__global__ void __launch_bounds__(kThreads) k_lzf_compose(const uint8_t* in, uint8_t* out, uint64_t nchunks, uint64_t d) {
+    const uint64_t total = nchunks * pcd::kLzfEntries;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t k = i / pcd::kLzfEntries;
+        const int e = (int)(i - k * pcd::kLzfEntries);
+        out[i] = k >= d ? pcd::lzf_compose(in + k * pcd::kLzfEntries, in + (k - d) * pcd::kLzfEntries, e) : in[i];
+    }
+}
+
+// the true entry of every chunk (chunk 0 starts at its first byte) and its chain's token and byte counts
+__global__ void __launch_bounds__(kThreads) k_lzf_true(const uint8_t* scanned, const uint32_t* tokens, const uint32_t* bytes, uint64_t nchunks,
+                                                       uint32_t* entry, uint32_t* ctok, uint32_t* cbyt) {
+    for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nchunks; k += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t e = k ? scanned[(k - 1) * pcd::kLzfEntries] : 0u;
+        entry[k] = e;
+        ctok[k] = tokens[k * pcd::kLzfEntries + e];
+        cbyt[k] = bytes[k * pcd::kLzfEntries + e];
+    }
+}
+
+// Stage B: one thread per chunk; the first broken rule of the stream wins an atomicMin
+__global__ void __launch_bounds__(kThreads) k_lzf_records(const uint8_t* s, uint64_t csize, uint64_t usize, uint64_t nchunks, const uint32_t* entry,
+                                                          const uint64_t* tok_off, const uint64_t* byte_off, pcd::LzfToken* rec,
+                                                          unsigned long long* err) {
+    for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nchunks; k += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t begin = k * kLzfChunk, end = min(begin + kLzfChunk, csize);
+        uint64_t e;
+        pcd::lzf_records(s, csize, usize, begin, end, entry[k], byte_off[k], rec + tok_off[k], &e);
+        if (e != ~0ull) atomicMin(err, (unsigned long long)e);
+    }
+}
+
+// Stage C
+__global__ void __launch_bounds__(kThreads) k_lzf_expand(const pcd::LzfToken* rec, uint64_t ntok, const uint8_t* s, uint8_t* out, uint32_t* src,
+                                                         uint64_t keep) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < ntok; i += (uint64_t)gridDim.x * blockDim.x)
+        if (rec[i].dst < keep) pcd::lzf_expand(rec[i], s, out, src, keep);
+}
+
+__global__ void __launch_bounds__(kThreads) k_lzf_jump(uint32_t* src, uint64_t keep, unsigned int* moved) {
+    bool any = false;
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < keep; j += (uint64_t)gridDim.x * blockDim.x)
+        any |= pcd::lzf_jump(src, j);
+    if (__syncthreads_or(any) && threadIdx.x == 0) atomicOr(moved, 1u);
+}
+
+__global__ void __launch_bounds__(kThreads) k_lzf_fill(const uint32_t* src, uint8_t* out, uint64_t keep) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < keep; j += (uint64_t)gridDim.x * blockDim.x)
+        pcd::lzf_fill(src, out, j);
 }
 
 uint32_t blocks_for(uint64_t n, int per, int cap) { return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + per - 1) / per, (uint64_t)cap)); }
@@ -364,6 +434,7 @@ struct erasor_pcd_ctx {
     std::string err;
     DevBuf text, chunk_cnt, chunk_off, lines, flags, rows, sums, out, stats;   // parse
     DevBuf pts, lens, offs, ftext;                                              // format
+    DevBuf lz_map0, lz_map1, lz_tok, lz_byt, lz_entry, lz_ctok, lz_cbyt, lz_tokoff, lz_byteoff, lz_rec, lz_src, lz_dec, lz_flags;   // load
     PcdStats* h_stats = nullptr;                                                // pinned
     int sm_count = 132;
     // erasor_pcd_format_ascii's text of its last call, kept for a following call with the same input
@@ -395,7 +466,92 @@ int scan_u32(erasor_pcd_t p, const uint32_t* in, uint64_t n, uint64_t* out, uint
     return ERASOR_OK;
 }
 
-const char* kHeadFmt = "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z intensity\nSIZE 4 4 4 4\nTYPE F F F F\n"
+// The header of a host or device file (from a device file, growing prefixes until the DATA line is in)
+int read_header(erasor_pcd_t p, const char* text, uint64_t len, int text_kind, Header& h, bool& found) {
+    found = false;
+    if (text_kind == ERASOR_PTR_HOST) {
+        found = parse_header(text, len, h);
+        return ERASOR_OK;
+    }
+    std::vector<char> pre;
+    for (uint64_t m = std::min<uint64_t>(len, 1 << 16);; m = std::min<uint64_t>(len, 4 * m)) {
+        pre.resize(m);
+        PCK(cudaMemcpy(pre.data(), text, m, cudaMemcpyDeviceToHost));
+        h = Header();
+        found = parse_header(pre.data(), m, h) && (h.data_off < m || m == len);   // the DATA line's end lies inside the prefix
+        if (found || m == len) break;
+    }
+    return ERASOR_OK;
+}
+
+// The LZF stream s (device) -> p->lz_dec, of which the first keep bytes are materialised; the whole stream is validated.
+int lzf_decode(erasor_pcd_t p, const uint8_t* s, uint64_t csize, uint64_t usize, uint64_t keep, uint64_t* ntok) {
+    const uint64_t nchunks = (csize + kLzfChunk - 1) / kLzfChunk;
+    const uint64_t nent = nchunks * pcd::kLzfEntries;
+    const uint32_t g_ent = blocks_for(nent, kThreads, p->sm_count * 16), g_ch = blocks_for(nchunks, kThreads, p->sm_count * 16);
+    *ntok = 0;
+    if (!nchunks) return usize ? fail(p, ERASOR_E_INVALID, "malformed LZF stream: it ends after 0 of " + std::to_string(usize) + " bytes") : ERASOR_OK;
+    // A. every chunk walked from each of its 33 possible entries, then the entry maps composed (log2(chunks) rounds)
+    PCK(p->lz_map0.ensure(nent));
+    PCK(p->lz_map1.ensure(nent));
+    PCK(p->lz_tok.ensure(sizeof(uint32_t) * nent));
+    PCK(p->lz_byt.ensure(sizeof(uint32_t) * nent));
+    k_lzf_walk<<<g_ent, kThreads, 0, p->st>>>(s, csize, nchunks, p->lz_map0.as<uint8_t>(), p->lz_tok.as<uint32_t>(), p->lz_byt.as<uint32_t>());
+    uint8_t *m_in = p->lz_map0.as<uint8_t>(), *m_out = p->lz_map1.as<uint8_t>();
+    for (uint64_t d = 1; d < nchunks; d *= 2) {
+        k_lzf_compose<<<g_ent, kThreads, 0, p->st>>>(m_in, m_out, nchunks, d);
+        std::swap(m_in, m_out);
+    }
+    PCK(p->lz_entry.ensure(sizeof(uint32_t) * nchunks));
+    PCK(p->lz_ctok.ensure(sizeof(uint32_t) * nchunks));
+    PCK(p->lz_cbyt.ensure(sizeof(uint32_t) * nchunks));
+    PCK(p->lz_tokoff.ensure(sizeof(uint64_t) * nchunks));
+    PCK(p->lz_byteoff.ensure(sizeof(uint64_t) * nchunks));
+    k_lzf_true<<<g_ch, kThreads, 0, p->st>>>(m_in, p->lz_tok.as<uint32_t>(), p->lz_byt.as<uint32_t>(), nchunks, p->lz_entry.as<uint32_t>(),
+                                             p->lz_ctok.as<uint32_t>(), p->lz_cbyt.as<uint32_t>());
+    PCK(cudaGetLastError());
+    uint64_t tokens = 0, bytes = 0;
+    int rc = scan_u32(p, p->lz_ctok.as<uint32_t>(), nchunks, p->lz_tokoff.as<uint64_t>(), &tokens);
+    if (rc == ERASOR_OK) rc = scan_u32(p, p->lz_cbyt.as<uint32_t>(), nchunks, p->lz_byteoff.as<uint64_t>(), &bytes);
+    if (rc != ERASOR_OK) return rc;
+    *ntok = tokens;
+    // B. token records along the true chain, every rule checked
+    PCK(p->lz_rec.ensure(sizeof(pcd::LzfToken) * tokens));
+    PCK(p->lz_flags.ensure(2 * sizeof(unsigned long long)));
+    unsigned long long* flags = p->lz_flags.as<unsigned long long>();
+    PCK(cudaMemsetAsync(flags, 0xFF, sizeof(unsigned long long), p->st));
+    k_lzf_records<<<g_ch, kThreads, 0, p->st>>>(s, csize, usize, nchunks, p->lz_entry.as<uint32_t>(), p->lz_tokoff.as<uint64_t>(),
+                                                p->lz_byteoff.as<uint64_t>(), p->lz_rec.as<pcd::LzfToken>(), flags);
+    PCK(cudaGetLastError());
+    unsigned long long err = 0;
+    PCK(cudaMemcpyAsync(&err, flags, sizeof(err), cudaMemcpyDeviceToHost, p->st));
+    PCK(cudaStreamSynchronize(p->st));
+    if (err != ~0ull) return fail(p, ERASOR_E_INVALID, pcd::lzf_error_message(err));
+    if (bytes != usize)
+        return fail(p, ERASOR_E_INVALID, "malformed LZF stream: it ends after " + std::to_string(bytes) + " of " + std::to_string(usize) + " bytes");
+    // C. literals copied, every other byte resolved to the literal it copies by pointer jumping
+    PCK(p->lz_dec.ensure(std::max<uint64_t>(keep, 1)));
+    PCK(p->lz_src.ensure(sizeof(uint32_t) * std::max<uint64_t>(keep, 1)));
+    uint8_t* dec = p->lz_dec.as<uint8_t>();
+    uint32_t* src = p->lz_src.as<uint32_t>();
+    const uint32_t g_keep = blocks_for(keep, kThreads, p->sm_count * 16);
+    k_lzf_expand<<<blocks_for(tokens, kThreads, p->sm_count * 16), kThreads, 0, p->st>>>(p->lz_rec.as<pcd::LzfToken>(), tokens, s, dec, src, keep);
+    PCK(cudaGetLastError());
+    unsigned int* moved = reinterpret_cast<unsigned int*>(flags + 1);
+    for (;;) {
+        unsigned int h_moved = 0;
+        PCK(cudaMemsetAsync(moved, 0, sizeof(unsigned int), p->st));
+        k_lzf_jump<<<g_keep, kThreads, 0, p->st>>>(src, keep, moved);
+        PCK(cudaMemcpyAsync(&h_moved, moved, sizeof(h_moved), cudaMemcpyDeviceToHost, p->st));
+        PCK(cudaStreamSynchronize(p->st));
+        if (!h_moved) break;
+    }
+    k_lzf_fill<<<g_keep, kThreads, 0, p->st>>>(src, dec, keep);
+    PCK(cudaGetLastError());
+    return ERASOR_OK;
+}
+
+const char* kHeadFmt ="# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z intensity\nSIZE 4 4 4 4\nTYPE F F F F\n"
                        "COUNT 1 1 1 1\nWIDTH %zu\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS %zu\nDATA ascii\n";
 }  // namespace
 
@@ -428,7 +584,8 @@ void erasor_pcd_destroy(erasor_pcd_t p) {
     cudaSetDevice(p->device);
     if (p->st) cudaStreamSynchronize(p->st);
     for (DevBuf* b : {&p->text, &p->chunk_cnt, &p->chunk_off, &p->lines, &p->flags, &p->rows, &p->sums, &p->out, &p->stats, &p->pts,
-                      &p->lens, &p->offs, &p->ftext}) b->release();
+                      &p->lens, &p->offs, &p->ftext, &p->lz_map0, &p->lz_map1, &p->lz_tok, &p->lz_byt, &p->lz_entry, &p->lz_ctok,
+                      &p->lz_cbyt, &p->lz_tokoff, &p->lz_byteoff, &p->lz_rec, &p->lz_src, &p->lz_dec, &p->lz_flags}) b->release();
     if (p->h_stats) cudaFreeHost(p->h_stats);
     if (p->st) cudaStreamDestroy(p->st);
     delete p;
@@ -448,21 +605,11 @@ int erasor_pcd_parse_ascii(erasor_pcd_t p, const char* text, size_t len, int tex
     PCK(cudaSetDevice(p->device));
     *n = 0;
     erasor_pcd_info_t inf{};
-    // 1. the header, on the host (from a device text, growing prefixes until the DATA line is in)
+    // 1. the header, on the host
     Header h;
     bool found = false;
-    if (text_kind == ERASOR_PTR_HOST) {
-        found = parse_header(text, len, h);
-    } else {
-        std::vector<char> pre;
-        for (uint64_t m = std::min<uint64_t>(len, 1 << 16);; m = std::min<uint64_t>(len, 4 * m)) {
-            pre.resize(m);
-            PCK(cudaMemcpy(pre.data(), text, m, cudaMemcpyDeviceToHost));
-            h = Header();
-            found = parse_header(pre.data(), m, h) && (h.data_off < m || m == len);   // the DATA line's end lies inside the prefix
-            if (found || m == len) break;
-        }
-    }
+    const int hrc = read_header(p, text, len, text_kind, h, found);
+    if (hrc != ERASOR_OK) return hrc;
     if (!found) return fail(p, ERASOR_E_INVALID, "no DATA line in the PCD header");
     for (size_t k = 0; k < h.fields.size(); ++k) {
         const std::string& f = h.fields[k];
@@ -613,6 +760,86 @@ int erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_
     PCK(cudaMemcpyAsync(out, p->ftext.p, p->c_len, out_kind == ERASOR_PTR_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, p->st));
     PCK(cudaStreamSynchronize(p->st));
     return ERASOR_OK;
+}
+
+int erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind, float* out_xyzi, size_t cap, int out_kind, size_t* n,
+                    erasor_pcd_load_info_t* info) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    p->cached = false;
+    erasor_pcd_load_info_t inf{};
+    if (info) *info = inf;
+    auto done = [&](int rc) { if (info) *info = inf; return rc; };
+    if (!n || (len && !file)) return fail(p, ERASOR_E_INVALID, "null argument");
+    if ((file_kind != ERASOR_PTR_HOST && file_kind != ERASOR_PTR_DEVICE) || (out_kind != ERASOR_PTR_HOST && out_kind != ERASOR_PTR_DEVICE))
+        return fail(p, ERASOR_E_INVALID, "file_kind and out_kind must be ERASOR_PTR_HOST or ERASOR_PTR_DEVICE");
+    PCK(cudaSetDevice(p->device));
+    *n = 0;
+    Header h;
+    bool found = false;
+    int rc = read_header(p, file, len, file_kind, h, found);
+    if (rc != ERASOR_OK) return rc;
+    if (!found) return fail(p, ERASOR_E_INVALID, "no DATA line in the PCD header");
+    pcd::Layout L;
+    std::string msg;
+    rc = pcd::resolve_layout(h, L, msg);
+    pcd::fill_load_info(h, L, inf);
+    if (rc != ERASOR_OK) return done(fail(p, rc, msg));
+    if (L.mode == pcd::DATA_ASCII) {
+        rc = erasor_pcd_parse_ascii(p, file, len, file_kind, out_xyzi, cap, out_kind, n, &inf.ascii);
+        inf.fields = inf.ascii.fields;
+        return done(rc);
+    }
+    if (L.mode == pcd::DATA_BINARY && (rc = pcd::check_binary_body(L, h.data_off, len, msg)) != ERASOR_OK) return done(fail(p, rc, msg));
+    if (!L.points) return done(ERASOR_OK);                                          // reads no data
+    uint64_t csize = 0, usize = 0;
+    if (L.mode == pcd::DATA_COMPRESSED) {
+        if (len - h.data_off < 8) return done(fail(p, ERASOR_E_INVALID, "the file ends before compressed_size and uncompressed_size"));
+        uint8_t sz[8];
+        if (file_kind == ERASOR_PTR_HOST) std::memcpy(sz, file + h.data_off, 8);
+        else PCK(cudaMemcpy(sz, file + h.data_off, 8, cudaMemcpyDeviceToHost));
+        csize = pcd::le32(sz);
+        usize = pcd::le32(sz + 4);
+        inf.compressed_size = csize;
+        inf.uncompressed_size = usize;
+        if ((rc = pcd::check_compressed_sizes(L, h.data_off, len, csize, usize, msg)) != ERASOR_OK) return done(fail(p, rc, msg));
+    }
+    if (!out_xyzi) { *n = (size_t)L.points; return done(ERASOR_OK); }
+    if (cap < L.points) return done(fail(p, ERASOR_E_CAPACITY, "out_xyzi holds fewer points than the header's POINTS"));
+    if (out_kind == ERASOR_PTR_DEVICE && (reinterpret_cast<uintptr_t>(out_xyzi) & 15u))
+        return done(fail(p, ERASOR_E_INVALID, "device clouds must be 16-byte aligned (one float4 per point)"));
+
+    // the body (binary) or the stream (binary_compressed) on the device
+    const uint64_t body = L.mode == pcd::DATA_BINARY ? L.points * L.point_step : csize;
+    const uint64_t at = h.data_off + (L.mode == pcd::DATA_BINARY ? 0 : 8);
+    const uint8_t* d_in = reinterpret_cast<const uint8_t*>(file) + at;
+    if (file_kind == ERASOR_PTR_HOST) {
+        PCK(p->text.ensure(std::max<uint64_t>(body, 1)));
+        PCK(cudaMemcpyAsync(p->text.p, file + at, body, cudaMemcpyHostToDevice, p->st));
+        d_in = p->text.as<uint8_t>();
+    }
+    uint4* d_out = reinterpret_cast<uint4*>(out_xyzi);
+    if (out_kind == ERASOR_PTR_HOST) { PCK(p->out.ensure(sizeof(uint4) * L.points)); d_out = p->out.as<uint4>(); }
+    const uint32_t g_pts = blocks_for(L.points, kGatherThreads, p->sm_count * 16);
+    if (L.mode == pcd::DATA_BINARY) {
+        if (L.point_step <= kGatherTile) {
+            const uint32_t per_tile = (uint32_t)std::min<uint64_t>(4 * kGatherThreads, kGatherTile / L.point_step);
+            k_pcd_gather_tile<<<blocks_for(L.points, per_tile, p->sm_count * 8), kGatherThreads, 0, p->st>>>(d_in, L.points, L.g, per_tile, d_out);
+        } else {
+            k_pcd_gather<<<g_pts, kGatherThreads, 0, p->st>>>(d_in, L.points, L.g, d_out);
+        }
+    } else {
+        uint64_t ntok = 0;
+        rc = lzf_decode(p, d_in, csize, usize, L.keep_end, &ntok);
+        inf.lzf_tokens = ntok;
+        if (rc != ERASOR_OK) { cudaStreamSynchronize(p->st); return done(rc); }
+        k_pcd_gather<<<g_pts, kGatherThreads, 0, p->st>>>(p->lz_dec.as<uint8_t>(), L.points, L.g, d_out);
+    }
+    PCK(cudaGetLastError());
+    if (out_kind == ERASOR_PTR_HOST) PCK(cudaMemcpyAsync(out_xyzi, d_out, sizeof(uint4) * L.points, cudaMemcpyDeviceToHost, p->st));
+    PCK(cudaStreamSynchronize(p->st));
+    *n = (size_t)L.points;
+    return done(ERASOR_OK);
 }
 
 }  // extern "C"

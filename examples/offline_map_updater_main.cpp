@@ -1,9 +1,9 @@
 // examples/offline_map_updater_main.cpp -- ROS-free counterpart of the reference's file-based driver
 // src/offline_map_updater/main_in_your_env.cpp:60-127: reads <data_dir>/dense_global_map.pcd,
 // <data_dir>/poses_lidar2body.csv (header line, then  idx,time,x,y,z,qx,qy,qz,qw ; columns 2..8 are used, :46-49)
-// and <data_dir>/pcds/%06d.pcd (ASCII files parsed on the device by PcdCodec, binary ones read by load_pcd and uploaded), feeds
-// every node to the device-resident OfflineMapUpdater and writes <save_path>/<data_name>_result.pcd with save_static_map(0.2)
-// (:123), formatted on the device.  The reference reads either kind with pcl::io::loadPCDFile.
+// and <data_dir>/pcds/%06d.pcd (each read on the device by PcdCodec::load, in any DATA mode: ascii, binary or binary_compressed, as
+// the reference's pcl::io::loadPCDFile reads them), feeds every node to the device-resident OfflineMapUpdater and writes
+// <save_path>/<data_name>_result.pcd with save_static_map(0.2) (:123), formatted on the device.
 //   usage: offline_map_updater_main <config.yaml> <data_dir> [init_idx]
 #include <cstdio>
 #include <cstdlib>
@@ -42,18 +42,9 @@ private:
     size_t n_ = 0, cap_ = 0;
 };
 
-// An ASCII scan is parsed on the device straight into `out`; a binary one (which the codec leaves to load_pcd) is read on the host
-// and copied up.  Either way the scan is complete in device memory on return.
+// The scan is read on the device straight into `out`, complete on return.
 static void read_scan(PcdCodec& codec, const std::string& path, DeviceCloud& out) {
-    try {
-        out.set_size(codec.read_device(path, [&](size_t n) { return out.reserve(n); }));
-    } catch (const UnsupportedPcd&) {
-        const PointCloud c = load_pcd(path);
-        float* d = out.reserve(c.size());
-        if (!c.empty() && cudaMemcpy(d, c.data(), sizeof(float) * 4 * c.size(), cudaMemcpyHostToDevice) != cudaSuccess)
-            throw std::runtime_error("cannot upload " + path);
-        out.set_size(c.size());
-    }
+    out.set_size(codec.load_device(path, [&](size_t n) { return out.reserve(n); }));
 }
 
 static std::vector<std::array<double, 7>> load_all_poses(const std::string& txt) {
@@ -81,15 +72,13 @@ int main(int argc, char** argv) {
         const std::string data_dir = argv[2];
         const int init_idx = argc > 3 ? std::atoi(argv[3]) : 0;
         cfg.initial_map_path = data_dir + "/dense_global_map.pcd";
-        // ASCII PCDs (what the reference writes) are parsed on the device; a binary map is read by load_pcd
         PcdCodec codec;
-        PointCloud map;
-        try { map = codec.read(cfg.initial_map_path); } catch (const UnsupportedPcd&) { map = load_pcd(cfg.initial_map_path); }
+        PointCloud map = codec.load(cfg.initial_map_path);
         OfflineMapUpdater updater(cfg, map);
         PointCloud().swap(map);
         const auto poses = load_all_poses(data_dir + "/poses_lidar2body.csv");
-        // Scans come from files, so the next one is known: it is parsed on the device (into device memory, complete when
-        // read_device returns) before the current node is processed and, when that next call will process its node
+        // Scans come from files, so the next one is known: it is read on the device (into device memory, complete when
+        // load_device returns) before the current node is processed and, when that next call will process its node
         // (removal_interval), handed to the updater's look-ahead -- its voxelisation then runs under the current node's path.
         auto scan_path = [&](int i) { char name[64]; std::snprintf(name, sizeof(name), "/pcds/%06d.pcd", i); return data_dir + name; };
         const int n_nodes = (int)poses.size();

@@ -102,7 +102,9 @@ inline Config load_config(const std::string& yaml_path) {
     return c;
 }
 
-// PCD readers / writer for the file layouts the reference uses (ASCII and binary, FIELDS containing x y z intensity)
+// PCD readers / writer for the file layouts the reference uses (ASCII and binary, FIELDS containing x y z intensity).  load_pcd's
+// binary branch ignores COUNT and copies intensity as four raw bytes whatever its TYPE; PcdCodec::load follows PCL's rules instead
+// (DESIGN.md section 12.1 records the divergence).
 inline PointCloud load_pcd(const std::string& path) {
     std::ifstream f(path, std::ios::binary);
     if (!f) throw std::invalid_argument("Maybe intiial map path is not correct!");      // OfflineMapUpdater.cpp:125 (sic)
@@ -150,9 +152,10 @@ inline void save_pcd_ascii(const std::string& path, const PointCloud& c) {
     for (const auto& p : c) f << p.x << ' ' << p.y << ' ' << p.z << ' ' << p.intensity << '\n';
 }
 
-// ASCII PCD files through the device codec (erasor_pcd_*): the reader gives what load_pcd gives bit for bit (intensity 0 when the
-// file has none), the writer the bytes save_pcd_ascii writes (NaN spelled "nan").  Binary files are not parsed here
-// (UnsupportedPcd): load_pcd reads them.
+// PCD files through the device codec (erasor_pcd_*).  read / read_device parse ASCII files and give what load_pcd gives bit for bit
+// (intensity 0 when the file has none); binary files are UnsupportedPcd there.  load / load_device read every DATA mode (ascii,
+// binary, binary_compressed) with PCL's field rules (DESIGN.md section 12.1).  The writer gives the bytes save_pcd_ascii writes
+// (NaN spelled "nan").
 struct UnsupportedPcd : std::runtime_error { using std::runtime_error::runtime_error; };
 
 class PcdCodec {
@@ -181,6 +184,25 @@ public:
         check(erasor_pcd_parse_ascii(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, nullptr, 0, ERASOR_PTR_HOST, &n, nullptr), path);
         PointCloud c(n);
         check(erasor_pcd_parse_ascii(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, reinterpret_cast<float*>(c.data()), n, ERASOR_PTR_HOST, &n, nullptr), path);
+        c.resize(n);
+        return c;
+    }
+    // erasor_pcd_load: the file at path, in any DATA mode, into device memory (device_buffer as for read_device) or a host cloud
+    template <class DeviceBuffer>
+    size_t load_device(const std::string& path, DeviceBuffer&& device_buffer) {
+        slurp(path);
+        size_t n = 0;
+        check(erasor_pcd_load(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, nullptr, 0, ERASOR_PTR_DEVICE, &n, nullptr), path);
+        float* out = device_buffer(n);
+        check(erasor_pcd_load(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, out, n, ERASOR_PTR_DEVICE, &n, nullptr), path);
+        return n;
+    }
+    PointCloud load(const std::string& path) {
+        slurp(path);
+        size_t n = 0;
+        check(erasor_pcd_load(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, nullptr, 0, ERASOR_PTR_HOST, &n, nullptr), path);
+        PointCloud c(n);
+        check(erasor_pcd_load(p_, text_.data(), text_.size(), ERASOR_PTR_HOST, reinterpret_cast<float*>(c.data()), n, ERASOR_PTR_HOST, &n, nullptr), path);
         c.resize(n);
         return c;
     }

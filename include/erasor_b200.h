@@ -397,6 +397,28 @@ int  erasor_pcd_parse_ascii(erasor_pcd_t p, const char* text, size_t len, int te
  * for the following call with the same (xyzi, n, in_kind), which then only copies it out.  out: host or device per out_kind. */
 int  erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_kind, char* out, size_t cap, int out_kind, size_t* len);
 
+/* Any PCD DATA mode on the device (DESIGN.md section 12.1), with the field rules of PCL 1.8's PCDReader and
+ * fromPCLPointCloud2<PointXYZI> (restated; PCL is not built here).  ascii goes to erasor_pcd_parse_ascii unchanged (results, errors
+ * and info->ascii).  binary and binary_compressed: SIZE and TYPE are required (F 4/8, I/U 1/2/4, else ERASOR_E_UNSUPPORTED); COUNT is
+ * optional (default 1); FIELDS/SIZE/TYPE/COUNT of different lengths, WIDTH x HEIGHT != POINTS, a file shorter than its header
+ * promises, uncompressed_size != POINTS x point_step and a malformed LZF stream are ERASOR_E_INVALID.  x, y and z must be F 4 COUNT
+ * 1 (else ERASOR_E_UNSUPPORTED); intensity is taken when it is F 4 COUNT 1 and is 0 otherwise, as is a missing one.  Values are
+ * copied bit for bit.  Arguments as erasor_pcd_parse_ascii: file in host or device memory, out_xyzi == NULL only asks for
+ * *n = POINTS, a device out_xyzi is 16-byte aligned, the call is synchronous and info (nullable) is written on every return. */
+typedef struct {
+    uint32_t data_mode;              /* 0 ascii, 1 binary, 2 binary_compressed */
+    uint32_t fields;                 /* bit 0 x, 1 y, 2 z, 3 intensity: which of them the cloud takes from the file */
+    uint32_t intensity_zero_filled;  /* binary modes: FIELDS names intensity, but not as TYPE F SIZE 4 COUNT 1 -> 0, as PCL does */
+    uint32_t point_step;             /* binary: bytes per point in the file; binary_compressed: sum of the non-"_" fields' bytes */
+    uint64_t width, height, points;
+    uint64_t data_offset;            /* first byte after the DATA line */
+    uint64_t compressed_size, uncompressed_size, lzf_tokens;   /* binary_compressed only */
+    erasor_pcd_info_t ascii;         /* the ascii branch's info, exactly as erasor_pcd_parse_ascii writes it */
+} erasor_pcd_load_info_t;
+
+int  erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind, float* out_xyzi, size_t cap, int out_kind,
+                     size_t* n, erasor_pcd_load_info_t* info);
+
 #ifdef __cplusplus
 }
 #endif
