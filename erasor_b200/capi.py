@@ -39,6 +39,8 @@ EXPORTS = [
     "erasor_eval_count_selected",
     "erasor_pcd_create", "erasor_pcd_destroy", "erasor_pcd_last_error", "erasor_pcd_parse_ascii", "erasor_pcd_format_ascii",
     "erasor_pcd_load",
+    "erasor_mapgen_create", "erasor_mapgen_destroy", "erasor_mapgen_last_error", "erasor_mapgen_accum", "erasor_mapgen_get_cloud",
+    "erasor_mapgen_device_cloud", "erasor_mapgen_synchronize", "erasor_mapgen_get_counters",
 ]
 NO_MATCH = 0xFFFFFFFF        # erasor_evaluate's match entry of a GT point without an inlier
 
@@ -64,6 +66,11 @@ class PcdLoadInfoC(ctypes.Structure):
     _fields_ = [(name, c_uint32) for name in ("data_mode", "fields", "intensity_zero_filled", "point_step")] + \
                [(name, c_uint64) for name in ("width", "height", "points", "data_offset", "compressed_size", "uncompressed_size", "lzf_tokens")] + \
                [("ascii", PcdInfoC)]
+
+
+class MapGenParamsC(ctypes.Structure):
+    """erasor_mapgen_params_t"""
+    _fields_ = [("leafsize", c_float), ("is_large_scale", c_int)]
 
 
 class UpdaterParamsC(ctypes.Structure):
@@ -182,6 +189,16 @@ def _load():
     L.erasor_pcd_parse_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdInfoC)]
     L.erasor_pcd_format_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t)]
     L.erasor_pcd_load.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdLoadInfoC)]
+    L.erasor_mapgen_create.argtypes = [POINTER(MapGenParamsC), c_int, POINTER(c_void_p)]
+    L.erasor_mapgen_destroy.restype = None
+    L.erasor_mapgen_destroy.argtypes = [c_void_p]
+    L.erasor_mapgen_last_error.restype = c_char_p
+    L.erasor_mapgen_last_error.argtypes = [c_void_p]
+    L.erasor_mapgen_accum.argtypes = [c_void_p, POINTER(c_double), c_void_p, c_size_t, c_int]
+    L.erasor_mapgen_get_cloud.argtypes = [c_void_p, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t)]
+    L.erasor_mapgen_device_cloud.argtypes = [c_void_p, c_int, POINTER(c_void_p), POINTER(c_size_t)]
+    L.erasor_mapgen_synchronize.argtypes = [c_void_p]
+    L.erasor_mapgen_get_counters.argtypes = [c_void_p, POINTER(c_uint64), POINTER(c_uint64), POINTER(c_uint64)]
     return L
 
 
@@ -949,3 +966,80 @@ class PcdCodec:
         out = self._format(xyzi)
         with open(path, "wb") as f:
             f.write(memoryview(out))
+
+
+class MapGen:
+    """One ``erasor_mapgen_t``: the reference's mapgen (src/mapgen/mapgen.hpp:198-305) with its map resident on the device
+    (DESIGN.md section 8.2).  ``accum`` is accumPointCloud -- one launch, no host synchronisation unless a buffer grows; ``cloud``
+    gives the four clouds of ``OracleMapGen`` by the same ids; ``save_naive_map`` is saveNaiveMap without the files."""
+    CLOUD_MAP, CLOUD_CURR, SAVED_ORIGINAL, SAVED_VOXELIZED = 0, 1, 2, 3
+
+    def __init__(self, leafsize: float = 0.05, is_large_scale: bool = False, device: int = 0):
+        self.L = lib()
+        self.device = device
+        self._p = MapGenParamsC(float(leafsize), 1 if is_large_scale else 0)
+        h = c_void_p()
+        rc = self.L.erasor_mapgen_create(ctypes.byref(self._p), device, ctypes.byref(h))
+        if rc != OK:
+            raise ErasorError(rc, (self.L.erasor_mapgen_last_error(None) or b"").decode())
+        self.h = h
+
+    def _ck(self, rc: int):
+        if rc != OK:
+            raise ErasorError(rc, (self.L.erasor_mapgen_last_error(self.h) or b"").decode())
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.erasor_mapgen_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def accum(self, odom7, lidar):
+        """accumPointCloud with a host scan (float32 [n, 4] in the lidar frame; odom7 = x y z qx qy qz qw)."""
+        o = np.ascontiguousarray(odom7, dtype=np.float64)
+        c = _cloud(lidar)
+        self._ck(self.L.erasor_mapgen_accum(self.h, o.ctypes.data_as(POINTER(c_double)), c.ctypes.data if len(c) else None, len(c), PTR_HOST))
+
+    def accum_ptr(self, odom7, lidar_ptr: int, n: int, ptr_kind: int = PTR_DEVICE):
+        """accumPointCloud with a raw pointer.  A device scan is read asynchronously: keep it unchanged until the next call that
+        returns data, or until synchronize()."""
+        o = np.ascontiguousarray(odom7, dtype=np.float64)
+        self._ck(self.L.erasor_mapgen_accum(self.h, o.ctypes.data_as(POINTER(c_double)), c_void_p(lidar_ptr) if lidar_ptr else None, n, ptr_kind))
+
+    def cloud(self, which: int) -> np.ndarray:
+        n = c_size_t(0)
+        self._ck(self.L.erasor_mapgen_get_cloud(self.h, which, None, 0, PTR_HOST, ctypes.byref(n)))
+        out = np.empty((n.value, 4), dtype=np.float32)
+        if n.value:
+            self._ck(self.L.erasor_mapgen_get_cloud(self.h, which, out.ctypes.data, n.value, PTR_HOST, ctypes.byref(n)))
+        return out
+
+    def device_cloud(self, which: int):
+        """(device pointer, n) of a cloud in the handle's memory, valid until the next accum."""
+        p, n = c_void_p(), c_size_t(0)
+        self._ck(self.L.erasor_mapgen_device_cloud(self.h, which, ctypes.byref(p), ctypes.byref(n)))
+        return int(p.value or 0), n.value
+
+    def save_naive_map(self):
+        """-> (original, voxelized): the clouds saveNaiveMap writes"""
+        return self.cloud(self.SAVED_ORIGINAL), self.cloud(self.SAVED_VOXELIZED)
+
+    def synchronize(self):
+        self._ck(self.L.erasor_mapgen_synchronize(self.h))
+
+    def counters(self) -> dict:
+        """kernel launches, host synchronisations and buffer regrowths since creation"""
+        a, b, c = c_uint64(), c_uint64(), c_uint64()
+        self._ck(self.L.erasor_mapgen_get_counters(self.h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)))
+        return {"launches": int(a.value), "host_syncs": int(b.value), "regrowths": int(c.value)}

@@ -153,6 +153,62 @@ __host__ __device__ inline VoxPlan vox_plan(void* tmp, uint32_t n) {
     return p;
 }
 
+// U1 of a fused launch, one function per phase (grid barriers between them are the caller's).
+// (0) selected points per chunk
+__device__ __forceinline__ void u1_count(const FusedJob& J, uint32_t pchunks, uint32_t* s_w) {
+    const int tid = threadIdx.x;
+    for (uint32_t vb = blockIdx.x; vb < pchunks; vb += gridDim.x) {
+        const uint32_t b0 = vb * PART_CHUNK, b1 = min(J.pn, b0 + PART_CHUNK);
+        uint32_t c = 0;
+        for (uint32_t i = b0 + tid; i < b1; i += FT) c += part_pred(J.P, J.pin[i]) ? 1u : 0u;
+        const uint32_t t = cta_sum(c, s_w);
+        if (tid == 0) J.chunk_tmp[vb] = t;
+    }
+}
+// (1) chunk offsets and the total (last CTA)
+__device__ __forceinline__ void u1_offsets(const FusedJob& J, uint32_t pchunks, uint32_t* s_part) {
+    if (blockIdx.x != gridDim.x - 1) return;
+    const uint32_t t = block_excl_scan(J.chunk_tmp, J.chunk_tmp, (int)pchunks, s_part);
+    if (threadIdx.x == 0) *J.d_total_sel = t;
+}
+// (2) stable scatter.  kChain: the selected points go through T_sel, then T_sel2 (two transformPointCloud calls in sequence, each
+// rounded on its own); the rest is not written.
+template <bool kChain>
+__device__ __forceinline__ void u1_scatter(const FusedJob& J, uint32_t pchunks, uint32_t* s_w) {
+    const int tid = threadIdx.x;
+    for (uint32_t vb = blockIdx.x; vb < pchunks; vb += gridDim.x) {
+        const uint32_t b0 = vb * PART_CHUNK, b1 = min(J.pn, b0 + PART_CHUNK);
+        uint32_t sel_base = J.chunk_tmp[vb];
+        uint32_t rest_base = b0 - sel_base;
+        for (uint32_t r0 = b0; r0 < b1; r0 += FT) {
+            const uint32_t i = r0 + tid;
+            const bool ok = i < b1;
+            const float4 p = ok ? J.pin[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+            const bool s = ok && part_pred(J.P, p);
+            uint32_t rank_sel, round;
+            cta_rank(s, s_w, rank_sel, round);
+            if (ok) {
+                if (kChain) {
+                    if (s) J.out_sel[sel_base + rank_sel] = pcl_affine(J.T_sel2.m, pcl_affine(J.T_sel.m, p));
+                } else {
+                    if (s) J.out_sel[sel_base + rank_sel] = J.xform_sel ? pcl_affine(J.T_sel.m, p) : p;
+                    else   J.out_rest[rest_base + (i - r0) - rank_sel] = p;
+                }
+            }
+            const uint32_t valid = min((uint32_t)FT, b1 - r0);
+            sel_base += round;
+            rest_base += valid - round;
+        }
+    }
+}
+
+// kChain = false: U1 and U3 are independent jobs and U1's phases ride in U3's first three (the updater's prologue).
+// kChain = true: the resident map generator's modes (FusedJob::map / d_map, DESIGN.md section 8).  With has_part, one mapgen
+// node: U1 runs first, then U3 voxelises U1's output out_sel[0 .. *d_total_sel) -- a count only the device knows -- and the voxels
+// go to vout and to the map at its tail d_map[0], which moves past them.  Without has_part, parking: U3 voxelises the map's current
+// chunk map[d_map[1] .. d_map[0]) into vout and, after a grid barrier (the 1-NN reads the chunk until then), moves the voxels to
+// the chunk's start, where the next chunk starts behind them.
+template <bool kChain>
 __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
     cg::grid_group grid = cg::this_grid();
     extern __shared__ uint32_t s_c[];        // [FW][RD] next free destination per digit, one row per warp (also the min/max staging)
@@ -160,21 +216,37 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
     __shared__ uint32_t s_part[34];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t G = gridDim.x, bid = blockIdx.x;
-    const uint32_t n = J.vn, pn = J.pn;
-    const VoxPlan vp = vox_plan(J.vtmp, n);
-    const uint32_t nseg = vp.nseg, SEG = vp.seg;
+    const uint32_t pchunks = (J.pn + PART_CHUNK - 1) / PART_CHUNK;
     VoxGrid* g = J.grid;
-    const uint32_t pchunks = (pn + PART_CHUNK - 1) / PART_CHUNK;
     // phase profile of CTA 0 (nanoseconds, %globaltimer): read back by erasor_updater_get_fused_profile
 #define PH(slot) do { if (bid == 0 && tid == 0) { unsigned long long t__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t__)); g->prof[slot] = t__; } } while (0)
     PH(0);
+    // the map's tail and chunk start, read by every CTA before the first barrier (CTA 0 moves them after one)
+    uint32_t map_tail = 0, map_chunk = 0;
+    if (kChain) {
+        const volatile uint32_t* dm = J.d_map;
+        map_tail = dm[0]; map_chunk = dm[1];
+        if (J.has_part) {
+            u1_count(J, pchunks, s_w);
+            grid.sync();
+            u1_offsets(J, pchunks, s_part);
+            grid.sync();
+            u1_scatter<true>(J, pchunks, s_w);
+            grid.sync();
+        }
+    }
+    const bool part = !kChain && J.has_part;             // the independent U1 job
+    const float4* const vin = !kChain ? J.vin : (J.has_part ? J.out_sel : J.map + map_chunk);
+    const uint32_t n = !kChain ? J.vn : (J.has_part ? *J.d_total_sel : map_tail - map_chunk);
+    const VoxPlan vp = vox_plan(J.vtmp, n);
+    const uint32_t nseg = vp.nseg, SEG = vp.seg;
 
     // ---- phase 0: getMinMax3D partials per CTA | partition: selected points per chunk ----
     if (n) {
         for (uint32_t i = bid * FT + tid; i < 2u * RD * (nseg + 1u); i += G * FT) vp.cnt_x[i] = 0u;      // both histogram matrices (contiguous)
         uint32_t mn[3] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu}, mx[3] = {0u, 0u, 0u};
         for (uint32_t i = bid * FT + tid; i < n; i += G * FT) {
-            const float4 p = J.vin[i];
+            const float4 p = vin[i];
             const uint32_t a = float_to_ordered(p.x + 0.0f), b = float_to_ordered(p.y + 0.0f), c = float_to_ordered(p.z + 0.0f);
             mn[0] = min(mn[0], a); mx[0] = max(mx[0], a);
             mn[1] = min(mn[1], b); mx[1] = max(mx[1], b);
@@ -193,15 +265,7 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
         }
         __syncthreads();
     }
-    if (J.has_part) {
-        for (uint32_t vb = bid; vb < pchunks; vb += G) {
-            const uint32_t b0 = vb * PART_CHUNK, b1 = min(pn, b0 + PART_CHUNK);
-            uint32_t c = 0;
-            for (uint32_t i = b0 + tid; i < b1; i += FT) c += part_pred(J.P, J.pin[i]) ? 1u : 0u;
-            const uint32_t t = cta_sum(c, s_w);
-            if (tid == 0) J.chunk_tmp[vb] = t;
-        }
-    }
+    if (part) u1_count(J, pchunks, s_w);
     grid.sync();
     PH(1);
 
@@ -234,10 +298,7 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
         }
         __syncthreads();
     }
-    if (J.has_part && bid == G - 1) {
-        const uint32_t t = block_excl_scan(J.chunk_tmp, J.chunk_tmp, (int)pchunks, s_part);
-        if (tid == 0) *J.d_total_sel = t;
-    }
+    if (part) u1_offsets(J, pchunks, s_part);
     grid.sync();
     PH(2);
 
@@ -248,34 +309,13 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
         const int ovf = g->overflow;
         const VoxelGridDims vg = g->dims;
         for (uint32_t e = bid * FT + tid; e < n; e += G * FT) {
-            const float4 p = J.vin[e];
+            const float4 p = vin[e];
             const uint32_t k = ovf ? e : voxel_key_of(vg, p.x, p.y, p.z);   // overflow ("Leaf size is too small"): one voxel per point
             vp.key_a[e] = k; vp.idx_a[e] = e;
             atomicAdd(&vp.cnt_x[(size_t)(k & (RD - 1u)) * nseg + e / SEG], 1u);      // pass 0's histogram (counts: order-free)
         }
     }
-    if (J.has_part) {
-        for (uint32_t vb = bid; vb < pchunks; vb += G) {
-            const uint32_t b0 = vb * PART_CHUNK, b1 = min(pn, b0 + PART_CHUNK);
-            uint32_t sel_base = J.chunk_tmp[vb];
-            uint32_t rest_base = b0 - sel_base;
-            for (uint32_t r0 = b0; r0 < b1; r0 += FT) {
-                const uint32_t i = r0 + tid;
-                const bool ok = i < b1;
-                const float4 p = ok ? J.pin[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-                const bool s = ok && part_pred(J.P, p);
-                uint32_t rank_sel, round;
-                cta_rank(s, s_w, rank_sel, round);
-                if (ok) {
-                    if (s) J.out_sel[sel_base + rank_sel] = J.xform_sel ? pcl_affine(J.T_sel.m, p) : p;
-                    else   J.out_rest[rest_base + (i - r0) - rank_sel] = p;
-                }
-                const uint32_t valid = min((uint32_t)FT, b1 - r0);
-                sel_base += round;
-                rest_base += valid - round;
-            }
-        }
-    }
+    if (part) u1_scatter<false>(J, pchunks, s_w);
     grid.sync();
     PH(3);
 
@@ -398,7 +438,13 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
     grid.sync();
     PH(13);
     const uint32_t n_vox = *J.d_n_out;
-    if (bid == 0 && tid == 0) { g->n_vox = n_vox; vp.vstart[n_vox] = n; }
+    if (bid == 0 && tid == 0) {
+        g->n_vox = n_vox; vp.vstart[n_vox] = n;
+        if (kChain) {                                  // every CTA has read the old values before the first barrier
+            if (J.has_part) { J.d_map[0] = map_tail + n_vox; }
+            else            { J.d_map[0] = map_chunk + n_vox; J.d_map[1] = map_chunk + n_vox; }
+        }
+    }
     for (uint32_t vb = bid; vb < hchunks; vb += G) {
         const uint32_t b0 = vb * PART_CHUNK, b1 = min(n, b0 + PART_CHUNK);
         uint32_t base = vp.chunk[vb];
@@ -418,14 +464,23 @@ __global__ void __launch_bounds__(FT, 1) k_node_fused(FusedJob J) {
     for (uint32_t v0 = ((uint32_t)warp * G + bid) * 32u; v0 < n_vox; v0 += G * FT) {     // 32 consecutive voxels per warp, warps dealt round-robin over the SMs
         const uint32_t v = v0 + lane;
         if (v >= n_vox) continue;
-        float4 c = voxel_centroid(J.vin, sidx, vp.vstart[v], vp.vstart[v + 1]);
+        float4 c = voxel_centroid(vin, sidx, vp.vstart[v], vp.vstart[v + 1]);
         if (!g->overflow) {        // else every point is its own voxel: the nearest point is itself (or an identical earlier one)
-            const uint32_t i = u3_nearest(J.vin, sidx, vp.vstart, vp.vkey, n_vox, g->dims, c);
-            if (i != kNoPoint) c.w = J.vin[i].w;
+            const uint32_t i = u3_nearest(vin, sidx, vp.vstart, vp.vkey, n_vox, g->dims, c);
+            if (i != kNoPoint) c.w = vin[i].w;
         }
-        J.vout[v] = J.xform_out ? pcl_affine(J.T_out.m, c) : c;
+        if (kChain) {
+            J.vout[v] = c;
+            if (J.has_part) J.map[map_tail + v] = c;          // cloud_map += cloud_curr
+        } else {
+            J.vout[v] = J.xform_out ? pcl_affine(J.T_out.m, c) : c;
+        }
     }
     PH(15);
+    if (kChain && !J.has_part) {                           // parking: the chunk is read; its voxels take its place
+        grid.sync();
+        for (uint32_t v = bid * FT + tid; v < n_vox; v += G * FT) J.map[map_chunk + v] = J.vout[v];
+    }
 #undef PH
 }
 
@@ -436,27 +491,42 @@ size_t voxelize_tmp_bytes(uint32_t n) {
     // key/idx ping-pong (4 arrays), two digit-histogram matrices + digit totals, head-chunk counters, voxel starts/keys, per-CTA min/max partials
     return sizeof(uint32_t) * ((size_t)4 * n + 2 * (size_t)RD * nseg + RD + partition_tmp_words(n) + 2 * ((size_t)n + 2) + 64 + 6 * (size_t)kFusedMaxGrid);
 }
+size_t voxelize_tmp_bytes_upto(uint32_t n) {
+    // every term of voxelize_tmp_bytes grows with n except the segment count, which drops where the segment length steps up;
+    // it never exceeds min(RS_MAX_SEGS, ceil(n / (32 RS_ROWS_MIN)))
+    const size_t nseg_max = std::min<size_t>(RS_MAX_SEGS, ((size_t)n + 32 * RS_ROWS_MIN - 1) / (32 * RS_ROWS_MIN));
+    const size_t nseg = ((size_t)n + rs_seg_len(n) - 1) / rs_seg_len(n);
+    return voxelize_tmp_bytes(n) + sizeof(uint32_t) * 2 * (size_t)RD * (nseg_max > nseg ? nseg_max - nseg : 0);
+}
 
-cudaError_t launch_node_fused(cudaStream_t st, const FusedJob& J, int sm_count, int max_ctas) {
+template <bool kChain>
+static cudaError_t launch_fused_kernel(cudaStream_t st, const FusedJob& J, uint32_t work, int sm_count, int max_ctas) {
     constexpr size_t SMEM = sizeof(uint32_t) * FW * RD;
     static int max_ctas_per_sm = -1;
     if (max_ctas_per_sm < 0) {
-        cudaError_t e = cudaFuncSetAttribute(k_node_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
+        cudaError_t e = cudaFuncSetAttribute(k_node_fused<kChain>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
         if (e != cudaSuccess) return e;
         int v = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_node_fused, FT, SMEM);
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_node_fused<kChain>, FT, SMEM);
         if (e != cudaSuccess) return e;
         max_ctas_per_sm = v;
     }
     if (max_ctas_per_sm < 1) return cudaErrorLaunchOutOfResources;
-    const uint32_t work = J.vn > J.pn ? J.vn : J.pn;
     uint32_t G = (work + FT - 1) / FT;
     const uint32_t cap = (uint32_t)std::min<long long>((long long)sm_count * max_ctas_per_sm, (long long)kFusedMaxGrid);
     G = G < 1u ? 1u : (G > cap ? cap : G);
     if (max_ctas > 0 && G > (uint32_t)max_ctas) G = (uint32_t)max_ctas;      // look-ahead jobs leave most SMs to the current node's path
     FusedJob jj = J;
     void* args[] = {&jj};
-    return cudaLaunchCooperativeKernel((const void*)k_node_fused, dim3(G), dim3(FT), args, SMEM, st);
+    return cudaLaunchCooperativeKernel((const void*)k_node_fused<kChain>, dim3(G), dim3(FT), args, SMEM, st);
+}
+
+cudaError_t launch_node_fused(cudaStream_t st, const FusedJob& J, int sm_count, int max_ctas) {
+    return launch_fused_kernel<false>(st, J, J.vn > J.pn ? J.vn : J.pn, sm_count, max_ctas);
+}
+
+cudaError_t launch_map_chained(cudaStream_t st, const FusedJob& J, int sm_count) {
+    return launch_fused_kernel<true>(st, J, J.vn > J.pn ? J.vn : J.pn, sm_count, 0);
 }
 
 }  // namespace erasor

@@ -39,10 +39,21 @@ struct FusedJob {
     // order; *d_total_sel receives the number selected
     int has_part; PartPred P; Mat4 T_sel; int xform_sel; const float4* pin; uint32_t pn; uint32_t* chunk_tmp /*partition_tmp_words(pn)*/;
     uint32_t* d_total_sel; float4* out_sel; float4* out_rest;
+    // chained mode only (launch_map_chained): the resident map of the map generator and its two device-held offsets,
+    // d_map[0] = tail (points in the map), d_map[1] = start of the current chunk; T_sel2 follows T_sel on the selected points
+    Mat4 T_sel2; float4* map; uint32_t* d_map;
 };
 size_t partition_tmp_words(uint32_t n);
 size_t voxelize_tmp_bytes(uint32_t n);
+size_t voxelize_tmp_bytes_upto(uint32_t n);   // enough for any cloud of at most n points (voxelize_tmp_bytes is not monotone in n)
 cudaError_t launch_node_fused(cudaStream_t st, const FusedJob& job, int sm_count, int max_ctas = 0 /*0: as many as the job wants, up to one per SM*/);
+// The chained mode of the same kernel (updater_kernels.cu), for the resident map generator (mapgen_capi.cu):
+//   has_part = 1  one mapgen node: U1 (P, T_sel then T_sel2 on the selected points, out_rest unused), grid barrier, U3 over
+//                 out_sel[0 .. *d_total_sel) into vout[0 .. *d_n_out) and map[d_map[0] ..); d_map[0] advances.
+//                 vin is unused; vn bounds the voxeliser's count (pn) and vtmp holds voxelize_tmp_bytes_upto(vn).
+//   has_part = 0  parking: U3 over map[d_map[1] .. d_map[0]) into vout, grid barrier, the voxels moved to map[d_map[1] ..);
+//                 both offsets end behind them.  vn bounds the chunk's size.
+cudaError_t launch_map_chained(cudaStream_t st, const FusedJob& job, int sm_count);
 
 cudaError_t launch_affine_copy(cudaStream_t st, const Mat4& T, bool do_transform, const float4* in, float4* out, uint32_t n);
 

@@ -13,6 +13,8 @@ device kernel behind `erasor_updater_voxelize` (`device_voxelizer()`), the same 
 oracle's C++ restatement of mapgen with the oracle's voxeliser injected.
 With `device_producer()` the whole per-node step (cut, lift, transform, voxelise) runs on the device through
 `erasor_updater_mapgen_node`; tests/test_gpu_mapgen.py holds both device compositions bit-identical to the oracle's mapgen.
+`device_generator()` (the default of `build_map`) keeps the map itself on the device too, behind `erasor_mapgen_*`
+(capi.MapGen): one launch per node, parking included; tests/test_gpu_mapgen_resident.py holds it to the oracle.
 """
 from __future__ import annotations
 
@@ -119,11 +121,49 @@ def device_producer(device: int = 0):
     return (lambda cloud, leaf: upd.voxelize(cloud, leaf)), (lambda odom7, lidar: upd.mapgen_node(odom7, lidar))
 
 
+class DeviceMapGenerator:
+    """NaiveMapGenerator's interface over the resident generator (capi.MapGen, DESIGN.md section 8.2): the map stays on the device,
+    one launch per node, no per-node copy back.  cloud_map / cloud_curr are read back on access."""
+
+    def __init__(self, leafsize: float = 0.05, is_large_scale: bool = False, device: int = 0):
+        from . import capi
+        self.leafsize, self.is_large_scale = float(leafsize), bool(is_large_scale)
+        self.gen = capi.MapGen(leafsize, is_large_scale, device=device)
+
+    def accum_point_cloud(self, odom7, lidar: np.ndarray) -> None:
+        self.gen.accum(odom7, lidar)
+
+    @property
+    def cloud_map(self) -> np.ndarray:
+        return self.gen.cloud(self.gen.CLOUD_MAP)
+
+    @property
+    def cloud_curr(self) -> np.ndarray:
+        return self.gen.cloud(self.gen.CLOUD_CURR)
+
+    def save_naive_map(self):
+        return self.gen.save_naive_map()
+
+    def close(self):
+        self.gen.close()
+
+
+def device_generator(leafsize: float = 0.05, is_large_scale: bool = False, device: int = 0) -> DeviceMapGenerator:
+    """The whole of mapgen on the device (needs a CUDA device: there is no CPU path)."""
+    return DeviceMapGenerator(leafsize, is_large_scale, device)
+
+
 def build_map(nodes, leafsize: float = 0.05, is_large_scale: bool = False, voxelize: Optional[Voxelizer] = None, node_producer=None):
     """nodes: iterable of (seq, odom7, cloud) (e.g. erasor_b200.kitti.iter_nodes) -> (original, voxelized) map clouds.
-    Without an injected voxeliser everything heavy runs on the device (needs a CUDA device)."""
+    Without an injected voxeliser everything runs on the device, map included (device_generator; needs a CUDA device)."""
     if voxelize is None:
-        voxelize, node_producer = device_producer()
+        gen = device_generator(leafsize, is_large_scale)
+        try:
+            for _, odom, cloud in nodes:
+                gen.accum_point_cloud(odom, cloud)
+            return gen.save_naive_map()
+        finally:
+            gen.close()
     gen = NaiveMapGenerator(voxelize, leafsize, is_large_scale, node_producer)
     for _, odom, cloud in nodes:
         gen.accum_point_cloud(odom, cloud)

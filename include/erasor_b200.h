@@ -419,6 +419,46 @@ typedef struct {
 int  erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind, float* out_xyzi, size_t cap, int out_kind,
                      size_t* n, erasor_pcd_load_info_t* info);
 
+/* ============================================================================================
+ * The naive map generator with its map resident on the device: the reference's mapgen (src/mapgen/mapgen.hpp:198-305,
+ * accumPointCloud / getPointClouds / saveNaiveMap without the files), DESIGN.md section 8.2.  A handle of its own: one CUDA
+ * device + one stream, not thread-safe; every function returns 0 or a negative error code and never throws.
+ * Per node: the 2.7 m vehicle-body cut, the 1.73 m lift, the pose, voxelize_preserving_labels at 0.2 m, appended to the map --
+ * one H2D copy (none for a device scan) and one kernel launch, with no host synchronisation unless a buffer has to grow.  In
+ * large-scale mode the map's current chunk is voxelised at leafsize and parked at the 2nd node, then every 500 nodes (one more
+ * launch).  Every call that returns data synchronises.
+ * ========================================================================================== */
+typedef struct erasor_mapgen_ctx* erasor_mapgen_t;
+
+typedef struct {
+    float leafsize;              /* /map/voxelsize (reference main.cpp:87, default 0.05) */
+    int   is_large_scale;        /* /large_scale/is_large_scale (main.cpp:95, default false) */
+} erasor_mapgen_params_t;
+
+/* cloud ids of erasor_mapgen_get_cloud / erasor_mapgen_device_cloud */
+enum { ERASOR_MAPGEN_CLOUD_MAP = 0,          /* cloud_map: the current chunk (the whole map unless large-scale) */
+       ERASOR_MAPGEN_CLOUD_CURR = 1,         /* cloud_curr: the last node's voxelised scan, map frame */
+       ERASOR_MAPGEN_SAVED_ORIGINAL = 2,     /* saveNaiveMap's <..>_original.pcd: the parked submaps, then cloud_map */
+       ERASOR_MAPGEN_SAVED_VOXELIZED = 3 };  /* saveNaiveMap's map: SAVED_ORIGINAL voxelised at leafsize (kept until the next accum) */
+
+/* ERASOR_E_INVALID: leafsize not positive and finite */
+int  erasor_mapgen_create(const erasor_mapgen_params_t* params, int device, erasor_mapgen_t* out);
+void erasor_mapgen_destroy(erasor_mapgen_t g);
+const char* erasor_mapgen_last_error(erasor_mapgen_t g);   /* g may be NULL: error of the last failed erasor_mapgen_create */
+/* accumPointCloud: odom7 = x y z qx qy qz qw (body -> map, double), lidar = n points x y z intensity in the lidar frame, host or
+ * device (ptr_kind; ERASOR_PTR_QUERY_XYZ is ERASOR_E_INVALID: the labels ride in intensity).  A DEVICE scan is read
+ * asynchronously: it must stay valid and unchanged until the next call that returns data, or until erasor_mapgen_synchronize.
+ * ERASOR_E_CAPACITY: n or the map would reach 2^31 points. */
+int  erasor_mapgen_accum(erasor_mapgen_t g, const double* odom7, const float* lidar_xyzi, size_t n, int ptr_kind);
+/* A cloud (ids above) into out_xyzi (host or device per out_kind); out_xyzi == NULL only returns *n; cap < *n is
+ * ERASOR_E_CAPACITY.  Synchronous. */
+int  erasor_mapgen_get_cloud(erasor_mapgen_t g, int which, float* out_xyzi, size_t cap, int out_kind, size_t* n);
+/* The same cloud in place, in the handle's device memory: no copy; valid until the next accum on this handle. */
+int  erasor_mapgen_device_cloud(erasor_mapgen_t g, int which, const float** d_xyzi, size_t* n);
+int  erasor_mapgen_synchronize(erasor_mapgen_t g);
+/* instrumentation: kernel launches, host synchronisations and buffer regrowths (each one synchronisation) since creation */
+int  erasor_mapgen_get_counters(erasor_mapgen_t g, uint64_t* launches, uint64_t* host_syncs, uint64_t* regrowths);
+
 #ifdef __cplusplus
 }
 #endif
