@@ -142,6 +142,7 @@ struct erasor_ctx {
     uint64_t desc_epoch = 0;                   // bumped whenever the descriptors are rebuilt (invalidates cached graphs)
     int      stat_F = 0;                       // frames of the last batch call (all its sub-batches): extent of the per-frame counters
     int      f0 = 0;                           // first frame of the sub-batch being submitted
+    std::vector<uint32_t> node_nvoi;           // node mode: |map_voi_| of the frames before f0 (the count tables hold the last sub-batch only)
     struct StepGraph { const void* ptr[8]; size_t fold_n; int kind, mode, f0; uint64_t epoch, alloc; cudaGraphExec_t exec; };
     std::vector<StepGraph> graphs;             // captured mask-mode steps, one per (pointers, geometry)
     bool     use_graphs = true;
@@ -1039,6 +1040,19 @@ int process_frames_impl(erasor_handle_t h, const float* map_xyzi, const uint64_t
     return async ? ERASOR_OK : erasor_wait(h);
 }
 
+// |map_voi_| of every node of the last submission = binned + complement counts of the map cloud (K1's tables), into out[0, F)
+int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
+    const size_t row = (size_t)h->B + 1;
+    std::vector<uint32_t> c((size_t)h->F * row);
+    CK(cudaMemcpy(c.data(), h->d_cnt.p, sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
+    for (int f = 0; f < h->F; ++f) {
+        uint64_t t = 0;
+        for (size_t b = 0; b < row; ++b) t += c[(size_t)f * row + b];
+        out[f] = (uint32_t)t;
+    }
+    return ERASOR_OK;
+}
+
 int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                        double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind, bool async) {
     if (!h || !poses7 || !query_offsets) { if (h) h->err = "null argument"; return ERASOR_E_INVALID; }
@@ -1080,8 +1094,12 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         S.poses = poses.data();
         S.keep_out = (f1 == n_frames) ? keep_out : nullptr;
         if ((rc = submit(h, S))) return rc;
+        if (f1 < n_frames) {                                         // the next sub-batch reuses the handle's buffers
+            if ((rc = erasor_wait(h))) return rc;
+            h->node_nvoi.resize((size_t)f1);
+            if ((rc = read_node_voi_counts(h, h->node_nvoi.data() + f0))) return rc;
+        }
         f0 = f1;
-        if (f0 < n_frames && (rc = erasor_wait(h))) return rc;
     }
     return async ? ERASOR_OK : erasor_wait(h);
 }
@@ -1235,15 +1253,9 @@ int erasor_get_node_stats(erasor_handle_t h, uint32_t* n_voi_points, uint32_t* n
     int rc;
     if ((rc = erasor_wait(h))) return rc;
     if (n_voi_points) {
-        // |map_voi_| of every node of the LAST submission = binned + complement counts of the map cloud (K1's tables)
-        const size_t row = (size_t)h->B + 1;
-        std::vector<uint32_t> c((size_t)h->F * row);
-        CK(cudaMemcpy(c.data(), h->d_cnt.p, sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
-        for (int f = 0; f < h->F; ++f) {
-            uint64_t t = 0;
-            for (size_t b = 0; b < row; ++b) t += c[(size_t)f * row + b];
-            n_voi_points[h->f0 + f] = (uint32_t)t;
-        }
+        // earlier sub-batches of the call were counted before the next one overwrote the tables; the last one is read here
+        std::copy(h->node_nvoi.begin(), h->node_nvoi.begin() + std::min<size_t>(h->node_nvoi.size(), (size_t)h->f0), n_voi_points);
+        if ((rc = read_node_voi_counts(h, n_voi_points + h->f0))) return rc;
     }
     if (n_flagged_bins) CK(cudaMemcpy(n_flagged_bins, h->d_nflag.p, sizeof(uint32_t) * h->stat_F, cudaMemcpyDeviceToHost));
     if (n_rejected_points) CK(cudaMemcpy(n_rejected_points, h->d_frame_rej.p, sizeof(uint32_t) * h->stat_F, cudaMemcpyDeviceToHost));
