@@ -30,6 +30,7 @@ EXPORTS = [
     "erasor_process_frames_fold_async", "erasor_fold_keep_masks", "erasor_reset_keep_mask", "erasor_get_frame_stats", "erasor_kernel_launch_count",
     "erasor_map_create", "erasor_map_destroy", "erasor_map_size", "erasor_map_reset_keep", "erasor_map_get_keep", "erasor_map_keep_device",
     "erasor_map_points_device", "erasor_attach_map", "erasor_process_nodes", "erasor_process_nodes_async", "erasor_get_node_stats",
+    "erasor_voxelize_batch",
     "erasor_comm_unique_id", "erasor_comm_init", "erasor_comm_destroy", "erasor_allgather_and_keep", "erasor_and_keep_masks",
     "erasor_get_kernel_time_ms", "erasor_reset_kernel_times", "erasor_get_rgpf_profile", "erasor_get_srt_profile", "erasor_profile_k1",
     "erasor_updater_create", "erasor_updater_destroy", "erasor_updater_reset", "erasor_updater_last_error", "erasor_updater_process_node", "erasor_updater_prefetch_scan",
@@ -141,6 +142,8 @@ def _load():
     L.erasor_process_nodes.argtypes = [c_void_p, POINTER(c_double), c_void_p, POINTER(c_uint64), c_int, c_double, c_void_p, c_void_p, c_int]
     L.erasor_process_nodes_async.argtypes = L.erasor_process_nodes.argtypes
     L.erasor_get_node_stats.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32), POINTER(c_uint32)]
+    L.erasor_voxelize_batch.argtypes = [c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p, c_float, POINTER(c_double), c_int,
+                                        POINTER(c_void_p), POINTER(c_uint64)]
     L.erasor_comm_unique_id.argtypes = [c_void_p]
     L.erasor_comm_init.argtypes = [c_void_p, c_void_p, c_int, c_int]
     L.erasor_comm_destroy.argtypes = [c_void_p]
@@ -203,6 +206,7 @@ def _load():
 
 
 _L = None
+_CUDART = None
 
 
 def lib():
@@ -210,6 +214,20 @@ def lib():
     if _L is None:
         _L = _load()
     return _L
+
+
+def _memcpy_from_device(dst: np.ndarray, src_ptr: int):
+    """dst <- the dst.nbytes bytes at device address src_ptr (cudaMemcpy of the runtime the library loaded)."""
+    global _CUDART
+    if _CUDART is None:
+        lib()
+        _CUDART = ctypes.CDLL("libcudart.so.12")
+        _CUDART.cudaMemcpy.restype = c_int
+        _CUDART.cudaMemcpy.argtypes = [c_void_p, c_void_p, c_size_t, c_int]
+    if dst.nbytes:
+        rc = _CUDART.cudaMemcpy(dst.ctypes.data, c_void_p(src_ptr), dst.nbytes, 2)      # cudaMemcpyDeviceToHost
+        if rc != 0:
+            raise ErasorError(E_CUDA, f"cudaMemcpy: error {rc}")
 
 
 def _cloud(a) -> np.ndarray:
@@ -233,6 +251,7 @@ class Handle:
         if rc != OK:
             raise ErasorError(rc, (self.L.erasor_last_error(None) or b"").decode())
         self.h = h
+        self._device = device
         self.n_map = 0
         self.n_query = 0
         self._keep = []   # keeps host arrays alive while the library may still read them
@@ -450,6 +469,66 @@ class Handle:
         self._ck(self.L.erasor_get_node_stats(self.h, nv.ctypes.data_as(POINTER(c_uint32)), nf.ctypes.data_as(POINTER(c_uint32)),
                                               nr.ctypes.data_as(POINTER(c_uint32))))
         return nv, nf, nr
+
+    # -- batched voxelize_preserving_labels (query preparation, saving node mode's map) -----------------------------------------
+    def voxelize_batch_ptr(self, xyzi_ptr: int, offsets, leaf: float, keep_ptr: int = 0, pose7=None, ptr_kind: int = PTR_HOST):
+        """erasor_voxelize_batch on raw pointers -> (device pointer of the voxels, uint64 output offsets [F+1]).  The voxels stay in
+        the handle's device memory until its next voxelize_batch call."""
+        off = np.ascontiguousarray(offsets, dtype=np.uint64)
+        F = len(off) - 1
+        oo = np.zeros(max(F + 1, 1), dtype=np.uint64)
+        P = None if pose7 is None else np.ascontiguousarray(pose7, dtype=np.float64).reshape(7)
+        d = c_void_p()
+        self._ck(self.L.erasor_voxelize_batch(self.h, c_void_p(xyzi_ptr) if xyzi_ptr else None, off.ctypes.data_as(POINTER(c_uint64)), F,
+                                              c_void_p(keep_ptr) if keep_ptr else None, float(leaf),
+                                              P.ctypes.data_as(POINTER(c_double)) if P is not None else None, ptr_kind, ctypes.byref(d),
+                                              oo.ctypes.data_as(POINTER(c_uint64))))
+        return int(d.value or 0), oo
+
+    def voxelize_batch(self, xyzi, offsets, leaf: float, keep=None, pose7=None):
+        """Host clouds (float32 [n,4], cloud c = xyzi[offsets[c]:offsets[c+1]]) -> (voxels float32 [m,4], output offsets [F+1]):
+        voxelize_preserving_labels of every cloud (keep: optional uint8 [n]), then pose7 (lidar -> body) when given."""
+        x = _cloud(xyzi)
+        k = None if keep is None else np.ascontiguousarray(keep, dtype=np.uint8)
+        d, oo = self.voxelize_batch_ptr(x.ctypes.data if len(x) else 0, offsets, leaf, k.ctypes.data if k is not None and len(k) else 0,
+                                        pose7, PTR_HOST)
+        out = np.empty((int(oo[-1]), 4), dtype=np.float32)
+        _memcpy_from_device(out, d)
+        return out, oo
+
+    def process_scans(self, poses7, raw_xyzi, raw_offsets, query_voxel_size: float, lidar2body7, voi_max_range: float = 0.0,
+                      want_frame_keep: bool = False, ptr_kind: int = PTR_HOST):
+        """Node mode from raw lidar scans (callback_node's query preparation, OfflineMapUpdater.cpp:237-241, then
+        erasor_process_nodes): every scan voxelised at query_voxel_size and moved to the body frame in one submission, then the batch
+        against the attached map, on the device throughout.  raw_xyzi: float32 [n,4] host array, or a device pointer with
+        ptr_kind = PTR_DEVICE.  Returns (the map's keep mask after this batch, per-frame masks or None)."""
+        if ptr_kind == PTR_DEVICE:
+            d, qo = self.voxelize_batch_ptr(int(raw_xyzi), raw_offsets, query_voxel_size, 0, lidar2body7, PTR_DEVICE)
+        else:
+            x = _cloud(raw_xyzi)
+            d, qo = self.voxelize_batch_ptr(x.ctypes.data if len(x) else 0, raw_offsets, query_voxel_size, 0, lidar2body7, PTR_HOST)
+        P = np.ascontiguousarray(poses7, dtype=np.float64).reshape(-1, 7)
+        F = len(qo) - 1
+        assert len(P) == F
+        fk_dev = None
+        if want_frame_keep:
+            import torch
+            fk_dev = torch.empty((F, self._map.size), dtype=torch.uint8, device=f"cuda:{self._device}")
+        self._ck(self.L.erasor_process_nodes(self.h, P.ctypes.data_as(POINTER(c_double)), c_void_p(d) if d else None,
+                                             qo.ctypes.data_as(POINTER(c_uint64)), F, float(voi_max_range),
+                                             c_void_p(fk_dev.data_ptr()) if fk_dev is not None else None, None, PTR_DEVICE))
+        self.n_frames = F
+        keep = self._map.get_keep()
+        return keep, (fk_dev.cpu().numpy() if fk_dev is not None else None)
+
+    def save_static_map(self, m: "Map", voxel: float) -> np.ndarray:
+        """save_static_map of node mode (OfflineMapUpdater.cpp:174-196 without the file): the resident map's points under its keep
+        mask, voxelised at `voxel`, in the map frame."""
+        self._ck(self.L.erasor_synchronize(self.h))
+        d, oo = self.voxelize_batch_ptr(m.points_ptr, [0, m.size], voxel, m.keep_ptr, None, PTR_DEVICE)
+        out = np.empty((int(oo[-1]), 4), dtype=np.float32)
+        _memcpy_from_device(out, d)
+        return out
 
     # -- the exchange step ------------------------------------------------------------------------
     def comm_init(self, id128: bytes, n_ranks: int, rank: int):

@@ -16,12 +16,15 @@ $NVCC $ARCH $CXXF -c updater_capi.cu -o ../_build/updater_capi.o
 $NVCC $ARCH $CXXF -c mapgen_capi.cu -o ../_build/mapgen_capi.o
 $NVCC $ARCH $CXXF -Xptxas -v -c eval_kernels.cu -o ../_build/eval_kernels.o 2> ../_build/eval_kernels.ptxas.log || { cat ../_build/eval_kernels.ptxas.log; exit 1; }
 $NVCC $ARCH $CXXF -Xptxas -v -c pcd_kernels.cu -o ../_build/pcd_kernels.o 2> ../_build/pcd_kernels.ptxas.log || { cat ../_build/pcd_kernels.ptxas.log; exit 1; }
+$NVCC $ARCH $CXXF -Xptxas -v -c voxelize_batch.cu -o ../_build/voxelize_batch.o 2> ../_build/voxelize_batch.ptxas.log || { cat ../_build/voxelize_batch.ptxas.log; exit 1; }
 g++ -O2 -std=c++17 -fPIC -ffp-contract=off -c binning_tables.cpp -o ../_build/binning_tables.o
-$NVCC $ARCH -shared -o ../_lib/liberasor_b200.so ../_build/kernels.o ../_build/erasor_capi.o ../_build/updater_kernels.o ../_build/updater_capi.o ../_build/mapgen_capi.o ../_build/eval_kernels.o ../_build/pcd_kernels.o ../_build/binning_tables.o -lquadmath -lcudart -ldl
+$NVCC $ARCH -shared -o ../_lib/liberasor_b200.so ../_build/kernels.o ../_build/erasor_capi.o ../_build/updater_kernels.o ../_build/updater_capi.o ../_build/mapgen_capi.o ../_build/eval_kernels.o ../_build/pcd_kernels.o ../_build/voxelize_batch.o ../_build/binning_tables.o -lquadmath -lcudart -ldl
 g++ -O2 -std=c++17 -fPIC -shared -ffp-contract=off -I/usr/local/cuda/include -o ../_lib/liberasor_b200_hostcheck.so host_selftest.cpp binning_tables.cpp -lquadmath
 g++ -std=c++17 -O2 -I/usr/local/cuda/include -o ../_lib/offline_map_updater_main ../../examples/offline_map_updater_main.cpp -L../_lib -lerasor_b200 -Wl,-rpath,'$ORIGIN' \
     -L/usr/local/cuda/lib64 -Wl,-rpath,/usr/local/cuda/lib64 -lcudart
 g++ -std=c++17 -O2 -I/usr/local/cuda/include -o ../_lib/mapgen_main ../../examples/mapgen_main.cpp -L../_lib -lerasor_b200 -Wl,-rpath,'$ORIGIN' \
+    -L/usr/local/cuda/lib64 -Wl,-rpath,/usr/local/cuda/lib64 -lcudart
+g++ -std=c++17 -O2 -I/usr/local/cuda/include -o ../_lib/static_map_nodes_main ../../examples/static_map_nodes_main.cpp -L../_lib -lerasor_b200 -Wl,-rpath,'$ORIGIN' \
     -L/usr/local/cuda/lib64 -Wl,-rpath,/usr/local/cuda/lib64 -lcudart
 echo "built: $(ls ../_lib)"
 # C++ host-class demo (include/erasor/erasor.hpp over the C ABI)

@@ -19,6 +19,7 @@
 #include "device_types.h"
 #include "kernels.h"
 #include "pose_math.h"
+#include "voxelize_batch.h"
 
 using namespace erasor;
 
@@ -159,6 +160,9 @@ struct erasor_ctx {
 
     // node mode
     erasor_map_ctx* map = nullptr;
+
+    // erasor_voxelize_batch: its scratch and output cloud (created on first use)
+    erasor::VoxBatch* vb = nullptr;
 
     // exchange
     ncclComm_t comm = nullptr;
@@ -569,6 +573,7 @@ void erasor_destroy(erasor_handle_t h) {
     h->graphs.clear();
     if (h->comm) { NcclApi* api = nccl_api(h->err); if (api) api->CommDestroy(h->comm); h->comm = nullptr; }
     for (DevBuf* b : h->all_bufs()) b->release();
+    vox_batch_destroy(h->vb);
     h->h_pose.release();
     h->h_words.release();
     h->h_stage.release();
@@ -1245,6 +1250,38 @@ int erasor_process_nodes(erasor_handle_t h, const double* poses7, const float* q
 int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind) {
     return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, frame_keep, keep_out, ptr_kind, true);
+}
+
+// voxelize_preserving_labels of n_clouds clouds in one submission (voxelize_batch.cu): the checks that need only the host arrays
+int erasor_voxelize_batch(erasor_handle_t h, const float* xyzi, const uint64_t* offsets, int n_clouds, const uint8_t* keep, float leaf,
+                          const double* pose7, int ptr_kind, const float** d_out, uint64_t* out_offsets) {
+    if (!h) return ERASOR_E_INVALID;
+    h->err.clear();
+    if (!offsets || !d_out || !out_offsets) { h->err = "null argument"; return ERASOR_E_INVALID; }
+    if (n_clouds < 1) { h->err = "n_clouds must be at least 1"; return ERASOR_E_INVALID; }
+    if (ptr_kind != ERASOR_PTR_HOST && ptr_kind != ERASOR_PTR_DEVICE) { h->err = "ptr_kind must be ERASOR_PTR_HOST or ERASOR_PTR_DEVICE"; return ERASOR_E_INVALID; }
+    if (!(leaf > 0.0f) || !std::isfinite(leaf)) { h->err = "leaf must be positive and finite"; return ERASOR_E_INVALID; }
+    if (offsets[0] != 0) { h->err = "offsets[0] must be 0 (offsets[n_clouds] is the point count)"; return ERASOR_E_INVALID; }
+    for (int c = 0; c < n_clouds; ++c)
+        if (offsets[c + 1] < offsets[c]) { h->err = "offsets are not monotone at cloud " + std::to_string(c); return ERASOR_E_INVALID; }
+    for (int c = 0; c < n_clouds; ++c)
+        if (offsets[c + 1] - offsets[c] >= (1ull << 31)) { h->err = "cloud " + std::to_string(c) + " has 2^31 points or more"; return ERASOR_E_CAPACITY; }
+    const uint64_t n = offsets[n_clouds];
+    if (n >= 0xFFFFFFFFull) { h->err = "a call takes fewer than 2^32 - 1 points"; return ERASOR_E_CAPACITY; }
+    if (n && !xyzi) { h->err = "null cloud pointer"; return ERASOR_E_INVALID; }
+    if (ptr_kind == ERASOR_PTR_DEVICE && (reinterpret_cast<uintptr_t>(xyzi) & 15u)) { h->err = "a device cloud must be 16-byte aligned (one float4 per point)"; return ERASOR_E_INVALID; }
+    CK(cudaSetDevice(h->device));
+    Mat4 T{};
+    if (pose7) {
+        // as the updater's tf_lidar2body_ (set_params, OfflineMapUpdater.cpp:89-104): geoPose2eigen(pose) * Identity
+        Mat4 G, I{};
+        for (int i = 0; i < 4; ++i) I.m[i * 5] = 1.0f;
+        pose_to_mat(pose7, G);
+        mat_mul(G, I, T);
+    }
+    if (!h->vb) h->vb = vox_batch_create();
+    return vox_batch_run(h->vb, h->stream, xyzi, offsets, n_clouds, keep, leaf, pose7 ? T.m : nullptr, ptr_kind == ERASOR_PTR_DEVICE, d_out,
+                         out_offsets, h->launches, h->err);
 }
 
 int erasor_get_node_stats(erasor_handle_t h, uint32_t* n_voi_points, uint32_t* n_flagged_bins, uint32_t* n_rejected_points) {

@@ -18,12 +18,13 @@
 
 #include "../../include/erasor_b200.h"
 #include "device_common.cuh"
+#include "radix_sort.h"
 
 namespace erasor {
 
 constexpr int      kThreads   = 256;
 constexpr int      kWarps     = kThreads / 32;
-constexpr uint32_t kSeg       = 4096;          // points per warp segment of the radix sort
+constexpr uint32_t kSeg       = kRadixSeg;     // points per warp segment of the radix sort
 constexpr uint32_t kHeadChunk = 4096;          // points per CTA chunk of the run-head scan
 constexpr uint32_t kNoKey     = 0xFFFFFFFFu;   // key of an estimate point the keep mask drops: sorts behind every cell key
 
@@ -199,6 +200,22 @@ __global__ void __launch_bounds__(kThreads) k_eval_radix_scatter(const uint32_t*
         }
         __syncwarp();
     }
+}
+
+cudaError_t radix_sort_passes(cudaStream_t st, uint32_t* scratch, uint32_t* const k[2], uint32_t* const v[2], uint32_t n, int first, int npass) {
+    const uint32_t nseg = (uint32_t)(((uint64_t)n + kSeg - 1) / kSeg);
+    uint32_t* cnt = scratch;
+    uint32_t* tot = cnt + 256ull * nseg;
+    const int seg_ctas = (int)((nseg + kWarps - 1) / kWarps);
+    for (int pass = 0; pass < npass; ++pass) {
+        const int a = pass & 1;
+        k_eval_radix_hist<<<seg_ctas, kThreads, 0, st>>>(k[a], n, nseg, 8 * (first + pass), cnt);
+        k_eval_radix_rows<<<256 / kWarps, kThreads, 0, st>>>(cnt, nseg, tot);
+        k_eval_radix_scatter<<<seg_ctas, kThreads, 0, st>>>(k[a], v[a], k[a ^ 1], v[a ^ 1], n, nseg, 8 * (first + pass), cnt, tot);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 // ---- 4. run heads of the sorted keys: count per chunk, one CTA scans the counts, ordered scatter -----------------------------
@@ -713,21 +730,10 @@ int grid_for(int n, int per_cta) { return std::max(1, (n + per_cta - 1) / per_ct
 // ceil(n / per) in 64 bits: n may be up to 2^32 - 2, where n + per - 1 wraps in uint32
 uint32_t ceil_div(uint64_t n, uint64_t per) { return (uint32_t)((n + per - 1) / per); }
 
-// npass 8-bit passes of the stable LSD radix sort of (k[0], v[0]) over n entries, digits first, first + 1, ...; k[1] and v[1]
-// are the ping-pong halves.  The result is in k[npass & 1], v[npass & 1].
+// npass 8-bit passes of the stable LSD radix sort (radix_sort.h) in the context's scratch
 int radix_passes(erasor_eval_t e, uint32_t* const k[2], uint32_t* const v[2], uint32_t n, int first, int npass) {
-    const uint32_t nseg = ceil_div(n, kSeg);
-    ECK(e->cnt.ensure(sizeof(uint32_t) * (256ull * nseg + 256ull)));
-    uint32_t* cnt = e->cnt.as<uint32_t>();
-    uint32_t* tot = cnt + 256ull * nseg;
-    const int seg_ctas = (int)((nseg + kWarps - 1) / kWarps);
-    for (int pass = 0; pass < npass; ++pass) {
-        const int a = pass & 1;
-        k_eval_radix_hist<<<seg_ctas, kThreads, 0, e->st>>>(k[a], n, nseg, 8 * (first + pass), cnt);
-        k_eval_radix_rows<<<256 / kWarps, kThreads, 0, e->st>>>(cnt, nseg, tot);
-        k_eval_radix_scatter<<<seg_ctas, kThreads, 0, e->st>>>(k[a], v[a], k[a ^ 1], v[a ^ 1], n, nseg, 8 * (first + pass), cnt, tot);
-        ECK(cudaGetLastError());
-    }
+    ECK(e->cnt.ensure(sizeof(uint32_t) * radix_scratch_words(n)));
+    ECK(radix_sort_passes(e->st, e->cnt.as<uint32_t>(), k, v, n, first, npass));
     return ERASOR_OK;
 }
 

@@ -43,6 +43,47 @@ def run_offline(nodes: Iterable[Node], initial_map: np.ndarray, up, ep, make_upd
     return {"static_map": static_map, "nodes": seen, "processed_scans": processed}
 
 
+def processed_nodes(nodes: Iterable[Node], removal_interval: int) -> list:
+    """The nodes callback_node processes: the k-th call (1-based) unless k % removal_interval != 0 ("PASS!", :328)."""
+    return [nd for k, nd in enumerate(nodes, 1) if k % int(removal_interval) == 0]
+
+
+def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep, batch: int = 20, save_voxel_size: Optional[float] = None,
+                          prepare: Optional[Callable] = None) -> dict:
+    """The frame-independent twin of run_offline: every node callback_node would process is tested against the same initial map
+    (node mode, erasor_process_nodes), in batches of `batch` nodes, each batch's raw scans voxelised at query_voxel_size and moved
+    to the body frame on the device in one submission (erasor_voxelize_batch); then save_static_map of the kept map.  prepare
+    (optional) replaces the device query preparation: prepare(raw_xyzi, raw_offsets) -> (queries, query_offsets).  Returns
+    run_offline's dict plus "keep", the map's keep mask.  Needs a CUDA device."""
+    from . import capi
+    if up.is_large_scale:
+        raise ValueError("node mode has no large-scale windowing: use run_offline")
+    nodes = list(nodes)
+    sel = processed_nodes(nodes, up.removal_interval)
+    m = capi.Map(np.ascontiguousarray(initial_map, dtype=np.float32))
+    h = capi.Handle(ep.replace(version=up.version))       # /erasor/version as the updater reads it (OfflineMapUpdater.cpp:81)
+    try:
+        h.attach_map(m)
+        l2b = np.asarray(up.lidar2body, dtype=np.float64)
+        for b0 in range(0, len(sel), int(batch)):
+            chunk = sel[b0:b0 + int(batch)]
+            poses = np.stack([np.asarray(o, dtype=np.float64).reshape(7) for _, o, _ in chunk])
+            scans = [np.ascontiguousarray(c, dtype=np.float32).reshape(-1, 4) for _, _, c in chunk]
+            off = np.cumsum([0] + [len(s) for s in scans]).astype(np.uint64)
+            raw = np.concatenate(scans)
+            if prepare is None:
+                h.process_scans(poses, raw, off, up.query_voxel_size, l2b, voi_max_range=up.max_range)
+            else:
+                q, qo = prepare(raw, off)
+                h.process_nodes(poses, q, qo, voi_max_range=up.max_range)
+        keep = m.get_keep()
+        static_map = h.save_static_map(m, up.map_voxel_size if save_voxel_size is None else save_voxel_size)
+    finally:
+        h.close()
+        m.close()
+    return {"static_map": static_map, "nodes": len(nodes), "processed_scans": len(sel), "keep": keep}
+
+
 def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, make_updater: Optional[Callable] = None,
                  map_leafsize: Optional[float] = None, out_dir: Optional[str] = None) -> dict:
     """mapgen -> updater -> evaluation on one node list.  GT for PR/RR = the naive map itself (it carries the labels), which is

@@ -162,7 +162,68 @@ public:
         keep.resize(erasor_map_size(map_));
         return keep;
     }
+    // the same, from a map already in device memory (16-byte aligned float4 per point), e.g. read by PcdCodec::load_device
+    void load_global_map_device(const float* d_map_xyzi, size_t n) {
+        if (map_) { erasor_attach_map(h_, nullptr); erasor_map_destroy(map_); map_ = nullptr; }
+        if (erasor_map_create(d_map_xyzi, n, ERASOR_PTR_DEVICE, device_, &map_) != ERASOR_OK)
+            throw std::runtime_error(std::string("ERASOR: ") + erasor_last_error(nullptr));
+        check(erasor_attach_map(h_, map_));
+    }
     void reset_static_mask() { if (map_ && erasor_map_reset_keep(map_) != ERASOR_OK) throw std::runtime_error("ERASOR: erasor_map_reset_keep"); }
+    // the map's keep mask (1 = static so far), after the work queued on this handle
+    std::vector<uint8_t> static_mask() {
+        if (!map_) throw std::logic_error("ERASOR: load_global_map first");
+        check(erasor_synchronize(h_));
+        std::vector<uint8_t> keep(std::max<size_t>(erasor_map_size(map_), 1));
+        if (erasor_map_get_keep(map_, keep.data(), ERASOR_PTR_HOST) != ERASOR_OK) throw std::runtime_error("ERASOR: erasor_map_get_keep");
+        keep.resize(erasor_map_size(map_));
+        return keep;
+    }
+
+    // ---- voxelize_preserving_labels of many clouds in one submission (erasor_voxelize_batch) ---------------------------------
+    // Voxels in the handle's device memory: cloud c is float4 points offsets[c] .. offsets[c+1] of d_xyzi, valid until the next
+    // voxelize_batch / process_scans / save_static_map on this handle.
+    struct DeviceClouds { const float* d_xyzi = nullptr; std::vector<uint64_t> offsets; };
+    // cloud c = xyzi points raw_offsets[c] .. raw_offsets[c+1] (host or device per ptr_kind); keep (nullable, same memory kind)
+    // selects points; pose7 (nullable) moves the voxels as the updater's tf_lidar2body_ does
+    DeviceClouds voxelize_batch(const float* xyzi, const std::vector<uint64_t>& offsets, float leaf, const uint8_t* keep = nullptr,
+                                const double* pose7 = nullptr, int ptr_kind = ERASOR_PTR_HOST) {
+        if (offsets.size() < 2) throw std::invalid_argument("ERASOR: voxelize_batch needs at least one cloud");
+        DeviceClouds out;
+        out.offsets.assign(offsets.size(), 0);
+        check(erasor_voxelize_batch(h_, xyzi, offsets.data(), static_cast<int>(offsets.size() - 1), keep, leaf, pose7, ptr_kind, &out.d_xyzi,
+                                    out.offsets.data()));
+        return out;
+    }
+    // Node mode from raw lidar scans: callback_node's query preparation (voxelize_preserving_labels at query_voxel_size, then
+    // lidar -> body, OfflineMapUpdater.cpp:237-241) for every scan in one submission, then process_nodes on the device-held queries.
+    // raw scans: host or device (ptr_kind).  The map's keep mask accumulates as in process_nodes (static_mask() reads it).
+    void process_scans(const std::vector<std::array<double, 7>>& poses, const float* raw_xyzi, const std::vector<uint64_t>& raw_offsets,
+                       double query_voxel_size, const std::array<double, 7>& lidar2body, double voi_max_range = 0.0,
+                       int ptr_kind = ERASOR_PTR_HOST) {
+        if (!map_) throw std::logic_error("ERASOR: load_global_map first");
+        if (poses.empty() || poses.size() + 1 != raw_offsets.size()) throw std::invalid_argument("ERASOR: one pose per raw scan");
+        const DeviceClouds q = voxelize_batch(raw_xyzi, raw_offsets, static_cast<float>(query_voxel_size), nullptr, lidar2body.data(), ptr_kind);
+        check(erasor_process_nodes(h_, poses[0].data(), q.d_xyzi, q.offsets.data(), static_cast<int>(poses.size()), voi_max_range, nullptr, nullptr,
+                                   ERASOR_PTR_DEVICE));
+    }
+    std::vector<uint8_t> process_scans(const std::vector<std::array<double, 7>>& poses, const std::vector<PointCloud>& raw_scans,
+                                       double query_voxel_size, const std::array<double, 7>& lidar2body, double voi_max_range = 0.0) {
+        std::vector<uint64_t> off(raw_scans.size() + 1, 0);
+        for (size_t f = 0; f < raw_scans.size(); ++f) off[f + 1] = off[f] + raw_scans[f].size();
+        PointCloud raw(off.back());
+        for (size_t f = 0; f < raw_scans.size(); ++f) std::copy(raw_scans[f].begin(), raw_scans[f].end(), raw.begin() + static_cast<std::ptrdiff_t>(off[f]));
+        process_scans(poses, reinterpret_cast<const float*>(raw.data()), off, query_voxel_size, lidar2body, voi_max_range, ERASOR_PTR_HOST);
+        return static_mask();
+    }
+    // save_static_map of node mode (OfflineMapUpdater.cpp:174-196 without the file): the map load_global_map holds, under its
+    // current keep mask, voxelised at voxel_size -- one cloud, in the handle's device memory (offsets {0, n})
+    DeviceClouds save_static_map(float voxel_size) {
+        if (!map_) throw std::logic_error("ERASOR: load_global_map first");
+        check(erasor_synchronize(h_));
+        const std::vector<uint64_t> off = {0, static_cast<uint64_t>(erasor_map_size(map_))};
+        return voxelize_batch(erasor_map_points_device(map_), off, voxel_size, erasor_map_keep_device(map_), nullptr, ERASOR_PTR_DEVICE);
+    }
     // frame-sharded job: every rank processes its own nodes, then ONE all-gather (bit-packed masks over NVLink) + AND gives
     // every rank the job's static mask.  id128 from erasor_comm_unique_id() on rank 0, shipped by the host program.
     void init_communicator(const uint8_t* id128, int n_ranks, int rank) { check(erasor_comm_init(h_, id128, n_ranks, rank)); }

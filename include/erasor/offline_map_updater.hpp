@@ -206,17 +206,19 @@ public:
         c.resize(n);
         return c;
     }
-    void write(const std::string& path, const PointCloud& c) {
-        const float* src = reinterpret_cast<const float*>(c.data());
+    void write(const std::string& path, const PointCloud& c) { write_from(path, reinterpret_cast<const float*>(c.data()), c.size(), ERASOR_PTR_HOST); }
+    // the same file from n points in device memory (e.g. ERASOR::save_static_map's cloud)
+    void write_device(const std::string& path, const float* d_xyzi, size_t n) { write_from(path, d_xyzi, n, ERASOR_PTR_DEVICE); }
+
+private:
+    void write_from(const std::string& path, const float* src, size_t n, int in_kind) {
         size_t len = 0;
-        check(erasor_pcd_format_ascii(p_, src, c.size(), ERASOR_PTR_HOST, nullptr, 0, ERASOR_PTR_HOST, &len), path);
+        check(erasor_pcd_format_ascii(p_, src, n, in_kind, nullptr, 0, ERASOR_PTR_HOST, &len), path);
         text_.resize(len);
-        check(erasor_pcd_format_ascii(p_, src, c.size(), ERASOR_PTR_HOST, text_.data(), len, ERASOR_PTR_HOST, &len), path);
+        check(erasor_pcd_format_ascii(p_, src, n, in_kind, text_.data(), len, ERASOR_PTR_HOST, &len), path);
         std::ofstream f(path, std::ios::binary);
         if (!f || !f.write(text_.data(), (std::streamsize)len)) throw std::runtime_error("cannot write " + path);
     }
-
-private:
     void slurp(const std::string& path) {
         std::ifstream f(path, std::ios::binary | std::ios::ate);
         if (!f) throw std::invalid_argument("cannot open " + path);

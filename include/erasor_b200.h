@@ -211,6 +211,22 @@ int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const fl
 /* per-node counters of the last erasor_process_nodes: points inside the VoI (|map_voi_|), flagged bins, rejected points */
 int erasor_get_node_stats(erasor_handle_t h, uint32_t* n_voi_points, uint32_t* n_flagged_bins, uint32_t* n_rejected_points);
 
+/* erasor_utils::voxelize_preserving_labels (erasor_utils.cpp:80-114) of n_clouds clouds in one submission, each on its own
+ * pcl::VoxelGrid, optionally followed by one pcl::transformPointCloud.  Cloud c is xyzi[offsets[c] .. offsets[c+1]) (offsets: HOST,
+ * n_clouds + 1 entries, offsets[0] = 0); keep (nullable, offsets[n_clouds] bytes) selects the points with keep != 0; xyzi and keep
+ * are host or device memory (ptr_kind; a device cloud 16-byte aligned).  pose7 (nullable, HOST, x y z qx qy qz qw) is applied to the
+ * output as the updater applies /tf/lidar2body (geoPose2eigen(pose) * Identity, OfflineMapUpdater.cpp:89-104,240).
+ * Cloud c's voxels are (*d_out)[out_offsets[c] .. out_offsets[c+1]) (float4 each; out_offsets: HOST, n_clouds + 1 entries), in
+ * ascending voxel key, centroids summed in cloud order, labels from the exact 1-NN among the cloud's selected points with ties to
+ * the lowest index; a cloud whose grid overflows int32 passes through with its labels restored.  *d_out is the handle's device
+ * memory on erasor_stream(h), valid until the next erasor_voxelize_batch on h: it can go straight into erasor_process_nodes with
+ * ERASOR_PTR_DEVICE, or erasor_map_points_device(m) with erasor_map_keep_device(m) can go in to save a node-mode map.
+ * Synchronous: one device -> host read of the offsets.  ERASOR_E_INVALID: n_clouds < 1, offsets[0] != 0 or not monotone, leaf not
+ * positive and finite, a non-finite x, y or z in a selected point (the message names the cloud and the point; the handle stays usable).
+ * ERASOR_E_CAPACITY: a cloud of 2^31 points or more, or 2^32 - 1 points or more in all. */
+int erasor_voxelize_batch(erasor_handle_t h, const float* xyzi, const uint64_t* offsets, int n_clouds, const uint8_t* keep, float leaf,
+                          const double* pose7, int ptr_kind, const float** d_out, uint64_t* out_offsets);
+
 /* ---- the path's single collective, behind the C ABI (north_star: one NCCL all-gather of the static masks) ------------ */
 /* A communicator owned by the handle (NCCL is loaded with dlopen("libnccl.so.2") on first use).  Rank 0 calls
  * erasor_comm_unique_id and ships the 128 bytes to the other ranks by whatever means the host program has
