@@ -99,6 +99,14 @@ ERASOR_HD int rgpf_bucket_of(uint32_t n) {
     return 8;
 }
 
+// K4b's global scratch (bins beyond its shared-memory cap, cloud mode): the region of bin b starts at this byte offset, where
+// dsq_b / dsm_b are the bin's scatter offsets in the query / map cloud.  The region holds 36 n + 4 bytes (n = qc + n_ground_final
+// <= qc + cm: X Y Z I KEY, VST with n + 1 entries, ORD ORD2 VK); the 16 bytes per bin beyond 36 (qc + cm) keep it clear of the
+// next bin's region when every map point of the bin is ground.  d_vox_scratch holds k4b_scratch_offset(NQ, NM, B) + 36 + 64 bytes.
+ERASOR_HD uint64_t k4b_scratch_offset(uint32_t dsq_b, uint32_t dsm_b, uint32_t b) {
+    return 36ull * ((uint64_t)dsq_b + dsm_b) + 16ull * b;
+}
+
 // Per flagged bin record written by K3 and completed by K4
 struct FlagRec {
     uint32_t frame;

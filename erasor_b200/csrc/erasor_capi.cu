@@ -640,7 +640,7 @@ int erasor_compare(erasor_handle_t h, int version, int frame) {
         CK(h->d_vox.ensure(sizeof(float4) * (NM + NQ + 1)));
         CK(h->d_vox_cnt.ensure(sizeof(uint32_t) * (size_t)B));
         CK(h->d_vox_start.ensure(sizeof(uint32_t) * (size_t)B));
-        CK(h->d_vox_scratch.ensure((size_t)36 * (NM + NQ + 1) + 64));
+        CK(h->d_vox_scratch.ensure((size_t)k4b_scratch_offset((uint32_t)NQ, (uint32_t)NM, (uint32_t)B) + 36 + 64));
     }
     CK(h->d_arranged.ensure(sizeof(float4) * (2 * NM + NQ + 1)));
     CK(h->d_map_rej.ensure(sizeof(float4) * std::max<size_t>(NM, 1)));

@@ -71,6 +71,12 @@ int erasor_hostcheck_node_pose(const double* odom7, double voi_max_range, double
     return 0;
 }
 
+// byte offset of each bin's region in K4b's global scratch (device_types.h): bin bins[k] with scatter offsets dsq[k], dsm[k]
+int erasor_hostcheck_k4b_scratch_offset(const uint32_t* dsq, const uint32_t* dsm, const uint32_t* bins, size_t n, uint64_t* out) {
+    for (size_t k = 0; k < n; ++k) out[k] = erasor::k4b_scratch_offset(dsq[k], dsm[k], bins[k]);
+    return 0;
+}
+
 // the float guard bands of the device's fast path (binning_tables.cpp): {up_k, dn_k} per ring threshold and around s_max
 int erasor_hostcheck_guards(const erasor_params_t* p, float* ring_guard, float* smax_lo_hi) {
     erasor::HostBinTables T;

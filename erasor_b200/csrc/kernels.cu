@@ -958,7 +958,7 @@ static void k2_smem_plan(int B, bool with_complement, uint32_t& SW, size_t& smem
     const uint32_t n_slots_max = with_complement ? (uint32_t)B + 1u : (uint32_t)B;
     const size_t full = sizeof(uint32_t) * (size_t)(W + 1) * n_slots_max + fixed;
     const size_t two_per_sm = 111 * 1024;                 // two CTAs per SM: (227 KB - static shared memory) / 2
-    const size_t budget = full <= two_per_sm ? full : two_per_sm;      // 40 x 360: 2304-slot windows (config 5 flags ~2060 bins per frame)
+    const size_t budget = full <= two_per_sm ? full : two_per_sm;      // 40 x 360: 2356-slot windows (config 5 flags ~2060 bins per frame)
     SW   = (uint32_t)std::min<size_t>(std::max<uint32_t>(n_slots_max, 1u), std::max<size_t>(1, (budget - fixed) / (sizeof(uint32_t) * (W + 1))));
     smem = sizeof(uint32_t) * (size_t)(W + 1) * SW + fixed;
 }
@@ -1937,7 +1937,7 @@ k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32
         const FlagRec& rc = recs[w];
         const uint32_t b = rc.bin, qc = cq[b], ng = rc.n_ground_final, n = qc + ng;
         const uint32_t region = dsq[b] + dsm[b];
-        unsigned char* base = (n <= smem_cap_points) ? smem_raw : (gscratch + (size_t)region * 36u);
+        unsigned char* base = (n <= smem_cap_points) ? smem_raw : (gscratch + k4b_scratch_offset(dsq[b], dsm[b], b));
         float*    X   = reinterpret_cast<float*>(base);
         float*    Y   = X + n;
         float*    Z   = Y + n;
