@@ -39,7 +39,7 @@ EXPORTS = [
     "erasor_eval_create", "erasor_eval_destroy", "erasor_eval_last_error", "erasor_evaluate", "erasor_eval_overlap",
     "erasor_eval_count_selected",
     "erasor_pcd_create", "erasor_pcd_destroy", "erasor_pcd_last_error", "erasor_pcd_parse_ascii", "erasor_pcd_format_ascii",
-    "erasor_pcd_load",
+    "erasor_pcd_load", "erasor_bag_index", "erasor_bag_nodes", "erasor_bag_load", "erasor_bag_load_list",
     "erasor_mapgen_create", "erasor_mapgen_destroy", "erasor_mapgen_last_error", "erasor_mapgen_accum", "erasor_mapgen_get_cloud",
     "erasor_mapgen_device_cloud", "erasor_mapgen_synchronize", "erasor_mapgen_get_counters",
 ]
@@ -67,6 +67,19 @@ class PcdLoadInfoC(ctypes.Structure):
     _fields_ = [(name, c_uint32) for name in ("data_mode", "fields", "intensity_zero_filled", "point_step")] + \
                [(name, c_uint64) for name in ("width", "height", "points", "data_offset", "compressed_size", "uncompressed_size", "lzf_tokens")] + \
                [("ascii", PcdInfoC)]
+
+
+class BagInfoC(ctypes.Structure):
+    """erasor_bag_info_t"""
+    _fields_ = [("version", c_uint32), ("pad_", c_uint32)] + \
+               [(name, c_uint64) for name in ("chunks", "connections", "messages", "selected", "unknown_records", "nodes", "total_points",
+                                               "intensity_zero_filled", "big_endian")] + [("md5sum", ctypes.c_char * 40)]
+
+
+class BagCloudC(ctypes.Structure):
+    """erasor_bag_cloud_t"""
+    _fields_ = [("data_offset", c_uint64), ("data_len", c_uint64)] + \
+               [(name, c_uint32) for name in ("width", "height", "point_step", "row_step", "fields", "big_endian")] + [("offset", c_uint32 * 4)]
 
 
 class MapGenParamsC(ctypes.Structure):
@@ -192,6 +205,10 @@ def _load():
     L.erasor_pcd_parse_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdInfoC)]
     L.erasor_pcd_format_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t)]
     L.erasor_pcd_load.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdLoadInfoC)]
+    L.erasor_bag_index.argtypes = [c_void_p, c_void_p, c_size_t, c_char_p, c_int, POINTER(c_size_t), POINTER(BagInfoC)]
+    L.erasor_bag_nodes.argtypes = [c_void_p, c_size_t, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.erasor_bag_load.argtypes = [c_void_p, c_size_t, c_size_t, c_void_p, c_size_t, c_int, POINTER(c_uint64)]
+    L.erasor_bag_load_list.argtypes = [c_void_p, POINTER(c_uint64), c_size_t, c_void_p, c_size_t, c_int, POINTER(c_uint64)]
     L.erasor_mapgen_create.argtypes = [POINTER(MapGenParamsC), c_int, POINTER(c_void_p)]
     L.erasor_mapgen_destroy.restype = None
     L.erasor_mapgen_destroy.argtypes = [c_void_p]
@@ -1021,6 +1038,84 @@ class PcdCodec:
         data_offset, compressed_size, uncompressed_size, lzf_tokens, and the ascii branch's info as a dict under "ascii" """
         info = getattr(self, "_load_info", None)
         return dict(info) if info is not None else None
+
+    # ---- erasor/node bags (DESIGN.md section 12.2) ----
+    BAG_TOPIC = "/node/combined/optimized"
+
+    def bag_index(self, data, topic: str = BAG_TOPIC, keep_first: bool = False) -> dict:
+        """Indexes a ROS bag 2.0 file of erasor/node messages (erasor_bag_index): data is the whole file, bytes-like or a CPU uint8
+        tensor (pinned memory is read by the device directly, pageable memory through pinned staging).  The codec keeps a reference
+        to it until the next bag_index.  The first message on the topic is dropped unless keep_first, as the reference's subscribers
+        drop it.  Returns erasor_bag_info_t as a dict."""
+        if hasattr(data, "data_ptr"):
+            if data.is_cuda:
+                raise ValueError("bags are indexed from host memory")
+            keep, ptr, nb = data, data.data_ptr(), data.numel() * data.element_size()
+        else:
+            keep = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data).view(np.uint8)
+            ptr, nb = (keep.ctypes.data if keep.size else 0), keep.size
+        n, info = c_size_t(0), BagInfoC()
+        self._bag = None
+        self._ck(self.L.erasor_bag_index(self.h, c_void_p(ptr) if ptr else None, nb, topic.encode(), int(bool(keep_first)), ctypes.byref(n),
+                                         ctypes.byref(info)))
+        self._bag, self._bag_n = keep, n.value
+        d = {name: int(getattr(info, name)) for name, _ in BagInfoC._fields_ if name not in ("md5sum", "pad_")}
+        d["md5sum"] = info.md5sum.decode()
+        return d
+
+    def _bag_range(self, first: int, count):
+        if getattr(self, "_bag", None) is None:
+            raise ErasorError(E_STATE, "no bag indexed: call bag_index first")
+        return int(first), (self._bag_n - int(first) if count is None else int(count))
+
+    def bag_meta(self, first: int = 0, count=None):
+        """(seq uint32 [k], stamp_ns uint64 [k], odom7 float64 [k, 7], clouds) of nodes [first, first + k); clouds: one dict per node
+        with erasor_bag_cloud_t's fields"""
+        first, count = self._bag_range(first, count)
+        seq, stamp, odom = np.zeros(max(count, 0), np.uint32), np.zeros(max(count, 0), np.uint64), np.zeros((max(count, 0), 7))
+        cl = (BagCloudC * max(count, 1))()
+        self._ck(self.L.erasor_bag_nodes(self.h, first, count, c_void_p(seq.ctypes.data), c_void_p(stamp.ctypes.data), c_void_p(odom.ctypes.data),
+                                         ctypes.addressof(cl)))
+        clouds = [dict({name: int(getattr(c, name)) for name, _ in BagCloudC._fields_ if name != "offset"}, offset=[int(v) for v in c.offset])
+                  for c in cl[:count]]
+        return seq, stamp, odom, clouds
+
+    def bag_load(self, first: int = 0, count=None, device_out: bool = False, nodes=None):
+        """(xyzi, offsets) of nodes [first, first + count), or of the listed nodes: their clouds back to back as float32 [n, 4] --
+        a numpy array, or a CUDA tensor with device_out -- and uint64 offsets [count + 1], from one erasor_bag_load (one gather
+        launch)"""
+        if nodes is None:
+            first, count = self._bag_range(first, count)
+            call = lambda out, cap, kind, op: self.L.erasor_bag_load(self.h, first, count, out, cap, kind, op)
+        else:
+            self._bag_range(0, None)
+            lst = np.ascontiguousarray(nodes, dtype=np.uint64)
+            count = len(lst)
+            lp = lst.ctypes.data_as(POINTER(c_uint64))
+            call = lambda out, cap, kind, op: self.L.erasor_bag_load_list(self.h, lp, count, out, cap, kind, op)
+        off = np.zeros(max(count, 0) + 1, dtype=np.uint64)
+        op = off.ctypes.data_as(POINTER(c_uint64))
+        self._ck(call(None, 0, PTR_HOST, op))
+        total = int(off[-1])
+        if device_out:
+            import torch
+            out = torch.empty((max(total, 1), 4), dtype=torch.float32, device=f"cuda:{self.device}")
+            self._ck(call(c_void_p(out.data_ptr()), total, PTR_DEVICE, op))
+        else:
+            out = np.empty((max(total, 1), 4), dtype=np.float32)
+            self._ck(call(c_void_p(out.ctypes.data), total, PTR_HOST, op))
+        return out[:total], off
+
+    def bag_nodes(self, batch: int = 64, device_out: bool = False):
+        """Yields (seq, odom7, cloud) per node of the indexed bag, as erasor_b200.kitti.iter_nodes yields them: clouds decoded
+        `batch` nodes per erasor_bag_load; with device_out each cloud is a view of a CUDA tensor holding its batch."""
+        _, count = self._bag_range(0, None)
+        for b0 in range(0, count, int(batch)):
+            nb = min(int(batch), count - b0)
+            seq, _, odom, _ = self.bag_meta(b0, nb)
+            xyzi, off = self.bag_load(b0, nb, device_out)
+            for k in range(nb):
+                yield int(seq[k]), odom[k].copy(), xyzi[int(off[k]):int(off[k + 1])]
 
     def _format(self, xyzi) -> np.ndarray:
         if hasattr(xyzi, "is_cuda") and xyzi.is_cuda:

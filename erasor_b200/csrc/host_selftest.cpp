@@ -1,6 +1,7 @@
 // host_selftest.cpp -- compiles binning.h, pcd_codec.h and pcd_binary.h for the HOST so that the CPU test-suite (-m "not gpu")
 // can check the exact-threshold bin arithmetic against the oracle, and the ASCII PCD codec's per-token arithmetic against
-// numpy and Python, and the binary PCD reader with its parallel LZF decoder run serially, without a GPU.
+// numpy and Python, the binary PCD reader with its parallel LZF decoder run serially, and the erasor/node bag index with its
+// per-point decode, without a GPU.
 // This library is loaded by tests only; the product API (erasor_capi.cu) has no host compute path.
 #include <algorithm>
 #include <cstdint>
@@ -8,6 +9,7 @@
 #include <string>
 #include <vector>
 
+#include "bag_index.h"
 #include "binning_tables.h"
 #include "pcd_binary.h"
 #include "pcd_codec.h"
@@ -234,6 +236,57 @@ int erasor_hostcheck_lzf_decode(const uint8_t* s, uint64_t csize, uint8_t* out, 
     const int rc = lzf_decode_stages(s, csize, usize, out, keep, chunk, ntok, msg);
     set_err(err, errcap, msg);
     return rc;
+}
+
+// ---- erasor/node bags: bag_index.h's index, and its per-point decode run serially (what erasor_bag_load's gather computes) ----
+static bag::Index g_bag;
+
+// erasor_bag_index on the host; the index is kept for the two calls below
+int erasor_hostcheck_bag_index(const char* file, size_t len, const char* topic, int keep_first, size_t* n_nodes, erasor_bag_info_t* info,
+                               char* err, size_t errcap) {
+    std::string msg;
+    *n_nodes = 0;
+    *info = erasor_bag_info_t{};
+    const int rc = bag::build_index(reinterpret_cast<const uint8_t*>(file), len, topic ? topic : "/node/combined/optimized", keep_first != 0, g_bag, msg);
+    set_err(err, errcap, msg);
+    if (rc != ERASOR_OK) return rc;
+    *n_nodes = g_bag.nodes.size();
+    bag::fill_info(g_bag, *info);
+    return ERASOR_OK;
+}
+
+int erasor_hostcheck_bag_nodes(size_t first, size_t count, uint32_t* seq, uint64_t* stamp_ns, double* odom7, erasor_bag_cloud_t* clouds) {
+    if (first > g_bag.nodes.size() || count > g_bag.nodes.size() - first) return ERASOR_E_INVALID;
+    for (size_t k = 0; k < count; ++k) {
+        const bag::Node& nd = g_bag.nodes[first + k];
+        seq[k] = nd.seq;
+        stamp_ns[k] = nd.stamp_ns;
+        std::memcpy(odom7 + 7 * k, nd.odom, sizeof(nd.odom));
+        bag::fill_cloud(nd.cloud, clouds[k]);
+    }
+    return ERASOR_OK;
+}
+
+// the clouds of nodes [first, first + count) of the indexed file, back to back; offsets: count + 1
+int erasor_hostcheck_bag_decode(const char* file, size_t first, size_t count, float* out, uint64_t* offsets, char* err, size_t errcap) {
+    uint64_t total = 0;
+    std::string msg;
+    std::vector<uint64_t> list(count);
+    for (size_t k = 0; k < count; ++k) list[k] = first + k;
+    int rc = bag::check_range(g_bag, first, count, msg);
+    if (rc == ERASOR_OK) rc = bag::check_list(g_bag, list.data(), count, &total, msg);
+    set_err(err, errcap, msg);
+    if (rc != ERASOR_OK) return rc;
+    offsets[0] = 0;
+    for (size_t k = 0; k < count; ++k) {
+        const bag::Cloud& c = g_bag.nodes[first + k].cloud;
+        const uint8_t* d = reinterpret_cast<const uint8_t*>(file) + c.data_off;
+        const uint64_t n = bag::cloud_points(c);
+        uint32_t* o = reinterpret_cast<uint32_t*>(out) + 4 * offsets[k];
+        for (uint64_t i = 0; i < n; ++i) bag::point_values(d + bag::point_offset(c, i), c, o + 4 * i);
+        offsets[k + 1] = offsets[k] + n;
+    }
+    return ERASOR_OK;
 }
 
 // A serial liblzf-style decoder (one token after the other, bytes copied one at a time): 0, or -1 for a malformed stream

@@ -14,6 +14,8 @@
 // Load (erasor_pcd_load, DESIGN.md section 12.1): ascii goes to the parse above; binary is one pass of k_pcd_gather_tile; a
 // binary_compressed stream is decoded by k_lzf_walk (speculative token discovery), k_lzf_compose (scan of the chunks' entry maps),
 // k_lzf_records, k_lzf_expand / k_lzf_jump / k_lzf_fill (pointer jumping over back-references), then gathered by k_pcd_gather.
+// Bags (erasor_bag_*, DESIGN.md section 12.2): the index is bag_index.h, on the host; one k_bag_gather launch decodes the clouds of a
+// load from the selected blobs.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -23,6 +25,7 @@
 #include <vector>
 
 #include "../../include/erasor_b200.h"
+#include "bag_index.h"
 #include "pcd_binary.h"
 #include "pcd_codec.h"
 
@@ -425,6 +428,67 @@ __global__ void __launch_bounds__(kThreads) k_lzf_fill(const uint32_t* src, uint
         pcd::lzf_fill(src, out, j);
 }
 
+// ---- erasor/node bags (DESIGN.md section 12.2; the index and the per-point decode are bag_index.h) --------------------------
+// One cloud of a erasor_bag_load call.  A cloud whose rows are contiguous (row_step == width x point_step, or one row) is one row
+// of n points; otherwise each of its rows is tiled on its own, so that a tile never spans row padding.
+struct BagDesc {
+    uint64_t src;                    // the cloud's data in the device copy of the blobs (16-byte aligned)
+    uint64_t out;                    // its first output point
+    uint64_t tile0;                  // its first tile
+    uint64_t cols;                   // points per row as tiled
+    uint64_t tiles_per_row;
+    uint32_t per_tile;               // points per tile
+    uint32_t staged;                 // 1: a tile's bytes are staged in shared memory; 0: read from global memory point by point
+    uint32_t reach;                  // bag::point_reach
+    bag::Cloud c;
+};
+
+// one CTA per tile: the cloud by binary search over tile0, then as k_pcd_gather_tile, at the cloud's row_step and point_step
+__global__ void __launch_bounds__(kGatherThreads) k_bag_gather(const uint8_t* blobs, const BagDesc* d, int nclouds, uint64_t ntiles, uint4* out) {
+    __shared__ __align__(16) uint8_t tile[kGatherTile + 32];
+    for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        int lo = 0, hi = nclouds - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (d[mid].tile0 <= t) lo = mid; else hi = mid - 1;
+        }
+        const BagDesc& D = d[lo];
+        const uint64_t lt = t - D.tile0, r = lt / D.tiles_per_row, c0 = (lt - r * D.tiles_per_row) * D.per_tile;
+        const uint32_t np = (uint32_t)min((uint64_t)D.per_tile, D.cols - c0);
+        const uint32_t step = D.c.point_step;
+        const uint8_t* src = blobs + D.src + r * D.c.row_step + c0 * step;
+        uint4* o = out + D.out + r * D.cols + c0;
+        if (D.staged) {
+            const uintptr_t lo_a = reinterpret_cast<uintptr_t>(src), hi_a = lo_a + (uint64_t)(np - 1) * step + D.reach;
+            const uintptr_t a0 = lo_a & ~uintptr_t(15), a1 = (hi_a + 15) & ~uintptr_t(15);
+            for (uintptr_t a = a0 + 16u * threadIdx.x; a < a1; a += 16u * blockDim.x) {
+                uint8_t* dst = tile + (a - a0);
+                if (a >= lo_a && a + 16 <= hi_a) {
+                    *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(a);
+                } else {
+                    for (int k = 0; k < 16; ++k) dst[k] = (a + k >= lo_a && a + k < hi_a) ? *reinterpret_cast<const uint8_t*>(a + k) : 0;
+                }
+            }
+            __syncthreads();
+            const uint8_t* s = tile + (lo_a - a0);
+            for (uint32_t j = threadIdx.x; j < np; j += blockDim.x) {
+                uint32_t v[4];
+                bag::point_values(s + (uint64_t)j * step, D.c, v);
+                o[j] = make_uint4(v[0], v[1], v[2], v[3]);
+            }
+            __syncthreads();
+        } else {
+            for (uint32_t j = threadIdx.x; j < np; j += blockDim.x) {
+                uint32_t v[4];
+                bag::point_values(src + (uint64_t)j * step, D.c, v);
+                o[j] = make_uint4(v[0], v[1], v[2], v[3]);
+            }
+        }
+    }
+}
+
+constexpr uint64_t kBagStage = 32ull << 20;          // bytes per pinned staging buffer (two) for a pageable file
+
 uint32_t blocks_for(uint64_t n, int per, int cap) { return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + per - 1) / per, (uint64_t)cap)); }
 }  // namespace
 
@@ -435,8 +499,15 @@ struct erasor_pcd_ctx {
     DevBuf text, chunk_cnt, chunk_off, lines, flags, rows, sums, out, stats;   // parse
     DevBuf pts, lens, offs, ftext;                                              // format
     DevBuf lz_map0, lz_map1, lz_tok, lz_byt, lz_entry, lz_ctok, lz_cbyt, lz_tokoff, lz_byteoff, lz_rec, lz_src, lz_dec, lz_flags;   // load
+    DevBuf bag_blobs, bag_desc;                                                 // erasor_bag_load
     PcdStats* h_stats = nullptr;                                                // pinned
     int sm_count = 132;
+    // erasor_bag_index's index and file (the caller's memory), and the pinned staging of a pageable file
+    bag::Index bag;
+    bool bag_ok = false, bag_pinned = false;
+    const uint8_t* bag_file = nullptr;
+    uint8_t* bag_stage[2] = {nullptr, nullptr};
+    cudaEvent_t bag_ev[2] = {nullptr, nullptr};
     // erasor_pcd_format_ascii's text of its last call, kept for a following call with the same input
     bool cached = false;
     const float* c_ptr = nullptr;
@@ -585,7 +656,12 @@ void erasor_pcd_destroy(erasor_pcd_t p) {
     if (p->st) cudaStreamSynchronize(p->st);
     for (DevBuf* b : {&p->text, &p->chunk_cnt, &p->chunk_off, &p->lines, &p->flags, &p->rows, &p->sums, &p->out, &p->stats, &p->pts,
                       &p->lens, &p->offs, &p->ftext, &p->lz_map0, &p->lz_map1, &p->lz_tok, &p->lz_byt, &p->lz_entry, &p->lz_ctok,
-                      &p->lz_cbyt, &p->lz_tokoff, &p->lz_byteoff, &p->lz_rec, &p->lz_src, &p->lz_dec, &p->lz_flags}) b->release();
+                      &p->lz_cbyt, &p->lz_tokoff, &p->lz_byteoff, &p->lz_rec, &p->lz_src, &p->lz_dec, &p->lz_flags, &p->bag_blobs,
+                      &p->bag_desc}) b->release();
+    for (int k = 0; k < 2; ++k) {
+        if (p->bag_stage[k]) cudaFreeHost(p->bag_stage[k]);
+        if (p->bag_ev[k]) cudaEventDestroy(p->bag_ev[k]);
+    }
     if (p->h_stats) cudaFreeHost(p->h_stats);
     if (p->st) cudaStreamDestroy(p->st);
     delete p;
@@ -840,6 +916,150 @@ int erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind,
     PCK(cudaStreamSynchronize(p->st));
     *n = (size_t)L.points;
     return done(ERASOR_OK);
+}
+
+int erasor_bag_index(erasor_pcd_t p, const char* file, size_t len, const char* topic, int keep_first, size_t* n_nodes, erasor_bag_info_t* info) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    p->cached = false;
+    p->bag_ok = false;
+    p->bag = bag::Index();
+    p->bag_file = nullptr;
+    if (info) *info = erasor_bag_info_t{};
+    if (!n_nodes || (len && !file)) return fail(p, ERASOR_E_INVALID, "null argument");
+    *n_nodes = 0;
+    PCK(cudaSetDevice(p->device));
+    std::string msg;
+    const int rc = bag::build_index(reinterpret_cast<const uint8_t*>(file), len, topic ? topic : "/node/combined/optimized", keep_first != 0, p->bag, msg);
+    if (rc != ERASOR_OK) { p->bag = bag::Index(); return fail(p, rc, msg); }
+    cudaPointerAttributes a{};
+    p->bag_pinned = cudaPointerGetAttributes(&a, file) == cudaSuccess && a.type == cudaMemoryTypeHost;
+    cudaGetLastError();
+    p->bag_file = reinterpret_cast<const uint8_t*>(file);
+    p->bag_ok = true;
+    *n_nodes = p->bag.nodes.size();
+    if (info) bag::fill_info(p->bag, *info);
+    return ERASOR_OK;
+}
+
+int erasor_bag_nodes(erasor_pcd_t p, size_t first, size_t count, uint32_t* seq, uint64_t* stamp_ns, double* odom7, erasor_bag_cloud_t* clouds) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    if (!p->bag_ok) return fail(p, ERASOR_E_STATE, "no bag indexed: call erasor_bag_index first");
+    std::string msg;
+    const int rc = bag::check_range(p->bag, first, count, msg);
+    if (rc != ERASOR_OK) return fail(p, rc, msg);
+    for (size_t k = 0; k < count; ++k) {
+        const bag::Node& nd = p->bag.nodes[first + k];
+        if (seq) seq[k] = nd.seq;
+        if (stamp_ns) stamp_ns[k] = nd.stamp_ns;
+        if (odom7) std::memcpy(odom7 + 7 * k, nd.odom, sizeof(nd.odom));
+        if (clouds) bag::fill_cloud(nd.cloud, clouds[k]);
+    }
+    return ERASOR_OK;
+}
+
+int erasor_bag_load(erasor_pcd_t p, size_t first, size_t count, float* out_xyzi, size_t cap, int out_kind, uint64_t* offsets) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    if (!p->bag_ok) return fail(p, ERASOR_E_STATE, "no bag indexed: call erasor_bag_index first");
+    std::string msg;
+    const int rc = bag::check_range(p->bag, first, count, msg);
+    if (rc != ERASOR_OK) return fail(p, rc, msg);
+    std::vector<uint64_t> list(count);
+    for (size_t k = 0; k < count; ++k) list[k] = first + k;
+    return erasor_bag_load_list(p, list.data(), count, out_xyzi, cap, out_kind, offsets);
+}
+
+int erasor_bag_load_list(erasor_pcd_t p, const uint64_t* nodes, size_t count, float* out_xyzi, size_t cap, int out_kind, uint64_t* offsets) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    p->cached = false;
+    if (!p->bag_ok) return fail(p, ERASOR_E_STATE, "no bag indexed: call erasor_bag_index first");
+    if (!offsets || (count && !nodes)) return fail(p, ERASOR_E_INVALID, "null argument");
+    if (out_kind != ERASOR_PTR_HOST && out_kind != ERASOR_PTR_DEVICE) return fail(p, ERASOR_E_INVALID, "out_kind must be ERASOR_PTR_HOST or ERASOR_PTR_DEVICE");
+    uint64_t total = 0;
+    std::string msg;
+    int rc = bag::check_list(p->bag, nodes, count, &total, msg);
+    if (rc != ERASOR_OK) return fail(p, rc, msg);
+    offsets[0] = 0;
+    for (size_t k = 0; k < count; ++k) offsets[k + 1] = offsets[k] + bag::cloud_points(p->bag.nodes[nodes[k]].cloud);
+    if (!out_xyzi) return ERASOR_OK;
+    if (cap < total) return fail(p, ERASOR_E_CAPACITY, "out_xyzi holds fewer points than the nodes' clouds");
+    if (out_kind == ERASOR_PTR_DEVICE && (reinterpret_cast<uintptr_t>(out_xyzi) & 15u))
+        return fail(p, ERASOR_E_INVALID, "device clouds must be 16-byte aligned (one float4 per point)");
+    if (!total) return ERASOR_OK;
+    PCK(cudaSetDevice(p->device));
+
+    // the clouds' descriptors and the device copy of their data, each blob at a 16-byte aligned offset
+    std::vector<BagDesc> desc;
+    uint64_t blob_bytes = 0, ntiles = 0;
+    for (size_t k = 0; k < count; ++k) {
+        const bag::Cloud& c = p->bag.nodes[nodes[k]].cloud;
+        const uint64_t n = bag::cloud_points(c);
+        if (!n) continue;
+        BagDesc D{};
+        D.c = c;
+        D.src = blob_bytes;
+        D.out = offsets[k];
+        D.tile0 = ntiles;
+        D.reach = bag::point_reach(c);
+        const bool rows_contiguous = c.height == 1 || (uint64_t)c.row_step == (uint64_t)c.width * c.point_step;
+        D.cols = rows_contiguous ? n : c.width;
+        const uint64_t rows = rows_contiguous ? 1 : c.height;
+        D.staged = D.reach <= kGatherTile;
+        D.per_tile = D.staged ? (uint32_t)std::min<uint64_t>(4 * kGatherThreads, 1 + (kGatherTile - D.reach) / std::max<uint32_t>(c.point_step, 1))
+                              : 4 * kGatherThreads;
+        D.tiles_per_row = (D.cols + D.per_tile - 1) / D.per_tile;
+        ntiles += rows * D.tiles_per_row;
+        blob_bytes += (c.data_len + 15) & ~15ull;
+        desc.push_back(D);
+    }
+    PCK(p->bag_blobs.ensure(blob_bytes));
+    PCK(p->bag_desc.ensure(sizeof(BagDesc) * desc.size()));
+    uint8_t* d_blobs = p->bag_blobs.as<uint8_t>();
+    if (p->bag_pinned) {
+        for (const BagDesc& D : desc) PCK(cudaMemcpyAsync(d_blobs + D.src, p->bag_file + D.c.data_off, D.c.data_len, cudaMemcpyHostToDevice, p->st));
+    } else {
+        // a window of the device layout at a time: filled on the host in one pinned buffer while the other one's copy runs
+        for (int k = 0; k < 2; ++k) {
+            if (!p->bag_stage[k]) PCK(cudaMallocHost(&p->bag_stage[k], kBagStage));
+            if (!p->bag_ev[k]) PCK(cudaEventCreateWithFlags(&p->bag_ev[k], cudaEventDisableTiming));
+        }
+        int cur = 0;
+        uint64_t w0 = 0, filled = 0;                  // the window [w0, w0 + kBagStage) of the device layout; bytes of it filled
+        auto flush = [&]() -> cudaError_t {
+            cudaError_t e = cudaMemcpyAsync(d_blobs + w0, p->bag_stage[cur], filled, cudaMemcpyHostToDevice, p->st);
+            if (e == cudaSuccess) e = cudaEventRecord(p->bag_ev[cur], p->st);
+            cur ^= 1;
+            w0 += filled;
+            filled = 0;
+            return e == cudaSuccess ? cudaEventSynchronize(p->bag_ev[cur]) : e;    // the buffer filled next is free again
+        };
+        PCK(cudaEventSynchronize(p->bag_ev[0]));
+        PCK(cudaEventSynchronize(p->bag_ev[1]));
+        for (const BagDesc& D : desc) {
+            uint64_t done = 0;
+            while (done < D.c.data_len) {
+                const uint64_t at = D.src + done;      // device offset of the next byte
+                if (at - w0 >= kBagStage) PCK(flush());
+                const uint64_t take = std::min(D.c.data_len - done, kBagStage - (at - w0));
+                std::memcpy(p->bag_stage[cur] + (at - w0), p->bag_file + D.c.data_off + done, take);
+                filled = at - w0 + take;
+                done += take;
+            }
+        }
+        if (filled) PCK(flush());
+    }
+    PCK(cudaMemcpyAsync(p->bag_desc.p, desc.data(), sizeof(BagDesc) * desc.size(), cudaMemcpyHostToDevice, p->st));
+    uint4* d_out = reinterpret_cast<uint4*>(out_xyzi);
+    if (out_kind == ERASOR_PTR_HOST) { PCK(p->out.ensure(sizeof(uint4) * total)); d_out = p->out.as<uint4>(); }
+    const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(ntiles, (uint64_t)p->sm_count * 8));
+    k_bag_gather<<<grid, kGatherThreads, 0, p->st>>>(d_blobs, p->bag_desc.as<BagDesc>(), (int)desc.size(), ntiles, d_out);
+    PCK(cudaGetLastError());
+    if (out_kind == ERASOR_PTR_HOST) PCK(cudaMemcpyAsync(out_xyzi, d_out, sizeof(uint4) * total, cudaMemcpyDeviceToHost, p->st));
+    PCK(cudaStreamSynchronize(p->st));
+    return ERASOR_OK;
 }
 
 }  // extern "C"

@@ -1,7 +1,7 @@
 """The reference's three-stage workflow in one call, ROS stripped (README "How to run": mapgen -> offline_map_updater ->
 scripts/analysis_runner.py):
 
-    nodes (erasor_b200.kitti.iter_nodes, or any iterable of (seq, odom7, cloud))
+    nodes (erasor_b200.kitti.iter_nodes, a reference bag through read_bag_nodes, or any iterable of (seq, odom7, cloud))
       -> naive map            erasor_b200.mapgen           (src/mapgen)
       -> static map           capi.Updater, one erasor_updater_process_node per node + save_static_map
                               (OfflineMapUpdater::callback_node / save_static_map, OfflineMapUpdater.cpp:174-330)
@@ -85,13 +85,19 @@ def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep
 
 
 def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, make_updater: Optional[Callable] = None,
-                 map_leafsize: Optional[float] = None, out_dir: Optional[str] = None) -> dict:
+                 map_leafsize: Optional[float] = None, out_dir: Optional[str] = None, frame_independent: bool = False) -> dict:
     """mapgen -> updater -> evaluation on one node list.  GT for PR/RR = the naive map itself (it carries the labels), which is
-    how the reference scores a run (analysis_runner.py compares <seq>_..._original / voxelised map with the result)."""
+    how the reference scores a run (analysis_runner.py compares <seq>_..._original / voxelised map with the result).
+    frame_independent runs node mode (run_frame_independent) on the naive map instead of the sequential updater."""
     nodes = list(nodes)
     leaf = float(up.map_voxel_size if map_leafsize is None else map_leafsize)
     original, naive = mapgen.build_map(nodes, leafsize=leaf, is_large_scale=bool(up.is_large_scale), voxelize=voxelize)
-    res = run_offline(nodes, naive, up, ep, make_updater=make_updater)
+    if frame_independent:
+        if make_updater is not None:
+            raise ValueError("node mode runs on the device: make_updater does not apply")
+        res = run_frame_independent(nodes, naive, up, ep)
+    else:
+        res = run_offline(nodes, naive, up, ep, make_updater=make_updater)
     res["naive_map"] = naive
     if make_updater is None:            # the device updater ran: score on the device too (same counts, same dict)
         from . import capi
@@ -119,3 +125,22 @@ def run_semantickitti(dataset_root: str, sequence: str, init_stamp: int, end_sta
     """SemanticKITTI files + a reference config/*.yaml -> static map and PR/RR."""
     ep, up = params.load_yaml(config_yaml)
     return run_sequence(kitti.iter_nodes(dataset_root, sequence, init_stamp, end_stamp, interval), up, ep, out_dir=out_dir, **kw)
+
+
+def read_bag_nodes(bag_path: str, topic: str = "/node/combined/optimized", keep_first: bool = False, device: int = 0) -> list:
+    """The (seq, odom7, cloud) list of a ROS bag of erasor/node messages (the reference's <seq>_..._node.bag), as the reference's
+    subscribers receive it: the first message dropped unless keep_first.  Indexed on the host, decoded on the device
+    (capi.PcdCodec.bag_index / bag_nodes)."""
+    from . import capi
+    with open(bag_path, "rb") as f:
+        data = f.read()
+    with capi.PcdCodec(device) as codec:
+        codec.bag_index(data, topic, keep_first)
+        return list(codec.bag_nodes())
+
+
+def run_bag(bag: str, config_yaml: str, out_dir: Optional[str] = None, frame_independent: bool = False, **kw) -> dict:
+    """A reference bag + a reference config/*.yaml -> naive map, static map and PR/RR: run_sequence on the bag's nodes, with the
+    sequential updater or, with frame_independent, node mode."""
+    ep, up = params.load_yaml(config_yaml)
+    return run_sequence(read_bag_nodes(bag), up, ep, out_dir=out_dir, frame_independent=frame_independent, **kw)

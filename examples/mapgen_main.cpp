@@ -6,7 +6,10 @@
 //   <save_path>/<seq>_<init>_to_<final>_w_interval<k>_voxel_<std::to_string(voxelsize)>.pcd            ... voxelised at voxelsize
 // seq, init, final and k come from the target name, split at '_' as parseRosbagName does (main.cpp:66-101), e.g.
 // 05_0_to_2502_w_interval_2_node.bag.
+// With a ROS bag of erasor/node messages instead (a path ending in .bag), the nodes are the bag's (NodeBag, as kitti_mapgen receives
+// them from rosbag play) and the target name is the bag's file name.
 //   usage: mapgen_main <data_dir> <target_name> <save_path> [voxelsize = 0.05] [is_large_scale = false]
+//          mapgen_main <file.bag> <save_path> [voxelsize = 0.05] [is_large_scale = false]
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -69,14 +72,18 @@ static std::vector<std::array<double, 7>> load_poses(const std::string& csv) {
 }
 
 int main(int argc, char** argv) {
-    if (argc < 4) {
-        std::fprintf(stderr, "usage: %s <data_dir> <target_name> <save_path> [voxelsize = 0.05] [is_large_scale = false]\n", argv[0]);
+    const bool from_bag = argc > 1 && is_bag_path(argv[1]);
+    const int a = from_bag ? 1 : 0;                   // the bag form has no target_name argument
+    if (argc < 4 - a) {
+        std::fprintf(stderr, "usage: %s <data_dir> <target_name> <save_path> [voxelsize = 0.05] [is_large_scale = false]\n"
+                             "       %s <file.bag> <save_path> [voxelsize = 0.05] [is_large_scale = false]\n", argv[0], argv[0]);
         return 2;
     }
     try {
-        const std::string data_dir = argv[1], target = argv[2], save_path = argv[3];
-        const float voxelsize = argc > 4 ? std::stof(argv[4]) : 0.05f;                       // /map/voxelsize (main.cpp:87)
-        const std::string ls = argc > 5 ? argv[5] : "false";                                  // /large_scale/is_large_scale (:95)
+        const std::string data_dir = argv[1], save_path = argv[3 - a];
+        const std::string target = from_bag ? data_dir.substr(data_dir.find_last_of('/') == std::string::npos ? 0 : data_dir.find_last_of('/') + 1) : argv[2];
+        const float voxelsize = argc > 4 - a ? std::stof(argv[4 - a]) : 0.05f;               // /map/voxelsize (main.cpp:87)
+        const std::string ls = argc > 5 - a ? argv[5 - a] : "false";                          // /large_scale/is_large_scale (:95)
         const bool is_large_scale = (ls == "true" || ls == "True" || ls == "1");
         const auto parsed = parse_target_name(target);
         if (parsed.size() < 7) throw std::invalid_argument("target name '" + target + "' has fewer than 7 '_'-separated fields before the last");
@@ -85,10 +92,25 @@ int main(int argc, char** argv) {
         const std::string stem = save_path + "/" + sequence + "_" + init_stamp + "_to_" + final_stamp + "_w_interval" + std::to_string(interval) +
                                  "_voxel_" + std::to_string(voxelsize);
 
+        NaiveMapGen gen(voxelsize, is_large_scale);
+        if (from_bag) {
+            NodeBag bag(data_dir);
+            std::cout << "[MAPGEN]: " << bag.size() << " nodes, voxelization size " << voxelsize << ", large-scale " << is_large_scale << std::endl;
+            DeviceCloud buf[2];                       // as below: node i + 1 is decoded while node i runs
+            auto read = [&](size_t i) { DeviceCloud& b = buf[i % 2]; b.set_size(bag.load_device(i, 1, [&](size_t n) { return b.reserve(n); })[1]); };
+            if (bag.size()) read(0);
+            for (size_t i = 0; i < bag.size(); ++i) {
+                gen.synchronize();
+                gen.accumPointCloud(bag.node(i).odom.data(), buf[i % 2].data(), buf[i % 2].size());
+                if (i + 1 < bag.size()) read(i + 1);
+            }
+            gen.saveNaiveMap(stem + "_original.pcd", stem + ".pcd");
+            std::cout << "[MAPGEN]: saved " << stem << ".pcd" << std::endl;
+            return 0;
+        }
         const auto poses = load_poses(data_dir + "/poses_lidar2body.csv");
         std::cout << "[MAPGEN]: " << poses.size() << " nodes, voxelization size " << voxelsize << ", large-scale " << is_large_scale << std::endl;
         PcdCodec codec;
-        NaiveMapGen gen(voxelsize, is_large_scale);
         auto scan_path = [&](size_t i) { char name[64]; std::snprintf(name, sizeof(name), "/pcds/%06zu.pcd", i); return data_dir + name; };
         // Two scan buffers: scan i + 1 is read on the device while node i runs.  The generator reads a device scan asynchronously,
         // so before node i is handed over, node i - 1 -- the last reader of the buffer scan i + 1 will go to -- must be finished.

@@ -4,7 +4,11 @@
 // and <data_dir>/pcds/%06d.pcd (each read on the device by PcdCodec::load, in any DATA mode: ascii, binary or binary_compressed, as
 // the reference's pcl::io::loadPCDFile reads them), feeds every node to the device-resident OfflineMapUpdater and writes
 // <save_path>/<data_name>_result.pcd with save_static_map(0.2) (:123), formatted on the device.
+// With a path ending in .bag instead of <data_dir>, the nodes come from a ROS bag of erasor/node messages (NodeBag, as the reference's
+// offline_map_updater receives them from rosbag play): the map is the yaml's initial_map_path, read by PcdCodec::load; seq is each
+// node's header.seq and its odom goes in as the bag's doubles; each next cloud is decoded on the device into the second buffer.
 //   usage: offline_map_updater_main <config.yaml> <data_dir> [init_idx]
+//          offline_map_updater_main <config.yaml> <file.bag> [init_idx]
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -65,12 +69,37 @@ static std::vector<std::array<double, 7>> load_all_poses(const std::string& txt)
     return poses;
 }
 
+// the bag form: the same loop over the bag's nodes
+static void run_bag(const Config& cfg, const std::string& bag_path, int init_idx) {
+    PcdCodec codec;
+    PointCloud map = codec.load(cfg.initial_map_path);
+    OfflineMapUpdater updater(cfg, map);
+    PointCloud().swap(map);
+    NodeBag bag(bag_path);
+    std::cout << "Total " << bag.size() << " nodes are loaded" << std::endl;
+    auto read = [&](size_t i, DeviceCloud& out) { out.set_size(bag.load_device(i, 1, [&](size_t n) { return out.reserve(n); })[1]); };
+    const size_t n_nodes = bag.size(), first = init_idx > 0 ? (size_t)init_idx : 0;
+    DeviceCloud cur, nxt;
+    if (first < n_nodes) read(first, cur);
+    for (size_t i = first; i < n_nodes; ++i) {
+        if (i + 1 < n_nodes) {
+            read(i + 1, nxt);
+            if (updater.processes_call(2)) updater.prefetch_device(nxt.data(), nxt.size());
+        }
+        updater.callback_node_device((int)bag.node(i).seq, bag.node(i).odom.data(), cur.data(), cur.size());
+        cur.swap(nxt);
+    }
+    updater.save_static_map(0.2f);
+    std::cout << "Static map building complete!" << std::endl;
+}
+
 int main(int argc, char** argv) {
-    if (argc < 3) { std::fprintf(stderr, "usage: %s <config.yaml> <data_dir> [init_idx]\n", argv[0]); return 2; }
+    if (argc < 3) { std::fprintf(stderr, "usage: %s <config.yaml> <data_dir | file.bag> [init_idx]\n", argv[0]); return 2; }
     try {
         Config cfg = load_config(argv[1]);
         const std::string data_dir = argv[2];
         const int init_idx = argc > 3 ? std::atoi(argv[3]) : 0;
+        if (is_bag_path(data_dir)) { run_bag(cfg, data_dir, init_idx); return 0; }
         cfg.initial_map_path = data_dir + "/dense_global_map.pcd";
         PcdCodec codec;
         PointCloud map = codec.load(cfg.initial_map_path);

@@ -5,7 +5,10 @@
 // batch's raw scans are voxelised and moved to the body frame on the device in one submission (ERASOR::process_scans).  The kept
 // map, voxelised at 0.2 m as offline_map_updater_main saves it (main_in_your_env.cpp:123), goes to <save_path>/<data_name>_result.pcd,
 // formatted on the device.  One GPU; multi-GPU callers shard the nodes and combine the masks with erasor_comm_*.
+// With a ROS bag of erasor/node messages instead of <data_dir> (a path ending in .bag), the map is the yaml's initial_map_path, the
+// poses are the bag's doubles, and each batch's clouds are decoded from the bag on the device in one call (NodeBag::load_device).
 //   usage: static_map_nodes_main <config.yaml> <data_dir> [init_idx] [batch]
+//          static_map_nodes_main <config.yaml> <file.bag> [init_idx] [batch]
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -74,11 +77,31 @@ int main(int argc, char** argv) {
         ERASOR erasor(ep);
         PcdCodec codec;
         DeviceBuffer map;
-        const size_t n_map = codec.load_device(data_dir + "/dense_global_map.pcd", [&](size_t n) { return map.reserve(n); });
+        const bool from_bag = is_bag_path(data_dir);
+        const size_t n_map = codec.load_device(from_bag ? cfg.initial_map_path : data_dir + "/dense_global_map.pcd", [&](size_t n) { return map.reserve(n); });
         erasor.load_global_map_device(map.data(), n_map);
-        const auto poses = load_all_poses(data_dir + "/poses_lidar2body.csv");
         std::array<double, 7> l2b;
         for (int i = 0; i < 7; ++i) l2b[i] = cfg.updater.lidar2body[i];
+        if (from_bag) {
+            NodeBag bag(data_dir);
+            std::vector<uint64_t> sel;
+            for (size_t i = init_idx > 0 ? (size_t)init_idx : 0; i < bag.size(); ++i)
+                if ((i - init_idx + 1) % cfg.updater.removal_interval == 0) sel.push_back(i);
+            DeviceBuffer raw;
+            for (size_t b0 = 0; b0 < sel.size(); b0 += (size_t)batch) {
+                const std::vector<uint64_t> nodes(sel.begin() + b0, sel.begin() + std::min(sel.size(), b0 + (size_t)batch));
+                std::vector<std::array<double, 7>> bp;
+                for (uint64_t i : nodes) bp.push_back(bag.node(i).odom);
+                const std::vector<uint64_t> off = bag.load_device(nodes, [&](size_t m) { return raw.reserve(m); });
+                erasor.process_scans(bp, raw.data(), off, cfg.updater.query_voxel_size, l2b, cfg.updater.max_range, ERASOR_PTR_DEVICE);
+            }
+            const ERASOR::DeviceClouds saved = erasor.save_static_map(0.2f);
+            const std::string target = cfg.save_path + "/" + cfg.data_name + "_result.pcd";
+            codec.write_device(target, saved.d_xyzi, saved.offsets[1]);
+            std::cout << sel.size() << " of " << bag.size() << " bag nodes processed; " << saved.offsets[1] << " points saved to " << target << std::endl;
+            return 0;
+        }
+        const auto poses = load_all_poses(data_dir + "/poses_lidar2body.csv");
         // the nodes callback_node processes: its k-th call (k = 1, 2, ...) unless k % removal_interval != 0 ("PASS!", :328)
         std::vector<int> sel;
         for (int i = init_idx; i < (int)poses.size(); ++i)

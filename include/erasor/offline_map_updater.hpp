@@ -8,6 +8,7 @@
 // Config: the reference's rosparam tree (config/*.yaml: /erasor/*, /MapUpdater/*, /large_scale/*, /tf/lidar2body,
 // /verbose) is read by load_config(); no yaml-cpp is needed for the two-level key: value files the reference ships.
 #pragma once
+#include <algorithm>
 #include <array>
 #include <cstdio>
 #include <cstring>
@@ -16,6 +17,7 @@
 #include <sstream>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "erasor.hpp"
@@ -236,6 +238,83 @@ private:
     erasor_pcd_t p_ = nullptr;
     std::vector<char> text_;
 };
+
+// A ROS bag of erasor/node messages (the reference's <seq>_..._node.bag, DESIGN.md section 12.2): indexed on the host when
+// constructed, clouds decoded on the device (erasor_bag_*).  The nodes are the messages on `topic` as the reference's subscribers
+// receive them: the first one is dropped unless keep_first.
+struct BagNode {
+    uint32_t seq;                    // header.seq
+    std::array<double, 7> odom;      // x y z qx qy qz qw, as stored
+};
+
+class NodeBag {
+public:
+    explicit NodeBag(const std::string& path, const std::string& topic = "/node/combined/optimized", bool keep_first = false, int device = 0)
+        : path_(path) {
+        if (erasor_pcd_create(device, &p_) != ERASOR_OK) throw std::runtime_error(std::string("NodeBag: ") + erasor_pcd_last_error(nullptr));
+        std::ifstream f(path, std::ios::binary | std::ios::ate);
+        if (!f) { erasor_pcd_destroy(p_); throw std::invalid_argument("cannot open " + path); }
+        file_.resize((size_t)f.tellg());
+        f.seekg(0);
+        if (!file_.empty() && !f.read(file_.data(), (std::streamsize)file_.size())) { erasor_pcd_destroy(p_); throw std::runtime_error("cannot read " + path); }
+        size_t n = 0;
+        int rc = erasor_bag_index(p_, file_.data(), file_.size(), topic.c_str(), keep_first ? 1 : 0, &n, &info_);
+        std::vector<uint32_t> seq(n);
+        std::vector<double> odom(7 * n);
+        if (rc == ERASOR_OK) rc = erasor_bag_nodes(p_, 0, n, seq.data(), nullptr, odom.data(), nullptr);
+        if (rc != ERASOR_OK) {
+            const std::string msg = path + ": " + erasor_pcd_last_error(p_);
+            erasor_pcd_destroy(p_);
+            if (rc == ERASOR_E_UNSUPPORTED) throw UnsupportedPcd(msg);
+            if (rc == ERASOR_E_INVALID) throw std::invalid_argument(msg);
+            throw std::runtime_error(msg);
+        }
+        nodes_.resize(n);
+        for (size_t i = 0; i < n; ++i) {
+            nodes_[i].seq = seq[i];
+            std::copy(odom.begin() + 7 * i, odom.begin() + 7 * i + 7, nodes_[i].odom.begin());
+        }
+    }
+    ~NodeBag() { erasor_pcd_destroy(p_); }
+    NodeBag(const NodeBag&) = delete;
+    NodeBag& operator=(const NodeBag&) = delete;
+
+    size_t size() const { return nodes_.size(); }
+    const BagNode& node(size_t i) const { return nodes_.at(i); }
+    const erasor_bag_info_t& info() const { return info_; }
+    // The clouds of nodes [first, first + count) -- or of the listed nodes -- back to back in device memory, from one gather
+    // launch.  device_buffer(n) must return a 16-byte aligned device pointer with room for n points (the caller owns the memory).
+    // Returns the count + 1 offsets.  Synchronous: the clouds are complete on return.
+    template <class DeviceBuffer>
+    std::vector<uint64_t> load_device(size_t first, size_t count, DeviceBuffer&& device_buffer) {
+        std::vector<uint64_t> list(count);
+        for (size_t k = 0; k < count; ++k) list[k] = first + k;
+        return load_device(list, std::forward<DeviceBuffer>(device_buffer));
+    }
+    template <class DeviceBuffer>
+    std::vector<uint64_t> load_device(const std::vector<uint64_t>& nodes, DeviceBuffer&& device_buffer) {
+        std::vector<uint64_t> off(nodes.size() + 1, 0);
+        check(erasor_bag_load_list(p_, nodes.data(), nodes.size(), nullptr, 0, ERASOR_PTR_DEVICE, off.data()));
+        float* out = device_buffer((size_t)off.back());
+        check(erasor_bag_load_list(p_, nodes.data(), nodes.size(), out, (size_t)off.back(), ERASOR_PTR_DEVICE, off.data()));
+        return off;
+    }
+
+private:
+    void check(int rc) const {
+        if (rc == ERASOR_OK) return;
+        const std::string msg = path_ + ": " + erasor_pcd_last_error(p_);
+        if (rc == ERASOR_E_INVALID) throw std::invalid_argument(msg);
+        throw std::runtime_error(msg);
+    }
+    std::string path_;
+    erasor_pcd_t p_ = nullptr;
+    std::vector<char> file_;
+    erasor_bag_info_t info_{};
+    std::vector<BagNode> nodes_;
+};
+
+inline bool is_bag_path(const std::string& path) { return path.size() > 4 && path.compare(path.size() - 4, 4, ".bag") == 0; }
 
 class OfflineMapUpdater {
 public:

@@ -435,6 +435,53 @@ typedef struct {
 int  erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind, float* out_xyzi, size_t cap, int out_kind,
                      size_t* n, erasor_pcd_load_info_t* info);
 
+/* ROS bag 2.0 files of erasor/node messages (DESIGN.md section 12.2; the format restated from its public description, rosbag is
+ * not built here).  erasor_bag_index walks the file on the host -- every record, chunks included; uncompressed chunks only -- and
+ * keeps the messages on `topic` (NULL: "/node/combined/optimized") in delivery order, a stable sort by record time.  Unless
+ * keep_first, the first of them is dropped, as the reference's subscribers drop it.  file: host memory, len bytes, which must stay
+ * valid and unchanged until the next erasor_bag_index on p; pinned memory is read by the device directly, pageable memory through
+ * a pinned staging buffer.  Errors: ERASOR_E_UNSUPPORTED for another bag version, a compressed chunk, a topic whose type is not
+ * erasor/node, a cloud without FLOAT32 x, y or z; ERASOR_E_INVALID (with the byte offset) for a record or field running past its
+ * container, a chunk whose data length differs from its size, a message on an undefined connection, a missing header field, a
+ * message longer or shorter than an erasor/node, a point read past its cloud's data; ERASOR_E_CAPACITY for a cloud of 2^31 points.
+ * A failed erasor_bag_index leaves no index: erasor_bag_nodes and erasor_bag_load then fail with ERASOR_E_STATE. */
+typedef struct {
+    uint32_t version;                /* 200 for V2.0 */
+    uint32_t pad_;
+    uint64_t chunks, connections;    /* chunk records; distinct connection ids */
+    uint64_t messages, selected;     /* message records in the file; those on the topic (before the first is dropped) */
+    uint64_t unknown_records;        /* records of an op this reader does not know, skipped */
+    uint64_t nodes;                  /* the nodes erasor_bag_nodes / erasor_bag_load index */
+    uint64_t total_points;           /* width x height summed over the nodes */
+    uint64_t intensity_zero_filled;  /* nodes whose cloud has no FLOAT32 intensity: read as 0 */
+    uint64_t big_endian;             /* nodes whose cloud sets is_bigendian (ignored, as PCL ignores it) */
+    char md5sum[40];                 /* the topic's connection md5sum, reported and not checked */
+} erasor_bag_info_t;
+
+/* one node's cloud as the gather reads it: point (r, c) at data_offset + r row_step + c point_step of the file; bit s of fields
+ * (x y z intensity) set when that value is read from offset[s], clear when it is 0 */
+typedef struct {
+    uint64_t data_offset, data_len;
+    uint32_t width, height, point_step, row_step;
+    uint32_t fields, big_endian;
+    uint32_t offset[4];
+} erasor_bag_cloud_t;
+
+int  erasor_bag_index(erasor_pcd_t p, const char* file, size_t len, const char* topic, int keep_first, size_t* n_nodes,
+                      erasor_bag_info_t* info);
+/* nodes [first, first + count): header.seq, the record time in ns, odom (x y z qx qy qz qw, doubles as stored) and the cloud
+ * layouts; every output host memory and nullable */
+int  erasor_bag_nodes(erasor_pcd_t p, size_t first, size_t count, uint32_t* seq, uint64_t* stamp_ns, double* odom7,
+                      erasor_bag_cloud_t* clouds);
+/* The clouds of nodes [first, first + count), one gather launch: float[n][4] x y z intensity back to back into out_xyzi (host or
+ * device per out_kind; a device cloud 16-byte aligned), offsets (host, count + 1) the first point of each node and the total.
+ * out_xyzi == NULL only writes the offsets.  Only the selected clouds' data crosses to the device.  Exactly the input of
+ * erasor_voxelize_batch and erasor_process_nodes, and node by node of erasor_updater_process_node and erasor_mapgen_accum.
+ * ERASOR_E_CAPACITY: cap below the total, or 2^32 - 1 points or more.  Synchronous. */
+int  erasor_bag_load(erasor_pcd_t p, size_t first, size_t count, float* out_xyzi, size_t cap, int out_kind, uint64_t* offsets);
+/* the same for the listed nodes, in list order (e.g. every removal_interval-th node); ERASOR_E_INVALID for an index past the bag */
+int  erasor_bag_load_list(erasor_pcd_t p, const uint64_t* nodes, size_t count, float* out_xyzi, size_t cap, int out_kind, uint64_t* offsets);
+
 /* ============================================================================================
  * The naive map generator with its map resident on the device: the reference's mapgen (src/mapgen/mapgen.hpp:198-305,
  * accumPointCloud / getPointClouds / saveNaiveMap without the files), DESIGN.md section 8.2.  A handle of its own: one CUDA
