@@ -256,31 +256,40 @@ def _cloud(a) -> np.ndarray:
     return a
 
 
-class Handle:
-    """One ``erasor_handle_t``: one CUDA device, one stream, fixed parameters."""
+class _Native:
+    """One handle ``h`` of a family of the C ABI, released by ``close`` (or ``with``, or garbage collection).  A subclass names
+    the family's ``*_destroy`` and ``*_last_error``; ``_create`` and ``_ck`` raise ``ErasorError`` with the family's message."""
+    _DESTROY = _LAST_ERROR = ""
+    h = None
 
-    def __init__(self, params: ErasorParams, device: int = 0):
+    def _create(self, create: str, *args):
+        """self.h = the handle L.<create>(*args, &h) makes"""
         self.L = lib()
-        self.params = params
-        self._pc = params.to_c()
         h = c_void_p()
-        rc = self.L.erasor_create(ctypes.byref(self._pc), device, ctypes.byref(h))
+        rc = getattr(self.L, create)(*args, ctypes.byref(h))
         if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_last_error(None) or b"").decode())
+            raise ErasorError(rc, self._message(None))
         self.h = h
-        self._device = device
-        self.n_map = 0
-        self.n_query = 0
-        self._keep = []   # keeps host arrays alive while the library may still read them
 
-    # -- plumbing ---------------------------------------------------------------------------
+    def _message(self, h) -> str:
+        return (getattr(self.L, self._LAST_ERROR)(h) or b"").decode()
+
     def _ck(self, rc: int):
         if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_last_error(self.h) or b"").decode())
+            raise ErasorError(rc, self._message(self.h))
+
+    def _read_cloud(self, call) -> np.ndarray:
+        """A float32 [n,4] cloud from a getter call(out, cap, &n) -> rc: asked for n without a buffer, then filled."""
+        n = c_size_t(0)
+        self._ck(call(None, 0, ctypes.byref(n)))
+        out = np.empty((n.value, 4), dtype=np.float32)
+        if n.value:
+            self._ck(call(out.ctypes.data, n.value, ctypes.byref(n)))
+        return out
 
     def close(self):
-        if getattr(self, "h", None):
-            self.L.erasor_destroy(self.h)
+        if self.h:
+            getattr(self.L, self._DESTROY)(self.h)
             self.h = None
 
     def __del__(self):
@@ -295,6 +304,21 @@ class Handle:
     def __exit__(self, *a):
         self.close()
 
+
+class Handle(_Native):
+    """One ``erasor_handle_t``: one CUDA device, one stream, fixed parameters."""
+    _DESTROY, _LAST_ERROR = "erasor_destroy", "erasor_last_error"
+
+    def __init__(self, params: ErasorParams, device: int = 0):
+        self.params = params
+        self._pc = params.to_c()
+        self._create("erasor_create", ctypes.byref(self._pc), device)
+        self._device = device
+        self.n_map = 0
+        self.n_query = 0
+        self._keep = []   # keeps host arrays alive while the library may still read them
+
+    # -- plumbing ---------------------------------------------------------------------------
     @property
     def stream(self) -> int:
         return self.L.erasor_stream(self.h) or 0
@@ -338,12 +362,7 @@ class Handle:
         return mr, cr
 
     def get_ground_viz(self) -> np.ndarray:
-        n = c_size_t(0)
-        self._ck(self.L.erasor_get_ground_viz(self.h, None, 0, ctypes.byref(n), PTR_HOST))
-        out = np.empty((n.value, 4), dtype=np.float32)
-        if n.value:
-            self._ck(self.L.erasor_get_ground_viz(self.h, out.ctypes.data, n.value, ctypes.byref(n), PTR_HOST))
-        return out
+        return self._read_cloud(lambda out, cap, n: self.L.erasor_get_ground_viz(self.h, out, cap, n, PTR_HOST))
 
     def get_max_range(self) -> float:
         return self.L.erasor_get_max_range(self.h)
@@ -615,20 +634,17 @@ def comm_unique_id() -> bytes:
     return bytes(buf)
 
 
-class Map:
-    """One ``erasor_map_t``: the global map resident in HBM plus its global keep mask."""
+class Map(_Native):
+    """One ``erasor_map_t``: the global map resident in HBM plus its global keep mask.  A map keeps no error message of its own:
+    erasor_last_error(NULL) reports a failed create, and the other calls' errors name the call."""
+    _DESTROY, _LAST_ERROR = "erasor_map_destroy", "erasor_last_error"
 
     def __init__(self, map_xyzi=None, device: int = 0, device_ptr: int = 0, n: int = 0):
-        self.L = lib()
-        h = c_void_p()
         if device_ptr:
-            rc = self.L.erasor_map_create(c_void_p(device_ptr), n, PTR_DEVICE, device, ctypes.byref(h))
+            self._create("erasor_map_create", c_void_p(device_ptr), n, PTR_DEVICE, device)
         else:
             m = _cloud(map_xyzi)
-            rc = self.L.erasor_map_create(m.ctypes.data, len(m), PTR_HOST, device, ctypes.byref(h))
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_last_error(None) or b"").decode())
-        self.h = h
+            self._create("erasor_map_create", m.ctypes.data, len(m), PTR_HOST, device)
 
     @property
     def size(self) -> int:
@@ -654,24 +670,13 @@ class Map:
             raise ErasorError(rc, "erasor_map_get_keep")
         return out
 
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.erasor_map_destroy(self.h)
-            self.h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class Updater:
+class Updater(_Native):
     """Device-resident mirror of ``erasor::OfflineMapUpdater`` (one ``erasor_updater_t``)."""
+    _DESTROY, _LAST_ERROR = "erasor_updater_destroy", "erasor_updater_last_error"
     MAP_ARRANGED, MAP_VOI, QUERY_VOI, MAP_REJECTED, OUTSKIRTS, SUBMAP_COMPLEMENT = 0, 1, 2, 5, 7, 8
 
     def __init__(self, up, ep: ErasorParams, initial_map, device: int = 0):
-        self.L = lib()
         self.ep, self.up = ep, up
         upc = UpdaterParamsC()
         upc.query_voxel_size, upc.map_voxel_size = up.query_voxel_size, up.map_voxel_size
@@ -681,26 +686,7 @@ class Updater:
             upc.lidar2body[i] = up.lidar2body[i]
         self._upc, self._epc = upc, ep.to_c()
         m = _cloud(initial_map)
-        h = c_void_p()
-        rc = self.L.erasor_updater_create(ctypes.byref(upc), ctypes.byref(self._epc), m.ctypes.data, len(m), device, ctypes.byref(h))
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_updater_last_error(None) or b"").decode())
-        self.h = h
-
-    def _ck(self, rc: int):
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_updater_last_error(self.h) or b"").decode())
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.erasor_updater_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._create("erasor_updater_create", ctypes.byref(upc), ctypes.byref(self._epc), m.ctypes.data, len(m), device)
 
     def reset(self, initial_map):
         m = _cloud(initial_map)
@@ -725,12 +711,7 @@ class Updater:
         return bool(done.value)
 
     def cloud(self, which: int) -> np.ndarray:
-        n = c_size_t(0)
-        self._ck(self.L.erasor_updater_get_cloud(self.h, which, None, 0, ctypes.byref(n), PTR_HOST))
-        out = np.empty((n.value, 4), dtype=np.float32)
-        if n.value:
-            self._ck(self.L.erasor_updater_get_cloud(self.h, which, out.ctypes.data, n.value, ctypes.byref(n), PTR_HOST))
-        return out
+        return self._read_cloud(lambda out, cap, n: self.L.erasor_updater_get_cloud(self.h, which, out, cap, n, PTR_HOST))
 
     def map_size(self) -> int:
         n = c_size_t(0)
@@ -738,12 +719,7 @@ class Updater:
         return n.value
 
     def save_static_map(self, voxel_size: float) -> np.ndarray:
-        n = c_size_t(0)
-        self._ck(self.L.erasor_updater_save_static_map(self.h, voxel_size, None, 0, ctypes.byref(n)))
-        out = np.empty((n.value, 4), dtype=np.float32)
-        if n.value:
-            self._ck(self.L.erasor_updater_save_static_map(self.h, voxel_size, out.ctypes.data, n.value, ctypes.byref(n)))
-        return out
+        return self._read_cloud(lambda out, cap, n: self.L.erasor_updater_save_static_map(self.h, voxel_size, out, cap, n))
 
     def voxelize(self, cloud, leaf: float) -> np.ndarray:
         c = _cloud(cloud)
@@ -772,42 +748,17 @@ class Updater:
         return [int(x) - int(t[0]) if x else None for x in t]
 
 
-class Evaluator:
+class Evaluator(_Native):
     """One ``erasor_eval_t``: PR / RR on the device, the counts of ``evaluate.evaluate`` by an exact grid-indexed 1-NN
     (DESIGN.md section 11).  ``evaluate`` and ``evaluate_map`` return exactly ``evaluate.evaluate``'s dict; ``last_counts()``
     adds ``inliers``, ``ambiguous_ties`` (inliers whose equally-nearest estimate points hold both classes -- the counts equal
     sklearn's whenever it is 0) and, when asked for, ``match``.  Unlike sklearn, an empty estimate is no error: no GT point
     is an inlier."""
+    _DESTROY, _LAST_ERROR = "erasor_eval_destroy", "erasor_eval_last_error"
 
     def __init__(self, device: int = 0):
-        self.L = lib()
-        h = c_void_p()
-        rc = self.L.erasor_eval_create(device, ctypes.byref(h))
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_eval_last_error(None) or b"").decode())
-        self.h = h
+        self._create("erasor_eval_create", device)
         self._last = None
-
-    def _ck(self, rc: int):
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_eval_last_error(self.h) or b"").decode())
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.erasor_eval_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
 
     def _finish(self, c: EvalCountsC, match) -> dict:
         from . import evaluate
@@ -921,43 +872,18 @@ class Evaluator:
         return self._report(d, self.overlap_map(m, voxelsize))
 
 
-class PcdCodec:
+class PcdCodec(_Native):
     """One ``erasor_pcd_t``: PCD files read and written on the device (DESIGN.md section 12).  ``parse`` / ``read`` give what
     ``evaluate.read_pcd_ascii`` gives, bit for bit (including its KeyError for a file without x, y, z or intensity); ``load`` /
     ``load_bytes`` read any DATA mode (ascii, binary, binary_compressed) as PCL does (section 12.1); ``format`` / ``write`` give the
     bytes ``evaluate.write_pcd_ascii`` writes, except that NaN is written "nan" whatever its sign.  Files are read and written as raw
     bytes."""
+    _DESTROY, _LAST_ERROR = "erasor_pcd_destroy", "erasor_pcd_last_error"
 
     def __init__(self, device: int = 0):
-        self.L = lib()
         self.device = device
-        h = c_void_p()
-        rc = self.L.erasor_pcd_create(device, ctypes.byref(h))
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_pcd_last_error(None) or b"").decode())
-        self.h = h
+        self._create("erasor_pcd_create", device)
         self._info = None
-
-    def _ck(self, rc: int):
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_pcd_last_error(self.h) or b"").decode())
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.erasor_pcd_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
 
     def _call_parse(self, ptr, n_bytes, kind, out_ptr, cap, out_kind, require_intensity):
         n, info = c_size_t(0), PcdInfoC()
@@ -1142,42 +1068,17 @@ class PcdCodec:
             f.write(memoryview(out))
 
 
-class MapGen:
+class MapGen(_Native):
     """One ``erasor_mapgen_t``: the reference's mapgen (src/mapgen/mapgen.hpp:198-305) with its map resident on the device
     (DESIGN.md section 8.2).  ``accum`` is accumPointCloud -- one launch, no host synchronisation unless a buffer grows; ``cloud``
     gives the four clouds of ``OracleMapGen`` by the same ids; ``save_naive_map`` is saveNaiveMap without the files."""
+    _DESTROY, _LAST_ERROR = "erasor_mapgen_destroy", "erasor_mapgen_last_error"
     CLOUD_MAP, CLOUD_CURR, SAVED_ORIGINAL, SAVED_VOXELIZED = 0, 1, 2, 3
 
     def __init__(self, leafsize: float = 0.05, is_large_scale: bool = False, device: int = 0):
-        self.L = lib()
         self.device = device
         self._p = MapGenParamsC(float(leafsize), 1 if is_large_scale else 0)
-        h = c_void_p()
-        rc = self.L.erasor_mapgen_create(ctypes.byref(self._p), device, ctypes.byref(h))
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_mapgen_last_error(None) or b"").decode())
-        self.h = h
-
-    def _ck(self, rc: int):
-        if rc != OK:
-            raise ErasorError(rc, (self.L.erasor_mapgen_last_error(self.h) or b"").decode())
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.erasor_mapgen_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
+        self._create("erasor_mapgen_create", ctypes.byref(self._p), device)
 
     def accum(self, odom7, lidar):
         """accumPointCloud with a host scan (float32 [n, 4] in the lidar frame; odom7 = x y z qx qy qz qw)."""
@@ -1192,12 +1093,7 @@ class MapGen:
         self._ck(self.L.erasor_mapgen_accum(self.h, o.ctypes.data_as(POINTER(c_double)), c_void_p(lidar_ptr) if lidar_ptr else None, n, ptr_kind))
 
     def cloud(self, which: int) -> np.ndarray:
-        n = c_size_t(0)
-        self._ck(self.L.erasor_mapgen_get_cloud(self.h, which, None, 0, PTR_HOST, ctypes.byref(n)))
-        out = np.empty((n.value, 4), dtype=np.float32)
-        if n.value:
-            self._ck(self.L.erasor_mapgen_get_cloud(self.h, which, out.ctypes.data, n.value, PTR_HOST, ctypes.byref(n)))
-        return out
+        return self._read_cloud(lambda out, cap, n: self.L.erasor_mapgen_get_cloud(self.h, which, out, cap, PTR_HOST, n))
 
     def device_cloud(self, which: int):
         """(device pointer, n) of a cloud in the handle's memory, valid until the next accum."""

@@ -16,6 +16,7 @@
 
 #include "../../include/erasor_b200.h"
 #include "binning_tables.h"
+#include "buffers.h"
 #include "device_types.h"
 #include "kernels.h"
 #include "pose_math.h"
@@ -26,40 +27,6 @@ using namespace erasor;
 namespace {
 
 thread_local std::string g_create_error;
-
-struct DevBuf {
-    void*     p = nullptr;
-    size_t    cap = 0;
-    uint64_t* epoch = nullptr;   // the owning handle's allocation epoch: bumped on every (re)allocation, captured graphs hold raw pointers
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
-        if (epoch) ++*epoch;
-        if (p) { cudaFree(p); p = nullptr; cap = 0; }
-        size_t want = bytes + bytes / 8 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e != cudaSuccess) { p = nullptr; return e; }
-        cap = want;
-        return cudaSuccess;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-struct PinnedBuf {
-    void*  p = nullptr;
-    size_t cap = 0;
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
-        if (p) { cudaFreeHost(p); p = nullptr; cap = 0; }
-        size_t want = bytes + bytes / 4 + 256;
-        cudaError_t e = cudaMallocHost(&p, want);
-        if (e != cudaSuccess) { p = nullptr; return e; }
-        cap = want;
-        return cudaSuccess;
-    }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
 
 constexpr int kNumTimers = 6;   // 0 whole pipeline, 1..5 = K1..K5
 constexpr size_t kMaxRecords = (size_t)1 << 21;   // flagged-bin records of one submission (larger batches are split)
@@ -74,8 +41,7 @@ struct Timer {
 
 struct erasor_map_ctx {
     int          device = 0;
-    float4*      d_pts = nullptr;
-    uint8_t*     d_keep = nullptr;
+    DeviceBuffer d_pts, d_keep;                // float4 [n + kMapPad], uint8 [max(n, 1)]
     size_t       n = 0;
     cudaStream_t st = nullptr;
     std::string  err;
@@ -98,36 +64,33 @@ struct erasor_ctx {
     int             sm_count = 132;
     std::string     err;
     HostBinTables   tables;
-    DevBuf          d_ring, d_pos, d_neg, d_guard;
+    // Captured graphs hold raw device pointers: every (re)allocation of a device buffer of this handle bumps alloc_epoch, which
+    // retires them.  HBuf cannot be built without the epoch, so a buffer added here cannot forget it.
+    uint64_t        alloc_epoch = 0;
+    struct HBuf : DeviceBuffer { explicit HBuf(uint64_t& e) : DeviceBuffer(&e) {} };
+    HBuf            d_ring{alloc_epoch}, d_pos{alloc_epoch}, d_neg{alloc_epoch}, d_guard{alloc_epoch};
     BinTablesView   view{};
     int             B = 0;
-    uint64_t        alloc_epoch = 0;           // bumped by every DevBuf (re)allocation of this handle
 
     // per-batch buffers
-    DevBuf d_map_in, d_qry_in;                 // staging when the caller's clouds are host memory
-    DevBuf d_bin_map, d_bin_qry;               // uint16 bin id per point
-    DevBuf d_chunks, d_chunk_range, d_frame_off;
-    DevBuf d_chcnt, d_zmin, d_zmax, d_cnt, d_dst_start, d_status, d_action, d_flag_slot, d_nflag;
-    DevBuf d_recs, d_nrecs, d_frame_rej, d_frame_rec_base, d_queue, d_bucket;
-    DevBuf d_map_sorted, d_map_src, d_qry_sorted, d_qry_src, d_part, d_scratch;
-    DevBuf d_keep, d_ground;
-    DevBuf d_arranged, d_map_rej, d_curr_rej, d_jobs, d_out_sizes, d_k5tmp;
-    DevBuf d_vox, d_vox_cnt, d_vox_start, d_vox_scratch;
-    DevBuf d_fence;                            // 4 x u64: negzero, empty fits, ambiguous, slow-path points
-    DevBuf d_poses;                            // node mode: NodePose per frame
-    DevBuf d_list_idx, d_list_cnt;             // node mode: per chunk, the map index of every VoI point (dense, map order) and their number
-    DevBuf d_k1prof;                           // erasor_profile_k1: per-warp cycle counters of K1's profiling build
-    DevBuf d_pack, d_gather;                   // exchange step: packed keep bits of this rank / of every rank
-    PinnedBuf h_stage, h_pose, h_words;        // h_words: small device -> host read-backs of a submission (pinned: an asynchronous copy into
+    HBuf d_map_in{alloc_epoch}, d_qry_in{alloc_epoch};       // staging when the caller's clouds are host memory
+    HBuf d_bin_map{alloc_epoch}, d_bin_qry{alloc_epoch};     // uint16 bin id per point
+    HBuf d_chunks{alloc_epoch}, d_chunk_range{alloc_epoch}, d_frame_off{alloc_epoch};
+    HBuf d_chcnt{alloc_epoch}, d_zmin{alloc_epoch}, d_zmax{alloc_epoch}, d_cnt{alloc_epoch}, d_dst_start{alloc_epoch}, d_status{alloc_epoch},
+         d_action{alloc_epoch}, d_flag_slot{alloc_epoch}, d_nflag{alloc_epoch};
+    HBuf d_recs{alloc_epoch}, d_nrecs{alloc_epoch}, d_frame_rej{alloc_epoch}, d_frame_rec_base{alloc_epoch}, d_queue{alloc_epoch}, d_bucket{alloc_epoch};
+    HBuf d_map_sorted{alloc_epoch}, d_map_src{alloc_epoch}, d_qry_sorted{alloc_epoch}, d_qry_src{alloc_epoch}, d_part{alloc_epoch}, d_scratch{alloc_epoch};
+    HBuf d_keep{alloc_epoch}, d_ground{alloc_epoch};
+    HBuf d_arranged{alloc_epoch}, d_map_rej{alloc_epoch}, d_curr_rej{alloc_epoch}, d_jobs{alloc_epoch}, d_out_sizes{alloc_epoch}, d_k5tmp{alloc_epoch};
+    HBuf d_vox{alloc_epoch}, d_vox_cnt{alloc_epoch}, d_vox_start{alloc_epoch}, d_vox_scratch{alloc_epoch};
+    HBuf d_fence{alloc_epoch};                 // 4 x u64: negzero, empty fits, ambiguous, slow-path points
+    HBuf d_poses{alloc_epoch};                 // node mode: NodePose per frame
+    HBuf d_list_idx{alloc_epoch}, d_list_cnt{alloc_epoch};   // node mode: per chunk, the map index of every VoI point (dense, map order) and their number
+    HBuf d_k1prof{alloc_epoch};                // erasor_profile_k1: per-warp cycle counters of K1's profiling build
+    HBuf d_pack{alloc_epoch}, d_gather{alloc_epoch};         // exchange step: packed keep bits of this rank / of every rank
+    PinnedBuffer h_stage, h_pose, h_words;     // h_words: small device -> host read-backs of a submission (pinned: an asynchronous copy into
                                                // pageable memory blocks the launching thread until the whole stream has drained, which
                                                // serialised overlapped handles)
-    std::vector<DevBuf*> all_bufs() {
-        return {&d_ring, &d_pos, &d_neg, &d_guard, &d_map_in, &d_qry_in, &d_bin_map, &d_bin_qry, &d_chunks, &d_chunk_range, &d_frame_off, &d_chcnt, &d_zmin,
-                &d_zmax, &d_cnt, &d_dst_start, &d_status, &d_action, &d_flag_slot, &d_nflag, &d_recs, &d_nrecs, &d_queue, &d_bucket, &d_frame_rej,
-                &d_map_sorted, &d_map_src, &d_qry_sorted, &d_qry_src, &d_part, &d_scratch, &d_keep, &d_ground, &d_arranged, &d_map_rej, &d_curr_rej,
-                &d_jobs, &d_out_sizes, &d_k5tmp, &d_fence, &d_vox, &d_vox_cnt, &d_vox_start, &d_vox_scratch, &d_frame_rec_base, &d_poses, &d_list_idx, &d_list_cnt, &d_pack,
-                &d_gather, &d_k1prof};
-    }
 
     // batch geometry of the last run
     int      F = 0;
@@ -182,14 +145,7 @@ struct erasor_ctx {
 
 namespace {
 
-#define CK(call)                                                                                   \
-    do {                                                                                           \
-        cudaError_t e__ = (call);                                                                  \
-        if (e__ != cudaSuccess) {                                                                  \
-            h->err = std::string(#call) + ": " + cudaGetErrorString(e__);                          \
-            return ERASOR_E_CUDA;                                                                  \
-        }                                                                                          \
-    } while (0)
+#define CK(call) ERASOR_CUDA_TRY(h->err, call, #call)
 
 // NCCL is bound at run time: single-GPU users need no libnccl, and inside a torch process dlopen returns the copy torch
 // already loaded (same soname), so the process keeps exactly one NCCL.
@@ -350,16 +306,16 @@ int prepare_batch(erasor_ctx* h, const uint64_t* map_off, const uint64_t* qry_of
     if (b0) std::memcpy(st, chunks.data(), b0);
     std::memcpy(st + b0, range.data(), b1);
     std::memcpy(st + b0 + b1, foff.data(), b2);
-    if (b0) CK(cudaMemcpyAsync(h->d_chunks.p, st, b0, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_chunk_range.p, st + b0, b1, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_frame_off.p, st + b0 + b1, b2, cudaMemcpyHostToDevice, h->stream));
+    if (b0) CK(cudaMemcpyAsync(h->d_chunks.p(), st, b0, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_chunk_range.p(), st + b0, b1, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_frame_off.p(), st + b0 + b1, b2, cudaMemcpyHostToDevice, h->stream));
     h->desc_mode = mode;
     h->desc_epoch++;
     return ERASOR_OK;
 }
 
 // one caller cloud -> device pointer (staged through `stage` when it lives in host memory)
-int stage_cloud(erasor_ctx* h, DevBuf& stage, const float* xyzi, size_t n, int ptr_kind, const float4** out, size_t bytes_per_point = sizeof(float4)) {
+int stage_cloud(erasor_ctx* h, DeviceBuffer& stage, const float* xyzi, size_t n, int ptr_kind, const float4** out, size_t bytes_per_point = sizeof(float4)) {
     if (ptr_kind == ERASOR_PTR_DEVICE) {
         const uintptr_t align = bytes_per_point == sizeof(float4) ? 15 : 3;
         if (n && (reinterpret_cast<uintptr_t>(xyzi) & align)) { h->err = "device clouds must be 16-byte aligned (float4; packed xyz: 4-byte)"; return ERASOR_E_INVALID; }
@@ -367,7 +323,7 @@ int stage_cloud(erasor_ctx* h, DevBuf& stage, const float* xyzi, size_t n, int p
         return ERASOR_OK;
     }
     CK(stage.ensure(sizeof(float4) * std::max<size_t>(n, 1)));
-    if (n) CK(cudaMemcpyAsync(stage.p, xyzi, bytes_per_point * n, cudaMemcpyHostToDevice, h->stream));
+    if (n) CK(cudaMemcpyAsync(stage.p(), xyzi, bytes_per_point * n, cudaMemcpyHostToDevice, h->stream));
     *out = stage.as<float4>();
     return ERASOR_OK;
 }
@@ -512,7 +468,6 @@ int erasor_create(const erasor_params_t* params, int device, erasor_handle_t* ou
     if (device < 0 || device >= ndev) { g_create_error = "bad device index"; return ERASOR_E_INVALID; }
     erasor_ctx* h = new erasor_ctx();
     h->p = p; h->device = device; h->B = (int)Bll;
-    for (DevBuf* b : h->all_bufs()) b->epoch = &h->alloc_epoch;
     if (const char* ng = std::getenv("ERASOR_B200_NO_GRAPH")) h->use_graphs = !(ng[0] == '1');
     if (const char* uf = std::getenv("ERASOR_B200_UNFUSED_SRT")) h->fused_srt = !(uf[0] == '1');
     if (const char* cs = std::getenv("ERASOR_B200_CTAS_PER_SM")) h->ctas_per_sm = std::max(1, std::min(8, std::atoi(cs)));
@@ -547,18 +502,18 @@ int erasor_create(const erasor_params_t* params, int device, erasor_handle_t* ou
     if ((e = cudaEventCreateWithFlags(&h->ev_join_b, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
     if ((e = cudaEventCreateWithFlags(&h->ev_join_c, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
     const size_t rb = sizeof(double) * h->tables.ring_thr.size(), sb = sizeof(SectorBoundary) * h->tables.sec_pos.size();
-    if ((e = h->h_words.ensure(128)) != cudaSuccess) return fail("cudaMallocHost", e);
-    std::memset(h->h_words.p, 0, 128);
+    if ((e = h->h_words.allocate(128)) != cudaSuccess) return fail("cudaMallocHost", e);
+    std::memset(h->h_words.p(), 0, 128);
     const size_t gb = sizeof(float) * h->tables.ring_guard.size();
     if ((e = h->d_guard.ensure(gb)) != cudaSuccess) return fail("cudaMalloc", e);
-    if ((e = cudaMemcpy(h->d_guard.p, h->tables.ring_guard.data(), gb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
+    if ((e = cudaMemcpy(h->d_guard.p(), h->tables.ring_guard.data(), gb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
     if ((e = h->d_ring.ensure(rb)) != cudaSuccess || (e = h->d_pos.ensure(sb)) != cudaSuccess || (e = h->d_neg.ensure(sb)) != cudaSuccess ||
         (e = h->d_fence.ensure(sizeof(unsigned long long) * 4)) != cudaSuccess)
         return fail("cudaMalloc", e);
-    if ((e = cudaMemcpy(h->d_ring.p, h->tables.ring_thr.data(), rb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
-    if ((e = cudaMemcpy(h->d_pos.p, h->tables.sec_pos.data(), sb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
-    if ((e = cudaMemcpy(h->d_neg.p, h->tables.sec_neg.data(), sb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
-    if ((e = cudaMemset(h->d_fence.p, 0, sizeof(unsigned long long) * 4)) != cudaSuccess) return fail("cudaMemset", e);
+    if ((e = cudaMemcpy(h->d_ring.p(), h->tables.ring_thr.data(), rb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
+    if ((e = cudaMemcpy(h->d_pos.p(), h->tables.sec_pos.data(), sb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
+    if ((e = cudaMemcpy(h->d_neg.p(), h->tables.sec_neg.data(), sb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
+    if ((e = cudaMemset(h->d_fence.p(), 0, sizeof(unsigned long long) * 4)) != cudaSuccess) return fail("cudaMemset", e);
     h->view = h->tables.view(h->d_ring.as<double>(), h->d_pos.as<SectorBoundary>(), h->d_neg.as<SectorBoundary>(), h->d_guard.as<float>());
     *out = h;
     return ERASOR_OK;
@@ -572,11 +527,7 @@ void erasor_destroy(erasor_handle_t h) {
     for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
     h->graphs.clear();
     if (h->comm) { NcclApi* api = nccl_api(h->err); if (api) api->CommDestroy(h->comm); h->comm = nullptr; }
-    for (DevBuf* b : h->all_bufs()) b->release();
     vox_batch_destroy(h->vb);
-    h->h_pose.release();
-    h->h_words.release();
-    h->h_stage.release();
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
     if (h->ev_join_a) cudaEventDestroy(h->ev_join_a);
     if (h->ev_join_b) cudaEventDestroy(h->ev_join_b);
@@ -628,8 +579,8 @@ int erasor_compare(erasor_handle_t h, int version, int frame) {
     const size_t NM = h->NM, NQ = h->NQ;
     CK(h->d_keep.ensure(std::max<size_t>(NM, 1)));
     CK(h->d_ground.ensure(std::max<size_t>(NM, 1)));
-    CK(cudaMemsetAsync(h->d_keep.p, 1, std::max<size_t>(NM, 1), h->stream));
-    CK(cudaMemsetAsync(h->d_ground.p, 0, std::max<size_t>(NM, 1), h->stream));
+    CK(cudaMemsetAsync(h->d_keep.p(), 1, std::max<size_t>(NM, 1), h->stream));
+    CK(cudaMemsetAsync(h->d_ground.p(), 0, std::max<size_t>(NM, 1), h->stream));
     // R-GPF class C (bins beyond 2560 points, 1024-thread CTAs) is launched only while such bins are being seen; if one turns up
     // unannounced the class runs after the fact and the output assembly is repeated (same policy as the mask modes, erasor_wait)
     const bool with_c = h->class_c_state != 0;
@@ -670,9 +621,9 @@ int erasor_compare(erasor_handle_t h, int version, int frame) {
                          h->d_k5tmp.as<uint32_t>(), h->sm_count * 4));
         }
         uint32_t* w = h->h_words.as<uint32_t>();
-        CK(cudaMemcpyAsync(w + 4, h->d_out_sizes.p, sizeof(uint32_t) * 5, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync(w + 4, h->d_out_sizes.p(), sizeof(uint32_t) * 5, cudaMemcpyDeviceToHost, h->stream));
         CK(cudaMemcpyAsync(w + 9, h->d_dst_start.as<uint32_t>() + B, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaMemcpyAsync(w + 10, h->d_nrecs.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync(w + 10, h->d_nrecs.p(), sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
         CK(cudaMemcpyAsync(w + 11, h->d_queue.as<uint32_t>() + kBucketC0, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
         return ERASOR_OK;
@@ -712,7 +663,7 @@ int erasor_get_static_estimate(erasor_handle_t h, float* arranged_xyzi, size_t c
     }
     CK(cudaSetDevice(h->device));
     int rc;
-    if (arranged_xyzi && (rc = copy_out(h, h->d_arranged.p, arranged_xyzi, sizeof(float4) * h->out_sizes[0], ptr_kind))) return rc;
+    if (arranged_xyzi && (rc = copy_out(h, h->d_arranged.p(), arranged_xyzi, sizeof(float4) * h->out_sizes[0], ptr_kind))) return rc;
     if (complement_xyzi && (rc = copy_out(h, h->d_map_sorted.as<float4>() + h->complement_start, complement_xyzi,
                                           sizeof(float4) * h->out_sizes[1], ptr_kind))) return rc;
     CK(cudaStreamSynchronize(h->stream));
@@ -730,8 +681,8 @@ int erasor_get_outliers(erasor_handle_t h, float* map_rejected_xyzi, size_t cap_
     }
     CK(cudaSetDevice(h->device));
     int rc;
-    if (map_rejected_xyzi && (rc = copy_out(h, h->d_map_rej.p, map_rejected_xyzi, sizeof(float4) * h->out_sizes[2], ptr_kind))) return rc;
-    if (curr_rejected_xyzi && (rc = copy_out(h, h->d_curr_rej.p, curr_rejected_xyzi, sizeof(float4) * h->out_sizes[3], ptr_kind))) return rc;
+    if (map_rejected_xyzi && (rc = copy_out(h, h->d_map_rej.p(), map_rejected_xyzi, sizeof(float4) * h->out_sizes[2], ptr_kind))) return rc;
+    if (curr_rejected_xyzi && (rc = copy_out(h, h->d_curr_rej.p(), curr_rejected_xyzi, sizeof(float4) * h->out_sizes[3], ptr_kind))) return rc;
     CK(cudaStreamSynchronize(h->stream));
     return ERASOR_OK;
 }
@@ -774,7 +725,7 @@ int erasor_get_bins(erasor_handle_t h, int which_cloud, int32_t* bin_of_point, f
     CK(cudaStreamSynchronize(h->stream));
     if (bin_of_point && n) {
         std::vector<uint16_t> tmp(n);
-        CK(cudaMemcpy(tmp.data(), which_cloud == 0 ? h->d_bin_map.p : h->d_bin_qry.p, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(tmp.data(), which_cloud == 0 ? h->d_bin_map.p() : h->d_bin_qry.p(), sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < n; ++i) bin_of_point[i] = tmp[i] == kNoBin16 ? -1 : (int32_t)tmp[i];
     }
     if (min_h || max_h || count) {
@@ -799,7 +750,7 @@ int erasor_get_status(erasor_handle_t h, float* status) {
     if (h->stage < 2) { h->err = "erasor_get_status before erasor_compare"; return ERASOR_E_STATE; }
     CK(cudaSetDevice(h->device));
     std::vector<uint8_t> st(h->B);
-    CK(cudaMemcpy(st.data(), h->d_status.p, h->B, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(st.data(), h->d_status.p(), h->B, cudaMemcpyDeviceToHost));
     for (int b = 0; b < h->B; ++b) status[b] = status_value(st[b]);
     return ERASOR_OK;
 }
@@ -814,7 +765,7 @@ int erasor_get_planes(erasor_handle_t h, int32_t* bin_ids, int32_t* n_points, in
     if (!bin_ids && !n_points && !n_seeds && !lpr_height && !normal_d && !n_ground) return ERASOR_OK;
     if (cap < n) { h->err = "plane buffer too small"; return ERASOR_E_CAPACITY; }
     std::vector<FlagRec> recs(n);
-    if (n) CK(cudaMemcpy(recs.data(), h->d_recs.p, sizeof(FlagRec) * n, cudaMemcpyDeviceToHost));
+    if (n) CK(cudaMemcpy(recs.data(), h->d_recs.p(), sizeof(FlagRec) * n, cudaMemcpyDeviceToHost));
     const int it = std::min(h->p.gf_iter, kMaxIter);
     for (size_t i = 0; i < n; ++i) {
         const FlagRec& r = recs[i];   // single frame: record index == slot == processing order (bin order)
@@ -834,8 +785,8 @@ int erasor_get_static_mask(erasor_handle_t h, uint8_t* keep_map, uint8_t* is_gro
     if (!h) return ERASOR_E_INVALID;
     if (h->stage < 2) { h->err = "erasor_get_static_mask before erasor_compare"; return ERASOR_E_STATE; }
     CK(cudaSetDevice(h->device));
-    if (keep_map && h->NM) CK(cudaMemcpy(keep_map, h->d_keep.p, h->NM, cudaMemcpyDeviceToHost));
-    if (is_ground && h->NM) CK(cudaMemcpy(is_ground, h->d_ground.p, h->NM, cudaMemcpyDeviceToHost));
+    if (keep_map && h->NM) CK(cudaMemcpy(keep_map, h->d_keep.p(), h->NM, cudaMemcpyDeviceToHost));
+    if (is_ground && h->NM) CK(cudaMemcpy(is_ground, h->d_ground.p(), h->NM, cudaMemcpyDeviceToHost));
     return ERASOR_OK;
 }
 
@@ -844,7 +795,7 @@ int erasor_get_fence_counts(erasor_handle_t h, uint64_t* negzero_points, uint64_
     CK(cudaSetDevice(h->device));
     CK(cudaStreamSynchronize(h->stream));
     unsigned long long v[4];
-    CK(cudaMemcpy(v, h->d_fence.p, sizeof(v), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(v, h->d_fence.p(), sizeof(v), cudaMemcpyDeviceToHost));
     if (negzero_points) *negzero_points = v[0];
     if (empty_plane_fits) *empty_plane_fits = v[1];
     if (ambiguous_sector) *ambiguous_sector = v[2];
@@ -901,9 +852,9 @@ int submit(erasor_ctx* h, const Submit& S) {
         CK(h->d_qry_in.ensure(sizeof(float4) * std::max<size_t>(h->NQ, 1)));
     }
     if (S.mode == 2) {
-        if (sizeof(NodePose) * (size_t)S.F > h->h_pose.cap) h->alloc_epoch++;      // captured graphs copy from this staging buffer
+        if (sizeof(NodePose) * (size_t)S.F > h->h_pose.cap()) h->alloc_epoch++;      // captured graphs copy from this staging buffer
         CK(h->h_pose.ensure(sizeof(NodePose) * (size_t)S.F));
-        std::memcpy(h->h_pose.p, S.poses, sizeof(NodePose) * (size_t)S.F);
+        std::memcpy(h->h_pose.p(), S.poses, sizeof(NodePose) * (size_t)S.F);
     }
     const bool with_c = h->class_c_state != 0;
     auto enqueue = [&]() -> int {
@@ -911,9 +862,9 @@ int submit(erasor_ctx* h, const Submit& S) {
         if (S.mode == 1) {
             if ((r = stage_inputs(h, S.map_xyzi, S.qry_xyzi, S.ptr_kind))) return r;
         } else {
-            h->cur_map = reinterpret_cast<const float4*>(h->map->d_pts);
+            h->cur_map = h->map->d_pts.as<const float4>();
             if ((r = stage_cloud(h, h->d_qry_in, S.qry_xyzi, h->NQ, S.ptr_kind, &h->cur_qry, S.qry_xyz ? 3 * sizeof(float) : sizeof(float4)))) return r;
-            CK(cudaMemcpyAsync(h->d_poses.p, h->h_pose.p, sizeof(NodePose) * (size_t)S.F, cudaMemcpyHostToDevice, h->stream));
+            CK(cudaMemcpyAsync(h->d_poses.p(), h->h_pose.p(), sizeof(NodePose) * (size_t)S.F, cudaMemcpyHostToDevice, h->stream));
         }
         uint8_t* d_keep = nullptr;
         if (n_keep) {
@@ -922,7 +873,7 @@ int submit(erasor_ctx* h, const Submit& S) {
         }
         if ((r = run_k1(h, S.mode))) return r;
         K4Fold fold{nullptr, nullptr, 0u, 0u};
-        if (S.mode == 2)        fold = K4Fold{h->map->d_keep, nullptr, (uint32_t)n_map_global, 0u};
+        if (S.mode == 2)        fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};
         else if (S.fold_global) fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
         if ((r = run_compare(h, h->p.version, S.mode, d_keep, nullptr, fold, with_c ? 7 : 3))) return r;
         h->last.with_c = with_c; h->last.host = host; h->last.mode = S.mode; h->last.d_keep = d_keep; h->last.user_keep = S.keep_mask; h->last.n_keep = n_keep;
@@ -930,8 +881,8 @@ int submit(erasor_ctx* h, const Submit& S) {
         CK(cudaMemcpyAsync(h->h_words.as<uint32_t>() + 1, h->d_queue.as<uint32_t>() + kBucketC0, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
         if (host && n_keep) CK(cudaMemcpyAsync(S.keep_mask, d_keep, n_keep, cudaMemcpyDeviceToHost, h->stream));
         if (S.keep_out && n_map_global)
-            CK(cudaMemcpyAsync(S.keep_out, h->map->d_keep, n_map_global, host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->h_words.as<uint32_t>(), h->d_nrecs.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+            CK(cudaMemcpyAsync(S.keep_out, h->map->d_keep.as<uint8_t>(), n_map_global, host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->h_words.as<uint32_t>(), h->d_nrecs.p(), sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
         return ERASOR_OK;
     };
     bool graphable = h->use_graphs && !h->timing;
@@ -992,7 +943,7 @@ int submit(erasor_ctx* h, const Submit& S) {
         h->last.with_c = with_c; h->last.host = hst; h->last.mode = S.mode; h->last.user_keep = S.keep_mask; h->last.n_keep = n_keep;
         h->last.d_keep = n_keep ? (hst ? h->d_keep.as<uint8_t>() : S.keep_mask) : nullptr;
         h->last.keep_out = S.keep_out; h->last.n_map_global = n_map_global;
-        if (S.mode == 2)        h->last.fold = K4Fold{h->map->d_keep, nullptr, (uint32_t)n_map_global, 0u};
+        if (S.mode == 2)        h->last.fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};
         else if (S.fold_global) h->last.fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
         else                    h->last.fold = K4Fold{nullptr, nullptr, 0u, 0u};
     }
@@ -1049,7 +1000,7 @@ int process_frames_impl(erasor_handle_t h, const float* map_xyzi, const uint64_t
 int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
     const size_t row = (size_t)h->B + 1;
     std::vector<uint32_t> c((size_t)h->F * row);
-    CK(cudaMemcpy(c.data(), h->d_cnt.p, sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(c.data(), h->d_cnt.p(), sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
     for (int f = 0; f < h->F; ++f) {
         uint64_t t = 0;
         for (size_t b = 0; b < row; ++b) t += c[(size_t)f * row + b];
@@ -1127,7 +1078,7 @@ int erasor_wait(erasor_handle_t h) {
             if (rc) return rc;
             if (h->last.host && h->last.n_keep) CK(cudaMemcpyAsync(h->last.user_keep, h->last.d_keep, h->last.n_keep, cudaMemcpyDeviceToHost, h->stream));
             if (h->last.keep_out && h->last.n_map_global)
-                CK(cudaMemcpyAsync(h->last.keep_out, h->map->d_keep, h->last.n_map_global, h->last.host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, h->stream));
+                CK(cudaMemcpyAsync(h->last.keep_out, h->map->d_keep.as<uint8_t>(), h->last.n_map_global, h->last.host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, h->stream));
             CK(cudaStreamSynchronize(h->stream));
         }
     }
@@ -1192,13 +1143,13 @@ int erasor_map_create(const float* map_xyzi, size_t n_map, int ptr_kind, int dev
     auto fail = [&](const char* what, cudaError_t ce) { g_create_error = std::string(what) + ": " + cudaGetErrorString(ce); erasor_map_destroy(m); return ERASOR_E_CUDA; };
     if ((e = cudaSetDevice(device)) != cudaSuccess) return fail("cudaSetDevice", e);
     if ((e = cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
-    if ((e = cudaMalloc(&m->d_pts, sizeof(float4) * (n_map + kMapPad))) != cudaSuccess) return fail("cudaMalloc", e);
-    if ((e = cudaMemsetAsync(m->d_pts + n_map, 0, sizeof(float4) * kMapPad, m->st)) != cudaSuccess) return fail("cudaMemset", e);
-    if ((e = cudaMalloc(&m->d_keep, std::max<size_t>(n_map, 1))) != cudaSuccess) return fail("cudaMalloc", e);
+    if ((e = m->d_pts.allocate(sizeof(float4) * (n_map + kMapPad))) != cudaSuccess) return fail("cudaMalloc", e);
+    if ((e = cudaMemsetAsync(m->d_pts.as<float4>() + n_map, 0, sizeof(float4) * kMapPad, m->st)) != cudaSuccess) return fail("cudaMemset", e);
+    if ((e = m->d_keep.allocate(std::max<size_t>(n_map, 1))) != cudaSuccess) return fail("cudaMalloc", e);
     if (n_map) {
         const cudaMemcpyKind k = ptr_kind == ERASOR_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-        if ((e = cudaMemcpyAsync(m->d_pts, map_xyzi, sizeof(float4) * n_map, k, m->st)) != cudaSuccess) return fail("cudaMemcpy", e);
-        if ((e = cudaMemsetAsync(m->d_keep, 1, n_map, m->st)) != cudaSuccess) return fail("cudaMemset", e);
+        if ((e = cudaMemcpyAsync(m->d_pts.p(), map_xyzi, sizeof(float4) * n_map, k, m->st)) != cudaSuccess) return fail("cudaMemcpy", e);
+        if ((e = cudaMemsetAsync(m->d_keep.as<uint8_t>(), 1, n_map, m->st)) != cudaSuccess) return fail("cudaMemset", e);
     }
     if ((e = cudaStreamSynchronize(m->st)) != cudaSuccess) return fail("cudaStreamSynchronize", e);
     *out = m;
@@ -1209,19 +1160,17 @@ void erasor_map_destroy(erasor_map_t m) {
     if (!m) return;
     cudaSetDevice(m->device);
     if (m->st) { cudaStreamSynchronize(m->st); cudaStreamDestroy(m->st); }
-    if (m->d_pts) cudaFree(m->d_pts);
-    if (m->d_keep) cudaFree(m->d_keep);
     delete m;
 }
 
 size_t erasor_map_size(erasor_map_t m) { return m ? m->n : 0; }
-uint8_t* erasor_map_keep_device(erasor_map_t m) { return m ? m->d_keep : nullptr; }
-const float* erasor_map_points_device(erasor_map_t m) { return m ? reinterpret_cast<const float*>(m->d_pts) : nullptr; }
+uint8_t* erasor_map_keep_device(erasor_map_t m) { return m ? m->d_keep.as<uint8_t>() : nullptr; }
+const float* erasor_map_points_device(erasor_map_t m) { return m ? m->d_pts.as<const float>() : nullptr; }
 
 int erasor_map_reset_keep(erasor_map_t m) {
     if (!m) return ERASOR_E_INVALID;
     if (cudaSetDevice(m->device) != cudaSuccess) return ERASOR_E_CUDA;
-    if (m->n && cudaMemsetAsync(m->d_keep, 1, m->n, m->st) != cudaSuccess) return ERASOR_E_CUDA;
+    if (m->n && cudaMemsetAsync(m->d_keep.as<uint8_t>(), 1, m->n, m->st) != cudaSuccess) return ERASOR_E_CUDA;
     return cudaStreamSynchronize(m->st) == cudaSuccess ? ERASOR_OK : ERASOR_E_CUDA;
 }
 
@@ -1229,7 +1178,7 @@ int erasor_map_get_keep(erasor_map_t m, uint8_t* keep, int ptr_kind) {
     if (!m || (m->n && !keep)) return ERASOR_E_INVALID;
     if (cudaSetDevice(m->device) != cudaSuccess) return ERASOR_E_CUDA;
     const cudaMemcpyKind k = ptr_kind == ERASOR_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    if (m->n && cudaMemcpyAsync(keep, m->d_keep, m->n, k, m->st) != cudaSuccess) return ERASOR_E_CUDA;
+    if (m->n && cudaMemcpyAsync(keep, m->d_keep.as<uint8_t>(), m->n, k, m->st) != cudaSuccess) return ERASOR_E_CUDA;
     return cudaStreamSynchronize(m->st) == cudaSuccess ? ERASOR_OK : ERASOR_E_CUDA;
 }
 
@@ -1294,8 +1243,8 @@ int erasor_get_node_stats(erasor_handle_t h, uint32_t* n_voi_points, uint32_t* n
         std::copy(h->node_nvoi.begin(), h->node_nvoi.begin() + std::min<size_t>(h->node_nvoi.size(), (size_t)h->f0), n_voi_points);
         if ((rc = read_node_voi_counts(h, n_voi_points + h->f0))) return rc;
     }
-    if (n_flagged_bins) CK(cudaMemcpy(n_flagged_bins, h->d_nflag.p, sizeof(uint32_t) * h->stat_F, cudaMemcpyDeviceToHost));
-    if (n_rejected_points) CK(cudaMemcpy(n_rejected_points, h->d_frame_rej.p, sizeof(uint32_t) * h->stat_F, cudaMemcpyDeviceToHost));
+    if (n_flagged_bins) CK(cudaMemcpy(n_flagged_bins, h->d_nflag.p(), sizeof(uint32_t) * h->stat_F, cudaMemcpyDeviceToHost));
+    if (n_rejected_points) CK(cudaMemcpy(n_rejected_points, h->d_frame_rej.p(), sizeof(uint32_t) * h->stat_F, cudaMemcpyDeviceToHost));
     return ERASOR_OK;
 }
 
@@ -1368,7 +1317,7 @@ int erasor_allgather_and_keep(erasor_handle_t h, uint8_t* global_keep, size_t n_
     CK(h->d_gather.ensure(sizeof(uint32_t) * words * (size_t)h->comm_ranks));
     h->launches += 2;
     CK(launch_pack_keep_bits(h->stream, global_keep, n_global, h->d_pack.as<uint32_t>()));
-    const ncclResult_t r = api->AllGather(h->d_pack.p, h->d_gather.p, words, ncclUint32, h->comm, h->stream);
+    const ncclResult_t r = api->AllGather(h->d_pack.p(), h->d_gather.p(), words, ncclUint32, h->comm, h->stream);
     if (r != ncclSuccess) { h->err = std::string("ncclAllGather: ") + api->GetErrorString(r); return ERASOR_E_CUDA; }
     CK(launch_and_unpack_keep(h->stream, h->d_gather.as<uint32_t>(), h->comm_ranks, n_global, global_keep));
     return ERASOR_OK;
@@ -1380,8 +1329,8 @@ int erasor_get_frame_stats(erasor_handle_t h, uint32_t* n_flagged_bins, uint32_t
     CK(cudaSetDevice(h->device));
     CK(cudaStreamSynchronize(h->stream));
     const int nf = std::max(h->stat_F, h->F);
-    if (n_flagged_bins) CK(cudaMemcpy(n_flagged_bins, h->d_nflag.p, sizeof(uint32_t) * nf, cudaMemcpyDeviceToHost));
-    if (n_rejected_points) CK(cudaMemcpy(n_rejected_points, h->d_frame_rej.p, sizeof(uint32_t) * nf, cudaMemcpyDeviceToHost));
+    if (n_flagged_bins) CK(cudaMemcpy(n_flagged_bins, h->d_nflag.p(), sizeof(uint32_t) * nf, cudaMemcpyDeviceToHost));
+    if (n_rejected_points) CK(cudaMemcpy(n_rejected_points, h->d_frame_rej.p(), sizeof(uint32_t) * nf, cudaMemcpyDeviceToHost));
     return ERASOR_OK;
 }
 
@@ -1392,14 +1341,14 @@ int erasor_get_rgpf_profile(erasor_handle_t h, uint32_t* n_points, uint32_t* pro
     CK(cudaSetDevice(h->device));
     CK(cudaStreamSynchronize(h->stream));
     uint32_t nr = 0;
-    CK(cudaMemcpy(&nr, h->d_nrecs.p, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&nr, h->d_nrecs.p(), sizeof(uint32_t), cudaMemcpyDeviceToHost));
     nr = std::min(nr, h->rec_capacity);
     const size_t cap = *n;
     *n = nr;
     if (!n_points && !prof8) return ERASOR_OK;
     if (cap < nr) { h->err = "profile buffer too small"; return ERASOR_E_CAPACITY; }
     std::vector<FlagRec> recs(nr);
-    if (nr) CK(cudaMemcpy(recs.data(), h->d_recs.p, sizeof(FlagRec) * nr, cudaMemcpyDeviceToHost));
+    if (nr) CK(cudaMemcpy(recs.data(), h->d_recs.p(), sizeof(FlagRec) * nr, cudaMemcpyDeviceToHost));
     for (size_t i = 0; i < nr; ++i) {
         if (n_points) n_points[i] = recs[i].n_points;
         if (prof8) for (int k = 0; k < 8; ++k) prof8[i * 8 + k] = recs[i].prof[k];
@@ -1428,7 +1377,7 @@ int erasor_profile_k1(erasor_handle_t h, uint32_t* out, size_t* n, int* warps_pe
     h->k1_prof = nullptr;
     if (rc) return rc;
     CK(cudaStreamSynchronize(h->stream));
-    CK(cudaMemcpy(out, h->d_k1prof.p, sizeof(uint32_t) * words, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(out, h->d_k1prof.p(), sizeof(uint32_t) * words, cudaMemcpyDeviceToHost));
     return ERASOR_OK;
 }
 
@@ -1436,7 +1385,7 @@ int erasor_get_srt_profile(erasor_handle_t h, uint32_t* cycles8) {
     if (!h || !cycles8) return ERASOR_E_INVALID;
     CK(cudaSetDevice(h->device));
     CK(cudaStreamSynchronize(h->stream));
-    if (!h->d_queue.p) { h->err = "no run yet"; return ERASOR_E_STATE; }
+    if (!h->d_queue.p()) { h->err = "no run yet"; return ERASOR_E_STATE; }
     CK(cudaMemcpy(cycles8, h->d_queue.as<uint32_t>() + 20, sizeof(uint32_t) * 8, cudaMemcpyDeviceToHost));
     return ERASOR_OK;
 }

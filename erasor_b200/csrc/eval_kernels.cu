@@ -17,6 +17,7 @@
 #include <string>
 
 #include "../../include/erasor_b200.h"
+#include "buffers.h"
 #include "device_common.cuh"
 #include "radix_sort.h"
 
@@ -654,19 +655,6 @@ __global__ void k_ovl_gather(const uint32_t* __restrict__ hi, const uint32_t* __
 using namespace erasor;
 
 namespace {
-struct DevBuf {
-    void* p = nullptr; size_t cap = 0;
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
-        if (p) { cudaFree(p); p = nullptr; cap = 0; }
-        const size_t want = bytes + bytes / 4 + 4096;
-        const cudaError_t e = cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
 thread_local std::string g_eval_err;
 }  // namespace
 
@@ -674,17 +662,17 @@ struct erasor_eval_ctx {
     int device = 0;
     cudaStream_t st = nullptr;
     std::string err;
-    DevBuf gt, est, keep, match;              // staging of host inputs / the match output
-    DevBuf key_a, key_b, idx_a, idx_b;        // 16 B per estimate point: the sort's ping-pong; the free half holds vox_key / vox_start
-    DevBuf cnt, chunk, stats;                 // per-segment digit counts + digit totals, per-chunk head counts, EvalStats
-    EvalStats* h_stats = nullptr;             // pinned
+    DeviceBuffer gt, est, keep, match;        // staging of host inputs / the match output
+    DeviceBuffer key_a, key_b, idx_a, idx_b;  // 16 B per estimate point: the sort's ping-pong; the free half holds vox_key / vox_start
+    DeviceBuffer cnt, chunk, stats;           // per-segment digit counts + digit totals, per-chunk head counts, EvalStats
+    PinnedBuffer h_stats;                     // EvalStats
     // erasor_eval_overlap: the coarse index's ping-pong, its boxes and EvalStats, the distances, counters + ranks + rank values
-    DevBuf ckey_a, ckey_b, cidx_a, cidx_b, cbox, cstats, dist, ovl;
+    DeviceBuffer ckey_a, ckey_b, cidx_a, cidx_b, cbox, cstats, dist, ovl;
     int sm_count = 132;
 };
 
 namespace {
-#define ECK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { e->err = std::string(#call) + ": " + cudaGetErrorString(e__); return ERASOR_E_CUDA; } } while (0)
+#define ECK(call) ERASOR_CUDA_TRY(e->err, call, #call)
 
 int fail(erasor_eval_t e, int rc, const char* msg) { e->err = msg; return rc; }
 
@@ -744,8 +732,8 @@ struct CellIndex { const uint32_t *order = nullptr, *vox_key = nullptr, *vox_sta
 // every cell key of that width, so it sorts behind the selected points), then the run heads over the selected prefix; nv goes to
 // st->nv.  kb / ib: the key and index ping-pong, 4 (n + 1) bytes each; the half the sort does not end in holds vox_key / vox_start.
 // With o (the overlap search's grids), the points are keyed by their coarse cell instead (k_ovl_ckeys; g is then o.g, no keep mask).
-int build_cells(erasor_eval_t e, const float4* pts, const uint8_t* keep, uint32_t n, uint32_t n_sel, const EvalGrid& g, DevBuf* const kb[2],
-                DevBuf* const ib[2], EvalStats* st, CellIndex& ix, const OvlGrid* o = nullptr) {
+int build_cells(erasor_eval_t e, const float4* pts, const uint8_t* keep, uint32_t n, uint32_t n_sel, const EvalGrid& g, DeviceBuffer* const kb[2],
+                DeviceBuffer* const ib[2], EvalStats* st, CellIndex& ix, const OvlGrid* o = nullptr) {
     unsigned long long cells = 1ull;
     for (int k = 0; k < 3; ++k) cells *= (unsigned long long)(o ? o->cdiv[k] : g.div[k]);
     const size_t words = (size_t)n + 1;
@@ -813,7 +801,7 @@ int erasor_eval_create(int device, erasor_eval_t* out) {
     e->device = device;
     cudaError_t c = cudaSetDevice(device);
     if (c == cudaSuccess) c = cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking);
-    if (c == cudaSuccess) c = cudaMallocHost(&e->h_stats, sizeof(EvalStats));
+    if (c == cudaSuccess) c = e->h_stats.allocate(sizeof(EvalStats));
     if (c == cudaSuccess) c = e->stats.ensure(sizeof(EvalStats));
     if (c == cudaSuccess) c = cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, device);
     if (c != cudaSuccess) {
@@ -829,9 +817,6 @@ void erasor_eval_destroy(erasor_eval_t e) {
     if (!e) return;
     cudaSetDevice(e->device);
     if (e->st) cudaStreamSynchronize(e->st);
-    for (DevBuf* b : {&e->gt, &e->est, &e->keep, &e->match, &e->key_a, &e->key_b, &e->idx_a, &e->idx_b, &e->cnt, &e->chunk, &e->stats,
-                      &e->ckey_a, &e->ckey_b, &e->cidx_a, &e->cidx_b, &e->cbox, &e->cstats, &e->dist, &e->ovl}) b->release();
-    if (e->h_stats) cudaFreeHost(e->h_stats);
     if (e->st) cudaStreamDestroy(e->st);
     delete e;
 }
@@ -857,13 +842,13 @@ int erasor_evaluate(erasor_eval_t e, const float* gt_xyzi, size_t n_gt, const fl
         if ((reinterpret_cast<uintptr_t>(gt_xyzi) | reinterpret_cast<uintptr_t>(est_xyzi)) & 15u)
             return fail(e, ERASOR_E_INVALID, "device clouds must be 16-byte aligned (one float4 per point)");
     } else {
-        if (ng) { ECK(e->gt.ensure(sizeof(float4) * n_gt)); ECK(cudaMemcpyAsync(e->gt.p, gt_xyzi, sizeof(float4) * n_gt, cudaMemcpyHostToDevice, e->st)); d_gt = e->gt.as<float4>(); }
-        if (ne) { ECK(e->est.ensure(sizeof(float4) * n_est)); ECK(cudaMemcpyAsync(e->est.p, est_xyzi, sizeof(float4) * n_est, cudaMemcpyHostToDevice, e->st)); d_est = e->est.as<float4>(); }
-        if (ne && est_keep) { ECK(e->keep.ensure(n_est)); ECK(cudaMemcpyAsync(e->keep.p, est_keep, n_est, cudaMemcpyHostToDevice, e->st)); d_keep = e->keep.as<uint8_t>(); }
+        if (ng) { ECK(e->gt.ensure(sizeof(float4) * n_gt)); ECK(cudaMemcpyAsync(e->gt.p(), gt_xyzi, sizeof(float4) * n_gt, cudaMemcpyHostToDevice, e->st)); d_gt = e->gt.as<float4>(); }
+        if (ne) { ECK(e->est.ensure(sizeof(float4) * n_est)); ECK(cudaMemcpyAsync(e->est.p(), est_xyzi, sizeof(float4) * n_est, cudaMemcpyHostToDevice, e->st)); d_est = e->est.as<float4>(); }
+        if (ne && est_keep) { ECK(e->keep.ensure(n_est)); ECK(cudaMemcpyAsync(e->keep.p(), est_keep, n_est, cudaMemcpyHostToDevice, e->st)); d_keep = e->keep.as<uint8_t>(); }
     }
     if (!ne) d_keep = nullptr;
     EvalStats* d_st = e->stats.as<EvalStats>();
-    EvalStats* h = e->h_stats;
+    EvalStats* h = e->h_stats.as<EvalStats>();
     std::memset(h, 0, sizeof(EvalStats));
     for (int k = 0; k < 3; ++k) h->mn[k] = ~0u;
     ECK(cudaMemcpyAsync(d_st, h, sizeof(EvalStats), cudaMemcpyHostToDevice, e->st));
@@ -885,8 +870,8 @@ int erasor_evaluate(erasor_eval_t e, const float* gt_xyzi, size_t n_gt, const fl
         for (int k = 0; k < 3; ++k) { mn[k] = ordered_to_float(h->mn[k]); mx[k] = ordered_to_float(h->mx[k]); }
         if (!eval_grid_setup(mn, mx, voxelsize, g)) return fail(e, ERASOR_E_INVALID, "no cell grid covers the estimate's extent");
         // 3. keys + radix sort, 4. run heads
-        DevBuf* kb[2] = {&e->key_a, &e->key_b};
-        DevBuf* ib[2] = {&e->idx_a, &e->idx_b};
+        DeviceBuffer* kb[2] = {&e->key_a, &e->key_b};
+        DeviceBuffer* ib[2] = {&e->idx_a, &e->idx_b};
         const int rc = build_cells(e, d_est, d_keep, ne, n_sel, g, kb, ib, d_st, ix);
         if (rc != ERASOR_OK) return rc;
     }
@@ -957,13 +942,13 @@ int erasor_eval_overlap(erasor_eval_t e, const float* gt_xyzi, size_t n_gt, cons
             return fail(e, ERASOR_E_INVALID, "device clouds must be 16-byte aligned (one float4 per point)");
         if (reinterpret_cast<uintptr_t>(est_dist) & 7u) return fail(e, ERASOR_E_INVALID, "est_dist must be 8-byte aligned");
     } else {
-        if (ng) { ECK(e->gt.ensure(sizeof(float4) * n_gt)); ECK(cudaMemcpyAsync(e->gt.p, gt_xyzi, sizeof(float4) * n_gt, cudaMemcpyHostToDevice, e->st)); d_gt = e->gt.as<float4>(); }
-        if (ne) { ECK(e->est.ensure(sizeof(float4) * n_est)); ECK(cudaMemcpyAsync(e->est.p, est_xyzi, sizeof(float4) * n_est, cudaMemcpyHostToDevice, e->st)); d_est = e->est.as<float4>(); }
-        if (ne && est_keep) { ECK(e->keep.ensure(n_est)); ECK(cudaMemcpyAsync(e->keep.p, est_keep, n_est, cudaMemcpyHostToDevice, e->st)); d_keep = e->keep.as<uint8_t>(); }
+        if (ng) { ECK(e->gt.ensure(sizeof(float4) * n_gt)); ECK(cudaMemcpyAsync(e->gt.p(), gt_xyzi, sizeof(float4) * n_gt, cudaMemcpyHostToDevice, e->st)); d_gt = e->gt.as<float4>(); }
+        if (ne) { ECK(e->est.ensure(sizeof(float4) * n_est)); ECK(cudaMemcpyAsync(e->est.p(), est_xyzi, sizeof(float4) * n_est, cudaMemcpyHostToDevice, e->st)); d_est = e->est.as<float4>(); }
+        if (ne && est_keep) { ECK(e->keep.ensure(n_est)); ECK(cudaMemcpyAsync(e->keep.p(), est_keep, n_est, cudaMemcpyHostToDevice, e->st)); d_keep = e->keep.as<uint8_t>(); }
     }
     if (!ne) d_keep = nullptr;
     EvalStats* d_st = e->stats.as<EvalStats>();
-    EvalStats* h = e->h_stats;
+    EvalStats* h = e->h_stats.as<EvalStats>();
     std::memset(h, 0, sizeof(EvalStats));
     for (int k = 0; k < 3; ++k) h->mn[k] = ~0u;
     ECK(cudaMemcpyAsync(d_st, h, sizeof(EvalStats), cudaMemcpyHostToDevice, e->st));
@@ -998,12 +983,12 @@ int erasor_eval_overlap(erasor_eval_t e, const float* gt_xyzi, size_t n_gt, cons
         float mn[3], mx[3];
         for (int k = 0; k < 3; ++k) { mn[k] = ordered_to_float(h->mn[k]); mx[k] = ordered_to_float(h->mx[k]); }
         if (!ovl_setup(mn, mx, voxelsize, o)) return fail(e, ERASOR_E_INVALID, "no cell grid covers the ground truth's extent");
-        DevBuf* kb[2] = {&e->key_a, &e->key_b};
-        DevBuf* ib[2] = {&e->idx_a, &e->idx_b};
+        DeviceBuffer* kb[2] = {&e->key_a, &e->key_b};
+        DeviceBuffer* ib[2] = {&e->idx_a, &e->idx_b};
         int rc = build_cells(e, d_gt, nullptr, ng, ng, o.g, kb, ib, d_st, fx);
         if (rc != ERASOR_OK) return rc;
-        DevBuf* ckb[2] = {&e->ckey_a, &e->ckey_b};
-        DevBuf* cib[2] = {&e->cidx_a, &e->cidx_b};
+        DeviceBuffer* ckb[2] = {&e->ckey_a, &e->ckey_b};
+        DeviceBuffer* cib[2] = {&e->cidx_a, &e->cidx_b};
         rc = build_cells(e, d_gt, nullptr, ng, ng, o.g, ckb, cib, d_cst, cx, &o);
         if (rc != ERASOR_OK) return rc;
         const uint32_t max_cells = (uint32_t)o.cdiv[0] * (uint32_t)o.cdiv[1] * (uint32_t)o.cdiv[2];

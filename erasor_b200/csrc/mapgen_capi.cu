@@ -11,8 +11,10 @@
 #include <algorithm>
 #include <cmath>
 #include <string>
+#include <utility>
 
 #include "../../include/erasor_b200.h"
+#include "buffers.h"
 #include "pose_math.h"
 #include "updater_kernels.h"
 
@@ -22,12 +24,6 @@ namespace {
 constexpr size_t kMaxPoints = size_t(1) << 31;   // the kernels count points in 32 bits and stride over them without wrapping
 constexpr int    kParkEvery = 500;               // mapgen.hpp:248
 enum { W_TAIL = 0, W_CHUNK = 1, W_SEL = 2, W_CURR = 3, W_PARK = 4, W_SAVE = 5, W_COUNT = 8 };
-
-struct DevBuf {
-    void* p = nullptr; size_t cap = 0;
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
 }  // namespace
 
 struct erasor_mapgen_ctx {
@@ -35,9 +31,9 @@ struct erasor_mapgen_ctx {
     int device = 0, sm_count = 132;
     cudaStream_t st = nullptr;
     std::string err;
-    DevBuf map;                                   // float4 [cap]: parked submaps, then the current chunk
-    DevBuf scan, sel, part_tmp, vox_tmp, curr, vox_out, grid, words;
-    uint32_t* h_words = nullptr;                  // pinned read-back of the device words
+    DeviceBuffer map;                             // float4 [cap]: parked submaps, then the current chunk
+    DeviceBuffer scan, sel, part_tmp, vox_tmp, curr, vox_out, grid, words;
+    PinnedBuffer h_words;                         // pinned read-back of the device words
     size_t ub_tail = 0, ub_chunk = 0;             // upper bounds on the map's size and on its current chunk's size
     size_t tail = 0, chunk = 0, n_curr = 0;       // exact values as of the last read-back
     bool fresh = false;                           // tail / chunk / n_curr describe the map as it is now
@@ -51,7 +47,7 @@ struct erasor_mapgen_ctx {
 
 namespace {
 thread_local std::string g_merr;
-#define MCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { g->err = std::string(#call) + ": " + cudaGetErrorString(e__); return ERASOR_E_CUDA; } } while (0)
+#define MCK(call) ERASOR_CUDA_TRY(g->err, call, #call)
 
 int host_sync(erasor_mapgen_ctx* g) {
     g->host_syncs += 1;
@@ -63,10 +59,11 @@ int host_sync(erasor_mapgen_ctx* g) {
 // the device words -> tail, chunk, n_curr (one synchronisation); the bounds become exact
 int read_state(erasor_mapgen_ctx* g) {
     if (g->fresh) return ERASOR_OK;
-    MCK(cudaMemcpyAsync(g->h_words, g->words.p, sizeof(uint32_t) * W_COUNT, cudaMemcpyDeviceToHost, g->st));
+    MCK(cudaMemcpyAsync(g->h_words.p(), g->words.p(), sizeof(uint32_t) * W_COUNT, cudaMemcpyDeviceToHost, g->st));
     int rc = host_sync(g);
     if (rc) return rc;
-    g->tail = g->h_words[W_TAIL]; g->chunk = g->h_words[W_CHUNK]; g->n_curr = g->h_words[W_CURR];
+    const uint32_t* w = g->h_words.as<uint32_t>();
+    g->tail = w[W_TAIL]; g->chunk = w[W_CHUNK]; g->n_curr = w[W_CURR];
     g->ub_tail = g->tail; g->ub_chunk = g->tail - g->chunk;
     g->fresh = true;
     return ERASOR_OK;
@@ -74,20 +71,19 @@ int read_state(erasor_mapgen_ctx* g) {
 
 // b holds at least `bytes`: otherwise wait for the stream (work in flight may use b) unless it is idle, reallocate with headroom
 // and keep the first keep_bytes.
-int grow(erasor_mapgen_ctx* g, DevBuf& b, size_t bytes, size_t keep_bytes = 0) {
-    if (bytes <= b.cap && b.p) return ERASOR_OK;
+int grow(erasor_mapgen_ctx* g, DeviceBuffer& b, size_t bytes, size_t keep_bytes = 0) {
+    if (bytes <= b.cap() && b.p()) return ERASOR_OK;
     int rc = g->idle ? ERASOR_OK : host_sync(g);
     if (rc) return rc;
-    const size_t want = std::max<size_t>(std::max(bytes, 2 * b.cap), 4096);
-    void* q = nullptr;
-    MCK(cudaMalloc(&q, want));
-    if (b.p && keep_bytes) {
-        cudaError_t e = cudaMemcpyAsync(q, b.p, keep_bytes, cudaMemcpyDeviceToDevice, g->st);
+    const size_t want = std::max<size_t>(std::max(bytes, 2 * b.cap()), 4096);
+    DeviceBuffer q;
+    MCK(q.allocate(want));
+    if (b.p() && keep_bytes) {
+        cudaError_t e = cudaMemcpyAsync(q.p(), b.p(), keep_bytes, cudaMemcpyDeviceToDevice, g->st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(g->st);
-        if (e != cudaSuccess) { cudaFree(q); g->err = std::string("regrowth copy: ") + cudaGetErrorString(e); return ERASOR_E_CUDA; }
+        if (e != cudaSuccess) { g->err = std::string("regrowth copy: ") + cudaGetErrorString(e); return ERASOR_E_CUDA; }
     }
-    b.release();
-    b.p = q; b.cap = want;
+    b = std::move(q);
     g->regrowths += 1;
     return ERASOR_OK;
 }
@@ -95,7 +91,7 @@ int grow(erasor_mapgen_ctx* g, DevBuf& b, size_t bytes, size_t keep_bytes = 0) {
 void base_job(erasor_mapgen_ctx* g, FusedJob& J) {
     Mat4 I{};
     for (int i = 0; i < 4; ++i) I.m[i * 5] = 1.0f;
-    J.vin = nullptr; J.vn = 0; J.leaf = 1.0f; J.grid = g->grid.as<VoxGrid>(); J.vtmp = g->vox_tmp.p; J.vout = nullptr; J.d_n_out = nullptr;
+    J.vin = nullptr; J.vn = 0; J.leaf = 1.0f; J.grid = g->grid.as<VoxGrid>(); J.vtmp = g->vox_tmp.p(); J.vout = nullptr; J.d_n_out = nullptr;
     J.T_out = I; J.xform_out = 0;
     J.has_part = 0; J.P = PartPred{PART_NOT_NEAR, 0, 0.0, 0.0, 0.0}; J.T_sel = I; J.xform_sel = 0; J.pin = nullptr; J.pn = 0;
     J.chunk_tmp = nullptr; J.d_total_sel = nullptr; J.out_sel = nullptr; J.out_rest = nullptr;
@@ -105,7 +101,7 @@ void base_job(erasor_mapgen_ctx* g, FusedJob& J) {
 // the current chunk -> voxelize_preserving_labels at leafsize -> parked in place (mapgen.hpp:249-256)
 int park(erasor_mapgen_ctx* g) {
     int rc;
-    if (g->ub_chunk > g->vox_out.cap / sizeof(float4) || voxelize_tmp_bytes_upto((uint32_t)g->ub_chunk) > g->vox_tmp.cap) {
+    if (g->ub_chunk > g->vox_out.cap() / sizeof(float4) || voxelize_tmp_bytes_upto((uint32_t)g->ub_chunk) > g->vox_tmp.cap()) {
         if ((rc = read_state(g))) return rc;             // tighten the bound before sizing scratch by it
     }
     if ((rc = grow(g, g->vox_out, sizeof(float4) * std::max<size_t>(g->ub_chunk, 1)))) return rc;
@@ -130,14 +126,14 @@ int ensure_saved(erasor_mapgen_ctx* g) {
     if ((rc = grow(g, g->vox_tmp, voxelize_tmp_bytes((uint32_t)g->tail)))) return rc;
     FusedJob J;
     base_job(g, J);
-    J.vin = g->map.as<float4>(); J.vn = (uint32_t)g->tail; J.leaf = g->prm.leafsize; J.vtmp = g->vox_tmp.p;
+    J.vin = g->map.as<float4>(); J.vn = (uint32_t)g->tail; J.leaf = g->prm.leafsize; J.vtmp = g->vox_tmp.p();
     J.vout = g->vox_out.as<float4>(); J.d_n_out = g->words.as<uint32_t>() + W_SAVE;
     g->launches += 1;
     MCK(launch_node_fused(g->st, J, g->sm_count));
     g->idle = false;
-    MCK(cudaMemcpyAsync(g->h_words, g->words.p, sizeof(uint32_t) * W_COUNT, cudaMemcpyDeviceToHost, g->st));
+    MCK(cudaMemcpyAsync(g->h_words.p(), g->words.p(), sizeof(uint32_t) * W_COUNT, cudaMemcpyDeviceToHost, g->st));
     if ((rc = host_sync(g))) return rc;
-    g->saved_n = g->h_words[W_SAVE];
+    g->saved_n = g->h_words.as<uint32_t>()[W_SAVE];
     g->saved_version = g->version;
     return ERASOR_OK;
 }
@@ -171,12 +167,10 @@ int erasor_mapgen_create(const erasor_mapgen_params_t* prm, int device, erasor_m
     if ((e = cudaSetDevice(device)) != cudaSuccess) return fail("cudaSetDevice", e);
     if ((e = cudaDeviceGetAttribute(&g->sm_count, cudaDevAttrMultiProcessorCount, device)) != cudaSuccess) return fail("cudaDeviceGetAttribute", e);
     if ((e = cudaStreamCreateWithFlags(&g->st, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
-    if ((e = cudaMallocHost(reinterpret_cast<void**>(&g->h_words), sizeof(uint32_t) * W_COUNT)) != cudaSuccess) return fail("cudaMallocHost", e);
-    if ((e = cudaMalloc(&g->words.p, sizeof(uint32_t) * W_COUNT)) != cudaSuccess) return fail("cudaMalloc", e);
-    g->words.cap = sizeof(uint32_t) * W_COUNT;
-    if ((e = cudaMalloc(&g->grid.p, sizeof(VoxGrid))) != cudaSuccess) return fail("cudaMalloc", e);
-    g->grid.cap = sizeof(VoxGrid);
-    if ((e = cudaMemsetAsync(g->words.p, 0, sizeof(uint32_t) * W_COUNT, g->st)) != cudaSuccess) return fail("cudaMemsetAsync", e);
+    if ((e = g->h_words.allocate(sizeof(uint32_t) * W_COUNT)) != cudaSuccess) return fail("cudaMallocHost", e);
+    if ((e = g->words.allocate(sizeof(uint32_t) * W_COUNT)) != cudaSuccess) return fail("cudaMalloc", e);
+    if ((e = g->grid.allocate(sizeof(VoxGrid))) != cudaSuccess) return fail("cudaMalloc", e);
+    if ((e = cudaMemsetAsync(g->words.p(), 0, sizeof(uint32_t) * W_COUNT, g->st)) != cudaSuccess) return fail("cudaMemsetAsync", e);
     if ((e = cudaStreamSynchronize(g->st)) != cudaSuccess) return fail("cudaStreamSynchronize", e);
     g->fresh = true;
     *out = g;
@@ -187,8 +181,6 @@ void erasor_mapgen_destroy(erasor_mapgen_t g) {
     if (!g) return;
     cudaSetDevice(g->device);
     if (g->st) { cudaStreamSynchronize(g->st); cudaStreamDestroy(g->st); }
-    for (DevBuf* b : {&g->map, &g->scan, &g->sel, &g->part_tmp, &g->vox_tmp, &g->curr, &g->vox_out, &g->grid, &g->words}) b->release();
-    if (g->h_words) cudaFreeHost(g->h_words);
     delete g;
 }
 
@@ -203,7 +195,7 @@ int erasor_mapgen_accum(erasor_mapgen_t g, const double* odom7, const float* lid
     int rc;
     // room for the worst case: every point survives the cut and is its own voxel.  When the bound would overflow the map buffer,
     // one synchronisation reads the true size back and the buffer doubles (at least), so the next one is as far away again.
-    const size_t map_cap = g->map.cap / sizeof(float4);
+    const size_t map_cap = g->map.cap() / sizeof(float4);
     if (g->ub_tail + n > map_cap) {
         if ((rc = read_state(g))) return rc;
         if (g->tail + n >= kMaxPoints) { g->err = "the map would reach 2^31 points"; return ERASOR_E_CAPACITY; }
@@ -218,7 +210,7 @@ int erasor_mapgen_accum(erasor_mapgen_t g, const double* odom7, const float* lid
     const float4* d_scan = reinterpret_cast<const float4*>(lidar_xyzi);
     if (ptr_kind == ERASOR_PTR_HOST) {
         if ((rc = grow(g, g->scan, sizeof(float4) * n1))) return rc;
-        if (n) MCK(cudaMemcpyAsync(g->scan.p, lidar_xyzi, sizeof(float4) * n, cudaMemcpyHostToDevice, g->st));
+        if (n) MCK(cudaMemcpyAsync(g->scan.p(), lidar_xyzi, sizeof(float4) * n, cudaMemcpyHostToDevice, g->st));
         g->idle = false;
         d_scan = g->scan.as<float4>();
     }
@@ -231,7 +223,7 @@ int erasor_mapgen_accum(erasor_mapgen_t g, const double* odom7, const float* lid
     J.pin = d_scan; J.pn = (uint32_t)n; J.chunk_tmp = g->part_tmp.as<uint32_t>();
     J.d_total_sel = g->words.as<uint32_t>() + W_SEL; J.out_sel = g->sel.as<float4>();
     J.vn = (uint32_t)n; J.leaf = 0.2f;                                         // :239 (fixed 0.2)
-    J.vtmp = g->vox_tmp.p; J.vout = g->curr.as<float4>(); J.d_n_out = g->words.as<uint32_t>() + W_CURR;
+    J.vtmp = g->vox_tmp.p(); J.vout = g->curr.as<float4>(); J.d_n_out = g->words.as<uint32_t>() + W_CURR;
     g->launches += 1;
     MCK(launch_map_chained(g->st, J, g->sm_count));
     g->idle = false;

@@ -26,6 +26,7 @@
 
 #include "../../include/erasor_b200.h"
 #include "bag_index.h"
+#include "buffers.h"
 #include "pcd_binary.h"
 #include "pcd_codec.h"
 
@@ -300,21 +301,10 @@ __global__ void __launch_bounds__(kThreads) k_pcd_fmt_write(const float4* pts, u
     }
 }
 
-struct DevBuf {
-    void* p = nullptr; size_t cap = 0;
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
-        if (p) { cudaFree(p); p = nullptr; cap = 0; }
-        const size_t want = bytes + bytes / 8 + 4096;
-        const cudaError_t e = cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
 thread_local std::string g_pcd_err;
 
+using erasor::DeviceBuffer;
+using erasor::PinnedBuffer;
 using pcd::Header;
 using pcd::parse_header;
 
@@ -496,17 +486,17 @@ struct erasor_pcd_ctx {
     int device = 0;
     cudaStream_t st = nullptr;
     std::string err;
-    DevBuf text, chunk_cnt, chunk_off, lines, flags, rows, sums, out, stats;   // parse
-    DevBuf pts, lens, offs, ftext;                                              // format
-    DevBuf lz_map0, lz_map1, lz_tok, lz_byt, lz_entry, lz_ctok, lz_cbyt, lz_tokoff, lz_byteoff, lz_rec, lz_src, lz_dec, lz_flags;   // load
-    DevBuf bag_blobs, bag_desc;                                                 // erasor_bag_load
-    PcdStats* h_stats = nullptr;                                                // pinned
+    DeviceBuffer text, chunk_cnt, chunk_off, lines, flags, rows, sums, out, stats;   // parse
+    DeviceBuffer pts, lens, offs, ftext;                                              // format
+    DeviceBuffer lz_map0, lz_map1, lz_tok, lz_byt, lz_entry, lz_ctok, lz_cbyt, lz_tokoff, lz_byteoff, lz_rec, lz_src, lz_dec, lz_flags;   // load
+    DeviceBuffer bag_blobs, bag_desc;                                                 // erasor_bag_load
+    PinnedBuffer h_stats;                                                             // PcdStats
     int sm_count = 132;
     // erasor_bag_index's index and file (the caller's memory), and the pinned staging of a pageable file
     bag::Index bag;
     bool bag_ok = false, bag_pinned = false;
     const uint8_t* bag_file = nullptr;
-    uint8_t* bag_stage[2] = {nullptr, nullptr};
+    PinnedBuffer bag_stage[2];
     cudaEvent_t bag_ev[2] = {nullptr, nullptr};
     // erasor_pcd_format_ascii's text of its last call, kept for a following call with the same input
     bool cached = false;
@@ -517,7 +507,7 @@ struct erasor_pcd_ctx {
 };
 
 namespace {
-#define PCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { p->err = std::string(#call) + ": " + cudaGetErrorString(e__); return ERASOR_E_CUDA; } } while (0)
+#define PCK(call) ERASOR_CUDA_TRY(p->err, call, #call)
 
 int fail(erasor_pcd_t p, int rc, const std::string& msg) { p->err = msg; return rc; }
 
@@ -638,7 +628,7 @@ int erasor_pcd_create(int device, erasor_pcd_t* out) {
     p->device = device;
     cudaError_t c = cudaSetDevice(device);
     if (c == cudaSuccess) c = cudaStreamCreateWithFlags(&p->st, cudaStreamNonBlocking);
-    if (c == cudaSuccess) c = cudaMallocHost(&p->h_stats, sizeof(PcdStats));
+    if (c == cudaSuccess) c = p->h_stats.allocate(sizeof(PcdStats));
     if (c == cudaSuccess) c = p->stats.ensure(sizeof(PcdStats));
     if (c == cudaSuccess) c = cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, device);
     if (c != cudaSuccess) {
@@ -654,15 +644,8 @@ void erasor_pcd_destroy(erasor_pcd_t p) {
     if (!p) return;
     cudaSetDevice(p->device);
     if (p->st) cudaStreamSynchronize(p->st);
-    for (DevBuf* b : {&p->text, &p->chunk_cnt, &p->chunk_off, &p->lines, &p->flags, &p->rows, &p->sums, &p->out, &p->stats, &p->pts,
-                      &p->lens, &p->offs, &p->ftext, &p->lz_map0, &p->lz_map1, &p->lz_tok, &p->lz_byt, &p->lz_entry, &p->lz_ctok,
-                      &p->lz_cbyt, &p->lz_tokoff, &p->lz_byteoff, &p->lz_rec, &p->lz_src, &p->lz_dec, &p->lz_flags, &p->bag_blobs,
-                      &p->bag_desc}) b->release();
-    for (int k = 0; k < 2; ++k) {
-        if (p->bag_stage[k]) cudaFreeHost(p->bag_stage[k]);
-        if (p->bag_ev[k]) cudaEventDestroy(p->bag_ev[k]);
-    }
-    if (p->h_stats) cudaFreeHost(p->h_stats);
+    for (cudaEvent_t ev : p->bag_ev)
+        if (ev) cudaEventDestroy(ev);
     if (p->st) cudaStreamDestroy(p->st);
     delete p;
 }
@@ -718,7 +701,7 @@ int erasor_pcd_parse_ascii(erasor_pcd_t p, const char* text, size_t len, int tex
     Text t{};
     if (text_kind == ERASOR_PTR_HOST) {
         PCK(p->text.ensure(dlen));
-        PCK(cudaMemcpyAsync(p->text.p, text + h.data_off, dlen, cudaMemcpyHostToDevice, p->st));
+        PCK(cudaMemcpyAsync(p->text.p(), text + h.data_off, dlen, cudaMemcpyHostToDevice, p->st));
         t.base = p->text.as<uint8_t>();
         t.o = 0;
     } else {
@@ -757,7 +740,7 @@ int erasor_pcd_parse_ascii(erasor_pcd_t p, const char* text, size_t len, int tex
     float4* d_out = reinterpret_cast<float4*>(out_xyzi);
     if (out_kind == ERASOR_PTR_HOST) { PCK(p->out.ensure(sizeof(float4) * std::max<uint64_t>(rows, 1))); d_out = p->out.as<float4>(); }
     PcdStats* d_st = p->stats.as<PcdStats>();
-    PcdStats* hs = p->h_stats;
+    PcdStats* hs = p->h_stats.as<PcdStats>();
     std::memset(hs, 0, sizeof(PcdStats));
     hs->err = ~0ull;
     PCK(cudaMemcpyAsync(d_st, hs, sizeof(PcdStats), cudaMemcpyHostToDevice, p->st));
@@ -805,7 +788,7 @@ int erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_
         const float4* d_pts = reinterpret_cast<const float4*>(xyzi);
         if (in_kind == ERASOR_PTR_HOST && n) {
             PCK(p->pts.ensure(sizeof(float4) * n));
-            PCK(cudaMemcpyAsync(p->pts.p, xyzi, sizeof(float4) * n, cudaMemcpyHostToDevice, p->st));
+            PCK(cudaMemcpyAsync(p->pts.p(), xyzi, sizeof(float4) * n, cudaMemcpyHostToDevice, p->st));
             d_pts = p->pts.as<float4>();
         }
         uint64_t body = 0;
@@ -820,7 +803,7 @@ int erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_
         }
         const uint64_t total = (uint64_t)hl + body;
         PCK(p->ftext.ensure(total));
-        PCK(cudaMemcpyAsync(p->ftext.p, head, hl, cudaMemcpyHostToDevice, p->st));
+        PCK(cudaMemcpyAsync(p->ftext.p(), head, hl, cudaMemcpyHostToDevice, p->st));
         if (n) {
             k_pcd_fmt_write<<<blocks_for(n, kThreads, p->sm_count * 16), kThreads, 0, p->st>>>(d_pts, n, p->offs.as<uint64_t>(), p->ftext.as<uint8_t>() + hl);
             PCK(cudaGetLastError());
@@ -833,7 +816,7 @@ int erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_
         p->cached = true;                             // the following call with the same input fetches this text
         return out ? fail(p, ERASOR_E_CAPACITY, "out holds fewer bytes than the formatted text") : ERASOR_OK;
     }
-    PCK(cudaMemcpyAsync(out, p->ftext.p, p->c_len, out_kind == ERASOR_PTR_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, p->st));
+    PCK(cudaMemcpyAsync(out, p->ftext.p(), p->c_len, out_kind == ERASOR_PTR_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, p->st));
     PCK(cudaStreamSynchronize(p->st));
     return ERASOR_OK;
 }
@@ -891,7 +874,7 @@ int erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind,
     const uint8_t* d_in = reinterpret_cast<const uint8_t*>(file) + at;
     if (file_kind == ERASOR_PTR_HOST) {
         PCK(p->text.ensure(std::max<uint64_t>(body, 1)));
-        PCK(cudaMemcpyAsync(p->text.p, file + at, body, cudaMemcpyHostToDevice, p->st));
+        PCK(cudaMemcpyAsync(p->text.p(), file + at, body, cudaMemcpyHostToDevice, p->st));
         d_in = p->text.as<uint8_t>();
     }
     uint4* d_out = reinterpret_cast<uint4*>(out_xyzi);
@@ -1023,13 +1006,13 @@ int erasor_bag_load_list(erasor_pcd_t p, const uint64_t* nodes, size_t count, fl
     } else {
         // a window of the device layout at a time: filled on the host in one pinned buffer while the other one's copy runs
         for (int k = 0; k < 2; ++k) {
-            if (!p->bag_stage[k]) PCK(cudaMallocHost(&p->bag_stage[k], kBagStage));
+            if (!p->bag_stage[k].p()) PCK(p->bag_stage[k].allocate(kBagStage));
             if (!p->bag_ev[k]) PCK(cudaEventCreateWithFlags(&p->bag_ev[k], cudaEventDisableTiming));
         }
         int cur = 0;
         uint64_t w0 = 0, filled = 0;                  // the window [w0, w0 + kBagStage) of the device layout; bytes of it filled
         auto flush = [&]() -> cudaError_t {
-            cudaError_t e = cudaMemcpyAsync(d_blobs + w0, p->bag_stage[cur], filled, cudaMemcpyHostToDevice, p->st);
+            cudaError_t e = cudaMemcpyAsync(d_blobs + w0, p->bag_stage[cur].p(), filled, cudaMemcpyHostToDevice, p->st);
             if (e == cudaSuccess) e = cudaEventRecord(p->bag_ev[cur], p->st);
             cur ^= 1;
             w0 += filled;
@@ -1044,14 +1027,14 @@ int erasor_bag_load_list(erasor_pcd_t p, const uint64_t* nodes, size_t count, fl
                 const uint64_t at = D.src + done;      // device offset of the next byte
                 if (at - w0 >= kBagStage) PCK(flush());
                 const uint64_t take = std::min(D.c.data_len - done, kBagStage - (at - w0));
-                std::memcpy(p->bag_stage[cur] + (at - w0), p->bag_file + D.c.data_off + done, take);
+                std::memcpy(p->bag_stage[cur].as<uint8_t>() + (at - w0), p->bag_file + D.c.data_off + done, take);
                 filled = at - w0 + take;
                 done += take;
             }
         }
         if (filled) PCK(flush());
     }
-    PCK(cudaMemcpyAsync(p->bag_desc.p, desc.data(), sizeof(BagDesc) * desc.size(), cudaMemcpyHostToDevice, p->st));
+    PCK(cudaMemcpyAsync(p->bag_desc.p(), desc.data(), sizeof(BagDesc) * desc.size(), cudaMemcpyHostToDevice, p->st));
     uint4* d_out = reinterpret_cast<uint4*>(out_xyzi);
     if (out_kind == ERASOR_PTR_HOST) { PCK(p->out.ensure(sizeof(uint4) * total)); d_out = p->out.as<uint4>(); }
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(ntiles, (uint64_t)p->sm_count * 8));

@@ -10,30 +10,11 @@
 #include <vector>
 
 #include "../../include/erasor_b200.h"
+#include "buffers.h"
 #include "pose_math.h"
 #include "updater_kernels.h"
 
 using namespace erasor;
-
-namespace {
-struct Buf {
-    void* p = nullptr; size_t cap = 0;
-    cudaError_t ensure(size_t bytes, bool keep = false, cudaStream_t st = nullptr, size_t keep_bytes = 0) {
-        if (bytes <= cap) return cudaSuccess;
-        void* q = nullptr;
-        const size_t want = bytes + bytes / 4 + 4096;
-        cudaError_t e = cudaMalloc(&q, want);
-        if (e != cudaSuccess) return e;
-        if (keep && p && keep_bytes) { e = cudaMemcpyAsync(q, p, keep_bytes, cudaMemcpyDeviceToDevice, st); if (e == cudaSuccess) e = cudaStreamSynchronize(st); }
-        if (p) cudaFree(p);
-        p = q; cap = want;
-        return e;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-}  // namespace
 
 struct erasor_updater_ctx {
     erasor_updater_params_t up{};
@@ -44,10 +25,10 @@ struct erasor_updater_ctx {
     std::string err;
     Mat4 tf_lidar2body{}, tf_body2origin{};
     // maps (origin frame), double-buffered
-    Buf map_a, map_b;        size_t n_map = 0;
-    Buf global_a;            size_t n_global = 0;      // large-scale: map_arranged_global_
-    Buf complement;          size_t n_complement = 0;  // large-scale: map_arranged_complement_
-    Buf scan, qvox, voi, outskirts, tmp_rej, part_tmp, vox_tmp, grid, counters, save_out;
+    DeviceBuffer map_a, map_b;        size_t n_map = 0;
+    DeviceBuffer global_a;            size_t n_global = 0;      // large-scale: map_arranged_global_
+    DeviceBuffer complement;          size_t n_complement = 0;  // large-scale: map_arranged_complement_
+    DeviceBuffer scan, qvox, voi, outskirts, tmp_rej, part_tmp, vox_tmp, grid, counters, save_out;
     size_t n_query = 0, n_voi = 0, n_out = 0, n_rej = 0;
     bool submap_uninit = true;
     double submap_cx = 0, submap_cy = 0;
@@ -57,15 +38,15 @@ struct erasor_updater_ctx {
     // look-ahead (erasor_updater_prefetch_scan): scans of coming nodes are uploaded and voxelised on a second stream while the current
     // node's path runs.  Two slots, so that the caller can hand in node k + 1's scan before it calls process_node for node k.
     struct Lookahead {
-        Buf scan, qvox, vox_tmp, grid, counters;
-        uint32_t* h_words = nullptr;
+        DeviceBuffer scan, qvox, vox_tmp, grid, counters;
+        PinnedBuffer h_words;
         cudaEvent_t ev = nullptr;
         const float* ptr = nullptr; size_t n = 0; int kind = 0; bool valid = false; uint64_t ticket = 0;
     };
     cudaStream_t st2 = nullptr;
     Lookahead la[2];
     uint64_t la_ticket = 0;
-    uint32_t* h_words = nullptr;                     // pinned read-back of the two device counters (a copy into pageable memory would
+    PinnedBuffer h_words;                            // pinned read-back of the two device counters (a copy into pageable memory would
                                                      // block until the stream has drained and then some)
     int sm_count = 132;
     uint64_t map_version = 0;                       // bumped whenever the map changes (processed node, reset)
@@ -74,15 +55,15 @@ struct erasor_updater_ctx {
 
 namespace {
 thread_local std::string g_uerr;
-#define UCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { u->err = std::string(#call) + ": " + cudaGetErrorString(e__); return ERASOR_E_CUDA; } } while (0)
+#define UCK(call) ERASOR_CUDA_TRY(u->err, call, #call)
 #define ECK(call) do { int rc__ = (call); if (rc__ != ERASOR_OK) { u->err = std::string(#call) + ": " + erasor_last_error(u->er); return rc__; } } while (0)
 
 // counters[0] = points selected by the partition, counters[1] = voxels: both read back with one synchronisation
 int read_counters(erasor_updater_ctx* u, size_t* n_sel, size_t* n_vox) {
-    UCK(cudaMemcpyAsync(u->h_words, u->counters.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, u->st));
+    UCK(cudaMemcpyAsync(u->h_words.p(), u->counters.p(), 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, u->st));
     UCK(cudaStreamSynchronize(u->st));
-    if (n_sel) *n_sel = u->h_words[0];
-    if (n_vox) *n_vox = u->h_words[1];
+    if (n_sel) *n_sel = u->h_words.as<uint32_t>()[0];
+    if (n_vox) *n_vox = u->h_words.as<uint32_t>()[1];
     return ERASOR_OK;
 }
 
@@ -91,11 +72,11 @@ void no_partition(FusedJob& J) {
     J.chunk_tmp = nullptr; J.d_total_sel = nullptr; J.out_sel = nullptr; J.out_rest = nullptr;
 }
 void no_voxelize(erasor_updater_ctx* u, FusedJob& J) {
-    J.vin = nullptr; J.vn = 0; J.leaf = 1.0f; J.grid = u->grid.as<VoxGrid>(); J.vtmp = u->vox_tmp.p; J.vout = nullptr;
+    J.vin = nullptr; J.vn = 0; J.leaf = 1.0f; J.grid = u->grid.as<VoxGrid>(); J.vtmp = u->vox_tmp.p(); J.vout = nullptr;
     J.d_n_out = u->counters.as<uint32_t>() + 1; J.T_out = Mat4{}; J.xform_out = 0;
 }
 // U1 job: stable partition of src[0..n) into sel / rest (both in order)
-int add_partition(erasor_updater_ctx* u, FusedJob& J, const PartPred& P, const Mat4& T, bool xform, const float4* src, size_t n, Buf& sel, Buf& rest) {
+int add_partition(erasor_updater_ctx* u, FusedJob& J, const PartPred& P, const Mat4& T, bool xform, const float4* src, size_t n, DeviceBuffer& sel, DeviceBuffer& rest) {
     UCK(sel.ensure(sizeof(float4) * std::max<size_t>(n, 1)));
     UCK(rest.ensure(sizeof(float4) * std::max<size_t>(n, 1)));
     UCK(u->part_tmp.ensure(sizeof(uint32_t) * partition_tmp_words((uint32_t)n)));
@@ -104,10 +85,10 @@ int add_partition(erasor_updater_ctx* u, FusedJob& J, const PartPred& P, const M
     return ERASOR_OK;
 }
 // U3 job: voxelize_preserving_labels of src[0..n) at `leaf` into out, optionally followed by the affine T_out
-int add_voxelize(erasor_updater_ctx* u, FusedJob& J, const float4* src, size_t n, float leaf, Buf& out, const Mat4* T_out) {
+int add_voxelize(erasor_updater_ctx* u, FusedJob& J, const float4* src, size_t n, float leaf, DeviceBuffer& out, const Mat4* T_out) {
     UCK(out.ensure(sizeof(float4) * std::max<size_t>(n, 1)));
     UCK(u->vox_tmp.ensure(voxelize_tmp_bytes((uint32_t)n)));
-    J.vin = src; J.vn = (uint32_t)n; J.leaf = leaf; J.grid = u->grid.as<VoxGrid>(); J.vtmp = u->vox_tmp.p; J.vout = out.as<float4>();
+    J.vin = src; J.vn = (uint32_t)n; J.leaf = leaf; J.grid = u->grid.as<VoxGrid>(); J.vtmp = u->vox_tmp.p(); J.vout = out.as<float4>();
     J.d_n_out = u->counters.as<uint32_t>() + 1; J.T_out = T_out ? *T_out : Mat4{}; J.xform_out = T_out ? 1 : 0;
     return ERASOR_OK;
 }
@@ -118,7 +99,7 @@ int launch_fused(erasor_updater_ctx* u, const FusedJob& J, int max_ctas = 0) {
 }
 
 // stable partition of src[0..n) into sel / rest (both in order); returns the number selected
-int partition(erasor_updater_ctx* u, const PartPred& P, const Mat4& T, bool xform, const float4* src, size_t n, Buf& sel, Buf& rest, size_t* n_sel) {
+int partition(erasor_updater_ctx* u, const PartPred& P, const Mat4& T, bool xform, const float4* src, size_t n, DeviceBuffer& sel, DeviceBuffer& rest, size_t* n_sel) {
     FusedJob J;
     no_voxelize(u, J);
     int rc = add_partition(u, J, P, T, xform, src, n, sel, rest);
@@ -126,7 +107,7 @@ int partition(erasor_updater_ctx* u, const PartPred& P, const Mat4& T, bool xfor
     return read_counters(u, n_sel, nullptr);
 }
 
-int voxelize(erasor_updater_ctx* u, const float4* src, size_t n, float leaf, Buf& out, size_t* n_out) {
+int voxelize(erasor_updater_ctx* u, const float4* src, size_t n, float leaf, DeviceBuffer& out, size_t* n_out) {
     FusedJob J;
     no_partition(J);
     int rc = add_voxelize(u, J, src, n, leaf, out, nullptr);
@@ -157,8 +138,8 @@ int reassign_submap(erasor_updater_ctx* u, double px, double py) {
         // map_arranged_global_ = map_arranged_ + map_arranged_complement_
         const size_t n = u->n_map + u->n_complement;
         UCK(u->global_a.ensure(sizeof(float4) * std::max<size_t>(n, 1)));
-        if (u->n_map) UCK(cudaMemcpyAsync(u->global_a.p, u->map_a.p, sizeof(float4) * u->n_map, cudaMemcpyDeviceToDevice, u->st));
-        if (u->n_complement) UCK(cudaMemcpyAsync(u->global_a.as<float4>() + u->n_map, u->complement.p, sizeof(float4) * u->n_complement, cudaMemcpyDeviceToDevice, u->st));
+        if (u->n_map) UCK(cudaMemcpyAsync(u->global_a.p(), u->map_a.p(), sizeof(float4) * u->n_map, cudaMemcpyDeviceToDevice, u->st));
+        if (u->n_complement) UCK(cudaMemcpyAsync(u->global_a.as<float4>() + u->n_map, u->complement.p(), sizeof(float4) * u->n_complement, cudaMemcpyDeviceToDevice, u->st));
         u->n_global = n;
         return split();
     }
@@ -184,13 +165,13 @@ int erasor_updater_create(const erasor_updater_params_t* up, const erasor_params
     u->st = (cudaStream_t)erasor_stream(u->er);
     auto fail = [&](const char* what, cudaError_t ce) { g_uerr = std::string(what) + ": " + cudaGetErrorString(ce); erasor_updater_destroy(u); return ERASOR_E_CUDA; };
     cudaError_t e;
-    if ((e = u->counters.ensure(64)) != cudaSuccess) return fail("cudaMalloc", e);
-    if ((e = cudaMallocHost(reinterpret_cast<void**>(&u->h_words), 64)) != cudaSuccess) return fail("cudaMallocHost", e);
+    if ((e = u->counters.allocate(64)) != cudaSuccess) return fail("cudaMalloc", e);
+    if ((e = u->h_words.allocate(64)) != cudaSuccess) return fail("cudaMallocHost", e);
     if ((e = cudaStreamCreateWithFlags(&u->st2, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
     for (auto& la : u->la) {
-        if ((e = cudaMallocHost(reinterpret_cast<void**>(&la.h_words), 64)) != cudaSuccess) return fail("cudaMallocHost", e);
+        if ((e = la.h_words.allocate(64)) != cudaSuccess) return fail("cudaMallocHost", e);
         if ((e = cudaEventCreateWithFlags(&la.ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
-        if ((e = la.counters.ensure(64)) != cudaSuccess) return fail("cudaMalloc", e);
+        if ((e = la.counters.allocate(64)) != cudaSuccess) return fail("cudaMalloc", e);
         if ((e = la.grid.ensure(sizeof(VoxGrid))) != cudaSuccess) return fail("cudaMalloc", e);
     }
     if ((e = cudaDeviceGetAttribute(&u->sm_count, cudaDevAttrMultiProcessorCount, device)) != cudaSuccess) return fail("cudaDeviceGetAttribute", e);
@@ -203,9 +184,9 @@ int erasor_updater_create(const erasor_updater_params_t* up, const erasor_params
     u->tf_body2origin = I;
     // load_global_map (OfflineMapUpdater.cpp:107-167), outdoor
     u->num_pcs_init = n_map;
-    Buf& dst = up->is_large_scale ? u->global_a : u->map_a;
+    DeviceBuffer& dst = up->is_large_scale ? u->global_a : u->map_a;
     if ((e = dst.ensure(sizeof(float4) * std::max<size_t>(n_map, 1))) != cudaSuccess) return fail("cudaMalloc", e);
-    if (n_map && (e = cudaMemcpy(dst.p, initial_map_xyzi, sizeof(float4) * n_map, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
+    if (n_map && (e = cudaMemcpy(dst.p(), initial_map_xyzi, sizeof(float4) * n_map, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
     if (up->is_large_scale) { u->n_global = n_map; u->n_map = 0; } else { u->n_map = n_map; }
     *out = u;
     return ERASOR_OK;
@@ -216,15 +197,8 @@ void erasor_updater_destroy(erasor_updater_t u) {
     cudaSetDevice(u->device);
     if (u->st) cudaStreamSynchronize(u->st);
     if (u->st2) { cudaStreamSynchronize(u->st2); cudaStreamDestroy(u->st2); }
-    for (auto& la : u->la) {
+    for (auto& la : u->la)
         if (la.ev) cudaEventDestroy(la.ev);
-        if (la.h_words) cudaFreeHost(la.h_words);
-        for (Buf* b : {&la.scan, &la.qvox, &la.vox_tmp, &la.grid, &la.counters}) b->release();
-    }
-    Buf* bufs[] = {&u->map_a, &u->map_b, &u->global_a, &u->complement, &u->scan, &u->qvox, &u->voi, &u->outskirts,
-                   &u->tmp_rej, &u->part_tmp, &u->vox_tmp, &u->grid, &u->counters, &u->save_out};
-    for (Buf* b : bufs) b->release();
-    if (u->h_words) cudaFreeHost(u->h_words);
     if (u->er) erasor_destroy(u->er);
     delete u;
 }
@@ -236,9 +210,9 @@ int erasor_updater_reset(erasor_updater_t u, const float* initial_map_xyzi, size
     UCK(cudaStreamSynchronize(u->st));
     UCK(cudaStreamSynchronize(u->st2));
     for (auto& la : u->la) la.valid = false;
-    Buf& dst = u->up.is_large_scale ? u->global_a : u->map_a;
+    DeviceBuffer& dst = u->up.is_large_scale ? u->global_a : u->map_a;
     UCK(dst.ensure(sizeof(float4) * std::max<size_t>(n_map, 1)));
-    if (n_map) UCK(cudaMemcpyAsync(dst.p, initial_map_xyzi, sizeof(float4) * n_map, cudaMemcpyHostToDevice, u->st));
+    if (n_map) UCK(cudaMemcpyAsync(dst.p(), initial_map_xyzi, sizeof(float4) * n_map, cudaMemcpyHostToDevice, u->st));
     UCK(cudaStreamSynchronize(u->st));
     u->num_pcs_init = n_map;
     u->n_map = u->up.is_large_scale ? 0 : n_map;
@@ -266,7 +240,7 @@ int erasor_updater_process_node(erasor_updater_t u, int seq, const double* odom7
     const float4* d_scan = reinterpret_cast<const float4*>(lidar_xyzi);
     if (!prefetched && ptr_kind != ERASOR_PTR_DEVICE) {
         UCK(u->scan.ensure(sizeof(float4) * std::max<size_t>(n_lidar, 1)));
-        if (n_lidar) UCK(cudaMemcpyAsync(u->scan.p, lidar_xyzi, sizeof(float4) * n_lidar, cudaMemcpyHostToDevice, u->st));
+        if (n_lidar) UCK(cudaMemcpyAsync(u->scan.p(), lidar_xyzi, sizeof(float4) * n_lidar, cudaMemcpyHostToDevice, u->st));
         d_scan = u->scan.as<float4>();
     }
     // 1 + 2 in ONE cooperative launch: the scan's voxelisation + lidar -> body (:237-241) and, independent of it, the map's
@@ -286,7 +260,7 @@ int erasor_updater_process_node(erasor_updater_t u, int seq, const double* odom7
         if ((rc = launch_fused(u, J, u->sm_count - std::max(1, u->sm_count / 4)))) return rc;
         UCK(cudaEventSynchronize(la->ev));                      // the look-ahead's counters are in its pinned words
         if ((rc = read_counters(u, &u->n_voi, nullptr))) return rc;
-        u->n_query = la->h_words[1];
+        u->n_query = la->h_words.as<uint32_t>()[1];
         std::swap(u->qvox, la->qvox);
         la->valid = false;
     } else {
@@ -336,18 +310,18 @@ int erasor_updater_prefetch_scan(erasor_updater_t u, const float* lidar_xyzi, si
     const float4* d_scan = reinterpret_cast<const float4*>(lidar_xyzi);
     if (ptr_kind != ERASOR_PTR_DEVICE) {
         UCK(la->scan.ensure(sizeof(float4) * std::max<size_t>(n_lidar, 1)));
-        if (n_lidar) UCK(cudaMemcpyAsync(la->scan.p, lidar_xyzi, sizeof(float4) * n_lidar, cudaMemcpyHostToDevice, u->st2));
+        if (n_lidar) UCK(cudaMemcpyAsync(la->scan.p(), lidar_xyzi, sizeof(float4) * n_lidar, cudaMemcpyHostToDevice, u->st2));
         d_scan = la->scan.as<float4>();
     }
     UCK(la->qvox.ensure(sizeof(float4) * std::max<size_t>(n_lidar, 1)));
     UCK(la->vox_tmp.ensure(voxelize_tmp_bytes((uint32_t)n_lidar)));
     FusedJob J;
     no_partition(J);
-    J.vin = d_scan; J.vn = (uint32_t)n_lidar; J.leaf = (float)u->up.query_voxel_size; J.grid = la->grid.as<VoxGrid>(); J.vtmp = la->vox_tmp.p;
+    J.vin = d_scan; J.vn = (uint32_t)n_lidar; J.leaf = (float)u->up.query_voxel_size; J.grid = la->grid.as<VoxGrid>(); J.vtmp = la->vox_tmp.p();
     J.vout = la->qvox.as<float4>(); J.d_n_out = la->counters.as<uint32_t>() + 1; J.T_out = u->tf_lidar2body; J.xform_out = 1;
     u->launches += 1;
     UCK(launch_node_fused(u->st2, J, u->sm_count, std::max(1, u->sm_count / 4)));
-    UCK(cudaMemcpyAsync(la->h_words, la->counters.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, u->st2));
+    UCK(cudaMemcpyAsync(la->h_words.p(), la->counters.p(), 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, u->st2));
     UCK(cudaEventRecord(la->ev, u->st2));
     la->ptr = lidar_xyzi; la->n = n_lidar; la->kind = ptr_kind; la->valid = true; la->ticket = ++u->la_ticket;
     return ERASOR_OK;
@@ -365,12 +339,12 @@ int erasor_updater_get_cloud(erasor_updater_t u, int which, float* xyzi, size_t 
     if (!u || !n) return ERASOR_E_INVALID;
     const void* src = nullptr; size_t k = 0;
     switch (which) {
-        case 0: src = u->map_a.p; k = u->n_map; break;
-        case 1: src = u->voi.p; k = u->n_voi; break;
-        case 2: src = u->qvox.p; k = u->n_query; break;
-        case 5: src = u->tmp_rej.p; k = u->n_rej; break;
-        case 7: src = u->outskirts.p; k = u->n_out; break;
-        case 8: src = u->complement.p; k = u->n_complement; break;
+        case 0: src = u->map_a.p(); k = u->n_map; break;
+        case 1: src = u->voi.p(); k = u->n_voi; break;
+        case 2: src = u->qvox.p(); k = u->n_query; break;
+        case 5: src = u->tmp_rej.p(); k = u->n_rej; break;
+        case 7: src = u->outskirts.p(); k = u->n_out; break;
+        case 8: src = u->complement.p(); k = u->n_complement; break;
         default: u->err = "unknown cloud id"; return ERASOR_E_INVALID;
     }
     *n = k;
@@ -391,8 +365,8 @@ int erasor_updater_save_static_map(erasor_updater_t u, float voxel_size, float* 
     if (u->up.is_large_scale) {
         // *ptr_src = *map_arranged_ + *map_arranged_complement_
         UCK(u->map_b.ensure(sizeof(float4) * std::max<size_t>(u->n_map + u->n_complement, 1)));
-        if (u->n_map) UCK(cudaMemcpyAsync(u->map_b.p, u->map_a.p, sizeof(float4) * u->n_map, cudaMemcpyDeviceToDevice, u->st));
-        if (u->n_complement) UCK(cudaMemcpyAsync(u->map_b.as<float4>() + u->n_map, u->complement.p, sizeof(float4) * u->n_complement, cudaMemcpyDeviceToDevice, u->st));
+        if (u->n_map) UCK(cudaMemcpyAsync(u->map_b.p(), u->map_a.p(), sizeof(float4) * u->n_map, cudaMemcpyDeviceToDevice, u->st));
+        if (u->n_complement) UCK(cudaMemcpyAsync(u->map_b.as<float4>() + u->n_map, u->complement.p(), sizeof(float4) * u->n_complement, cudaMemcpyDeviceToDevice, u->st));
         src = u->map_b.as<float4>(); ns = u->n_map + u->n_complement;
     }
     // the usual call pattern is size query (out == NULL) followed by the fetch: the second call reuses the first one's result
@@ -406,7 +380,7 @@ int erasor_updater_save_static_map(erasor_updater_t u, float voxel_size, float* 
     *n = k;
     if (!out_xyzi) return ERASOR_OK;
     if (cap < k) { u->err = "output buffer too small"; return ERASOR_E_CAPACITY; }
-    if (k) UCK(cudaMemcpyAsync(out_xyzi, u->save_out.p, sizeof(float4) * k, cudaMemcpyDeviceToHost, u->st));
+    if (k) UCK(cudaMemcpyAsync(out_xyzi, u->save_out.p(), sizeof(float4) * k, cudaMemcpyDeviceToHost, u->st));
     UCK(cudaStreamSynchronize(u->st));
     return ERASOR_OK;
 }
@@ -416,7 +390,7 @@ int erasor_updater_voxelize(erasor_updater_t u, const float* xyzi, size_t n_in, 
     if (!u || !n || (n_in && !xyzi)) return ERASOR_E_INVALID;
     UCK(cudaSetDevice(u->device));
     UCK(u->scan.ensure(sizeof(float4) * std::max<size_t>(n_in, 1)));
-    if (n_in) UCK(cudaMemcpyAsync(u->scan.p, xyzi, sizeof(float4) * n_in, cudaMemcpyHostToDevice, u->st));
+    if (n_in) UCK(cudaMemcpyAsync(u->scan.p(), xyzi, sizeof(float4) * n_in, cudaMemcpyHostToDevice, u->st));
     size_t k = 0;
     u->save_version = ~0ull;                         // save_out is about to hold something else
     int rc = voxelize(u, u->scan.as<float4>(), n_in, leaf, u->save_out, &k);
@@ -424,7 +398,7 @@ int erasor_updater_voxelize(erasor_updater_t u, const float* xyzi, size_t n_in, 
     *n = k;
     if (!out_xyzi) return ERASOR_OK;
     if (cap < k) { u->err = "output buffer too small"; return ERASOR_E_CAPACITY; }
-    if (k) UCK(cudaMemcpyAsync(out_xyzi, u->save_out.p, sizeof(float4) * k, cudaMemcpyDeviceToHost, u->st));
+    if (k) UCK(cudaMemcpyAsync(out_xyzi, u->save_out.p(), sizeof(float4) * k, cudaMemcpyDeviceToHost, u->st));
     UCK(cudaStreamSynchronize(u->st));
     return ERASOR_OK;
 }
@@ -439,7 +413,7 @@ int erasor_updater_mapgen_node(erasor_updater_t u, const double* odom7, const fl
     const float4* d_scan = reinterpret_cast<const float4*>(lidar_xyzi);
     if (ptr_kind != ERASOR_PTR_DEVICE) {
         UCK(u->scan.ensure(sizeof(float4) * std::max<size_t>(n_lidar, 1)));
-        if (n_lidar) UCK(cudaMemcpyAsync(u->scan.p, lidar_xyzi, sizeof(float4) * n_lidar, cudaMemcpyHostToDevice, u->st));
+        if (n_lidar) UCK(cudaMemcpyAsync(u->scan.p(), lidar_xyzi, sizeof(float4) * n_lidar, cudaMemcpyHostToDevice, u->st));
         d_scan = u->scan.as<float4>();
     }
     const float max_dist_square = (float)std::pow(2.7, 2);                    // `float max_dist_square = pow(CAR_BODY_SIZE, 2)` (:219)
@@ -461,7 +435,7 @@ int erasor_updater_mapgen_node(erasor_updater_t u, const double* odom7, const fl
     *n = k;
     if (!out_xyzi) return ERASOR_OK;
     if (cap < k) { u->err = "output buffer too small"; return ERASOR_E_CAPACITY; }
-    if (k) UCK(cudaMemcpyAsync(out_xyzi, u->save_out.p, sizeof(float4) * k, ptr_kind == ERASOR_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, u->st));
+    if (k) UCK(cudaMemcpyAsync(out_xyzi, u->save_out.p(), sizeof(float4) * k, ptr_kind == ERASOR_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, u->st));
     UCK(cudaStreamSynchronize(u->st));
     return ERASOR_OK;
 }
@@ -471,7 +445,7 @@ int erasor_updater_get_fused_profile(erasor_updater_t u, uint64_t* ns16) {
     UCK(cudaSetDevice(u->device));
     UCK(cudaStreamSynchronize(u->st));
     VoxGrid g;
-    UCK(cudaMemcpy(&g, u->grid.p, sizeof(VoxGrid), cudaMemcpyDeviceToHost));
+    UCK(cudaMemcpy(&g, u->grid.p(), sizeof(VoxGrid), cudaMemcpyDeviceToHost));
     for (int i = 0; i < 16; ++i) ns16[i] = g.prof[i];
     return ERASOR_OK;
 }

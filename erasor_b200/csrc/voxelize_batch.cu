@@ -24,6 +24,7 @@
 #include <string>
 
 #include "../../include/erasor_b200.h"
+#include "buffers.h"
 #include "device_common.cuh"
 #include "radix_sort.h"
 #include "voxelize_batch.h"
@@ -286,55 +287,21 @@ __global__ void __launch_bounds__(kVbThreads) k_vb_voxels(const float4* __restri
 // host side
 // ============================================================================================================================
 namespace {
-struct VbBuf {
-    void* p = nullptr; size_t cap = 0;
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
-        if (p) { cudaFree(p); p = nullptr; cap = 0; }
-        const size_t want = bytes + bytes / 8 + 256;
-        const cudaError_t e = cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-struct VbPinned {
-    void* p = nullptr; size_t cap = 0;
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
-        if (p) { cudaFreeHost(p); p = nullptr; cap = 0; }
-        const size_t want = bytes + bytes / 4 + 256;
-        const cudaError_t e = cudaMallocHost(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
 int grid_of(uint64_t n, uint64_t per) { return (int)std::max<uint64_t>(1, (n + per - 1) / per); }
 }  // namespace
 
 struct VoxBatch {
-    VbBuf in, keep, off, clouds, head, key_a, key_b, idx_a, idx_b, vkey, vcloud, chunk, radix, out;
-    VbPinned h_off, h_back;            // offsets on their way up, head + output offsets on their way back (pinned: DESIGN.md 6(i))
+    DeviceBuffer in, keep, off, clouds, head, key_a, key_b, idx_a, idx_b, vkey, vcloud, chunk, radix, out;
+    PinnedBuffer h_off, h_back;        // offsets on their way up, head + output offsets on their way back (pinned: DESIGN.md 6(i))
     bool in_flight = false;            // a failed call may have left copies from h_off queued
     int  sm_count = 0;
 };
 
 VoxBatch* vox_batch_create() { return new VoxBatch(); }
 
-void vox_batch_destroy(VoxBatch* b) {
-    if (!b) return;
-    for (VbBuf* x : {&b->in, &b->keep, &b->off, &b->clouds, &b->head, &b->key_a, &b->key_b, &b->idx_a, &b->idx_b, &b->vkey, &b->vcloud, &b->chunk,
-                     &b->radix, &b->out})
-        x->release();
-    b->h_off.release();
-    b->h_back.release();
-    delete b;
-}
+void vox_batch_destroy(VoxBatch* b) { delete b; }
 
-#define VCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e__); return ERASOR_E_CUDA; } } while (0)
+#define VCK(call) ERASOR_CUDA_TRY(err, call, #call)
 
 int vox_batch_run(VoxBatch* b, cudaStream_t st, const float* xyzi, const uint64_t* offsets, int F, const uint8_t* keep, float leaf,
                   const float* T12, bool dev, const float** d_out, uint64_t* out_offsets, uint64_t& launches, std::string& err) {
@@ -355,11 +322,11 @@ int vox_batch_run(VoxBatch* b, cudaStream_t st, const float* xyzi, const uint64_
     const uint8_t* d_keep = keep;
     if (!dev) {
         VCK(b->in.ensure(sizeof(float4) * N64));
-        VCK(cudaMemcpyAsync(b->in.p, xyzi, sizeof(float4) * N64, cudaMemcpyHostToDevice, st));
+        VCK(cudaMemcpyAsync(b->in.p(), xyzi, sizeof(float4) * N64, cudaMemcpyHostToDevice, st));
         pts = b->in.as<const float4>();
         if (keep) {
             VCK(b->keep.ensure(N64));
-            VCK(cudaMemcpyAsync(b->keep.p, keep, N64, cudaMemcpyHostToDevice, st));
+            VCK(cudaMemcpyAsync(b->keep.p(), keep, N64, cudaMemcpyHostToDevice, st));
             d_keep = b->keep.as<const uint8_t>();
         }
     }
@@ -367,13 +334,13 @@ int vox_batch_run(VoxBatch* b, cudaStream_t st, const float* xyzi, const uint64_
     uint32_t* ho = b->h_off.as<uint32_t>();
     for (int c = 0; c <= F; ++c) ho[c] = (uint32_t)offsets[c];
     VCK(b->off.ensure(sizeof(uint32_t) * (F + 1)));
-    VCK(cudaMemcpyAsync(b->off.p, ho, sizeof(uint32_t) * (F + 1), cudaMemcpyHostToDevice, st));
+    VCK(cudaMemcpyAsync(b->off.p(), ho, sizeof(uint32_t) * (F + 1), cudaMemcpyHostToDevice, st));
     b->in_flight = true;
 
     const size_t words = (size_t)N + 1;
     VCK(b->clouds.ensure(sizeof(VbCloud) * F));
     VCK(b->head.ensure(sizeof(VbHead) + sizeof(uint32_t) * (F + 1)));
-    for (VbBuf* x : {&b->key_a, &b->key_b, &b->idx_a, &b->idx_b, &b->vkey, &b->vcloud}) VCK(x->ensure(sizeof(uint32_t) * words));
+    for (DeviceBuffer* x : {&b->key_a, &b->key_b, &b->idx_a, &b->idx_b, &b->vkey, &b->vcloud}) VCK(x->ensure(sizeof(uint32_t) * words));
     const uint32_t nch = (uint32_t)((N64 + kVbChunk - 1) / kVbChunk);
     VCK(b->chunk.ensure(sizeof(uint32_t) * nch));
     VCK(b->radix.ensure(sizeof(uint32_t) * radix_scratch_words(N)));
@@ -421,7 +388,7 @@ int vox_batch_run(VoxBatch* b, cudaStream_t st, const float* xyzi, const uint64_
     // the one read-back: scalars + output offsets
     const size_t back = sizeof(VbHead) + sizeof(uint32_t) * (F + 1);
     VCK(b->h_back.ensure(back));
-    VCK(cudaMemcpyAsync(b->h_back.p, hd, back, cudaMemcpyDeviceToHost, st));
+    VCK(cudaMemcpyAsync(b->h_back.p(), hd, back, cudaMemcpyDeviceToHost, st));
     VCK(cudaStreamSynchronize(st));
     b->in_flight = false;
     const VbHead* h = b->h_back.as<const VbHead>();
