@@ -31,6 +31,8 @@ EXPORTS = [
     "erasor_map_create", "erasor_map_destroy", "erasor_map_size", "erasor_map_reset_keep", "erasor_map_get_keep", "erasor_map_keep_device",
     "erasor_map_points_device", "erasor_attach_map", "erasor_process_nodes", "erasor_process_nodes_async", "erasor_get_node_stats",
     "erasor_voxelize_batch",
+    "erasor_set_node_inserts", "erasor_get_node_inserts", "erasor_map_append_inserts", "erasor_map_inserts", "erasor_map_clear_inserts",
+    "erasor_save_node_map",
     "erasor_comm_unique_id", "erasor_comm_init", "erasor_comm_destroy", "erasor_allgather_and_keep", "erasor_and_keep_masks",
     "erasor_get_kernel_time_ms", "erasor_reset_kernel_times", "erasor_get_rgpf_profile", "erasor_get_srt_profile", "erasor_profile_k1",
     "erasor_updater_create", "erasor_updater_destroy", "erasor_updater_reset", "erasor_updater_last_error", "erasor_updater_process_node", "erasor_updater_prefetch_scan",
@@ -157,6 +159,12 @@ def _load():
     L.erasor_get_node_stats.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32), POINTER(c_uint32)]
     L.erasor_voxelize_batch.argtypes = [c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p, c_float, POINTER(c_double), c_int,
                                         POINTER(c_void_p), POINTER(c_uint64)]
+    L.erasor_set_node_inserts.argtypes = [c_void_p, c_int]
+    L.erasor_get_node_inserts.argtypes = [c_void_p, POINTER(c_void_p), POINTER(c_uint64)]
+    L.erasor_map_append_inserts.argtypes = [c_void_p, c_void_p]
+    L.erasor_map_inserts.argtypes = [c_void_p, POINTER(c_void_p), POINTER(c_size_t)]
+    L.erasor_map_clear_inserts.argtypes = [c_void_p]
+    L.erasor_save_node_map.argtypes = [c_void_p, c_void_p, c_float, POINTER(c_void_p), POINTER(c_size_t)]
     L.erasor_comm_unique_id.argtypes = [c_void_p]
     L.erasor_comm_init.argtypes = [c_void_p, c_void_p, c_int, c_int]
     L.erasor_comm_destroy.argtypes = [c_void_p]
@@ -559,12 +567,31 @@ class Handle(_Native):
 
     def save_static_map(self, m: "Map", voxel: float) -> np.ndarray:
         """save_static_map of node mode (OfflineMapUpdater.cpp:174-196 without the file): the resident map's points under its keep
-        mask, voxelised at `voxel`, in the map frame."""
-        self._ck(self.L.erasor_synchronize(self.h))
-        d, oo = self.voxelize_batch_ptr(m.points_ptr, [0, m.size], voxel, m.keep_ptr, None, PTR_DEVICE)
-        out = np.empty((int(oo[-1]), 4), dtype=np.float32)
-        _memcpy_from_device(out, d)
+        mask, followed by the map's insert store (empty unless inserts were appended), voxelised at `voxel`, in the map frame."""
+        d, n = c_void_p(), c_size_t()
+        self._ck(self.L.erasor_save_node_map(self.h, m.h, float(voxel), ctypes.byref(d), ctypes.byref(n)))
+        out = np.empty((n.value, 4), dtype=np.float32)
+        _memcpy_from_device(out, d.value or 0)
         return out
+
+    # -- node-mode inserts (DESIGN.md section 8.4) -------------------------------------------------------------------------------
+    def set_node_inserts(self, enable: bool):
+        """Opt in (or out) of building each node's inserted points in process_nodes / process_scans."""
+        self._ck(self.L.erasor_set_node_inserts(self.h, 1 if enable else 0))
+
+    def node_inserts_ptr(self):
+        """The last node call's inserts: (device pointer of float4 points, uint64 offsets [F+1]), valid until the next submission."""
+        off = np.zeros(self.n_frames + 1, dtype=np.uint64)
+        d = c_void_p()
+        self._ck(self.L.erasor_get_node_inserts(self.h, ctypes.byref(d), off.ctypes.data_as(POINTER(c_uint64))))
+        return int(d.value or 0), off
+
+    def node_inserts(self):
+        """The last node call's inserts in the map frame: (float32 [n,4], uint64 offsets [F+1]; node f = [off[f], off[f+1]))."""
+        d, off = self.node_inserts_ptr()
+        out = np.empty((int(off[-1]), 4), dtype=np.float32)
+        _memcpy_from_device(out, d)
+        return out, off
 
     # -- the exchange step ------------------------------------------------------------------------
     def comm_init(self, id128: bytes, n_ranks: int, rank: int):
@@ -669,6 +696,26 @@ class Map(_Native):
         if rc != OK:
             raise ErasorError(rc, "erasor_map_get_keep")
         return out
+
+    def append_inserts(self, h: "Handle"):
+        """Append h's last node call's inserts to the map's store (callers append in node order)."""
+        rc = self.L.erasor_map_append_inserts(self.h, h.h)
+        if rc != OK:
+            raise ErasorError(rc, h._message(h.h))
+
+    def inserts(self) -> np.ndarray:
+        d, n = c_void_p(), c_size_t()
+        rc = self.L.erasor_map_inserts(self.h, ctypes.byref(d), ctypes.byref(n))
+        if rc != OK:
+            raise ErasorError(rc, "erasor_map_inserts")
+        out = np.empty((n.value, 4), dtype=np.float32)
+        _memcpy_from_device(out, d.value or 0)
+        return out
+
+    def clear_inserts(self):
+        rc = self.L.erasor_map_clear_inserts(self.h)
+        if rc != OK:
+            raise ErasorError(rc, "erasor_map_clear_inserts")
 
 
 class Updater(_Native):

@@ -43,6 +43,8 @@ struct erasor_map_ctx {
     int          device = 0;
     DeviceBuffer d_pts, d_keep;                // float4 [n + kMapPad], uint8 [max(n, 1)]
     size_t       n = 0;
+    DeviceBuffer d_ins;                        // node-mode inserts appended by the callers (erasor_map_append_inserts), float4 [n_ins]
+    size_t       n_ins = 0;
     cudaStream_t st = nullptr;
     std::string  err;
 };
@@ -123,6 +125,15 @@ struct erasor_ctx {
 
     // node mode
     erasor_map_ctx* map = nullptr;
+    // node-mode inserts (erasor_set_node_inserts, DESIGN.md section 8.4): per submission the query scatter plan, the assembled
+    // inserts of its frames and their offsets; per call (all its sub-batches) the inserts in frame order
+    bool node_inserts = false;
+    HBuf d_ins{alloc_epoch}, d_ins_fwd{alloc_epoch}, d_ins_slot{alloc_epoch}, d_ins_n{alloc_epoch}, d_ins_bin_off{alloc_epoch},
+         d_ins_frame_cnt{alloc_epoch}, d_ins_off{alloc_epoch};
+    PinnedBuffer h_ins_fwd, h_ins_off;         // body -> origin rows [F][12] / offsets [F+1] of the submission
+    DeviceBuffer d_ins_call;                   // the last call's inserts (never in a captured graph)
+    std::vector<uint64_t> ins_call_off;        // its offsets: F + 1 entries once the call has completed
+    DeviceBuffer d_save, d_save_keep;          // erasor_save_node_map: map ++ inserts and its keep bytes
 
     // erasor_voxelize_batch: its scratch and output cloud (created on first use)
     erasor::VoxBatch* vb = nullptr;
@@ -356,15 +367,25 @@ int run_k1(erasor_ctx* h, int mode) {
 
 // K3 -> K2 -> K4 ; mode 0: every bin scattered + partitioned copies (cloud outputs), mode 1 / 2: flagged only + masks
 // classes: which R-GPF size classes to launch (bits 0|1: A and B, bit 2: C); 0x8 alone = R-GPF only, for the class-C fix-up
-int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes = 7, bool only_rgpf = false) {
-    const int B = h->B, F = h->F;
-    const NodePose* poses = mode == 2 ? h->d_poses.as<NodePose>() : nullptr;
-    uint32_t* nflag = h->d_nflag.as<uint32_t>() + h->f0;
+SrtParams srt_params(const erasor_ctx* h, int version, int mode) {
     SrtParams sp{};
     sp.scan_ratio_threshold = h->p.scan_ratio_threshold;
     sp.th_bin_max_h = h->p.th_bin_max_h;
     sp.minimum_num_pts = h->p.minimum_num_pts;
-    sp.version = version; sp.R = h->p.num_rings; sp.S = h->p.num_sectors; sp.B = B; sp.scatter_mode = mode == 0 ? 0 : 1;
+    sp.version = version; sp.R = h->p.num_rings; sp.S = h->p.num_sectors; sp.B = h->B; sp.scatter_mode = mode == 0 ? 0 : 1;
+    return sp;
+}
+
+// node mode with inserts: R-GPF also writes its partitioned copy (ground first), which the inserts read
+bool inserts_on(const erasor_ctx* h, int mode) { return mode == 2 && h->node_inserts; }
+
+int run_insert_plan(erasor_ctx* h);
+
+int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes = 7, bool only_rgpf = false) {
+    const int B = h->B, F = h->F;
+    const NodePose* poses = mode == 2 ? h->d_poses.as<NodePose>() : nullptr;
+    uint32_t* nflag = h->d_nflag.as<uint32_t>() + h->f0;
+    const SrtParams sp = srt_params(h, version, mode);
     const bool fused = mode != 0 && h->fused_srt;      // mask modes: SRT inside the scatter kernel
     if (!fused && !only_rgpf) {
         Scope s(h, 3);
@@ -413,15 +434,102 @@ int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_
         if (with_c) CK(cudaStreamWaitEvent(h->stream_c, h->ev_fork, 0));
         CK(launch_k4(h->stream_a, h->stream_b, h->stream_c, gp, h->d_recs.as<FlagRec>(), h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->rec_capacity,
                      h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), h->cur_map,
-                     h->d_frame_off.as<uint32_t>(), mode == 0 ? h->d_part.as<float4>() : nullptr, keep_mask, ground_mask,
+                     h->d_frame_off.as<uint32_t>(), (mode == 0 || inserts_on(h, mode)) ? h->d_part.as<float4>() : nullptr, keep_mask, ground_mask,
                      h->d_frame_rej.as<uint32_t>() + h->f0, h->d_scratch.as<unsigned char>(), h->sm_count, h->d_fence.as<unsigned long long>(), fold, classes));
         CK(cudaEventRecord(h->ev_join_a, h->stream_a));
         CK(cudaEventRecord(h->ev_join_b, h->stream_b));
         if (with_c) CK(cudaEventRecord(h->ev_join_c, h->stream_c));
+        // node-mode inserts: the plan and the query scatter need only K1's tables, so they run on the main stream under R-GPF
+        if (inserts_on(h, mode) && !only_rgpf) { int rc = run_insert_plan(h); if (rc) return rc; }
         CK(cudaStreamWaitEvent(h->stream, h->ev_join_a, 0));
         CK(cudaStreamWaitEvent(h->stream, h->ev_join_b, 0));
         if (with_c) CK(cudaStreamWaitEvent(h->stream, h->ev_join_c, 0));
     }
+    return ERASOR_OK;
+}
+
+// Node-mode inserts of one submission: buffers (before any capture -- a reallocation retires the cached graphs) ...
+int ensure_insert_buffers(erasor_ctx* h) {
+    const size_t B = (size_t)h->B, F = (size_t)h->F, NM = h->NM, NQ = h->NQ;
+    CK(h->d_part.ensure(sizeof(float4) * std::max<size_t>(NM, 1)));
+    CK(h->d_qry_sorted.ensure(sizeof(float4) * std::max<size_t>(NQ, 1)));
+    CK(h->d_qry_src.ensure(sizeof(uint32_t) * std::max<size_t>(NQ, 1)));
+    CK(h->d_ins_slot.ensure(sizeof(uint32_t) * F * B));
+    CK(h->d_ins_n.ensure(sizeof(uint32_t) * F));
+    CK(h->d_ins_bin_off.ensure(sizeof(uint32_t) * F * B));
+    CK(h->d_ins_frame_cnt.ensure(sizeof(uint32_t) * F));
+    CK(h->d_ins_off.ensure(sizeof(uint32_t) * (F + 1)));
+    CK(h->d_ins_fwd.ensure(sizeof(float) * 12 * F));
+    CK(h->d_ins.ensure(sizeof(float4) * (NQ + NM + 1)));      // a frame inserts at most its binned queries + its flagged map points
+    if (h->p.version == 3 && !h->p.skip_voxelize) {
+        CK(h->d_vox.ensure(sizeof(float4) * (NM + NQ + 1)));
+        CK(h->d_vox_cnt.ensure(sizeof(uint32_t) * std::max<size_t>(h->rec_capacity, 1)));
+        CK(h->d_vox_start.ensure(sizeof(uint32_t) * std::max<size_t>(h->rec_capacity, 1)));
+        CK(h->d_vox_scratch.ensure((size_t)k4b_scratch_offset((uint32_t)NQ, (uint32_t)NM, (uint32_t)(F * B)) + 36 + 64));
+    }
+    if (sizeof(float) * 12 * F > h->h_ins_fwd.cap() || sizeof(uint32_t) * (F + 1) > h->h_ins_off.cap()) h->alloc_epoch++;   // captured copies
+    CK(h->h_ins_fwd.ensure(sizeof(float) * 12 * F));
+    CK(h->h_ins_off.ensure(sizeof(uint32_t) * (F + 1)));
+    return ERASOR_OK;
+}
+
+// ... after K1: the action of every bin and the stable scatter of the inserting bins' query points ...
+int run_insert_plan(erasor_ctx* h) {
+    const int B = h->B, F = h->F;
+    CK(cudaMemcpyAsync(h->d_ins_fwd.p(), h->h_ins_fwd.p(), sizeof(float) * 12 * (size_t)F, cudaMemcpyHostToDevice, h->stream));
+    h->launches += 1 + (h->n_chunks_qry ? 1 : 0);
+    CK(launch_ins_plan(h->stream, srt_params(h, h->p.version, 2), F, h->d_chunk_range.as<uint32_t>(), h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(),
+                       h->d_zmax.as<uint32_t>(), h->d_cnt.as<uint32_t>(), h->d_action.as<uint8_t>(), h->d_flag_slot.as<uint32_t>(),
+                       h->d_ins_slot.as<uint32_t>(), h->d_ins_n.as<uint32_t>(), h->d_dst_start.as<uint32_t>()));
+    CK(launch_k2(h->stream, h->d_chunks.as<ChunkDesc>(), h->n_chunks_map, h->n_chunks_qry, h->d_bin_qry.as<uint16_t>(), h->cur_qry, nullptr,
+                 h->d_chcnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>() + (size_t)F * (B + 2), h->d_ins_slot.as<uint32_t>(), h->d_ins_n.as<uint32_t>(),
+                 h->d_qry_sorted.as<float4>(), h->d_qry_src.as<uint32_t>(), B, nullptr, nullptr, 8));
+    return ERASOR_OK;
+}
+
+// ... after R-GPF: K4b over every frame's flagged bins (v3), then sizes, offsets and the copy; the offsets are read back through
+// pinned memory (again after a late class-C run, which changes the ground of its bins)
+int run_insert_assemble(erasor_ctx* h) {
+    const int B = h->B, F = h->F;
+    const bool vox = h->p.version == 3 && !h->p.skip_voxelize;
+    const uint32_t* qoff = h->d_frame_off.as<uint32_t>() + (F + 1);
+    if (vox) {
+        h->launches++;
+        CK(launch_k4b(h->stream, (float)h->p.map_voxel_size, B, F, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
+                      h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(), qoff, h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(),
+                      h->d_vox.as<float4>(), h->d_vox_cnt.as<uint32_t>(), h->d_vox_start.as<uint32_t>(), h->d_vox_scratch.as<unsigned char>(), h->sm_count));
+    }
+    h->launches += kInsAssembleLaunches;
+    CK(launch_ins_assemble(h->stream, B, F, vox ? 1 : 0, h->d_action.as<uint8_t>(), h->d_flag_slot.as<uint32_t>(), h->d_frame_rec_base.as<uint32_t>(),
+                           h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity, h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(),
+                           qoff, vox ? h->d_vox_cnt.as<uint32_t>() : nullptr, vox ? h->d_vox_start.as<uint32_t>() : nullptr,
+                           h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(), vox ? h->d_vox.as<float4>() : nullptr, h->d_ins_fwd.as<float>(),
+                           h->d_ins_bin_off.as<uint32_t>(), h->d_ins_frame_cnt.as<uint32_t>(), h->d_ins_off.as<uint32_t>(), h->d_ins.as<float4>(),
+                           h->sm_count));
+    CK(cudaMemcpyAsync(h->h_ins_off.p(), h->d_ins_off.p(), sizeof(uint32_t) * ((size_t)F + 1), cudaMemcpyDeviceToHost, h->stream));
+    return ERASOR_OK;
+}
+
+// room for n_new float4 in buf, its first n_old kept (the copy is ordered on st and finished before the old allocation goes)
+cudaError_t grow_points(DeviceBuffer& buf, size_t n_old, size_t n_new, cudaStream_t st) {
+    const size_t bytes = sizeof(float4) * n_new;
+    if (bytes <= buf.cap()) return cudaSuccess;
+    DeviceBuffer nb;
+    cudaError_t e = nb.allocate(bytes + bytes / 4 + 4096);
+    if (e == cudaSuccess && n_old) e = cudaMemcpyAsync(nb.p(), buf.p(), sizeof(float4) * n_old, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) buf = std::move(nb);
+    return e;
+}
+
+// a completed submission's inserts, appended to the call's (sub-batches in frame order)
+int collect_inserts(erasor_ctx* h) {
+    const uint32_t* off = h->h_ins_off.as<uint32_t>();
+    const size_t base = h->ins_call_off.back(), n = off[h->F];
+    CK(grow_points(h->d_ins_call, base, base + n, h->stream));
+    if (n) CK(cudaMemcpyAsync(h->d_ins_call.as<float4>() + base, h->d_ins.p(), sizeof(float4) * n, cudaMemcpyDeviceToDevice, h->stream));
+    for (int f = 1; f <= h->F; ++f) h->ins_call_off.push_back(base + off[f]);
+    CK(cudaStreamSynchronize(h->stream));
     return ERASOR_OK;
 }
 
@@ -557,6 +665,7 @@ int erasor_set_inputs(erasor_handle_t h, const float* map_voi_xyzi, size_t n_map
     if (h->pending && (rc = erasor_wait(h))) return rc;
     h->stage = 0;
     h->f0 = 0; h->stat_F = 1;
+    h->ins_call_off.clear();                   // the inserts of an earlier node call end with this submission
     h->qry_xyz = false;
     if (ptr_kind != ERASOR_PTR_HOST && ptr_kind != ERASOR_PTR_DEVICE) { h->err = "erasor_set_inputs: ptr_kind must be HOST or DEVICE (the cloud outputs carry the query's intensity)"; return ERASOR_E_INVALID; }
     const uint64_t mo[2] = {0, n_map}, qo[2] = {0, n_query};
@@ -604,8 +713,8 @@ int erasor_compare(erasor_handle_t h, int version, int frame) {
         if (vox) {
             Scope s(h, 4);
             h->launches++;
-            CK(launch_k4b(h->stream, (float)h->p.map_voxel_size, B, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
-                          h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(), h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(),
+            CK(launch_k4b(h->stream, (float)h->p.map_voxel_size, B, 1, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
+                          h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(), h->d_frame_off.as<uint32_t>() + 2, h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(),
                           h->d_vox.as<float4>(), h->d_vox_cnt.as<uint32_t>(), h->d_vox_start.as<uint32_t>(),
                           h->d_vox_scratch.as<unsigned char>(), h->sm_count));
         }
@@ -819,6 +928,7 @@ struct Submit {
     uint8_t*        fold_global = nullptr;
     size_t          fold_n = 0;
     const NodePose* poses = nullptr;        // mode 2: host array [F]
+    const double*   poses7 = nullptr;       // mode 2: the caller's odom7 of these frames (the inserts' body -> origin)
     uint8_t*        keep_out = nullptr;     // mode 2 (nullable)
     int             f0 = 0;                 // index of the first frame within the caller's batch (per-frame counters)
 };
@@ -856,6 +966,15 @@ int submit(erasor_ctx* h, const Submit& S) {
         CK(h->h_pose.ensure(sizeof(NodePose) * (size_t)S.F));
         std::memcpy(h->h_pose.p(), S.poses, sizeof(NodePose) * (size_t)S.F);
     }
+    const bool ins = inserts_on(h, S.mode);
+    if (ins) {
+        if ((rc = ensure_insert_buffers(h))) return rc;
+        for (int f = 0; f < S.F; ++f) {
+            Mat4 T;
+            pose_to_mat(S.poses7 + 7 * (size_t)f, T);       // tf_body2origin_ = geoPose2eigen(odom), as body2origin applies it
+            std::memcpy(h->h_ins_fwd.as<float>() + 12 * (size_t)f, T.m, sizeof(float) * 12);
+        }
+    }
     const bool with_c = h->class_c_state != 0;
     auto enqueue = [&]() -> int {
         int r;
@@ -876,6 +995,7 @@ int submit(erasor_ctx* h, const Submit& S) {
         if (S.mode == 2)        fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};
         else if (S.fold_global) fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
         if ((r = run_compare(h, h->p.version, S.mode, d_keep, nullptr, fold, with_c ? 7 : 3))) return r;
+        if (ins && (r = run_insert_assemble(h))) return r;      // (run_compare ran the plan and the query scatter under R-GPF)
         h->last.with_c = with_c; h->last.host = host; h->last.mode = S.mode; h->last.d_keep = d_keep; h->last.user_keep = S.keep_mask; h->last.n_keep = n_keep;
         h->last.keep_out = S.keep_out; h->last.n_map_global = n_map_global; h->last.fold = fold;
         CK(cudaMemcpyAsync(h->h_words.as<uint32_t>() + 1, h->d_queue.as<uint32_t>() + kBucketC0, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
@@ -897,7 +1017,7 @@ int submit(erasor_ctx* h, const Submit& S) {
         erasor_ctx::StepGraph key{};
         key.ptr[0] = S.map_xyzi; key.ptr[1] = S.qry_xyzi; key.ptr[2] = S.keep_mask; key.ptr[3] = S.fold_index; key.ptr[4] = S.fold_global;
         key.ptr[5] = S.keep_out; key.ptr[6] = S.mode == 2 ? (const void*)h->map : nullptr; key.ptr[7] = with_c ? (const void*)h : nullptr;
-        key.fold_n = S.fold_n; key.kind = S.ptr_kind | (S.qry_xyz ? ERASOR_PTR_QUERY_XYZ : 0); key.mode = S.mode; key.f0 = S.f0; key.epoch = h->desc_epoch; key.alloc = h->alloc_epoch;
+        key.fold_n = S.fold_n; key.kind = S.ptr_kind | (S.qry_xyz ? ERASOR_PTR_QUERY_XYZ : 0) | (ins ? 0x100 : 0); key.mode = S.mode; key.f0 = S.f0; key.epoch = h->desc_epoch; key.alloc = h->alloc_epoch;
         auto same = [&](const erasor_ctx::StepGraph& g) {
             return std::equal(g.ptr, g.ptr + 8, key.ptr) && g.fold_n == key.fold_n && g.kind == key.kind && g.mode == key.mode && g.f0 == key.f0 &&
                    g.epoch == key.epoch && g.alloc == key.alloc;
@@ -971,6 +1091,7 @@ int process_frames_impl(erasor_handle_t h, const float* map_xyzi, const uint64_t
     int rc;
     if (h->pending && (rc = erasor_wait(h))) return rc;
     h->stat_F = n_frames;
+    h->ins_call_off.clear();                   // the inserts of an earlier node call end with this submission
     std::vector<uint64_t> mo, qo;
     for (int f0 = 0; f0 < n_frames;) {
         const int f1 = sub_batch_end(h, map_offsets, query_offsets, f0, n_frames);
@@ -1017,22 +1138,31 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
     const bool qxyz = (ptr_kind & ERASOR_PTR_QUERY_XYZ) != 0;
     ptr_kind &= ~ERASOR_PTR_QUERY_XYZ;
     if (ptr_kind != ERASOR_PTR_HOST && ptr_kind != ERASOR_PTR_DEVICE) { h->err = "bad ptr_kind"; return ERASOR_E_INVALID; }
+    if (qxyz && h->node_inserts) {
+        h->err = "node inserts carry the query's intensity: packed x y z queries (ERASOR_PTR_QUERY_XYZ) need erasor_set_node_inserts(h, 0)";
+        return ERASOR_E_INVALID;
+    }
     int rc;
     if (h->pending && (rc = erasor_wait(h))) return rc;
     const size_t N = h->map->n;
     const double range = voi_max_range > 0.0 ? voi_max_range : h->p.max_range;
     h->stat_F = n_frames;
-    // scratch per (frame, map point): bin id 2 + scattered point 16 + source index 4 + class-C scratch 24 bytes
+    h->ins_call_off.assign(h->node_inserts ? 1 : 0, 0);
+    // scratch per (frame, map point): bin id 2 + scattered point 16 + source index 4 + class-C scratch 24 bytes; with inserts also
+    // R-GPF's partitioned copy 16 + the inserts 16 + K4b's voxels 16 and scratch 36 bytes
     size_t budget = (size_t)16 << 30;
     if (const char* e = std::getenv("ERASOR_B200_NODE_SCRATCH_GB")) budget = (size_t)std::max(1.0, std::atof(e)) << 30;
-    const size_t by_mem = std::max<size_t>(1, budget / (46 * std::max<size_t>(N, 1)));
+    const size_t by_mem = std::max<size_t>(1, budget / ((h->node_inserts ? 130 : 46) * std::max<size_t>(N, 1)));
     const size_t by_idx = std::max<size_t>(1, (size_t)0xFFFFFFF0ull / std::max<size_t>(N, 1) - 1);
     const int max_frames = (int)std::min<size_t>({by_mem, by_idx, std::max<size_t>(1, kMaxRecords / (size_t)h->B), (size_t)n_frames});
     std::vector<uint64_t> mo, qo;
     std::vector<NodePose> poses;
     for (int f0 = 0; f0 < n_frames;) {
         int f1 = f0;
-        while (f1 < n_frames && f1 - f0 < max_frames && query_offsets[f1 + 1] - query_offsets[f0] < 0xFFFFFFF0ull) ++f1;
+        // with inserts, the scattered query and map points of a sub-batch index one array (K4b's voxels, the inserts)
+        auto fits = [&](int f) { return query_offsets[f + 1] - query_offsets[f0] < 0xFFFFFFF0ull &&
+                                        (!h->node_inserts || (uint64_t)(f + 1 - f0) * N + (query_offsets[f + 1] - query_offsets[f0]) < 0xFFFFFFF0ull); };
+        while (f1 < n_frames && f1 - f0 < max_frames && fits(f1)) ++f1;
         if (f1 == f0) { h->err = "a single query exceeds 2^32 points"; return ERASOR_E_INVALID; }
         const int F = f1 - f0;
         mo.resize((size_t)F + 1);
@@ -1048,6 +1178,7 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         S.qry_xyzi = query_xyzi ? query_xyzi + (qxyz ? 3 : 4) * q0 : nullptr;
         S.keep_mask = frame_keep ? frame_keep + (size_t)f0 * N : nullptr;
         S.poses = poses.data();
+        S.poses7 = poses7 + 7 * (size_t)f0;
         S.keep_out = (f1 == n_frames) ? keep_out : nullptr;
         if ((rc = submit(h, S))) return rc;
         if (f1 < n_frames) {                                         // the next sub-batch reuses the handle's buffers
@@ -1076,11 +1207,13 @@ int erasor_wait(erasor_handle_t h) {
             // bins are independent, the masks only gain zeros), then repeat the output copies.  The next submissions launch it up front.
             int rc = run_compare(h, h->p.version, h->last.mode, h->last.d_keep, nullptr, h->last.fold, 4, true);
             if (rc) return rc;
+            if (inserts_on(h, h->last.mode) && (rc = run_insert_assemble(h))) return rc;
             if (h->last.host && h->last.n_keep) CK(cudaMemcpyAsync(h->last.user_keep, h->last.d_keep, h->last.n_keep, cudaMemcpyDeviceToHost, h->stream));
             if (h->last.keep_out && h->last.n_map_global)
                 CK(cudaMemcpyAsync(h->last.keep_out, h->map->d_keep.as<uint8_t>(), h->last.n_map_global, h->last.host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, h->stream));
             CK(cudaStreamSynchronize(h->stream));
         }
+        if (inserts_on(h, h->last.mode)) return collect_inserts(h);
     }
     return ERASOR_OK;
 }
@@ -1245,6 +1378,86 @@ int erasor_get_node_stats(erasor_handle_t h, uint32_t* n_voi_points, uint32_t* n
     }
     if (n_flagged_bins) CK(cudaMemcpy(n_flagged_bins, h->d_nflag.p(), sizeof(uint32_t) * h->stat_F, cudaMemcpyDeviceToHost));
     if (n_rejected_points) CK(cudaMemcpy(n_rejected_points, h->d_frame_rej.p(), sizeof(uint32_t) * h->stat_F, cudaMemcpyDeviceToHost));
+    return ERASOR_OK;
+}
+
+int erasor_set_node_inserts(erasor_handle_t h, int enable) {
+    if (!h) return ERASOR_E_INVALID;
+    if (h->pending) { h->err = "erasor_set_node_inserts while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
+    h->node_inserts = enable != 0;
+    h->ins_call_off.clear();
+    return ERASOR_OK;
+}
+
+int erasor_get_node_inserts(erasor_handle_t h, const float** d_xyzi, uint64_t* offsets) {
+    if (!h) return ERASOR_E_INVALID;
+    if (!d_xyzi || !offsets) { h->err = "null argument"; return ERASOR_E_INVALID; }
+    int rc;
+    if ((rc = erasor_wait(h))) return rc;
+    if (!h->node_inserts || h->ins_call_off.size() != (size_t)h->stat_F + 1) {
+        h->err = "no erasor_process_nodes call with inserts on has completed"; return ERASOR_E_STATE;
+    }
+    *d_xyzi = h->d_ins_call.as<const float>();
+    std::copy(h->ins_call_off.begin(), h->ins_call_off.end(), offsets);
+    return ERASOR_OK;
+}
+
+int erasor_map_append_inserts(erasor_map_t m, erasor_handle_t h) {
+    if (!h) return ERASOR_E_INVALID;
+    if (!m) { h->err = "null map"; return ERASOR_E_INVALID; }
+    if (m->device != h->device) { h->err = "map and handle live on different devices"; return ERASOR_E_INVALID; }
+    CK(cudaSetDevice(h->device));
+    int rc;
+    if ((rc = erasor_wait(h))) return rc;
+    if (!h->node_inserts || h->ins_call_off.size() != (size_t)h->stat_F + 1) {
+        h->err = "no erasor_process_nodes call with inserts on has completed"; return ERASOR_E_STATE;
+    }
+    const size_t n = h->ins_call_off.back();
+    CK(grow_points(m->d_ins, m->n_ins, m->n_ins + n, h->stream));
+    if (n) CK(cudaMemcpyAsync(m->d_ins.as<float4>() + m->n_ins, h->d_ins_call.p(), sizeof(float4) * n, cudaMemcpyDeviceToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    m->n_ins += n;
+    return ERASOR_OK;
+}
+
+int erasor_map_inserts(erasor_map_t m, const float** d_xyzi, size_t* n) {
+    if (!m || !d_xyzi || !n) return ERASOR_E_INVALID;
+    *d_xyzi = m->d_ins.as<const float>();
+    *n = m->n_ins;
+    return ERASOR_OK;
+}
+
+int erasor_map_clear_inserts(erasor_map_t m) {
+    if (!m) return ERASOR_E_INVALID;
+    m->n_ins = 0;
+    return ERASOR_OK;
+}
+
+// node mode's save_static_map: voxelize_preserving_labels(map[keep] ++ the map's inserts, leaf), one erasor_voxelize_batch cloud
+int erasor_save_node_map(erasor_handle_t h, erasor_map_t m, float leaf, const float** d_out, size_t* n_out) {
+    if (!h) return ERASOR_E_INVALID;
+    if (!m || !d_out || !n_out) { h->err = "null argument"; return ERASOR_E_INVALID; }
+    if (m->device != h->device) { h->err = "map and handle live on different devices"; return ERASOR_E_INVALID; }
+    CK(cudaSetDevice(h->device));
+    int rc;
+    if ((rc = erasor_wait(h))) return rc;
+    const size_t n = m->n + m->n_ins;
+    const float* pts = m->d_pts.as<const float>();
+    const uint8_t* keep = m->d_keep.as<const uint8_t>();
+    if (m->n_ins) {
+        CK(h->d_save.ensure(sizeof(float4) * n));
+        CK(h->d_save_keep.ensure(n));
+        CK(cudaMemcpyAsync(h->d_save.p(), m->d_pts.p(), sizeof(float4) * m->n, cudaMemcpyDeviceToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d_save.as<float4>() + m->n, m->d_ins.p(), sizeof(float4) * m->n_ins, cudaMemcpyDeviceToDevice, h->stream));
+        if (m->n) CK(cudaMemcpyAsync(h->d_save_keep.p(), m->d_keep.p(), m->n, cudaMemcpyDeviceToDevice, h->stream));
+        CK(cudaMemsetAsync(h->d_save_keep.as<uint8_t>() + m->n, 1, m->n_ins, h->stream));
+        pts = h->d_save.as<const float>();
+        keep = h->d_save_keep.as<const uint8_t>();
+    }
+    const uint64_t off[2] = {0, n};
+    uint64_t out_off[2] = {0, 0};
+    if ((rc = erasor_voxelize_batch(h, pts, off, 1, keep, leaf, nullptr, ERASOR_PTR_DEVICE, d_out, out_off))) return rc;
+    *n_out = out_off[1];
     return ERASOR_OK;
 }
 

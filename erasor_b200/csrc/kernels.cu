@@ -395,6 +395,20 @@ __device__ __forceinline__ bool srt_is_flagged(const SrtParams& P, uint32_t mc, 
     return (P.version == 3) ? (map_dh > 0.5) : (map_max > P.th_bin_max_h);
 }
 
+// The action k3_srt gives a bin (what r_pod_selected takes from it), without the curr_rejected bit: version 3 -- ACT_FLAG or
+// ACT_MAP (erasor.cpp:493-563); version 2 -- erasor.cpp:346-427, as k3_srt's version-2 pass.
+__device__ __forceinline__ uint8_t srt_action(const SrtParams& P, uint32_t mc, uint32_t qc, uint32_t zmx_m, uint32_t zmn_m, uint32_t zmx_q, uint32_t zmn_q) {
+    if (srt_is_flagged(P, mc, qc, zmx_m, zmn_m, zmx_q, zmn_q)) return ACT_FLAG;
+    if (P.version == 3 || P.minimum_num_pts < 0 || qc < (uint32_t)P.minimum_num_pts) return ACT_MAP;
+    if (qc != 0u && mc != 0u) {
+        const double map_dh  = (double)ordered_to_float(zmx_m) - (double)ordered_to_float(zmn_m);
+        const double curr_dh = (double)ordered_to_float(zmx_q) - (double)ordered_to_float(zmn_q);
+        const double ratio   = std_min_d(map_dh / curr_dh, curr_dh / map_dh);
+        return (ratio < P.scan_ratio_threshold) ? ACT_MAP : ACT_MERGE;
+    }
+    return qc != 0u ? ACT_CURR : (mc != 0u ? ACT_MAP : ACT_NONE);
+}
+
 __global__ void __launch_bounds__(1024)
 k3_srt(SrtParams P, int F, const uint32_t* __restrict__ chunk_range /*[2][F+1]*/, uint32_t* __restrict__ ch_cnt,
        const uint32_t* __restrict__ zmin, const uint32_t* __restrict__ zmax, const uint32_t* __restrict__ frame_off /*[2][F+1]*/,
@@ -1916,9 +1930,9 @@ struct XyziPts {                      // a bin's points as K4b holds them: separ
 };
 
 __global__ void __launch_bounds__(K4B_THREADS)
-k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32_t* __restrict__ n_recs, uint32_t rec_capacity,
-             const uint32_t* __restrict__ cnt /*[2][1][B+1]*/, const uint32_t* __restrict__ dst_start /*[2][1][B+2]*/,
-             const float4* __restrict__ qry_sorted, const float4* __restrict__ part_pts,
+k4b_voxelize(float leaf_f, int B, int F, const FlagRec* __restrict__ recs, const uint32_t* __restrict__ n_recs, uint32_t rec_capacity,
+             const uint32_t* __restrict__ cnt /*[2][F][B+1]*/, const uint32_t* __restrict__ dst_start /*[2][F][B+2]*/,
+             const uint32_t* __restrict__ qry_off /*[F+1]*/, const float4* __restrict__ qry_sorted, const float4* __restrict__ part_pts,
              float4* __restrict__ vox_pts, uint32_t* __restrict__ vox_cnt, uint32_t* __restrict__ vox_start,
              unsigned char* __restrict__ gscratch, uint32_t smem_cap_points) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1929,15 +1943,18 @@ k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32
     __shared__ uint32_t s_tot[256];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t nrec = min(*n_recs, rec_capacity);
-    const uint32_t* cq  = cnt + (B + 1);
-    const uint32_t* dsm = dst_start;
-    const uint32_t* dsq = dst_start + (B + 2);
 
+    // Per record (one frame's flagged bin): its query points start at q0 in the scattered query array, its map points at
+    // src_begin in the scattered map array.  Both grow with (frame, bin) by at least the bin's qc / cm points, so the output
+    // region q0 + src_begin (qc + ng <= qc + cm points) and the scratch region are disjoint between records; one frame (cloud
+    // mode: record w == slot, src_begin == dsm[b]) gives the single-frame layout.
     for (uint32_t w = blockIdx.x; w < nrec; w += gridDim.x) {
         const FlagRec& rc = recs[w];
-        const uint32_t b = rc.bin, qc = cq[b], ng = rc.n_ground_final, n = qc + ng;
-        const uint32_t region = dsq[b] + dsm[b];
-        unsigned char* base = (n <= smem_cap_points) ? smem_raw : (gscratch + k4b_scratch_offset(dsq[b], dsm[b], b));
+        const uint32_t b = rc.bin, f = rc.frame;
+        const uint32_t qc = cnt[((size_t)F + f) * (B + 1) + b], ng = rc.n_ground_final, n = qc + ng;
+        const uint32_t q0 = qry_off[f] + dst_start[((size_t)F + f) * (B + 2) + b];
+        const uint32_t region = q0 + rc.src_begin;
+        unsigned char* base = (n <= smem_cap_points) ? smem_raw : (gscratch + k4b_scratch_offset(q0, rc.src_begin, f * (uint32_t)B + b));
         float*    X   = reinterpret_cast<float*>(base);
         float*    Y   = X + n;
         float*    Z   = Y + n;
@@ -1948,11 +1965,11 @@ k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32
         uint32_t* ORD2 = ORD + n;                 // ... pong of the radix sort
         uint32_t* VK  = ORD2 + n;                 // voxel key per voxel, ascending (<= n entries)
         if (n == 0) {
-            if (tid == 0) { vox_cnt[rc.slot] = 0u; vox_start[rc.slot] = region; }
+            if (tid == 0) { vox_cnt[w] = 0u; vox_start[w] = region; }
             continue;
         }
         for (uint32_t i = tid; i < n; i += K4B_THREADS) {
-            const float4 p = (i < qc) ? qry_sorted[dsq[b] + i] : part_pts[rc.src_begin + (i - qc)];
+            const float4 p = (i < qc) ? qry_sorted[q0 + i] : part_pts[rc.src_begin + (i - qc)];
             X[i] = p.x; Y[i] = p.y; Z[i] = p.z; I[i] = p.w; ORD[i] = i;
         }
         __syncthreads();
@@ -2088,21 +2105,164 @@ k4b_voxelize(float leaf_f, int B, const FlagRec* __restrict__ recs, const uint32
             }
             out[v].w = I[bi];
         }
-        if (tid == 0) { vox_cnt[rc.slot] = nv; vox_start[rc.slot] = region; }
+        if (tid == 0) { vox_cnt[w] = nv; vox_start[w] = region; }
         __syncthreads();
     }
 }
 
-cudaError_t launch_k4b(cudaStream_t st, float leaf, int B, const FlagRec* recs, const uint32_t* n_recs, uint32_t rec_capacity,
-                       const uint32_t* cnt, const uint32_t* dst_start, const float4* qry_sorted, const float4* part_pts,
+cudaError_t launch_k4b(cudaStream_t st, float leaf, int B, int F, const FlagRec* recs, const uint32_t* n_recs, uint32_t rec_capacity,
+                       const uint32_t* cnt, const uint32_t* dst_start, const uint32_t* qry_off, const float4* qry_sorted, const float4* part_pts,
                        float4* vox_pts, uint32_t* vox_cnt, uint32_t* vox_start, unsigned char* gscratch, int grid) {
     constexpr uint32_t SMEM_BYTES = 160 * 1024;     // one CTA per SM (a frame flags a few dozen bins): bins up to ~4500 points stay in shared memory
     // 16 n (xyzi) + 4 n (key) + 4 (n+1) (voxel starts) + 2 x 4 n (point order, ping-pong) + 4 n (voxel keys) = 36 n + 4
     const uint32_t cap = (SMEM_BYTES - 64) / 36u;
     cudaError_t e = ensure_dyn_smem(k4b_voxelize, SMEM_BYTES);
     if (e != cudaSuccess) return e;
-    k4b_voxelize<<<grid, K4B_THREADS, SMEM_BYTES, st>>>(leaf, B, recs, n_recs, rec_capacity, cnt, dst_start, qry_sorted, part_pts,
+    k4b_voxelize<<<grid, K4B_THREADS, SMEM_BYTES, st>>>(leaf, B, F, recs, n_recs, rec_capacity, cnt, dst_start, qry_off, qry_sorted, part_pts,
                                                        vox_pts, vox_cnt, vox_start, gscratch, cap);
+    return cudaGetLastError();
+}
+
+// ============================================================================================
+// Node-mode inserts (DESIGN.md section 8.4): per frame, the query points (and R-GPF ground / K4b voxels) its static estimate puts
+// back into the map, bin by bin in r_pod2pc order, moved body -> origin.
+// ============================================================================================
+// One CTA per frame, after K1: the action of every bin (d_action), the flag slot of every flagged bin (its record is the
+// frame's first record + slot), and the query scatter plan of the bins that insert (ACT_FLAG, ACT_MERGE, ACT_CURR): dense slots
+// in bin order, scatter offsets in the query half of dst_start, and the frame's query-chunk count rows turned into
+// exclusive prefixes -- what k2_scatter_win takes.
+__global__ void __launch_bounds__(1024)
+k_ins_plan(SrtParams P, int F, const uint32_t* __restrict__ chunk_range /*[2][F+1]*/, uint32_t* __restrict__ ch_cnt,
+           const uint32_t* __restrict__ zmin, const uint32_t* __restrict__ zmax, const uint32_t* __restrict__ cnt /*[2][F][B+1]*/,
+           uint8_t* __restrict__ action /*[F][B]*/, uint32_t* __restrict__ flag_slot /*[F][B]*/, uint32_t* __restrict__ ins_slot /*[F][B]*/,
+           uint32_t* __restrict__ n_ins /*[F]*/, uint32_t* __restrict__ dst_start /*[2][F][B+2]*/) {
+    extern __shared__ uint32_t s_sz[];      // B + 1
+    __shared__ uint32_t s_part[34];
+    const int B = P.B, f = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+    const uint32_t* cm = cnt + (size_t)f * (B + 1);
+    const uint32_t* cq = cnt + ((size_t)F + f) * (B + 1);
+    const uint32_t* mnm = zmin + (size_t)f * B; const uint32_t* mxm = zmax + (size_t)f * B;
+    const uint32_t* mnq = zmin + ((size_t)F + f) * B; const uint32_t* mxq = zmax + ((size_t)F + f) * B;
+    uint8_t* act = action + (size_t)f * B;
+    for (int b = tid; b < B; b += nt) act[b] = srt_action(P, cm[b], cq[b], mxm[b], mnm[b], mxq[b], mnq[b]);
+    __syncthreads();
+    auto inserts = [&](int b) { const uint8_t a = act[b]; return a == ACT_FLAG || a == ACT_MERGE || a == ACT_CURR; };
+
+    for (int b = tid; b < B; b += nt) s_sz[b] = act[b] == ACT_FLAG ? 1u : 0u;
+    __syncthreads();
+    block_excl_scan(s_sz, s_sz, B, s_part);
+    for (int b = tid; b < B; b += nt) flag_slot[(size_t)f * B + b] = act[b] == ACT_FLAG ? s_sz[b] : kSkip;
+    __syncthreads();
+    for (int b = tid; b < B; b += nt) s_sz[b] = inserts(b) ? 1u : 0u;
+    __syncthreads();
+    const uint32_t n = block_excl_scan(s_sz, s_sz, B, s_part);
+    for (int b = tid; b < B; b += nt) ins_slot[(size_t)f * B + b] = inserts(b) ? s_sz[b] : kSkip;
+    if (tid == 0) n_ins[f] = n;
+    __syncthreads();
+    for (int b = tid; b <= B; b += nt) s_sz[b] = (b < B && inserts(b)) ? cq[b] : 0u;
+    __syncthreads();
+    const uint32_t tot = block_excl_scan(s_sz, s_sz, B + 1, s_part);
+    uint32_t* dsq = dst_start + ((size_t)F + f) * (B + 2);
+    for (int b = tid; b <= B; b += nt) dsq[b] = (b < B && inserts(b)) ? s_sz[b] : kSkip;
+    if (tid == 0) dsq[B + 1] = tot;
+    const uint32_t c0 = chunk_range[(F + 1) + f], c1 = chunk_range[(F + 1) + f + 1];
+    for (int b = tid; b < B; b += nt) {
+        if (!inserts(b)) continue;
+        uint32_t run = 0;
+        for (uint32_t k = c0; k < c1; ++k) { const uint32_t v = ch_cnt[(size_t)k * (B + 1) + b]; ch_cnt[(size_t)k * (B + 1) + b] = run; run += v; }
+    }
+}
+
+cudaError_t launch_ins_plan(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt, const uint32_t* zmin,
+                            const uint32_t* zmax, const uint32_t* cnt, uint8_t* action, uint32_t* flag_slot, uint32_t* ins_slot, uint32_t* n_ins,
+                            uint32_t* dst_start) {
+    const size_t smem = sizeof(uint32_t) * ((size_t)P.B + 1);
+    cudaError_t e = ensure_dyn_smem(k_ins_plan, smem);
+    if (e != cudaSuccess) return e;
+    k_ins_plan<<<F, 1024, smem, st>>>(P, F, chunk_range, ch_cnt, zmin, zmax, cnt, action, flag_slot, ins_slot, n_ins, dst_start);
+    return cudaGetLastError();
+}
+
+// record index of every frame's first flagged bin (node mode hands each frame a contiguous block of records, in slot order)
+__global__ void k_ins_recs(const FlagRec* __restrict__ recs, const uint32_t* __restrict__ n_recs, uint32_t rec_capacity, uint32_t* __restrict__ frame_rec_base) {
+    const uint32_t n = min(*n_recs, rec_capacity);
+    for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < n; w += gridDim.x * blockDim.x)
+        if (recs[w].slot == 0u) frame_rec_base[recs[w].frame] = w;
+}
+
+// one CTA per frame: points each bin inserts, turned into the bin's offset inside the frame's inserts; the frame's total
+__global__ void __launch_bounds__(1024)
+k_ins_size(int B, int F, int vox, const uint8_t* __restrict__ action, const uint32_t* __restrict__ flag_slot, const uint32_t* __restrict__ frame_rec_base,
+           const FlagRec* __restrict__ recs, const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ vox_cnt /*per record*/,
+           uint32_t* __restrict__ bin_off /*[F][B]*/, uint32_t* __restrict__ frame_cnt /*[F]*/) {
+    __shared__ uint32_t s_part[34];
+    const int f = blockIdx.x;
+    const uint32_t* cq = cnt + ((size_t)F + f) * (B + 1);
+    uint32_t* out = bin_off + (size_t)f * B;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        const uint8_t a = action[(size_t)f * B + b];
+        uint32_t sz = 0;
+        if (a == ACT_FLAG) {
+            const uint32_t w = frame_rec_base[f] + flag_slot[(size_t)f * B + b];
+            sz = vox ? vox_cnt[w] : cq[b] + recs[w].n_ground_final;       // voxelize(bin_curr + ground) or bin_curr + ground
+        } else if (a == ACT_MERGE || a == ACT_CURR) {
+            sz = cq[b];                                                     // bin_curr (the map points of a merged bin stay kept)
+        }
+        out[b] = sz;
+    }
+    __syncthreads();
+    const uint32_t tot = block_excl_scan(out, out, B, s_part);
+    if (threadIdx.x == 0) frame_cnt[f] = tot;
+}
+
+__global__ void __launch_bounds__(1024) k_ins_offsets(const uint32_t* __restrict__ frame_cnt, int F, uint32_t* __restrict__ ins_off /*[F+1]*/) {
+    __shared__ uint32_t s_part[34];
+    const uint32_t tot = block_excl_scan(frame_cnt, ins_off, F, s_part);
+    if (threadIdx.x == 0) ins_off[F] = tot;
+}
+
+// one warp per (frame, bin): the bin's inserts, body -> origin on the way (the updater's body2origin, OfflineMapUpdater.cpp:441-449)
+__global__ void __launch_bounds__(256)
+k_ins_copy(int B, int F, int vox, const uint8_t* __restrict__ action, const uint32_t* __restrict__ flag_slot, const uint32_t* __restrict__ frame_rec_base,
+           const FlagRec* __restrict__ recs, const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ dst_start, const uint32_t* __restrict__ qry_off,
+           const uint32_t* __restrict__ vox_cnt, const uint32_t* __restrict__ vox_start, const float4* __restrict__ qry_sorted,
+           const float4* __restrict__ part_pts, const float4* __restrict__ vox_pts, const float* __restrict__ fwd /*[F][12]*/,
+           const uint32_t* __restrict__ bin_off, const uint32_t* __restrict__ ins_off, float4* __restrict__ out) {
+    const uint32_t lane = threadIdx.x & 31;
+    const size_t nw = ((size_t)gridDim.x * blockDim.x) >> 5;
+    for (size_t j = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < (size_t)F * B; j += nw) {
+        const uint8_t a = action[j];
+        if (a != ACT_FLAG && a != ACT_MERGE && a != ACT_CURR) continue;
+        const uint32_t f = (uint32_t)(j / (size_t)B), b = (uint32_t)(j - (size_t)f * B);
+        const float* T = fwd + 12 * (size_t)f;
+        float4* dst = out + ins_off[f] + bin_off[j];
+        auto copy = [&](const float4* src, uint32_t n, float4* d) { for (uint32_t i = lane; i < n; i += 32) d[i] = pcl_affine(T, src[i]); };
+        const uint32_t qc = cnt[((size_t)F + f) * (B + 1) + b];
+        const float4* q = qry_sorted + qry_off[f] + dst_start[((size_t)F + f) * (B + 2) + b];
+        if (a == ACT_FLAG) {
+            const uint32_t w = frame_rec_base[f] + flag_slot[j];
+            if (vox) {
+                copy(vox_pts + vox_start[w], vox_cnt[w], dst);
+            } else {
+                copy(q, qc, dst);
+                copy(part_pts + recs[w].src_begin, recs[w].n_ground_final, dst + qc);
+            }
+        } else {
+            copy(q, qc, dst);
+        }
+    }
+}
+
+cudaError_t launch_ins_assemble(cudaStream_t st, int B, int F, int vox, const uint8_t* action, const uint32_t* flag_slot, uint32_t* frame_rec_base,
+                                const FlagRec* recs, const uint32_t* n_recs, uint32_t rec_capacity, const uint32_t* cnt, const uint32_t* dst_start,
+                                const uint32_t* qry_off, const uint32_t* vox_cnt, const uint32_t* vox_start, const float4* qry_sorted,
+                                const float4* part_pts, const float4* vox_pts, const float* fwd, uint32_t* bin_off, uint32_t* frame_cnt,
+                                uint32_t* ins_off, float4* out, int sm_count) {
+    k_ins_recs<<<sm_count, 256, 0, st>>>(recs, n_recs, rec_capacity, frame_rec_base);
+    k_ins_size<<<F, 1024, 0, st>>>(B, F, vox, action, flag_slot, frame_rec_base, recs, cnt, vox_cnt, bin_off, frame_cnt);
+    k_ins_offsets<<<1, 1024, 0, st>>>(frame_cnt, F, ins_off);
+    k_ins_copy<<<sm_count * 8, 256, 0, st>>>(B, F, vox, action, flag_slot, frame_rec_base, recs, cnt, dst_start, qry_off, vox_cnt, vox_start,
+                                             qry_sorted, part_pts, vox_pts, fwd, bin_off, ins_off, out);
     return cudaGetLastError();
 }
 

@@ -64,9 +64,23 @@ cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, con
                       float4* part_pts, uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected, unsigned char* gscratch,
                       int sm_count, unsigned long long* fence, const K4Fold& fold, int classes /*bit 0|1: A and B, bit 2: C*/);
 
-cudaError_t launch_k4b(cudaStream_t st, float leaf, int B, const FlagRec* recs, const uint32_t* n_recs, uint32_t rec_capacity,
-                       const uint32_t* cnt, const uint32_t* dst_start, const float4* qry_sorted, const float4* part_pts,
+// every record of the batch (F frames; cnt / dst_start [2][F][...], qry_off: the query half of frame_off); vox_cnt / vox_start
+// per record
+cudaError_t launch_k4b(cudaStream_t st, float leaf, int B, int F, const FlagRec* recs, const uint32_t* n_recs, uint32_t rec_capacity,
+                       const uint32_t* cnt, const uint32_t* dst_start, const uint32_t* qry_off, const float4* qry_sorted, const float4* part_pts,
                        float4* vox_pts, uint32_t* vox_cnt, uint32_t* vox_start, unsigned char* gscratch, int grid);
+
+// node-mode inserts: after K1, the action / flag slot of every (frame, bin) and the query scatter plan of the inserting bins
+cudaError_t launch_ins_plan(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt, const uint32_t* zmin,
+                            const uint32_t* zmax, const uint32_t* cnt, uint8_t* action, uint32_t* flag_slot, uint32_t* ins_slot, uint32_t* n_ins,
+                            uint32_t* dst_start);
+// after R-GPF (and K4b): per-frame sizes and offsets ins_off [F+1], then every frame's inserts into out, body -> origin by fwd [F][12]
+cudaError_t launch_ins_assemble(cudaStream_t st, int B, int F, int vox, const uint8_t* action, const uint32_t* flag_slot, uint32_t* frame_rec_base,
+                                const FlagRec* recs, const uint32_t* n_recs, uint32_t rec_capacity, const uint32_t* cnt, const uint32_t* dst_start,
+                                const uint32_t* qry_off, const uint32_t* vox_cnt, const uint32_t* vox_start, const float4* qry_sorted,
+                                const float4* part_pts, const float4* vox_pts, const float* fwd, uint32_t* bin_off, uint32_t* frame_cnt,
+                                uint32_t* ins_off, float4* out, int sm_count);
+constexpr int kInsAssembleLaunches = 4;
 
 cudaError_t launch_k5(cudaStream_t st, int B, int version, int skip_voxelize, const uint32_t* cnt, const uint32_t* dst_start,
                       const uint8_t* action, const uint32_t* flag_slot, const FlagRec* recs, const uint32_t* n_recs,

@@ -49,12 +49,13 @@ def processed_nodes(nodes: Iterable[Node], removal_interval: int) -> list:
 
 
 def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep, batch: int = 20, save_voxel_size: Optional[float] = None,
-                          prepare: Optional[Callable] = None) -> dict:
+                          prepare: Optional[Callable] = None, inserts: bool = False) -> dict:
     """The frame-independent twin of run_offline: every node callback_node would process is tested against the same initial map
     (node mode, erasor_process_nodes), in batches of `batch` nodes, each batch's raw scans voxelised at query_voxel_size and moved
     to the body frame on the device in one submission (erasor_voxelize_batch); then save_static_map of the kept map.  prepare
-    (optional) replaces the device query preparation: prepare(raw_xyzi, raw_offsets) -> (queries, query_offsets).  Returns
-    run_offline's dict plus "keep", the map's keep mask.  Needs a CUDA device."""
+    (optional) replaces the device query preparation: prepare(raw_xyzi, raw_offsets) -> (queries, query_offsets).  inserts: also
+    put back the query points each node's static estimate holds (node-mode inserts), saved with the kept map in node order.
+    Returns run_offline's dict plus "keep", the map's keep mask.  Needs a CUDA device."""
     from . import capi
     if up.is_large_scale:
         raise ValueError("node mode has no large-scale windowing: use run_offline")
@@ -64,6 +65,7 @@ def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep
     h = capi.Handle(ep.replace(version=up.version))       # /erasor/version as the updater reads it (OfflineMapUpdater.cpp:81)
     try:
         h.attach_map(m)
+        h.set_node_inserts(inserts)
         l2b = np.asarray(up.lidar2body, dtype=np.float64)
         for b0 in range(0, len(sel), int(batch)):
             chunk = sel[b0:b0 + int(batch)]
@@ -76,6 +78,8 @@ def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep
             else:
                 q, qo = prepare(raw, off)
                 h.process_nodes(poses, q, qo, voi_max_range=up.max_range)
+            if inserts:
+                m.append_inserts(h)
         keep = m.get_keep()
         static_map = h.save_static_map(m, up.map_voxel_size if save_voxel_size is None else save_voxel_size)
     finally:
@@ -85,18 +89,22 @@ def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep
 
 
 def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, make_updater: Optional[Callable] = None,
-                 map_leafsize: Optional[float] = None, out_dir: Optional[str] = None, frame_independent: bool = False) -> dict:
+                 map_leafsize: Optional[float] = None, out_dir: Optional[str] = None, frame_independent: bool = False,
+                 inserts: bool = False) -> dict:
     """mapgen -> updater -> evaluation on one node list.  GT for PR/RR = the naive map itself (it carries the labels), which is
     how the reference scores a run (analysis_runner.py compares <seq>_..._original / voxelised map with the result).
-    frame_independent runs node mode (run_frame_independent) on the naive map instead of the sequential updater."""
+    frame_independent runs node mode (run_frame_independent) on the naive map instead of the sequential updater; inserts (node
+    mode only) puts each node's inserted query points back into its static map."""
     nodes = list(nodes)
     leaf = float(up.map_voxel_size if map_leafsize is None else map_leafsize)
     original, naive = mapgen.build_map(nodes, leafsize=leaf, is_large_scale=bool(up.is_large_scale), voxelize=voxelize)
     if frame_independent:
         if make_updater is not None:
             raise ValueError("node mode runs on the device: make_updater does not apply")
-        res = run_frame_independent(nodes, naive, up, ep)
+        res = run_frame_independent(nodes, naive, up, ep, inserts=inserts)
     else:
+        if inserts:
+            raise ValueError("inserts are a node-mode option: the sequential updater always inserts")
         res = run_offline(nodes, naive, up, ep, make_updater=make_updater)
     res["naive_map"] = naive
     if make_updater is None:            # the device updater ran: score on the device too (same counts, same dict)
@@ -141,6 +149,6 @@ def read_bag_nodes(bag_path: str, topic: str = "/node/combined/optimized", keep_
 
 def run_bag(bag: str, config_yaml: str, out_dir: Optional[str] = None, frame_independent: bool = False, **kw) -> dict:
     """A reference bag + a reference config/*.yaml -> naive map, static map and PR/RR: run_sequence on the bag's nodes, with the
-    sequential updater or, with frame_independent, node mode."""
+    sequential updater or, with frame_independent, node mode (inserts=True in kw: with node-mode inserts)."""
     ep, up = params.load_yaml(config_yaml)
     return run_sequence(read_bag_nodes(bag), up, ep, out_dir=out_dir, frame_independent=frame_independent, **kw)

@@ -7,8 +7,9 @@
 // formatted on the device.  One GPU; multi-GPU callers shard the nodes and combine the masks with erasor_comm_*.
 // With a ROS bag of erasor/node messages instead of <data_dir> (a path ending in .bag), the map is the yaml's initial_map_path, the
 // poses are the bag's doubles, and each batch's clouds are decoded from the bag on the device in one call (NodeBag::load_device).
-//   usage: static_map_nodes_main <config.yaml> <data_dir> [init_idx] [batch]
-//          static_map_nodes_main <config.yaml> <file.bag> [init_idx] [batch]
+// inserts = 1 turns node-mode inserts on: the query points each node's static estimate puts back into the map are saved with it.
+//   usage: static_map_nodes_main <config.yaml> <data_dir> [init_idx] [batch] [inserts]
+//          static_map_nodes_main <config.yaml> <file.bag> [init_idx] [batch] [inserts]
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -64,17 +65,19 @@ static std::vector<std::array<double, 7>> load_all_poses(const std::string& txt)
 }
 
 int main(int argc, char** argv) {
-    if (argc < 3) { std::fprintf(stderr, "usage: %s <config.yaml> <data_dir> [init_idx] [batch]\n", argv[0]); return 2; }
+    if (argc < 3) { std::fprintf(stderr, "usage: %s <config.yaml> <data_dir> [init_idx] [batch] [inserts]\n", argv[0]); return 2; }
     try {
         Config cfg = load_config(argv[1]);
         const std::string data_dir = argv[2];
         const int init_idx = argc > 3 ? std::atoi(argv[3]) : 0;
         const int batch = argc > 4 ? std::max(1, std::atoi(argv[4])) : 20;
+        const bool inserts = argc > 5 && std::atoi(argv[5]) != 0;
         if (cfg.updater.is_large_scale) throw std::invalid_argument("node mode has no large-scale windowing: use offline_map_updater_main");
         if (cfg.updater.removal_interval < 1) throw std::invalid_argument("removal_interval must be >= 1");
         erasor_params_t ep = cfg.erasor;
         ep.version = cfg.updater.version;                               // /erasor/version as the updater reads it (:81)
         ERASOR erasor(ep);
+        erasor.set_node_inserts(inserts);
         PcdCodec codec;
         DeviceBuffer map;
         const bool from_bag = is_bag_path(data_dir);

@@ -159,9 +159,14 @@ public:
         std::vector<uint8_t> keep(std::max<size_t>(erasor_map_size(map_), 1));
         check(erasor_process_nodes(h_, poses[0].data(), reinterpret_cast<const float*>(q.data()), qo.data(), static_cast<int>(F), voi_max_range,
                                    nullptr, keep.data(), ERASOR_PTR_HOST));
+        if (inserts_) check(erasor_map_append_inserts(map_, h_));
         keep.resize(erasor_map_size(map_));
         return keep;
     }
+    // Node-mode inserts (DESIGN.md section 8.4): with enable, process_nodes / process_scans also append the query points each node's
+    // static estimate puts back into the map to the map's store, and save_static_map voxelises them with the kept map.
+    void set_node_inserts(bool enable) { check(erasor_set_node_inserts(h_, enable ? 1 : 0)); inserts_ = enable; }
+    void clear_node_inserts() { if (map_ && erasor_map_clear_inserts(map_) != ERASOR_OK) throw std::runtime_error("ERASOR: erasor_map_clear_inserts"); }
     // the same, from a map already in device memory (16-byte aligned float4 per point), e.g. read by PcdCodec::load_device
     void load_global_map_device(const float* d_map_xyzi, size_t n) {
         if (map_) { erasor_attach_map(h_, nullptr); erasor_map_destroy(map_); map_ = nullptr; }
@@ -206,6 +211,7 @@ public:
         const DeviceClouds q = voxelize_batch(raw_xyzi, raw_offsets, static_cast<float>(query_voxel_size), nullptr, lidar2body.data(), ptr_kind);
         check(erasor_process_nodes(h_, poses[0].data(), q.d_xyzi, q.offsets.data(), static_cast<int>(poses.size()), voi_max_range, nullptr, nullptr,
                                    ERASOR_PTR_DEVICE));
+        if (inserts_) check(erasor_map_append_inserts(map_, h_));
     }
     std::vector<uint8_t> process_scans(const std::vector<std::array<double, 7>>& poses, const std::vector<PointCloud>& raw_scans,
                                        double query_voxel_size, const std::array<double, 7>& lidar2body, double voi_max_range = 0.0) {
@@ -217,12 +223,15 @@ public:
         return static_mask();
     }
     // save_static_map of node mode (OfflineMapUpdater.cpp:174-196 without the file): the map load_global_map holds, under its
-    // current keep mask, voxelised at voxel_size -- one cloud, in the handle's device memory (offsets {0, n})
+    // current keep mask, followed by the map's insert store (empty unless inserts are on), voxelised at voxel_size -- one cloud,
+    // in the handle's device memory (offsets {0, n})
     DeviceClouds save_static_map(float voxel_size) {
         if (!map_) throw std::logic_error("ERASOR: load_global_map first");
-        check(erasor_synchronize(h_));
-        const std::vector<uint64_t> off = {0, static_cast<uint64_t>(erasor_map_size(map_))};
-        return voxelize_batch(erasor_map_points_device(map_), off, voxel_size, erasor_map_keep_device(map_), nullptr, ERASOR_PTR_DEVICE);
+        DeviceClouds out;
+        size_t n = 0;
+        check(erasor_save_node_map(h_, map_, voxel_size, &out.d_xyzi, &n));
+        out.offsets = {0, static_cast<uint64_t>(n)};
+        return out;
     }
     // frame-sharded job: every rank processes its own nodes, then ONE all-gather (bit-packed masks over NVLink) + AND gives
     // every rank the job's static mask.  id128 from erasor_comm_unique_id() on rank 0, shipped by the host program.
@@ -259,6 +268,7 @@ private:
     int             device_ = 0;
     erasor_handle_t h_ = nullptr;
     erasor_map_t    map_ = nullptr;
+    bool            inserts_ = false;
 };
 
 }  // namespace erasor_b200

@@ -211,6 +211,27 @@ int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const fl
 /* per-node counters of the last erasor_process_nodes: points inside the VoI (|map_voi_|), flagged bins, rejected points */
 int erasor_get_node_stats(erasor_handle_t h, uint32_t* n_voi_points, uint32_t* n_flagged_bins, uint32_t* n_rejected_points);
 
+/* ---- node-mode inserts: the query points each node's static estimate puts back into the map (DESIGN.md section 8.4) ---- */
+/* Opt-in per handle (default off; off changes nothing).  With it on, erasor_process_nodes also builds, per node f, inserted_f:
+ * bin by bin in r_pod2pc order, the bins whose selected points hold query points -- R-GPF bins: bin_curr then the R-GPF ground
+ * (version 3 without skip_voxelize: voxelize_preserving_labels of that, at map_voxel_size); version 2 also MERGE_BINS bins and
+ * bins with query points only: bin_curr -- moved body -> origin with the node's pose (OfflineMapUpdater.cpp:281-290, 441-449),
+ * intensity carried through.  The masks and counters are those of inserts off.
+ * erasor_set_node_inserts: ERASOR_E_STATE while a submission is pending.  With inserts on, ERASOR_PTR_QUERY_XYZ queries are
+ * refused (ERASOR_E_INVALID: the inserts need the intensity). */
+int erasor_set_node_inserts(erasor_handle_t h, int enable);
+/* after erasor_process_nodes (erasor_wait for the asynchronous form): the last call's inserts, node after node -- *d_xyzi: float4
+ * device memory valid until the handle's next submission; offsets (HOST, n_frames + 1): node f is [offsets[f], offsets[f+1]) */
+int erasor_get_node_inserts(erasor_handle_t h, const float** d_xyzi, uint64_t* offsets);
+/* The map's insert store: erasor_map_append_inserts appends h's last call (synchronous); callers append in node order -- lanes
+ * sharing a map append after their own erasor_wait.  erasor_map_inserts: device pointer and point count; clear empties it. */
+int erasor_map_append_inserts(erasor_map_t m, erasor_handle_t h);
+int erasor_map_inserts(erasor_map_t m, const float** d_xyzi, size_t* n);
+int erasor_map_clear_inserts(erasor_map_t m);
+/* node mode's save_static_map: voxelize_preserving_labels(map[keep] ++ the map's inserts, leaf) through erasor_voxelize_batch
+ * (its output rules and errors); with an empty store, the kept map alone.  Waits for h; *d_out valid until h's next voxelize. */
+int erasor_save_node_map(erasor_handle_t h, erasor_map_t m, float leaf, const float** d_out, size_t* n_out);
+
 /* erasor_utils::voxelize_preserving_labels (erasor_utils.cpp:80-114) of n_clouds clouds in one submission, each on its own
  * pcl::VoxelGrid, optionally followed by one pcl::transformPointCloud.  Cloud c is xyzi[offsets[c] .. offsets[c+1]) (offsets: HOST,
  * n_clouds + 1 entries, offsets[0] = 0); keep (nullable, offsets[n_clouds] bytes) selects the points with keep != 0; xyzi and keep
