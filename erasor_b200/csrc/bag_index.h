@@ -8,6 +8,11 @@
 // 0x05 chunk (its data holds further records), 0x07 connection, 0x02 message data, 0x04 index data, 0x06 chunk info.  The
 // records are walked in file order, chunks included; the index section is checked for structure only.
 //
+// An lz4 chunk (DESIGN.md section 12.2.1) is not walked: its frame descriptor and block table are read (lz4_frame.h), and its
+// messages are the entries (time, offset in the decoded chunk) of the index data records that follow it.  The nodes in it are
+// parsed after the chunks that hold a kept node are decoded, by the same parse_node_core, on the device (or serially by the
+// host build): plan_lz4 lays the decode out, finish_lz4 takes the parsed nodes back.
+//
 // An erasor/node message serialises, in order: header (seq, stamp, frame_id); odom, a Pose of 7 doubles (position x y z, then
 // orientation x y z w); odomCov, 36 doubles; lidar, a PointCloud2 (header; height, width; the field list, each a name string,
 // offset, datatype byte and count; is_bigendian; point_step, row_step; data as a length-prefixed byte array; is_dense);
@@ -26,6 +31,7 @@
 #include <vector>
 
 #include "../../include/erasor_b200.h"
+#include "lz4_frame.h"
 #include "pcd_binary.h"
 
 namespace bag {
@@ -49,7 +55,17 @@ struct Node {
     uint32_t seq;                    // header.seq
     uint64_t stamp_ns;               // the record's time
     double odom[7];
-    Cloud cloud;
+    Cloud cloud;                     // data_off: in the file, or in the decoded chunk when lz >= 0
+    int64_t lz = -1;                 // the LZ4 chunk (Index::lz4) holding the node, else -1
+    uint64_t rec = 0;                // lz >= 0: the index entry's offset of the message record in the decoded chunk
+    uint32_t conn = 0;               // lz >= 0: the index entry's connection
+};
+
+// an LZ4 chunk: the record, its data in the file, its decoded length and its frame's block table
+struct Lz4Chunk {
+    uint64_t rec, data, len;
+    uint32_t size;
+    lz4::Frame frame;
 };
 
 struct Index {
@@ -57,7 +73,131 @@ struct Index {
     std::string md5sum;
     uint64_t chunks = 0, connections = 0, messages = 0, selected = 0, unknown = 0;
     uint64_t total_points = 0, intensity_zero_filled = 0, big_endian = 0;
+    std::vector<Lz4Chunk> lz4;       // every LZ4 chunk of the file, in file order
+    std::vector<uint64_t> pending;   // the nodes in LZ4 chunks, parsed after their chunks are decoded (finish_lz4)
+    int fail_rc = 0;                 // the first node parsed on the host that failed, when it follows a pending one
+    std::string fail_msg;
 };
+
+// ---- the node layout, shared by the host walk and the device parse of nodes in LZ4 chunks ----------------------------------
+// why a message is not an erasor/node (0: it is); a and b carry the numbers the message names
+enum : uint32_t {
+    NF_OK = 0, NF_HEADER, NF_ODOM, NF_ODOMCOV, NF_LIDAR, NF_FIELDS, NF_DATA_PAST, NF_LIDARODOM, NF_IMAGE, NF_GPS,
+    NF_LONGER,                       // a: the bytes past the structure
+    NF_NO_FIELD,                     // a: the slot (x y z), b: 1 when a field of that name exists
+    NF_CAPACITY,                     // 2^31 points or more
+    NF_POINT_PAST,                   // a: the byte the last point reads up to, b: lidar.data's length
+    NF_REC_PAST,                     // (LZ4) the index entry's record runs past the decoded chunk
+    NF_REC_OP,                       // (LZ4) the record there is not a message data record
+    NF_REC_CONN,                     // (LZ4) a: its connection
+    NF_REC_TIME,                     // (LZ4) a: its time in ns
+};
+
+struct Rd {
+    const uint8_t* f;
+    uint64_t pos, end;
+    PCD_HD bool take(uint64_t n) { if (n > end - pos) return false; pos += n; return true; }
+    PCD_HD bool u8(uint8_t& v) { if (end - pos < 1) return false; v = f[pos++]; return true; }
+    PCD_HD bool u32(uint32_t& v) { if (end - pos < 4) return false; v = pcd::le32(f + pos); pos += 4; return true; }
+    PCD_HD bool f64(double& v) {
+        if (end - pos < 8) return false;
+        const uint64_t u = (uint64_t)pcd::le32(f + pos) | (uint64_t)pcd::le32(f + pos + 4) << 32;
+        memcpy(&v, &u, 8);
+        pos += 8;
+        return true;
+    }
+    PCD_HD bool skip_str() { uint32_t n; return u32(n) && take(n); }
+    PCD_HD bool header(uint32_t* seq) { uint32_t s, t0, t1; if (!u32(s) || !u32(t0) || !u32(t1) || !skip_str()) return false; if (seq) *seq = s; return true; }
+};
+
+// The erasor/node message f[d0, end): seq, odom and the cloud layout (data_off from f), or the first broken rule.  Only the
+// rules; detail::parse_node turns a code back into its message.
+PCD_HD uint32_t parse_node_core(const uint8_t* f, uint64_t d0, uint64_t end, uint32_t* seq, double odom[7], Cloud& cl, uint64_t* a, uint64_t* b) {
+    Rd c{f, d0, end};
+    if (!c.header(seq)) return NF_HEADER;
+    for (int i = 0; i < 7; ++i) if (!c.f64(odom[i])) return NF_ODOM;
+    if (!c.take(36 * 8)) return NF_ODOMCOV;
+    cl = Cloud{};
+    uint32_t nf;
+    if (!c.header(nullptr) || !c.u32(cl.height) || !c.u32(cl.width) || !c.u32(nf)) return NF_LIDAR;
+    bool taken[4] = {false, false, false, false}, named[4] = {false, false, false, false};
+    const char* kNames[4] = {"x", "y", "z", "intensity"};
+    for (uint32_t j = 0; j < nf; ++j) {
+        uint32_t len, off, count;
+        uint8_t dt;
+        if (!c.u32(len) || len > c.end - c.pos) return NF_FIELDS;
+        const uint8_t* name = f + c.pos;
+        c.pos += len;
+        if (!c.u32(off) || !c.u8(dt) || !c.u32(count)) return NF_FIELDS;
+        for (int s = 0; s < 4; ++s) {
+            uint32_t k = 0;
+            while (kNames[s][k] && k < len && (uint8_t)kNames[s][k] == name[k]) ++k;
+            if (kNames[s][k] || k != len) continue;
+            named[s] = true;
+            if (!taken[s] && dt == kFloat32 && count <= 1) { taken[s] = true; cl.off[s] = off; cl.fields |= 1u << s; }
+        }
+    }
+    uint8_t be, dense;
+    uint32_t dlen;
+    if (!c.u8(be) || !c.u32(cl.point_step) || !c.u32(cl.row_step) || !c.u32(dlen)) return NF_LIDAR;
+    cl.big_endian = be ? 1u : 0u;
+    cl.data_off = c.pos;
+    cl.data_len = dlen;
+    if (!c.take(dlen)) return NF_DATA_PAST;
+    if (!c.u8(dense)) return NF_LIDAR;
+    for (int i = 0; i < 7; ++i) { double d; if (!c.f64(d)) return NF_LIDARODOM; }
+    if (!c.header(nullptr) || !c.skip_str() || !c.skip_str()) return NF_IMAGE;
+    uint8_t st, ct;                  // gps: status (int8 status + uint16 service), latitude .. covariance, covariance type
+    if (!c.header(nullptr) || !c.u8(st) || !c.take(2) || !c.take(3 * 8 + 9 * 8) || !c.u8(ct)) return NF_GPS;
+    if (c.pos != c.end) { *a = c.end - c.pos; return NF_LONGER; }
+    for (int s = 0; s < 3; ++s)
+        if (!(cl.fields >> s & 1u)) { *a = s; *b = named[s] ? 1 : 0; return NF_NO_FIELD; }
+    const uint64_t n = (uint64_t)cl.width * cl.height;
+    if (n >= kMaxCloudPoints) return NF_CAPACITY;
+    if (n) {
+        uint64_t hi = 0;             // in 64 bits: once this check passes, point_reach's 32-bit sum cannot wrap (data_len < 2^32)
+        for (int s = 0; s < 4; ++s)
+            if (cl.fields >> s & 1u) hi = hi > (uint64_t)cl.off[s] + 4u ? hi : (uint64_t)cl.off[s] + 4u;
+        const uint64_t last = (uint64_t)(cl.height - 1) * cl.row_step + (uint64_t)(cl.width - 1) * cl.point_step;
+        if (last + hi > cl.data_len) { *a = last + hi; *b = cl.data_len; return NF_POINT_PAST; }
+    }
+    return NF_OK;
+}
+
+// The message data record at offset `off` of a decoded chunk f[0, len) that an index entry (conn, time_ns) points to: [*d0, *d1)
+// its data, or the broken rule
+PCD_HD uint32_t record_core(const uint8_t* f, uint64_t len, uint64_t off, uint32_t conn, uint64_t time_ns, uint64_t* d0, uint64_t* d1, uint64_t* a) {
+    if (off > len || len - off < 4) return NF_REC_PAST;
+    const uint32_t hl = pcd::le32(f + off);
+    const uint64_t h0 = off + 4, h1 = h0 + hl;
+    if (hl > len - h0 || len - h1 < 4) return NF_REC_PAST;
+    const uint32_t dl = pcd::le32(f + h1);
+    if (dl > len - h1 - 4) return NF_REC_PAST;
+    int have = 0;
+    uint32_t c = 0;
+    uint64_t t = 0;
+    for (uint64_t p = h0; p < h1;) {
+        if (h1 - p < 4) return NF_REC_OP;
+        const uint32_t n = pcd::le32(f + p);
+        if (n > h1 - p - 4) return NF_REC_OP;
+        const uint8_t* s = f + p + 4;
+        uint32_t k = 0;
+        while (k < n && s[k] != '=') ++k;
+        if (k == n) return NF_REC_OP;
+        const uint8_t* v = s + k + 1;
+        const uint32_t vl = n - k - 1;
+        if (k == 2 && s[0] == 'o' && s[1] == 'p' && vl == 1 && v[0] == OP_MSG) have |= 1;
+        if (k == 4 && s[0] == 'c' && s[1] == 'o' && s[2] == 'n' && s[3] == 'n' && vl == 4) { c = pcd::le32(v); have |= 2; }
+        if (k == 4 && s[0] == 't' && s[1] == 'i' && s[2] == 'm' && s[3] == 'e' && vl == 8) { t = (uint64_t)pcd::le32(v) * 1000000000ull + pcd::le32(v + 4); have |= 4; }
+        p += 4ull + n;
+    }
+    if (have != 7) return NF_REC_OP;
+    if (c != conn) { *a = c; return NF_REC_CONN; }
+    if (t != time_ns) { *a = t; return NF_REC_TIME; }
+    *d0 = h1 + 4;
+    *d1 = h1 + 4 + dl;
+    return NF_OK;
+}
 
 PCD_HD uint64_t cloud_points(const Cloud& c) { return (uint64_t)c.width * c.height; }
 
@@ -92,24 +232,6 @@ struct Err {
 inline uint32_t rd32(const uint8_t* p) { uint32_t v; std::memcpy(&v, p, 4); return v; }
 inline uint64_t rd64(const uint8_t* p) { uint64_t v; std::memcpy(&v, p, 8); return v; }
 inline std::string at(uint64_t pos) { return " at byte " + std::to_string(pos); }
-
-// a bounded reader over [pos, end) of the file
-struct Cur {
-    const uint8_t* f;
-    uint64_t pos, end;
-    bool take(uint64_t n) { if (n > end - pos) return false; pos += n; return true; }
-    bool u8(uint8_t& v) { if (end - pos < 1) return false; v = f[pos++]; return true; }
-    bool u32(uint32_t& v) { if (end - pos < 4) return false; v = rd32(f + pos); pos += 4; return true; }
-    bool f64(double& v) { if (end - pos < 8) return false; std::memcpy(&v, f + pos, 8); pos += 8; return true; }
-    bool str(std::string& s) {
-        uint32_t n;
-        if (!u32(n) || n > end - pos) return false;
-        s.assign(reinterpret_cast<const char*>(f + pos), n);
-        pos += n;
-        return true;
-    }
-    bool skip_str() { uint32_t n; return u32(n) && take(n); }
-};
 
 // header fields (name -> [value offset, length]) of the field block [pos, end)
 struct Field { std::string name; uint64_t off, len; };
@@ -147,7 +269,8 @@ inline const Field* need(const std::vector<Field>& fs, const char* name, uint64_
 }
 
 struct Conn { std::string topic, type, md5sum; bool defined = false; };
-struct Msg { uint32_t conn; uint64_t time_ns, rec, data, len; };
+// a message: its record and data in the file; or (lz >= 0) an index entry of LZ4 chunk lz, rec its offset in the decoded chunk
+struct Msg { uint32_t conn; uint64_t time_ns, rec, data, len; int64_t lz = -1; };
 
 struct Walk {
     const uint8_t* f;
@@ -155,7 +278,23 @@ struct Walk {
     std::vector<uint32_t> conn_ids;   // ids seen, in first-definition order
     std::vector<Msg> msgs;
     uint64_t chunks = 0, unknown = 0;
+    std::vector<Lz4Chunk> lz4;
+    std::vector<Msg> entries;         // the index entries of the last LZ4 chunk, while its index data records follow it
     Err e;
+
+    // the last LZ4 chunk's messages, from the index data records that followed it: in file order, by offset in the chunk
+    bool close_lz4() {
+        if (!open) return true;
+        if (entries.empty())
+            return e.set(ERASOR_E_UNSUPPORTED, "chunk" + at(lz4.back().rec) + " is lz4-compressed and no index data record follows it: "
+                                                   "an unindexed bag is not read");
+        std::stable_sort(entries.begin(), entries.end(), [](const Msg& a, const Msg& b) { return a.rec < b.rec; });
+        msgs.insert(msgs.end(), entries.begin(), entries.end());
+        entries.clear();
+        open = false;
+        return true;
+    }
+    bool open = false;                // an LZ4 chunk was the last chunk and its index data records are being read
 
     Conn& conn(uint32_t id) {
         if (id >= conns.size()) conns.resize((size_t)id + 1);
@@ -196,9 +335,20 @@ struct Walk {
             const Field* c = need(fs, "compression", 0, rec, "chunk", e);
             const Field* s = c ? need(fs, "size", 4, rec, "chunk", e) : nullptr;
             if (!s) return false;
+            if (!close_lz4()) return false;
             const std::string comp(reinterpret_cast<const char*>(f + c->off), c->len);
+            if (comp == "lz4") {
+                Lz4Chunk k{rec, d0, dl, rd32(f + s->off), lz4::Frame()};
+                std::string m;
+                const int fr = lz4::parse_frame(f + d0, dl, k.size, k.frame, m);
+                if (fr != lz4::F_OK) return e.set(fr == lz4::F_UNSUPPORTED ? ERASOR_E_UNSUPPORTED : ERASOR_E_INVALID, "lz4 chunk" + at(rec) + ": " + m);
+                ++chunks;
+                lz4.push_back(std::move(k));
+                open = true;
+                return true;
+            }
             if (comp != "none")
-                return e.set(ERASOR_E_UNSUPPORTED, "chunk" + at(rec) + " is compressed with '" + comp + "': only uncompressed chunks are read");
+                return e.set(ERASOR_E_UNSUPPORTED, "chunk" + at(rec) + " is compressed with '" + comp + "': only uncompressed and lz4 chunks are read");
             if (rd32(f + s->off) != dl)
                 return e.set(ERASOR_E_INVALID, "chunk" + at(rec) + " holds " + std::to_string(dl) + " bytes of data, its 'size' says " +
                                                    std::to_string(rd32(f + s->off)));
@@ -238,6 +388,12 @@ struct Walk {
             if ((uint64_t)rd32(f + c->off) * 12u != dl)
                 return e.set(ERASOR_E_INVALID, "index data record" + at(rec) + ": " + std::to_string(dl) + " bytes of data for " +
                                                    std::to_string(rd32(f + c->off)) + " entries of 12");
+            if (open && !in_chunk) {
+                const Field* cn = find(fs, "conn");
+                for (uint64_t q = d0; q < d0 + dl; q += 12)
+                    entries.push_back(Msg{rd32(f + cn->off), (uint64_t)rd32(f + q) * 1000000000ull + rd32(f + q + 4), rd32(f + q + 8), 0, 0,
+                                          (int64_t)lz4.size() - 1});
+            }
             return true;
         }
         case OP_CHUNK_INFO: {
@@ -257,70 +413,42 @@ struct Walk {
     }
 };
 
-// a std_msgs/Header: seq, stamp, frame_id
-inline bool skip_header(Cur& c, uint32_t* seq) {
-    uint32_t s, t0, t1;
-    if (!c.u32(s) || !c.u32(t0) || !c.u32(t1) || !c.skip_str()) return false;
-    if (seq) *seq = s;
-    return true;
+// the message of a parse_node_core / record_core code for the node `who`; false with e set (true for NF_OK)
+inline bool node_fail(uint32_t code, uint64_t a, uint64_t b, const std::string& who, Err& e) {
+    static const char* kNames[4] = {"x", "y", "z", "intensity"};
+    auto bad = [&](const std::string& what) { return e.set(ERASOR_E_INVALID, who + ": " + what); };
+    switch (code) {
+    case NF_OK: return true;
+    case NF_HEADER: return bad("the message ends inside its header");
+    case NF_ODOM: return bad("the message ends inside odom");
+    case NF_ODOMCOV: return bad("the message ends inside odomCov");
+    case NF_LIDAR: return bad("the message ends inside lidar");
+    case NF_FIELDS: return bad("the message ends inside lidar.fields");
+    case NF_DATA_PAST: return bad("lidar.data runs past the message");
+    case NF_LIDARODOM: return bad("the message ends inside lidarOdom");
+    case NF_IMAGE: return bad("the message ends inside image");
+    case NF_GPS: return bad("the message ends inside gps");
+    case NF_LONGER: return bad("the message is " + std::to_string(a) + " bytes longer than an erasor/node");
+    case NF_NO_FIELD:
+        return e.set(ERASOR_E_UNSUPPORTED, who + ": lidar has no field '" + kNames[a] + (b ? "' of datatype FLOAT32 and count 1" : "'"));
+    case NF_CAPACITY: return e.set(ERASOR_E_CAPACITY, who + ": a cloud of 2^31 points or more");
+    case NF_POINT_PAST:
+        return bad("its last point reads up to byte " + std::to_string(a) + " of lidar.data, which holds " + std::to_string(b));
+    case NF_REC_PAST: return bad("the index entry's record runs past the decoded chunk");
+    case NF_REC_OP: return bad("the index entry does not point to a message data record");
+    case NF_REC_CONN: return bad("the record there is on connection " + std::to_string(a) + ", not the index entry's");
+    case NF_REC_TIME: return bad("the record there has time " + std::to_string(a) + " ns, not the index entry's");
+    default: return bad("unknown node error");
+    }
 }
 
 // one erasor/node message -> node; false with e set when it is malformed or its cloud cannot be decoded
 inline bool parse_node(const uint8_t* f, const Msg& m, uint64_t k, Node& nd, Err& e, uint64_t& zero_filled) {
-    const std::string who = "node " + std::to_string(k) + " (message record" + at(m.rec) + ")";
-    Cur c{f, m.data, m.data + m.len};
-    auto bad = [&](const char* what) { return e.set(ERASOR_E_INVALID, who + ": " + what); };
     nd.stamp_ns = m.time_ns;
-    if (!skip_header(c, &nd.seq)) return bad("the message ends inside its header");
-    for (int i = 0; i < 7; ++i) if (!c.f64(nd.odom[i])) return bad("the message ends inside odom");
-    if (!c.take(36 * 8)) return bad("the message ends inside odomCov");
-    // lidar: sensor_msgs/PointCloud2
-    Cloud& cl = nd.cloud;
-    cl = Cloud{};
-    uint32_t nf;
-    if (!skip_header(c, nullptr) || !c.u32(cl.height) || !c.u32(cl.width) || !c.u32(nf)) return bad("the message ends inside lidar");
-    int slot_field[4] = {-1, -1, -1, -1};
-    bool named[4] = {false, false, false, false};
-    static const char* kNames[4] = {"x", "y", "z", "intensity"};
-    for (uint32_t j = 0; j < nf; ++j) {
-        std::string name;
-        uint32_t off, count;
-        uint8_t dt;
-        if (!c.str(name) || !c.u32(off) || !c.u8(dt) || !c.u32(count)) return bad("the message ends inside lidar.fields");
-        for (int s = 0; s < 4; ++s) {
-            if (name != kNames[s]) continue;
-            named[s] = true;
-            if (slot_field[s] < 0 && dt == kFloat32 && count <= 1) { slot_field[s] = (int)j; cl.off[s] = off; cl.fields |= 1u << s; }
-        }
-    }
-    uint8_t be, dense;
-    uint32_t dlen;
-    if (!c.u8(be) || !c.u32(cl.point_step) || !c.u32(cl.row_step) || !c.u32(dlen)) return bad("the message ends inside lidar");
-    cl.big_endian = be ? 1u : 0u;
-    cl.data_off = c.pos;
-    cl.data_len = dlen;
-    if (!c.take(dlen)) return bad("lidar.data runs past the message");
-    if (!c.u8(dense)) return bad("the message ends inside lidar");
-    for (int i = 0; i < 7; ++i) { double d; if (!c.f64(d)) return bad("the message ends inside lidarOdom"); }
-    if (!skip_header(c, nullptr) || !c.skip_str() || !c.skip_str()) return bad("the message ends inside image");
-    uint8_t st, ct;                  // gps: status (int8 status + uint16 service), latitude .. covariance, covariance type
-    if (!skip_header(c, nullptr) || !c.u8(st) || !c.take(2) || !c.take(3 * 8 + 9 * 8) || !c.u8(ct)) return bad("the message ends inside gps");
-    if (c.pos != c.end) return e.set(ERASOR_E_INVALID, who + ": the message is " + std::to_string(c.end - c.pos) + " bytes longer than an erasor/node");
-    for (int s = 0; s < 3; ++s)
-        if (!(cl.fields >> s & 1u))
-            return e.set(ERASOR_E_UNSUPPORTED, who + ": lidar has no field '" + kNames[s] + (named[s] ? "' of datatype FLOAT32 and count 1" : "'"));
-    if (!(cl.fields & 8u)) ++zero_filled;
-    const uint64_t n = cloud_points(cl);
-    if (n >= kMaxCloudPoints) return e.set(ERASOR_E_CAPACITY, who + ": a cloud of 2^31 points or more");
-    if (n) {
-        uint64_t hi = 0;             // in 64 bits: once this check passes, point_reach's 32-bit sum cannot wrap (data_len < 2^32)
-        for (int s = 0; s < 4; ++s)
-            if (cl.fields >> s & 1u) hi = std::max<uint64_t>(hi, (uint64_t)cl.off[s] + 4u);
-        const uint64_t last = (uint64_t)(cl.height - 1) * cl.row_step + (uint64_t)(cl.width - 1) * cl.point_step;
-        if (last + hi > cl.data_len)
-            return e.set(ERASOR_E_INVALID, who + ": its last point reads up to byte " + std::to_string(last + hi) + " of lidar.data, which holds " +
-                                               std::to_string(cl.data_len));
-    }
+    uint64_t a = 0, b = 0;
+    const uint32_t code = parse_node_core(f, m.data, m.data + m.len, &nd.seq, nd.odom, nd.cloud, &a, &b);
+    if (!node_fail(code, a, b, "node " + std::to_string(k) + " (message record" + at(m.rec) + ")", e)) return false;
+    if (!(nd.cloud.fields & 8u)) ++zero_filled;
     return true;
 }
 
@@ -338,7 +466,8 @@ inline int build_index(const uint8_t* file, uint64_t len, const std::string& top
         return ERASOR_E_UNSUPPORTED;
     }
     detail::Walk w{file};
-    if (!w.records(13, len, false)) { msg = w.e.msg; return w.e.rc; }
+    if (!w.records(13, len, false) || !w.close_lz4()) { msg = w.e.msg; return w.e.rc; }
+    out.lz4 = std::move(w.lz4);
     out.chunks = w.chunks;
     out.unknown = w.unknown;
     out.connections = w.conn_ids.size();
@@ -364,9 +493,143 @@ inline int build_index(const uint8_t* file, uint64_t len, const std::string& top
     detail::Err e;
     for (size_t k = first; k < sel.size(); ++k) {
         Node& nd = out.nodes[k - first];
-        if (!detail::parse_node(file, sel[k], k - first, nd, e, out.intensity_zero_filled)) { msg = e.msg; const int rc = e.rc; out.nodes.clear(); return rc; }
+        if (sel[k].lz >= 0) {                         // parsed once its chunk is decoded (finish_lz4)
+            nd.lz = sel[k].lz;
+            nd.rec = sel[k].rec;
+            nd.conn = sel[k].conn;
+            nd.stamp_ns = sel[k].time_ns;
+            out.pending.push_back(k - first);
+            continue;
+        }
+        if (!detail::parse_node(file, sel[k], k - first, nd, e, out.intensity_zero_filled)) {
+            if (!out.pending.empty()) { out.fail_rc = e.rc; out.fail_msg = e.msg; out.nodes.resize(k - first + 1); break; }
+            msg = e.msg; const int rc = e.rc; out.nodes.clear(); return rc;
+        }
         out.total_points += cloud_points(nd.cloud);
         out.big_endian += nd.cloud.big_endian;
+    }
+    return ERASOR_OK;
+}
+
+// ---- nodes in LZ4 chunks: what the device (or the host build, serially) decodes and parses ---------------------------------
+// A block of the decode, a chunk, and a node to parse, as the kernels read them
+struct Lz4Block {
+    uint64_t src;                    // its data in the device copy of the compressed chunks
+    uint32_t csize, stored, cap;     // cap: the frame's block max
+    uint32_t chunk;                  // its chunk in Lz4Plan::chunks
+    uint32_t has_sum, sum;
+};
+struct Lz4ChunkDesc {
+    uint64_t src, dec;               // its compressed data in the device copy, its decoded data in the decoded buffer
+    uint32_t size, block0, nblocks, has_sum, sum, pad_;
+};
+struct Lz4NodeIn { uint64_t dec, len, rec, time_ns; uint32_t conn, pad_; };   // the decoded chunk [dec, dec + len), the index entry
+struct NodeOut {
+    uint32_t code, seq;
+    uint64_t a, b;
+    double odom[7];
+    Cloud cloud;
+};
+
+struct Lz4Plan {
+    std::vector<uint32_t> chunks;    // Index::lz4 ids holding a kept node, in file order
+    std::vector<Lz4ChunkDesc> cd;
+    std::vector<Lz4Block> blocks;
+    std::vector<Lz4NodeIn> nodes;    // Index::pending, in order
+    std::vector<int64_t> slot;       // Index::lz4 id -> its entry of chunks / cd, or -1
+    uint64_t src_bytes = 0, dec_bytes = 0, stored = 0, block_sums = 0, content_sums = 0;
+};
+
+// where node nd (in an LZ4 chunk) has its decoded chunk in the decoded buffer
+inline uint64_t dec_of(const Lz4Plan& p, const Node& nd) { return p.cd[p.slot[nd.lz]].dec; }
+
+inline void fill_lz4_stats(const Index& x, const Lz4Plan& p, erasor_bag_lz4_stats_t& s) {
+    s = erasor_bag_lz4_stats_t{};
+    s.chunks = x.lz4.size();
+    s.decoded_chunks = p.chunks.size();
+    for (uint32_t c : p.chunks) { s.compressed_bytes += x.lz4[c].len; s.decoded_bytes += x.lz4[c].size; }
+    s.blocks = p.blocks.size();
+    s.stored_blocks = p.stored;
+    s.block_checksums = p.block_sums;
+    s.content_checksums = p.content_sums;
+}
+
+// the decode error key: the first broken rule in (block, byte) order wins an atomicMin
+// unit: the position in file order of what broke, counting each decoded chunk's blocks, then one unit for the chunk as a whole
+// (its decoded length and content checksum); block b of chunk c is unit b + c, chunk c's own unit block0 + nblocks + c, so a
+// chunk without blocks still has a unit of its own
+PCD_HD uint64_t err_key(uint64_t unit, uint32_t byte, uint32_t reason) { return unit << 28 | (uint64_t)(byte & 0x7FFFFFu) << 5 | reason; }
+PCD_HD uint64_t block_key(const Lz4Block& B, uint64_t b, uint32_t byte, uint32_t reason) { return err_key(b + B.chunk, byte, reason); }
+PCD_HD uint64_t chunk_key(const Lz4ChunkDesc& d, uint64_t c, uint32_t reason) {
+    return err_key((uint64_t)d.block0 + d.nblocks + c, reason == lz4::R_SIZE ? 0 : 1, reason);    // a short frame before its checksum
+}
+
+inline void plan_lz4(const Index& x, Lz4Plan& p) {
+    p = Lz4Plan();
+    std::vector<int64_t>& slot = p.slot;
+    slot.assign(x.lz4.size(), -1);
+    for (uint64_t k : x.pending) slot[x.nodes[k].lz] = 0;
+    for (size_t c = 0; c < x.lz4.size(); ++c) {
+        if (slot[c] < 0) continue;
+        slot[c] = (int64_t)p.chunks.size();
+        p.chunks.push_back((uint32_t)c);
+        const Lz4Chunk& k = x.lz4[c];
+        Lz4ChunkDesc d{p.src_bytes, p.dec_bytes, k.size, (uint32_t)p.blocks.size(), (uint32_t)k.frame.blocks.size(), k.frame.content_sum, k.frame.sum, 0};
+        for (const lz4::Block& b : k.frame.blocks) {
+            p.blocks.push_back(Lz4Block{d.src + b.off, b.csize, b.stored, k.frame.block_max, (uint32_t)(p.cd.size()), k.frame.block_sums, b.sum});
+            p.stored += b.stored;
+            p.block_sums += k.frame.block_sums;
+        }
+        p.content_sums += k.frame.content_sum;
+        p.cd.push_back(d);
+        p.src_bytes += (k.len + 15) & ~15ull;
+        p.dec_bytes += ((uint64_t)k.size + 15) & ~15ull;
+    }
+    for (uint64_t k : x.pending) {
+        const Node& nd = x.nodes[k];
+        const Lz4ChunkDesc& d = p.cd[slot[nd.lz]];
+        p.nodes.push_back(Lz4NodeIn{d.dec, d.size, nd.rec, nd.stamp_ns, nd.conn, 0});
+    }
+}
+
+// the message of a decode error key
+inline std::string lz4_error(const Index& x, const Lz4Plan& p, uint64_t key) {
+    const uint64_t u = key >> 28;
+    const uint32_t byte = (uint32_t)(key >> 5) & 0x7FFFFFu, r = (uint32_t)key & 31u;
+    size_t c = 0;                                    // the chunk whose units [block0 + c, block0 + c + nblocks] hold u
+    while (c + 1 < p.cd.size() && (uint64_t)p.cd[c + 1].block0 + c + 1 <= u) ++c;
+    const Lz4Chunk& k = x.lz4[p.chunks[c]];
+    const uint64_t blk = u - p.cd[c].block0 - c;     // == nblocks: the chunk as a whole
+    const std::string m = "lz4 chunk" + detail::at(k.rec) + ": ";
+    if (r == lz4::R_SIZE) return m + "its frame does not decode to the chunk's 'size' of " + std::to_string(k.size) + " bytes";
+    if (r == lz4::R_CONTENT_SUM) return m + "the content checksum does not match";
+    if (r == lz4::R_BLOCK_SUM) return m + "block " + std::to_string(blk) + ": the block checksum does not match";
+    return m + "malformed block " + std::to_string(blk) + ": " + lz4::reason_text(r) + " (byte " + std::to_string(k.frame.blocks[blk].off + byte) +
+           " of the frame)";
+}
+
+// The nodes of x.pending from their parse (res, in x.pending's order), then the first failure in delivery order: ERASOR_OK or an
+// error code with msg (the index is then cleared)
+inline int finish_lz4(Index& x, const NodeOut* res, std::string& msg) {
+    detail::Err e;
+    for (size_t i = 0; i < x.pending.size() && e.rc == ERASOR_OK; ++i) {
+        const uint64_t k = x.pending[i];
+        Node& nd = x.nodes[k];
+        const NodeOut& r = res[i];
+        const std::string who = "node " + std::to_string(k) + " (message record at byte " + std::to_string(nd.rec) + " of lz4 chunk" +
+                                detail::at(x.lz4[nd.lz].rec) + ")";
+        if (!detail::node_fail(r.code, r.a, r.b, who, e)) break;
+        nd.seq = r.seq;
+        std::memcpy(nd.odom, r.odom, sizeof(nd.odom));
+        nd.cloud = r.cloud;
+    }
+    if (e.rc == ERASOR_OK && x.fail_rc) e.set(x.fail_rc, x.fail_msg);
+    if (e.rc != ERASOR_OK) { msg = e.msg; x.nodes.clear(); return e.rc; }
+    for (uint64_t k : x.pending) {
+        const Cloud& c = x.nodes[k].cloud;
+        x.total_points += cloud_points(c);
+        x.big_endian += c.big_endian;
+        x.intensity_zero_filled += (c.fields & 8u) ? 0 : 1;
     }
     return ERASOR_OK;
 }

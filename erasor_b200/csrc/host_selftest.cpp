@@ -240,6 +240,62 @@ int erasor_hostcheck_lzf_decode(const uint8_t* s, uint64_t csize, uint8_t* out, 
 
 // ---- erasor/node bags: bag_index.h's index, and its per-point decode run serially (what erasor_bag_load's gather computes) ----
 static bag::Index g_bag;
+static bag::Lz4Plan g_plan;
+static std::vector<uint8_t> g_dec;                   // the decoded LZ4 chunks, laid out as the device's decoded buffer
+
+// The stages of erasor_bag_index's LZ4 decode and node parse (pcd_kernels.cu), serially: the key of the first broken rule or ~0;
+// res gets one NodeOut per pending node
+static uint64_t lz4_stages(const uint8_t* file, const bag::Index& x, const bag::Lz4Plan& p, std::vector<uint8_t>& dec, std::vector<bag::NodeOut>& res) {
+    std::vector<uint8_t> src(std::max<uint64_t>(p.src_bytes, 1));
+    for (size_t c = 0; c < p.chunks.size(); ++c) {
+        const bag::Lz4Chunk& k = x.lz4[p.chunks[c]];
+        std::memcpy(src.data() + p.cd[c].src, file + k.data, k.len);
+    }
+    dec.assign(std::max<uint64_t>(p.dec_bytes, 1), 0);
+    uint64_t err = ~0ull;
+    const size_t nb = p.blocks.size();
+    std::vector<uint32_t> bsize(nb, 0);
+    std::vector<uint64_t> boff(nb, ~0ull);
+    for (size_t b = 0; b < nb; ++b) {                 // k_lz4_size
+        const bag::Lz4Block& B = p.blocks[b];
+        uint32_t o = B.csize, at = 0, r = lz4::R_OK;
+        if (!B.stored) r = lz4::block(lz4::Serial{}, src.data() + B.src, B.csize, nullptr, B.cap, &o, &at);
+        if (r != lz4::R_OK) err = std::min(err, bag::block_key(B, b, at, r));
+        bsize[b] = r == lz4::R_OK ? o : 0;
+    }
+    for (size_t c = 0; c < p.cd.size(); ++c) {       // k_lz4_place
+        const bag::Lz4ChunkDesc& d = p.cd[c];
+        uint64_t s = 0;
+        for (uint32_t b = d.block0; b < d.block0 + d.nblocks; ++b) s += bsize[b];
+        if (s != d.size) { err = std::min(err, bag::chunk_key(d, c, lz4::R_SIZE)); continue; }
+        s = 0;
+        for (uint32_t b = d.block0; b < d.block0 + d.nblocks; ++b) { boff[b] = d.dec + s; s += bsize[b]; }
+    }
+    for (size_t b = 0; b < nb; ++b) {                 // k_lz4_decode
+        const bag::Lz4Block& B = p.blocks[b];
+        if (boff[b] == ~0ull) continue;
+        uint32_t o = 0, at = 0;
+        if (B.stored) std::memcpy(dec.data() + boff[b], src.data() + B.src, B.csize);
+        else lz4::block(lz4::Serial{}, src.data() + B.src, B.csize, dec.data() + boff[b], bsize[b], &o, &at);
+    }
+    for (size_t b = 0; b < nb; ++b) {                 // k_lz4_sums
+        const bag::Lz4Block& B = p.blocks[b];
+        if (B.has_sum && lz4::xxh32(src.data() + B.src, B.csize, 0) != B.sum) err = std::min(err, bag::block_key(B, b, B.csize, lz4::R_BLOCK_SUM));
+    }
+    for (size_t c = 0; c < p.cd.size(); ++c) {       // k_lz4_content
+        const bag::Lz4ChunkDesc& d = p.cd[c];
+        if (d.has_sum && lz4::xxh32(dec.data() + d.dec, d.size, 0) != d.sum) err = std::min(err, bag::chunk_key(d, c, lz4::R_CONTENT_SUM));
+    }
+    res.assign(p.nodes.size(), bag::NodeOut{});
+    for (size_t i = 0; i < p.nodes.size(); ++i) {     // k_bag_parse
+        const bag::Lz4NodeIn& n = p.nodes[i];
+        bag::NodeOut& r = res[i];
+        uint64_t d0 = 0, d1 = 0;
+        r.code = bag::record_core(dec.data() + n.dec, n.len, n.rec, n.conn, n.time_ns, &d0, &d1, &r.a);
+        if (r.code == bag::NF_OK) r.code = bag::parse_node_core(dec.data() + n.dec, d0, d1, &r.seq, r.odom, r.cloud, &r.a, &r.b);
+    }
+    return err;
+}
 
 // erasor_bag_index on the host; the index is kept for the two calls below
 int erasor_hostcheck_bag_index(const char* file, size_t len, const char* topic, int keep_first, size_t* n_nodes, erasor_bag_info_t* info,
@@ -247,11 +303,27 @@ int erasor_hostcheck_bag_index(const char* file, size_t len, const char* topic, 
     std::string msg;
     *n_nodes = 0;
     *info = erasor_bag_info_t{};
-    const int rc = bag::build_index(reinterpret_cast<const uint8_t*>(file), len, topic ? topic : "/node/combined/optimized", keep_first != 0, g_bag, msg);
+    g_plan = bag::Lz4Plan();
+    g_dec.clear();
+    const uint8_t* f = reinterpret_cast<const uint8_t*>(file);
+    int rc = bag::build_index(f, len, topic ? topic : "/node/combined/optimized", keep_first != 0, g_bag, msg);
+    if (rc == ERASOR_OK && !g_bag.pending.empty()) {
+        bag::plan_lz4(g_bag, g_plan);
+        std::vector<bag::NodeOut> res;
+        const uint64_t key = lz4_stages(f, g_bag, g_plan, g_dec, res);
+        if (key != ~0ull) { msg = bag::lz4_error(g_bag, g_plan, key); rc = ERASOR_E_INVALID; }
+        else rc = bag::finish_lz4(g_bag, res.data(), msg);
+    }
     set_err(err, errcap, msg);
-    if (rc != ERASOR_OK) return rc;
+    if (rc != ERASOR_OK) { g_bag = bag::Index(); g_plan = bag::Lz4Plan(); return rc; }
     *n_nodes = g_bag.nodes.size();
     bag::fill_info(g_bag, *info);
+    return ERASOR_OK;
+}
+
+// erasor_bag_lz4_stats of the last erasor_hostcheck_bag_index
+int erasor_hostcheck_bag_lz4_stats(erasor_bag_lz4_stats_t* s) {
+    bag::fill_lz4_stats(g_bag, g_plan, *s);
     return ERASOR_OK;
 }
 
@@ -279,14 +351,84 @@ int erasor_hostcheck_bag_decode(const char* file, size_t first, size_t count, fl
     if (rc != ERASOR_OK) return rc;
     offsets[0] = 0;
     for (size_t k = 0; k < count; ++k) {
-        const bag::Cloud& c = g_bag.nodes[first + k].cloud;
-        const uint8_t* d = reinterpret_cast<const uint8_t*>(file) + c.data_off;
+        const bag::Node& nd = g_bag.nodes[first + k];
+        const bag::Cloud& c = nd.cloud;
+        const uint8_t* d = (nd.lz >= 0 ? g_dec.data() + bag::dec_of(g_plan, nd) : reinterpret_cast<const uint8_t*>(file)) + c.data_off;
         const uint64_t n = bag::cloud_points(c);
         uint32_t* o = reinterpret_cast<uint32_t*>(out) + 4 * offsets[k];
         for (uint64_t i = 0; i < n; ++i) bag::point_values(d + bag::point_offset(c, i), c, o + 4 * i);
         offsets[k + 1] = offsets[k] + n;
     }
     return ERASOR_OK;
+}
+
+// A greedy LZ4 block encoder for inputs too large for tests/lz4_model.py: a table keyed by a hash of the four bytes at each
+// position holds the last position they were seen at; a match within 65535 bytes is extended while it lasts.  As liblz4 requires of
+// its input, the last match starts 12 bytes or more before the end and the last 5 bytes are literals.
+static uint64_t lz4_block_greedy(const uint8_t* in, uint32_t n, uint8_t* out) {
+    std::vector<int64_t> table(1u << 16, -1);
+    uint64_t o = 0;
+    auto len_ext = [&](uint32_t v) { for (; v >= 255; v -= 255) out[o++] = 255; out[o++] = (uint8_t)v; };
+    auto emit = [&](uint32_t a, uint32_t lit, uint32_t off, uint32_t mlen) {
+        out[o++] = (uint8_t)((std::min<uint32_t>(lit, 15) << 4) | (off ? std::min<uint32_t>(mlen - 4, 15) : 0));
+        if (lit >= 15) len_ext(lit - 15);
+        std::memcpy(out + o, in + a, lit);
+        o += lit;
+        if (!off) return;
+        out[o++] = (uint8_t)off;
+        out[o++] = (uint8_t)(off >> 8);
+        if (mlen - 4 >= 15) len_ext(mlen - 4 - 15);
+    };
+    uint32_t i = 0, anchor = 0;
+    const uint32_t limit = n >= 13 ? n - 12 : 0, mend = n >= 5 ? n - 5 : 0;
+    while (i < limit) {
+        uint32_t v;
+        std::memcpy(&v, in + i, 4);
+        const uint32_t h = (v * 2654435761u) >> 16;
+        const int64_t cand = table[h];
+        table[h] = i;
+        uint32_t w = 0;
+        if (cand >= 0) std::memcpy(&w, in + cand, 4);
+        if (cand >= 0 && i - cand <= 65535 && w == v) {
+            uint32_t len = 4;
+            while (i + len < mend && in[cand + len] == in[i + len]) ++len;
+            emit(anchor, i - anchor, (uint32_t)(i - cand), len);
+            i += len;
+            anchor = i;
+        } else {
+            ++i;
+        }
+    }
+    emit(anchor, n - anchor, 0, 0);
+    return o;
+}
+
+// The LZ4 frame of in[0, n) with block max id bsid (4..7), block checksums and a content checksum when asked; a block that does
+// not shrink is stored.  *clen = the frame's length; -1 when out (cap bytes) is too small.
+int erasor_hostcheck_lz4_frame(const uint8_t* in, uint64_t n, int bsid, int block_sums, int content_sum, uint8_t* out, uint64_t cap, uint64_t* clen) {
+    const uint64_t bmax = 1ull << (8 + 2 * bsid);
+    if (cap < 15 + n + (n / bmax + 1) * (8 + bmax / 255 + 16)) return -1;
+    uint64_t o = 0;
+    auto put32 = [&](uint32_t v) { for (int k = 0; k < 4; ++k) out[o++] = (uint8_t)(v >> (8 * k)); };
+    put32(lz4::kMagic);
+    out[o++] = (uint8_t)(0x60 | (block_sums ? 0x10 : 0) | (content_sum ? 0x04 : 0));
+    out[o++] = (uint8_t)(bsid << 4);
+    out[o] = (uint8_t)((lz4::xxh32(out + 4, 2, 0) >> 8) & 0xFF);
+    ++o;
+    for (uint64_t a = 0; a < n; a += bmax) {
+        const uint32_t m = (uint32_t)std::min<uint64_t>(bmax, n - a);
+        const uint64_t c = lz4_block_greedy(in + a, m, out + o + 4);
+        const bool stored = c >= m;
+        if (stored) std::memcpy(out + o + 4, in + a, m);
+        const uint32_t bs = stored ? m : (uint32_t)c;
+        put32(bs | (stored ? 0x80000000u : 0u));
+        o += bs;
+        if (block_sums) put32(lz4::xxh32(out + o - bs, bs, 0));
+    }
+    put32(0);
+    if (content_sum) put32(lz4::xxh32(in, n, 0));
+    *clen = o;
+    return 0;
 }
 
 // A serial liblzf-style decoder (one token after the other, bytes copied one at a time): 0, or -1 for a malformed stream

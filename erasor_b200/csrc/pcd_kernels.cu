@@ -422,7 +422,7 @@ __global__ void __launch_bounds__(kThreads) k_lzf_fill(const uint32_t* src, uint
 // One cloud of a erasor_bag_load call.  A cloud whose rows are contiguous (row_step == width x point_step, or one row) is one row
 // of n points; otherwise each of its rows is tiled on its own, so that a tile never spans row padding.
 struct BagDesc {
-    uint64_t src;                    // the cloud's data in the device copy of the blobs (16-byte aligned)
+    uint64_t src;                    // the cloud's data in the device copy of the blobs (16-byte aligned), or in the decoded chunks
     uint64_t out;                    // its first output point
     uint64_t tile0;                  // its first tile
     uint64_t cols;                   // points per row as tiled
@@ -430,11 +430,13 @@ struct BagDesc {
     uint32_t per_tile;               // points per tile
     uint32_t staged;                 // 1: a tile's bytes are staged in shared memory; 0: read from global memory point by point
     uint32_t reach;                  // bag::point_reach
+    uint32_t lz4;                    // 1: src is in the decoded LZ4 chunks
     bag::Cloud c;
 };
 
 // one CTA per tile: the cloud by binary search over tile0, then as k_pcd_gather_tile, at the cloud's row_step and point_step
-__global__ void __launch_bounds__(kGatherThreads) k_bag_gather(const uint8_t* blobs, const BagDesc* d, int nclouds, uint64_t ntiles, uint4* out) {
+__global__ void __launch_bounds__(kGatherThreads) k_bag_gather(const uint8_t* blobs, const uint8_t* dec, const BagDesc* d, int nclouds, uint64_t ntiles,
+                                                                uint4* out) {
     __shared__ __align__(16) uint8_t tile[kGatherTile + 32];
     for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
         int lo = 0, hi = nclouds - 1;
@@ -446,7 +448,7 @@ __global__ void __launch_bounds__(kGatherThreads) k_bag_gather(const uint8_t* bl
         const uint64_t lt = t - D.tile0, r = lt / D.tiles_per_row, c0 = (lt - r * D.tiles_per_row) * D.per_tile;
         const uint32_t np = (uint32_t)min((uint64_t)D.per_tile, D.cols - c0);
         const uint32_t step = D.c.point_step;
-        const uint8_t* src = blobs + D.src + r * D.c.row_step + c0 * step;
+        const uint8_t* src = (D.lz4 ? dec : blobs) + D.src + r * D.c.row_step + c0 * step;
         uint4* o = out + D.out + r * D.cols + c0;
         if (D.staged) {
             const uintptr_t lo_a = reinterpret_cast<uintptr_t>(src), hi_a = lo_a + (uint64_t)(np - 1) * step + D.reach;
@@ -477,6 +479,112 @@ __global__ void __launch_bounds__(kGatherThreads) k_bag_gather(const uint8_t* bl
     }
 }
 
+// ---- lz4 chunks of a bag (DESIGN.md section 12.2.1; the rules are lz4_frame.h, the plan and the node layout bag_index.h) --------
+// A warp walking one block: lane 0 parses each sequence and broadcasts it, the copies use all 32 lanes
+struct Warp {
+    PCD_HD uint32_t lane() const {
+#ifdef __CUDA_ARCH__
+        return threadIdx.x & 31u;
+#else
+        return 0;
+#endif
+    }
+    PCD_HD uint32_t lanes() const { return 32; }
+    PCD_HD void sync() const {
+#ifdef __CUDA_ARCH__
+        __syncwarp();
+#endif
+    }
+    PCD_HD uint32_t bcast(uint32_t v) const {
+#ifdef __CUDA_ARCH__
+        return __shfl_sync(0xFFFFFFFFu, v, 0);
+#else
+        return v;
+#endif
+    }
+};
+
+// 1. one thread per block: its decoded size, from the token walk without copies (every rule checked)
+__global__ void __launch_bounds__(kThreads) k_lz4_size(const uint8_t* src, const bag::Lz4Block* blk, uint64_t nb, uint32_t* bsize,
+                                                       unsigned long long* err) {
+    for (uint64_t b = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += (uint64_t)gridDim.x * blockDim.x) {
+        const bag::Lz4Block B = blk[b];
+        uint32_t o = B.csize, at = 0, r = lz4::R_OK;
+        if (!B.stored) r = lz4::block(lz4::Serial{}, src + B.src, B.csize, nullptr, B.cap, &o, &at);
+        if (r != lz4::R_OK) atomicMin(err, (unsigned long long)bag::block_key(B, b, at, r));
+        bsize[b] = r == lz4::R_OK ? o : 0u;
+    }
+}
+
+// 2. one thread per chunk: its blocks' places in the decoded buffer (a serial scan: a chunk holds a few blocks), ~0 for every block
+// of a chunk that does not decode to its size
+__global__ void __launch_bounds__(kThreads) k_lz4_place(const bag::Lz4ChunkDesc* cd, uint64_t nc, const uint32_t* bsize, uint64_t* boff,
+                                                        unsigned long long* err) {
+    for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (uint64_t)gridDim.x * blockDim.x) {
+        const bag::Lz4ChunkDesc d = cd[c];
+        uint64_t s = 0;
+        for (uint32_t b = d.block0; b < d.block0 + d.nblocks; ++b) s += bsize[b];
+        const bool ok = s == d.size;
+        if (!ok) atomicMin(err, (unsigned long long)bag::chunk_key(d, c, lz4::R_SIZE));
+        s = 0;
+        for (uint32_t b = d.block0; b < d.block0 + d.nblocks; ++b) { boff[b] = ok ? d.dec + s : ~0ull; s += bsize[b]; }
+    }
+}
+
+// 3. one warp per block: the decode straight into place
+__global__ void __launch_bounds__(kThreads) k_lz4_decode(const uint8_t* src, const bag::Lz4Block* blk, uint64_t nb, const uint32_t* bsize,
+                                                         const uint64_t* boff, uint8_t* dec) {
+    const uint64_t nw = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t b = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < nb; b += nw) {
+        const uint64_t at = boff[b];
+        if (at == ~0ull) continue;
+        const bag::Lz4Block B = blk[b];
+        if (B.stored) {
+            for (uint32_t k = threadIdx.x & 31u; k < B.csize; k += 32) dec[at + k] = src[B.src + k];
+        } else {
+            uint32_t o, e;
+            lz4::block(Warp{}, src + B.src, B.csize, dec + at, bsize[b], &o, &e);
+        }
+    }
+}
+
+// 4. XXH32 is one serial chain per input: one thread per block checksum (blocks are small)
+__global__ void __launch_bounds__(kThreads) k_lz4_sums(const uint8_t* src, const bag::Lz4Block* blk, uint64_t nb, unsigned long long* err) {
+    for (uint64_t b = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += (uint64_t)gridDim.x * blockDim.x) {
+        const bag::Lz4Block B = blk[b];
+        if (B.has_sum && lz4::xxh32(src + B.src, B.csize, 0) != B.sum) atomicMin(err, (unsigned long long)bag::block_key(B, b, B.csize, lz4::R_BLOCK_SUM));
+    }
+}
+
+// ... and four threads per content checksum, one per XXH32 accumulator (independent chains over the 16-byte stripes of the chunk,
+// 16-byte aligned in the decoded buffer, so each reads aligned words); CTAs of kContentThreads spread the chunks over the SMs
+constexpr int kContentThreads = 32;
+__global__ void __launch_bounds__(kContentThreads) k_lz4_content(const bag::Lz4ChunkDesc* cd, uint64_t nc, const uint8_t* dec, unsigned long long* err) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, c = t >> 2;
+    const uint32_t j = (uint32_t)(t & 3u);
+    const bool live = c < nc;
+    const bag::Lz4ChunkDesc d = live ? cd[c] : bag::Lz4ChunkDesc{};
+    const uint8_t* p = dec + d.dec;
+    uint32_t v[4];
+    const uint32_t mine = live && d.has_sum ? lz4::xxh32_lane(p, d.size, 0, j) : 0u;
+    const uint32_t q = threadIdx.x & ~3u;
+    for (uint32_t k = 0; k < 4; ++k) v[k] = __shfl_sync(0xFFFFFFFFu, mine, q + k);
+    if (live && j == 0 && d.has_sum && lz4::xxh32_merge(v, p, d.size, 0) != d.sum)
+        atomicMin(err, (unsigned long long)bag::chunk_key(d, c, lz4::R_CONTENT_SUM));
+}
+
+// 5. one thread per kept node in an LZ4 chunk: the record its index entry points to, then the node layout (bag::parse_node_core)
+__global__ void __launch_bounds__(kThreads) k_bag_parse(const uint8_t* dec, const bag::Lz4NodeIn* in, uint64_t n, bag::NodeOut* out) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const bag::Lz4NodeIn q = in[i];
+        bag::NodeOut r{};
+        uint64_t d0 = 0, d1 = 0;
+        r.code = bag::record_core(dec + q.dec, q.len, q.rec, q.conn, q.time_ns, &d0, &d1, &r.a);
+        if (r.code == bag::NF_OK) r.code = bag::parse_node_core(dec + q.dec, d0, d1, &r.seq, r.odom, r.cloud, &r.a, &r.b);
+        out[i] = r;
+    }
+}
+
 constexpr uint64_t kBagStage = 32ull << 20;          // bytes per pinned staging buffer (two) for a pageable file
 
 uint32_t blocks_for(uint64_t n, int per, int cap) { return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + per - 1) / per, (uint64_t)cap)); }
@@ -498,6 +606,12 @@ struct erasor_pcd_ctx {
     const uint8_t* bag_file = nullptr;
     PinnedBuffer bag_stage[2];
     cudaEvent_t bag_ev[2] = {nullptr, nullptr};
+    // the LZ4 chunks of the index: the plan, the decoded chunks (kept until the next erasor_bag_index), the decode's scratch (the
+    // compressed copy z4_src is released when the index returns)
+    bag::Lz4Plan z4;
+    DeviceBuffer z4_src, z4_dec, z4_blk, z4_cd, z4_in, z4_bsize, z4_boff, z4_res;
+    cudaEvent_t z4_ev[3] = {nullptr, nullptr, nullptr};
+    double z4_decode_ms = 0, z4_sums_ms = 0;
     // erasor_pcd_format_ascii's text of its last call, kept for a following call with the same input
     bool cached = false;
     const float* c_ptr = nullptr;
@@ -612,6 +726,107 @@ int lzf_decode(erasor_pcd_t p, const uint8_t* s, uint64_t csize, uint64_t usize,
     return ERASOR_OK;
 }
 
+// Bytes of the bag file to the device: span k is host[k][0, len) -> d + at (at increasing).  From a pinned file each span is one
+// cudaMemcpyAsync; from a pageable one a window of the device layout at a time is filled on the host in one pinned buffer while
+// the other one's copy runs.
+struct Span { const uint8_t* host; uint64_t len, at; };
+
+int upload_spans(erasor_pcd_t p, uint8_t* d, const std::vector<Span>& spans) {
+    if (p->bag_pinned) {
+        for (const Span& s : spans) PCK(cudaMemcpyAsync(d + s.at, s.host, s.len, cudaMemcpyHostToDevice, p->st));
+        return ERASOR_OK;
+    }
+    for (int k = 0; k < 2; ++k) {
+        if (!p->bag_stage[k].p()) PCK(p->bag_stage[k].allocate(kBagStage));
+        if (!p->bag_ev[k]) PCK(cudaEventCreateWithFlags(&p->bag_ev[k], cudaEventDisableTiming));
+    }
+    int cur = 0;
+    uint64_t w0 = 0, filled = 0;                      // the window [w0, w0 + kBagStage) of the device layout; bytes of it filled
+    auto flush = [&]() -> cudaError_t {
+        cudaError_t e = cudaMemcpyAsync(d + w0, p->bag_stage[cur].p(), filled, cudaMemcpyHostToDevice, p->st);
+        if (e == cudaSuccess) e = cudaEventRecord(p->bag_ev[cur], p->st);
+        cur ^= 1;
+        w0 += filled;
+        filled = 0;
+        return e == cudaSuccess ? cudaEventSynchronize(p->bag_ev[cur]) : e;    // the buffer filled next is free again
+    };
+    PCK(cudaEventSynchronize(p->bag_ev[0]));
+    PCK(cudaEventSynchronize(p->bag_ev[1]));
+    for (const Span& s : spans) {
+        uint64_t done = 0;
+        while (done < s.len) {
+            const uint64_t at = s.at + done;          // device offset of the next byte
+            if (at - w0 >= kBagStage) PCK(flush());
+            const uint64_t take = std::min(s.len - done, kBagStage - (at - w0));
+            std::memcpy(p->bag_stage[cur].as<uint8_t>() + (at - w0), s.host + done, take);
+            filled = at - w0 + take;
+            done += take;
+        }
+    }
+    if (filled) PCK(flush());
+    return ERASOR_OK;
+}
+
+// erasor_bag_index's nodes in LZ4 chunks: the chunks holding one uploaded, decoded and checked in one submission, the nodes parsed,
+// one read-back; then bag::finish_lz4
+int bag_lz4(erasor_pcd_t p, std::string& msg) {
+    bag::Lz4Plan& P = p->z4;
+    bag::plan_lz4(p->bag, P);
+    const uint64_t nb = P.blocks.size(), nc = P.cd.size(), nn = P.nodes.size();
+    PCK(p->z4_src.ensure(std::max<uint64_t>(P.src_bytes, 16)));
+    PCK(p->z4_dec.ensure(std::max<uint64_t>(P.dec_bytes, 16)));
+    PCK(p->z4_blk.ensure(sizeof(bag::Lz4Block) * std::max<uint64_t>(nb, 1)));
+    PCK(p->z4_cd.ensure(sizeof(bag::Lz4ChunkDesc) * nc));
+    PCK(p->z4_in.ensure(sizeof(bag::Lz4NodeIn) * nn));
+    PCK(p->z4_bsize.ensure(sizeof(uint32_t) * std::max<uint64_t>(nb, 1)));
+    PCK(p->z4_boff.ensure(sizeof(uint64_t) * std::max<uint64_t>(nb, 1)));
+    PCK(p->z4_res.ensure(sizeof(bag::NodeOut) * nn + sizeof(unsigned long long)));
+    for (cudaEvent_t& ev : p->z4_ev)
+        if (!ev) PCK(cudaEventCreate(&ev));
+    std::vector<Span> spans;
+    for (size_t c = 0; c < nc; ++c) {
+        const bag::Lz4Chunk& k = p->bag.lz4[P.chunks[c]];
+        spans.push_back(Span{p->bag_file + k.data, k.len, P.cd[c].src});
+    }
+    uint8_t* src = p->z4_src.as<uint8_t>();
+    uint8_t* dec = p->z4_dec.as<uint8_t>();
+    const int rc = upload_spans(p, src, spans);
+    if (rc != ERASOR_OK) return rc;
+    if (nb) PCK(cudaMemcpyAsync(p->z4_blk.p(), P.blocks.data(), sizeof(bag::Lz4Block) * nb, cudaMemcpyHostToDevice, p->st));
+    PCK(cudaMemcpyAsync(p->z4_cd.p(), P.cd.data(), sizeof(bag::Lz4ChunkDesc) * nc, cudaMemcpyHostToDevice, p->st));
+    PCK(cudaMemcpyAsync(p->z4_in.p(), P.nodes.data(), sizeof(bag::Lz4NodeIn) * nn, cudaMemcpyHostToDevice, p->st));
+    bag::NodeOut* d_res = p->z4_res.as<bag::NodeOut>();
+    unsigned long long* d_err = reinterpret_cast<unsigned long long*>(d_res + nn);
+    PCK(cudaMemsetAsync(d_err, 0xFF, sizeof(unsigned long long), p->st));
+    const bag::Lz4Block* blk = p->z4_blk.as<bag::Lz4Block>();
+    const bag::Lz4ChunkDesc* cd = p->z4_cd.as<bag::Lz4ChunkDesc>();
+    uint32_t* bsize = p->z4_bsize.as<uint32_t>();
+    uint64_t* boff = p->z4_boff.as<uint64_t>();
+    const int cap = p->sm_count * 16;
+    PCK(cudaEventRecord(p->z4_ev[0], p->st));
+    if (nb) k_lz4_size<<<blocks_for(nb, kThreads, cap), kThreads, 0, p->st>>>(src, blk, nb, bsize, d_err);
+    k_lz4_place<<<blocks_for(nc, kThreads, cap), kThreads, 0, p->st>>>(cd, nc, bsize, boff, d_err);
+    if (nb) k_lz4_decode<<<blocks_for(nb, kThreads / 32, cap), kThreads, 0, p->st>>>(src, blk, nb, bsize, boff, dec);
+    PCK(cudaEventRecord(p->z4_ev[1], p->st));
+    if (nb) k_lz4_sums<<<blocks_for(nb, kThreads, cap), kThreads, 0, p->st>>>(src, blk, nb, d_err);
+    k_lz4_content<<<(unsigned)((4 * nc + kContentThreads - 1) / kContentThreads), kContentThreads, 0, p->st>>>(cd, nc, dec, d_err);
+    PCK(cudaEventRecord(p->z4_ev[2], p->st));
+    k_bag_parse<<<blocks_for(nn, kThreads, cap), kThreads, 0, p->st>>>(dec, p->z4_in.as<bag::Lz4NodeIn>(), nn, d_res);
+    PCK(cudaGetLastError());
+    std::vector<bag::NodeOut> res(nn);
+    unsigned long long err = 0;
+    PCK(cudaMemcpyAsync(res.data(), d_res, sizeof(bag::NodeOut) * nn, cudaMemcpyDeviceToHost, p->st));
+    PCK(cudaMemcpyAsync(&err, d_err, sizeof(err), cudaMemcpyDeviceToHost, p->st));
+    PCK(cudaStreamSynchronize(p->st));
+    float t0 = 0, t1 = 0;
+    PCK(cudaEventElapsedTime(&t0, p->z4_ev[0], p->z4_ev[1]));
+    PCK(cudaEventElapsedTime(&t1, p->z4_ev[1], p->z4_ev[2]));
+    p->z4_decode_ms = t0;
+    p->z4_sums_ms = t1;
+    if (err != ~0ull) { msg = bag::lz4_error(p->bag, P, err); return ERASOR_E_INVALID; }
+    return bag::finish_lz4(p->bag, res.data(), msg);
+}
+
 const char* kHeadFmt ="# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z intensity\nSIZE 4 4 4 4\nTYPE F F F F\n"
                        "COUNT 1 1 1 1\nWIDTH %zu\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS %zu\nDATA ascii\n";
 }  // namespace
@@ -645,6 +860,8 @@ void erasor_pcd_destroy(erasor_pcd_t p) {
     cudaSetDevice(p->device);
     if (p->st) cudaStreamSynchronize(p->st);
     for (cudaEvent_t ev : p->bag_ev)
+        if (ev) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : p->z4_ev)
         if (ev) cudaEventDestroy(ev);
     if (p->st) cudaStreamDestroy(p->st);
     delete p;
@@ -907,18 +1124,30 @@ int erasor_bag_index(erasor_pcd_t p, const char* file, size_t len, const char* t
     p->cached = false;
     p->bag_ok = false;
     p->bag = bag::Index();
+    p->z4 = bag::Lz4Plan();
+    p->z4_decode_ms = p->z4_sums_ms = 0;
     p->bag_file = nullptr;
     if (info) *info = erasor_bag_info_t{};
     if (!n_nodes || (len && !file)) return fail(p, ERASOR_E_INVALID, "null argument");
     *n_nodes = 0;
     PCK(cudaSetDevice(p->device));
     std::string msg;
-    const int rc = bag::build_index(reinterpret_cast<const uint8_t*>(file), len, topic ? topic : "/node/combined/optimized", keep_first != 0, p->bag, msg);
+    int rc = bag::build_index(reinterpret_cast<const uint8_t*>(file), len, topic ? topic : "/node/combined/optimized", keep_first != 0, p->bag, msg);
     if (rc != ERASOR_OK) { p->bag = bag::Index(); return fail(p, rc, msg); }
     cudaPointerAttributes a{};
     p->bag_pinned = cudaPointerGetAttributes(&a, file) == cudaSuccess && a.type == cudaMemoryTypeHost;
     cudaGetLastError();
     p->bag_file = reinterpret_cast<const uint8_t*>(file);
+    if (!p->bag.pending.empty()) {
+        rc = bag_lz4(p, msg);
+        p->z4_src = DeviceBuffer();                  // the compressed copy is not needed past the index: only the decoded chunks stay
+        if (rc != ERASOR_OK) {
+            p->bag = bag::Index();
+            p->z4 = bag::Lz4Plan();
+            p->bag_file = nullptr;
+            return rc == ERASOR_E_CUDA ? rc : fail(p, rc, msg);
+        }
+    }
     p->bag_ok = true;
     *n_nodes = p->bag.nodes.size();
     if (info) bag::fill_info(p->bag, *info);
@@ -974,16 +1203,20 @@ int erasor_bag_load_list(erasor_pcd_t p, const uint64_t* nodes, size_t count, fl
     if (!total) return ERASOR_OK;
     PCK(cudaSetDevice(p->device));
 
-    // the clouds' descriptors and the device copy of their data, each blob at a 16-byte aligned offset
+    // the clouds' descriptors and the device copy of their data, each blob at a 16-byte aligned offset (a node in an LZ4 chunk is
+    // read where its chunk was decoded)
     std::vector<BagDesc> desc;
+    std::vector<Span> spans;
     uint64_t blob_bytes = 0, ntiles = 0;
     for (size_t k = 0; k < count; ++k) {
-        const bag::Cloud& c = p->bag.nodes[nodes[k]].cloud;
+        const bag::Node& nd = p->bag.nodes[nodes[k]];
+        const bag::Cloud& c = nd.cloud;
         const uint64_t n = bag::cloud_points(c);
         if (!n) continue;
         BagDesc D{};
         D.c = c;
-        D.src = blob_bytes;
+        D.lz4 = nd.lz >= 0;
+        D.src = D.lz4 ? bag::dec_of(p->z4, nd) + c.data_off : blob_bytes;
         D.out = offsets[k];
         D.tile0 = ntiles;
         D.reach = bag::point_reach(c);
@@ -995,53 +1228,35 @@ int erasor_bag_load_list(erasor_pcd_t p, const uint64_t* nodes, size_t count, fl
                               : 4 * kGatherThreads;
         D.tiles_per_row = (D.cols + D.per_tile - 1) / D.per_tile;
         ntiles += rows * D.tiles_per_row;
-        blob_bytes += (c.data_len + 15) & ~15ull;
+        if (!D.lz4) {
+            spans.push_back(Span{p->bag_file + c.data_off, c.data_len, blob_bytes});
+            blob_bytes += (c.data_len + 15) & ~15ull;
+        }
         desc.push_back(D);
     }
     PCK(p->bag_blobs.ensure(blob_bytes));
     PCK(p->bag_desc.ensure(sizeof(BagDesc) * desc.size()));
     uint8_t* d_blobs = p->bag_blobs.as<uint8_t>();
-    if (p->bag_pinned) {
-        for (const BagDesc& D : desc) PCK(cudaMemcpyAsync(d_blobs + D.src, p->bag_file + D.c.data_off, D.c.data_len, cudaMemcpyHostToDevice, p->st));
-    } else {
-        // a window of the device layout at a time: filled on the host in one pinned buffer while the other one's copy runs
-        for (int k = 0; k < 2; ++k) {
-            if (!p->bag_stage[k].p()) PCK(p->bag_stage[k].allocate(kBagStage));
-            if (!p->bag_ev[k]) PCK(cudaEventCreateWithFlags(&p->bag_ev[k], cudaEventDisableTiming));
-        }
-        int cur = 0;
-        uint64_t w0 = 0, filled = 0;                  // the window [w0, w0 + kBagStage) of the device layout; bytes of it filled
-        auto flush = [&]() -> cudaError_t {
-            cudaError_t e = cudaMemcpyAsync(d_blobs + w0, p->bag_stage[cur].p(), filled, cudaMemcpyHostToDevice, p->st);
-            if (e == cudaSuccess) e = cudaEventRecord(p->bag_ev[cur], p->st);
-            cur ^= 1;
-            w0 += filled;
-            filled = 0;
-            return e == cudaSuccess ? cudaEventSynchronize(p->bag_ev[cur]) : e;    // the buffer filled next is free again
-        };
-        PCK(cudaEventSynchronize(p->bag_ev[0]));
-        PCK(cudaEventSynchronize(p->bag_ev[1]));
-        for (const BagDesc& D : desc) {
-            uint64_t done = 0;
-            while (done < D.c.data_len) {
-                const uint64_t at = D.src + done;      // device offset of the next byte
-                if (at - w0 >= kBagStage) PCK(flush());
-                const uint64_t take = std::min(D.c.data_len - done, kBagStage - (at - w0));
-                std::memcpy(p->bag_stage[cur].as<uint8_t>() + (at - w0), p->bag_file + D.c.data_off + done, take);
-                filled = at - w0 + take;
-                done += take;
-            }
-        }
-        if (filled) PCK(flush());
-    }
+    rc = upload_spans(p, d_blobs, spans);
+    if (rc != ERASOR_OK) return rc;
     PCK(cudaMemcpyAsync(p->bag_desc.p(), desc.data(), sizeof(BagDesc) * desc.size(), cudaMemcpyHostToDevice, p->st));
     uint4* d_out = reinterpret_cast<uint4*>(out_xyzi);
     if (out_kind == ERASOR_PTR_HOST) { PCK(p->out.ensure(sizeof(uint4) * total)); d_out = p->out.as<uint4>(); }
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(ntiles, (uint64_t)p->sm_count * 8));
-    k_bag_gather<<<grid, kGatherThreads, 0, p->st>>>(d_blobs, p->bag_desc.as<BagDesc>(), (int)desc.size(), ntiles, d_out);
+    k_bag_gather<<<grid, kGatherThreads, 0, p->st>>>(d_blobs, p->z4_dec.as<uint8_t>(), p->bag_desc.as<BagDesc>(), (int)desc.size(), ntiles, d_out);
     PCK(cudaGetLastError());
     if (out_kind == ERASOR_PTR_HOST) PCK(cudaMemcpyAsync(out_xyzi, d_out, sizeof(uint4) * total, cudaMemcpyDeviceToHost, p->st));
     PCK(cudaStreamSynchronize(p->st));
+    return ERASOR_OK;
+}
+
+int erasor_bag_lz4_stats(erasor_pcd_t p, erasor_bag_lz4_stats_t* stats) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    if (!stats) return fail(p, ERASOR_E_INVALID, "null argument");
+    bag::fill_lz4_stats(p->bag, p->z4, *stats);
+    stats->decode_ms = p->z4_decode_ms;
+    stats->checksum_ms = p->z4_sums_ms;
     return ERASOR_OK;
 }
 

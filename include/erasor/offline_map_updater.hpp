@@ -282,6 +282,12 @@ public:
     size_t size() const { return nodes_.size(); }
     const BagNode& node(size_t i) const { return nodes_.at(i); }
     const erasor_bag_info_t& info() const { return info_; }
+    // the bag's lz4 chunks: how many were uploaded and decoded, bytes, blocks, checksums (erasor_bag_lz4_stats)
+    erasor_bag_lz4_stats_t lz4_stats() const {
+        erasor_bag_lz4_stats_t s{};
+        check(erasor_bag_lz4_stats(p_, &s));
+        return s;
+    }
     // The clouds of nodes [first, first + count) -- or of the listed nodes -- back to back in device memory, from one gather
     // launch.  device_buffer(n) must return a 16-byte aligned device pointer with room for n points (the caller owns the memory).
     // Returns the count + 1 offsets.  Synchronous: the clouds are complete on return.

@@ -457,21 +457,34 @@ int  erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind
                      size_t* n, erasor_pcd_load_info_t* info);
 
 /* ROS bag 2.0 files of erasor/node messages (DESIGN.md section 12.2; the format restated from its public description, rosbag is
- * not built here).  erasor_bag_index walks the file on the host -- every record, chunks included; uncompressed chunks only -- and
- * keeps the messages on `topic` (NULL: "/node/combined/optimized") in delivery order, a stable sort by record time.  Unless
- * keep_first, the first of them is dropped, as the reference's subscribers drop it.  file: host memory, len bytes, which must stay
- * valid and unchanged until the next erasor_bag_index on p; pinned memory is read by the device directly, pageable memory through
- * a pinned staging buffer.  Errors: ERASOR_E_UNSUPPORTED for another bag version, a compressed chunk, a topic whose type is not
- * erasor/node, a cloud without FLOAT32 x, y or z; ERASOR_E_INVALID (with the byte offset) for a record or field running past its
- * container, a chunk whose data length differs from its size, a message on an undefined connection, a missing header field, a
+ * not built here).  erasor_bag_index walks the file on the host -- every record, uncompressed chunks included -- and keeps the
+ * messages on `topic` (NULL: "/node/combined/optimized") in delivery order, a stable sort by record time.  Unless keep_first, the
+ * first of them is dropped, as the reference's subscribers drop it.  file: host memory, len bytes, which must stay valid and
+ * unchanged until the next erasor_bag_index on p; pinned memory is read by the device directly, pageable memory through a pinned
+ * staging buffer.  Errors: ERASOR_E_UNSUPPORTED for another bag version, a chunk compressed with anything but lz4, a topic whose type
+ * is not erasor/node, a cloud without FLOAT32 x, y or z; ERASOR_E_INVALID (with the byte offset) for a record or field running past
+ * its container, a chunk whose data length differs from its size, a message on an undefined connection, a missing header field, a
  * message longer or shorter than an erasor/node, a point read past its cloud's data; ERASOR_E_CAPACITY for a cloud of 2^31 points.
- * A failed erasor_bag_index leaves no index: erasor_bag_nodes and erasor_bag_load then fail with ERASOR_E_STATE. */
+ * A failed erasor_bag_index leaves no index: erasor_bag_nodes and erasor_bag_load then fail with ERASOR_E_STATE.
+ *
+ * lz4 chunks (DESIGN.md section 12.2.1): the messages of such a chunk are the entries of the index data records that follow it;
+ * the chunks holding a kept node are copied to the device, decoded there (LZ4 frames of independent blocks; block and content
+ * checksums verified) and their nodes parsed there.  The call then uses the device and is synchronous; the decoded chunks stay in
+ * device memory held by p until the next erasor_bag_index or erasor_pcd_destroy (erasor_bag_lz4_stats: decoded_bytes); the
+ * compressed copy is released before the call returns.  Further
+ * errors: ERASOR_E_UNSUPPORTED for chunk data that is not an LZ4 frame, frame version other than 1, a dictionary, linked blocks, an
+ * lz4 chunk no index data record follows; ERASOR_E_INVALID for a reserved bit, a block max id below 4, a header checksum, content
+ * size or decoded length other than the chunk's size, a block above the block max, a malformed block (naming the chunk, the block
+ * and the byte of the frame), a block or content checksum mismatch, an index entry that does not point to its message record.  A
+ * bag without lz4 chunks does no device work here. */
 typedef struct {
     uint32_t version;                /* 200 for V2.0 */
     uint32_t pad_;
     uint64_t chunks, connections;    /* chunk records; distinct connection ids */
-    uint64_t messages, selected;     /* message records in the file; those on the topic (before the first is dropped) */
-    uint64_t unknown_records;        /* records of an op this reader does not know, skipped */
+    uint64_t messages, selected;     /* message records in the file (the index entries of lz4 chunks, the records walked in the
+                                        others); those on the topic (before the first is dropped) */
+    uint64_t unknown_records;        /* records of an op this reader does not know, skipped: only records the walk sees, so none
+                                        inside lz4 chunks */
     uint64_t nodes;                  /* the nodes erasor_bag_nodes / erasor_bag_load index */
     uint64_t total_points;           /* width x height summed over the nodes */
     uint64_t intensity_zero_filled;  /* nodes whose cloud has no FLOAT32 intensity: read as 0 */
@@ -479,8 +492,9 @@ typedef struct {
     char md5sum[40];                 /* the topic's connection md5sum, reported and not checked */
 } erasor_bag_info_t;
 
-/* one node's cloud as the gather reads it: point (r, c) at data_offset + r row_step + c point_step of the file; bit s of fields
- * (x y z intensity) set when that value is read from offset[s], clear when it is 0 */
+/* one node's cloud as the gather reads it: point (r, c) at data_offset + r row_step + c point_step of the file -- of the chunk's
+ * decoded data for a node in an lz4 chunk; bit s of fields (x y z intensity) set when that value is read from offset[s], clear
+ * when it is 0 */
 typedef struct {
     uint64_t data_offset, data_len;
     uint32_t width, height, point_step, row_step;
@@ -502,6 +516,22 @@ int  erasor_bag_nodes(erasor_pcd_t p, size_t first, size_t count, uint32_t* seq,
 int  erasor_bag_load(erasor_pcd_t p, size_t first, size_t count, float* out_xyzi, size_t cap, int out_kind, uint64_t* offsets);
 /* the same for the listed nodes, in list order (e.g. every removal_interval-th node); ERASOR_E_INVALID for an index past the bag */
 int  erasor_bag_load_list(erasor_pcd_t p, const uint64_t* nodes, size_t count, float* out_xyzi, size_t cap, int out_kind, uint64_t* offsets);
+
+/* The lz4 chunks of the last erasor_bag_index (all 0 after a failed one, or for a bag without lz4 chunks).  Only the chunks
+ * holding a kept node are uploaded and decoded; the nodes of a load in them are read from the decoded chunks (no upload). */
+typedef struct {
+    uint64_t chunks;                 /* lz4 chunks in the file */
+    uint64_t decoded_chunks;         /* of them, those holding a kept node: copied to the device and decoded */
+    uint64_t compressed_bytes;       /* their frames, copied host to device */
+    uint64_t decoded_bytes;          /* their decoded data, held on the device until the next erasor_bag_index */
+    uint64_t blocks, stored_blocks;  /* the blocks of the decoded chunks; of them stored (not compressed) */
+    uint64_t block_checksums;        /* block checksums verified */
+    uint64_t content_checksums;      /* content checksums verified */
+    double decode_ms;                /* device time of the size pass, placement and block decode (CUDA events) */
+    double checksum_ms;              /* device time of the checksum kernel (CUDA events) */
+} erasor_bag_lz4_stats_t;
+
+int  erasor_bag_lz4_stats(erasor_pcd_t p, erasor_bag_lz4_stats_t* stats);
 
 /* ============================================================================================
  * The naive map generator with its map resident on the device: the reference's mapgen (src/mapgen/mapgen.hpp:198-305,
