@@ -41,7 +41,7 @@ EXPORTS = [
     "erasor_eval_create", "erasor_eval_destroy", "erasor_eval_last_error", "erasor_evaluate", "erasor_eval_overlap",
     "erasor_eval_count_selected",
     "erasor_pcd_create", "erasor_pcd_destroy", "erasor_pcd_last_error", "erasor_pcd_parse_ascii", "erasor_pcd_format_ascii",
-    "erasor_pcd_load", "erasor_bag_index", "erasor_bag_nodes", "erasor_bag_load", "erasor_bag_load_list", "erasor_bag_lz4_stats",
+    "erasor_pcd_load", "erasor_bag_index", "erasor_bag_nodes", "erasor_bag_load", "erasor_bag_load_list", "erasor_bag_lz4_stats", "erasor_bag_bz2_stats",
     "erasor_mapgen_create", "erasor_mapgen_destroy", "erasor_mapgen_last_error", "erasor_mapgen_accum", "erasor_mapgen_get_cloud",
     "erasor_mapgen_device_cloud", "erasor_mapgen_synchronize", "erasor_mapgen_get_counters",
 ]
@@ -88,6 +88,13 @@ class BagLz4StatsC(ctypes.Structure):
     """erasor_bag_lz4_stats_t"""
     _fields_ = [(name, c_uint64) for name in ("chunks", "decoded_chunks", "compressed_bytes", "decoded_bytes", "blocks", "stored_blocks",
                                                "block_checksums", "content_checksums")] + [("decode_ms", c_double), ("checksum_ms", c_double)]
+
+
+class BagBz2StatsC(ctypes.Structure):
+    """erasor_bag_bz2_stats_t"""
+    _fields_ = [(name, c_uint64) for name in ("chunks", "decoded_chunks", "compressed_bytes", "decoded_bytes", "blocks", "candidates")] + \
+               [("streams_by_level", c_uint64 * 9), ("scratch_bytes", c_uint64)] + \
+               [(name, c_double) for name in ("scan_ms", "decode_ms", "bwt_ms", "rle_ms")]
 
 
 class MapGenParamsC(ctypes.Structure):
@@ -224,6 +231,7 @@ def _load():
     L.erasor_bag_load.argtypes = [c_void_p, c_size_t, c_size_t, c_void_p, c_size_t, c_int, POINTER(c_uint64)]
     L.erasor_bag_load_list.argtypes = [c_void_p, POINTER(c_uint64), c_size_t, c_void_p, c_size_t, c_int, POINTER(c_uint64)]
     L.erasor_bag_lz4_stats.argtypes = [c_void_p, POINTER(BagLz4StatsC)]
+    L.erasor_bag_bz2_stats.argtypes = [c_void_p, POINTER(BagBz2StatsC)]
     L.erasor_mapgen_create.argtypes = [POINTER(MapGenParamsC), c_int, POINTER(c_void_p)]
     L.erasor_mapgen_destroy.restype = None
     L.erasor_mapgen_destroy.argtypes = [c_void_p]
@@ -1093,6 +1101,16 @@ class PcdCodec(_Native):
         st = BagLz4StatsC()
         self._ck(self.L.erasor_bag_lz4_stats(self.h, ctypes.byref(st)))
         return {name: (float if name.endswith("_ms") else int)(getattr(st, name)) for name, _ in BagLz4StatsC._fields_}
+
+    def bag_bz2_stats(self) -> dict:
+        """erasor_bag_bz2_stats_t of the last bag_index as a dict: bz2 chunks in the file and decoded, compressed bytes uploaded,
+        decoded bytes held on the device, true blocks and block-magic candidates, streams by level (a list of 9), the decode's peak
+        scratch, and the device ms of its stage groups (scan + walk + chain, decode, inverse BWT, RLE1 + CRC)"""
+        st = BagBz2StatsC()
+        self._ck(self.L.erasor_bag_bz2_stats(self.h, ctypes.byref(st)))
+        out = {name: (float if name.endswith("_ms") else int)(getattr(st, name)) for name, _ in BagBz2StatsC._fields_ if name != "streams_by_level"}
+        out["streams_by_level"] = [int(v) for v in st.streams_by_level]
+        return out
 
     def bag_nodes(self, batch: int = 64, device_out: bool = False):
         """Yields (seq, odom7, cloud) per node of the indexed bag, as erasor_b200.kitti.iter_nodes yields them: clouds decoded

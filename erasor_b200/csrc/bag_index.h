@@ -9,9 +9,10 @@
 // records are walked in file order, chunks included; the index section is checked for structure only.
 //
 // An lz4 chunk (DESIGN.md section 12.2.1) is not walked: its frame descriptor and block table are read (lz4_frame.h), and its
-// messages are the entries (time, offset in the decoded chunk) of the index data records that follow it.  The nodes in it are
-// parsed after the chunks that hold a kept node are decoded, by the same parse_node_core, on the device (or serially by the
-// host build): plan_lz4 lays the decode out, finish_lz4 takes the parsed nodes back.
+// messages are the entries (time, offset in the decoded chunk) of the index data records that follow it.  A bz2 chunk (section
+// 12.2.2, bz2_stream.h) is indexed the same way; the host reads only its 4-byte stream header.  The nodes in compressed chunks are
+// parsed after the chunks that hold a kept node are decoded, by the same parse_node_core, on the device (or serially by the host
+// build): plan_chunks lays the decode out, finish_chunks takes the parsed nodes back.
 //
 // An erasor/node message serialises, in order: header (seq, stamp, frame_id); odom, a Pose of 7 doubles (position x y z, then
 // orientation x y z w); odomCov, 36 doubles; lidar, a PointCloud2 (header; height, width; the field list, each a name string,
@@ -31,6 +32,7 @@
 #include <vector>
 
 #include "../../include/erasor_b200.h"
+#include "bz2_stream.h"
 #include "lz4_frame.h"
 #include "pcd_binary.h"
 
@@ -55,10 +57,12 @@ struct Node {
     uint32_t seq;                    // header.seq
     uint64_t stamp_ns;               // the record's time
     double odom[7];
-    Cloud cloud;                     // data_off: in the file, or in the decoded chunk when lz >= 0
+    Cloud cloud;                     // data_off: in the file, or in the decoded chunk when lz >= 0 or bz >= 0
     int64_t lz = -1;                 // the LZ4 chunk (Index::lz4) holding the node, else -1
-    uint64_t rec = 0;                // lz >= 0: the index entry's offset of the message record in the decoded chunk
-    uint32_t conn = 0;               // lz >= 0: the index entry's connection
+    int64_t bz = -1;                 // the bz2 chunk (Index::bz2) holding the node, else -1
+    uint64_t rec = 0;                // in a compressed chunk: the index entry's offset of the message record in the decoded chunk
+    uint32_t conn = 0;               // in a compressed chunk: the index entry's connection
+    bool decoded() const { return lz >= 0 || bz >= 0; }
 };
 
 // an LZ4 chunk: the record, its data in the file, its decoded length and its frame's block table
@@ -68,13 +72,20 @@ struct Lz4Chunk {
     lz4::Frame frame;
 };
 
+// a bz2 chunk: the record, its data in the file, its decoded length and its stream's level (the host reads the 4-byte header only)
+struct Bz2Chunk {
+    uint64_t rec, data, len;
+    uint32_t size, level;
+};
+
 struct Index {
     std::vector<Node> nodes;         // selected, in delivery order, the first dropped unless keep_first
     std::string md5sum;
     uint64_t chunks = 0, connections = 0, messages = 0, selected = 0, unknown = 0;
     uint64_t total_points = 0, intensity_zero_filled = 0, big_endian = 0;
     std::vector<Lz4Chunk> lz4;       // every LZ4 chunk of the file, in file order
-    std::vector<uint64_t> pending;   // the nodes in LZ4 chunks, parsed after their chunks are decoded (finish_lz4)
+    std::vector<Bz2Chunk> bz2;       // every bz2 chunk of the file, in file order
+    std::vector<uint64_t> pending;   // the nodes in compressed chunks, parsed after their chunks are decoded (finish_chunks)
     int fail_rc = 0;                 // the first node parsed on the host that failed, when it follows a pending one
     std::string fail_msg;
 };
@@ -268,9 +279,19 @@ inline const Field* need(const std::vector<Field>& fs, const char* name, uint64_
     return x;
 }
 
+// the 4-byte header of the bzip2 stream b[0, len): ERASOR_OK with *level, or the code with msg
+inline int bz2_header(const uint8_t* b, uint64_t len, uint32_t* level, std::string& msg) {
+    if (len < 3 || b[0] != 'B' || b[1] != 'Z' || b[2] != 'h') { msg = "its data does not start with 'BZh' (a bzip1 or other stream?)"; return ERASOR_E_UNSUPPORTED; }
+    if (len < 4) { msg = "the stream runs past the chunk (bit 24 of the chunk data)"; return ERASOR_E_INVALID; }
+    if (b[3] < '1' || b[3] > '9') { msg = "level digit " + std::to_string(b[3]) + " is not '1'..'9' (bit 24 of the chunk data)"; return ERASOR_E_INVALID; }
+    *level = (uint32_t)(b[3] - '0');
+    return ERASOR_OK;
+}
+
 struct Conn { std::string topic, type, md5sum; bool defined = false; };
-// a message: its record and data in the file; or (lz >= 0) an index entry of LZ4 chunk lz, rec its offset in the decoded chunk
-struct Msg { uint32_t conn; uint64_t time_ns, rec, data, len; int64_t lz = -1; };
+// a message: its record and data in the file; or (lz >= 0 / bz >= 0) an index entry of LZ4 chunk lz / bz2 chunk bz, rec its offset
+// in the decoded chunk
+struct Msg { uint32_t conn; uint64_t time_ns, rec, data, len; int64_t lz = -1, bz = -1; };
 
 struct Walk {
     const uint8_t* f;
@@ -279,22 +300,24 @@ struct Walk {
     std::vector<Msg> msgs;
     uint64_t chunks = 0, unknown = 0;
     std::vector<Lz4Chunk> lz4;
-    std::vector<Msg> entries;         // the index entries of the last LZ4 chunk, while its index data records follow it
+    std::vector<Bz2Chunk> bz2;
+    std::vector<Msg> entries;         // the index entries of the last compressed chunk, while its index data records follow it
     Err e;
 
-    // the last LZ4 chunk's messages, from the index data records that followed it: in file order, by offset in the chunk
+    // the last compressed chunk's messages, from the index data records that followed it: in file order, by offset in the chunk
     bool close_lz4() {
         if (!open) return true;
         if (entries.empty())
-            return e.set(ERASOR_E_UNSUPPORTED, "chunk" + at(lz4.back().rec) + " is lz4-compressed and no index data record follows it: "
-                                                   "an unindexed bag is not read");
+            return e.set(ERASOR_E_UNSUPPORTED, "chunk" + at(open_bz2 ? bz2.back().rec : lz4.back().rec) + " is " + (open_bz2 ? "bz2" : "lz4") +
+                                                   "-compressed and no index data record follows it: an unindexed bag is not read");
         std::stable_sort(entries.begin(), entries.end(), [](const Msg& a, const Msg& b) { return a.rec < b.rec; });
         msgs.insert(msgs.end(), entries.begin(), entries.end());
         entries.clear();
         open = false;
         return true;
     }
-    bool open = false;                // an LZ4 chunk was the last chunk and its index data records are being read
+    bool open = false;                // a compressed chunk was the last chunk and its index data records are being read
+    bool open_bz2 = false;            // ... and it is a bz2 chunk
 
     Conn& conn(uint32_t id) {
         if (id >= conns.size()) conns.resize((size_t)id + 1);
@@ -345,10 +368,22 @@ struct Walk {
                 ++chunks;
                 lz4.push_back(std::move(k));
                 open = true;
+                open_bz2 = false;
+                return true;
+            }
+            if (comp == "bz2") {             // the stream header only: the device finds the blocks (DESIGN.md section 12.2.2)
+                uint32_t level = 0;
+                std::string m;
+                const int hr = bz2_header(f + d0, dl, &level, m);
+                if (hr != ERASOR_OK) return e.set(hr, "bz2 chunk" + at(rec) + ": " + m);
+                ++chunks;
+                bz2.push_back(Bz2Chunk{rec, d0, dl, rd32(f + s->off), level});
+                open = true;
+                open_bz2 = true;
                 return true;
             }
             if (comp != "none")
-                return e.set(ERASOR_E_UNSUPPORTED, "chunk" + at(rec) + " is compressed with '" + comp + "': only uncompressed and lz4 chunks are read");
+                return e.set(ERASOR_E_UNSUPPORTED, "chunk" + at(rec) + " is compressed with '" + comp + "': only uncompressed, lz4 and bz2 chunks are read");
             if (rd32(f + s->off) != dl)
                 return e.set(ERASOR_E_INVALID, "chunk" + at(rec) + " holds " + std::to_string(dl) + " bytes of data, its 'size' says " +
                                                    std::to_string(rd32(f + s->off)));
@@ -392,7 +427,7 @@ struct Walk {
                 const Field* cn = find(fs, "conn");
                 for (uint64_t q = d0; q < d0 + dl; q += 12)
                     entries.push_back(Msg{rd32(f + cn->off), (uint64_t)rd32(f + q) * 1000000000ull + rd32(f + q + 4), rd32(f + q + 8), 0, 0,
-                                          (int64_t)lz4.size() - 1});
+                                          open_bz2 ? -1 : (int64_t)lz4.size() - 1, open_bz2 ? (int64_t)bz2.size() - 1 : -1});
             }
             return true;
         }
@@ -468,6 +503,7 @@ inline int build_index(const uint8_t* file, uint64_t len, const std::string& top
     detail::Walk w{file};
     if (!w.records(13, len, false) || !w.close_lz4()) { msg = w.e.msg; return w.e.rc; }
     out.lz4 = std::move(w.lz4);
+    out.bz2 = std::move(w.bz2);
     out.chunks = w.chunks;
     out.unknown = w.unknown;
     out.connections = w.conn_ids.size();
@@ -493,8 +529,9 @@ inline int build_index(const uint8_t* file, uint64_t len, const std::string& top
     detail::Err e;
     for (size_t k = first; k < sel.size(); ++k) {
         Node& nd = out.nodes[k - first];
-        if (sel[k].lz >= 0) {                         // parsed once its chunk is decoded (finish_lz4)
+        if (sel[k].lz >= 0 || sel[k].bz >= 0) {       // parsed once its chunk is decoded (finish_chunks)
             nd.lz = sel[k].lz;
+            nd.bz = sel[k].bz;
             nd.rec = sel[k].rec;
             nd.conn = sel[k].conn;
             nd.stamp_ns = sel[k].time_ns;
@@ -511,17 +548,24 @@ inline int build_index(const uint8_t* file, uint64_t len, const std::string& top
     return ERASOR_OK;
 }
 
-// ---- nodes in LZ4 chunks: what the device (or the host build, serially) decodes and parses ---------------------------------
-// A block of the decode, a chunk, and a node to parse, as the kernels read them
+// ---- nodes in compressed chunks: what the device (or the host build, serially) decodes and parses --------------------------------
+// A block of the LZ4 decode, an LZ4 chunk, a bz2 chunk, and a node to parse, as the kernels read them
 struct Lz4Block {
     uint64_t src;                    // its data in the device copy of the compressed chunks
     uint32_t csize, stored, cap;     // cap: the frame's block max
-    uint32_t chunk;                  // its chunk in Lz4Plan::chunks
+    uint32_t chunk;                  // its chunk in ChunkPlan::chunks
     uint32_t has_sum, sum;
 };
 struct Lz4ChunkDesc {
     uint64_t src, dec;               // its compressed data in the device copy, its decoded data in the decoded buffer
     uint32_t size, block0, nblocks, has_sum, sum, pad_;
+};
+struct Bz2ChunkDesc {
+    uint64_t src, len;               // its stream in the device copy of the bz2 chunks, its length
+    uint64_t dec;                    // its decoded data in the decoded buffer
+    uint64_t tt;                     // its blocks' slots in the BWT buffers: ceil(5 size / 4) bytes
+    uint64_t cand_cap;               // max_candidates(len)
+    uint32_t size, level;
 };
 struct Lz4NodeIn { uint64_t dec, len, rec, time_ns; uint32_t conn, pad_; };   // the decoded chunk [dec, dec + len), the index entry
 struct NodeOut {
@@ -531,19 +575,27 @@ struct NodeOut {
     Cloud cloud;
 };
 
-struct Lz4Plan {
+// the BWT buffers of a bz2 chunk of decoded length `size`: the tt bytes of its true blocks total at most ceil(5 size / 4), as RLE1
+// turns at most 5 bytes into 4
+PCD_HD uint64_t tt_cap(uint32_t size) { return (5ull * size + 3) / 4; }
+
+struct ChunkPlan {
     std::vector<uint32_t> chunks;    // Index::lz4 ids holding a kept node, in file order
     std::vector<Lz4ChunkDesc> cd;
     std::vector<Lz4Block> blocks;
+    std::vector<uint32_t> bz_chunks; // Index::bz2 ids holding a kept node, in file order
+    std::vector<Bz2ChunkDesc> bd;
     std::vector<Lz4NodeIn> nodes;    // Index::pending, in order
     std::vector<int64_t> slot;       // Index::lz4 id -> its entry of chunks / cd, or -1
+    std::vector<int64_t> bz_slot;    // Index::bz2 id -> its entry of bz_chunks / bd, or -1
     uint64_t src_bytes = 0, dec_bytes = 0, stored = 0, block_sums = 0, content_sums = 0;
+    uint64_t bz_src_bytes = 0, bz_tt_bytes = 0, bz_cands = 0;   // bz2: the bounds every buffer is sized from
 };
 
-// where node nd (in an LZ4 chunk) has its decoded chunk in the decoded buffer
-inline uint64_t dec_of(const Lz4Plan& p, const Node& nd) { return p.cd[p.slot[nd.lz]].dec; }
+// where node nd (in a compressed chunk) has its decoded chunk in the decoded buffer
+inline uint64_t dec_of(const ChunkPlan& p, const Node& nd) { return nd.lz >= 0 ? p.cd[p.slot[nd.lz]].dec : p.bd[p.bz_slot[nd.bz]].dec; }
 
-inline void fill_lz4_stats(const Index& x, const Lz4Plan& p, erasor_bag_lz4_stats_t& s) {
+inline void fill_lz4_stats(const Index& x, const ChunkPlan& p, erasor_bag_lz4_stats_t& s) {
     s = erasor_bag_lz4_stats_t{};
     s.chunks = x.lz4.size();
     s.decoded_chunks = p.chunks.size();
@@ -552,6 +604,22 @@ inline void fill_lz4_stats(const Index& x, const Lz4Plan& p, erasor_bag_lz4_stat
     s.stored_blocks = p.stored;
     s.block_checksums = p.block_sums;
     s.content_checksums = p.content_sums;
+}
+
+// what the bz2 decode found: per decoded chunk its true blocks; the candidates of all
+struct Bz2Found {
+    std::vector<uint32_t> blocks;
+    uint64_t candidates = 0;
+};
+
+inline void fill_bz2_stats(const Index& x, const ChunkPlan& p, const Bz2Found& f, erasor_bag_bz2_stats_t& s) {
+    s = erasor_bag_bz2_stats_t{};
+    s.chunks = x.bz2.size();
+    for (const Bz2Chunk& k : x.bz2) ++s.streams_by_level[k.level - 1];
+    s.decoded_chunks = p.bz_chunks.size();
+    for (uint32_t c : p.bz_chunks) { s.compressed_bytes += x.bz2[c].len; s.decoded_bytes += x.bz2[c].size; }
+    for (uint32_t b : f.blocks) s.blocks += b;
+    s.candidates = f.candidates;
 }
 
 // the decode error key: the first broken rule in (block, byte) order wins an atomicMin
@@ -563,15 +631,101 @@ PCD_HD uint64_t block_key(const Lz4Block& B, uint64_t b, uint32_t byte, uint32_t
 PCD_HD uint64_t chunk_key(const Lz4ChunkDesc& d, uint64_t c, uint32_t reason) {
     return err_key((uint64_t)d.block0 + d.nblocks + c, reason == lz4::R_SIZE ? 0 : 1, reason);    // a short frame before its checksum
 }
+// the bz2 error key, its own atomicMin: the decoded bz2 chunk (file order), then the bit of its data where the rule broke (the
+// block's magic for a rule checked after the walk, the chunk's end for its decoded length), then the reason
+PCD_HD uint64_t bz2_key(uint64_t c, uint64_t bit, uint32_t reason) { return c << 44 | (bit & 0xFFFFFFFFFull) << 8 | reason; }
+constexpr uint64_t kMaxBz2Chunks = 1ull << 20;
 
-inline void plan_lz4(const Index& x, Lz4Plan& p) {
-    p = Lz4Plan();
-    std::vector<int64_t>& slot = p.slot;
-    slot.assign(x.lz4.size(), -1);
-    for (uint64_t k : x.pending) slot[x.nodes[k].lz] = 0;
-    for (size_t c = 0; c < x.lz4.size(); ++c) {
-        if (slot[c] < 0) continue;
-        slot[c] = (int64_t)p.chunks.size();
+// a candidate block of the bz2 decode: the bit of its chunk's data holding the block magic, and the chunk (ChunkPlan::bd)
+struct Bz2Cand { uint64_t bit; uint32_t chunk, pad_; };
+
+// The chain of decoded bz2 chunk c (data d, candidates [c0, c1) in bit order, walked): from bit 32, each position must hold a
+// candidate whose walk succeeded (a true block, given block number blkno and, while the blocks' lengths fit tt_cap, its BWT slot
+// tt_off) or the end-of-stream magic, its stream CRC and the chunk's end.  The key of the first broken rule, or ~0 with *nblocks.
+PCD_HD uint64_t bz2_chain(uint64_t c, const Bz2ChunkDesc& D, const uint8_t* d, const Bz2Cand* cand, uint64_t c0, uint64_t c1,
+                          const bz2::Walk* walk, int32_t* blkno, uint64_t* tt_off, uint32_t* nblocks) {
+    const uint64_t nbits = 8 * D.len, cap = tt_cap(D.size);
+    uint64_t pos = 32, tt = 0, i = c0, key = ~0ull;
+    uint32_t blk = 0, comb = 0;
+    for (;;) {
+        while (i < c1 && cand[i].bit < pos) ++i;
+        if (i < c1 && cand[i].bit == pos) {
+            const bz2::Walk w = walk[i];
+            blkno[i] = (int32_t)blk;
+            if (w.reason != bz2::R_OK) return bz2_key(c, w.where, w.reason);
+            if (key == ~0ull && w.n <= cap - tt) { tt_off[i] = D.tt + tt; tt += w.n; }
+            else key = bz2_key(c, nbits, bz2::R_SIZE);        // more than the chunk's size can need: decode no further block
+            comb = (comb << 1 | comb >> 31) ^ w.crc;
+            pos = w.end;
+            ++blk;
+            continue;
+        }
+        uint64_t k;
+        if (nbits - pos < 48) k = bz2_key(c, pos, bz2::R_PAST);
+        else if (bz2::magic_at(d, pos) != bz2::kEosMagic) k = bz2_key(c, pos, bz2::R_NO_MAGIC);
+        else if (nbits - pos - 48 < 32) k = bz2_key(c, pos + 48, bz2::R_PAST);
+        else {
+            bz2::Bits b{d, pos + 48, nbits};
+            const uint32_t stored = b.get(32);
+            const uint64_t end = (pos + 80 + 7) / 8;
+            if (end != D.len) {
+                const bool bzh = D.len - end >= 3 && d[end] == 'B' && d[end + 1] == 'Z' && d[end + 2] == 'h';
+                k = bz2_key(c, 8 * end, bzh ? bz2::R_SECOND_STREAM : bz2::R_TRAILING);
+            } else if (stored != comb) {
+                k = bz2_key(c, pos + 48, bz2::R_STREAM_CRC);
+            } else {
+                *nblocks = blk;
+                return key;
+            }
+        }
+        return k < key ? k : key;
+    }
+}
+
+// The placement of decoded bz2 chunk c's blocks (RLE1 output lengths osize, ~0 for a block that failed): their offsets in the
+// decoded buffer, or ~0 for all unless they add up to the chunk's size.  The key of a wrong decoded length, or ~0.
+PCD_HD uint64_t bz2_place(uint64_t c, const Bz2ChunkDesc& D, uint64_t c0, uint64_t c1, const uint64_t* tt_off, const uint64_t* osize, uint64_t* out_off) {
+    uint64_t s = 0;
+    bool failed = false;
+    for (uint64_t i = c0; i < c1; ++i)
+        if (tt_off[i] != ~0ull) { if (osize[i] == ~0ull) failed = true; else s += osize[i]; }
+    const bool ok = !failed && s == D.size;
+    s = 0;
+    for (uint64_t i = c0; i < c1; ++i)
+        if (tt_off[i] != ~0ull) { out_off[i] = ok ? D.dec + s : ~0ull; s += ok ? osize[i] : 0; }
+    return ok || failed ? ~0ull : bz2_key(c, 8 * D.len, bz2::R_SIZE);
+}
+
+inline void plan_chunks(const Index& x, ChunkPlan& p) {
+    p = ChunkPlan();
+    p.slot.assign(x.lz4.size(), -1);
+    p.bz_slot.assign(x.bz2.size(), -1);
+    for (uint64_t k : x.pending) {
+        const Node& nd = x.nodes[k];
+        if (nd.lz >= 0) p.slot[nd.lz] = 0;
+        else p.bz_slot[nd.bz] = 0;
+    }
+    // the kept chunks of both kinds in file order: the decoded buffer holds their slots in that order
+    std::vector<std::pair<uint64_t, int64_t>> order;      // (record, lz4 id or -1 - bz2 id)
+    for (size_t c = 0; c < x.lz4.size(); ++c) if (p.slot[c] >= 0) order.push_back({x.lz4[c].rec, (int64_t)c});
+    for (size_t c = 0; c < x.bz2.size(); ++c) if (p.bz_slot[c] >= 0) order.push_back({x.bz2[c].rec, -1 - (int64_t)c});
+    std::sort(order.begin(), order.end());
+    for (const auto& o : order) {
+        if (o.second < 0) {
+            const size_t c = (size_t)(-1 - o.second);
+            const Bz2Chunk& k = x.bz2[c];
+            p.bz_slot[c] = (int64_t)p.bz_chunks.size();
+            p.bz_chunks.push_back((uint32_t)c);
+            const uint64_t cands = bz2::max_candidates(k.len);
+            p.bd.push_back(Bz2ChunkDesc{p.bz_src_bytes, k.len, p.dec_bytes, p.bz_tt_bytes, cands, k.size, k.level});
+            p.bz_src_bytes += (k.len + 15) & ~15ull;
+            p.bz_tt_bytes += (tt_cap(k.size) + 15) & ~15ull;
+            p.bz_cands += cands;
+            p.dec_bytes += ((uint64_t)k.size + 15) & ~15ull;
+            continue;
+        }
+        const size_t c = (size_t)o.second;
+        p.slot[c] = (int64_t)p.chunks.size();
         p.chunks.push_back((uint32_t)c);
         const Lz4Chunk& k = x.lz4[c];
         Lz4ChunkDesc d{p.src_bytes, p.dec_bytes, k.size, (uint32_t)p.blocks.size(), (uint32_t)k.frame.blocks.size(), k.frame.content_sum, k.frame.sum, 0};
@@ -587,13 +741,13 @@ inline void plan_lz4(const Index& x, Lz4Plan& p) {
     }
     for (uint64_t k : x.pending) {
         const Node& nd = x.nodes[k];
-        const Lz4ChunkDesc& d = p.cd[slot[nd.lz]];
-        p.nodes.push_back(Lz4NodeIn{d.dec, d.size, nd.rec, nd.stamp_ns, nd.conn, 0});
+        const uint64_t dec = dec_of(p, nd), size = nd.lz >= 0 ? x.lz4[nd.lz].size : x.bz2[nd.bz].size;
+        p.nodes.push_back(Lz4NodeIn{dec, size, nd.rec, nd.stamp_ns, nd.conn, 0});
     }
 }
 
-// the message of a decode error key
-inline std::string lz4_error(const Index& x, const Lz4Plan& p, uint64_t key) {
+// the message of an LZ4 decode error key
+inline std::string lz4_error(const Index& x, const ChunkPlan& p, uint64_t key) {
     const uint64_t u = key >> 28;
     const uint32_t byte = (uint32_t)(key >> 5) & 0x7FFFFFu, r = (uint32_t)key & 31u;
     size_t c = 0;                                    // the chunk whose units [block0 + c, block0 + c + nblocks] hold u
@@ -608,16 +762,49 @@ inline std::string lz4_error(const Index& x, const Lz4Plan& p, uint64_t key) {
            " of the frame)";
 }
 
+// the message of a bz2 decode error key; blk: the last block of the chunk starting at or before the key's bit (-1: none)
+inline std::string bz2_error(const Index& x, const ChunkPlan& p, uint64_t key, int64_t blk, int* rc) {
+    const uint64_t c = key >> 44, bit = (key >> 8) & 0xFFFFFFFFFull;
+    const uint32_t r = (uint32_t)key & 0xFFu;
+    const Bz2Chunk& k = x.bz2[p.bz_chunks[c]];
+    *rc = bz2::unsupported(r) ? ERASOR_E_UNSUPPORTED : ERASOR_E_INVALID;
+    const std::string m = "bz2 chunk" + detail::at(k.rec) + ": ";
+    if (r == bz2::R_SIZE) return m + "its stream does not decode to the chunk's 'size' of " + std::to_string(k.size) + " bytes";
+    if (r == bz2::R_TRAILING || r == bz2::R_SECOND_STREAM) return m + bz2::reason_text(r) + " (byte " + std::to_string(bit / 8) + " of the chunk data)";
+    const std::string where = " (bit " + std::to_string(bit) + " of the chunk data)";
+    if (r == bz2::R_STREAM_CRC) return m + bz2::reason_text(r) + where;
+    if (r == bz2::R_NO_MAGIC || (r == bz2::R_PAST && blk < 0))
+        return m + bz2::reason_text(r) + (blk < 0 ? " after the stream header" : " after block " + std::to_string(blk)) + where;
+    return m + "block " + std::to_string(blk) + ": " + bz2::reason_text(r) + where;
+}
+
+// the first of the two decode errors in file order (an LZ4 key and a bz2 key, ~0 for none): its code and message, or ERASOR_OK
+inline int decode_error(const Index& x, const ChunkPlan& p, uint64_t lz_key, uint64_t bz_key, int64_t bz_blk, std::string& msg) {
+    if (lz_key == ~0ull && bz_key == ~0ull) return ERASOR_OK;
+    uint64_t lz_rec = ~0ull, bz_rec = ~0ull;
+    if (lz_key != ~0ull) {
+        const uint64_t u = lz_key >> 28;
+        size_t c = 0;
+        while (c + 1 < p.cd.size() && (uint64_t)p.cd[c + 1].block0 + c + 1 <= u) ++c;
+        lz_rec = x.lz4[p.chunks[c]].rec;
+    }
+    if (bz_key != ~0ull) bz_rec = x.bz2[p.bz_chunks[bz_key >> 44]].rec;
+    if (lz_rec < bz_rec) { msg = lz4_error(x, p, lz_key); return ERASOR_E_INVALID; }
+    int rc = ERASOR_E_INVALID;
+    msg = bz2_error(x, p, bz_key, bz_blk, &rc);
+    return rc;
+}
+
 // The nodes of x.pending from their parse (res, in x.pending's order), then the first failure in delivery order: ERASOR_OK or an
 // error code with msg (the index is then cleared)
-inline int finish_lz4(Index& x, const NodeOut* res, std::string& msg) {
+inline int finish_chunks(Index& x, const NodeOut* res, std::string& msg) {
     detail::Err e;
     for (size_t i = 0; i < x.pending.size() && e.rc == ERASOR_OK; ++i) {
         const uint64_t k = x.pending[i];
         Node& nd = x.nodes[k];
         const NodeOut& r = res[i];
-        const std::string who = "node " + std::to_string(k) + " (message record at byte " + std::to_string(nd.rec) + " of lz4 chunk" +
-                                detail::at(x.lz4[nd.lz].rec) + ")";
+        const std::string who = "node " + std::to_string(k) + " (message record at byte " + std::to_string(nd.rec) + " of " +
+                                (nd.lz >= 0 ? "lz4 chunk" + detail::at(x.lz4[nd.lz].rec) : "bz2 chunk" + detail::at(x.bz2[nd.bz].rec)) + ")";
         if (!detail::node_fail(r.code, r.a, r.b, who, e)) break;
         nd.seq = r.seq;
         std::memcpy(nd.odom, r.odom, sizeof(nd.odom));

@@ -240,12 +240,13 @@ int erasor_hostcheck_lzf_decode(const uint8_t* s, uint64_t csize, uint8_t* out, 
 
 // ---- erasor/node bags: bag_index.h's index, and its per-point decode run serially (what erasor_bag_load's gather computes) ----
 static bag::Index g_bag;
-static bag::Lz4Plan g_plan;
-static std::vector<uint8_t> g_dec;                   // the decoded LZ4 chunks, laid out as the device's decoded buffer
+static bag::ChunkPlan g_plan;
+static bag::Bz2Found g_found;
+static std::vector<uint8_t> g_dec;                   // the decoded lz4 and bz2 chunks, laid out as the device's decoded buffer
 
-// The stages of erasor_bag_index's LZ4 decode and node parse (pcd_kernels.cu), serially: the key of the first broken rule or ~0;
-// res gets one NodeOut per pending node
-static uint64_t lz4_stages(const uint8_t* file, const bag::Index& x, const bag::Lz4Plan& p, std::vector<uint8_t>& dec, std::vector<bag::NodeOut>& res) {
+// The stages of erasor_bag_index's LZ4 decode (pcd_kernels.cu), serially, into dec (sized here): the key of the first broken rule
+// or ~0
+static uint64_t lz4_stages(const uint8_t* file, const bag::Index& x, const bag::ChunkPlan& p, std::vector<uint8_t>& dec) {
     std::vector<uint8_t> src(std::max<uint64_t>(p.src_bytes, 1));
     for (size_t c = 0; c < p.chunks.size(); ++c) {
         const bag::Lz4Chunk& k = x.lz4[p.chunks[c]];
@@ -286,6 +287,74 @@ static uint64_t lz4_stages(const uint8_t* file, const bag::Index& x, const bag::
         const bag::Lz4ChunkDesc& d = p.cd[c];
         if (d.has_sum && lz4::xxh32(dec.data() + d.dec, d.size, 0) != d.sum) err = std::min(err, bag::chunk_key(d, c, lz4::R_CONTENT_SUM));
     }
+    return err;
+}
+
+// The stages of erasor_bag_index's bz2 decode (pcd_kernels.cu), serially, into dec: the bz2 key of the first broken rule or ~0, *blk
+// the block it names; found gets the blocks and candidates
+static uint64_t bz2_stages(const uint8_t* file, const bag::Index& x, const bag::ChunkPlan& p, std::vector<uint8_t>& dec, int64_t* blk, bag::Bz2Found& found) {
+    const size_t nc = p.bd.size();
+    std::vector<uint8_t> src(std::max<uint64_t>(p.bz_src_bytes, 1));
+    for (size_t c = 0; c < nc; ++c) std::memcpy(src.data() + p.bd[c].src, file + x.bz2[p.bz_chunks[c]].data, p.bd[c].len);
+    std::vector<bag::Bz2Cand> cand;                   // k_bz2_scan, the scan, k_bz2_emit
+    std::vector<uint64_t> c0(nc + 1);
+    for (size_t c = 0; c < nc; ++c) {
+        const bag::Bz2ChunkDesc& D = p.bd[c];
+        c0[c] = cand.size();
+        for (uint64_t q = 0; q < D.len; ++q)
+            if (const uint32_t j = bz2::candidate_at(src.data() + D.src, D.len, q)) cand.push_back(bag::Bz2Cand{8 * q + j - 1, (uint32_t)c, 0});
+    }
+    c0[nc] = cand.size();
+    const size_t n = cand.size();
+    found.candidates = n;
+    found.blocks.assign(nc, 0);
+    static bz2::Tables T;
+    std::vector<bz2::Walk> walk(n);                   // k_bz2_walk
+    for (size_t i = 0; i < n; ++i) {
+        const bag::Bz2ChunkDesc& D = p.bd[cand[i].chunk];
+        walk[i] = bz2::block(src.data() + D.src, 8 * D.len, cand[i].bit, D.level, T, nullptr, nullptr);
+    }
+    std::vector<int32_t> blkno(n, -1);
+    std::vector<uint64_t> tt_off(n, ~0ull), osize(n, ~0ull), out_off(n, ~0ull);
+    uint64_t err = ~0ull;
+    for (size_t c = 0; c < nc; ++c)                   // k_bz2_chain
+        err = std::min(err, bag::bz2_chain(c, p.bd[c], src.data() + p.bd[c].src, cand.data(), c0[c], c0[c + 1], walk.data(), blkno.data(), tt_off.data(),
+                                           &found.blocks[c]));
+    std::vector<uint8_t> tt(std::max<uint64_t>(p.bz_tt_bytes, 1)), bw(tt.size());
+    std::vector<uint32_t> lf(tt.size());
+    uint32_t tab[256];
+    bz2::crc_table(tab);
+    for (size_t i = 0; i < n; ++i) {
+        if (tt_off[i] == ~0ull) continue;
+        const bag::Bz2ChunkDesc& D = p.bd[cand[i].chunk];
+        uint32_t hist[256];                           // k_bz2_decode
+        const bz2::Walk w = bz2::block(src.data() + D.src, 8 * D.len, cand[i].bit, D.level, T, tt.data() + tt_off[i], hist);
+        bz2::lf_vector(tt.data() + tt_off[i], w.n, hist, lf.data() + tt_off[i]);
+        bz2::unbwt_serial(tt.data() + tt_off[i], lf.data() + tt_off[i], w.n, w.orig, bw.data() + tt_off[i]);               // k_bz2_bwt
+        uint64_t os = 0;
+        uint32_t crc = 0;
+        uint32_t r = bz2::rle1(bw.data() + tt_off[i], w.n, tab, nullptr, &os, &crc);                                     // k_bz2_rle
+        if (r == bz2::R_OK && crc != w.crc) r = bz2::R_BLOCK_CRC;
+        if (r != bz2::R_OK) err = std::min(err, bag::bz2_key(cand[i].chunk, cand[i].bit, r));
+        osize[i] = r == bz2::R_OK ? os : ~0ull;
+    }
+    for (size_t c = 0; c < nc; ++c)                   // k_bz2_place
+        err = std::min(err, bag::bz2_place(c, p.bd[c], c0[c], c0[c + 1], tt_off.data(), osize.data(), out_off.data()));
+    for (size_t i = 0; i < n; ++i) {                  // k_bz2_expand
+        if (out_off[i] == ~0ull) continue;
+        uint64_t os = 0;
+        uint32_t crc = 0;
+        bz2::rle1(bw.data() + tt_off[i], walk[i].n, tab, dec.data() + out_off[i], &os, &crc);
+    }
+    *blk = -1;                                        // k_bz2_errblock
+    if (err != ~0ull)
+        for (size_t i = 0; i < n; ++i)
+            if (blkno[i] >= 0 && cand[i].chunk == err >> 44 && cand[i].bit <= ((err >> 8) & 0xFFFFFFFFFull)) *blk = std::max<int64_t>(*blk, blkno[i]);
+    return err;
+}
+
+// k_bag_parse, serially
+static void parse_stage(const bag::ChunkPlan& p, const std::vector<uint8_t>& dec, std::vector<bag::NodeOut>& res) {
     res.assign(p.nodes.size(), bag::NodeOut{});
     for (size_t i = 0; i < p.nodes.size(); ++i) {     // k_bag_parse
         const bag::Lz4NodeIn& n = p.nodes[i];
@@ -294,7 +363,6 @@ static uint64_t lz4_stages(const uint8_t* file, const bag::Index& x, const bag::
         r.code = bag::record_core(dec.data() + n.dec, n.len, n.rec, n.conn, n.time_ns, &d0, &d1, &r.a);
         if (r.code == bag::NF_OK) r.code = bag::parse_node_core(dec.data() + n.dec, d0, d1, &r.seq, r.odom, r.cloud, &r.a, &r.b);
     }
-    return err;
 }
 
 // erasor_bag_index on the host; the index is kept for the two calls below
@@ -303,19 +371,23 @@ int erasor_hostcheck_bag_index(const char* file, size_t len, const char* topic, 
     std::string msg;
     *n_nodes = 0;
     *info = erasor_bag_info_t{};
-    g_plan = bag::Lz4Plan();
+    g_plan = bag::ChunkPlan();
+    g_found = bag::Bz2Found();
     g_dec.clear();
     const uint8_t* f = reinterpret_cast<const uint8_t*>(file);
     int rc = bag::build_index(f, len, topic ? topic : "/node/combined/optimized", keep_first != 0, g_bag, msg);
     if (rc == ERASOR_OK && !g_bag.pending.empty()) {
-        bag::plan_lz4(g_bag, g_plan);
+        bag::plan_chunks(g_bag, g_plan);
         std::vector<bag::NodeOut> res;
-        const uint64_t key = lz4_stages(f, g_bag, g_plan, g_dec, res);
-        if (key != ~0ull) { msg = bag::lz4_error(g_bag, g_plan, key); rc = ERASOR_E_INVALID; }
-        else rc = bag::finish_lz4(g_bag, res.data(), msg);
+        const uint64_t key = lz4_stages(f, g_bag, g_plan, g_dec);
+        int64_t blk = -1;
+        const uint64_t bz_key = bz2_stages(f, g_bag, g_plan, g_dec, &blk, g_found);
+        parse_stage(g_plan, g_dec, res);
+        rc = bag::decode_error(g_bag, g_plan, key, bz_key, blk, msg);
+        if (rc == ERASOR_OK) rc = bag::finish_chunks(g_bag, res.data(), msg);
     }
     set_err(err, errcap, msg);
-    if (rc != ERASOR_OK) { g_bag = bag::Index(); g_plan = bag::Lz4Plan(); return rc; }
+    if (rc != ERASOR_OK) { g_bag = bag::Index(); g_plan = bag::ChunkPlan(); g_found = bag::Bz2Found(); return rc; }
     *n_nodes = g_bag.nodes.size();
     bag::fill_info(g_bag, *info);
     return ERASOR_OK;
@@ -324,6 +396,36 @@ int erasor_hostcheck_bag_index(const char* file, size_t len, const char* topic, 
 // erasor_bag_lz4_stats of the last erasor_hostcheck_bag_index
 int erasor_hostcheck_bag_lz4_stats(erasor_bag_lz4_stats_t* s) {
     bag::fill_lz4_stats(g_bag, g_plan, *s);
+    return ERASOR_OK;
+}
+
+// One bzip2 stream s[0, len) of decoded length `size` through the bz2 stages, as a bz2 chunk at byte 0 of a file: out (size bytes)
+// gets the decoded data; the return is what erasor_bag_index returns for such a chunk, err its message
+int erasor_hostcheck_bz2_stream(const uint8_t* s, uint64_t len, uint32_t size, uint8_t* out, char* err, size_t errcap) {
+    bag::Index x;
+    uint32_t level = 0;
+    std::string msg;
+    int rc = bag::detail::bz2_header(s, len, &level, msg);
+    if (rc != ERASOR_OK) { set_err(err, errcap, "bz2 chunk at byte 0: " + msg); return rc; }
+    x.bz2.push_back(bag::Bz2Chunk{0, 0, len, size, level});
+    x.nodes.resize(1);
+    x.nodes[0].bz = 0;
+    x.pending.push_back(0);
+    bag::ChunkPlan p;
+    bag::plan_chunks(x, p);
+    std::vector<uint8_t> dec(std::max<uint64_t>(p.dec_bytes, 1));
+    bag::Bz2Found found;
+    int64_t blk = -1;
+    const uint64_t key = bz2_stages(s, x, p, dec, &blk, found);
+    rc = bag::decode_error(x, p, ~0ull, key, blk, msg);
+    set_err(err, errcap, msg);
+    if (rc == ERASOR_OK) std::memcpy(out, dec.data(), size);
+    return rc;
+}
+
+// erasor_bag_bz2_stats of the last erasor_hostcheck_bag_index, without the times and the scratch
+int erasor_hostcheck_bag_bz2_stats(erasor_bag_bz2_stats_t* s) {
+    bag::fill_bz2_stats(g_bag, g_plan, g_found, *s);
     return ERASOR_OK;
 }
 
@@ -353,7 +455,7 @@ int erasor_hostcheck_bag_decode(const char* file, size_t first, size_t count, fl
     for (size_t k = 0; k < count; ++k) {
         const bag::Node& nd = g_bag.nodes[first + k];
         const bag::Cloud& c = nd.cloud;
-        const uint8_t* d = (nd.lz >= 0 ? g_dec.data() + bag::dec_of(g_plan, nd) : reinterpret_cast<const uint8_t*>(file)) + c.data_off;
+        const uint8_t* d = (nd.decoded() ? g_dec.data() + bag::dec_of(g_plan, nd) : reinterpret_cast<const uint8_t*>(file)) + c.data_off;
         const uint64_t n = bag::cloud_points(c);
         uint32_t* o = reinterpret_cast<uint32_t*>(out) + 4 * offsets[k];
         for (uint64_t i = 0; i < n; ++i) bag::point_values(d + bag::point_offset(c, i), c, o + 4 * i);

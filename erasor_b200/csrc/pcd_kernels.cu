@@ -430,7 +430,7 @@ struct BagDesc {
     uint32_t per_tile;               // points per tile
     uint32_t staged;                 // 1: a tile's bytes are staged in shared memory; 0: read from global memory point by point
     uint32_t reach;                  // bag::point_reach
-    uint32_t lz4;                    // 1: src is in the decoded LZ4 chunks
+    uint32_t lz4;                    // 1: src is in the decoded chunks (lz4 or bz2)
     bag::Cloud c;
 };
 
@@ -585,6 +585,176 @@ __global__ void __launch_bounds__(kThreads) k_bag_parse(const uint8_t* dec, cons
     }
 }
 
+// ---- bz2 chunks of a bag (DESIGN.md section 12.2.2; the rules are bz2_stream.h, the plan, chain and placement bag_index.h) -----
+constexpr int kBzWalkThreads = 8;                    // walk and decode: one bz2::Tables per thread in shared memory
+constexpr int kBzBwtThreads = 512;                   // inverse BWT: one CTA per block
+
+// the decoded bz2 chunk holding byte q of the device copy
+__device__ uint32_t bz2_chunk_of(const bag::Bz2ChunkDesc* bd, uint32_t nc, uint64_t q) {
+    uint32_t lo = 0, hi = nc - 1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (bd[mid].src <= q) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// 1a. one thread per byte of the copy: 1 when the block magic starts at one of its bits, else 0
+__global__ void __launch_bounds__(kThreads) k_bz2_scan(const uint8_t* src, uint64_t nbytes, const bag::Bz2ChunkDesc* bd, uint32_t nc, uint32_t* flag) {
+    for (uint64_t q = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; q < nbytes; q += (uint64_t)gridDim.x * blockDim.x) {
+        const bag::Bz2ChunkDesc& D = bd[bz2_chunk_of(bd, nc, q)];
+        const uint64_t p = q - D.src;
+        flag[q] = p < D.len && bz2::candidate_at(src + D.src, D.len, p) ? 1u : 0u;
+    }
+}
+
+// 1b. ... and after the scan of the flags, the candidates in bit order
+__global__ void __launch_bounds__(kThreads) k_bz2_emit(const uint8_t* src, uint64_t nbytes, const bag::Bz2ChunkDesc* bd, uint32_t nc, const uint32_t* flag,
+                                                       const uint64_t* off, bag::Bz2Cand* cand) {
+    for (uint64_t q = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; q < nbytes; q += (uint64_t)gridDim.x * blockDim.x) {
+        if (!flag[q]) continue;
+        const uint32_t c = bz2_chunk_of(bd, nc, q);
+        const bag::Bz2ChunkDesc& D = bd[c];
+        const uint64_t p = q - D.src;
+        cand[off[q]] = bag::Bz2Cand{8 * p + bz2::candidate_at(src + D.src, D.len, p) - 1, c, 0};
+    }
+}
+
+// 2. one thread per candidate: the speculative walk (header, tables, symbols to the end-of-block symbol; no writes)
+__global__ void __launch_bounds__(kBzWalkThreads) k_bz2_walk(const uint8_t* src, const bag::Bz2ChunkDesc* bd, const bag::Bz2Cand* cand,
+                                                             const uint64_t* ncand, bz2::Walk* walk) {
+    extern __shared__ __align__(16) uint8_t bz_sh[];
+    bz2::Tables& T = reinterpret_cast<bz2::Tables*>(bz_sh)[threadIdx.x];
+    const uint64_t n = *ncand;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const bag::Bz2Cand C = cand[i];
+        const bag::Bz2ChunkDesc& D = bd[C.chunk];
+        walk[i] = bz2::block(src + D.src, 8 * D.len, C.bit, D.level, T, nullptr, nullptr);
+    }
+}
+
+// 3. one thread per chunk: the chain of true blocks (bag::bz2_chain)
+__global__ void __launch_bounds__(kThreads) k_bz2_chain(const uint8_t* src, const bag::Bz2ChunkDesc* bd, uint32_t nc, const bag::Bz2Cand* cand,
+                                                        const uint64_t* off, const uint64_t* ncand, const bz2::Walk* walk, int32_t* blkno,
+                                                        uint64_t* tt_off, uint32_t* nblocks, unsigned long long* err) {
+    for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += gridDim.x * blockDim.x) {
+        const bag::Bz2ChunkDesc& D = bd[c];
+        const uint64_t c0 = off[D.src], c1 = c + 1 < nc ? off[bd[c + 1].src] : *ncand;
+        const uint64_t k = bag::bz2_chain(c, D, src + D.src, cand, c0, c1, walk, blkno, tt_off, nblocks + c);
+        if (k != ~0ull) atomicMin(err, (unsigned long long)k);
+    }
+}
+
+// 4. one thread per true block: the walk again, now with the MTF and run output into its tt slot, then its LF vector
+__global__ void __launch_bounds__(kBzWalkThreads) k_bz2_decode(const uint8_t* src, const bag::Bz2ChunkDesc* bd, const bag::Bz2Cand* cand,
+                                                               const uint64_t* ncand, const uint64_t* tt_off, uint8_t* tt, uint32_t* lf) {
+    extern __shared__ __align__(16) uint8_t bz_sh[];
+    bz2::Tables& T = reinterpret_cast<bz2::Tables*>(bz_sh)[threadIdx.x];
+    const uint64_t n = *ncand;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t at = tt_off[i];
+        if (at == ~0ull) continue;
+        const bag::Bz2Cand C = cand[i];
+        const bag::Bz2ChunkDesc& D = bd[C.chunk];
+        uint32_t hist[256];
+        const bz2::Walk w = bz2::block(src + D.src, 8 * D.len, C.bit, D.level, T, tt + at, hist);
+        bz2::lf_vector(tt + at, w.n, hist, lf + at);
+    }
+}
+
+// 5. one CTA per true block: the inverse BWT by splitters (bz2_stream.h): every thread walks sublists to the next splitter, thread
+// 0 ranks the splitters from origPtr's, every thread walks its sublists again, writing each byte at its rank, and a periodic
+// block's cycle is repeated to its length
+__global__ void __launch_bounds__(kBzBwtThreads) k_bz2_bwt(const uint64_t* ncand, const bz2::Walk* walk, const uint64_t* tt_off, const uint8_t* tt,
+                                                           const uint32_t* lf, uint8_t* bw) {
+    __shared__ uint32_t nxt[bz2::kMaxSplitters], len[bz2::kMaxSplitters], rank[bz2::kMaxSplitters];
+    __shared__ uint32_t cycle;
+    const uint64_t nc = *ncand;
+    for (uint64_t i = blockIdx.x; i < nc; i += gridDim.x) {
+        const uint64_t at = tt_off[i];
+        if (at == ~0ull) continue;
+        const uint32_t n = walk[i].n;
+        const uint8_t* L = tt + at;
+        const uint32_t* T = lf + at;
+        const uint32_t p0 = T[walk[i].orig], ns = bz2::split_count(n);
+        for (uint32_t s = threadIdx.x; s < ns; s += blockDim.x) {
+            rank[s] = ~0u;
+            if (s + 1 < ns || p0 % bz2::kSplit) len[s] = bz2::split_walk(T, bz2::split_pos(s, p0, n), p0, n, &nxt[s]);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            const uint32_t id0 = bz2::split_id(p0, p0, n);
+            uint32_t s = id0, r = 0;
+            do { rank[s] = r; r += len[s]; s = nxt[s]; } while (s != id0);
+            cycle = r;
+        }
+        __syncthreads();
+        for (uint32_t s = threadIdx.x; s < ns; s += blockDim.x) {
+            if (rank[s] == ~0u) continue;
+            uint32_t q = bz2::split_pos(s, p0, n), r = rank[s];
+            for (uint32_t k = 0; k < len[s]; ++k) { bw[at + r + k] = L[q]; q = T[q]; }
+        }
+        __syncthreads();
+        const uint32_t m = cycle;
+        for (uint32_t k = m + threadIdx.x; k < n; k += blockDim.x) bw[at + k] = bw[at + k % m];
+        __syncthreads();
+    }
+}
+
+// 6. one thread per true block: RLE1's output length and the block CRC over it, checked
+__global__ void __launch_bounds__(kThreads) k_bz2_rle(const bag::Bz2Cand* cand, const uint64_t* ncand, const bz2::Walk* walk, const uint64_t* tt_off,
+                                                      const uint8_t* bw, uint64_t* osize, unsigned long long* err) {
+    __shared__ uint32_t tab[256];
+    if (threadIdx.x == 0) bz2::crc_table(tab);
+    __syncthreads();
+    const uint64_t nc = *ncand;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nc; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t at = tt_off[i];
+        if (at == ~0ull) continue;
+        uint64_t os = 0;
+        uint32_t crc = 0;
+        uint32_t r = bz2::rle1(bw + at, walk[i].n, tab, nullptr, &os, &crc);
+        if (r == bz2::R_OK && crc != walk[i].crc) r = bz2::R_BLOCK_CRC;
+        if (r != bz2::R_OK) atomicMin(err, (unsigned long long)bag::bz2_key(cand[i].chunk, cand[i].bit, r));
+        osize[i] = r == bz2::R_OK ? os : ~0ull;
+    }
+}
+
+// 7. one thread per chunk: the blocks' places in the decoded buffer (bag::bz2_place)
+__global__ void __launch_bounds__(kThreads) k_bz2_place(const bag::Bz2ChunkDesc* bd, uint32_t nc, const uint64_t* off, const uint64_t* ncand,
+                                                        const uint64_t* tt_off, const uint64_t* osize, uint64_t* out_off, unsigned long long* err) {
+    for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += gridDim.x * blockDim.x) {
+        const bag::Bz2ChunkDesc& D = bd[c];
+        const uint64_t c0 = off[D.src], c1 = c + 1 < nc ? off[bd[c + 1].src] : *ncand;
+        const uint64_t k = bag::bz2_place(c, D, c0, c1, tt_off, osize, out_off);
+        if (k != ~0ull) atomicMin(err, (unsigned long long)k);
+    }
+}
+
+// 8. one thread per true block: RLE1 into place
+__global__ void __launch_bounds__(kThreads) k_bz2_expand(const uint64_t* ncand, const bz2::Walk* walk, const uint64_t* tt_off, const uint64_t* out_off,
+                                                         const uint8_t* bw, uint8_t* dec) {
+    __shared__ uint32_t tab[256];
+    if (threadIdx.x == 0) bz2::crc_table(tab);
+    __syncthreads();
+    const uint64_t nc = *ncand;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nc; i += (uint64_t)gridDim.x * blockDim.x) {
+        if (out_off[i] == ~0ull) continue;
+        uint64_t os = 0;
+        uint32_t crc = 0;
+        bz2::rle1(bw + tt_off[i], walk[i].n, tab, dec + out_off[i], &os, &crc);
+    }
+}
+
+// 9. the block an error key names: the last block of its chunk starting at or before its bit
+__global__ void __launch_bounds__(kThreads) k_bz2_errblock(const bag::Bz2Cand* cand, const uint64_t* ncand, const int32_t* blkno,
+                                                           const unsigned long long* err, int* blk) {
+    const uint64_t key = *err, nc = *ncand;
+    if (key == ~0ull) return;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nc; i += (uint64_t)gridDim.x * blockDim.x)
+        if (blkno[i] >= 0 && cand[i].chunk == key >> 44 && cand[i].bit <= ((key >> 8) & 0xFFFFFFFFFull)) atomicMax(blk, blkno[i]);
+}
+
 constexpr uint64_t kBagStage = 32ull << 20;          // bytes per pinned staging buffer (two) for a pageable file
 
 uint32_t blocks_for(uint64_t n, int per, int cap) { return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + per - 1) / per, (uint64_t)cap)); }
@@ -608,10 +778,16 @@ struct erasor_pcd_ctx {
     cudaEvent_t bag_ev[2] = {nullptr, nullptr};
     // the LZ4 chunks of the index: the plan, the decoded chunks (kept until the next erasor_bag_index), the decode's scratch (the
     // compressed copy z4_src is released when the index returns)
-    bag::Lz4Plan z4;
+    bag::ChunkPlan z4;
     DeviceBuffer z4_src, z4_dec, z4_blk, z4_cd, z4_in, z4_bsize, z4_boff, z4_res;
     cudaEvent_t z4_ev[3] = {nullptr, nullptr, nullptr};
     double z4_decode_ms = 0, z4_sums_ms = 0;
+    // the bz2 chunks' decode scratch (all of it released when the index returns), what it found and its stage times
+    DeviceBuffer z2_src, z2_bd, z2_flag, z2_off, z2_cand, z2_walk, z2_blkno, z2_tt_off, z2_osize, z2_out_off, z2_tt, z2_lf, z2_bw;
+    cudaEvent_t z2_ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    bag::Bz2Found z2_found;
+    uint64_t z2_scratch = 0;
+    double z2_ms[4] = {0, 0, 0, 0};
     // erasor_pcd_format_ascii's text of its last call, kept for a following call with the same input
     bool cached = false;
     const float* c_ptr = nullptr;
@@ -767,64 +943,168 @@ int upload_spans(erasor_pcd_t p, uint8_t* d, const std::vector<Span>& spans) {
     return ERASOR_OK;
 }
 
-// erasor_bag_index's nodes in LZ4 chunks: the chunks holding one uploaded, decoded and checked in one submission, the nodes parsed,
-// one read-back; then bag::finish_lz4
-int bag_lz4(erasor_pcd_t p, std::string& msg) {
-    bag::Lz4Plan& P = p->z4;
-    bag::plan_lz4(p->bag, P);
-    const uint64_t nb = P.blocks.size(), nc = P.cd.size(), nn = P.nodes.size();
-    PCK(p->z4_src.ensure(std::max<uint64_t>(P.src_bytes, 16)));
-    PCK(p->z4_dec.ensure(std::max<uint64_t>(P.dec_bytes, 16)));
-    PCK(p->z4_blk.ensure(sizeof(bag::Lz4Block) * std::max<uint64_t>(nb, 1)));
-    PCK(p->z4_cd.ensure(sizeof(bag::Lz4ChunkDesc) * nc));
-    PCK(p->z4_in.ensure(sizeof(bag::Lz4NodeIn) * nn));
-    PCK(p->z4_bsize.ensure(sizeof(uint32_t) * std::max<uint64_t>(nb, 1)));
-    PCK(p->z4_boff.ensure(sizeof(uint64_t) * std::max<uint64_t>(nb, 1)));
-    PCK(p->z4_res.ensure(sizeof(bag::NodeOut) * nn + sizeof(unsigned long long)));
-    for (cudaEvent_t& ev : p->z4_ev)
+// The bz2 chunks of p->z4 into dec, launched on p->st after the LZ4 stages (no read-back): err gets the first broken rule's key,
+// res[0] the total of candidates, blk the block the key names and nblocks each chunk's true blocks
+int bz2_launch(erasor_pcd_t p, uint8_t* dec, unsigned long long* err, uint64_t* d_ncand_out, int* d_blk, uint32_t* d_nblocks) {
+    const bag::ChunkPlan& P = p->z4;
+    const uint32_t nc = (uint32_t)P.bd.size();
+    const uint64_t nbytes = P.bz_src_bytes, cap_c = std::max<uint64_t>(P.bz_cands, 1), tt_bytes = std::max<uint64_t>(P.bz_tt_bytes, 16);
+    const uint64_t ntiles = (nbytes + kScanTile - 1) / kScanTile;
+    // every buffer sized from what the host has: the streams' bytes, the candidate bound and the BWT bound (bag_index.h)
+    PCK(p->z2_src.ensure(nbytes));
+    PCK(p->z2_bd.ensure(sizeof(bag::Bz2ChunkDesc) * nc));
+    PCK(p->z2_flag.ensure(sizeof(uint32_t) * nbytes));
+    PCK(p->z2_off.ensure(sizeof(uint64_t) * nbytes));
+    PCK(p->z2_cand.ensure(sizeof(bag::Bz2Cand) * cap_c));
+    PCK(p->z2_walk.ensure(sizeof(bz2::Walk) * cap_c));
+    PCK(p->z2_blkno.ensure(sizeof(int32_t) * cap_c));
+    PCK(p->z2_tt_off.ensure(sizeof(uint64_t) * cap_c));
+    PCK(p->z2_osize.ensure(sizeof(uint64_t) * cap_c));
+    PCK(p->z2_out_off.ensure(sizeof(uint64_t) * cap_c));
+    PCK(p->z2_tt.ensure(tt_bytes));
+    PCK(p->z2_lf.ensure(sizeof(uint32_t) * tt_bytes));
+    PCK(p->z2_bw.ensure(tt_bytes));
+    PCK(p->sums.ensure(sizeof(uint64_t) * (ntiles + 1)));
+    p->z2_scratch = nbytes * (1 + sizeof(uint32_t) + sizeof(uint64_t)) + sizeof(bag::Bz2ChunkDesc) * nc + sizeof(uint64_t) * (ntiles + 1) +
+                    cap_c * (sizeof(bag::Bz2Cand) + sizeof(bz2::Walk) + sizeof(int32_t) + 3 * sizeof(uint64_t)) + tt_bytes * (2 + sizeof(uint32_t));
+    for (cudaEvent_t& ev : p->z2_ev)
         if (!ev) PCK(cudaEventCreate(&ev));
     std::vector<Span> spans;
-    for (size_t c = 0; c < nc; ++c) {
-        const bag::Lz4Chunk& k = p->bag.lz4[P.chunks[c]];
-        spans.push_back(Span{p->bag_file + k.data, k.len, P.cd[c].src});
-    }
-    uint8_t* src = p->z4_src.as<uint8_t>();
-    uint8_t* dec = p->z4_dec.as<uint8_t>();
-    const int rc = upload_spans(p, src, spans);
+    for (uint32_t c = 0; c < nc; ++c) spans.push_back(Span{p->bag_file + p->bag.bz2[P.bz_chunks[c]].data, P.bd[c].len, P.bd[c].src});
+    uint8_t* src = p->z2_src.as<uint8_t>();
+    int rc = upload_spans(p, src, spans);
     if (rc != ERASOR_OK) return rc;
-    if (nb) PCK(cudaMemcpyAsync(p->z4_blk.p(), P.blocks.data(), sizeof(bag::Lz4Block) * nb, cudaMemcpyHostToDevice, p->st));
-    PCK(cudaMemcpyAsync(p->z4_cd.p(), P.cd.data(), sizeof(bag::Lz4ChunkDesc) * nc, cudaMemcpyHostToDevice, p->st));
-    PCK(cudaMemcpyAsync(p->z4_in.p(), P.nodes.data(), sizeof(bag::Lz4NodeIn) * nn, cudaMemcpyHostToDevice, p->st));
+    PCK(cudaMemcpyAsync(p->z2_bd.p(), P.bd.data(), sizeof(bag::Bz2ChunkDesc) * nc, cudaMemcpyHostToDevice, p->st));
+    PCK(cudaMemsetAsync(p->z2_blkno.p(), 0xFF, sizeof(int32_t) * cap_c, p->st));
+    PCK(cudaMemsetAsync(p->z2_tt_off.p(), 0xFF, sizeof(uint64_t) * cap_c, p->st));
+    PCK(cudaMemsetAsync(p->z2_out_off.p(), 0xFF, sizeof(uint64_t) * cap_c, p->st));
+    PCK(cudaMemsetAsync(d_nblocks, 0, sizeof(uint32_t) * nc, p->st));
+    PCK(cudaMemsetAsync(d_blk, 0xFF, sizeof(int), p->st));
+    const bag::Bz2ChunkDesc* bd = p->z2_bd.as<bag::Bz2ChunkDesc>();
+    uint32_t* flag = p->z2_flag.as<uint32_t>();
+    uint64_t* off = p->z2_off.as<uint64_t>();
+    bag::Bz2Cand* cand = p->z2_cand.as<bag::Bz2Cand>();
+    bz2::Walk* walk = p->z2_walk.as<bz2::Walk>();
+    int32_t* blkno = p->z2_blkno.as<int32_t>();
+    uint64_t *tt_off = p->z2_tt_off.as<uint64_t>(), *osize = p->z2_osize.as<uint64_t>(), *out_off = p->z2_out_off.as<uint64_t>();
+    uint8_t *tt = p->z2_tt.as<uint8_t>(), *bw = p->z2_bw.as<uint8_t>();
+    uint32_t* lf = p->z2_lf.as<uint32_t>();
+    const uint64_t* ncand = p->sums.as<uint64_t>() + ntiles;          // the scan's total
+    const int cap = p->sm_count * 16;
+    const size_t sh_walk = sizeof(bz2::Tables) * kBzWalkThreads;
+    const uint32_t g_walk = blocks_for(cap_c, kBzWalkThreads, p->sm_count * 32);
+    PCK(cudaEventRecord(p->z2_ev[0], p->st));
+    k_bz2_scan<<<blocks_for(nbytes, kThreads, cap), kThreads, 0, p->st>>>(src, nbytes, bd, nc, flag);
+    rc = scan_u32(p, flag, nbytes, off, nullptr);
+    if (rc != ERASOR_OK) return rc;
+    k_bz2_emit<<<blocks_for(nbytes, kThreads, cap), kThreads, 0, p->st>>>(src, nbytes, bd, nc, flag, off, cand);
+    k_bz2_walk<<<g_walk, kBzWalkThreads, sh_walk, p->st>>>(src, bd, cand, ncand, walk);
+    k_bz2_chain<<<blocks_for(nc, kThreads, cap), kThreads, 0, p->st>>>(src, bd, nc, cand, off, ncand, walk, blkno, tt_off, d_nblocks, err);
+    PCK(cudaEventRecord(p->z2_ev[1], p->st));
+    k_bz2_decode<<<g_walk, kBzWalkThreads, sh_walk, p->st>>>(src, bd, cand, ncand, tt_off, tt, lf);
+    PCK(cudaEventRecord(p->z2_ev[2], p->st));
+    k_bz2_bwt<<<blocks_for(cap_c, 1, p->sm_count * 4), kBzBwtThreads, 0, p->st>>>(ncand, walk, tt_off, tt, lf, bw);
+    PCK(cudaEventRecord(p->z2_ev[3], p->st));
+    k_bz2_rle<<<blocks_for(cap_c, kThreads, cap), kThreads, 0, p->st>>>(cand, ncand, walk, tt_off, bw, osize, err);
+    k_bz2_place<<<blocks_for(nc, kThreads, cap), kThreads, 0, p->st>>>(bd, nc, off, ncand, tt_off, osize, out_off, err);
+    k_bz2_expand<<<blocks_for(cap_c, kThreads, cap), kThreads, 0, p->st>>>(ncand, walk, tt_off, out_off, bw, dec);
+    PCK(cudaEventRecord(p->z2_ev[4], p->st));
+    k_bz2_errblock<<<blocks_for(cap_c, kThreads, cap), kThreads, 0, p->st>>>(cand, ncand, blkno, err, d_blk);
+    PCK(cudaMemcpyAsync(d_ncand_out, ncand, sizeof(uint64_t), cudaMemcpyDeviceToDevice, p->st));
+    PCK(cudaGetLastError());
+    return ERASOR_OK;
+}
+
+// erasor_bag_index's nodes in compressed chunks: the chunks holding one uploaded, decoded and checked in one submission (the LZ4
+// stages, then the bz2 stages, into one decoded buffer), the nodes parsed, one read-back; then bag::finish_chunks
+int bag_decode(erasor_pcd_t p, std::string& msg) {
+    bag::ChunkPlan& P = p->z4;
+    bag::plan_chunks(p->bag, P);
+    const uint64_t nb = P.blocks.size(), nc = P.cd.size(), nn = P.nodes.size(), nz = P.bd.size();
+    if (nz > bag::kMaxBz2Chunks) { msg = "more than 2^20 bz2 chunks hold kept nodes"; return ERASOR_E_CAPACITY; }
+    if (nc) PCK(p->z4_src.ensure(std::max<uint64_t>(P.src_bytes, 16)));
+    PCK(p->z4_dec.ensure(std::max<uint64_t>(P.dec_bytes, 16)));
+    if (nc) {
+        PCK(p->z4_blk.ensure(sizeof(bag::Lz4Block) * std::max<uint64_t>(nb, 1)));
+        PCK(p->z4_cd.ensure(sizeof(bag::Lz4ChunkDesc) * nc));
+        PCK(p->z4_bsize.ensure(sizeof(uint32_t) * std::max<uint64_t>(nb, 1)));
+        PCK(p->z4_boff.ensure(sizeof(uint64_t) * std::max<uint64_t>(nb, 1)));
+    }
+    PCK(p->z4_in.ensure(sizeof(bag::Lz4NodeIn) * nn));
+    // the node results, then the LZ4 key, the bz2 key, the bz2 candidates, the block the bz2 key names, the bz2 chunks' blocks
+    const size_t res_bytes = sizeof(bag::NodeOut) * nn + 3 * sizeof(unsigned long long) + sizeof(int) + sizeof(uint32_t) * nz;
+    PCK(p->z4_res.ensure(res_bytes));
+    for (cudaEvent_t& ev : p->z4_ev)
+        if (!ev) PCK(cudaEventCreate(&ev));
+    uint8_t* dec = p->z4_dec.as<uint8_t>();
     bag::NodeOut* d_res = p->z4_res.as<bag::NodeOut>();
     unsigned long long* d_err = reinterpret_cast<unsigned long long*>(d_res + nn);
-    PCK(cudaMemsetAsync(d_err, 0xFF, sizeof(unsigned long long), p->st));
-    const bag::Lz4Block* blk = p->z4_blk.as<bag::Lz4Block>();
-    const bag::Lz4ChunkDesc* cd = p->z4_cd.as<bag::Lz4ChunkDesc>();
-    uint32_t* bsize = p->z4_bsize.as<uint32_t>();
-    uint64_t* boff = p->z4_boff.as<uint64_t>();
-    const int cap = p->sm_count * 16;
-    PCK(cudaEventRecord(p->z4_ev[0], p->st));
-    if (nb) k_lz4_size<<<blocks_for(nb, kThreads, cap), kThreads, 0, p->st>>>(src, blk, nb, bsize, d_err);
-    k_lz4_place<<<blocks_for(nc, kThreads, cap), kThreads, 0, p->st>>>(cd, nc, bsize, boff, d_err);
-    if (nb) k_lz4_decode<<<blocks_for(nb, kThreads / 32, cap), kThreads, 0, p->st>>>(src, blk, nb, bsize, boff, dec);
-    PCK(cudaEventRecord(p->z4_ev[1], p->st));
-    if (nb) k_lz4_sums<<<blocks_for(nb, kThreads, cap), kThreads, 0, p->st>>>(src, blk, nb, d_err);
-    k_lz4_content<<<(unsigned)((4 * nc + kContentThreads - 1) / kContentThreads), kContentThreads, 0, p->st>>>(cd, nc, dec, d_err);
-    PCK(cudaEventRecord(p->z4_ev[2], p->st));
-    k_bag_parse<<<blocks_for(nn, kThreads, cap), kThreads, 0, p->st>>>(dec, p->z4_in.as<bag::Lz4NodeIn>(), nn, d_res);
+    PCK(cudaMemsetAsync(d_err, 0xFF, 2 * sizeof(unsigned long long), p->st));
+    if (nc) {
+        std::vector<Span> spans;
+        for (size_t c = 0; c < nc; ++c) {
+            const bag::Lz4Chunk& k = p->bag.lz4[P.chunks[c]];
+            spans.push_back(Span{p->bag_file + k.data, k.len, P.cd[c].src});
+        }
+        uint8_t* src = p->z4_src.as<uint8_t>();
+        const int rc = upload_spans(p, src, spans);
+        if (rc != ERASOR_OK) return rc;
+        if (nb) PCK(cudaMemcpyAsync(p->z4_blk.p(), P.blocks.data(), sizeof(bag::Lz4Block) * nb, cudaMemcpyHostToDevice, p->st));
+        PCK(cudaMemcpyAsync(p->z4_cd.p(), P.cd.data(), sizeof(bag::Lz4ChunkDesc) * nc, cudaMemcpyHostToDevice, p->st));
+        PCK(cudaMemcpyAsync(p->z4_in.p(), P.nodes.data(), sizeof(bag::Lz4NodeIn) * nn, cudaMemcpyHostToDevice, p->st));
+        const bag::Lz4Block* blk = p->z4_blk.as<bag::Lz4Block>();
+        const bag::Lz4ChunkDesc* cd = p->z4_cd.as<bag::Lz4ChunkDesc>();
+        uint32_t* bsize = p->z4_bsize.as<uint32_t>();
+        uint64_t* boff = p->z4_boff.as<uint64_t>();
+        const int cap = p->sm_count * 16;
+        PCK(cudaEventRecord(p->z4_ev[0], p->st));
+        if (nb) k_lz4_size<<<blocks_for(nb, kThreads, cap), kThreads, 0, p->st>>>(src, blk, nb, bsize, d_err);
+        k_lz4_place<<<blocks_for(nc, kThreads, cap), kThreads, 0, p->st>>>(cd, nc, bsize, boff, d_err);
+        if (nb) k_lz4_decode<<<blocks_for(nb, kThreads / 32, cap), kThreads, 0, p->st>>>(src, blk, nb, bsize, boff, dec);
+        PCK(cudaEventRecord(p->z4_ev[1], p->st));
+        if (nb) k_lz4_sums<<<blocks_for(nb, kThreads, cap), kThreads, 0, p->st>>>(src, blk, nb, d_err);
+        k_lz4_content<<<(unsigned)((4 * nc + kContentThreads - 1) / kContentThreads), kContentThreads, 0, p->st>>>(cd, nc, dec, d_err);
+        PCK(cudaEventRecord(p->z4_ev[2], p->st));
+    } else {
+        PCK(cudaMemcpyAsync(p->z4_in.p(), P.nodes.data(), sizeof(bag::Lz4NodeIn) * nn, cudaMemcpyHostToDevice, p->st));
+    }
+    uint64_t* d_ncand = reinterpret_cast<uint64_t*>(d_err + 2);
+    int* d_blk = reinterpret_cast<int*>(d_err + 3);
+    uint32_t* d_nblocks = reinterpret_cast<uint32_t*>(d_blk + 1);
+    if (nz) {
+        const int rc = bz2_launch(p, dec, d_err + 1, d_ncand, d_blk, d_nblocks);
+        if (rc != ERASOR_OK) return rc;
+    }
+    k_bag_parse<<<blocks_for(nn, kThreads, p->sm_count * 16), kThreads, 0, p->st>>>(dec, p->z4_in.as<bag::Lz4NodeIn>(), nn, d_res);
     PCK(cudaGetLastError());
-    std::vector<bag::NodeOut> res(nn);
-    unsigned long long err = 0;
-    PCK(cudaMemcpyAsync(res.data(), d_res, sizeof(bag::NodeOut) * nn, cudaMemcpyDeviceToHost, p->st));
-    PCK(cudaMemcpyAsync(&err, d_err, sizeof(err), cudaMemcpyDeviceToHost, p->st));
+    std::vector<uint8_t> res(res_bytes);
+    PCK(cudaMemcpyAsync(res.data(), d_res, res_bytes, cudaMemcpyDeviceToHost, p->st));
     PCK(cudaStreamSynchronize(p->st));
-    float t0 = 0, t1 = 0;
-    PCK(cudaEventElapsedTime(&t0, p->z4_ev[0], p->z4_ev[1]));
-    PCK(cudaEventElapsedTime(&t1, p->z4_ev[1], p->z4_ev[2]));
-    p->z4_decode_ms = t0;
-    p->z4_sums_ms = t1;
-    if (err != ~0ull) { msg = bag::lz4_error(p->bag, P, err); return ERASOR_E_INVALID; }
-    return bag::finish_lz4(p->bag, res.data(), msg);
+    if (nc) {
+        float t0 = 0, t1 = 0;
+        PCK(cudaEventElapsedTime(&t0, p->z4_ev[0], p->z4_ev[1]));
+        PCK(cudaEventElapsedTime(&t1, p->z4_ev[1], p->z4_ev[2]));
+        p->z4_decode_ms = t0;
+        p->z4_sums_ms = t1;
+    }
+    const uint8_t* tail = res.data() + sizeof(bag::NodeOut) * nn;
+    uint64_t keys[3];
+    int blk = -1;
+    std::memcpy(keys, tail, sizeof(keys));
+    std::memcpy(&blk, tail + sizeof(keys), sizeof(int));
+    if (nz) {
+        p->z2_found.blocks.resize(nz);
+        std::memcpy(p->z2_found.blocks.data(), tail + sizeof(keys) + sizeof(int), sizeof(uint32_t) * nz);
+        p->z2_found.candidates = keys[2];
+        for (int k = 0; k < 4; ++k) {
+            float t = 0;
+            PCK(cudaEventElapsedTime(&t, p->z2_ev[k], p->z2_ev[k + 1]));
+            p->z2_ms[k] = t;
+        }
+    }
+    const int rc = bag::decode_error(p->bag, P, keys[0], nz ? keys[1] : ~0ull, blk, msg);
+    if (rc != ERASOR_OK) return rc;
+    return bag::finish_chunks(p->bag, reinterpret_cast<const bag::NodeOut*>(res.data()), msg);
 }
 
 const char* kHeadFmt ="# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z intensity\nSIZE 4 4 4 4\nTYPE F F F F\n"
@@ -862,6 +1142,8 @@ void erasor_pcd_destroy(erasor_pcd_t p) {
     for (cudaEvent_t ev : p->bag_ev)
         if (ev) cudaEventDestroy(ev);
     for (cudaEvent_t ev : p->z4_ev)
+        if (ev) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : p->z2_ev)
         if (ev) cudaEventDestroy(ev);
     if (p->st) cudaStreamDestroy(p->st);
     delete p;
@@ -1124,8 +1406,11 @@ int erasor_bag_index(erasor_pcd_t p, const char* file, size_t len, const char* t
     p->cached = false;
     p->bag_ok = false;
     p->bag = bag::Index();
-    p->z4 = bag::Lz4Plan();
+    p->z4 = bag::ChunkPlan();
     p->z4_decode_ms = p->z4_sums_ms = 0;
+    p->z2_found = bag::Bz2Found();
+    p->z2_scratch = 0;
+    for (double& t : p->z2_ms) t = 0;
     p->bag_file = nullptr;
     if (info) *info = erasor_bag_info_t{};
     if (!n_nodes || (len && !file)) return fail(p, ERASOR_E_INVALID, "null argument");
@@ -1139,11 +1424,15 @@ int erasor_bag_index(erasor_pcd_t p, const char* file, size_t len, const char* t
     cudaGetLastError();
     p->bag_file = reinterpret_cast<const uint8_t*>(file);
     if (!p->bag.pending.empty()) {
-        rc = bag_lz4(p, msg);
+        rc = bag_decode(p, msg);
         p->z4_src = DeviceBuffer();                  // the compressed copy is not needed past the index: only the decoded chunks stay
+        for (DeviceBuffer* b : {&p->z2_src, &p->z2_bd, &p->z2_flag, &p->z2_off, &p->z2_cand, &p->z2_walk, &p->z2_blkno, &p->z2_tt_off,
+                                &p->z2_osize, &p->z2_out_off, &p->z2_tt, &p->z2_lf, &p->z2_bw})
+            *b = DeviceBuffer();                     // nor is any of the bz2 scratch
         if (rc != ERASOR_OK) {
             p->bag = bag::Index();
-            p->z4 = bag::Lz4Plan();
+            p->z4 = bag::ChunkPlan();
+            p->z2_found = bag::Bz2Found();
             p->bag_file = nullptr;
             return rc == ERASOR_E_CUDA ? rc : fail(p, rc, msg);
         }
@@ -1215,7 +1504,7 @@ int erasor_bag_load_list(erasor_pcd_t p, const uint64_t* nodes, size_t count, fl
         if (!n) continue;
         BagDesc D{};
         D.c = c;
-        D.lz4 = nd.lz >= 0;
+        D.lz4 = nd.decoded();
         D.src = D.lz4 ? bag::dec_of(p->z4, nd) + c.data_off : blob_bytes;
         D.out = offsets[k];
         D.tile0 = ntiles;
@@ -1257,6 +1546,20 @@ int erasor_bag_lz4_stats(erasor_pcd_t p, erasor_bag_lz4_stats_t* stats) {
     bag::fill_lz4_stats(p->bag, p->z4, *stats);
     stats->decode_ms = p->z4_decode_ms;
     stats->checksum_ms = p->z4_sums_ms;
+    return ERASOR_OK;
+}
+
+int erasor_bag_bz2_stats(erasor_pcd_t p, erasor_bag_bz2_stats_t* stats) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    if (!stats) return fail(p, ERASOR_E_INVALID, "null argument");
+    if (!p->bag_ok) { *stats = erasor_bag_bz2_stats_t{}; return ERASOR_OK; }
+    bag::fill_bz2_stats(p->bag, p->z4, p->z2_found, *stats);
+    stats->scratch_bytes = p->z2_scratch;
+    stats->scan_ms = p->z2_ms[0];
+    stats->decode_ms = p->z2_ms[1];
+    stats->bwt_ms = p->z2_ms[2];
+    stats->rle_ms = p->z2_ms[3];
     return ERASOR_OK;
 }
 

@@ -288,6 +288,12 @@ public:
         check(erasor_bag_lz4_stats(p_, &s));
         return s;
     }
+    // the bag's bz2 chunks: how many were uploaded and decoded, bytes, blocks and candidates, scratch, stage times (erasor_bag_bz2_stats)
+    erasor_bag_bz2_stats_t bz2_stats() const {
+        erasor_bag_bz2_stats_t s{};
+        check(erasor_bag_bz2_stats(p_, &s));
+        return s;
+    }
     // The clouds of nodes [first, first + count) -- or of the listed nodes -- back to back in device memory, from one gather
     // launch.  device_buffer(n) must return a 16-byte aligned device pointer with room for n points (the caller owns the memory).
     // Returns the count + 1 offsets.  Synchronous: the clouds are complete on return.

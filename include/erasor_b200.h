@@ -461,7 +461,7 @@ int  erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind
  * messages on `topic` (NULL: "/node/combined/optimized") in delivery order, a stable sort by record time.  Unless keep_first, the
  * first of them is dropped, as the reference's subscribers drop it.  file: host memory, len bytes, which must stay valid and
  * unchanged until the next erasor_bag_index on p; pinned memory is read by the device directly, pageable memory through a pinned
- * staging buffer.  Errors: ERASOR_E_UNSUPPORTED for another bag version, a chunk compressed with anything but lz4, a topic whose type
+ * staging buffer.  Errors: ERASOR_E_UNSUPPORTED for another bag version, a chunk compressed with anything but lz4 or bz2, a topic whose type
  * is not erasor/node, a cloud without FLOAT32 x, y or z; ERASOR_E_INVALID (with the byte offset) for a record or field running past
  * its container, a chunk whose data length differs from its size, a message on an undefined connection, a missing header field, a
  * message longer or shorter than an erasor/node, a point read past its cloud's data; ERASOR_E_CAPACITY for a cloud of 2^31 points.
@@ -476,7 +476,17 @@ int  erasor_pcd_load(erasor_pcd_t p, const char* file, size_t len, int file_kind
  * lz4 chunk no index data record follows; ERASOR_E_INVALID for a reserved bit, a block max id below 4, a header checksum, content
  * size or decoded length other than the chunk's size, a block above the block max, a malformed block (naming the chunk, the block
  * and the byte of the frame), a block or content checksum mismatch, an index entry that does not point to its message record.  A
- * bag without lz4 chunks does no device work here. */
+ * bag without lz4 or bz2 chunks does no device work here.
+ *
+ * bz2 chunks (DESIGN.md section 12.2.2) are indexed as lz4 chunks are; each holds one bzip2 stream, decoded on the device in the
+ * same submission as the lz4 chunks, into the same decoded buffer (erasor_bag_bz2_stats).  The error reported is the first in file
+ * order across both kinds.  Further errors, naming the chunk and, where they apply, the block and the bit of the chunk data:
+ * ERASOR_E_UNSUPPORTED for data that does not start with "BZh", a randomised block, a second stream after the first, a bz2 chunk
+ * no index data record follows; ERASOR_E_INVALID for a level digit outside 1..9, a stream running past the chunk or followed by
+ * other bytes, a missing block or end-of-stream magic, an empty symbol map, nGroups outside 2..6, nSelectors of 0, a selector
+ * index at or above nGroups, a code length outside 1..20, an over-subscribed or incomplete code, a run or block longer than
+ * level x 100 000 bytes, no end-of-block symbol, origPtr at or past the block length, four equal
+ * bytes ending a block without their count, a block or stream CRC mismatch, a decoded length other than the chunk's size. */
 typedef struct {
     uint32_t version;                /* 200 for V2.0 */
     uint32_t pad_;
@@ -532,6 +542,25 @@ typedef struct {
 } erasor_bag_lz4_stats_t;
 
 int  erasor_bag_lz4_stats(erasor_pcd_t p, erasor_bag_lz4_stats_t* stats);
+
+/* The bz2 chunks of the last erasor_bag_index (all 0 after a failed one, or for a bag without bz2 chunks).  As for lz4, only the
+ * chunks holding a kept node are uploaded and decoded, and a load reads their nodes from the decoded chunks. */
+typedef struct {
+    uint64_t chunks;                 /* bz2 chunks in the file */
+    uint64_t decoded_chunks;         /* of them, those holding a kept node: copied to the device and decoded */
+    uint64_t compressed_bytes;       /* their streams, copied host to device */
+    uint64_t decoded_bytes;          /* their decoded data, held on the device until the next erasor_bag_index */
+    uint64_t blocks;                 /* the true blocks of the decoded streams */
+    uint64_t candidates;             /* bit offsets holding the block magic: blocks, and false positives inside blocks */
+    uint64_t streams_by_level[9];    /* the bz2 chunks of the file by their stream's level 1..9 */
+    uint64_t scratch_bytes;          /* the peak device scratch of the decode, released before erasor_bag_index returns */
+    double scan_ms;                  /* device time of the candidate scan, the speculative walks and the chain (CUDA events) */
+    double decode_ms;                /* ... of the Huffman, RUNA/RUNB and MTF decode and the LF vectors */
+    double bwt_ms;                   /* ... of the inverse BWT */
+    double rle_ms;                   /* ... of RLE1, the block CRCs and the placement */
+} erasor_bag_bz2_stats_t;
+
+int  erasor_bag_bz2_stats(erasor_pcd_t p, erasor_bag_bz2_stats_t* stats);
 
 /* ============================================================================================
  * The naive map generator with its map resident on the device: the reference's mapgen (src/mapgen/mapgen.hpp:198-305,
