@@ -41,7 +41,7 @@ EXPORTS = [
     "erasor_eval_create", "erasor_eval_destroy", "erasor_eval_last_error", "erasor_evaluate", "erasor_eval_overlap",
     "erasor_eval_count_selected",
     "erasor_pcd_create", "erasor_pcd_destroy", "erasor_pcd_last_error", "erasor_pcd_parse_ascii", "erasor_pcd_format_ascii",
-    "erasor_pcd_load", "erasor_bag_index", "erasor_bag_nodes", "erasor_bag_load", "erasor_bag_load_list", "erasor_bag_lz4_stats", "erasor_bag_bz2_stats",
+    "erasor_pcd_format", "erasor_pcd_load", "erasor_bag_index", "erasor_bag_nodes", "erasor_bag_load", "erasor_bag_load_list", "erasor_bag_lz4_stats", "erasor_bag_bz2_stats",
     "erasor_mapgen_create", "erasor_mapgen_destroy", "erasor_mapgen_last_error", "erasor_mapgen_accum", "erasor_mapgen_get_cloud",
     "erasor_mapgen_device_cloud", "erasor_mapgen_synchronize", "erasor_mapgen_get_counters",
 ]
@@ -69,6 +69,15 @@ class PcdLoadInfoC(ctypes.Structure):
     _fields_ = [(name, c_uint32) for name in ("data_mode", "fields", "intensity_zero_filled", "point_step")] + \
                [(name, c_uint64) for name in ("width", "height", "points", "data_offset", "compressed_size", "uncompressed_size", "lzf_tokens")] + \
                [("ascii", PcdInfoC)]
+
+
+class PcdFormatInfoC(ctypes.Structure):
+    """erasor_pcd_format_info_t"""
+    _fields_ = [("data_mode", c_uint32), ("segments", c_uint32)] + \
+               [(name, c_uint64) for name in ("header_bytes", "uncompressed_size", "compressed_size", "lzf_tokens")]
+
+
+PCD_MODES = {"ascii": 0, "binary": 1, "binary_compressed": 2}     # ERASOR_PCD_ASCII / _BINARY / _BINARY_COMPRESSED
 
 
 class BagInfoC(ctypes.Structure):
@@ -225,6 +234,7 @@ def _load():
     L.erasor_pcd_last_error.argtypes = [c_void_p]
     L.erasor_pcd_parse_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdInfoC)]
     L.erasor_pcd_format_ascii.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t)]
+    L.erasor_pcd_format.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdFormatInfoC)]
     L.erasor_pcd_load.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_int, POINTER(c_size_t), POINTER(PcdLoadInfoC)]
     L.erasor_bag_index.argtypes = [c_void_p, c_void_p, c_size_t, c_char_p, c_int, POINTER(c_size_t), POINTER(BagInfoC)]
     L.erasor_bag_nodes.argtypes = [c_void_p, c_size_t, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p]
@@ -938,8 +948,8 @@ class PcdCodec(_Native):
     """One ``erasor_pcd_t``: PCD files read and written on the device (DESIGN.md section 12).  ``parse`` / ``read`` give what
     ``evaluate.read_pcd_ascii`` gives, bit for bit (including its KeyError for a file without x, y, z or intensity); ``load`` /
     ``load_bytes`` read any DATA mode (ascii, binary, binary_compressed) as PCL does (section 12.1); ``format`` / ``write`` give the
-    bytes ``evaluate.write_pcd_ascii`` writes, except that NaN is written "nan" whatever its sign.  Files are read and written as raw
-    bytes."""
+    bytes ``evaluate.write_pcd_ascii`` writes, except that NaN is written "nan" whatever its sign, or with ``mode`` a binary or
+    binary_compressed file (section 12.3).  Files are read and written as raw bytes."""
     _DESTROY, _LAST_ERROR = "erasor_pcd_destroy", "erasor_pcd_last_error"
 
     def __init__(self, device: int = 0):
@@ -1123,7 +1133,9 @@ class PcdCodec(_Native):
             for k in range(nb):
                 yield int(seq[k]), odom[k].copy(), xyzi[int(off[k]):int(off[k + 1])]
 
-    def _format(self, xyzi) -> np.ndarray:
+    def _format(self, xyzi, mode: str) -> np.ndarray:
+        if mode not in PCD_MODES:
+            raise ValueError(f"mode must be one of {sorted(PCD_MODES)}")
         if hasattr(xyzi, "is_cuda") and xyzi.is_cuda:
             if str(xyzi.dtype) != "torch.float32" or xyzi.dim() != 2 or xyzi.shape[1] != 4 or not xyzi.is_contiguous():
                 raise ValueError("device clouds are contiguous float32 [n,4] tensors")
@@ -1131,21 +1143,31 @@ class PcdCodec(_Native):
         else:
             keep = _cloud(xyzi)
             ptr, n, kind = c_void_p(keep.ctypes.data if len(keep) else 0), len(keep), PTR_HOST
-        size = c_size_t(0)
-        self._ck(self.L.erasor_pcd_format_ascii(self.h, ptr, n, kind, None, 0, PTR_HOST, ctypes.byref(size)))
+        size, info = c_size_t(0), PcdFormatInfoC()
+        m = PCD_MODES[mode]
+        self._ck(self.L.erasor_pcd_format(self.h, ptr, n, kind, m, None, 0, PTR_HOST, ctypes.byref(size), ctypes.byref(info)))
         out = np.empty(size.value, dtype=np.uint8)
-        self._ck(self.L.erasor_pcd_format_ascii(self.h, ptr, n, kind, c_void_p(out.ctypes.data), size.value, PTR_HOST, ctypes.byref(size)))
+        self._ck(self.L.erasor_pcd_format(self.h, ptr, n, kind, m, c_void_p(out.ctypes.data), size.value, PTR_HOST, ctypes.byref(size),
+                                          ctypes.byref(info)))
+        self._format_info = {name: int(getattr(info, name)) for name, _ in PcdFormatInfoC._fields_}
         del keep
         return out
 
-    def format(self, xyzi) -> bytes:
-        """the whole file for a float32 [n, 4] cloud (numpy, or a CUDA tensor)"""
-        return self._format(xyzi).tobytes()
+    def format(self, xyzi, mode: str = "ascii") -> bytes:
+        """the whole file for a float32 [n, 4] cloud (numpy, or a CUDA tensor) in DATA mode "ascii", "binary" or
+        "binary_compressed" (erasor_pcd_format, DESIGN.md section 12.3)"""
+        return self._format(xyzi, mode).tobytes()
 
-    def write(self, path: str, xyzi):
-        out = self._format(xyzi)
+    def write(self, path: str, xyzi, mode: str = "ascii"):
+        out = self._format(xyzi, mode)
         with open(path, "wb") as f:
             f.write(memoryview(out))
+
+    def last_format_info(self) -> dict:
+        """erasor_pcd_format_info_t of the last format / write: data_mode, segments, header_bytes, uncompressed_size,
+        compressed_size, lzf_tokens"""
+        info = getattr(self, "_format_info", None)
+        return dict(info) if info is not None else None
 
 
 class MapGen(_Native):

@@ -1,7 +1,7 @@
 #!/bin/bash
 # build.sh -- compiles the product library for sm_90a (nvcc cross-compiles without a GPU).
 #   erasor_b200/_lib/liberasor_b200.so            the C-ABI library (include/erasor_b200.h)
-#   erasor_b200/_lib/liberasor_b200_hostcheck.so  host-only build of binning.h, pcd_codec.h, pcd_binary.h, bag_index.h, lz4_frame.h and bz2_stream.h for the CPU test-suite
+#   erasor_b200/_lib/liberasor_b200_hostcheck.so  host-only build of binning.h, pcd_codec.h, pcd_binary.h, lzf_encode.h, bag_index.h, lz4_frame.h and bz2_stream.h for the CPU test-suite
 set -euo pipefail
 cd "$(dirname "$0")"
 mkdir -p ../_lib ../_build

@@ -11,6 +11,7 @@
 
 #include "bag_index.h"
 #include "binning_tables.h"
+#include "lzf_encode.h"
 #include "pcd_binary.h"
 #include "pcd_codec.h"
 #include "pose_math.h"
@@ -597,5 +598,73 @@ int erasor_hostcheck_lzf_compress(const uint8_t* in, uint64_t n, uint8_t* out, u
     if (!flush(n)) return -1;
     *clen = o;
     return 0;
+}
+
+// lzf_encode.h's segmented encoder run serially over n bytes: the stream at out (cap bytes; -1 when it does not fit), its length
+// in *clen, its tokens in *tokens and its segments in *segments
+int erasor_hostcheck_lzf_encode(const uint8_t* in, uint64_t n, uint8_t* out, uint64_t cap, uint64_t* clen, uint64_t* tokens, uint64_t* segments) {
+    std::vector<uint16_t> table(pcd::kLzfHashSize);
+    std::vector<uint8_t> slot(pcd::lzf_segment_cap(pcd::kLzfSeg));
+    uint64_t o = 0, ntok = 0, nseg = 0;
+    for (uint64_t b = 0; b < n; b += pcd::kLzfSeg, ++nseg) {
+        const uint32_t len = (uint32_t)std::min<uint64_t>(pcd::kLzfSeg, n - b);
+        uint32_t t = 0;
+        const uint32_t m = pcd::lzf_encode_segment(in + b, len, table.data(), slot.data(), &t);
+        if (o + m > cap) return -1;
+        std::memcpy(out + o, slot.data(), m);
+        o += m;
+        ntok += t;
+    }
+    *clen = o;
+    *tokens = ntok;
+    *segments = nseg;
+    return 0;
+}
+
+// erasor_pcd_format's size rule for binary_compressed: POINTS x 16 uncompressed bytes and a stream of csize bytes
+int erasor_hostcheck_pcd_sizes_fit(uint64_t usize, uint64_t csize) { return pcd::compressed_sizes_fit(usize, csize); }
+
+// erasor_pcd_format's binary and binary_compressed files on the host (the same header, SoA and encoder, run serially); ascii is
+// ERASOR_E_INVALID here (erasor_pcd_format_ascii's text is checked elsewhere).  out == NULL or cap too small gives the size
+// (ERASOR_E_CAPACITY for the latter).
+int erasor_hostcheck_pcd_format_file(const float* xyzi, size_t n, int data_mode, char* out, size_t cap, size_t* len, erasor_pcd_format_info_t* info) {
+    erasor_pcd_format_info_t inf{};
+    if (data_mode != ERASOR_PCD_BINARY && data_mode != ERASOR_PCD_BINARY_COMPRESSED) return ERASOR_E_INVALID;
+    const bool compressed = data_mode == ERASOR_PCD_BINARY_COMPRESSED;
+    if (compressed && (n > 0xFFFFFFFFull / 16 || pcd::compressed_sizes_fit(16ull * n, 0) != ERASOR_OK)) return ERASOR_E_UNSUPPORTED;
+    char head[512];
+    const int hl = pcd::format_header(head, sizeof(head), n, data_mode);
+    inf.data_mode = (uint32_t)data_mode;
+    inf.header_bytes = (uint64_t)hl;
+    const uint64_t body = 16ull * n;
+    std::vector<uint8_t> file(head, head + hl);
+    if (!compressed) {
+        file.resize(hl + body);
+        if (n) std::memcpy(file.data() + hl, xyzi, body);
+    } else {
+        const uint32_t* w = reinterpret_cast<const uint32_t*>(xyzi);
+        std::vector<uint32_t> soa(4 * n);
+        for (size_t i = 0; i < n; ++i)
+            for (int s = 0; s < 4; ++s) soa[s * n + i] = w[4 * i + s];
+        const uint64_t nseg = (body + pcd::kLzfSeg - 1) / pcd::kLzfSeg;
+        std::vector<uint8_t> stream(nseg * pcd::lzf_segment_cap(pcd::kLzfSeg));
+        uint64_t csize = 0, ntok = 0, segs = 0;
+        erasor_hostcheck_lzf_encode(reinterpret_cast<const uint8_t*>(soa.data()), body, stream.data(), stream.size(), &csize, &ntok, &segs);
+        if (pcd::compressed_sizes_fit(body, csize) != ERASOR_OK) return ERASOR_E_UNSUPPORTED;
+        const uint32_t sizes[2] = {(uint32_t)csize, (uint32_t)body};
+        file.resize(hl + 8 + csize);
+        std::memcpy(file.data() + hl, sizes, 8);
+        if (csize) std::memcpy(file.data() + hl + 8, stream.data(), csize);
+        inf.segments = (uint32_t)segs;
+        inf.uncompressed_size = body;
+        inf.compressed_size = csize;
+        inf.lzf_tokens = ntok;
+    }
+    *len = file.size();
+    if (info) *info = inf;
+    if (!out) return ERASOR_OK;
+    if (cap < file.size()) return ERASOR_E_CAPACITY;
+    std::memcpy(out, file.data(), file.size());
+    return ERASOR_OK;
 }
 }

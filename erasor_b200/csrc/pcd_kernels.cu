@@ -14,6 +14,8 @@
 // Load (erasor_pcd_load, DESIGN.md section 12.1): ascii goes to the parse above; binary is one pass of k_pcd_gather_tile; a
 // binary_compressed stream is decoded by k_lzf_walk (speculative token discovery), k_lzf_compose (scan of the chunks' entry maps),
 // k_lzf_records, k_lzf_expand / k_lzf_jump / k_lzf_fill (pointer jumping over back-references), then gathered by k_pcd_gather.
+// Write (erasor_pcd_format, DESIGN.md section 12.3): binary is the header and the cloud copied; binary_compressed is k_pcd_soa, then
+// k_lzf_encode (lzf_encode.h's segmented rule, one warp per segment) and k_lzf_compact after a scan of the segments' sizes.
 // Bags (erasor_bag_*, DESIGN.md section 12.2): the index is bag_index.h, on the host; one k_bag_gather launch decodes the clouds of a
 // load from the selected blobs.
 #include <cuda_runtime.h>
@@ -27,6 +29,7 @@
 #include "../../include/erasor_b200.h"
 #include "bag_index.h"
 #include "buffers.h"
+#include "lzf_encode.h"
 #include "pcd_binary.h"
 #include "pcd_codec.h"
 
@@ -418,6 +421,95 @@ __global__ void __launch_bounds__(kThreads) k_lzf_fill(const uint32_t* src, uint
         pcd::lzf_fill(src, out, j);
 }
 
+// ---- the binary_compressed writer (DESIGN.md section 12.3; the rule is lzf_encode.h) ---------------------------------------
+// the float4 cloud as x[n] | y[n] | z[n] | intensity[n]
+__global__ void __launch_bounds__(kThreads) k_pcd_soa(const uint4* pts, uint64_t n, uint32_t* soa) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint4 v = pts[i];
+        soa[i] = v.x;
+        soa[n + i] = v.y;
+        soa[2 * n + i] = v.z;
+        soa[3 * n + i] = v.w;
+    }
+}
+
+// warp-wide literal stretch s[0, n) as tokens at o (the byte layout of pcd::lzf_put_lits)
+__device__ __forceinline__ void warp_put_lits(uint8_t* o, const uint8_t* s, uint32_t n, int lane) {
+    for (uint32_t r = lane; r < pcd::lzf_lit_runs(n); r += 32) o[r * (pcd::kLzfMaxLit + 1)] = pcd::lzf_lit_control(n, r);
+    for (uint32_t k = lane; k < n; k += 32) o[pcd::lzf_lit_at(k)] = s[k];
+}
+
+// pcd::lzf_match_len, 32 byte pairs per step: the first pair that differs, or the end, ends the match
+__device__ __forceinline__ uint32_t warp_match_len(const uint8_t* s, uint32_t len, uint32_t i, uint32_t c, int lane) {
+    const uint32_t most = min(len - i, pcd::kLzfMaxRef);
+    for (uint32_t b = 3;; b += 32) {
+        const uint32_t j = b + lane;
+        const unsigned stop = __ballot_sync(0xFFFFFFFFu, j >= most || s[c + j] != s[i + j]);
+        if (stop) return b + __ffs(stop) - 1;
+    }
+}
+
+// One warp per segment.  The table sweep goes 32 positions a step: lanes whose three bytes hash alike (__match_any_sync) take
+// the nearest lower such lane as their candidate, the lowest of them the table's entry; then the highest of them enters the table.
+// This is cand(i) of lzf_encode.h for every position.  The greedy parse trails the sweep: in each step's window it takes the first
+// position at or past its own whose candidate counts (a ballot), extends the match 32 bytes at a time, and writes the literals
+// before it and the reference.  Tokens go to the segment's slot of pcd::lzf_segment_cap(kLzfSeg) bytes.
+__global__ void __launch_bounds__(32) k_lzf_encode(const uint8_t* soa, uint64_t usize, uint8_t* slots, uint64_t slot_cap, uint32_t* seg_len,
+                                                     uint32_t* seg_tok) {
+    __shared__ uint16_t table[pcd::kLzfHashSize];
+    const int lane = threadIdx.x;
+    const uint64_t seg = blockIdx.x, base0 = seg * pcd::kLzfSeg;
+    const uint32_t len = (uint32_t)min((uint64_t)pcd::kLzfSeg, usize - base0);
+    const uint8_t* s = soa + base0;
+    uint8_t* o = slots + seg * slot_cap;
+    for (uint32_t h = lane; h < pcd::kLzfHashSize; h += 32) table[h] = 0;
+    __syncwarp();
+    const uint32_t npos = pcd::lzf_positions(len);
+    uint32_t olen = 0, ntok = 0, lit = 0, p = 0;                        // warp-uniform
+    for (uint32_t base = 0; base < npos; base += 32) {
+        const uint32_t i = base + lane;
+        const bool act = i < npos;
+        const uint32_t h = act ? pcd::lzf_hash(s + i) : pcd::kLzfHashSize + lane;   // idle lanes match nobody
+        const unsigned same = __match_any_sync(0xFFFFFFFFu, h);
+        const unsigned lower = same & ((1u << lane) - 1u);
+        uint32_t c = 0;
+        bool has = false;
+        if (lower) { c = base + 31 - __clz(lower); has = true; }
+        else if (act) { const uint32_t t = table[h]; has = t != 0; c = t - 1; }
+        const bool ok = act && has && pcd::lzf_cand_ok(s, i, c);
+        __syncwarp();
+        if (act && (same >> lane) == 1u) table[h] = (uint16_t)(i + 1);   // the group's highest lane
+        __syncwarp();
+        const unsigned valid = __ballot_sync(0xFFFFFFFFu, ok);
+        while (p < base + 32) {
+            const unsigned m = valid & (~0u << (p - base));
+            if (!m) { p = base + 32; break; }
+            const uint32_t q = base + __ffs(m) - 1;
+            const uint32_t cq = __shfl_sync(0xFFFFFFFFu, c, q - base);
+            const uint32_t l = warp_match_len(s, len, q, cq, lane);
+            warp_put_lits(o + olen, s + lit, q - lit, lane);
+            olen += q - lit + pcd::lzf_lit_runs(q - lit);
+            ntok += pcd::lzf_lit_runs(q - lit) + 1;
+            if (lane == 0) pcd::lzf_put_ref(o + olen, l, q - cq);
+            olen += l - 2 < 7 ? 2 : 3;
+            p = lit = q + l;
+        }
+    }
+    warp_put_lits(o + olen, s + lit, len - lit, lane);
+    olen += len - lit + pcd::lzf_lit_runs(len - lit);
+    ntok += pcd::lzf_lit_runs(len - lit);
+    if (lane == 0) { seg_len[seg] = olen; seg_tok[seg] = ntok; }
+}
+
+// segment k's tokens from its slot to the stream at off[k]
+__global__ void __launch_bounds__(kThreads) k_lzf_compact(const uint8_t* slots, uint64_t slot_cap, const uint32_t* seg_len, const uint64_t* off,
+                                                          uint8_t* stream) {
+    const uint64_t k = blockIdx.x;
+    const uint8_t* src = slots + k * slot_cap;
+    uint8_t* dst = stream + off[k];
+    for (uint32_t j = threadIdx.x; j < seg_len[k]; j += blockDim.x) dst[j] = src[j];
+}
+
 // ---- erasor/node bags (DESIGN.md section 12.2; the index and the per-point decode are bag_index.h) --------------------------
 // One cloud of a erasor_bag_load call.  A cloud whose rows are contiguous (row_step == width x point_step, or one row) is one row
 // of n points; otherwise each of its rows is tiled on its own, so that a tile never spans row padding.
@@ -766,6 +858,7 @@ struct erasor_pcd_ctx {
     std::string err;
     DeviceBuffer text, chunk_cnt, chunk_off, lines, flags, rows, sums, out, stats;   // parse
     DeviceBuffer pts, lens, offs, ftext;                                              // format
+    DeviceBuffer soa, lz_slots, lz_seglen, lz_segtok, lz_segoff, lz_segtokoff;          // format, binary_compressed
     DeviceBuffer lz_map0, lz_map1, lz_tok, lz_byt, lz_entry, lz_ctok, lz_cbyt, lz_tokoff, lz_byteoff, lz_rec, lz_src, lz_dec, lz_flags;   // load
     DeviceBuffer bag_blobs, bag_desc;                                                 // erasor_bag_load
     PinnedBuffer h_stats;                                                             // PcdStats
@@ -788,12 +881,13 @@ struct erasor_pcd_ctx {
     bag::Bz2Found z2_found;
     uint64_t z2_scratch = 0;
     double z2_ms[4] = {0, 0, 0, 0};
-    // erasor_pcd_format_ascii's text of its last call, kept for a following call with the same input
+    // erasor_pcd_format(_ascii)'s file of its last call (in ftext), kept for a following call with the same input and mode
     bool cached = false;
     const float* c_ptr = nullptr;
     size_t c_n = 0;
-    int c_kind = -1;
+    int c_kind = -1, c_mode = -1;
     uint64_t c_len = 0;
+    erasor_pcd_format_info_t c_info{};
 };
 
 namespace {
@@ -1107,8 +1201,6 @@ int bag_decode(erasor_pcd_t p, std::string& msg) {
     return bag::finish_chunks(p->bag, reinterpret_cast<const bag::NodeOut*>(res.data()), msg);
 }
 
-const char* kHeadFmt ="# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z intensity\nSIZE 4 4 4 4\nTYPE F F F F\n"
-                       "COUNT 1 1 1 1\nWIDTH %zu\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS %zu\nDATA ascii\n";
 }  // namespace
 
 extern "C" {
@@ -1279,11 +1371,11 @@ int erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_
     if (in_kind == ERASOR_PTR_DEVICE && (reinterpret_cast<uintptr_t>(xyzi) & 15u))
         return fail(p, ERASOR_E_INVALID, "device clouds must be 16-byte aligned (one float4 per point)");
     PCK(cudaSetDevice(p->device));
-    const bool hit = p->cached && p->c_ptr == xyzi && p->c_n == n && p->c_kind == in_kind;
+    const bool hit = p->cached && p->c_ptr == xyzi && p->c_n == n && p->c_kind == in_kind && p->c_mode == ERASOR_PCD_ASCII;
     p->cached = false;
     if (!hit) {
         char head[512];
-        const int hl = std::snprintf(head, sizeof(head), kHeadFmt, n, n);
+        const int hl = pcd::format_header(head, sizeof(head), n, ERASOR_PCD_ASCII);
         const float4* d_pts = reinterpret_cast<const float4*>(xyzi);
         if (in_kind == ERASOR_PTR_HOST && n) {
             PCK(p->pts.ensure(sizeof(float4) * n));
@@ -1308,12 +1400,113 @@ int erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_
             PCK(cudaGetLastError());
         }
         PCK(cudaStreamSynchronize(p->st));
-        p->c_ptr = xyzi; p->c_n = n; p->c_kind = in_kind; p->c_len = total;
+        p->c_ptr = xyzi; p->c_n = n; p->c_kind = in_kind; p->c_mode = ERASOR_PCD_ASCII; p->c_len = total;
+        p->c_info = erasor_pcd_format_info_t{};
+        p->c_info.header_bytes = (uint64_t)hl;
     }
     *len = (size_t)p->c_len;
     if (!out || cap < p->c_len) {
         p->cached = true;                             // the following call with the same input fetches this text
         return out ? fail(p, ERASOR_E_CAPACITY, "out holds fewer bytes than the formatted text") : ERASOR_OK;
+    }
+    PCK(cudaMemcpyAsync(out, p->ftext.p(), p->c_len, out_kind == ERASOR_PTR_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, p->st));
+    PCK(cudaStreamSynchronize(p->st));
+    return ERASOR_OK;
+}
+
+int erasor_pcd_format(erasor_pcd_t p, const float* xyzi, size_t n, int in_kind, int data_mode, char* out, size_t cap, int out_kind,
+                      size_t* len, erasor_pcd_format_info_t* info) {
+    if (!p) return ERASOR_E_INVALID;
+    p->err.clear();
+    if (data_mode == ERASOR_PCD_ASCII) {
+        const int rc = erasor_pcd_format_ascii(p, xyzi, n, in_kind, out, cap, out_kind, len);
+        if ((rc == ERASOR_OK || rc == ERASOR_E_CAPACITY) && info) *info = p->c_info;
+        return rc;
+    }
+    if (data_mode != ERASOR_PCD_BINARY && data_mode != ERASOR_PCD_BINARY_COMPRESSED)
+        return fail(p, ERASOR_E_INVALID, "data_mode must be ERASOR_PCD_ASCII, ERASOR_PCD_BINARY or ERASOR_PCD_BINARY_COMPRESSED");
+    if (!len || (n && !xyzi)) return fail(p, ERASOR_E_INVALID, "null argument");
+    if ((in_kind != ERASOR_PTR_HOST && in_kind != ERASOR_PTR_DEVICE) || (out_kind != ERASOR_PTR_HOST && out_kind != ERASOR_PTR_DEVICE))
+        return fail(p, ERASOR_E_INVALID, "in_kind and out_kind must be ERASOR_PTR_HOST or ERASOR_PTR_DEVICE");
+    if (in_kind == ERASOR_PTR_DEVICE && (reinterpret_cast<uintptr_t>(xyzi) & 15u))
+        return fail(p, ERASOR_E_INVALID, "device clouds must be 16-byte aligned (one float4 per point)");
+    const bool compressed = data_mode == ERASOR_PCD_BINARY_COMPRESSED;
+    if (compressed && (n > 0xFFFFFFFFull / 16 || pcd::compressed_sizes_fit(16ull * n, 0) != ERASOR_OK))
+        return fail(p, ERASOR_E_UNSUPPORTED, "binary_compressed: POINTS x 16 exceeds the format's uint32 uncompressed_size");
+    PCK(cudaSetDevice(p->device));
+    const bool hit = p->cached && p->c_ptr == xyzi && p->c_n == n && p->c_kind == in_kind && p->c_mode == data_mode;
+    p->cached = false;
+    if (!hit) {
+        p->c_mode = -1;                               // ftext is about to change
+        char head[512];
+        const int hl = pcd::format_header(head, sizeof(head), n, data_mode);
+        erasor_pcd_format_info_t inf{};
+        inf.data_mode = (uint32_t)data_mode;
+        inf.header_bytes = (uint64_t)hl;
+        const uint64_t body = 16ull * n;
+        if (!compressed) {                            // the points as they are
+            PCK(p->ftext.ensure(hl + body));
+            PCK(cudaMemcpyAsync(p->ftext.p(), head, hl, cudaMemcpyHostToDevice, p->st));
+            if (n) PCK(cudaMemcpyAsync(p->ftext.as<uint8_t>() + hl, xyzi, body, in_kind == ERASOR_PTR_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, p->st));
+            PCK(cudaStreamSynchronize(p->st));
+            p->c_len = hl + body;
+        } else {
+            // the cloud as SoA, one warp per segment into worst-case slots, a scan of the segment sizes, then the slots compacted
+            const uint64_t nseg = (body + pcd::kLzfSeg - 1) / pcd::kLzfSeg;
+            const uint64_t slot = pcd::lzf_segment_cap(pcd::kLzfSeg);
+            uint64_t csize = 0, ntok = 0;
+            if (n) {
+                const uint4* d_pts = reinterpret_cast<const uint4*>(xyzi);
+                if (in_kind == ERASOR_PTR_HOST) {
+                    PCK(p->pts.ensure(body));
+                    PCK(cudaMemcpyAsync(p->pts.p(), xyzi, body, cudaMemcpyHostToDevice, p->st));
+                    d_pts = p->pts.as<uint4>();
+                }
+                PCK(p->soa.ensure(body));
+                PCK(p->lz_slots.ensure(nseg * slot));
+                PCK(p->lz_seglen.ensure(sizeof(uint32_t) * nseg));
+                PCK(p->lz_segtok.ensure(sizeof(uint32_t) * nseg));
+                PCK(p->lz_segoff.ensure(sizeof(uint64_t) * nseg));
+                PCK(p->lz_segtokoff.ensure(sizeof(uint64_t) * nseg));
+                k_pcd_soa<<<blocks_for(n, kThreads, p->sm_count * 16), kThreads, 0, p->st>>>(d_pts, n, p->soa.as<uint32_t>());
+                k_lzf_encode<<<(unsigned)nseg, 32, 0, p->st>>>(p->soa.as<uint8_t>(), body, p->lz_slots.as<uint8_t>(), slot, p->lz_seglen.as<uint32_t>(),
+                                                              p->lz_segtok.as<uint32_t>());
+                PCK(cudaGetLastError());
+                int rc = scan_u32(p, p->lz_segtok.as<uint32_t>(), nseg, p->lz_segtokoff.as<uint64_t>(), nullptr);
+                if (rc == ERASOR_OK) rc = scan_u32(p, p->lz_seglen.as<uint32_t>(), nseg, p->lz_segoff.as<uint64_t>(), &csize);
+                if (rc != ERASOR_OK) return rc;
+                PCK(cudaMemcpyAsync(&ntok, p->lz_segtokoff.as<uint64_t>() + (nseg - 1), sizeof(uint64_t), cudaMemcpyDeviceToHost, p->st));
+                uint32_t last = 0;
+                PCK(cudaMemcpyAsync(&last, p->lz_segtok.as<uint32_t>() + (nseg - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, p->st));
+                PCK(cudaStreamSynchronize(p->st));
+                ntok += last;
+                if (pcd::compressed_sizes_fit(body, csize) != ERASOR_OK)
+                    return fail(p, ERASOR_E_UNSUPPORTED, "binary_compressed: the LZF stream exceeds the format's uint32 compressed_size");
+            }
+            const uint64_t total = (uint64_t)hl + 8 + csize;
+            PCK(p->ftext.ensure(total));
+            const uint32_t sizes[2] = {(uint32_t)csize, (uint32_t)body};   // little-endian, as the device is
+            PCK(cudaMemcpyAsync(p->ftext.p(), head, hl, cudaMemcpyHostToDevice, p->st));
+            PCK(cudaMemcpyAsync(p->ftext.as<uint8_t>() + hl, sizes, 8, cudaMemcpyHostToDevice, p->st));
+            if (n) {
+                k_lzf_compact<<<(unsigned)nseg, kThreads, 0, p->st>>>(p->lz_slots.as<uint8_t>(), slot, p->lz_seglen.as<uint32_t>(), p->lz_segoff.as<uint64_t>(),
+                                                                     p->ftext.as<uint8_t>() + hl + 8);
+                PCK(cudaGetLastError());
+            }
+            PCK(cudaStreamSynchronize(p->st));
+            p->c_len = total;
+            inf.segments = (uint32_t)nseg;
+            inf.uncompressed_size = body;
+            inf.compressed_size = csize;
+            inf.lzf_tokens = ntok;
+        }
+        p->c_ptr = xyzi; p->c_n = n; p->c_kind = in_kind; p->c_mode = data_mode; p->c_info = inf;
+    }
+    *len = (size_t)p->c_len;
+    if (info) *info = p->c_info;
+    if (!out || cap < p->c_len) {
+        p->cached = true;                             // the following call with the same input and mode fetches this file
+        return out ? fail(p, ERASOR_E_CAPACITY, "out holds fewer bytes than the formatted file") : ERASOR_OK;
     }
     PCK(cudaMemcpyAsync(out, p->ftext.p(), p->c_len, out_kind == ERASOR_PTR_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, p->st));
     PCK(cudaStreamSynchronize(p->st));

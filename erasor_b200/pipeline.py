@@ -7,7 +7,8 @@ scripts/analysis_runner.py):
                               (OfflineMapUpdater::callback_node / save_static_map, OfflineMapUpdater.cpp:174-330)
       -> PR / RR              capi.Evaluator (device), or erasor_b200.evaluate when the updater is injected
                               (scripts/analysis_runner.py)
-      -> <name>_naive_map.pcd, <name>_result.pcd (out_dir): capi.PcdCodec (device), or write_pcd_ascii when the updater is injected
+      -> <name>_naive_map.pcd, <name>_result.pcd (out_dir): capi.PcdCodec (device; ascii, binary or binary_compressed), or
+                              write_pcd_ascii when the updater is injected
 
 Everything heavy runs on the device behind the C ABI; this module only sequences the calls.  The updater and the voxeliser are
 injectable so that tests/test_pipeline.py can drive the same code with the oracle's objects on a machine without a GPU; with an
@@ -90,11 +91,18 @@ def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep
 
 def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, make_updater: Optional[Callable] = None,
                  map_leafsize: Optional[float] = None, out_dir: Optional[str] = None, frame_independent: bool = False,
-                 inserts: bool = False) -> dict:
+                 inserts: bool = False, pcd_mode: str = "ascii") -> dict:
     """mapgen -> updater -> evaluation on one node list.  GT for PR/RR = the naive map itself (it carries the labels), which is
     how the reference scores a run (analysis_runner.py compares <seq>_..._original / voxelised map with the result).
     frame_independent runs node mode (run_frame_independent) on the naive map instead of the sequential updater; inserts (node
-    mode only) puts each node's inserted query points back into its static map."""
+    mode only) puts each node's inserted query points back into its static map.  pcd_mode: the DATA mode of the two files written
+    to out_dir ("ascii", as the reference writes them, "binary" or "binary_compressed"; the binary modes need the device writer,
+    so an injected updater takes only "ascii")."""
+    from . import capi
+    if pcd_mode not in capi.PCD_MODES:
+        raise ValueError(f"pcd_mode must be one of {sorted(capi.PCD_MODES)}")
+    if pcd_mode != "ascii" and make_updater is not None:
+        raise ValueError("binary PCD files are written on the device: an injected updater writes ascii only")
     nodes = list(nodes)
     leaf = float(up.map_voxel_size if map_leafsize is None else map_leafsize)
     original, naive = mapgen.build_map(nodes, leafsize=leaf, is_large_scale=bool(up.is_large_scale), voxelize=voxelize)
@@ -120,8 +128,8 @@ def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, mak
         if make_updater is None:        # the device updater ran: format the files on the device too (the same bytes)
             from . import capi
             with capi.PcdCodec() as codec:
-                codec.write(paths[0], naive)
-                codec.write(paths[1], res["static_map"])
+                codec.write(paths[0], naive, mode=pcd_mode)
+                codec.write(paths[1], res["static_map"], mode=pcd_mode)
         else:
             evaluate.write_pcd_ascii(paths[0], naive)
             evaluate.write_pcd_ascii(paths[1], res["static_map"])

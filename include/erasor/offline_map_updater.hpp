@@ -157,7 +157,7 @@ inline void save_pcd_ascii(const std::string& path, const PointCloud& c) {
 // PCD files through the device codec (erasor_pcd_*).  read / read_device parse ASCII files and give what load_pcd gives bit for bit
 // (intensity 0 when the file has none); binary files are UnsupportedPcd there.  load / load_device read every DATA mode (ascii,
 // binary, binary_compressed) with PCL's field rules (DESIGN.md section 12.1).  The writer gives the bytes save_pcd_ascii writes
-// (NaN spelled "nan").
+// (NaN spelled "nan"), or a binary or binary_compressed file (DESIGN.md section 12.3).
 struct UnsupportedPcd : std::runtime_error { using std::runtime_error::runtime_error; };
 
 class PcdCodec {
@@ -208,16 +208,21 @@ public:
         c.resize(n);
         return c;
     }
-    void write(const std::string& path, const PointCloud& c) { write_from(path, reinterpret_cast<const float*>(c.data()), c.size(), ERASOR_PTR_HOST); }
+    // data_mode: ERASOR_PCD_ASCII (save_pcd_ascii's bytes), ERASOR_PCD_BINARY or ERASOR_PCD_BINARY_COMPRESSED (erasor_pcd_format)
+    void write(const std::string& path, const PointCloud& c, int data_mode = ERASOR_PCD_ASCII) {
+        write_from(path, reinterpret_cast<const float*>(c.data()), c.size(), ERASOR_PTR_HOST, data_mode);
+    }
     // the same file from n points in device memory (e.g. ERASOR::save_static_map's cloud)
-    void write_device(const std::string& path, const float* d_xyzi, size_t n) { write_from(path, d_xyzi, n, ERASOR_PTR_DEVICE); }
+    void write_device(const std::string& path, const float* d_xyzi, size_t n, int data_mode = ERASOR_PCD_ASCII) {
+        write_from(path, d_xyzi, n, ERASOR_PTR_DEVICE, data_mode);
+    }
 
 private:
-    void write_from(const std::string& path, const float* src, size_t n, int in_kind) {
+    void write_from(const std::string& path, const float* src, size_t n, int in_kind, int data_mode) {
         size_t len = 0;
-        check(erasor_pcd_format_ascii(p_, src, n, in_kind, nullptr, 0, ERASOR_PTR_HOST, &len), path);
+        check(erasor_pcd_format(p_, src, n, in_kind, data_mode, nullptr, 0, ERASOR_PTR_HOST, &len, nullptr), path);
         text_.resize(len);
-        check(erasor_pcd_format_ascii(p_, src, n, in_kind, text_.data(), len, ERASOR_PTR_HOST, &len), path);
+        check(erasor_pcd_format(p_, src, n, in_kind, data_mode, text_.data(), len, ERASOR_PTR_HOST, &len, nullptr), path);
         std::ofstream f(path, std::ios::binary);
         if (!f || !f.write(text_.data(), (std::streamsize)len)) throw std::runtime_error("cannot write " + path);
     }

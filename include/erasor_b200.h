@@ -434,6 +434,32 @@ int  erasor_pcd_parse_ascii(erasor_pcd_t p, const char* text, size_t len, int te
  * for the following call with the same (xyzi, n, in_kind), which then only copies it out.  out: host or device per out_kind. */
 int  erasor_pcd_format_ascii(erasor_pcd_t p, const float* xyzi, size_t n, int in_kind, char* out, size_t cap, int out_kind, size_t* len);
 
+/* A PCD file in any DATA mode for n points (DESIGN.md section 12.3), with the same header as erasor_pcd_format_ascii (only the DATA
+ * word differs).  ERASOR_PCD_ASCII is erasor_pcd_format_ascii, unchanged.  ERASOR_PCD_BINARY: the header, then the cloud's 16-byte
+ * points in order, bit for bit.  ERASOR_PCD_BINARY_COMPRESSED: the header, uint32 compressed_size and uint32 uncompressed_size
+ * (little-endian), then one LZF stream over x[n] | y[n] | z[n] | intensity[n] (PCL 1.8's writeBinaryCompressed layout for these
+ * fields), encoded in independent segments by the rule of DESIGN.md section 12.3; erasor_pcd_load and PCL's reader rules read it
+ * back bit for bit.  Byte identity with PCL's writers is not claimed.  Arguments and caching as erasor_pcd_format_ascii, keyed on
+ * (xyzi, n, in_kind, data_mode); one cache serves both functions.  Errors: an unknown data_mode, a misaligned device cloud
+ * (ERASOR_E_INVALID); binary_compressed with n x 16 > 0xFFFFFFFF (checked before anything is read) or a stream longer than
+ * 0xFFFFFFFF bytes (ERASOR_E_UNSUPPORTED: the format's sizes are uint32).  n == 0 is a header-only file (binary_compressed: and
+ * two zero sizes).  info (nullable) is written whenever *len is.  Synchronous. */
+#define ERASOR_PCD_ASCII              0   /* the same numbering as erasor_pcd_load_info_t.data_mode */
+#define ERASOR_PCD_BINARY             1
+#define ERASOR_PCD_BINARY_COMPRESSED  2
+
+typedef struct {
+    uint32_t data_mode;
+    uint32_t segments;            /* binary_compressed: independently encoded LZF segments */
+    uint64_t header_bytes;
+    uint64_t uncompressed_size;   /* binary_compressed: POINTS x 16 */
+    uint64_t compressed_size;     /* binary_compressed: bytes of the LZF stream */
+    uint64_t lzf_tokens;          /* binary_compressed: literal runs + back-references */
+} erasor_pcd_format_info_t;
+
+int  erasor_pcd_format(erasor_pcd_t p, const float* xyzi, size_t n, int in_kind, int data_mode, char* out, size_t cap, int out_kind,
+                       size_t* len, erasor_pcd_format_info_t* info);
+
 /* Any PCD DATA mode on the device (DESIGN.md section 12.1), with the field rules of PCL 1.8's PCDReader and
  * fromPCLPointCloud2<PointXYZI> (restated; PCL is not built here).  ascii goes to erasor_pcd_parse_ascii unchanged (results, errors
  * and info->ascii).  binary and binary_compressed: SIZE and TYPE are required (F 4/8, I/U 1/2/4, else ERASOR_E_UNSUPPORTED); COUNT is
