@@ -30,6 +30,7 @@ EXPORTS = [
     "erasor_process_frames_fold_async", "erasor_fold_keep_masks", "erasor_reset_keep_mask", "erasor_get_frame_stats", "erasor_kernel_launch_count",
     "erasor_map_create", "erasor_map_destroy", "erasor_map_size", "erasor_map_reset_keep", "erasor_map_get_keep", "erasor_map_keep_device",
     "erasor_map_points_device", "erasor_attach_map", "erasor_process_nodes", "erasor_process_nodes_async", "erasor_get_node_stats",
+    "erasor_process_nodes_sweep", "erasor_process_nodes_sweep_async", "erasor_get_sweep_stats",
     "erasor_voxelize_batch",
     "erasor_set_node_inserts", "erasor_get_node_inserts", "erasor_map_append_inserts", "erasor_map_inserts", "erasor_map_clear_inserts",
     "erasor_save_node_map",
@@ -56,6 +57,15 @@ class EvalCountsC(ctypes.Structure):
 class EvalOverlapC(ctypes.Structure):
     """erasor_eval_overlap_t"""
     _fields_ = [(name, c_uint64) for name in ("n", "est_static", "est_dynamic", "below_half", "below_one", "below_two", "far_points")] + [("max", c_double)]
+
+
+class SrtVariantC(ctypes.Structure):
+    """erasor_srt_variant_t"""
+    _fields_ = [("scan_ratio_threshold", c_double), ("th_bin_max_h", c_double), ("minimum_num_pts", c_int), ("reserved", c_int)]
+
+
+SRT_SWEEP_FIELDS = ("scan_ratio_threshold", "th_bin_max_h", "minimum_num_pts")     # what a Scan Ratio Test sweep varies
+MAX_SWEEP_VARIANTS = 32
 
 
 class PcdInfoC(ctypes.Structure):
@@ -179,6 +189,10 @@ def _load():
     L.erasor_process_nodes.argtypes = [c_void_p, POINTER(c_double), c_void_p, POINTER(c_uint64), c_int, c_double, c_void_p, c_void_p, c_int]
     L.erasor_process_nodes_async.argtypes = L.erasor_process_nodes.argtypes
     L.erasor_get_node_stats.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32), POINTER(c_uint32)]
+    L.erasor_process_nodes_sweep.argtypes = [c_void_p, POINTER(c_double), c_void_p, POINTER(c_uint64), c_int, c_double, POINTER(SrtVariantC), c_int,
+                                             c_void_p, c_int]
+    L.erasor_process_nodes_sweep_async.argtypes = L.erasor_process_nodes_sweep.argtypes
+    L.erasor_get_sweep_stats.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32)]
     L.erasor_voxelize_batch.argtypes = [c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p, c_float, POINTER(c_double), c_int,
                                         POINTER(c_void_p), POINTER(c_uint64)]
     L.erasor_set_node_inserts.argtypes = [c_void_p, c_int]
@@ -538,6 +552,51 @@ class Handle(_Native):
         self._ck(self.L.erasor_get_node_stats(self.h, nv.ctypes.data_as(POINTER(c_uint32)), nf.ctypes.data_as(POINTER(c_uint32)),
                                               nr.ctypes.data_as(POINTER(c_uint32))))
         return nv, nf, nr
+
+    # -- Scan Ratio Test sweep (DESIGN.md section 8.5) ----------------------------------------------------------------------------
+    def sweep_variants(self, variants):
+        """variants (dicts or objects with any of SRT_SWEEP_FIELDS; a missing field takes the handle's value) -> SrtVariantC array"""
+        vs = list(variants)
+        arr = (SrtVariantC * max(len(vs), 1))()
+        for i, v in enumerate(vs):
+            get = v.get if isinstance(v, dict) else (lambda k, d, v=v: getattr(v, k, d))
+            arr[i].scan_ratio_threshold = float(get("scan_ratio_threshold", self.params.scan_ratio_threshold))
+            arr[i].th_bin_max_h = float(get("th_bin_max_h", self.params.th_bin_max_h))
+            arr[i].minimum_num_pts = int(get("minimum_num_pts", self.params.minimum_num_pts))
+        return arr, len(vs)
+
+    def process_nodes_sweep(self, poses7, query_xyzi, query_offsets, variants, keep_ptr: int, voi_max_range: float = 0.0,
+                            packed_xyz: bool = False, asynchronous: bool = False):
+        """erasor_process_nodes_sweep: the node batch against the attached map under every Scan Ratio Test setting of `variants`
+        (1..32), mask v folded into the device bytes [keep_ptr + v n_map, keep_ptr + (v + 1) n_map) (they accumulate: start with
+        reset_keep_mask(keep_ptr, V n_map)).  query_xyzi: a host float32 [n,4] array (shipped as packed x y z with packed_xyz) or a
+        device pointer (int; packed x y z with packed_xyz).  The map's own keep mask is left as it is."""
+        P = np.ascontiguousarray(poses7, dtype=np.float64).reshape(-1, 7)
+        qo = np.ascontiguousarray(query_offsets, dtype=np.uint64)
+        F = len(qo) - 1
+        assert len(P) == F
+        arr, V = self.sweep_variants(variants)
+        if isinstance(query_xyzi, (int, np.integer)):
+            qptr, kind = c_void_p(int(query_xyzi)) if int(query_xyzi) else None, PTR_DEVICE
+        else:
+            q = _cloud(query_xyzi)
+            if packed_xyz:
+                q = np.ascontiguousarray(q[:, :3])
+            self._keep = [q]
+            qptr, kind = q.ctypes.data, PTR_HOST
+        fn = self.L.erasor_process_nodes_sweep_async if asynchronous else self.L.erasor_process_nodes_sweep
+        self._sweep_args = (P, qo, arr)      # alive until the asynchronous submission has been waited for
+        self._ck(fn(self.h, P.ctypes.data_as(POINTER(c_double)), qptr, qo.ctypes.data_as(POINTER(c_uint64)), F, float(voi_max_range),
+                    arr, V, c_void_p(keep_ptr) if keep_ptr else None, kind | (PTR_QUERY_XYZ if packed_xyz else 0)))
+        self.n_frames = F
+        self.n_variants = V
+
+    def sweep_stats(self):
+        """(flagged bins, rejected points) of the last sweep, uint32 [V, F] each"""
+        V, F = self.n_variants, self.n_frames
+        nf, nr = np.zeros((V, F), dtype=np.uint32), np.zeros((V, F), dtype=np.uint32)
+        self._ck(self.L.erasor_get_sweep_stats(self.h, nf.ctypes.data_as(POINTER(c_uint32)), nr.ctypes.data_as(POINTER(c_uint32))))
+        return nf, nr
 
     # -- batched voxelize_preserving_labels (query preparation, saving node mode's map) -----------------------------------------
     def voxelize_batch_ptr(self, xyzi_ptr: int, offsets, leaf: float, keep_ptr: int = 0, pose7=None, ptr_kind: int = PTR_HOST):

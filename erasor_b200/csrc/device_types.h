@@ -60,6 +60,31 @@ struct SrtParams {
     int    scatter_mode;       // 0: every bin (cloud outputs), 1: flagged bins only (mask outputs)
 };
 
+// Scan Ratio Test sweep (erasor_process_nodes_sweep, DESIGN.md section 8.5): the three per-setting fields of one variant (the
+// layout of erasor_srt_variant_t) and the variants of one K2 launch, passed by value (32 x 24 = 768 bytes of kernel parameters)
+constexpr int kMaxSweepVariants = 32;
+struct SrtVariant {
+    double scan_ratio_threshold;
+    double th_bin_max_h;
+    int    minimum_num_pts;
+    int    reserved;
+};
+struct SrtSweep {
+    SrtVariant v[kMaxSweepVariants];
+    int        n;                  // variants in use, 1..32
+    int        pad_;
+    uint32_t*  n_flagged;          // [F][32] flagged bins per (frame, variant) of the submission
+};
+
+// The sweep's fold in K4's epilogue: keep[v * n + src] = 0 for every rejected point and every variant v whose bit the bin's
+// record carries (FlagRec::cursor); rejected[frame * 32 + v] counts them.
+struct K4Sweep {
+    uint8_t*  keep;                // [V][n] variant masks
+    uint32_t* rejected;            // [F][32]
+    uint32_t  n;                   // map points (writes beyond it are dropped)
+    uint32_t  pad_;
+};
+
 struct GpfParams {
     double th_dist;            // gf_dist_thr
     double th_seeds;           // gf_th_seeds_height
@@ -117,7 +142,7 @@ struct FlagRec {
     uint32_t n_seeds;
     uint32_t n_empty_fits;
     uint32_t n_ground_final;
-    uint32_t cursor;           // reserved
+    uint32_t cursor;           // a sweep's variants that flag the bin (bit v); 0 outside a sweep
     uint32_t n_rejected;       // points handed to map_rejected (0 when gf_iter == 0: the reference fills no outliers then)
     double   lpr_height;
     double   normal_d[kMaxIter][4];

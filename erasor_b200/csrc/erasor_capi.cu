@@ -7,6 +7,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -90,6 +91,7 @@ struct erasor_ctx {
     HBuf d_list_idx{alloc_epoch}, d_list_cnt{alloc_epoch};   // node mode: per chunk, the map index of every VoI point (dense, map order) and their number
     HBuf d_k1prof{alloc_epoch};                // erasor_profile_k1: per-warp cycle counters of K1's profiling build
     HBuf d_pack{alloc_epoch}, d_gather{alloc_epoch};         // exchange step: packed keep bits of this rank / of every rank
+    HBuf d_sweep_flag{alloc_epoch}, d_sweep_rej{alloc_epoch};  // Scan Ratio Test sweep: flagged bins / rejected points per (frame, variant), [stat_F][32]
     PinnedBuffer h_stage, h_pose, h_words;     // h_words: small device -> host read-backs of a submission (pinned: an asynchronous copy into
                                                // pageable memory blocks the launching thread until the whole stream has drained, which
                                                // serialised overlapped handles)
@@ -109,7 +111,8 @@ struct erasor_ctx {
     int      stat_F = 0;                       // frames of the last batch call (all its sub-batches): extent of the per-frame counters
     int      f0 = 0;                           // first frame of the sub-batch being submitted
     std::vector<uint32_t> node_nvoi;           // node mode: |map_voi_| of the frames before f0 (the count tables hold the last sub-batch only)
-    struct StepGraph { const void* ptr[8]; size_t fold_n; int kind, mode, f0; uint64_t epoch, alloc; cudaGraphExec_t exec; };
+    struct StepGraph { const void* ptr[8]; size_t fold_n; int kind, mode, f0; uint64_t epoch, alloc; cudaGraphExec_t exec;
+                       const void* vkeep; int nv; SrtVariant var[kMaxSweepVariants]; };   // vkeep / nv / var: a sweep's masks and variants
     std::vector<StepGraph> graphs;             // captured mask-mode steps, one per (pointers, geometry)
     bool     use_graphs = true;
     int      ctas_per_sm = 4;                  // K1 / K2 grid target: one wave of sm_count * ctas_per_sm CTAs (ERASOR_B200_CTAS_PER_SM)
@@ -121,7 +124,9 @@ struct erasor_ctx {
     int      class_c_state = -1;               // -1 unknown (launch it), 0 none in the last run, > 0 seen
     uint32_t class_c_count_host = 0;           // queue[kBucketC0] of the submission in flight
     struct { bool with_c = true, host = false; int mode = 1; uint8_t* d_keep = nullptr; uint8_t* user_keep = nullptr; size_t n_keep = 0;
-             uint8_t* keep_out = nullptr; size_t n_map_global = 0; K4Fold fold{nullptr, nullptr, 0u, 0u}; } last;
+             uint8_t* keep_out = nullptr; size_t n_map_global = 0; K4Fold fold{nullptr, nullptr, 0u, 0u};
+             bool sweep = false; K4Sweep ksweep{nullptr, nullptr, 0u, 0u}; } last;
+    int      sweep_V = 0;                      // variants of the last node call when it was a sweep (erasor_get_sweep_stats), else 0
 
     // node mode
     erasor_map_ctx* map = nullptr;
@@ -381,12 +386,14 @@ bool inserts_on(const erasor_ctx* h, int mode) { return mode == 2 && h->node_ins
 
 int run_insert_plan(erasor_ctx* h);
 
-int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes = 7, bool only_rgpf = false) {
+// sweep / k4sweep: a Scan Ratio Test sweep (node mode): the variants' flags in K2, their masks in K4's epilogue
+int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes = 7, bool only_rgpf = false,
+                const SrtSweep* sweep = nullptr, const K4Sweep* k4sweep = nullptr) {
     const int B = h->B, F = h->F;
     const NodePose* poses = mode == 2 ? h->d_poses.as<NodePose>() : nullptr;
     uint32_t* nflag = h->d_nflag.as<uint32_t>() + h->f0;
     const SrtParams sp = srt_params(h, version, mode);
-    const bool fused = mode != 0 && h->fused_srt;      // mask modes: SRT inside the scatter kernel
+    const bool fused = mode != 0 && (h->fused_srt || sweep);      // mask modes: SRT inside the scatter kernel (a sweep has no K3 form)
     if (!fused && !only_rgpf) {
         Scope s(h, 3);
         h->launches++;
@@ -410,7 +417,7 @@ int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_
                              h->cur_map, poses, h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(), h->d_zmax.as<uint32_t>(), h->d_cnt.as<uint32_t>(),
                              h->d_frame_off.as<uint32_t>(), nflag, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
                              h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
-                             poses ? h->d_list_idx.as<uint32_t>() : nullptr, poses ? h->d_list_cnt.as<uint32_t>() : nullptr));
+                             poses ? h->d_list_idx.as<uint32_t>() : nullptr, poses ? h->d_list_cnt.as<uint32_t>() : nullptr, sweep));
         } else {
             // mask modes, unfused (ERASOR_B200_UNFUSED_SRT=1): the same stable scatter, restricted to the flagged bins (K3's dense slots)
             if (h->n_chunks_map) h->launches++;
@@ -435,7 +442,7 @@ int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_
         CK(launch_k4(h->stream_a, h->stream_b, h->stream_c, gp, h->d_recs.as<FlagRec>(), h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->rec_capacity,
                      h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), h->cur_map,
                      h->d_frame_off.as<uint32_t>(), (mode == 0 || inserts_on(h, mode)) ? h->d_part.as<float4>() : nullptr, keep_mask, ground_mask,
-                     h->d_frame_rej.as<uint32_t>() + h->f0, h->d_scratch.as<unsigned char>(), h->sm_count, h->d_fence.as<unsigned long long>(), fold, classes));
+                     h->d_frame_rej.as<uint32_t>() + h->f0, h->d_scratch.as<unsigned char>(), h->sm_count, h->d_fence.as<unsigned long long>(), fold, classes, k4sweep));
         CK(cudaEventRecord(h->ev_join_a, h->stream_a));
         CK(cudaEventRecord(h->ev_join_b, h->stream_b));
         if (with_c) CK(cudaEventRecord(h->ev_join_c, h->stream_c));
@@ -931,6 +938,9 @@ struct Submit {
     const double*   poses7 = nullptr;       // mode 2: the caller's odom7 of these frames (the inserts' body -> origin)
     uint8_t*        keep_out = nullptr;     // mode 2 (nullable)
     int             f0 = 0;                 // index of the first frame within the caller's batch (per-frame counters)
+    const SrtVariant* variants = nullptr;   // mode 2: a Scan Ratio Test sweep of n_variants settings into variant_keep [V][n_map]
+    int             n_variants = 0;
+    uint8_t*        variant_keep = nullptr;
 };
 
 bool is_pinned_host(const void* p) {
@@ -976,6 +986,18 @@ int submit(erasor_ctx* h, const Submit& S) {
         }
     }
     const bool with_c = h->class_c_state != 0;
+    const bool sweep = S.n_variants > 0;
+    SrtSweep ssw{};
+    K4Sweep  ksw{nullptr, nullptr, 0u, 0u};
+    if (sweep) {
+        const size_t rows = (size_t)kMaxSweepVariants * (size_t)std::max(h->stat_F, h->f0 + S.F);
+        CK(h->d_sweep_flag.ensure(sizeof(uint32_t) * rows));
+        CK(h->d_sweep_rej.ensure(sizeof(uint32_t) * rows));
+        std::copy(S.variants, S.variants + S.n_variants, ssw.v);
+        ssw.n = S.n_variants;
+        ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + (size_t)kMaxSweepVariants * S.f0;
+        ksw = K4Sweep{S.variant_keep, h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * S.f0, (uint32_t)n_map_global, 0u};
+    }
     auto enqueue = [&]() -> int {
         int r;
         if (S.mode == 1) {
@@ -990,11 +1012,15 @@ int submit(erasor_ctx* h, const Submit& S) {
             d_keep = host ? h->d_keep.as<uint8_t>() : S.keep_mask;
             CK(cudaMemsetAsync(d_keep, 1, n_keep, h->stream));
         }
+        if (sweep) {
+            CK(cudaMemsetAsync(ssw.n_flagged, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)S.F, h->stream));
+            CK(cudaMemsetAsync(ksw.rejected, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)S.F, h->stream));
+        }
         if ((r = run_k1(h, S.mode))) return r;
         K4Fold fold{nullptr, nullptr, 0u, 0u};
-        if (S.mode == 2)        fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};
-        else if (S.fold_global) fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
-        if ((r = run_compare(h, h->p.version, S.mode, d_keep, nullptr, fold, with_c ? 7 : 3))) return r;
+        if (S.mode == 2 && !sweep) fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};   // a sweep leaves the map's mask alone
+        else if (S.fold_global)    fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
+        if ((r = run_compare(h, h->p.version, S.mode, d_keep, nullptr, fold, with_c ? 7 : 3, false, sweep ? &ssw : nullptr, sweep ? &ksw : nullptr))) return r;
         if (ins && (r = run_insert_assemble(h))) return r;      // (run_compare ran the plan and the query scatter under R-GPF)
         h->last.with_c = with_c; h->last.host = host; h->last.mode = S.mode; h->last.d_keep = d_keep; h->last.user_keep = S.keep_mask; h->last.n_keep = n_keep;
         h->last.keep_out = S.keep_out; h->last.n_map_global = n_map_global; h->last.fold = fold;
@@ -1018,9 +1044,12 @@ int submit(erasor_ctx* h, const Submit& S) {
         key.ptr[0] = S.map_xyzi; key.ptr[1] = S.qry_xyzi; key.ptr[2] = S.keep_mask; key.ptr[3] = S.fold_index; key.ptr[4] = S.fold_global;
         key.ptr[5] = S.keep_out; key.ptr[6] = S.mode == 2 ? (const void*)h->map : nullptr; key.ptr[7] = with_c ? (const void*)h : nullptr;
         key.fold_n = S.fold_n; key.kind = S.ptr_kind | (S.qry_xyz ? ERASOR_PTR_QUERY_XYZ : 0) | (ins ? 0x100 : 0); key.mode = S.mode; key.f0 = S.f0; key.epoch = h->desc_epoch; key.alloc = h->alloc_epoch;
+        key.vkeep = S.variant_keep; key.nv = S.n_variants;
+        if (sweep) std::copy(S.variants, S.variants + S.n_variants, key.var);
         auto same = [&](const erasor_ctx::StepGraph& g) {
             return std::equal(g.ptr, g.ptr + 8, key.ptr) && g.fold_n == key.fold_n && g.kind == key.kind && g.mode == key.mode && g.f0 == key.f0 &&
-                   g.epoch == key.epoch && g.alloc == key.alloc;
+                   g.epoch == key.epoch && g.alloc == key.alloc && g.vkeep == key.vkeep && g.nv == key.nv &&
+                   std::memcmp(g.var, key.var, sizeof(SrtVariant) * (size_t)key.nv) == 0;
         };
         cudaGraphExec_t exec = nullptr;
         for (auto& g : h->graphs) if (same(g)) exec = g.exec;
@@ -1063,9 +1092,10 @@ int submit(erasor_ctx* h, const Submit& S) {
         h->last.with_c = with_c; h->last.host = hst; h->last.mode = S.mode; h->last.user_keep = S.keep_mask; h->last.n_keep = n_keep;
         h->last.d_keep = n_keep ? (hst ? h->d_keep.as<uint8_t>() : S.keep_mask) : nullptr;
         h->last.keep_out = S.keep_out; h->last.n_map_global = n_map_global;
-        if (S.mode == 2)        h->last.fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};
-        else if (S.fold_global) h->last.fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
-        else                    h->last.fold = K4Fold{nullptr, nullptr, 0u, 0u};
+        if (S.mode == 2 && !sweep) h->last.fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};
+        else if (S.fold_global)    h->last.fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
+        else                       h->last.fold = K4Fold{nullptr, nullptr, 0u, 0u};
+        h->last.sweep = sweep; h->last.ksweep = ksw;
     }
     h->pending = true;
     return ERASOR_OK;
@@ -1091,6 +1121,7 @@ int process_frames_impl(erasor_handle_t h, const float* map_xyzi, const uint64_t
     int rc;
     if (h->pending && (rc = erasor_wait(h))) return rc;
     h->stat_F = n_frames;
+    h->sweep_V = 0;
     h->ins_call_off.clear();                   // the inserts of an earlier node call end with this submission
     std::vector<uint64_t> mo, qo;
     for (int f0 = 0; f0 < n_frames;) {
@@ -1131,7 +1162,8 @@ int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
 }
 
 int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
-                       double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind, bool async) {
+                       double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind, bool async,
+                       const SrtVariant* variants = nullptr, int n_variants = 0, uint8_t* variant_keep = nullptr) {
     if (!h || !poses7 || !query_offsets) { if (h) h->err = "null argument"; return ERASOR_E_INVALID; }
     if (!h->map) { h->err = "erasor_process_nodes: no map attached (erasor_attach_map)"; return ERASOR_E_STATE; }
     if (n_frames <= 0) { h->err = "n_frames must be positive"; return ERASOR_E_INVALID; }
@@ -1147,6 +1179,7 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
     const size_t N = h->map->n;
     const double range = voi_max_range > 0.0 ? voi_max_range : h->p.max_range;
     h->stat_F = n_frames;
+    h->sweep_V = n_variants;
     h->ins_call_off.assign(h->node_inserts ? 1 : 0, 0);
     // scratch per (frame, map point): bin id 2 + scattered point 16 + source index 4 + class-C scratch 24 bytes; with inserts also
     // R-GPF's partitioned copy 16 + the inserts 16 + K4b's voxels 16 and scratch 36 bytes
@@ -1180,6 +1213,7 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         S.poses = poses.data();
         S.poses7 = poses7 + 7 * (size_t)f0;
         S.keep_out = (f1 == n_frames) ? keep_out : nullptr;
+        S.variants = variants; S.n_variants = n_variants; S.variant_keep = variant_keep;
         if ((rc = submit(h, S))) return rc;
         if (f1 < n_frames) {                                         // the next sub-batch reuses the handle's buffers
             if ((rc = erasor_wait(h))) return rc;
@@ -1205,7 +1239,8 @@ int erasor_wait(erasor_handle_t h) {
         if (!h->last.with_c && h->class_c_count_host > 0) {
             // bins beyond class B's capacity turned up in a submission that ran without class C: run that class now (R-GPF only; the
             // bins are independent, the masks only gain zeros), then repeat the output copies.  The next submissions launch it up front.
-            int rc = run_compare(h, h->p.version, h->last.mode, h->last.d_keep, nullptr, h->last.fold, 4, true);
+            int rc = run_compare(h, h->p.version, h->last.mode, h->last.d_keep, nullptr, h->last.fold, 4, true, nullptr,
+                                 h->last.sweep ? &h->last.ksweep : nullptr);
             if (rc) return rc;
             if (inserts_on(h, h->last.mode) && (rc = run_insert_assemble(h))) return rc;
             if (h->last.host && h->last.n_keep) CK(cudaMemcpyAsync(h->last.user_keep, h->last.d_keep, h->last.n_keep, cudaMemcpyDeviceToHost, h->stream));
@@ -1332,6 +1367,48 @@ int erasor_process_nodes(erasor_handle_t h, const double* poses7, const float* q
 int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind) {
     return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, frame_keep, keep_out, ptr_kind, true);
+}
+
+namespace {
+int process_nodes_sweep_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                             double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind, bool async) {
+    static_assert(sizeof(erasor_srt_variant_t) == sizeof(SrtVariant) && offsetof(erasor_srt_variant_t, minimum_num_pts) == offsetof(SrtVariant, minimum_num_pts),
+                  "erasor_srt_variant_t and SrtVariant share one layout");
+    if (!h) return ERASOR_E_INVALID;
+    if (n_variants < 1 || n_variants > kMaxSweepVariants) { h->err = "n_variants must be in [1, 32]"; return ERASOR_E_INVALID; }
+    if (!variants || !variant_keep) { h->err = "null variants or variant_keep"; return ERASOR_E_INVALID; }
+    if (!h->map) { h->err = "erasor_process_nodes_sweep: no map attached (erasor_attach_map)"; return ERASOR_E_INVALID; }
+    if (h->node_inserts) { h->err = "a sweep has no node inserts: erasor_set_node_inserts(h, 0) first"; return ERASOR_E_INVALID; }
+    if (h->pending) { h->err = "erasor_process_nodes_sweep while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
+    return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, nullptr, nullptr, ptr_kind, async,
+                              reinterpret_cast<const SrtVariant*>(variants), n_variants, variant_keep);
+}
+}  // namespace
+
+int erasor_process_nodes_sweep(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                               double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind) {
+    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants, variant_keep, ptr_kind, false);
+}
+int erasor_process_nodes_sweep_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                     double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind) {
+    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants, variant_keep, ptr_kind, true);
+}
+
+int erasor_get_sweep_stats(erasor_handle_t h, uint32_t* n_flagged_bins, uint32_t* n_rejected_points) {
+    if (!h) return ERASOR_E_INVALID;
+    if (h->sweep_V <= 0 || h->desc_mode != 2) { h->err = "no erasor_process_nodes_sweep call has run"; return ERASOR_E_STATE; }
+    int rc;
+    if ((rc = erasor_wait(h))) return rc;
+    const size_t F = (size_t)h->stat_F, V = (size_t)h->sweep_V;
+    std::vector<uint32_t> t((size_t)kMaxSweepVariants * F);
+    for (int k = 0; k < 2; ++k) {
+        uint32_t* out = k == 0 ? n_flagged_bins : n_rejected_points;
+        if (!out) continue;
+        CK(cudaMemcpy(t.data(), (k == 0 ? h->d_sweep_flag : h->d_sweep_rej).p(), sizeof(uint32_t) * t.size(), cudaMemcpyDeviceToHost));
+        for (size_t v = 0; v < V; ++v)
+            for (size_t f = 0; f < F; ++f) out[v * F + f] = t[f * kMaxSweepVariants + v];
+    }
+    return ERASOR_OK;
 }
 
 // voxelize_preserving_labels of n_clouds clouds in one submission (voxelize_batch.cu): the checks that need only the host arrays

@@ -808,16 +808,37 @@ k2_scatter_win(const ChunkDesc* __restrict__ chunks, uint32_t chunk_base, const 
 //   destination = (points of earlier flagged bins of the frame) + (points of the bin in earlier chunks of the frame) + earlier warps.
 // The first chunk of each frame is its LEADER: it also publishes n_flagged[frame] and the flagged-bin records + size
 // buckets R-GPF consumes (what k3_srt does in cloud mode).
-template <int W, bool NODE>
-__global__ void __launch_bounds__(W * 32, 4)
-k2_srt_scatter(SrtParams P, int F, const ChunkDesc* __restrict__ chunks, const uint32_t* __restrict__ chunk_range /*[2][F+1]*/,
-               const uint16_t* __restrict__ bin_ids, const float4* __restrict__ pts, const NodePose* __restrict__ poses,
-               const uint32_t* __restrict__ ch_cnt /*raw per-chunk counts*/, const uint32_t* __restrict__ zmin, const uint32_t* __restrict__ zmax,
-               const uint32_t* __restrict__ cnt /*[2][F][B+1]*/, const uint32_t* __restrict__ frame_off /*[2][F+1]*/,
-               uint32_t* __restrict__ n_flagged /*[F]*/, FlagRec* __restrict__ recs, uint32_t* __restrict__ n_recs, uint32_t rec_capacity,
-               uint32_t* __restrict__ queue, uint32_t* __restrict__ bucket_list,
-               float4* __restrict__ out_pts, uint32_t* __restrict__ out_src, uint32_t SW,
-               const uint32_t* __restrict__ list_idx, const uint32_t* __restrict__ list_cnt, int k1_warps) {
+// Scan Ratio Test sweep: the variants that flag a bin (bit v for sweep.v[v]).  The FP64 work of srt_is_flagged once, then one
+// comparison per variant; the same decisions as srt_is_flagged with each variant's three fields in P's place.
+__device__ __forceinline__ uint32_t srt_variant_mask(const SrtSweep& S, int version, uint32_t mc, uint32_t qc, uint32_t zmx_m, uint32_t zmn_m,
+                                                     uint32_t zmx_q, uint32_t zmn_q) {
+    if (mc == 0u || qc == 0u) return 0u;
+    const double map_max = (double)ordered_to_float(zmx_m);
+    const double map_dh  = map_max - (double)ordered_to_float(zmn_m);
+    const double curr_dh = (double)ordered_to_float(zmx_q) - (double)ordered_to_float(zmn_q);
+    const double ratio   = std_min_d(map_dh / curr_dh, curr_dh / map_dh);
+    if (!(map_dh >= curr_dh)) return 0u;
+    uint32_t m = 0u;
+    for (int v = 0; v < S.n; ++v) {
+        const SrtVariant& x = S.v[v];
+        if (x.minimum_num_pts < 0 || qc < (uint32_t)x.minimum_num_pts || !(ratio < x.scan_ratio_threshold)) continue;   // App. B-9: < 0 flags nothing
+        if ((version == 3) ? (map_dh > 0.5) : (map_max > x.th_bin_max_h)) m |= 1u << v;
+    }
+    return m;
+}
+
+// The body of k2_srt_scatter (SWEEP == false) and of its sweep form k2_srt_sweep_scatter (SWEEP == true: a bin gets a slot when
+// any variant flags it, and its record carries the variants' mask in FlagRec::cursor).
+template <int W, bool NODE, bool SWEEP>
+__device__ __forceinline__ void
+k2_srt_scatter_body(const SrtParams& P, int F, const ChunkDesc* __restrict__ chunks, const uint32_t* __restrict__ chunk_range /*[2][F+1]*/,
+                    const uint16_t* __restrict__ bin_ids, const float4* __restrict__ pts, const NodePose* __restrict__ poses,
+                    const uint32_t* __restrict__ ch_cnt /*raw per-chunk counts*/, const uint32_t* __restrict__ zmin, const uint32_t* __restrict__ zmax,
+                    const uint32_t* __restrict__ cnt /*[2][F][B+1]*/, const uint32_t* __restrict__ frame_off /*[2][F+1]*/,
+                    uint32_t* __restrict__ n_flagged /*[F]*/, FlagRec* __restrict__ recs, uint32_t* __restrict__ n_recs, uint32_t rec_capacity,
+                    uint32_t* __restrict__ queue, uint32_t* __restrict__ bucket_list,
+                    float4* __restrict__ out_pts, uint32_t* __restrict__ out_src, uint32_t SW,
+                    const uint32_t* __restrict__ list_idx, const uint32_t* __restrict__ list_cnt, int k1_warps, const SrtSweep* sweep) {
     extern __shared__ uint32_t s_tab[];   // [W][ns] rows | [SW] bases | u16 slot of every bin [B+1]
     __shared__ float    s_T[12];
     __shared__ uint32_t s_part[34];
@@ -838,13 +859,29 @@ k2_srt_scatter(SrtParams P, int F, const ChunkDesc* __restrict__ chunks, const u
     const uint32_t* mnq = zmin + ((size_t)1 * F + f) * B; const uint32_t* mxq = zmax + ((size_t)1 * F + f) * B;
 
     // ---- Scan Ratio Test: flagged bit per bin (coalesced over the tables) ----
-    for (int b = tid; b <= B; b += NT) {
-        bool fl = false;
-        if (b < B) {
-            const uint32_t mc = cm[b], qc = cq[b];
-            if (mc != 0u && qc != 0u) fl = srt_is_flagged(P, mc, qc, mxm[b], mnm[b], mxq[b], mnq[b]);
+    if constexpr (SWEEP) {
+        // a bin takes a slot when any variant flags it; the leader counts the flagged bins of every variant
+        __shared__ uint32_t s_vcnt[kMaxSweepVariants];
+        if (tid < kMaxSweepVariants) s_vcnt[tid] = 0u;
+        __syncthreads();
+        for (int b = tid; b <= B; b += NT) {
+            uint32_t m = 0u;
+            if (b < B) m = srt_variant_mask(*sweep, P.version, cm[b], cq[b], mxm[b], mnm[b], mxq[b], mnq[b]);
+            s_slot[b] = m ? (uint16_t)0u : (uint16_t)0xFFFFu;
+            if (leader)
+                for (uint32_t r = m; r; r &= r - 1u) atomicAdd(&s_vcnt[__ffs(r) - 1], 1u);
         }
-        s_slot[b] = fl ? (uint16_t)0u : (uint16_t)0xFFFFu;
+        __syncthreads();
+        if (leader && tid < sweep->n) sweep->n_flagged[(size_t)f * kMaxSweepVariants + tid] = s_vcnt[tid];
+    } else {
+        for (int b = tid; b <= B; b += NT) {
+            bool fl = false;
+            if (b < B) {
+                const uint32_t mc = cm[b], qc = cq[b];
+                if (mc != 0u && qc != 0u) fl = srt_is_flagged(P, mc, qc, mxm[b], mnm[b], mxq[b], mnq[b]);
+            }
+            s_slot[b] = fl ? (uint16_t)0u : (uint16_t)0xFFFFu;
+        }
     }
     if (NODE && tid < 12) s_T[tid] = poses[f].T[tid];
     __syncthreads();
@@ -931,6 +968,7 @@ k2_srt_scatter(SrtParams P, int F, const ChunkDesc* __restrict__ chunks, const u
                     rc.frame = (uint32_t)f; rc.bin = b; rc.slot = slot; rc.n_points = sz;
                     rc.src_begin = fbase + win_carry + s_base[j];
                     rc.n_seeds = 0; rc.n_empty_fits = 0; rc.n_ground_final = 0; rc.lpr_height = 0.0; rc.cursor = 0u; rc.n_rejected = 0u;
+                    if constexpr (SWEEP) rc.cursor = srt_variant_mask(*sweep, P.version, sz, cq[b], mxm[b], mnm[b], mxq[b], mnq[b]);
                     if (sz != 0u) {
                         const int bk = rgpf_bucket_of(sz);
                         bucket_list[(size_t)bk * rec_capacity + atomicAdd(&queue[bk], 1u)] = ri;
@@ -964,6 +1002,25 @@ k2_srt_scatter(SrtParams P, int F, const ChunkDesc* __restrict__ chunks, const u
     }
 }
 
+#define K2_SRT_PARAMS                                                                                                                       \
+    SrtParams P, int F, const ChunkDesc* __restrict__ chunks, const uint32_t* __restrict__ chunk_range,                                     \
+    const uint16_t* __restrict__ bin_ids, const float4* __restrict__ pts, const NodePose* __restrict__ poses,                               \
+    const uint32_t* __restrict__ ch_cnt, const uint32_t* __restrict__ zmin, const uint32_t* __restrict__ zmax,                              \
+    const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ frame_off,                                                               \
+    uint32_t* __restrict__ n_flagged, FlagRec* __restrict__ recs, uint32_t* __restrict__ n_recs, uint32_t rec_capacity,                     \
+    uint32_t* __restrict__ queue, uint32_t* __restrict__ bucket_list, float4* __restrict__ out_pts, uint32_t* __restrict__ out_src,         \
+    uint32_t SW, const uint32_t* __restrict__ list_idx, const uint32_t* __restrict__ list_cnt, int k1_warps
+#define K2_SRT_ARGS P, F, chunks, chunk_range, bin_ids, pts, poses, ch_cnt, zmin, zmax, cnt, frame_off, n_flagged, recs, n_recs, rec_capacity, \
+                    queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps
+
+template <int W, bool NODE>
+__global__ void __launch_bounds__(W * 32, 4)
+k2_srt_scatter(K2_SRT_PARAMS) { k2_srt_scatter_body<W, NODE, false>(K2_SRT_ARGS, nullptr); }
+
+template <int W, bool NODE>
+__global__ void __launch_bounds__(W * 32, 4)
+k2_srt_sweep_scatter(K2_SRT_PARAMS, const __grid_constant__ SrtSweep sweep) { k2_srt_scatter_body<W, NODE, true>(K2_SRT_ARGS, &sweep); }
+
 static void k2_smem_plan(int B, bool with_complement, uint32_t& SW, size_t& smem) {
     constexpr int W = 8;
     const size_t fixed  = ((sizeof(uint16_t) * ((size_t)B + 2)) + 15) & ~(size_t)15;
@@ -981,14 +1038,19 @@ cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const Chun
                           const uint16_t* bin_ids, const float4* pts, const NodePose* poses, const uint32_t* ch_cnt, const uint32_t* zmin,
                           const uint32_t* zmax, const uint32_t* cnt, const uint32_t* frame_off, uint32_t* n_flagged, FlagRec* recs, uint32_t* n_recs,
                           uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list, float4* out_pts, uint32_t* out_src,
-                          const uint32_t* list_idx, const uint32_t* list_cnt) {
+                          const uint32_t* list_idx, const uint32_t* list_cnt, const SrtSweep* sweep) {
     if (n_chunks_map == 0) return cudaSuccess;
     constexpr int W = 8;
     const int k1_warps = k1_big_tables(P.R, P.B) ? 32 : 8;       // the split K1 compacted the chunk's VoI points in
     uint32_t SW; size_t smem;
     k2_smem_plan(P.B, false, SW, smem);
     cudaError_t e;
-    if (poses) {
+    if (sweep) {                                                  // node mode only
+        auto kern = k2_srt_sweep_scatter<W, true>;
+        if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
+        kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, bin_ids, pts, poses, ch_cnt, zmin, zmax, cnt, frame_off, n_flagged, recs, n_recs,
+                                                 rec_capacity, queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps, *sweep);
+    } else if (poses) {
         auto kern = k2_srt_scatter<W, true>;
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
         kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, bin_ids, pts, poses, ch_cnt, zmin, zmax, cnt, frame_off, n_flagged, recs, n_recs,
@@ -1516,13 +1578,14 @@ struct K4Shared {
 };
 
 // One flagged bin, handled by one group.  X/Y/Z/ORD/FLG live in shared memory or in the bin's slice of the global scratch.
-template <int G, bool kShared>
+// SWEEP: the bin's rejected points are also folded into the mask of every variant in rc.cursor (sweep: K4Sweep).
+template <int G, bool kShared, bool SWEEP>
 __device__ __forceinline__ void k4_process_bin(const GpfParams& P, FlagRec& rc, unsigned char* base, float* prd, uint32_t* cnt_scratch, K4Shared& sh,
                                                const float4* __restrict__ sorted_pts, uint32_t* __restrict__ sorted_src,
                                                const float4* __restrict__ in_pts, const uint32_t* __restrict__ frame_off,
                                                float4* __restrict__ part_pts, uint8_t* __restrict__ keep_mask,
                                                uint8_t* __restrict__ ground_mask, uint32_t* __restrict__ frame_rejected,
-                                               unsigned long long* __restrict__ fence, const K4Fold& fold) {
+                                               unsigned long long* __restrict__ fence, const K4Fold& fold, const K4Sweep* sweep) {
     const int tid = group_tid<G>(), lane = tid & 31, warp = tid >> 5;
     const uint32_t n = rc.n_points, src_begin = rc.src_begin;
     const uint32_t fbase = frame_off[rc.frame];
@@ -1755,10 +1818,12 @@ __device__ __forceinline__ void k4_process_bin(const GpfParams& P, FlagRec& rc, 
         rc.n_ground_final = m; rc.n_empty_fits = n_empty; rc.n_rejected = (P.iters > 0) ? n - m : 0u;
         if (n_empty) atomicAdd(&fence[1], (unsigned long long)n_empty);
         if (frame_rejected) atomicAdd(&frame_rejected[rc.frame], n - m);
+        if constexpr (SWEEP)
+            for (uint32_t r = rc.cursor; r; r &= r - 1u) atomicAdd(&sweep->rejected[(size_t)rc.frame * kMaxSweepVariants + (__ffs(r) - 1)], n - m);
     }
 
     // ---- outputs ----
-    if (keep_mask || ground_mask || fold.keep) {
+    if (keep_mask || ground_mask || fold.keep || SWEEP) {
         for (uint32_t i0 = tid; i0 < n; i0 += 4u * G) {
             uint32_t s[4];
 #pragma unroll
@@ -1777,6 +1842,11 @@ __device__ __forceinline__ void k4_process_bin(const GpfParams& P, FlagRec& rc, 
                         // Only zeros are ever written, so concurrent bins / frames / handles need no atomics.
                         const uint32_t g = fold.index ? fold.index[fbase + s[u]] : s[u];
                         if (g < fold.n) fold.keep[g] = 0;
+                    }
+                    if constexpr (SWEEP) {
+                        // the sweep's fold: one plain zero store per variant that flags the bin (node mode: the source index is global)
+                        if (!FLG[i] && s[u] < sweep->n)
+                            for (uint32_t r = rc.cursor; r; r &= r - 1u) sweep->keep[(size_t)(__ffs(r) - 1) * sweep->n + s[u]] = 0;
                     }
                 }
             }
@@ -1798,8 +1868,62 @@ __device__ __forceinline__ void k4_process_bin(const GpfParams& P, FlagRec& rc, 
 #undef K4_TICK
 }
 
-// One launch per size class.  Groups pull records of the class from the bucketed queue (largest bins first) through
-// an atomic cursor until the class is drained.
+// The queue loop of k4_rgpf and k4_rgpf_sweep: groups pull records of the class from the bucketed queue (largest bins first)
+// through an atomic cursor until the class is drained.  One text for both kernels; the sweep form differs only in what
+// k4_process_bin folds.
+#define K4_RGPF_LOOP(SWEEP, SWEEP_PTR)                                                                                                       \
+    extern __shared__ __align__(16) unsigned char smem_raw[];                                                                               \
+    constexpr int NG = THREADS / G;                                                                                                         \
+    constexpr int HT = (G == 32) ? 32 : (G == 128 ? 96 : 128);                                                                              \
+    constexpr int NCNT = (G >= 128) ? 8 * G : 1;         /* radix counters: class C, and class B's bins beyond 2048 points */               \
+    __shared__ K4Shared sh[NG];                                                                                                             \
+    __shared__ float    s_prd[NG][2 * 9 * (HT + 1)];                                                                                        \
+    __shared__ uint32_t s_cnt[NG][NCNT];                                                                                                    \
+    __shared__ uint32_t s_fetch;                                                                                                            \
+    const int grp = (G == 32) ? (threadIdx.x >> 5) : 0;                                                                                     \
+    uint32_t bcnt[4] = {0u, 0u, 0u, 0u}, total = 0u;     /* a class spans at most four buckets */                                           \
+    _Pragma("unroll")                                                                                                                       \
+    for (int k = 0; k < 4; ++k) {                                                                                                           \
+        if (bk0 + k < bk1) { bcnt[k] = min(queue[bk0 + k], rec_capacity); total += bcnt[k]; }                                              \
+    }                                                                                                                                       \
+    for (;;) {                                                                                                                              \
+        uint32_t i;                                                                                                                         \
+        if (G == 32) {                                                                                                                      \
+            i = 0u;                                                                                                                         \
+            if ((threadIdx.x & 31) == 0) i = atomicAdd(&queue[kQueueCursor + cls], 1u);                                                     \
+            i = __shfl_sync(FULL_MASK, i, 0);                                                                                               \
+        } else {                                                                                                                            \
+            if (threadIdx.x == 0) s_fetch = atomicAdd(&queue[kQueueCursor + cls], 1u);                                                      \
+            __syncthreads();                                                                                                                \
+            i = s_fetch;                                                                                                                    \
+            __syncthreads();                                                                                                                \
+        }                                                                                                                                   \
+        if (i >= total) break;                                                                                                              \
+        int bk = bk0;                                                                                                                       \
+        _Pragma("unroll")                                                                                                                   \
+        for (int k = 0; k < 3; ++k) {                                                                                                       \
+            if (bk == bk0 + k && i >= bcnt[k]) { i -= bcnt[k]; ++bk; }                                                                      \
+        }                                                                                                                                   \
+        const uint32_t w = bucket_list[(size_t)bk * rec_capacity + i];                                                                      \
+        FlagRec& rc = recs[w];                                                                                                              \
+        const uint32_t n = rc.n_points;                                                                                                     \
+        if constexpr (G <= 256) {                                                                                                           \
+            /* classes A and B: the launch sizes the slices for the class maximum (kClassAMax / kClassBMax), so the bin always fits */      \
+            k4_process_bin<G, true, SWEEP>(P, rc, smem_raw + (size_t)grp * slice_bytes, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts,        \
+                                           sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,    \
+                                           SWEEP_PTR);                                                                                      \
+        } else if (n <= smem_cap_points) {                                                                                                  \
+            k4_process_bin<G, true, SWEEP>(P, rc, smem_raw + (size_t)grp * slice_bytes, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts,        \
+                                           sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,    \
+                                           SWEEP_PTR);                                                                                      \
+        } else {                                                                                                                            \
+            k4_process_bin<G, false, SWEEP>(P, rc, gscratch + (size_t)rc.src_begin * 24u, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts,      \
+                                            sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,   \
+                                            SWEEP_PTR);                                                                                     \
+        }                                                                                                                                   \
+    }
+
+// One launch per size class.
 // G == 32: every warp of the CTA is a group with its own shared-memory slice (slice_bytes).
 // G == THREADS: the CTA is the group; bins above smem_cap_points work in their slice of the global scratch.
 template <int THREADS, int G>
@@ -1811,67 +1935,42 @@ k4_rgpf(GpfParams P, FlagRec* __restrict__ recs, uint32_t* __restrict__ queue, c
         uint8_t* __restrict__ ground_mask /*nullable*/, uint32_t* __restrict__ frame_rejected /*[F] nullable*/,
         unsigned char* __restrict__ gscratch, uint32_t smem_cap_points, uint32_t slice_bytes,
         unsigned long long* __restrict__ fence, K4Fold fold) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    constexpr int NG = THREADS / G;
-    constexpr int HT = (G == 32) ? 32 : (G == 128 ? 96 : 128);
-    constexpr int NCNT = (G >= 128) ? 8 * G : 1;         // radix counters: class C, and class B's bins beyond 2048 points
-    __shared__ K4Shared sh[NG];
-    __shared__ float    s_prd[NG][2 * 9 * (HT + 1)];
-    __shared__ uint32_t s_cnt[NG][NCNT];
-    __shared__ uint32_t s_fetch;
-    const int grp = (G == 32) ? (threadIdx.x >> 5) : 0;
-    uint32_t bcnt[4] = {0u, 0u, 0u, 0u}, total = 0u;     // a class spans at most four buckets
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        if (bk0 + k < bk1) { bcnt[k] = min(queue[bk0 + k], rec_capacity); total += bcnt[k]; }
-    }
-    for (;;) {
-        uint32_t i;
-        if (G == 32) {
-            i = 0u;
-            if ((threadIdx.x & 31) == 0) i = atomicAdd(&queue[kQueueCursor + cls], 1u);
-            i = __shfl_sync(FULL_MASK, i, 0);
-        } else {
-            if (threadIdx.x == 0) s_fetch = atomicAdd(&queue[kQueueCursor + cls], 1u);
-            __syncthreads();
-            i = s_fetch;
-            __syncthreads();
-        }
-        if (i >= total) break;
-        int bk = bk0;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            if (bk == bk0 + k && i >= bcnt[k]) { i -= bcnt[k]; ++bk; }
-        }
-        const uint32_t w = bucket_list[(size_t)bk * rec_capacity + i];
-        FlagRec& rc = recs[w];
-        const uint32_t n = rc.n_points;
-        if constexpr (G <= 256) {
-            // classes A and B: the launch sizes the slices for the class maximum (kClassAMax / kClassBMax), so the bin always fits
-            k4_process_bin<G, true>(P, rc, smem_raw + (size_t)grp * slice_bytes, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts, sorted_src, in_pts,
-                                    frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold);
-        } else if (n <= smem_cap_points) {
-            k4_process_bin<G, true>(P, rc, smem_raw + (size_t)grp * slice_bytes, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts, sorted_src, in_pts,
-                                    frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold);
-        } else {
-            k4_process_bin<G, false>(P, rc, gscratch + (size_t)rc.src_begin * 24u, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts, sorted_src, in_pts,
-                                     frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold);
-        }
-    }
+    K4_RGPF_LOOP(false, nullptr)
 }
+
+// k4_rgpf of a Scan Ratio Test sweep: the records carry the variants' mask, the epilogue folds into the variant masks
+template <int THREADS, int G>
+__global__ void __launch_bounds__(THREADS, (THREADS == 256) ? 3 : (THREADS == 128 ? 6 : 1))
+k4_rgpf_sweep(GpfParams P, FlagRec* __restrict__ recs, uint32_t* __restrict__ queue, const uint32_t* __restrict__ bucket_list,
+              uint32_t rec_capacity, int bk0, int bk1, int cls, const float4* __restrict__ sorted_pts, uint32_t* __restrict__ sorted_src,
+              const float4* __restrict__ in_pts, const uint32_t* __restrict__ frame_off, float4* __restrict__ part_pts,
+              uint8_t* __restrict__ keep_mask, uint8_t* __restrict__ ground_mask, uint32_t* __restrict__ frame_rejected,
+              unsigned char* __restrict__ gscratch, uint32_t smem_cap_points, uint32_t slice_bytes,
+              unsigned long long* __restrict__ fence, K4Fold fold, K4Sweep sweep) {
+    K4_RGPF_LOOP(true, &sweep)
+}
+#undef K4_RGPF_LOOP
 
 template <int THREADS, int G>
 static cudaError_t launch_k4_class(cudaStream_t st, const GpfParams& P, FlagRec* recs, uint32_t* queue, const uint32_t* bucket_list,
                                    uint32_t rec_capacity, int bk0, int bk1, int cls, uint32_t smem_bytes, const float4* sorted_pts,
                                    uint32_t* sorted_src, const float4* in_pts, const uint32_t* frame_off, float4* part_pts,
                                    uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected, unsigned char* gscratch, int grid,
-                                   unsigned long long* fence, const K4Fold& fold) {
+                                   unsigned long long* fence, const K4Fold& fold, const K4Sweep* sweep) {
     // per bin: 12 n (xyz) + 4 n (order) + n (flags) = 17 n for warp groups, + 4 n (second half of the order / exchange area) = 21 n
     constexpr int NG = THREADS / G;
     constexpr uint32_t per_pt = (G == 32) ? 17u : 21u;
     const uint32_t slice = (smem_bytes / NG) & ~15u;
     const uint32_t cap = (slice - 32) / per_pt;
     if ((G == 32 && cap < kClassAMax) || (G == 128 && cap < kClassBMax)) return cudaErrorInvalidConfiguration;   // A / B have no scratch path
+    if (sweep) {
+        auto kern = k4_rgpf_sweep<THREADS, G>;
+        cudaError_t e = ensure_dyn_smem(kern, smem_bytes);
+        if (e != cudaSuccess) return e;
+        kern<<<grid, THREADS, smem_bytes, st>>>(P, recs, queue, bucket_list, rec_capacity, bk0, bk1, cls, sorted_pts, sorted_src, in_pts, frame_off,
+                                                part_pts, keep_mask, ground_mask, frame_rejected, gscratch, cap, slice, fence, fold, *sweep);
+        return cudaGetLastError();
+    }
     auto kern = k4_rgpf<THREADS, G>;
     cudaError_t e = ensure_dyn_smem(kern, smem_bytes);
     if (e != cudaSuccess) return e;
@@ -1885,7 +1984,7 @@ int k4_num_launches(bool with_class_c) { return with_class_c ? 3 : 2; }
 cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, const GpfParams& P, FlagRec* recs, uint32_t* queue,
                       const uint32_t* bucket_list, uint32_t rec_capacity, const float4* sorted_pts, uint32_t* sorted_src, const float4* in_pts,
                       const uint32_t* frame_off, float4* part_pts, uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected,
-                      unsigned char* gscratch, int sm_count, unsigned long long* fence, const K4Fold& fold, int classes) {
+                      unsigned char* gscratch, int sm_count, unsigned long long* fence, const K4Fold& fold, int classes, const K4Sweep* sweep) {
     // The three size classes touch disjoint bins, so they run concurrently on three streams (the caller forks / joins).
     // Shared memory: A  8 x 8.75 KB slices + 18.7 KB products ~ 90 KB per CTA (8 bins);  B  52.6 KB + 11 KB products / radix counters ~ 64 KB
     // per CTA (1 bin, 4 warps).  Registers (80 per thread): A 20 K per 8 bins, B 10 K per bin.
@@ -1899,19 +1998,19 @@ cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, con
     // runs it afterwards (classes == 4) if one turns up.
     if (classes & 4) {
         e = launch_k4_class<1024, 1024>(st_c, P, recs, queue, bucket_list, rec_capacity, kBucketC0, kBucketB0, 2, 180 * 1024, sorted_pts, sorted_src,
-                                        in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count, fence, fold);
+                                        in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count, fence, fold, sweep);
         if (e != cudaSuccess) return e;
     }
     if (!(classes & 3)) return cudaSuccess;
     // class B: 512 < n <= 2560, one 128-thread CTA per bin
     e = launch_k4_class<128, 128>(st_b, P, recs, queue, bucket_list, rec_capacity, kBucketB0, kBucketA0, 1, 21 * kClassBMax + 64, sorted_pts,
-                                  sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 3, fence, fold);
+                                  sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 3, fence, fold, sweep);
     if (e != cudaSuccess) return e;
     // class A: n <= 512, one warp per bin, 8 warps per CTA
     // (two CTAs per SM fit by shared memory: with tens of thousands of small flagged bins per step -- 40 x 360 bins, 2 M-point map --
     //  R-GPF is bound by resident chains per SM, and CTAs that find the queue empty exit at once)
     return launch_k4_class<256, 32>(st, P, recs, queue, bucket_list, rec_capacity, kBucketA0, kNumBuckets, 0, 8 * (17 * kClassAMax + 48), sorted_pts,
-                                    sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 2, fence, fold);
+                                    sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 2, fence, fold, sweep);
 }
 
 // ============================================================================================

@@ -42,7 +42,7 @@ cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const Chun
                           const uint16_t* bin_ids, const float4* pts, const NodePose* poses, const uint32_t* ch_cnt, const uint32_t* zmin,
                           const uint32_t* zmax, const uint32_t* cnt, const uint32_t* frame_off, uint32_t* n_flagged, FlagRec* recs, uint32_t* n_recs,
                           uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list, float4* out_pts, uint32_t* out_src,
-                          const uint32_t* list_idx, const uint32_t* list_cnt);
+                          const uint32_t* list_idx, const uint32_t* list_cnt, const SrtSweep* sweep = nullptr /*node mode: a Scan Ratio Test sweep*/);
 
 // flag_slot == null: every bin of dst_start's cloud that has an offset is scattered (cloud mode); otherwise the flagged bins only
 cudaError_t launch_k2(cudaStream_t st, const ChunkDesc* chunks, uint32_t chunk_base, uint32_t n_chunks,
@@ -62,7 +62,8 @@ int k4_num_launches(bool with_class_c);
 cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, const GpfParams& P, FlagRec* recs, uint32_t* queue,
                       const uint32_t* bucket_list, uint32_t rec_capacity, const float4* sorted_pts, uint32_t* sorted_src, const float4* in_pts, const uint32_t* frame_off,
                       float4* part_pts, uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected, unsigned char* gscratch,
-                      int sm_count, unsigned long long* fence, const K4Fold& fold, int classes /*bit 0|1: A and B, bit 2: C*/);
+                      int sm_count, unsigned long long* fence, const K4Fold& fold, int classes /*bit 0|1: A and B, bit 2: C*/,
+                      const K4Sweep* sweep = nullptr /*a sweep's per-variant fold (node mode, records from k2_srt_sweep_scatter)*/);
 
 // every record of the batch (F frames; cnt / dst_start [2][F][...], qry_off: the query half of frame_off); vox_cnt / vox_start
 // per record

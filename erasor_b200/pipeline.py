@@ -89,6 +89,69 @@ def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep
     return {"static_map": static_map, "nodes": len(nodes), "processed_scans": len(sel), "keep": keep}
 
 
+def sweep_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep, variants, gt: Optional[np.ndarray] = None, batch: int = 20,
+                            save_voxel_size: Optional[float] = None) -> list:
+    """run_frame_independent under every Scan Ratio Test setting of `variants` (1..32 dicts of scan_ratio_threshold, th_bin_max_h,
+    minimum_num_pts; a missing field comes from ep) in one node-mode pass (erasor_process_nodes_sweep, DESIGN.md section 8.5): the
+    binning and R-GPF run once per batch, each setting's verdicts go to its own mask.  One row per setting: its three fields, PR /
+    RR / F1 of its saved map against gt (default: the initial map, as run_sequence scores) at voxelsize 0.2, the kept map points,
+    the saved map's size and the flagged-bin / rejected-point totals.  Row v equals run_frame_independent(nodes, initial_map, up,
+    ep.replace(**variants[v])) scored with capi.Evaluator.  Needs a CUDA device."""
+    import torch
+
+    from . import capi
+    if up.is_large_scale:
+        raise ValueError("node mode has no large-scale windowing: use run_offline")
+    variants = [dict(v) for v in variants]
+    if not 1 <= len(variants) <= capi.MAX_SWEEP_VARIANTS:
+        raise ValueError(f"a sweep takes 1 to {capi.MAX_SWEEP_VARIANTS} settings")
+    for v in variants:
+        if set(v) - set(capi.SRT_SWEEP_FIELDS):
+            raise ValueError(f"a sweep varies only {capi.SRT_SWEEP_FIELDS}, not {sorted(set(v) - set(capi.SRT_SWEEP_FIELDS))}")
+    nodes = list(nodes)
+    sel = processed_nodes(nodes, up.removal_interval)
+    initial_map = np.ascontiguousarray(initial_map, dtype=np.float32)
+    m = capi.Map(initial_map)
+    h = capi.Handle(ep.replace(version=up.version))       # /erasor/version as the updater reads it (OfflineMapUpdater.cpp:81)
+    V, n = len(variants), m.size
+    leaf = up.map_voxel_size if save_voxel_size is None else save_voxel_size
+    rows = []
+    try:
+        h.attach_map(m)
+        keep = torch.empty(max(V * n, 1), dtype=torch.uint8, device=f"cuda:{h._device}")
+        h.reset_keep_mask(keep.data_ptr(), V * n)
+        flagged, rejected = np.zeros(V, dtype=np.int64), np.zeros(V, dtype=np.int64)
+        l2b = np.asarray(up.lidar2body, dtype=np.float64)
+        for b0 in range(0, len(sel), int(batch)):
+            chunk = sel[b0:b0 + int(batch)]
+            poses = np.stack([np.asarray(o, dtype=np.float64).reshape(7) for _, o, _ in chunk])
+            scans = [np.ascontiguousarray(c, dtype=np.float32).reshape(-1, 4) for _, _, c in chunk]
+            off = np.cumsum([0] + [len(s) for s in scans]).astype(np.uint64)
+            raw = np.concatenate(scans)
+            d, qo = h.voxelize_batch_ptr(raw.ctypes.data if len(raw) else 0, off, up.query_voxel_size, 0, l2b, capi.PTR_HOST)
+            h.process_nodes_sweep(poses, d, qo, variants, keep.data_ptr(), voi_max_range=up.max_range)
+            nf, nr = h.sweep_stats()
+            flagged += nf.sum(axis=1, dtype=np.int64)
+            rejected += nr.sum(axis=1, dtype=np.int64)
+        masks = keep[:V * n].reshape(V, n).cpu().numpy()
+        ref = initial_map if gt is None else gt
+        with capi.Evaluator() as ev:
+            for v in range(V):
+                d, oo = h.voxelize_batch_ptr(m.points_ptr, [0, n], leaf, keep.data_ptr() + v * n, None, capi.PTR_DEVICE)
+                static_map = np.empty((int(oo[-1]), 4), dtype=np.float32)
+                capi._memcpy_from_device(static_map, d)
+                q = ev.evaluate(ref, static_map, voxelsize=0.2)
+                arr, _ = h.sweep_variants([variants[v]])
+                rows.append(dict(scan_ratio_threshold=arr[0].scan_ratio_threshold, th_bin_max_h=arr[0].th_bin_max_h,
+                                 minimum_num_pts=arr[0].minimum_num_pts, PR=q["PR"], RR=q["RR"], F1=q["F1"],
+                                 kept=int(np.count_nonzero(masks[v])), saved=len(static_map),
+                                 flagged=int(flagged[v]), rejected=int(rejected[v])))
+    finally:
+        h.close()
+        m.close()
+    return rows
+
+
 def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, make_updater: Optional[Callable] = None,
                  map_leafsize: Optional[float] = None, out_dir: Optional[str] = None, frame_independent: bool = False,
                  inserts: bool = False, pcd_mode: str = "ascii") -> dict:

@@ -1,0 +1,98 @@
+"""Tune the Scan Ratio Test on new data in one node-mode pass: every setting of the Cartesian product of the listed values (at most
+32) runs through pipeline.sweep_frame_independent, which bins each node and fits R-GPF once and keeps one map mask per setting
+(DESIGN.md section 8.5).  Prints one row per setting (PR / RR / F1 against the GT, kept and saved points, flagged bins and rejected
+points) and marks the F1 maximum with '*'; --save-best writes that setting's saved map.
+
+    python -m erasor_b200.sweep <config.yaml> <file.bag | data_dir> [--scan-ratio 0.10,0.15,0.20,0.25,0.30] [--min-pts 6,10]
+                                [--th-bin-max-h 0.05,0.2] [--gt gt.pcd] [--save-best out.pcd] [--pcd-mode ascii] [--batch 20]
+
+A field left out keeps the yaml's value; --save-best reruns run_frame_independent for the chosen setting.  Inputs are read on
+the device: a ROS bag of erasor/node messages (the map is the yaml's initial_map_path, as static_map_nodes_main reads it), or
+<data_dir>/dense_global_map.pcd, <data_dir>/poses_lidar2body.csv and <data_dir>/pcds/%06d.pcd.  GT defaults to the initial map,
+as run_sequence scores.
+"""
+from __future__ import annotations
+
+import argparse
+import itertools
+import os
+import sys
+
+import numpy as np
+
+from . import capi, params, pipeline
+
+
+def _floats(s):
+    return [float(x) for x in s.split(",") if x.strip()]
+
+
+def _ints(s):
+    return [int(x) for x in s.split(",") if x.strip()]
+
+
+def variants_of(scan_ratio=None, min_pts=None, th_bin_max_h=None) -> list:
+    """The Cartesian product of the listed values, as sweep settings (a field with no list is left to the yaml)."""
+    axes = [(k, v) for k, v in (("scan_ratio_threshold", scan_ratio), ("minimum_num_pts", min_pts), ("th_bin_max_h", th_bin_max_h)) if v]
+    if not axes:
+        return [{}]
+    return [dict(zip([k for k, _ in axes], combo)) for combo in itertools.product(*[v for _, v in axes])]
+
+
+def best_row(rows) -> int:
+    """Index of the F1 maximum (the first one on ties)."""
+    return int(np.argmax([r["F1"] for r in rows]))
+
+
+def format_rows(rows) -> str:
+    best = best_row(rows)
+    head = f"{'':1} {'scan_ratio':>10} {'min_pts':>7} {'th_bin_max_h':>12} {'PR%':>8} {'RR%':>8} {'F1':>7} {'kept':>10} {'saved':>10} {'flagged':>9} {'rejected':>10}"
+    lines = [head]
+    for i, r in enumerate(rows):
+        lines.append(f"{'*' if i == best else ' '} {r['scan_ratio_threshold']:>10.4g} {r['minimum_num_pts']:>7d} {r['th_bin_max_h']:>12.4g} "
+                     f"{r['PR']:>8.3f} {r['RR']:>8.3f} {r['F1']:>7.4f} {r['kept']:>10d} {r['saved']:>10d} {r['flagged']:>9d} {r['rejected']:>10d}")
+    return "\n".join(lines) + "\n"
+
+
+def read_data_dir(codec, data_dir: str):
+    """(nodes, initial map) of the env layout: poses_lidar2body.csv rows idx,time,x,y,z,qx,qy,qz,qw and pcds/%06d.pcd in node order."""
+    rows = np.loadtxt(os.path.join(data_dir, "poses_lidar2body.csv"), delimiter=",", skiprows=1, dtype=np.float64, ndmin=2)
+    nodes = [(int(r[1]), r[2:9].copy(), codec.load(os.path.join(data_dir, "pcds", f"{i:06d}.pcd"))) for i, r in enumerate(rows)]
+    return nodes, codec.load(os.path.join(data_dir, "dense_global_map.pcd"))
+
+
+def main(argv=None) -> int:
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("config")
+    ap.add_argument("data", help="a .bag of erasor/node messages, or a data directory")
+    ap.add_argument("--scan-ratio", type=_floats)
+    ap.add_argument("--min-pts", type=_ints)
+    ap.add_argument("--th-bin-max-h", type=_floats)
+    ap.add_argument("--gt", help="GT cloud (default: the initial map)")
+    ap.add_argument("--save-best", help="write the F1 maximum's saved map here")
+    ap.add_argument("--pcd-mode", default="ascii", choices=sorted(capi.PCD_MODES))
+    ap.add_argument("--batch", type=int, default=20)
+    args = ap.parse_args(argv)
+    variants = variants_of(args.scan_ratio, args.min_pts, args.th_bin_max_h)
+    if len(variants) > capi.MAX_SWEEP_VARIANTS:
+        ap.error(f"{len(variants)} settings: a sweep takes at most {capi.MAX_SWEEP_VARIANTS}")
+    ep, up = params.load_yaml(args.config)
+    with capi.PcdCodec() as codec:
+        if args.data.endswith(".bag"):
+            nodes = pipeline.read_bag_nodes(args.data)
+            initial = codec.load(up.initial_map_path)
+        else:
+            nodes, initial = read_data_dir(codec, args.data)
+        gt = codec.load(args.gt) if args.gt else None
+    rows = pipeline.sweep_frame_independent(nodes, initial, up, ep, variants, gt=gt, batch=args.batch)
+    sys.stdout.write(format_rows(rows))
+    if args.save_best:
+        best = variants[best_row(rows)]
+        res = pipeline.run_frame_independent(nodes, initial, up, ep.replace(**best), batch=args.batch)
+        with capi.PcdCodec() as codec:
+            codec.write(args.save_best, res["static_map"], mode=args.pcd_mode)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

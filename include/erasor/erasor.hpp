@@ -163,6 +163,17 @@ public:
         keep.resize(erasor_map_size(map_));
         return keep;
     }
+    // Scan Ratio Test sweep (DESIGN.md section 8.5): the batch of process_nodes under every setting of `variants` (1..32) in one pass.
+    // d_variant_keep: DEVICE, variants.size() x n_map bytes; mask v accumulates setting v's verdicts (reset it with
+    // erasor_reset_keep_mask).  The map's own keep mask is left as it is.  Queries: host or device per ptr_kind, as erasor_process_nodes.
+    void process_nodes_sweep(const std::vector<std::array<double, 7>>& poses, const float* query_xyzi, const std::vector<uint64_t>& query_offsets,
+                             const std::vector<erasor_srt_variant_t>& variants, uint8_t* d_variant_keep, double voi_max_range = 0.0,
+                             int ptr_kind = ERASOR_PTR_HOST) {
+        if (!map_) throw std::logic_error("ERASOR: load_global_map first");
+        if (poses.empty() || poses.size() + 1 != query_offsets.size()) throw std::invalid_argument("ERASOR: one pose per query VoI");
+        check(erasor_process_nodes_sweep(h_, poses[0].data(), query_xyzi, query_offsets.data(), static_cast<int>(poses.size()), voi_max_range,
+                                         variants.data(), static_cast<int>(variants.size()), d_variant_keep, ptr_kind));
+    }
     // Node-mode inserts (DESIGN.md section 8.4): with enable, process_nodes / process_scans also append the query points each node's
     // static estimate puts back into the map to the map's store, and save_static_map voxelises them with the kept map.
     void set_node_inserts(bool enable) { check(erasor_set_node_inserts(h_, enable ? 1 : 0)); inserts_ = enable; }

@@ -211,6 +211,31 @@ int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const fl
 /* per-node counters of the last erasor_process_nodes: points inside the VoI (|map_voi_|), flagged bins, rejected points */
 int erasor_get_node_stats(erasor_handle_t h, uint32_t* n_voi_points, uint32_t* n_flagged_bins, uint32_t* n_rejected_points);
 
+/* ---- Scan Ratio Test sweep: one node-mode pass, one keep mask per setting (DESIGN.md section 8.5) ---- */
+/* The three per-sensor knobs of the Scan Ratio Test, one setting of a sweep (reserved: 0). */
+typedef struct {
+    double scan_ratio_threshold;
+    double th_bin_max_h;
+    int    minimum_num_pts;
+    int    reserved;
+} erasor_srt_variant_t;
+/* erasor_process_nodes (same map, voi_max_range, queries, ptr_kind, sub-batches, geometry, version, gf_* and cov_mode) run under
+ * n_variants settings of the Scan Ratio Test at once: K1's binning and R-GPF run once, over the union of the bins the settings
+ * flag, and each setting's verdicts go to its own mask.  The handle's own scan_ratio_threshold, th_bin_max_h and minimum_num_pts
+ * are not read.  variant_keep: DEVICE, n_variants x n_map bytes, mask v at [v * n_map, (v + 1) * n_map); it ACCUMULATES like
+ * erasor_process_frames_fold's global_keep (start with erasor_reset_keep_mask(h, variant_keep, n_variants * n_map)); handles
+ * may share one.  Mask v equals the map's keep mask after erasor_process_nodes with setting v on a fresh map.  The map's own
+ * keep mask is not written.  ERASOR_E_INVALID: n_variants outside [1, 32], a null variants or variant_keep, no attached map,
+ * node inserts on; ERASOR_E_STATE: a submission pending. */
+int erasor_process_nodes_sweep(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                               double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind);
+int erasor_process_nodes_sweep_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                     double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind);
+/* per (setting, node) counters of the last sweep, HOST arrays [n_variants][n_frames] (nullable): flagged bins and rejected points,
+ * as erasor_get_node_stats reports them for that setting.  After a sweep, erasor_get_node_stats gives n_voi_points as usual and
+ * the counts of the union of the settings' flagged bins.  ERASOR_E_STATE when the last node call was not a sweep. */
+int erasor_get_sweep_stats(erasor_handle_t h, uint32_t* n_flagged_bins, uint32_t* n_rejected_points);
+
 /* ---- node-mode inserts: the query points each node's static estimate puts back into the map (DESIGN.md section 8.4) ---- */
 /* Opt-in per handle (default off; off changes nothing).  With it on, erasor_process_nodes also builds, per node f, inserted_f:
  * bin by bin in r_pod2pc order, the bins whose selected points hold query points -- R-GPF bins: bin_curr then the R-GPF ground
