@@ -31,6 +31,7 @@ EXPORTS = [
     "erasor_map_create", "erasor_map_destroy", "erasor_map_size", "erasor_map_reset_keep", "erasor_map_get_keep", "erasor_map_keep_device",
     "erasor_map_points_device", "erasor_attach_map", "erasor_process_nodes", "erasor_process_nodes_async", "erasor_get_node_stats",
     "erasor_process_nodes_sweep", "erasor_process_nodes_sweep_async", "erasor_get_sweep_stats",
+    "erasor_process_nodes_sweep_ex", "erasor_process_nodes_sweep_ex_async",
     "erasor_voxelize_batch",
     "erasor_set_node_inserts", "erasor_get_node_inserts", "erasor_map_append_inserts", "erasor_map_inserts", "erasor_map_clear_inserts",
     "erasor_save_node_map",
@@ -65,7 +66,14 @@ class SrtVariantC(ctypes.Structure):
 
 
 SRT_SWEEP_FIELDS = ("scan_ratio_threshold", "th_bin_max_h", "minimum_num_pts")     # what a Scan Ratio Test sweep varies
+GF_SWEEP_FIELDS = ("gf_dist_thr", "gf_th_seeds_height", "gf_num_lpr", "num_lowest_pts", "gf_iter")   # R-GPF's, added by sweep_ex
 MAX_SWEEP_VARIANTS = 32
+
+
+class SweepSettingC(ctypes.Structure):
+    """erasor_sweep_setting_t"""
+    _fields_ = [(name, c_double) for name in ("scan_ratio_threshold", "th_bin_max_h", "gf_dist_thr", "gf_th_seeds_height")] + \
+               [(name, c_int) for name in ("minimum_num_pts", "num_lowest_pts", "gf_num_lpr", "gf_iter")]
 
 
 class PcdInfoC(ctypes.Structure):
@@ -192,6 +200,8 @@ def _load():
     L.erasor_process_nodes_sweep.argtypes = [c_void_p, POINTER(c_double), c_void_p, POINTER(c_uint64), c_int, c_double, POINTER(SrtVariantC), c_int,
                                              c_void_p, c_int]
     L.erasor_process_nodes_sweep_async.argtypes = L.erasor_process_nodes_sweep.argtypes
+    L.erasor_process_nodes_sweep_ex.argtypes = L.erasor_process_nodes_sweep.argtypes[:6] + [POINTER(SweepSettingC)] + L.erasor_process_nodes_sweep.argtypes[7:]
+    L.erasor_process_nodes_sweep_ex_async.argtypes = L.erasor_process_nodes_sweep_ex.argtypes
     L.erasor_get_sweep_stats.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32)]
     L.erasor_voxelize_batch.argtypes = [c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p, c_float, POINTER(c_double), c_int,
                                         POINTER(c_void_p), POINTER(c_uint64)]
@@ -553,7 +563,7 @@ class Handle(_Native):
                                               nr.ctypes.data_as(POINTER(c_uint32))))
         return nv, nf, nr
 
-    # -- Scan Ratio Test sweep (DESIGN.md section 8.5) ----------------------------------------------------------------------------
+    # -- sweeps of the Scan Ratio Test and ground-filter fields (DESIGN.md sections 8.5 and 8.6) -----------------------------------
     def sweep_variants(self, variants):
         """variants (dicts or objects with any of SRT_SWEEP_FIELDS; a missing field takes the handle's value) -> SrtVariantC array"""
         vs = list(variants)
@@ -565,17 +575,40 @@ class Handle(_Native):
             arr[i].minimum_num_pts = int(get("minimum_num_pts", self.params.minimum_num_pts))
         return arr, len(vs)
 
+    def sweep_settings(self, settings):
+        """settings (dicts or objects with any of SRT_SWEEP_FIELDS + GF_SWEEP_FIELDS; a missing field takes the handle's value)
+        -> SweepSettingC array"""
+        ss = list(settings)
+        arr = (SweepSettingC * max(len(ss), 1))()
+        for i, v in enumerate(ss):
+            get = v.get if isinstance(v, dict) else (lambda k, d, v=v: getattr(v, k, d))
+            for name, typ in SweepSettingC._fields_:
+                setattr(arr[i], name, (float if typ is c_double else int)(get(name, getattr(self.params, name))))
+        return arr, len(ss)
+
     def process_nodes_sweep(self, poses7, query_xyzi, query_offsets, variants, keep_ptr: int, voi_max_range: float = 0.0,
                             packed_xyz: bool = False, asynchronous: bool = False):
         """erasor_process_nodes_sweep: the node batch against the attached map under every Scan Ratio Test setting of `variants`
         (1..32), mask v folded into the device bytes [keep_ptr + v n_map, keep_ptr + (v + 1) n_map) (they accumulate: start with
         reset_keep_mask(keep_ptr, V n_map)).  query_xyzi: a host float32 [n,4] array (shipped as packed x y z with packed_xyz) or a
         device pointer (int; packed x y z with packed_xyz).  The map's own keep mask is left as it is."""
+        arr, V = self.sweep_variants(variants)
+        fn = self.L.erasor_process_nodes_sweep_async if asynchronous else self.L.erasor_process_nodes_sweep
+        self._sweep(fn, poses7, query_xyzi, query_offsets, arr, V, keep_ptr, voi_max_range, packed_xyz)
+
+    def process_nodes_sweep_ex(self, poses7, query_xyzi, query_offsets, settings, keep_ptr: int, voi_max_range: float = 0.0,
+                               packed_xyz: bool = False, asynchronous: bool = False):
+        """erasor_process_nodes_sweep_ex: process_nodes_sweep over settings that may also vary GF_SWEEP_FIELDS (DESIGN.md
+        section 8.6); arguments as process_nodes_sweep, settings as sweep_settings takes them."""
+        arr, V = self.sweep_settings(settings)
+        fn = self.L.erasor_process_nodes_sweep_ex_async if asynchronous else self.L.erasor_process_nodes_sweep_ex
+        self._sweep(fn, poses7, query_xyzi, query_offsets, arr, V, keep_ptr, voi_max_range, packed_xyz)
+
+    def _sweep(self, fn, poses7, query_xyzi, query_offsets, arr, V, keep_ptr, voi_max_range, packed_xyz):
         P = np.ascontiguousarray(poses7, dtype=np.float64).reshape(-1, 7)
         qo = np.ascontiguousarray(query_offsets, dtype=np.uint64)
         F = len(qo) - 1
         assert len(P) == F
-        arr, V = self.sweep_variants(variants)
         if isinstance(query_xyzi, (int, np.integer)):
             qptr, kind = c_void_p(int(query_xyzi)) if int(query_xyzi) else None, PTR_DEVICE
         else:
@@ -584,7 +617,6 @@ class Handle(_Native):
                 q = np.ascontiguousarray(q[:, :3])
             self._keep = [q]
             qptr, kind = q.ctypes.data, PTR_HOST
-        fn = self.L.erasor_process_nodes_sweep_async if asynchronous else self.L.erasor_process_nodes_sweep
         self._sweep_args = (P, qo, arr)      # alive until the asynchronous submission has been waited for
         self._ck(fn(self.h, P.ctypes.data_as(POINTER(c_double)), qptr, qo.ctypes.data_as(POINTER(c_uint64)), F, float(voi_max_range),
                     arr, V, c_void_p(keep_ptr) if keep_ptr else None, kind | (PTR_QUERY_XYZ if packed_xyz else 0)))

@@ -60,8 +60,8 @@ struct SrtParams {
     int    scatter_mode;       // 0: every bin (cloud outputs), 1: flagged bins only (mask outputs)
 };
 
-// Scan Ratio Test sweep (erasor_process_nodes_sweep, DESIGN.md section 8.5): the three per-setting fields of one variant (the
-// layout of erasor_srt_variant_t) and the variants of one K2 launch, passed by value (32 x 24 = 768 bytes of kernel parameters)
+// Sweeps (erasor_process_nodes_sweep[_ex], DESIGN.md sections 8.5 and 8.6): the Scan Ratio Test fields of one setting and the
+// settings of one K2 launch, passed by value (32 x 24 = 768 bytes of kernel parameters)
 constexpr int kMaxSweepVariants = 32;
 struct SrtVariant {
     double scan_ratio_threshold;
@@ -76,15 +76,6 @@ struct SrtSweep {
     uint32_t*  n_flagged;          // [F][32] flagged bins per (frame, variant) of the submission
 };
 
-// The sweep's fold in K4's epilogue: keep[v * n + src] = 0 for every rejected point and every variant v whose bit the bin's
-// record carries (FlagRec::cursor); rejected[frame * 32 + v] counts them.
-struct K4Sweep {
-    uint8_t*  keep;                // [V][n] variant masks
-    uint32_t* rejected;            // [F][32]
-    uint32_t  n;                   // map points (writes beyond it are dropped)
-    uint32_t  pad_;
-};
-
 struct GpfParams {
     double th_dist;            // gf_dist_thr
     double th_seeds;           // gf_th_seeds_height
@@ -92,6 +83,20 @@ struct GpfParams {
     int    num_lpr;
     int    iters;
     int    cov_mode;
+};
+
+// The sweep's R-GPF and fold (DESIGN.md sections 8.5 and 8.6).  The settings are grouped by their ground-filter fields: group g
+// fits with gp[g] and holds the settings in bits[g] (the groups partition the settings and are ordered by their lowest setting).
+// A bin fits once per group that shares a setting with its record (FlagRec::cursor) and zeroes keep[v * n + src] for every
+// point that fit rejects and every such setting v; rejected[frame * 32 + v] counts them.  Passed as a __grid_constant__
+// kernel parameter (32 x 36 bytes of groups).
+struct K4Sweep {
+    uint8_t*  keep;                // [V][n] variant masks
+    uint32_t* rejected;            // [F][32]
+    uint32_t  n;                   // map points (writes beyond it are dropped)
+    int       n_groups;            // 1..32
+    uint32_t  bits[kMaxSweepVariants];
+    GpfParams gp[kMaxSweepVariants];
 };
 
 // The multi-GPU fold, done in K4's epilogue: global_keep[index ? index[frame_base + src] : src] = 0 for every rejected point.

@@ -7,7 +7,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -112,7 +111,8 @@ struct erasor_ctx {
     int      f0 = 0;                           // first frame of the sub-batch being submitted
     std::vector<uint32_t> node_nvoi;           // node mode: |map_voi_| of the frames before f0 (the count tables hold the last sub-batch only)
     struct StepGraph { const void* ptr[8]; size_t fold_n; int kind, mode, f0; uint64_t epoch, alloc; cudaGraphExec_t exec;
-                       const void* vkeep; int nv; SrtVariant var[kMaxSweepVariants]; };   // vkeep / nv / var: a sweep's masks and variants
+                       const void* vkeep; int nv; SrtVariant var[kMaxSweepVariants]; K4Sweep gf; };   // vkeep / nv / var / gf: a sweep's
+                                                                                                      // masks, variants and ground-filter groups
     std::vector<StepGraph> graphs;             // captured mask-mode steps, one per (pointers, geometry)
     bool     use_graphs = true;
     int      ctas_per_sm = 4;                  // K1 / K2 grid target: one wave of sm_count * ctas_per_sm CTAs (ERASOR_B200_CTAS_PER_SM)
@@ -125,7 +125,7 @@ struct erasor_ctx {
     uint32_t class_c_count_host = 0;           // queue[kBucketC0] of the submission in flight
     struct { bool with_c = true, host = false; int mode = 1; uint8_t* d_keep = nullptr; uint8_t* user_keep = nullptr; size_t n_keep = 0;
              uint8_t* keep_out = nullptr; size_t n_map_global = 0; K4Fold fold{nullptr, nullptr, 0u, 0u};
-             bool sweep = false; K4Sweep ksweep{nullptr, nullptr, 0u, 0u}; } last;
+             bool sweep = false; K4Sweep ksweep{}; } last;
     int      sweep_V = 0;                      // variants of the last node call when it was a sweep (erasor_get_sweep_stats), else 0
 
     // node mode
@@ -938,9 +938,10 @@ struct Submit {
     const double*   poses7 = nullptr;       // mode 2: the caller's odom7 of these frames (the inserts' body -> origin)
     uint8_t*        keep_out = nullptr;     // mode 2 (nullable)
     int             f0 = 0;                 // index of the first frame within the caller's batch (per-frame counters)
-    const SrtVariant* variants = nullptr;   // mode 2: a Scan Ratio Test sweep of n_variants settings into variant_keep [V][n_map]
-    int             n_variants = 0;
+    const SrtVariant* variants = nullptr;   // mode 2: a sweep of n_variants settings into variant_keep [V][n_map]: their Scan Ratio
+    int             n_variants = 0;         // Test fields, and their ground-filter groups (groups->n_groups, bits, gp)
     uint8_t*        variant_keep = nullptr;
+    const K4Sweep*  groups = nullptr;
 };
 
 bool is_pinned_host(const void* p) {
@@ -988,7 +989,7 @@ int submit(erasor_ctx* h, const Submit& S) {
     const bool with_c = h->class_c_state != 0;
     const bool sweep = S.n_variants > 0;
     SrtSweep ssw{};
-    K4Sweep  ksw{nullptr, nullptr, 0u, 0u};
+    K4Sweep  ksw{};
     if (sweep) {
         const size_t rows = (size_t)kMaxSweepVariants * (size_t)std::max(h->stat_F, h->f0 + S.F);
         CK(h->d_sweep_flag.ensure(sizeof(uint32_t) * rows));
@@ -996,7 +997,8 @@ int submit(erasor_ctx* h, const Submit& S) {
         std::copy(S.variants, S.variants + S.n_variants, ssw.v);
         ssw.n = S.n_variants;
         ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + (size_t)kMaxSweepVariants * S.f0;
-        ksw = K4Sweep{S.variant_keep, h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * S.f0, (uint32_t)n_map_global, 0u};
+        ksw = *S.groups;
+        ksw.keep = S.variant_keep; ksw.rejected = h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * S.f0; ksw.n = (uint32_t)n_map_global;
     }
     auto enqueue = [&]() -> int {
         int r;
@@ -1045,11 +1047,13 @@ int submit(erasor_ctx* h, const Submit& S) {
         key.ptr[5] = S.keep_out; key.ptr[6] = S.mode == 2 ? (const void*)h->map : nullptr; key.ptr[7] = with_c ? (const void*)h : nullptr;
         key.fold_n = S.fold_n; key.kind = S.ptr_kind | (S.qry_xyz ? ERASOR_PTR_QUERY_XYZ : 0) | (ins ? 0x100 : 0); key.mode = S.mode; key.f0 = S.f0; key.epoch = h->desc_epoch; key.alloc = h->alloc_epoch;
         key.vkeep = S.variant_keep; key.nv = S.n_variants;
-        if (sweep) std::copy(S.variants, S.variants + S.n_variants, key.var);
+        if (sweep) { std::copy(S.variants, S.variants + S.n_variants, key.var); key.gf = ksw; }
         auto same = [&](const erasor_ctx::StepGraph& g) {
             return std::equal(g.ptr, g.ptr + 8, key.ptr) && g.fold_n == key.fold_n && g.kind == key.kind && g.mode == key.mode && g.f0 == key.f0 &&
                    g.epoch == key.epoch && g.alloc == key.alloc && g.vkeep == key.vkeep && g.nv == key.nv &&
-                   std::memcmp(g.var, key.var, sizeof(SrtVariant) * (size_t)key.nv) == 0;
+                   std::memcmp(g.var, key.var, sizeof(SrtVariant) * (size_t)key.nv) == 0 && g.gf.n_groups == key.gf.n_groups &&
+                   std::memcmp(g.gf.bits, key.gf.bits, sizeof(uint32_t) * (size_t)key.gf.n_groups) == 0 &&
+                   std::memcmp(g.gf.gp, key.gf.gp, sizeof(GpfParams) * (size_t)key.gf.n_groups) == 0;
         };
         cudaGraphExec_t exec = nullptr;
         for (auto& g : h->graphs) if (same(g)) exec = g.exec;
@@ -1163,7 +1167,7 @@ int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
 
 int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                        double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind, bool async,
-                       const SrtVariant* variants = nullptr, int n_variants = 0, uint8_t* variant_keep = nullptr) {
+                       const SrtVariant* variants = nullptr, int n_variants = 0, uint8_t* variant_keep = nullptr, const K4Sweep* groups = nullptr) {
     if (!h || !poses7 || !query_offsets) { if (h) h->err = "null argument"; return ERASOR_E_INVALID; }
     if (!h->map) { h->err = "erasor_process_nodes: no map attached (erasor_attach_map)"; return ERASOR_E_STATE; }
     if (n_frames <= 0) { h->err = "n_frames must be positive"; return ERASOR_E_INVALID; }
@@ -1213,7 +1217,7 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         S.poses = poses.data();
         S.poses7 = poses7 + 7 * (size_t)f0;
         S.keep_out = (f1 == n_frames) ? keep_out : nullptr;
-        S.variants = variants; S.n_variants = n_variants; S.variant_keep = variant_keep;
+        S.variants = variants; S.n_variants = n_variants; S.variant_keep = variant_keep; S.groups = groups;
         if ((rc = submit(h, S))) return rc;
         if (f1 < n_frames) {                                         // the next sub-batch reuses the handle's buffers
             if ((rc = erasor_wait(h))) return rc;
@@ -1370,28 +1374,63 @@ int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const fl
 }
 
 namespace {
+// The sweeps' common path: the settings' Scan Ratio Test fields go to K2, their ground-filter fields are grouped for K4 (one
+// GpfParams per distinct tuple, in order of first appearance, with the settings that carry it).
 int process_nodes_sweep_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
-                             double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind, bool async) {
-    static_assert(sizeof(erasor_srt_variant_t) == sizeof(SrtVariant) && offsetof(erasor_srt_variant_t, minimum_num_pts) == offsetof(SrtVariant, minimum_num_pts),
-                  "erasor_srt_variant_t and SrtVariant share one layout");
+                             double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind, bool async) {
     if (!h) return ERASOR_E_INVALID;
-    if (n_variants < 1 || n_variants > kMaxSweepVariants) { h->err = "n_variants must be in [1, 32]"; return ERASOR_E_INVALID; }
-    if (!variants || !variant_keep) { h->err = "null variants or variant_keep"; return ERASOR_E_INVALID; }
+    if (n_settings < 1 || n_settings > kMaxSweepVariants) { h->err = "n_variants must be in [1, 32]"; return ERASOR_E_INVALID; }
+    if (!settings || !variant_keep) { h->err = "null variants or variant_keep"; return ERASOR_E_INVALID; }
+    for (int v = 0; v < n_settings; ++v)
+        if (settings[v].gf_iter > kMaxIter) { h->err = "gf_iter above the tap capacity (8)"; return ERASOR_E_UNSUPPORTED; }
     if (!h->map) { h->err = "erasor_process_nodes_sweep: no map attached (erasor_attach_map)"; return ERASOR_E_INVALID; }
     if (h->node_inserts) { h->err = "a sweep has no node inserts: erasor_set_node_inserts(h, 0) first"; return ERASOR_E_INVALID; }
     if (h->pending) { h->err = "erasor_process_nodes_sweep while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
+    SrtVariant variants[kMaxSweepVariants];
+    K4Sweep groups{};
+    for (int v = 0; v < n_settings; ++v) {
+        const erasor_sweep_setting_t& x = settings[v];
+        variants[v] = SrtVariant{x.scan_ratio_threshold, x.th_bin_max_h, x.minimum_num_pts, 0};
+        GpfParams gp{};
+        gp.th_dist = x.gf_dist_thr; gp.th_seeds = x.gf_th_seeds_height; gp.num_lowest_pts = x.num_lowest_pts;
+        gp.num_lpr = x.gf_num_lpr; gp.iters = x.gf_iter; gp.cov_mode = h->p.cov_mode;
+        int g = 0;
+        while (g < groups.n_groups && std::memcmp(&groups.gp[g], &gp, sizeof(GpfParams)) != 0) ++g;
+        if (g == groups.n_groups) groups.gp[groups.n_groups++] = gp;
+        groups.bits[g] |= 1u << v;
+    }
     return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, nullptr, nullptr, ptr_kind, async,
-                              reinterpret_cast<const SrtVariant*>(variants), n_variants, variant_keep);
+                              variants, n_settings, variant_keep, &groups);
+}
+
+// erasor_process_nodes_sweep: the settings with the handle's ground-filter fields (one group)
+int process_nodes_srt_sweep(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                            double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind, bool async) {
+    erasor_sweep_setting_t settings[kMaxSweepVariants];
+    const bool ok = h && variants && n_variants >= 1 && n_variants <= kMaxSweepVariants;     // otherwise the common path refuses
+    for (int v = 0; ok && v < n_variants; ++v)
+        settings[v] = erasor_sweep_setting_t{variants[v].scan_ratio_threshold, variants[v].th_bin_max_h, h->p.gf_dist_thr, h->p.gf_th_seeds_height,
+                                             variants[v].minimum_num_pts, h->p.num_lowest_pts, h->p.gf_num_lpr, h->p.gf_iter};
+    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, ok ? settings : nullptr, n_variants,
+                                    variant_keep, ptr_kind, async);
 }
 }  // namespace
 
 int erasor_process_nodes_sweep(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind) {
-    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants, variant_keep, ptr_kind, false);
+    return process_nodes_srt_sweep(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants, variant_keep, ptr_kind, false);
 }
 int erasor_process_nodes_sweep_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                      double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind) {
-    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants, variant_keep, ptr_kind, true);
+    return process_nodes_srt_sweep(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants, variant_keep, ptr_kind, true);
+}
+int erasor_process_nodes_sweep_ex(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                  double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind) {
+    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, false);
+}
+int erasor_process_nodes_sweep_ex_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                        double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind) {
+    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, true);
 }
 
 int erasor_get_sweep_stats(erasor_handle_t h, uint32_t* n_flagged_bins, uint32_t* n_rejected_points) {

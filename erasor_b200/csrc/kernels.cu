@@ -1578,9 +1578,11 @@ struct K4Shared {
 };
 
 // One flagged bin, handled by one group.  X/Y/Z/ORD/FLG live in shared memory or in the bin's slice of the global scratch.
-// SWEEP: the bin's rejected points are also folded into the mask of every variant in rc.cursor (sweep: K4Sweep).
+// SWEEP: after the load and the z sort, the bin is fitted once per ground-filter group that shares a setting with rc.cursor,
+// each fit with the group's parameters (sweep: K4Sweep; P_handle is not read), and its rejected points are folded into the mask
+// of every setting of rc.cursor in that group.
 template <int G, bool kShared, bool SWEEP>
-__device__ __forceinline__ void k4_process_bin(const GpfParams& P, FlagRec& rc, unsigned char* base, float* prd, uint32_t* cnt_scratch, K4Shared& sh,
+__device__ __forceinline__ void k4_process_bin(const GpfParams& P_handle, FlagRec& rc, unsigned char* base, float* prd, uint32_t* cnt_scratch, K4Shared& sh,
                                                const float4* __restrict__ sorted_pts, uint32_t* __restrict__ sorted_src,
                                                const float4* __restrict__ in_pts, const uint32_t* __restrict__ frame_off,
                                                float4* __restrict__ part_pts, uint8_t* __restrict__ keep_mask,
@@ -1589,11 +1591,12 @@ __device__ __forceinline__ void k4_process_bin(const GpfParams& P, FlagRec& rc, 
     const int tid = group_tid<G>(), lane = tid & 31, warp = tid >> 5;
     const uint32_t n = rc.n_points, src_begin = rc.src_begin;
     const uint32_t fbase = frame_off[rc.frame];
-    // slice layout: [ORD n u32][TMP n u32 (CTA groups only)][X][Y][Z n f32 each][FLG n u8]; ORD|TMP is also the 8n-byte
-    // exchange area of the class-B sort, hence first (the slice base is 16-byte aligned)
+    // slice layout: [ORD n u32][TMP n u32 (CTA groups, and warp groups of a sweep with more than one group)][X][Y][Z n f32 each]
+    // [FLG n u8]; ORD|TMP is also the 8n-byte exchange area of the class-B sort, hence first (the slice base is 16-byte aligned).
+    // A sweep keeps the z order in TMP while the groups' fits rewrite ORD (with one group it is never needed again).
     uint32_t* ORD = reinterpret_cast<uint32_t*>(base);
     uint32_t* TMP = ORD + n;
-    float*    X   = reinterpret_cast<float*>((G == 32) ? TMP : TMP + n);
+    float*    X   = reinterpret_cast<float*>((G == 32 && !(SWEEP && sweep->n_groups > 1)) ? TMP : TMP + n);
     float*    Y   = X + n;
     float*    Z   = Y + n;
     uint8_t*  FLG = reinterpret_cast<uint8_t*>(Z + n);
@@ -1650,217 +1653,241 @@ __device__ __forceinline__ void k4_process_bin(const GpfParams& P, FlagRec& rc, 
     }
     K4_TICK(1);
 
-    // extract_initial_seeds_ (erasor.cpp:204-231)
-    if (tid == 0) {
-        double sum = 0.0;
-        int    cnt = 0;
-        if (P.num_lowest_pts >= 0) {
-            for (uint32_t i = (uint32_t)P.num_lowest_pts; i < n && cnt < P.num_lpr; ++i) { sum += (double)Z[ORD[i]]; ++cnt; }
+    // A sweep's groups in ascending order of their lowest setting.  The first group that runs writes the record's taps,
+    // frame_rejected and the empty-fit count; each group folds into the masks of its settings (vm).  The z order is copied to
+    // TMP when a later group needs it (TMP is free once the sort is done: k4_compact rewrites ORD only, and a sweep has no
+    // part_pts) and restored before each later group's seeds.
+    uint32_t todo = SWEEP ? rc.cursor : 0u;      // settings of the record whose group has not run yet
+    bool first = true;
+    for (int grp_i = 0; grp_i < (SWEEP ? sweep->n_groups : 1); ++grp_i) {
+        uint32_t vm = 0u;
+        if constexpr (SWEEP) {
+            vm = todo & sweep->bits[grp_i];
+            if (vm == 0u) continue;
+            todo &= ~vm;
+            if (!first)    { for (uint32_t i = tid; i < n; i += G) ORD[i] = TMP[i]; group_sync<G>(); }
+            else if (todo) { for (uint32_t i = tid; i < n; i += G) TMP[i] = ORD[i]; group_sync<G>(); }
         }
-        const double lpr = cnt != 0 ? sum / cnt : 0.0;
-        rc.lpr_height = lpr;
-        sh.seed_thr   = lpr + P.th_seeds;
-    }
-    group_sync<G>();
-    const double seed_thr = sh.seed_thr;
-    uint32_t m;   // seeds = sorted prefix with z < lpr + th_seeds
-    {
-        uint32_t c = 0;
-        for (uint32_t i = tid; i < n; i += G) c += ((double)Z[ORD[i]] < seed_thr) ? 1u : 0u;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(FULL_MASK, c, o);
-        if (G == 32) {
-            m = c;
-        } else {
-            if (lane == 0) sh.warp[warp] = c;
-            __syncthreads();
-            m = 0;
-#pragma unroll
-            for (int ww = 0; ww < G / 32; ++ww) m += sh.warp[ww];
-            __syncthreads();
-        }
-    }
-    if (tid == 0) rc.n_seeds = m;
-    K4_TICK(2);
+        const GpfParams& P = SWEEP ? sweep->gp[grp_i] : P_handle;
+        const bool taps = !SWEEP || first;
 
-    uint32_t n_empty = 0;
-    for (int it = 0; it < P.iters; ++it) {
-        // ---- estimate_plane_ over ORD[0..m) (erasor.cpp:183-198) ----
-        // pcl::computeMeanAndCovarianceMatrix: nine float accumulators walked in list order.  The nine products of a
-        // half tile of list elements are staged in shared memory (row stride HT+1: conflict-free for the nine summing
-        // lanes), then lane L of warp 0 adds row L in order: the serial FADD chain is fed by independent, prefetchable
-        // shared-memory loads (4-5 cycles per element instead of a dependent gather).
-        float K0 = 0.0f, K1 = 0.0f, K2 = 0.0f;
-        if (P.cov_mode == 1 && m > 0) { const uint32_t f0 = ORD[0]; K0 = X[f0]; K1 = Y[f0]; K2 = Z[f0]; }
-        float acc = 0.0f;
-        if (m > 0) {
-            // PRD holds two buffers of 9 x (HT + 1): while the nine lanes add the rows of one buffer in order, the next
-            // HT list elements are staged into the other.  A warp group does both in one instruction stream (the staging
-            // loads are in flight under the serial FADD chain; every lane runs the chain, lanes >= 9 on a copy of row 8,
-            // so that there is no branch between the two); in a CTA group warp 0 adds and the next 128 threads stage.
-            auto stage_prod = [&](float x, float y, float z, float* buf, uint32_t k) {
-                x = FS(x, K0); y = FS(y, K1); z = FS(z, K2);
-                buf[0 * (HT + 1) + k] = FM(x, x);
-                buf[1 * (HT + 1) + k] = FM(x, y);
-                buf[2 * (HT + 1) + k] = FM(x, z);
-                buf[3 * (HT + 1) + k] = FM(y, y);
-                buf[4 * (HT + 1) + k] = FM(y, z);
-                buf[5 * (HT + 1) + k] = FM(z, z);
-                buf[6 * (HT + 1) + k] = x;
-                buf[7 * (HT + 1) + k] = y;
-                buf[8 * (HT + 1) + k] = z;
-            };
-            auto chain = [&](const float* buf, uint32_t cntk) {
-                const float* row = buf + min(lane, 8) * (HT + 1);
-                if (cntk == (uint32_t)HT) {
-#pragma unroll
-                    for (int k = 0; k < HT; k += 16) {
-                        float q[16];
-#pragma unroll
-                        for (int u = 0; u < 16; ++u) q[u] = row[k + u];
-#pragma unroll
-                        for (int u = 0; u < 16; ++u) acc = FA(acc, q[u]);
-                    }
-                } else {
-                    for (uint32_t k = 0; k < cntk; k += 16u) {
-                        float q[16];
-#pragma unroll
-                        for (uint32_t u = 0; u < 16u; ++u) q[u] = row[min(k + u, (uint32_t)HT)];
-#pragma unroll
-                        for (uint32_t u = 0; u < 16u; ++u) { if (k + u < cntk) acc = FA(acc, q[u]); }
-                    }
-                }
-            };
-            {   // prologue: list elements [0, HT) -> buffer 0
-                const uint32_t k = (G == 32) ? (uint32_t)lane : (uint32_t)tid;
-                if (k < (uint32_t)HT) { const uint32_t idx = ORD[min(k, m - 1u)]; stage_prod(X[idx], Y[idx], Z[idx], PRD, k); }
+        // extract_initial_seeds_ (erasor.cpp:204-231)
+        if (tid == 0) {
+            double sum = 0.0;
+            int    cnt = 0;
+            if (P.num_lowest_pts >= 0) {
+                for (uint32_t i = (uint32_t)P.num_lowest_pts; i < n && cnt < P.num_lpr; ++i) { sum += (double)Z[ORD[i]]; ++cnt; }
             }
-            group_sync<G>();
-            uint32_t t = 0;
-            for (uint32_t base_i = 0; base_i < m; base_i += HT, ++t) {
-                float* cur = PRD + (t & 1u) * PB;
-                float* nxt = PRD + ((t & 1u) ^ 1u) * PB;
-                const uint32_t cntk = min((uint32_t)HT, m - base_i);
-                const bool more = base_i + HT < m;                      // group-uniform
-                if (G == 32) {
-                    float sx = 0.0f, sy = 0.0f, sz = 0.0f;
-                    if (more) { const uint32_t idx = ORD[min(base_i + HT + lane, m - 1u)]; sx = X[idx]; sy = Y[idx]; sz = Z[idx]; }
-                    chain(cur, cntk);
-                    if (more) stage_prod(sx, sy, sz, nxt, (uint32_t)lane);
-                    __syncwarp();
-                } else {
-                    if (warp == 0) {
+            const double lpr = cnt != 0 ? sum / cnt : 0.0;
+            if (taps) rc.lpr_height = lpr;
+            sh.seed_thr   = lpr + P.th_seeds;
+        }
+        group_sync<G>();
+        const double seed_thr = sh.seed_thr;
+        uint32_t m;   // seeds = sorted prefix with z < lpr + th_seeds
+        {
+            uint32_t c = 0;
+            for (uint32_t i = tid; i < n; i += G) c += ((double)Z[ORD[i]] < seed_thr) ? 1u : 0u;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(FULL_MASK, c, o);
+            if (G == 32) {
+                m = c;
+            } else {
+                if (lane == 0) sh.warp[warp] = c;
+                __syncthreads();
+                m = 0;
+#pragma unroll
+                for (int ww = 0; ww < G / 32; ++ww) m += sh.warp[ww];
+                __syncthreads();
+            }
+        }
+        if (tid == 0 && taps) rc.n_seeds = m;
+        K4_TICK(2);
+
+        uint32_t n_empty = 0;
+        for (int it = 0; it < P.iters; ++it) {
+            // ---- estimate_plane_ over ORD[0..m) (erasor.cpp:183-198) ----
+            // pcl::computeMeanAndCovarianceMatrix: nine float accumulators walked in list order.  The nine products of a
+            // half tile of list elements are staged in shared memory (row stride HT+1: conflict-free for the nine summing
+            // lanes), then lane L of warp 0 adds row L in order: the serial FADD chain is fed by independent, prefetchable
+            // shared-memory loads (4-5 cycles per element instead of a dependent gather).
+            float K0 = 0.0f, K1 = 0.0f, K2 = 0.0f;
+            if (P.cov_mode == 1 && m > 0) { const uint32_t f0 = ORD[0]; K0 = X[f0]; K1 = Y[f0]; K2 = Z[f0]; }
+            float acc = 0.0f;
+            if (m > 0) {
+                // PRD holds two buffers of 9 x (HT + 1): while the nine lanes add the rows of one buffer in order, the next
+                // HT list elements are staged into the other.  A warp group does both in one instruction stream (the staging
+                // loads are in flight under the serial FADD chain; every lane runs the chain, lanes >= 9 on a copy of row 8,
+                // so that there is no branch between the two); in a CTA group warp 0 adds and the next 128 threads stage.
+                auto stage_prod = [&](float x, float y, float z, float* buf, uint32_t k) {
+                    x = FS(x, K0); y = FS(y, K1); z = FS(z, K2);
+                    buf[0 * (HT + 1) + k] = FM(x, x);
+                    buf[1 * (HT + 1) + k] = FM(x, y);
+                    buf[2 * (HT + 1) + k] = FM(x, z);
+                    buf[3 * (HT + 1) + k] = FM(y, y);
+                    buf[4 * (HT + 1) + k] = FM(y, z);
+                    buf[5 * (HT + 1) + k] = FM(z, z);
+                    buf[6 * (HT + 1) + k] = x;
+                    buf[7 * (HT + 1) + k] = y;
+                    buf[8 * (HT + 1) + k] = z;
+                };
+                auto chain = [&](const float* buf, uint32_t cntk) {
+                    const float* row = buf + min(lane, 8) * (HT + 1);
+                    if (cntk == (uint32_t)HT) {
+#pragma unroll
+                        for (int k = 0; k < HT; k += 16) {
+                            float q[16];
+#pragma unroll
+                            for (int u = 0; u < 16; ++u) q[u] = row[k + u];
+#pragma unroll
+                            for (int u = 0; u < 16; ++u) acc = FA(acc, q[u]);
+                        }
+                    } else {
+                        for (uint32_t k = 0; k < cntk; k += 16u) {
+                            float q[16];
+#pragma unroll
+                            for (uint32_t u = 0; u < 16u; ++u) q[u] = row[min(k + u, (uint32_t)HT)];
+#pragma unroll
+                            for (uint32_t u = 0; u < 16u; ++u) { if (k + u < cntk) acc = FA(acc, q[u]); }
+                        }
+                    }
+                };
+                {   // prologue: list elements [0, HT) -> buffer 0
+                    const uint32_t k = (G == 32) ? (uint32_t)lane : (uint32_t)tid;
+                    if (k < (uint32_t)HT) { const uint32_t idx = ORD[min(k, m - 1u)]; stage_prod(X[idx], Y[idx], Z[idx], PRD, k); }
+                }
+                group_sync<G>();
+                uint32_t t = 0;
+                for (uint32_t base_i = 0; base_i < m; base_i += HT, ++t) {
+                    float* cur = PRD + (t & 1u) * PB;
+                    float* nxt = PRD + ((t & 1u) ^ 1u) * PB;
+                    const uint32_t cntk = min((uint32_t)HT, m - base_i);
+                    const bool more = base_i + HT < m;                      // group-uniform
+                    if (G == 32) {
+                        float sx = 0.0f, sy = 0.0f, sz = 0.0f;
+                        if (more) { const uint32_t idx = ORD[min(base_i + HT + lane, m - 1u)]; sx = X[idx]; sy = Y[idx]; sz = Z[idx]; }
                         chain(cur, cntk);
-                    } else if (more && tid - 32 < HT) {
-                        const uint32_t k = (uint32_t)tid - 32u;
-                        const uint32_t idx = ORD[min(base_i + HT + k, m - 1u)];
-                        stage_prod(X[idx], Y[idx], Z[idx], nxt, k);
+                        if (more) stage_prod(sx, sy, sz, nxt, (uint32_t)lane);
+                        __syncwarp();
+                    } else {
+                        if (warp == 0) {
+                            chain(cur, cntk);
+                        } else if (more && tid - 32 < HT) {
+                            const uint32_t k = (uint32_t)tid - 32u;
+                            const uint32_t idx = ORD[min(base_i + HT + k, m - 1u)];
+                            stage_prod(X[idx], Y[idx], Z[idx], nxt, k);
+                        }
+                        __syncthreads();
                     }
-                    __syncthreads();
                 }
             }
-        }
-        if (warp == 0) {
-            if (lane < 9 && m != 0) acc = FD(acc, (float)m);
-            K4_TICK(3);
-            float a[9];
+            if (warp == 0) {
+                if (lane < 9 && m != 0) acc = FD(acc, (float)m);
+                K4_TICK(3);
+                float a[9];
 #pragma unroll
-            for (int k = 0; k < 9; ++k) a[k] = __shfl_sync(FULL_MASK, acc, k);
-            if (lane == 0) {
-                float cov[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, mean[3] = {0, 0, 0};
-                if (m != 0) {
-                    mean[0] = (P.cov_mode == 1) ? FA(a[6], K0) : a[6];
-                    mean[1] = (P.cov_mode == 1) ? FA(a[7], K1) : a[7];
-                    mean[2] = (P.cov_mode == 1) ? FA(a[8], K2) : a[8];
-                    cov[0] = FS(a[0], FM(a[6], a[6]));
-                    cov[1] = FS(a[1], FM(a[6], a[7]));
-                    cov[2] = FS(a[2], FM(a[6], a[8]));
-                    cov[4] = FS(a[3], FM(a[7], a[7]));
-                    cov[5] = FS(a[4], FM(a[7], a[8]));
-                    cov[8] = FS(a[5], FM(a[8], a[8]));
-                    cov[3] = cov[1]; cov[6] = cov[2]; cov[7] = cov[5];
-                }
-                float nrm[3];
-                prof[7] += jacobi_svd_normal(cov, nrm);
-                const float dot = FA(FA(FM(nrm[0], mean[0]), FM(nrm[1], mean[1])), FM(nrm[2], mean[2]));
-                const double d  = (double)(-dot);
-                sh.normal[0] = nrm[0]; sh.normal[1] = nrm[1]; sh.normal[2] = nrm[2];
-                sh.thd = P.th_dist - d;
-                if (it < kMaxIter) {
-                    rc.normal_d[it][0] = nrm[0]; rc.normal_d[it][1] = nrm[1]; rc.normal_d[it][2] = nrm[2]; rc.normal_d[it][3] = d;
+                for (int k = 0; k < 9; ++k) a[k] = __shfl_sync(FULL_MASK, acc, k);
+                if (lane == 0) {
+                    float cov[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, mean[3] = {0, 0, 0};
+                    if (m != 0) {
+                        mean[0] = (P.cov_mode == 1) ? FA(a[6], K0) : a[6];
+                        mean[1] = (P.cov_mode == 1) ? FA(a[7], K1) : a[7];
+                        mean[2] = (P.cov_mode == 1) ? FA(a[8], K2) : a[8];
+                        cov[0] = FS(a[0], FM(a[6], a[6]));
+                        cov[1] = FS(a[1], FM(a[6], a[7]));
+                        cov[2] = FS(a[2], FM(a[6], a[8]));
+                        cov[4] = FS(a[3], FM(a[7], a[7]));
+                        cov[5] = FS(a[4], FM(a[7], a[8]));
+                        cov[8] = FS(a[5], FM(a[8], a[8]));
+                        cov[3] = cov[1]; cov[6] = cov[2]; cov[7] = cov[5];
+                    }
+                    float nrm[3];
+                    prof[7] += jacobi_svd_normal(cov, nrm);
+                    const float dot = FA(FA(FM(nrm[0], mean[0]), FM(nrm[1], mean[1])), FM(nrm[2], mean[2]));
+                    const double d  = (double)(-dot);
+                    sh.normal[0] = nrm[0]; sh.normal[1] = nrm[1]; sh.normal[2] = nrm[2];
+                    sh.thd = P.th_dist - d;
+                    if (taps && it < kMaxIter) {
+                        rc.normal_d[it][0] = nrm[0]; rc.normal_d[it][1] = nrm[1]; rc.normal_d[it][2] = nrm[2]; rc.normal_d[it][3] = d;
+                    }
                 }
             }
+            if (m == 0) ++n_empty;
+            group_sync<G>();
+            K4_TICK(4);
+            const float n0 = sh.normal[0], n1 = sh.normal[1], n2 = sh.normal[2];
+            const double thd = sh.thd;
+            // ---- classify every point of the bin in source order (erasor.cpp:265-281) ----
+            // (classification fused into the stable compaction: one pass over the bin instead of two)
+            m = k4_compact<G>(n, ORD, sh.warp, [&](uint32_t i) {
+                const float r = FA(FA(FM(X[i], n0), FM(Y[i], n1)), FM(Z[i], n2));
+                const bool  g = (double)r < thd;
+                FLG[i] = g ? 1 : 0;
+                return g;
+            });
+            if (tid == 0 && taps && it < kMaxIter) rc.n_ground[it] = m;
+            K4_TICK(5);
         }
-        if (m == 0) ++n_empty;
-        group_sync<G>();
-        K4_TICK(4);
-        const float n0 = sh.normal[0], n1 = sh.normal[1], n2 = sh.normal[2];
-        const double thd = sh.thd;
-        // ---- classify every point of the bin in source order (erasor.cpp:265-281) ----
-        // (classification fused into the stable compaction: one pass over the bin instead of two)
-        m = k4_compact<G>(n, ORD, sh.warp, [&](uint32_t i) {
-            const float r = FA(FA(FM(X[i], n0), FM(Y[i], n1)), FM(Z[i], n2));
-            const bool  g = (double)r < thd;
-            FLG[i] = g ? 1 : 0;
-            return g;
-        });
-        if (tid == 0 && it < kMaxIter) rc.n_ground[it] = m;
-        K4_TICK(5);
-    }
-    // gf_iter == 0: the reference returns the seeds as ground and fills no outliers (erasor.cpp:260-285)
-    if (P.iters <= 0) {
-        for (uint32_t i = tid; i < n; i += G) FLG[i] = 0;
-        group_sync<G>();
-        for (uint32_t i = tid; i < m; i += G) FLG[ORD[i]] = 1;
-        group_sync<G>();
-    }
-    if (tid == 0) {
-        rc.n_ground_final = m; rc.n_empty_fits = n_empty; rc.n_rejected = (P.iters > 0) ? n - m : 0u;
-        if (n_empty) atomicAdd(&fence[1], (unsigned long long)n_empty);
-        if (frame_rejected) atomicAdd(&frame_rejected[rc.frame], n - m);
-        if constexpr (SWEEP)
-            for (uint32_t r = rc.cursor; r; r &= r - 1u) atomicAdd(&sweep->rejected[(size_t)rc.frame * kMaxSweepVariants + (__ffs(r) - 1)], n - m);
-    }
+        // gf_iter == 0: the reference returns the seeds as ground and fills no outliers (erasor.cpp:260-285)
+        if (P.iters <= 0) {
+            for (uint32_t i = tid; i < n; i += G) FLG[i] = 0;
+            group_sync<G>();
+            for (uint32_t i = tid; i < m; i += G) FLG[ORD[i]] = 1;
+            group_sync<G>();
+        }
+        if (tid == 0) {
+            if (taps) {
+                rc.n_ground_final = m; rc.n_empty_fits = n_empty; rc.n_rejected = (P.iters > 0) ? n - m : 0u;
+                if (n_empty) atomicAdd(&fence[1], (unsigned long long)n_empty);
+                if (frame_rejected) atomicAdd(&frame_rejected[rc.frame], n - m);
+            }
+            if constexpr (SWEEP)
+                for (uint32_t r = vm; r; r &= r - 1u) atomicAdd(&sweep->rejected[(size_t)rc.frame * kMaxSweepVariants + (__ffs(r) - 1)], n - m);
+        }
 
-    // ---- outputs ----
-    if (keep_mask || ground_mask || fold.keep || SWEEP) {
-        for (uint32_t i0 = tid; i0 < n; i0 += 4u * G) {
-            uint32_t s[4];
+        // ---- outputs ----
+        if (keep_mask || ground_mask || fold.keep || SWEEP) {
+            for (uint32_t i0 = tid; i0 < n; i0 += 4u * G) {
+                uint32_t s[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {                  // four independent index loads in flight per thread
-                const uint32_t i = i0 + (uint32_t)u * G;
-                s[u] = (i < n) ? sorted_src[src_begin + i] : 0u;
-            }
+                for (int u = 0; u < 4; ++u) {                  // four independent index loads in flight per thread
+                    const uint32_t i = i0 + (uint32_t)u * G;
+                    s[u] = (i < n) ? sorted_src[src_begin + i] : 0u;
+                }
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const uint32_t i = i0 + (uint32_t)u * G;
-                if (i < n) {
-                    if (keep_mask && !FLG[i]) keep_mask[fbase + s[u]] = 0;      // not in the selected bin any more (gf_iter == 0: dropped silently)
-                    if (ground_mask && FLG[i]) ground_mask[fbase + s[u]] = 1;
-                    if (fold.keep && !FLG[i]) {
-                        // the multi-GPU fold, in the epilogue: a global map point survives unless some frame rejected it.
-                        // Only zeros are ever written, so concurrent bins / frames / handles need no atomics.
-                        const uint32_t g = fold.index ? fold.index[fbase + s[u]] : s[u];
-                        if (g < fold.n) fold.keep[g] = 0;
-                    }
-                    if constexpr (SWEEP) {
-                        // the sweep's fold: one plain zero store per variant that flags the bin (node mode: the source index is global)
-                        if (!FLG[i] && s[u] < sweep->n)
-                            for (uint32_t r = rc.cursor; r; r &= r - 1u) sweep->keep[(size_t)(__ffs(r) - 1) * sweep->n + s[u]] = 0;
+                for (int u = 0; u < 4; ++u) {
+                    const uint32_t i = i0 + (uint32_t)u * G;
+                    if (i < n) {
+                        if (keep_mask && !FLG[i]) keep_mask[fbase + s[u]] = 0;      // not in the selected bin any more (gf_iter == 0: dropped silently)
+                        if (ground_mask && FLG[i]) ground_mask[fbase + s[u]] = 1;
+                        if (fold.keep && !FLG[i]) {
+                            // the multi-GPU fold, in the epilogue: a global map point survives unless some frame rejected it.
+                            // Only zeros are ever written, so concurrent bins / frames / handles need no atomics.
+                            const uint32_t g = fold.index ? fold.index[fbase + s[u]] : s[u];
+                            if (g < fold.n) fold.keep[g] = 0;
+                        }
+                        if constexpr (SWEEP) {
+                            // the sweep's fold: one plain zero store per setting of the group that flags the bin (node mode: the
+                            // source index is global)
+                            if (!FLG[i] && s[u] < sweep->n)
+                                for (uint32_t r = vm; r; r &= r - 1u) sweep->keep[(size_t)(__ffs(r) - 1) * sweep->n + s[u]] = 0;
+                        }
                     }
                 }
             }
         }
-    }
-    if (part_pts) {
-        // partitioned copy of the bin: [ground, source order][non-ground, source order]
-        for (uint32_t i = tid; i < m; i += G) part_pts[src_begin + i] = sorted_pts[src_begin + ORD[i]];
+        if (part_pts) {
+            // partitioned copy of the bin: [ground, source order][non-ground, source order]
+            for (uint32_t i = tid; i < m; i += G) part_pts[src_begin + i] = sorted_pts[src_begin + ORD[i]];
+            group_sync<G>();
+            const uint32_t m2 = k4_compact<G>(n, ORD, sh.warp, [&](uint32_t i) { return FLG[i] == 0; });
+            for (uint32_t i = tid; i < m2; i += G) part_pts[src_begin + m + i] = sorted_pts[src_begin + ORD[i]];
+        }
         group_sync<G>();
-        const uint32_t m2 = k4_compact<G>(n, ORD, sh.warp, [&](uint32_t i) { return FLG[i] == 0; });
-        for (uint32_t i = tid; i < m2; i += G) part_pts[src_begin + m + i] = sorted_pts[src_begin + ORD[i]];
+        K4_TICK(6);
+        first = false;
+        if (SWEEP && todo == 0u) break;
     }
-    group_sync<G>();
-    K4_TICK(6);
     if (tid == 0) {
 #pragma unroll
         for (int k = 0; k < 8; ++k) rc.prof[k] = prof[k];
@@ -1869,8 +1896,8 @@ __device__ __forceinline__ void k4_process_bin(const GpfParams& P, FlagRec& rc, 
 }
 
 // The queue loop of k4_rgpf and k4_rgpf_sweep: groups pull records of the class from the bucketed queue (largest bins first)
-// through an atomic cursor until the class is drained.  One text for both kernels; the sweep form differs only in what
-// k4_process_bin folds.
+// through an atomic cursor until the class is drained.  One text for both kernels; the sweep form differs only in
+// k4_process_bin's fits per ground-filter group and what it folds.
 #define K4_RGPF_LOOP(SWEEP, SWEEP_PTR)                                                                                                       \
     extern __shared__ __align__(16) unsigned char smem_raw[];                                                                               \
     constexpr int NG = THREADS / G;                                                                                                         \
@@ -1938,7 +1965,8 @@ k4_rgpf(GpfParams P, FlagRec* __restrict__ recs, uint32_t* __restrict__ queue, c
     K4_RGPF_LOOP(false, nullptr)
 }
 
-// k4_rgpf of a Scan Ratio Test sweep: the records carry the variants' mask, the epilogue folds into the variant masks
+// k4_rgpf of a sweep: the records carry the settings' mask, each bin is fitted once per ground-filter group among them and
+// folded into those settings' masks (the groups: about 1.2 KB, hence a __grid_constant__ parameter)
 template <int THREADS, int G>
 __global__ void __launch_bounds__(THREADS, (THREADS == 256) ? 3 : (THREADS == 128 ? 6 : 1))
 k4_rgpf_sweep(GpfParams P, FlagRec* __restrict__ recs, uint32_t* __restrict__ queue, const uint32_t* __restrict__ bucket_list,
@@ -1946,7 +1974,7 @@ k4_rgpf_sweep(GpfParams P, FlagRec* __restrict__ recs, uint32_t* __restrict__ qu
               const float4* __restrict__ in_pts, const uint32_t* __restrict__ frame_off, float4* __restrict__ part_pts,
               uint8_t* __restrict__ keep_mask, uint8_t* __restrict__ ground_mask, uint32_t* __restrict__ frame_rejected,
               unsigned char* __restrict__ gscratch, uint32_t smem_cap_points, uint32_t slice_bytes,
-              unsigned long long* __restrict__ fence, K4Fold fold, K4Sweep sweep) {
+              unsigned long long* __restrict__ fence, K4Fold fold, const __grid_constant__ K4Sweep sweep) {
     K4_RGPF_LOOP(true, &sweep)
 }
 #undef K4_RGPF_LOOP
@@ -1957,9 +1985,10 @@ static cudaError_t launch_k4_class(cudaStream_t st, const GpfParams& P, FlagRec*
                                    uint32_t* sorted_src, const float4* in_pts, const uint32_t* frame_off, float4* part_pts,
                                    uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected, unsigned char* gscratch, int grid,
                                    unsigned long long* fence, const K4Fold& fold, const K4Sweep* sweep) {
-    // per bin: 12 n (xyz) + 4 n (order) + n (flags) = 17 n for warp groups, + 4 n (second half of the order / exchange area) = 21 n
+    // per bin: 12 n (xyz) + 4 n (order) + n (flags) = 17 n for warp groups, + 4 n (second half of the order / exchange area, or the
+    // saved z order of a sweep with more than one ground-filter group) = 21 n
     constexpr int NG = THREADS / G;
-    constexpr uint32_t per_pt = (G == 32) ? 17u : 21u;
+    const uint32_t per_pt = (G == 32 && !(sweep && sweep->n_groups > 1)) ? 17u : 21u;
     const uint32_t slice = (smem_bytes / NG) & ~15u;
     const uint32_t cap = (slice - 32) / per_pt;
     if ((G == 32 && cap < kClassAMax) || (G == 128 && cap < kClassBMax)) return cudaErrorInvalidConfiguration;   // A / B have no scratch path
@@ -2009,7 +2038,11 @@ cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, con
     // class A: n <= 512, one warp per bin, 8 warps per CTA
     // (two CTAs per SM fit by shared memory: with tens of thousands of small flagged bins per step -- 40 x 360 bins, 2 M-point map --
     //  R-GPF is bound by resident chains per SM, and CTAs that find the queue empty exit at once)
-    return launch_k4_class<256, 32>(st, P, recs, queue, bucket_list, rec_capacity, kBucketA0, kNumBuckets, 0, 8 * (17 * kClassAMax + 48), sorted_pts,
+    // a sweep with more than one ground-filter group keeps the z order in its slices too (21 n): 8 x 10.5 KB + 19.9 KB static
+    // ~ 104 KB per CTA, two CTAs per SM still fit
+    const bool saved_order = sweep && sweep->n_groups > 1;
+    return launch_k4_class<256, 32>(st, P, recs, queue, bucket_list, rec_capacity, kBucketA0, kNumBuckets, 0,
+                                    8 * ((saved_order ? 21 : 17) * kClassAMax + 48), sorted_pts,
                                     sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 2, fence, fold, sweep);
 }
 

@@ -63,7 +63,7 @@ cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, con
                       const uint32_t* bucket_list, uint32_t rec_capacity, const float4* sorted_pts, uint32_t* sorted_src, const float4* in_pts, const uint32_t* frame_off,
                       float4* part_pts, uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected, unsigned char* gscratch,
                       int sm_count, unsigned long long* fence, const K4Fold& fold, int classes /*bit 0|1: A and B, bit 2: C*/,
-                      const K4Sweep* sweep = nullptr /*a sweep's per-variant fold (node mode, records from k2_srt_sweep_scatter)*/);
+                      const K4Sweep* sweep = nullptr /*a sweep's ground-filter groups and per-setting fold (node mode, records from k2_srt_sweep_scatter)*/);
 
 // every record of the batch (F frames; cnt / dst_start [2][F][...], qry_off: the query half of frame_off); vox_cnt / vox_start
 // per record

@@ -97,6 +97,22 @@ def sweep_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, 
     RR / F1 of its saved map against gt (default: the initial map, as run_sequence scores) at voxelsize 0.2, the kept map points,
     the saved map's size and the flagged-bin / rejected-point totals.  Row v equals run_frame_independent(nodes, initial_map, up,
     ep.replace(**variants[v])) scored with capi.Evaluator.  Needs a CUDA device."""
+    from . import capi
+    return _sweep_rows(nodes, initial_map, up, ep, variants, capi.SRT_SWEEP_FIELDS, gt, batch, save_voxel_size)
+
+
+def tune_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep, settings, gt: Optional[np.ndarray] = None, batch: int = 20,
+                           save_voxel_size: Optional[float] = None) -> list:
+    """sweep_frame_independent over settings that may also vary R-GPF's fields (1..32 dicts of capi.SRT_SWEEP_FIELDS +
+    capi.GF_SWEEP_FIELDS; a missing field comes from ep) in one node-mode pass (erasor_process_nodes_sweep_ex, DESIGN.md section
+    8.6): each flagged bin is sorted by z once and fitted once per distinct ground-filter tuple.  Rows as sweep_frame_independent's,
+    with all eight fields.  Needs a CUDA device."""
+    from . import capi
+    return _sweep_rows(nodes, initial_map, up, ep, settings, capi.SRT_SWEEP_FIELDS + capi.GF_SWEEP_FIELDS, gt, batch, save_voxel_size)
+
+
+def _sweep_rows(nodes, initial_map, up, ep, variants, fields, gt, batch, save_voxel_size) -> list:
+    """The rows of sweep_frame_independent (fields: the Scan Ratio Test's) and tune_frame_independent (all eight)."""
     import torch
 
     from . import capi
@@ -106,13 +122,15 @@ def sweep_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, 
     if not 1 <= len(variants) <= capi.MAX_SWEEP_VARIANTS:
         raise ValueError(f"a sweep takes 1 to {capi.MAX_SWEEP_VARIANTS} settings")
     for v in variants:
-        if set(v) - set(capi.SRT_SWEEP_FIELDS):
-            raise ValueError(f"a sweep varies only {capi.SRT_SWEEP_FIELDS}, not {sorted(set(v) - set(capi.SRT_SWEEP_FIELDS))}")
+        if set(v) - set(fields):
+            raise ValueError(f"a sweep varies only {fields}, not {sorted(set(v) - set(fields))}")
+    ex = len(fields) > len(capi.SRT_SWEEP_FIELDS)
     nodes = list(nodes)
     sel = processed_nodes(nodes, up.removal_interval)
     initial_map = np.ascontiguousarray(initial_map, dtype=np.float32)
     m = capi.Map(initial_map)
     h = capi.Handle(ep.replace(version=up.version))       # /erasor/version as the updater reads it (OfflineMapUpdater.cpp:81)
+    run, settings_of = (h.process_nodes_sweep_ex, h.sweep_settings) if ex else (h.process_nodes_sweep, h.sweep_variants)
     V, n = len(variants), m.size
     leaf = up.map_voxel_size if save_voxel_size is None else save_voxel_size
     rows = []
@@ -129,7 +147,7 @@ def sweep_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, 
             off = np.cumsum([0] + [len(s) for s in scans]).astype(np.uint64)
             raw = np.concatenate(scans)
             d, qo = h.voxelize_batch_ptr(raw.ctypes.data if len(raw) else 0, off, up.query_voxel_size, 0, l2b, capi.PTR_HOST)
-            h.process_nodes_sweep(poses, d, qo, variants, keep.data_ptr(), voi_max_range=up.max_range)
+            run(poses, d, qo, variants, keep.data_ptr(), voi_max_range=up.max_range)
             nf, nr = h.sweep_stats()
             flagged += nf.sum(axis=1, dtype=np.int64)
             rejected += nr.sum(axis=1, dtype=np.int64)
@@ -141,11 +159,9 @@ def sweep_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, 
                 static_map = np.empty((int(oo[-1]), 4), dtype=np.float32)
                 capi._memcpy_from_device(static_map, d)
                 q = ev.evaluate(ref, static_map, voxelsize=0.2)
-                arr, _ = h.sweep_variants([variants[v]])
-                rows.append(dict(scan_ratio_threshold=arr[0].scan_ratio_threshold, th_bin_max_h=arr[0].th_bin_max_h,
-                                 minimum_num_pts=arr[0].minimum_num_pts, PR=q["PR"], RR=q["RR"], F1=q["F1"],
-                                 kept=int(np.count_nonzero(masks[v])), saved=len(static_map),
-                                 flagged=int(flagged[v]), rejected=int(rejected[v])))
+                arr, _ = settings_of([variants[v]])
+                rows.append(dict(**{f: getattr(arr[0], f) for f in fields}, PR=q["PR"], RR=q["RR"], F1=q["F1"],
+                                 kept=int(np.count_nonzero(masks[v])), saved=len(static_map), flagged=int(flagged[v]), rejected=int(rejected[v])))
     finally:
         h.close()
         m.close()

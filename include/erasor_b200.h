@@ -231,10 +231,36 @@ int erasor_process_nodes_sweep(erasor_handle_t h, const double* poses7, const fl
                                double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind);
 int erasor_process_nodes_sweep_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                      double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind);
-/* per (setting, node) counters of the last sweep, HOST arrays [n_variants][n_frames] (nullable): flagged bins and rejected points,
- * as erasor_get_node_stats reports them for that setting.  After a sweep, erasor_get_node_stats gives n_voi_points as usual and
- * the counts of the union of the settings' flagged bins.  ERASOR_E_STATE when the last node call was not a sweep. */
+/* per (setting, node) counters of the last sweep (erasor_process_nodes_sweep or erasor_process_nodes_sweep_ex), HOST arrays
+ * [n_variants][n_frames] (nullable): flagged bins and rejected points, as erasor_get_node_stats reports them for that setting.
+ * After a sweep, erasor_get_node_stats gives n_voi_points as usual and the counts of the union of the settings' flagged bins
+ * (rejected points: each union bin's fit under the ground-filter fields of the lowest setting that flags it).  ERASOR_E_STATE
+ * when the last node call was not a sweep. */
 int erasor_get_sweep_stats(erasor_handle_t h, uint32_t* n_flagged_bins, uint32_t* n_rejected_points);
+
+/* ---- Scan Ratio Test and ground-filter sweep (DESIGN.md section 8.6) ---- */
+/* The eight per-sensor knobs of one setting: the Scan Ratio Test's three and R-GPF's five. */
+typedef struct {
+    double scan_ratio_threshold;
+    double th_bin_max_h;
+    double gf_dist_thr;
+    double gf_th_seeds_height;
+    int    minimum_num_pts;
+    int    num_lowest_pts;
+    int    gf_num_lpr;
+    int    gf_iter;
+} erasor_sweep_setting_t;
+/* erasor_process_nodes_sweep with settings that also carry the ground-filter fields (geometry, version, cov_mode, skip_voxelize
+ * and max_range still come from the handle, whose eight fields above are not read).  The settings are grouped by their five
+ * ground-filter fields: each bin of the union of the settings' flagged bins is loaded and sorted by z once, then fitted once per
+ * group among the settings that flag it.  Mask v equals the map's keep mask after erasor_process_nodes with setting v on a fresh
+ * map; erasor_get_sweep_stats gives that run's flagged and rejected counts.  With every setting's ground-filter fields equal to
+ * the handle's, it returns what erasor_process_nodes_sweep returns.  Arguments and refusals as erasor_process_nodes_sweep, and
+ * ERASOR_E_UNSUPPORTED for a gf_iter above 8 (as erasor_create). */
+int erasor_process_nodes_sweep_ex(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                  double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind);
+int erasor_process_nodes_sweep_ex_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                        double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind);
 
 /* ---- node-mode inserts: the query points each node's static estimate puts back into the map (DESIGN.md section 8.4) ---- */
 /* Opt-in per handle (default off; off changes nothing).  With it on, erasor_process_nodes also builds, per node f, inserted_f:
