@@ -36,7 +36,7 @@ EXPORTS = [
     "erasor_set_node_inserts", "erasor_get_node_inserts", "erasor_map_append_inserts", "erasor_map_inserts", "erasor_map_clear_inserts",
     "erasor_save_node_map",
     "erasor_comm_unique_id", "erasor_comm_init", "erasor_comm_destroy", "erasor_allgather_and_keep", "erasor_and_keep_masks",
-    "erasor_get_kernel_time_ms", "erasor_reset_kernel_times", "erasor_get_rgpf_profile", "erasor_get_srt_profile", "erasor_profile_k1",
+    "erasor_get_kernel_time_ms", "erasor_reset_kernel_times", "erasor_forget_run_history", "erasor_get_rgpf_profile", "erasor_get_srt_profile", "erasor_profile_k1",
     "erasor_updater_create", "erasor_updater_destroy", "erasor_updater_reset", "erasor_updater_last_error", "erasor_updater_process_node", "erasor_updater_prefetch_scan",
     "erasor_updater_map_size", "erasor_updater_get_cloud", "erasor_updater_save_static_map", "erasor_updater_voxelize", "erasor_updater_mapgen_node",
     "erasor_updater_erasor", "erasor_updater_kernel_launch_count", "erasor_updater_get_fused_profile",
@@ -221,6 +221,7 @@ def _load():
     L.erasor_kernel_launch_count.argtypes = [c_void_p]
     L.erasor_get_kernel_time_ms.argtypes = [c_void_p, c_int, POINTER(c_double), POINTER(c_uint64)]
     L.erasor_reset_kernel_times.argtypes = [c_void_p, c_int]
+    L.erasor_forget_run_history.argtypes = [c_void_p]
     L.erasor_get_rgpf_profile.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32), POINTER(c_size_t)]
     L.erasor_get_srt_profile.argtypes = [c_void_p, POINTER(c_uint32)]
     L.erasor_profile_k1.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_size_t), POINTER(c_int)]

@@ -1721,6 +1721,12 @@ int erasor_get_srt_profile(erasor_handle_t h, uint32_t* cycles8) {
 
 uint64_t erasor_kernel_launch_count(erasor_handle_t h) { return h ? h->launches : 0; }
 
+int erasor_forget_run_history(erasor_handle_t h) {
+    if (!h) return ERASOR_E_INVALID;
+    h->class_c_state = -1;
+    return ERASOR_OK;
+}
+
 int erasor_reset_kernel_times(erasor_handle_t h, int enable_timing) {
     if (!h) return ERASOR_E_INVALID;
     CK(cudaSetDevice(h->device));

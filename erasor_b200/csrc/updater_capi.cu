@@ -145,6 +145,14 @@ int reassign_submap(erasor_updater_ctx* u, double px, double py) {
     }
     return ERASOR_OK;
 }
+
+// map_arranged_: in large-scale mode, until the first processed node splits the window off, the whole initial map
+// (load_global_map copies it to both map_arranged_ and map_arranged_global_; the complement is still empty)
+const DeviceBuffer& arranged(const erasor_updater_ctx* u, size_t* n) {
+    const bool whole = u->up.is_large_scale && u->submap_uninit;
+    *n = whole ? u->n_global : u->n_map;
+    return whole ? u->global_a : u->map_a;
+}
 }  // namespace
 
 extern "C" {
@@ -220,6 +228,7 @@ int erasor_updater_reset(erasor_updater_t u, const float* initial_map_xyzi, size
     u->n_complement = 0; u->n_query = u->n_voi = u->n_out = u->n_rej = 0;
     u->submap_uninit = true; u->stack_count = 0;
     u->map_version++;
+    ECK(erasor_forget_run_history(u->er));            // a re-armed pass launches what the first pass did
     return ERASOR_OK;
 }
 
@@ -329,7 +338,7 @@ int erasor_updater_prefetch_scan(erasor_updater_t u, const float* lidar_xyzi, si
 
 int erasor_updater_map_size(erasor_updater_t u, size_t* n) {
     if (!u || !n) return ERASOR_E_INVALID;
-    *n = u->n_map;
+    arranged(u, n);
     return ERASOR_OK;
 }
 
@@ -339,7 +348,7 @@ int erasor_updater_get_cloud(erasor_updater_t u, int which, float* xyzi, size_t 
     if (!u || !n) return ERASOR_E_INVALID;
     const void* src = nullptr; size_t k = 0;
     switch (which) {
-        case 0: src = u->map_a.p(); k = u->n_map; break;
+        case 0: src = arranged(u, &k).p(); break;
         case 1: src = u->voi.p(); k = u->n_voi; break;
         case 2: src = u->qvox.p(); k = u->n_query; break;
         case 5: src = u->tmp_rej.p(); k = u->n_rej; break;
@@ -360,9 +369,9 @@ int erasor_updater_get_cloud(erasor_updater_t u, int which, float* xyzi, size_t 
 int erasor_updater_save_static_map(erasor_updater_t u, float voxel_size, float* out_xyzi, size_t cap, size_t* n) {
     if (!u || !n) return ERASOR_E_INVALID;
     UCK(cudaSetDevice(u->device));
-    const float4* src = u->map_a.as<float4>();
-    size_t ns = u->n_map;
-    if (u->up.is_large_scale) {
+    size_t ns = 0;
+    const float4* src = arranged(u, &ns).as<float4>();
+    if (u->up.is_large_scale && !u->submap_uninit) {
         // *ptr_src = *map_arranged_ + *map_arranged_complement_
         UCK(u->map_b.ensure(sizeof(float4) * std::max<size_t>(u->n_map + u->n_complement, 1)));
         if (u->n_map) UCK(cudaMemcpyAsync(u->map_b.p(), u->map_a.p(), sizeof(float4) * u->n_map, cudaMemcpyDeviceToDevice, u->st));

@@ -332,6 +332,9 @@ uint64_t erasor_kernel_launch_count(erasor_handle_t h);
 /* CUDA-event time (ms) spent in the binning kernel (K1) since the last reset, and its launch count */
 int erasor_get_kernel_time_ms(erasor_handle_t h, int kernel_id, double* total_ms, uint64_t* launches);
 int erasor_reset_kernel_times(erasor_handle_t h, int enable_timing);
+/* forget what earlier runs taught the handle (whether R-GPF's class C, bins beyond 2560 points, has been seen): the next run
+ * launches what a new handle's first run would.  Results never depend on it, only which kernels are launched. */
+int erasor_forget_run_history(erasor_handle_t h);
 
 /* ============================================================================================
  * The caller, device-resident: erasor::OfflineMapUpdater (reference include/erasor/OfflineMapUpdater.h,
@@ -357,7 +360,8 @@ typedef struct {
 int  erasor_updater_create(const erasor_updater_params_t* up, const erasor_params_t* ep, const float* initial_map_xyzi, size_t n_map,
                            int device, erasor_updater_t* out);
 void erasor_updater_destroy(erasor_updater_t u);
-/* load_global_map again (:107-167) on a live updater: new initial map, counters reset, device buffers kept */
+/* load_global_map again (:107-167) on a live updater: new initial map, counters and the handle's run history
+ * (erasor_forget_run_history) reset, device buffers kept */
 int  erasor_updater_reset(erasor_updater_t u, const float* initial_map_xyzi, size_t n_map);
 const char* erasor_updater_last_error(erasor_updater_t u);
 /* replaces OfflineMapUpdater::callback_node(msg) (:203-330): seq = msg->header.seq, odom7 = msg->odom as x y z qx qy qz qw
