@@ -49,6 +49,49 @@ struct erasor_map_ctx {
     std::string  err;
 };
 
+namespace {
+
+// One submission of a mask mode, as enqueue() runs it: everything its copies and launches read besides the handle's buffers and
+// chunk descriptors (whose changes alloc_epoch and desc_epoch track).  The caller fills in the first part, submit() the rest.  A
+// captured graph replays the step it was captured from, so the graph cache is keyed on it; erasor_wait's class-C fix-up and
+// erasor_profile_k1 read the last one.
+struct Step {
+    int           mode = 1;                   // 1: batch of (map_voi, query_voi) pairs, 2: nodes against the resident map
+    int           ptr_kind = ERASOR_PTR_HOST; // of the caller's buffers: HOST or DEVICE
+    bool          qry_xyz = false;            // the query cloud is packed x y z (ERASOR_PTR_QUERY_XYZ)
+    int           f0 = 0;                     // first frame of the sub-batch within the caller's batch (per-frame counters)
+    const float*  map_xyzi = nullptr;         // mode 1
+    const float*  qry_xyzi = nullptr;
+    uint8_t*      user_keep = nullptr;        // mode 1: one byte per VoI point; mode 2: frame_keep [F][n_map] (nullable)
+    uint8_t*      keep_out = nullptr;         // mode 2: receives the map's mask (nullable)
+    K4Fold        fold{nullptr, nullptr, 0u, 0u};   // mode 1: onto the caller's global mask (mode 2: submit() sets the map's)
+    SrtSweep      ssw{};                      // mode 2, a sweep (ssw.n > 0): the settings' Scan Ratio Test fields, and their
+    K4Sweep       ksw{};                      // ground-filter groups with the settings' masks ksw.keep
+    // set by submit()
+    bool          inserts = false;            // node-mode inserts
+    bool          with_c = true;              // R-GPF class C launched up front
+    const float4* cur_map = nullptr;          // what K1 reads: the caller's device clouds, their staging buffers or the resident map
+    const float4* cur_qry = nullptr;
+    uint8_t*      d_keep = nullptr;           // where R-GPF writes user_keep (itself, or staging for a host mask) ...
+    size_t        n_keep = 0;                 // ... and its bytes (0: none)
+    const erasor_map_ctx* map = nullptr;      // mode 2
+    size_t        n_map_global = 0;           // mode 2: map points
+};
+
+bool same_step(const Step& a, const Step& b) {
+    return a.mode == b.mode && a.ptr_kind == b.ptr_kind && a.qry_xyz == b.qry_xyz && a.inserts == b.inserts && a.with_c == b.with_c &&
+           a.f0 == b.f0 && a.map_xyzi == b.map_xyzi && a.qry_xyzi == b.qry_xyzi && a.cur_map == b.cur_map && a.cur_qry == b.cur_qry &&
+           a.user_keep == b.user_keep && a.d_keep == b.d_keep && a.n_keep == b.n_keep && a.keep_out == b.keep_out &&
+           a.n_map_global == b.n_map_global && a.map == b.map &&
+           a.fold.keep == b.fold.keep && a.fold.index == b.fold.index && a.fold.n == b.fold.n &&
+           a.ssw.n == b.ssw.n && a.ssw.n_flagged == b.ssw.n_flagged && std::memcmp(a.ssw.v, b.ssw.v, sizeof(SrtVariant) * (size_t)a.ssw.n) == 0 &&
+           a.ksw.keep == b.ksw.keep && a.ksw.rejected == b.ksw.rejected && a.ksw.n == b.ksw.n && a.ksw.n_groups == b.ksw.n_groups &&
+           std::memcmp(a.ksw.bits, b.ksw.bits, sizeof(uint32_t) * (size_t)a.ksw.n_groups) == 0 &&
+           std::memcmp(a.ksw.gp, b.ksw.gp, sizeof(GpfParams) * (size_t)a.ksw.n_groups) == 0;
+}
+
+}  // namespace
+
 struct NcclApi {
     void* lib = nullptr;
     ncclResult_t (*GetUniqueId)(ncclUniqueId*) = nullptr;
@@ -100,9 +143,8 @@ struct erasor_ctx {
     size_t   NM = 0, NQ = 0;                   // points of the map-side arrays (node mode: F * n_map) / of the queries
     uint32_t n_chunks_map = 0, n_chunks_qry = 0;
     uint32_t rec_capacity = 0;
-    const float4* cur_map = nullptr;
+    const float4* cur_map = nullptr;           // K1's inputs: erasor_set_inputs's, or the last step's
     const float4* cur_qry = nullptr;
-    bool     qry_xyz = false;                  // the staged query cloud is packed x y z (ERASOR_PTR_QUERY_XYZ, mask modes)
     uint32_t* k1_prof = nullptr;               // set only inside erasor_profile_k1: run_k1 launches K1's profiling build
     std::vector<uint64_t> map_off, qry_off;
     int      desc_mode = -1;                   // mode the uploaded chunk descriptors were built for (-1: none; 0 cloud, 1 batch masks, 2 node masks)
@@ -110,22 +152,17 @@ struct erasor_ctx {
     int      stat_F = 0;                       // frames of the last batch call (all its sub-batches): extent of the per-frame counters
     int      f0 = 0;                           // first frame of the sub-batch being submitted
     std::vector<uint32_t> node_nvoi;           // node mode: |map_voi_| of the frames before f0 (the count tables hold the last sub-batch only)
-    struct StepGraph { const void* ptr[8]; size_t fold_n; int kind, mode, f0; uint64_t epoch, alloc; cudaGraphExec_t exec;
-                       const void* vkeep; int nv; SrtVariant var[kMaxSweepVariants]; K4Sweep gf; };   // vkeep / nv / var / gf: a sweep's
-                                                                                                      // masks, variants and ground-filter groups
-    std::vector<StepGraph> graphs;             // captured mask-mode steps, one per (pointers, geometry)
+    struct StepGraph { Step step; uint64_t desc_epoch, alloc_epoch; cudaGraphExec_t exec; uint64_t kernel_nodes; };
+    std::vector<StepGraph> graphs;             // captured mask-mode steps (same_step, and the epochs they were captured at)
     bool     use_graphs = true;
     int      ctas_per_sm = 4;                  // K1 / K2 grid target: one wave of sm_count * ctas_per_sm CTAs (ERASOR_B200_CTAS_PER_SM)
     bool     fused_srt = true;                 // mask modes: Scan Ratio Test inside the scatter kernel (ERASOR_B200_UNFUSED_SRT=1: separate k3_srt)
-    uint64_t graph_kernel_nodes = 0;
     bool     pending = false;                  // an asynchronous submission has not been waited for yet
     // R-GPF class C (bins beyond 2560 points) is launched only while such bins are being seen (its CTAs need whole SMs even to
     // find their queue empty, which serialises overlapped submissions); if one turns up unannounced, erasor_wait runs the class.
     int      class_c_state = -1;               // -1 unknown (launch it), 0 none in the last run, > 0 seen
     uint32_t class_c_count_host = 0;           // queue[kBucketC0] of the submission in flight
-    struct { bool with_c = true, host = false; int mode = 1; uint8_t* d_keep = nullptr; uint8_t* user_keep = nullptr; size_t n_keep = 0;
-             uint8_t* keep_out = nullptr; size_t n_map_global = 0; K4Fold fold{nullptr, nullptr, 0u, 0u};
-             bool sweep = false; K4Sweep ksweep{}; } last;
+    Step     last;                             // the last mask-mode submission
     int      sweep_V = 0;                      // variants of the last node call when it was a sweep (erasor_get_sweep_stats), else 0
 
     // node mode
@@ -330,8 +367,9 @@ int prepare_batch(erasor_ctx* h, const uint64_t* map_off, const uint64_t* qry_of
     return ERASOR_OK;
 }
 
-// one caller cloud -> device pointer (staged through `stage` when it lives in host memory)
-int stage_cloud(erasor_ctx* h, DeviceBuffer& stage, const float* xyzi, size_t n, int ptr_kind, const float4** out, size_t bytes_per_point = sizeof(float4)) {
+// one caller cloud -> the device pointer the kernels read: the cloud itself (device memory) or its staging buffer (host memory,
+// copied in by stage_host_clouds)
+int device_cloud(erasor_ctx* h, DeviceBuffer& stage, const float* xyzi, size_t n, int ptr_kind, const float4** out, size_t bytes_per_point = sizeof(float4)) {
     if (ptr_kind == ERASOR_PTR_DEVICE) {
         const uintptr_t align = bytes_per_point == sizeof(float4) ? 15 : 3;
         if (n && (reinterpret_cast<uintptr_t>(xyzi) & align)) { h->err = "device clouds must be 16-byte aligned (float4; packed xyz: 4-byte)"; return ERASOR_E_INVALID; }
@@ -339,15 +377,16 @@ int stage_cloud(erasor_ctx* h, DeviceBuffer& stage, const float* xyzi, size_t n,
         return ERASOR_OK;
     }
     CK(stage.ensure(sizeof(float4) * std::max<size_t>(n, 1)));
-    if (n) CK(cudaMemcpyAsync(stage.p(), xyzi, bytes_per_point * n, cudaMemcpyHostToDevice, h->stream));
     *out = stage.as<float4>();
     return ERASOR_OK;
 }
 
-int stage_inputs(erasor_ctx* h, const float* map_xyzi, const float* qry_xyzi, int ptr_kind) {
-    int rc;
-    if ((rc = stage_cloud(h, h->d_map_in, map_xyzi, h->NM, ptr_kind, &h->cur_map))) return rc;
-    return stage_cloud(h, h->d_qry_in, qry_xyzi, h->NQ, ptr_kind, &h->cur_qry, h->qry_xyz ? 3 * sizeof(float) : sizeof(float4));
+// host clouds into their staging buffers (map_xyzi null: node mode, whose map is resident)
+int stage_host_clouds(erasor_ctx* h, int ptr_kind, const float* map_xyzi, const float* qry_xyzi, size_t qry_bytes_per_point) {
+    if (ptr_kind == ERASOR_PTR_DEVICE) return ERASOR_OK;
+    if (map_xyzi && h->NM) CK(cudaMemcpyAsync(h->d_map_in.p(), map_xyzi, sizeof(float4) * h->NM, cudaMemcpyHostToDevice, h->stream));
+    if (h->NQ) CK(cudaMemcpyAsync(h->d_qry_in.p(), qry_xyzi, qry_bytes_per_point * h->NQ, cudaMemcpyHostToDevice, h->stream));
+    return ERASOR_OK;
 }
 
 int run_k1(erasor_ctx* h, int mode) {
@@ -365,7 +404,7 @@ int run_k1(erasor_ctx* h, int mode) {
                      h->d_bin_map.as<uint16_t>(), h->d_bin_qry.as<uint16_t>(), h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(),
                      h->d_zmax.as<uint32_t>(), h->d_cnt.as<uint32_t>(), B, F, h->d_fence.as<unsigned long long>(),
                      mode == 2 ? h->d_poses.as<NodePose>() : nullptr, mode == 2 ? h->d_list_idx.as<uint32_t>() : nullptr,
-                     mode == 2 ? h->d_list_cnt.as<uint32_t>() : nullptr, mode != 0 && h->qry_xyz, mode == 2 ? h->k1_prof : nullptr));
+                     mode == 2 ? h->d_list_cnt.as<uint32_t>() : nullptr, mode != 0 && h->last.qry_xyz, mode == 2 ? h->k1_prof : nullptr));
     }
     return ERASOR_OK;
 }
@@ -440,8 +479,8 @@ int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_
         CK(cudaStreamWaitEvent(h->stream_b, h->ev_fork, 0));
         if (with_c) CK(cudaStreamWaitEvent(h->stream_c, h->ev_fork, 0));
         CK(launch_k4(h->stream_a, h->stream_b, h->stream_c, gp, h->d_recs.as<FlagRec>(), h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->rec_capacity,
-                     h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), h->cur_map,
-                     h->d_frame_off.as<uint32_t>(), (mode == 0 || inserts_on(h, mode)) ? h->d_part.as<float4>() : nullptr, keep_mask, ground_mask,
+                     h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), h->d_frame_off.as<uint32_t>(),
+                     (mode == 0 || inserts_on(h, mode)) ? h->d_part.as<float4>() : nullptr, keep_mask, ground_mask,
                      h->d_frame_rej.as<uint32_t>() + h->f0, h->d_scratch.as<unsigned char>(), h->sm_count, h->d_fence.as<unsigned long long>(), fold, classes, k4sweep));
         CK(cudaEventRecord(h->ev_join_a, h->stream_a));
         CK(cudaEventRecord(h->ev_join_b, h->stream_b));
@@ -673,12 +712,13 @@ int erasor_set_inputs(erasor_handle_t h, const float* map_voi_xyzi, size_t n_map
     h->stage = 0;
     h->f0 = 0; h->stat_F = 1;
     h->ins_call_off.clear();                   // the inserts of an earlier node call end with this submission
-    h->qry_xyz = false;
     if (ptr_kind != ERASOR_PTR_HOST && ptr_kind != ERASOR_PTR_DEVICE) { h->err = "erasor_set_inputs: ptr_kind must be HOST or DEVICE (the cloud outputs carry the query's intensity)"; return ERASOR_E_INVALID; }
     const uint64_t mo[2] = {0, n_map}, qo[2] = {0, n_query};
     rc = prepare_batch(h, mo, qo, 1, 0);
     if (rc) return rc;
-    if ((rc = stage_inputs(h, map_voi_xyzi, query_voi_xyzi, ptr_kind))) return rc;
+    if ((rc = device_cloud(h, h->d_map_in, map_voi_xyzi, h->NM, ptr_kind, &h->cur_map)) ||
+        (rc = device_cloud(h, h->d_qry_in, query_voi_xyzi, h->NQ, ptr_kind, &h->cur_qry)) ||
+        (rc = stage_host_clouds(h, ptr_kind, map_voi_xyzi, query_voi_xyzi, sizeof(float4)))) return rc;
     if ((rc = run_k1(h, 0))) return rc;
     h->stage = 1;
     return ERASOR_OK;
@@ -920,186 +960,140 @@ int erasor_get_fence_counts(erasor_handle_t h, uint64_t* negzero_points, uint64_
 
 namespace {
 
-// One submission of a mask mode: a batch of (map_voi, query_voi) pairs (mode 1) or of nodes against the resident map (mode 2).
-struct Submit {
-    int mode = 1;
-    const float*    map_xyzi = nullptr;     // mode 1
-    const uint64_t* map_off = nullptr;      // mode 1: caller's offsets; mode 2: {0, n_map, 2 n_map, ...}
-    const float*    qry_xyzi = nullptr;
-    const uint64_t* qry_off = nullptr;
-    int             F = 0;
-    uint8_t*        keep_mask = nullptr;    // mode 1: one byte per VoI point; mode 2: frame_keep [F][n_map] (nullable)
-    int             ptr_kind = ERASOR_PTR_HOST;
-    bool            qry_xyz = false;        // the query cloud is packed x y z (ERASOR_PTR_QUERY_XYZ)
-    const uint32_t* fold_index = nullptr;   // mode 1 fold (nullable)
-    uint8_t*        fold_global = nullptr;
-    size_t          fold_n = 0;
-    const NodePose* poses = nullptr;        // mode 2: host array [F]
-    const double*   poses7 = nullptr;       // mode 2: the caller's odom7 of these frames (the inserts' body -> origin)
-    uint8_t*        keep_out = nullptr;     // mode 2 (nullable)
-    int             f0 = 0;                 // index of the first frame within the caller's batch (per-frame counters)
-    const SrtVariant* variants = nullptr;   // mode 2: a sweep of n_variants settings into variant_keep [V][n_map]: their Scan Ratio
-    int             n_variants = 0;         // Test fields, and their ground-filter groups (groups->n_groups, bits, gp)
-    uint8_t*        variant_keep = nullptr;
-    const K4Sweep*  groups = nullptr;
-};
-
 bool is_pinned_host(const void* p) {
     cudaPointerAttributes a{};
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
     return a.type == cudaMemoryTypeHost;
 }
 
-// Enqueue one submission on the handle's stream (CUDA graph when possible) and return without waiting.
-// The whole step (copies, memset, K1, K3, K2, the three concurrent K4 classes with the fold in their epilogue, mask /
-// counter read-back) is a fixed launch sequence once the batch geometry and the buffers are known: it is captured into a
-// CUDA graph the first time and replayed afterwards (one launch instead of ~15 API calls).
-int submit(erasor_ctx* h, const Submit& S) {
+// the step's masks back to the caller: a host caller's per-frame masks from their staging, and the map's mask into keep_out
+int copy_masks_out(erasor_ctx* h, const Step& s) {
+    const bool host = s.ptr_kind != ERASOR_PTR_DEVICE;
+    if (host && s.n_keep) CK(cudaMemcpyAsync(s.user_keep, s.d_keep, s.n_keep, cudaMemcpyDeviceToHost, h->stream));
+    if (s.keep_out && s.n_map_global)
+        CK(cudaMemcpyAsync(s.keep_out, s.map->d_keep.as<uint8_t>(), s.n_map_global, host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, h->stream));
+    return ERASOR_OK;
+}
+
+// Enqueue one step on the handle's stream without waiting: copies, memsets, K1, K3, K2, the three concurrent K4 classes with the
+// fold in their epilogue, the node inserts, the mask / counter read-back.  Once the batch geometry and the buffers are known this
+// is a fixed launch sequence, so submit() captures it into a CUDA graph the first time and replays it afterwards (one launch
+// instead of ~15 API calls).
+int enqueue(erasor_ctx* h, const Step& s) {
+    int rc;
+    if ((rc = stage_host_clouds(h, s.ptr_kind, s.mode == 1 ? s.map_xyzi : nullptr, s.qry_xyzi, s.qry_xyz ? 3 * sizeof(float) : sizeof(float4)))) return rc;
+    if (s.mode == 2) CK(cudaMemcpyAsync(h->d_poses.p(), h->h_pose.p(), sizeof(NodePose) * (size_t)h->F, cudaMemcpyHostToDevice, h->stream));
+    if (s.n_keep) CK(cudaMemsetAsync(s.d_keep, 1, s.n_keep, h->stream));
+    if (s.ssw.n) {
+        CK(cudaMemsetAsync(s.ssw.n_flagged, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
+        CK(cudaMemsetAsync(s.ksw.rejected, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
+    }
+    if ((rc = run_k1(h, s.mode))) return rc;
+    if ((rc = run_compare(h, h->p.version, s.mode, s.d_keep, nullptr, s.fold, s.with_c ? 7 : 3, false, s.ssw.n ? &s.ssw : nullptr,
+                          s.ssw.n ? &s.ksw : nullptr))) return rc;
+    if (s.inserts && (rc = run_insert_assemble(h))) return rc;      // (run_compare ran the plan and the query scatter under R-GPF)
+    CK(cudaMemcpyAsync(h->h_words.as<uint32_t>() + 1, h->d_queue.as<uint32_t>() + kBucketC0, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    if ((rc = copy_masks_out(h, s))) return rc;
+    CK(cudaMemcpyAsync(h->h_words.as<uint32_t>(), h->d_nrecs.p(), sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    return ERASOR_OK;
+}
+
+// The graph of step s at the handle's current epochs: the cached one, or one captured now.  *out stays null when capture is not
+// possible here, which turns graphs off for the handle.
+int step_graph(erasor_ctx* h, const Step& s, const erasor_ctx::StepGraph** out) {
+    *out = nullptr;
+    for (const auto& g : h->graphs)
+        if (g.desc_epoch == h->desc_epoch && g.alloc_epoch == h->alloc_epoch && same_step(g.step, s)) { *out = &g; return ERASOR_OK; }
+    // drop graphs of older geometries, bound the cache
+    for (size_t i = 0; i < h->graphs.size();) {
+        if (h->graphs[i].desc_epoch != h->desc_epoch || h->graphs[i].alloc_epoch != h->alloc_epoch || h->graphs.size() > 64) { cudaGraphExecDestroy(h->graphs[i].exec); h->graphs.erase(h->graphs.begin() + i); }
+        else ++i;
+    }
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    const uint64_t launches_before = h->launches, alloc_epoch = h->alloc_epoch;
+    CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeRelaxed));
+    const int rc = enqueue(h, s);
+    const uint64_t kernel_nodes = h->launches - launches_before;   // init, K1, K3, K2, K4 classes, inserts
+    h->launches = launches_before;                                  // captured, not launched
+    const cudaError_t ce = cudaStreamEndCapture(h->stream, &graph);
+    if (rc == ERASOR_OK && ce == cudaSuccess && graph && h->alloc_epoch == alloc_epoch && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
+        h->graphs.push_back({s, h->desc_epoch, alloc_epoch, exec, kernel_nodes});
+        *out = &h->graphs.back();
+    } else {
+        cudaGetLastError();
+        h->use_graphs = false;                                      // capture not possible here: plain launches for good
+    }
+    if (graph) cudaGraphDestroy(graph);
+    return ERASOR_OK;
+}
+
+// Complete the caller's step (map_off / qry_off / F: the batch geometry; mode 2: poses [F] and the caller's poses7 of these
+// frames) and enqueue it: as a replay of the graph captured from an equal step, a new capture, or plain launches.
+int submit(erasor_ctx* h, Step st, const uint64_t* map_off, const uint64_t* qry_off, int F, const NodePose* poses = nullptr, const double* poses7 = nullptr) {
     int rc;
     CK(cudaSetDevice(h->device));
     if (h->pending && (rc = erasor_wait(h))) return rc;      // one submission in flight per handle (buffers and staging are reused)
     h->stage = 0;
-    h->f0 = S.f0;
-    h->qry_xyz = S.qry_xyz;
-    if ((rc = prepare_batch(h, S.map_off, S.qry_off, S.F, S.mode))) return rc;
-    const bool host = S.ptr_kind != ERASOR_PTR_DEVICE;
-    const size_t n_keep = S.keep_mask ? h->NM : 0;          // bytes of the per-frame mask output
-    const size_t n_map_global = S.mode == 2 ? h->map->n : 0;
-    if (S.mode == 1 && ((h->NM && !S.map_xyzi) || (h->NQ && !S.qry_xyzi))) { h->err = "null cloud"; return ERASOR_E_INVALID; }
-    if (S.mode == 2 && h->NQ && !S.qry_xyzi) { h->err = "null cloud"; return ERASOR_E_INVALID; }
-    if (host) {
-        if (n_keep) CK(h->d_keep.ensure(std::max<size_t>(n_keep, 1)));
-        if (S.mode == 1) CK(h->d_map_in.ensure(sizeof(float4) * std::max<size_t>(h->NM, 1)));
-        CK(h->d_qry_in.ensure(sizeof(float4) * std::max<size_t>(h->NQ, 1)));
+    h->f0 = st.f0;
+    if ((rc = prepare_batch(h, map_off, qry_off, F, st.mode))) return rc;
+    if (st.mode == 1 && ((h->NM && !st.map_xyzi) || (h->NQ && !st.qry_xyzi))) { h->err = "null cloud"; return ERASOR_E_INVALID; }
+    if (st.mode == 2 && h->NQ && !st.qry_xyzi) { h->err = "null cloud"; return ERASOR_E_INVALID; }
+    st.inserts = inserts_on(h, st.mode);
+    st.with_c = h->class_c_state != 0;
+    const bool host = st.ptr_kind != ERASOR_PTR_DEVICE;
+    if (st.mode == 2) {
+        st.map = h->map; st.n_map_global = h->map->n; st.cur_map = h->map->d_pts.as<const float4>();
+    } else if ((rc = device_cloud(h, h->d_map_in, st.map_xyzi, h->NM, st.ptr_kind, &st.cur_map))) {
+        return rc;
     }
-    if (S.mode == 2) {
-        if (sizeof(NodePose) * (size_t)S.F > h->h_pose.cap()) h->alloc_epoch++;      // captured graphs copy from this staging buffer
-        CK(h->h_pose.ensure(sizeof(NodePose) * (size_t)S.F));
-        std::memcpy(h->h_pose.p(), S.poses, sizeof(NodePose) * (size_t)S.F);
+    if ((rc = device_cloud(h, h->d_qry_in, st.qry_xyzi, h->NQ, st.ptr_kind, &st.cur_qry, st.qry_xyz ? 3 * sizeof(float) : sizeof(float4)))) return rc;
+    st.n_keep = st.user_keep ? h->NM : 0;
+    if (st.n_keep) {
+        if (host) CK(h->d_keep.ensure(st.n_keep));
+        st.d_keep = host ? h->d_keep.as<uint8_t>() : st.user_keep;
     }
-    const bool ins = inserts_on(h, S.mode);
-    if (ins) {
+    if (st.mode == 2) {
+        if (sizeof(NodePose) * (size_t)F > h->h_pose.cap()) h->alloc_epoch++;      // captured graphs copy from this staging buffer
+        CK(h->h_pose.ensure(sizeof(NodePose) * (size_t)F));
+        std::memcpy(h->h_pose.p(), poses, sizeof(NodePose) * (size_t)F);
+    }
+    if (st.inserts) {
         if ((rc = ensure_insert_buffers(h))) return rc;
-        for (int f = 0; f < S.F; ++f) {
+        for (int f = 0; f < F; ++f) {
             Mat4 T;
-            pose_to_mat(S.poses7 + 7 * (size_t)f, T);       // tf_body2origin_ = geoPose2eigen(odom), as body2origin applies it
+            pose_to_mat(poses7 + 7 * (size_t)f, T);         // tf_body2origin_ = geoPose2eigen(odom), as body2origin applies it
             std::memcpy(h->h_ins_fwd.as<float>() + 12 * (size_t)f, T.m, sizeof(float) * 12);
         }
     }
-    const bool with_c = h->class_c_state != 0;
-    const bool sweep = S.n_variants > 0;
-    SrtSweep ssw{};
-    K4Sweep  ksw{};
-    if (sweep) {
-        const size_t rows = (size_t)kMaxSweepVariants * (size_t)std::max(h->stat_F, h->f0 + S.F);
+    if (st.ssw.n) {
+        const size_t rows = (size_t)kMaxSweepVariants * (size_t)std::max(h->stat_F, h->f0 + F);
         CK(h->d_sweep_flag.ensure(sizeof(uint32_t) * rows));
         CK(h->d_sweep_rej.ensure(sizeof(uint32_t) * rows));
-        std::copy(S.variants, S.variants + S.n_variants, ssw.v);
-        ssw.n = S.n_variants;
-        ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + (size_t)kMaxSweepVariants * S.f0;
-        ksw = *S.groups;
-        ksw.keep = S.variant_keep; ksw.rejected = h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * S.f0; ksw.n = (uint32_t)n_map_global;
+        st.ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + (size_t)kMaxSweepVariants * st.f0;
+        st.ksw.rejected = h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * st.f0;
+        st.ksw.n = (uint32_t)st.n_map_global;
+    } else if (st.mode == 2) {
+        st.fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)st.n_map_global, 0u};   // a sweep leaves the map's mask alone
     }
-    auto enqueue = [&]() -> int {
-        int r;
-        if (S.mode == 1) {
-            if ((r = stage_inputs(h, S.map_xyzi, S.qry_xyzi, S.ptr_kind))) return r;
-        } else {
-            h->cur_map = h->map->d_pts.as<const float4>();
-            if ((r = stage_cloud(h, h->d_qry_in, S.qry_xyzi, h->NQ, S.ptr_kind, &h->cur_qry, S.qry_xyz ? 3 * sizeof(float) : sizeof(float4)))) return r;
-            CK(cudaMemcpyAsync(h->d_poses.p(), h->h_pose.p(), sizeof(NodePose) * (size_t)S.F, cudaMemcpyHostToDevice, h->stream));
-        }
-        uint8_t* d_keep = nullptr;
-        if (n_keep) {
-            d_keep = host ? h->d_keep.as<uint8_t>() : S.keep_mask;
-            CK(cudaMemsetAsync(d_keep, 1, n_keep, h->stream));
-        }
-        if (sweep) {
-            CK(cudaMemsetAsync(ssw.n_flagged, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)S.F, h->stream));
-            CK(cudaMemsetAsync(ksw.rejected, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)S.F, h->stream));
-        }
-        if ((r = run_k1(h, S.mode))) return r;
-        K4Fold fold{nullptr, nullptr, 0u, 0u};
-        if (S.mode == 2 && !sweep) fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};   // a sweep leaves the map's mask alone
-        else if (S.fold_global)    fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
-        if ((r = run_compare(h, h->p.version, S.mode, d_keep, nullptr, fold, with_c ? 7 : 3, false, sweep ? &ssw : nullptr, sweep ? &ksw : nullptr))) return r;
-        if (ins && (r = run_insert_assemble(h))) return r;      // (run_compare ran the plan and the query scatter under R-GPF)
-        h->last.with_c = with_c; h->last.host = host; h->last.mode = S.mode; h->last.d_keep = d_keep; h->last.user_keep = S.keep_mask; h->last.n_keep = n_keep;
-        h->last.keep_out = S.keep_out; h->last.n_map_global = n_map_global; h->last.fold = fold;
-        CK(cudaMemcpyAsync(h->h_words.as<uint32_t>() + 1, h->d_queue.as<uint32_t>() + kBucketC0, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-        if (host && n_keep) CK(cudaMemcpyAsync(S.keep_mask, d_keep, n_keep, cudaMemcpyDeviceToHost, h->stream));
-        if (S.keep_out && n_map_global)
-            CK(cudaMemcpyAsync(S.keep_out, h->map->d_keep.as<uint8_t>(), n_map_global, host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->h_words.as<uint32_t>(), h->d_nrecs.p(), sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-        return ERASOR_OK;
-    };
+    h->last = st;                                            // erasor_wait and erasor_profile_k1 read the step that ran, replayed or not
+    h->cur_map = st.cur_map; h->cur_qry = st.cur_qry;
     bool graphable = h->use_graphs && !h->timing;
     if (graphable && host) {
         // host buffers must be pinned for copies to be capturable
-        if (S.mode == 1 && h->NM && !is_pinned_host(S.map_xyzi)) graphable = false;
-        if (h->NQ && !is_pinned_host(S.qry_xyzi)) graphable = false;
-        if (n_keep && !is_pinned_host(S.keep_mask)) graphable = false;
-        if (S.keep_out && n_map_global && !is_pinned_host(S.keep_out)) graphable = false;
+        if (st.mode == 1 && h->NM && !is_pinned_host(st.map_xyzi)) graphable = false;
+        if (h->NQ && !is_pinned_host(st.qry_xyzi)) graphable = false;
+        if (st.n_keep && !is_pinned_host(st.user_keep)) graphable = false;
+        if (st.keep_out && st.n_map_global && !is_pinned_host(st.keep_out)) graphable = false;
     }
-    if (graphable) {
-        erasor_ctx::StepGraph key{};
-        key.ptr[0] = S.map_xyzi; key.ptr[1] = S.qry_xyzi; key.ptr[2] = S.keep_mask; key.ptr[3] = S.fold_index; key.ptr[4] = S.fold_global;
-        key.ptr[5] = S.keep_out; key.ptr[6] = S.mode == 2 ? (const void*)h->map : nullptr; key.ptr[7] = with_c ? (const void*)h : nullptr;
-        key.fold_n = S.fold_n; key.kind = S.ptr_kind | (S.qry_xyz ? ERASOR_PTR_QUERY_XYZ : 0) | (ins ? 0x100 : 0); key.mode = S.mode; key.f0 = S.f0; key.epoch = h->desc_epoch; key.alloc = h->alloc_epoch;
-        key.vkeep = S.variant_keep; key.nv = S.n_variants;
-        if (sweep) { std::copy(S.variants, S.variants + S.n_variants, key.var); key.gf = ksw; }
-        auto same = [&](const erasor_ctx::StepGraph& g) {
-            return std::equal(g.ptr, g.ptr + 8, key.ptr) && g.fold_n == key.fold_n && g.kind == key.kind && g.mode == key.mode && g.f0 == key.f0 &&
-                   g.epoch == key.epoch && g.alloc == key.alloc && g.vkeep == key.vkeep && g.nv == key.nv &&
-                   std::memcmp(g.var, key.var, sizeof(SrtVariant) * (size_t)key.nv) == 0 && g.gf.n_groups == key.gf.n_groups &&
-                   std::memcmp(g.gf.bits, key.gf.bits, sizeof(uint32_t) * (size_t)key.gf.n_groups) == 0 &&
-                   std::memcmp(g.gf.gp, key.gf.gp, sizeof(GpfParams) * (size_t)key.gf.n_groups) == 0;
-        };
-        cudaGraphExec_t exec = nullptr;
-        for (auto& g : h->graphs) if (same(g)) exec = g.exec;
-        if (!exec) {
-            // drop graphs of older geometries, bound the cache
-            for (size_t i = 0; i < h->graphs.size();) {
-                if (h->graphs[i].epoch != h->desc_epoch || h->graphs[i].alloc != h->alloc_epoch || h->graphs.size() > 64) { cudaGraphExecDestroy(h->graphs[i].exec); h->graphs.erase(h->graphs.begin() + i); }
-                else ++i;
-            }
-            cudaGraph_t graph = nullptr;
-            const uint64_t launches_before = h->launches;
-            CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeRelaxed));
-            rc = enqueue();
-            h->graph_kernel_nodes = h->launches - launches_before;
-            h->launches = launches_before;                              // captured, not launched
-            cudaError_t ce = cudaStreamEndCapture(h->stream, &graph);
-            if (rc == ERASOR_OK && ce == cudaSuccess && graph && h->alloc_epoch == key.alloc) {
-                ce = cudaGraphInstantiate(&exec, graph, 0);
-                cudaGraphDestroy(graph);
-                if (ce == cudaSuccess) { key.exec = exec; h->graphs.push_back(key); }
-                else exec = nullptr;
-            } else {
-                if (graph) cudaGraphDestroy(graph);
-                exec = nullptr;
-            }
-            if (!exec) { cudaGetLastError(); h->use_graphs = false; }      // capture not possible here: fall back to plain launches for good
-        }
-        if (exec) {
-            CK(cudaGraphLaunch(exec, h->stream));
-            h->launches += h->graph_kernel_nodes;                        // kernel nodes of the graph: init, K1, K3, K2, K4 classes
-        } else if ((rc = enqueue())) {
-            return rc;
-        }
+    const erasor_ctx::StepGraph* g = nullptr;
+    if (graphable && (rc = step_graph(h, st, &g))) return rc;
+    if (g) {
+        CK(cudaGraphLaunch(g->exec, h->stream));
+        h->launches += g->kernel_nodes;
     } else {
         Scope whole(h, 0);
-        if ((rc = enqueue())) return rc;
-    }
-    {   // what erasor_wait needs for the class-C fix-up (set here as well: a replayed graph does not run enqueue())
-        const bool hst = S.ptr_kind != ERASOR_PTR_DEVICE;
-        h->last.with_c = with_c; h->last.host = hst; h->last.mode = S.mode; h->last.user_keep = S.keep_mask; h->last.n_keep = n_keep;
-        h->last.d_keep = n_keep ? (hst ? h->d_keep.as<uint8_t>() : S.keep_mask) : nullptr;
-        h->last.keep_out = S.keep_out; h->last.n_map_global = n_map_global;
-        if (S.mode == 2 && !sweep) h->last.fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)n_map_global, 0u};
-        else if (S.fold_global)    h->last.fold = K4Fold{S.fold_global, S.fold_index, (uint32_t)std::min<size_t>(S.fold_n, 0xFFFFFFFFu), 0u};
-        else                       h->last.fold = K4Fold{nullptr, nullptr, 0u, 0u};
-        h->last.sweep = sweep; h->last.ksweep = ksw;
+        if ((rc = enqueue(h, st))) return rc;
     }
     h->pending = true;
     return ERASOR_OK;
@@ -1131,21 +1125,21 @@ int process_frames_impl(erasor_handle_t h, const float* map_xyzi, const uint64_t
     for (int f0 = 0; f0 < n_frames;) {
         const int f1 = sub_batch_end(h, map_offsets, query_offsets, f0, n_frames);
         if (f1 == f0) { h->err = "a single frame exceeds 2^32 points"; return ERASOR_E_INVALID; }
-        Submit S;
-        S.mode = 1; S.F = f1 - f0; S.ptr_kind = ptr_kind; S.f0 = f0; S.qry_xyz = qxyz;
         const uint64_t m0 = map_offsets[f0], q0 = query_offsets[f0];
-        if (f0 == 0 && f1 == n_frames) { S.map_off = map_offsets; S.qry_off = query_offsets; }
-        else {
+        const uint64_t *mof = map_offsets, *qof = query_offsets;
+        if (f0 != 0 || f1 != n_frames) {
             mo.assign(map_offsets + f0, map_offsets + f1 + 1); qo.assign(query_offsets + f0, query_offsets + f1 + 1);
             for (auto& v : mo) v -= m0;
             for (auto& v : qo) v -= q0;
-            S.map_off = mo.data(); S.qry_off = qo.data();
+            mof = mo.data(); qof = qo.data();
         }
-        S.map_xyzi = map_xyzi ? map_xyzi + 4 * m0 : nullptr;
-        S.qry_xyzi = query_xyzi ? query_xyzi + (qxyz ? 3 : 4) * q0 : nullptr;
-        S.keep_mask = keep_mask + m0;
-        S.fold_index = fold_index ? fold_index + m0 : nullptr; S.fold_global = fold_global; S.fold_n = fold_n_global;
-        if ((rc = submit(h, S))) return rc;
+        Step st;
+        st.mode = 1; st.ptr_kind = ptr_kind; st.qry_xyz = qxyz; st.f0 = f0;
+        st.map_xyzi = map_xyzi ? map_xyzi + 4 * m0 : nullptr;
+        st.qry_xyzi = query_xyzi ? query_xyzi + (qxyz ? 3 : 4) * q0 : nullptr;
+        st.user_keep = keep_mask + m0;
+        if (fold_global) st.fold = K4Fold{fold_global, fold_index ? fold_index + m0 : nullptr, (uint32_t)std::min<size_t>(fold_n_global, 0xFFFFFFFFu), 0u};
+        if ((rc = submit(h, st, mof, qof, f1 - f0))) return rc;
         f0 = f1;
         if (f0 < n_frames && (rc = erasor_wait(h))) return rc;      // the next sub-batch reuses the handle's buffers
     }
@@ -1167,7 +1161,7 @@ int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
 
 int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                        double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind, bool async,
-                       const SrtVariant* variants = nullptr, int n_variants = 0, uint8_t* variant_keep = nullptr, const K4Sweep* groups = nullptr) {
+                       const SrtSweep* sweep = nullptr, const K4Sweep* groups = nullptr) {
     if (!h || !poses7 || !query_offsets) { if (h) h->err = "null argument"; return ERASOR_E_INVALID; }
     if (!h->map) { h->err = "erasor_process_nodes: no map attached (erasor_attach_map)"; return ERASOR_E_STATE; }
     if (n_frames <= 0) { h->err = "n_frames must be positive"; return ERASOR_E_INVALID; }
@@ -1183,7 +1177,7 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
     const size_t N = h->map->n;
     const double range = voi_max_range > 0.0 ? voi_max_range : h->p.max_range;
     h->stat_F = n_frames;
-    h->sweep_V = n_variants;
+    h->sweep_V = sweep ? sweep->n : 0;
     h->ins_call_off.assign(h->node_inserts ? 1 : 0, 0);
     // scratch per (frame, map point): bin id 2 + scattered point 16 + source index 4 + class-C scratch 24 bytes; with inserts also
     // R-GPF's partitioned copy 16 + the inserts 16 + K4b's voxels 16 and scratch 36 bytes
@@ -1209,16 +1203,13 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         for (auto& v : qo) v -= q0;
         poses.resize(F);
         for (int f = 0; f < F; ++f) node_pose_of(poses7 + 7 * (size_t)(f0 + f), range, poses[f]);
-        Submit S;
-        S.mode = 2; S.F = F; S.ptr_kind = ptr_kind; S.f0 = f0; S.qry_xyz = qxyz;
-        S.map_off = mo.data(); S.qry_off = qo.data();
-        S.qry_xyzi = query_xyzi ? query_xyzi + (qxyz ? 3 : 4) * q0 : nullptr;
-        S.keep_mask = frame_keep ? frame_keep + (size_t)f0 * N : nullptr;
-        S.poses = poses.data();
-        S.poses7 = poses7 + 7 * (size_t)f0;
-        S.keep_out = (f1 == n_frames) ? keep_out : nullptr;
-        S.variants = variants; S.n_variants = n_variants; S.variant_keep = variant_keep; S.groups = groups;
-        if ((rc = submit(h, S))) return rc;
+        Step st;
+        st.mode = 2; st.ptr_kind = ptr_kind; st.qry_xyz = qxyz; st.f0 = f0;
+        st.qry_xyzi = query_xyzi ? query_xyzi + (qxyz ? 3 : 4) * q0 : nullptr;
+        st.user_keep = frame_keep ? frame_keep + (size_t)f0 * N : nullptr;
+        st.keep_out = (f1 == n_frames) ? keep_out : nullptr;
+        if (sweep) { st.ssw = *sweep; st.ksw = *groups; }
+        if ((rc = submit(h, st, mo.data(), qo.data(), F, poses.data(), poses7 + 7 * (size_t)f0))) return rc;
         if (f1 < n_frames) {                                         // the next sub-batch reuses the handle's buffers
             if ((rc = erasor_wait(h))) return rc;
             h->node_nvoi.resize((size_t)f1);
@@ -1240,19 +1231,17 @@ int erasor_wait(erasor_handle_t h) {
         h->class_c_count_host = h->words()[1];
         if (h->n_recs_host > h->rec_capacity) { h->err = "internal: flagged-bin records overflowed the work queue"; return ERASOR_E_CAPACITY; }
         h->class_c_state = (int)std::min<uint32_t>(h->class_c_count_host, 0x7FFFFFFFu);
-        if (!h->last.with_c && h->class_c_count_host > 0) {
+        const Step& s = h->last;
+        if (!s.with_c && h->class_c_count_host > 0) {
             // bins beyond class B's capacity turned up in a submission that ran without class C: run that class now (R-GPF only; the
             // bins are independent, the masks only gain zeros), then repeat the output copies.  The next submissions launch it up front.
-            int rc = run_compare(h, h->p.version, h->last.mode, h->last.d_keep, nullptr, h->last.fold, 4, true, nullptr,
-                                 h->last.sweep ? &h->last.ksweep : nullptr);
+            int rc = run_compare(h, h->p.version, s.mode, s.d_keep, nullptr, s.fold, 4, true, nullptr, s.ssw.n ? &s.ksw : nullptr);
             if (rc) return rc;
-            if (inserts_on(h, h->last.mode) && (rc = run_insert_assemble(h))) return rc;
-            if (h->last.host && h->last.n_keep) CK(cudaMemcpyAsync(h->last.user_keep, h->last.d_keep, h->last.n_keep, cudaMemcpyDeviceToHost, h->stream));
-            if (h->last.keep_out && h->last.n_map_global)
-                CK(cudaMemcpyAsync(h->last.keep_out, h->map->d_keep.as<uint8_t>(), h->last.n_map_global, h->last.host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, h->stream));
+            if (s.inserts && (rc = run_insert_assemble(h))) return rc;
+            if ((rc = copy_masks_out(h, s))) return rc;
             CK(cudaStreamSynchronize(h->stream));
         }
-        if (inserts_on(h, h->last.mode)) return collect_inserts(h);
+        if (s.inserts) return collect_inserts(h);
     }
     return ERASOR_OK;
 }
@@ -1386,11 +1375,13 @@ int process_nodes_sweep_impl(erasor_handle_t h, const double* poses7, const floa
     if (!h->map) { h->err = "erasor_process_nodes_sweep: no map attached (erasor_attach_map)"; return ERASOR_E_INVALID; }
     if (h->node_inserts) { h->err = "a sweep has no node inserts: erasor_set_node_inserts(h, 0) first"; return ERASOR_E_INVALID; }
     if (h->pending) { h->err = "erasor_process_nodes_sweep while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
-    SrtVariant variants[kMaxSweepVariants];
+    SrtSweep variants{};
     K4Sweep groups{};
+    variants.n = n_settings;
+    groups.keep = variant_keep;
     for (int v = 0; v < n_settings; ++v) {
         const erasor_sweep_setting_t& x = settings[v];
-        variants[v] = SrtVariant{x.scan_ratio_threshold, x.th_bin_max_h, x.minimum_num_pts, 0};
+        variants.v[v] = SrtVariant{x.scan_ratio_threshold, x.th_bin_max_h, x.minimum_num_pts, 0};
         GpfParams gp{};
         gp.th_dist = x.gf_dist_thr; gp.th_seeds = x.gf_th_seeds_height; gp.num_lowest_pts = x.num_lowest_pts;
         gp.num_lpr = x.gf_num_lpr; gp.iters = x.gf_iter; gp.cov_mode = h->p.cov_mode;
@@ -1399,8 +1390,7 @@ int process_nodes_sweep_impl(erasor_handle_t h, const double* poses7, const floa
         if (g == groups.n_groups) groups.gp[groups.n_groups++] = gp;
         groups.bits[g] |= 1u << v;
     }
-    return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, nullptr, nullptr, ptr_kind, async,
-                              variants, n_settings, variant_keep, &groups);
+    return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, nullptr, nullptr, ptr_kind, async, &variants, &groups);
 }
 
 // erasor_process_nodes_sweep: the settings with the handle's ground-filter fields (one group)

@@ -144,7 +144,7 @@ __device__ __forceinline__ bool in_voi_radius(const NodePose& P, float x, float 
 // and are not counted anywhere (they are the reference's map_outskirts_, which never reach ERASOR).
 // PROF: the profiling build behind erasor_profile_k1 -- lane 0 of every warp adds the SM cycles between consecutive phase
 // boundaries of the node-mode map path to its warp's slots (kK1Prof*); with PROF false none of it is compiled.
-template <int THREADS, int UNROLL, bool ROWS, bool NODE, bool PROF = false>
+template <int THREADS, int UNROLL, bool NODE, bool PROF = false>
 __global__ void __launch_bounds__(THREADS, THREADS == 256 ? 4 : 1)      // four 8-warp CTAs per SM (64 registers) or one 32-warp CTA
 k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* __restrict__ qry_pts,
             const ChunkDesc* __restrict__ chunks, uint16_t* __restrict__ bin_map, uint16_t* __restrict__ bin_qry,
@@ -294,14 +294,14 @@ k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* _
     }
     __syncthreads();
 
-    // flush: per-bin count / min / max by RED to the frame tables (non-empty bins only); in cloud mode also the dense
-    // per-chunk count row that K3 turns into prefixes for K2's stable scatter
-    uint32_t* __restrict__ row = ROWS ? ch_cnt + (size_t)blockIdx.x * (B + 1) : nullptr;
+    // flush: per-bin count / min / max by RED to the frame tables (non-empty bins only), and the dense per-chunk count row
+    // that K3 (or the fused scatter) turns into prefixes for K2's stable scatter
+    uint32_t* __restrict__ row = ch_cnt + (size_t)blockIdx.x * (B + 1);
     const size_t ft = ((size_t)cd.cloud * F + cd.frame) * B;
     const size_t ct = ((size_t)cd.cloud * F + cd.frame) * (B + 1);
     for (int i = tid; i <= B; i += THREADS) {
         const uint32_t c = s_cnt[i];
-        if (ROWS) row[i] = c;
+        row[i] = c;
         if (c != 0u) {
             atomicAdd(&cnt_tab[ct + i], c);
             if (i < B) {
@@ -335,44 +335,19 @@ cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map
                       uint32_t* zmin, uint32_t* zmax, uint32_t* cnt_tab, int B, int F, unsigned long long* fence, const NodePose* poses,
                       uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz, uint32_t* prof) {
     if (n_chunks == 0) return cudaSuccess;
-    const int qx = qry_xyz ? 1 : 0;
-    constexpr int UNROLL = 4;
-    const size_t smem = k1_smem_bytes(T.R, B);
-    cudaError_t e;
     if (prof && !poses) return cudaErrorInvalidValue;      // the profiling build covers node mode only
+    constexpr int UNROLL = 4;
     // Bin tables beyond ~56 KB (40 x 360 bins: 173 KB) leave one CTA per SM: give that CTA 32 warps instead of 8, the
     // kernel needs ~32 resident warps per SM to cover its latencies.
-    if (k1_big_tables(T.R, B)) {
-        constexpr int THREADS = 1024;
-        if (prof) {
-            auto kern = k1_rpod_bin<THREADS, UNROLL, true, true, true>;
-            if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-            kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx, prof);
-        } else if (poses) {
-            auto kern = k1_rpod_bin<THREADS, UNROLL, true, true>;
-            if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-            kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx, nullptr);
-        } else {
-            auto kern = k1_rpod_bin<THREADS, UNROLL, true, false>;
-            if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-            kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, nullptr, nullptr, nullptr, qx, nullptr);
-        }
-        return cudaGetLastError();
-    }
-    constexpr int THREADS = 256;
-    if (prof) {
-        auto kern = k1_rpod_bin<THREADS, UNROLL, true, true, true>;
-        if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx, prof);
-    } else if (poses) {
-        auto kern = k1_rpod_bin<THREADS, UNROLL, true, true>;
-        if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses, list_idx, list_cnt, qx, nullptr);
-    } else {
-        auto kern = k1_rpod_bin<THREADS, UNROLL, true, false>;
-        if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks, THREADS, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, nullptr, nullptr, nullptr, qx, nullptr);
-    }
+    const bool big = k1_big_tables(T.R, B);
+    auto kern = prof  ? (big ? k1_rpod_bin<1024, UNROLL, true, true> : k1_rpod_bin<256, UNROLL, true, true>)
+              : poses ? (big ? k1_rpod_bin<1024, UNROLL, true> : k1_rpod_bin<256, UNROLL, true>)
+                      : (big ? k1_rpod_bin<1024, UNROLL, false> : k1_rpod_bin<256, UNROLL, false>);
+    const size_t smem = k1_smem_bytes(T.R, B);
+    cudaError_t e = ensure_dyn_smem(kern, smem);
+    if (e != cudaSuccess) return e;
+    kern<<<n_chunks, big ? 1024 : 256, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses,
+                                                   list_idx, list_cnt, qry_xyz ? 1 : 0, prof);
     return cudaGetLastError();
 }
 
@@ -1050,15 +1025,10 @@ cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const Chun
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
         kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, bin_ids, pts, poses, ch_cnt, zmin, zmax, cnt, frame_off, n_flagged, recs, n_recs,
                                                  rec_capacity, queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps, *sweep);
-    } else if (poses) {
-        auto kern = k2_srt_scatter<W, true>;
+    } else {
+        auto kern = poses ? k2_srt_scatter<W, true> : k2_srt_scatter<W, false>;
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
         kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, bin_ids, pts, poses, ch_cnt, zmin, zmax, cnt, frame_off, n_flagged, recs, n_recs,
-                                                 rec_capacity, queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps);
-    } else {
-        auto kern = k2_srt_scatter<W, false>;
-        if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, bin_ids, pts, nullptr, ch_cnt, zmin, zmax, cnt, frame_off, n_flagged, recs, n_recs,
                                                  rec_capacity, queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps);
     }
     return cudaGetLastError();
@@ -1584,7 +1554,7 @@ struct K4Shared {
 template <int G, bool kShared, bool SWEEP>
 __device__ __forceinline__ void k4_process_bin(const GpfParams& P_handle, FlagRec& rc, unsigned char* base, float* prd, uint32_t* cnt_scratch, K4Shared& sh,
                                                const float4* __restrict__ sorted_pts, uint32_t* __restrict__ sorted_src,
-                                               const float4* __restrict__ in_pts, const uint32_t* __restrict__ frame_off,
+                                               const uint32_t* __restrict__ frame_off,
                                                float4* __restrict__ part_pts, uint8_t* __restrict__ keep_mask,
                                                uint8_t* __restrict__ ground_mask, uint32_t* __restrict__ frame_rejected,
                                                unsigned long long* __restrict__ fence, const K4Fold& fold, const K4Sweep* sweep) {
@@ -1937,15 +1907,15 @@ __device__ __forceinline__ void k4_process_bin(const GpfParams& P_handle, FlagRe
         if constexpr (G <= 256) {                                                                                                           \
             /* classes A and B: the launch sizes the slices for the class maximum (kClassAMax / kClassBMax), so the bin always fits */      \
             k4_process_bin<G, true, SWEEP>(P, rc, smem_raw + (size_t)grp * slice_bytes, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts,        \
-                                           sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,    \
+                                           sorted_src, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,            \
                                            SWEEP_PTR);                                                                                      \
         } else if (n <= smem_cap_points) {                                                                                                  \
             k4_process_bin<G, true, SWEEP>(P, rc, smem_raw + (size_t)grp * slice_bytes, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts,        \
-                                           sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,    \
+                                           sorted_src, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,            \
                                            SWEEP_PTR);                                                                                      \
         } else {                                                                                                                            \
             k4_process_bin<G, false, SWEEP>(P, rc, gscratch + (size_t)rc.src_begin * 24u, s_prd[grp], s_cnt[grp], sh[grp], sorted_pts,      \
-                                            sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,   \
+                                            sorted_src, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, fence, fold,           \
                                             SWEEP_PTR);                                                                                     \
         }                                                                                                                                   \
     }
@@ -1957,7 +1927,7 @@ template <int THREADS, int G>
 __global__ void __launch_bounds__(THREADS, (THREADS == 256) ? 3 : (THREADS == 128 ? 6 : 1))
 k4_rgpf(GpfParams P, FlagRec* __restrict__ recs, uint32_t* __restrict__ queue, const uint32_t* __restrict__ bucket_list,
         uint32_t rec_capacity, int bk0, int bk1, int cls, const float4* __restrict__ sorted_pts, uint32_t* __restrict__ sorted_src,
-        const float4* __restrict__ in_pts, const uint32_t* __restrict__ frame_off /*map cloud [F+1]*/,
+        const uint32_t* __restrict__ frame_off /*map cloud [F+1]*/,
         float4* __restrict__ part_pts /*nullable*/, uint8_t* __restrict__ keep_mask /*nullable*/,
         uint8_t* __restrict__ ground_mask /*nullable*/, uint32_t* __restrict__ frame_rejected /*[F] nullable*/,
         unsigned char* __restrict__ gscratch, uint32_t smem_cap_points, uint32_t slice_bytes,
@@ -1971,7 +1941,7 @@ template <int THREADS, int G>
 __global__ void __launch_bounds__(THREADS, (THREADS == 256) ? 3 : (THREADS == 128 ? 6 : 1))
 k4_rgpf_sweep(GpfParams P, FlagRec* __restrict__ recs, uint32_t* __restrict__ queue, const uint32_t* __restrict__ bucket_list,
               uint32_t rec_capacity, int bk0, int bk1, int cls, const float4* __restrict__ sorted_pts, uint32_t* __restrict__ sorted_src,
-              const float4* __restrict__ in_pts, const uint32_t* __restrict__ frame_off, float4* __restrict__ part_pts,
+              const uint32_t* __restrict__ frame_off, float4* __restrict__ part_pts,
               uint8_t* __restrict__ keep_mask, uint8_t* __restrict__ ground_mask, uint32_t* __restrict__ frame_rejected,
               unsigned char* __restrict__ gscratch, uint32_t smem_cap_points, uint32_t slice_bytes,
               unsigned long long* __restrict__ fence, K4Fold fold, const __grid_constant__ K4Sweep sweep) {
@@ -1982,7 +1952,7 @@ k4_rgpf_sweep(GpfParams P, FlagRec* __restrict__ recs, uint32_t* __restrict__ qu
 template <int THREADS, int G>
 static cudaError_t launch_k4_class(cudaStream_t st, const GpfParams& P, FlagRec* recs, uint32_t* queue, const uint32_t* bucket_list,
                                    uint32_t rec_capacity, int bk0, int bk1, int cls, uint32_t smem_bytes, const float4* sorted_pts,
-                                   uint32_t* sorted_src, const float4* in_pts, const uint32_t* frame_off, float4* part_pts,
+                                   uint32_t* sorted_src, const uint32_t* frame_off, float4* part_pts,
                                    uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected, unsigned char* gscratch, int grid,
                                    unsigned long long* fence, const K4Fold& fold, const K4Sweep* sweep) {
     // per bin: 12 n (xyz) + 4 n (order) + n (flags) = 17 n for warp groups, + 4 n (second half of the order / exchange area, or the
@@ -1996,14 +1966,14 @@ static cudaError_t launch_k4_class(cudaStream_t st, const GpfParams& P, FlagRec*
         auto kern = k4_rgpf_sweep<THREADS, G>;
         cudaError_t e = ensure_dyn_smem(kern, smem_bytes);
         if (e != cudaSuccess) return e;
-        kern<<<grid, THREADS, smem_bytes, st>>>(P, recs, queue, bucket_list, rec_capacity, bk0, bk1, cls, sorted_pts, sorted_src, in_pts, frame_off,
+        kern<<<grid, THREADS, smem_bytes, st>>>(P, recs, queue, bucket_list, rec_capacity, bk0, bk1, cls, sorted_pts, sorted_src, frame_off,
                                                 part_pts, keep_mask, ground_mask, frame_rejected, gscratch, cap, slice, fence, fold, *sweep);
         return cudaGetLastError();
     }
     auto kern = k4_rgpf<THREADS, G>;
     cudaError_t e = ensure_dyn_smem(kern, smem_bytes);
     if (e != cudaSuccess) return e;
-    kern<<<grid, THREADS, smem_bytes, st>>>(P, recs, queue, bucket_list, rec_capacity, bk0, bk1, cls, sorted_pts, sorted_src, in_pts, frame_off,
+    kern<<<grid, THREADS, smem_bytes, st>>>(P, recs, queue, bucket_list, rec_capacity, bk0, bk1, cls, sorted_pts, sorted_src, frame_off,
                                             part_pts, keep_mask, ground_mask, frame_rejected, gscratch, cap, slice, fence, fold);
     return cudaGetLastError();
 }
@@ -2011,7 +1981,7 @@ static cudaError_t launch_k4_class(cudaStream_t st, const GpfParams& P, FlagRec*
 int k4_num_launches(bool with_class_c) { return with_class_c ? 3 : 2; }
 
 cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, const GpfParams& P, FlagRec* recs, uint32_t* queue,
-                      const uint32_t* bucket_list, uint32_t rec_capacity, const float4* sorted_pts, uint32_t* sorted_src, const float4* in_pts,
+                      const uint32_t* bucket_list, uint32_t rec_capacity, const float4* sorted_pts, uint32_t* sorted_src,
                       const uint32_t* frame_off, float4* part_pts, uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected,
                       unsigned char* gscratch, int sm_count, unsigned long long* fence, const K4Fold& fold, int classes, const K4Sweep* sweep) {
     // The three size classes touch disjoint bins, so they run concurrently on three streams (the caller forks / joins).
@@ -2027,13 +1997,13 @@ cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, con
     // runs it afterwards (classes == 4) if one turns up.
     if (classes & 4) {
         e = launch_k4_class<1024, 1024>(st_c, P, recs, queue, bucket_list, rec_capacity, kBucketC0, kBucketB0, 2, 180 * 1024, sorted_pts, sorted_src,
-                                        in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count, fence, fold, sweep);
+                                        frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count, fence, fold, sweep);
         if (e != cudaSuccess) return e;
     }
     if (!(classes & 3)) return cudaSuccess;
     // class B: 512 < n <= 2560, one 128-thread CTA per bin
     e = launch_k4_class<128, 128>(st_b, P, recs, queue, bucket_list, rec_capacity, kBucketB0, kBucketA0, 1, 21 * kClassBMax + 64, sorted_pts,
-                                  sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 3, fence, fold, sweep);
+                                  sorted_src, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 3, fence, fold, sweep);
     if (e != cudaSuccess) return e;
     // class A: n <= 512, one warp per bin, 8 warps per CTA
     // (two CTAs per SM fit by shared memory: with tens of thousands of small flagged bins per step -- 40 x 360 bins, 2 M-point map --
@@ -2043,7 +2013,7 @@ cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, con
     const bool saved_order = sweep && sweep->n_groups > 1;
     return launch_k4_class<256, 32>(st, P, recs, queue, bucket_list, rec_capacity, kBucketA0, kNumBuckets, 0,
                                     8 * ((saved_order ? 21 : 17) * kClassAMax + 48), sorted_pts,
-                                    sorted_src, in_pts, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 2, fence, fold, sweep);
+                                    sorted_src, frame_off, part_pts, keep_mask, ground_mask, frame_rejected, gscratch, sm_count * 2, fence, fold, sweep);
 }
 
 // ============================================================================================

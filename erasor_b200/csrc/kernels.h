@@ -56,11 +56,10 @@ cudaError_t launch_k2_both(cudaStream_t st, const ChunkDesc* chunks, uint32_t n_
                            const uint16_t* bin_qry, const float4* qry_pts, const uint32_t* dst_start_qry, float4* out_qry, uint32_t* src_qry);
 
 int k4_num_launches(bool with_class_c);
-// sorted_pts / sorted_src: K2's output (bins contiguous in source order + source index of every slot); in_pts is unused
-// since K2 also serves mask mode, kept in the signature for ABI stability of the launch wrapper.
+// sorted_pts / sorted_src: K2's output (bins contiguous in source order + source index of every slot).
 // queue / bucket_list: the size-bucketed work queue K3 filled (device_types.h).
 cudaError_t launch_k4(cudaStream_t st, cudaStream_t st_b, cudaStream_t st_c, const GpfParams& P, FlagRec* recs, uint32_t* queue,
-                      const uint32_t* bucket_list, uint32_t rec_capacity, const float4* sorted_pts, uint32_t* sorted_src, const float4* in_pts, const uint32_t* frame_off,
+                      const uint32_t* bucket_list, uint32_t rec_capacity, const float4* sorted_pts, uint32_t* sorted_src, const uint32_t* frame_off,
                       float4* part_pts, uint8_t* keep_mask, uint8_t* ground_mask, uint32_t* frame_rejected, unsigned char* gscratch,
                       int sm_count, unsigned long long* fence, const K4Fold& fold, int classes /*bit 0|1: A and B, bit 2: C*/,
                       const K4Sweep* sweep = nullptr /*a sweep's ground-filter groups and per-setting fold (node mode, records from k2_srt_sweep_scatter)*/);
