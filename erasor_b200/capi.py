@@ -31,7 +31,7 @@ EXPORTS = [
     "erasor_map_create", "erasor_map_destroy", "erasor_map_size", "erasor_map_reset_keep", "erasor_map_get_keep", "erasor_map_keep_device",
     "erasor_map_points_device", "erasor_attach_map", "erasor_process_nodes", "erasor_process_nodes_async", "erasor_get_node_stats",
     "erasor_process_nodes_sweep", "erasor_process_nodes_sweep_async", "erasor_get_sweep_stats",
-    "erasor_process_nodes_sweep_ex", "erasor_process_nodes_sweep_ex_async",
+    "erasor_process_nodes_sweep_ex", "erasor_process_nodes_sweep_ex_async", "erasor_process_nodes_tune", "erasor_process_nodes_tune_async",
     "erasor_voxelize_batch",
     "erasor_set_node_inserts", "erasor_get_node_inserts", "erasor_map_append_inserts", "erasor_map_inserts", "erasor_map_clear_inserts",
     "erasor_save_node_map",
@@ -74,6 +74,19 @@ class SweepSettingC(ctypes.Structure):
     """erasor_sweep_setting_t"""
     _fields_ = [(name, c_double) for name in ("scan_ratio_threshold", "th_bin_max_h", "gf_dist_thr", "gf_th_seeds_height")] + \
                [(name, c_int) for name in ("minimum_num_pts", "num_lowest_pts", "gf_num_lpr", "gf_iter")]
+
+
+GEOMETRY_SWEEP_FIELDS = ("max_range", "num_rings", "num_sectors", "min_h", "max_h")    # ERASOR's polar geometry and z window, added by tune
+
+
+class GeometryC(ctypes.Structure):
+    """erasor_geometry_t"""
+    _fields_ = [(name, c_double) for name in ("max_range", "min_h", "max_h")] + [(name, c_int) for name in ("num_rings", "num_sectors")]
+
+
+class TuneSettingC(ctypes.Structure):
+    """erasor_tune_setting_t"""
+    _fields_ = [("geometry", GeometryC), ("s", SweepSettingC)]
 
 
 class PcdInfoC(ctypes.Structure):
@@ -202,6 +215,8 @@ def _load():
     L.erasor_process_nodes_sweep_async.argtypes = L.erasor_process_nodes_sweep.argtypes
     L.erasor_process_nodes_sweep_ex.argtypes = L.erasor_process_nodes_sweep.argtypes[:6] + [POINTER(SweepSettingC)] + L.erasor_process_nodes_sweep.argtypes[7:]
     L.erasor_process_nodes_sweep_ex_async.argtypes = L.erasor_process_nodes_sweep_ex.argtypes
+    L.erasor_process_nodes_tune.argtypes = L.erasor_process_nodes_sweep.argtypes[:6] + [POINTER(TuneSettingC)] + L.erasor_process_nodes_sweep.argtypes[7:]
+    L.erasor_process_nodes_tune_async.argtypes = L.erasor_process_nodes_tune.argtypes
     L.erasor_get_sweep_stats.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32)]
     L.erasor_voxelize_batch.argtypes = [c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p, c_float, POINTER(c_double), c_int,
                                         POINTER(c_void_p), POINTER(c_uint64)]
@@ -603,6 +618,27 @@ class Handle(_Native):
         section 8.6); arguments as process_nodes_sweep, settings as sweep_settings takes them."""
         arr, V = self.sweep_settings(settings)
         fn = self.L.erasor_process_nodes_sweep_ex_async if asynchronous else self.L.erasor_process_nodes_sweep_ex
+        self._sweep(fn, poses7, query_xyzi, query_offsets, arr, V, keep_ptr, voi_max_range, packed_xyz)
+
+    def tune_settings(self, settings):
+        """settings (dicts or objects with any of SRT_SWEEP_FIELDS + GF_SWEEP_FIELDS + GEOMETRY_SWEEP_FIELDS; a missing field takes
+        the handle's value) -> TuneSettingC array"""
+        ss = list(settings)
+        arr = (TuneSettingC * max(len(ss), 1))()
+        for i, v in enumerate(ss):
+            get = v.get if isinstance(v, dict) else (lambda k, d, v=v: getattr(v, k, d))
+            for part, ctype in ((arr[i].geometry, GeometryC), (arr[i].s, SweepSettingC)):
+                for name, typ in ctype._fields_:
+                    setattr(part, name, (float if typ is c_double else int)(get(name, getattr(self.params, name))))
+        return arr, len(ss)
+
+    def process_nodes_tune(self, poses7, query_xyzi, query_offsets, settings, keep_ptr: int, voi_max_range: float = 0.0,
+                           packed_xyz: bool = False, asynchronous: bool = False):
+        """erasor_process_nodes_tune: process_nodes_sweep_ex over settings that may also vary GEOMETRY_SWEEP_FIELDS (DESIGN.md
+        section 8.7); arguments as process_nodes_sweep, settings as tune_settings takes them.  voi_max_range <= 0 takes the
+        settings' common max_range (refused when they differ)."""
+        arr, V = self.tune_settings(settings)
+        fn = self.L.erasor_process_nodes_tune_async if asynchronous else self.L.erasor_process_nodes_tune
         self._sweep(fn, poses7, query_xyzi, query_offsets, arr, V, keep_ptr, voi_max_range, packed_xyz)
 
     def _sweep(self, fn, poses7, query_xyzi, query_offsets, arr, V, keep_ptr, voi_max_range, packed_xyz):

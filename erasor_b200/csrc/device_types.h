@@ -99,6 +99,27 @@ struct K4Sweep {
     GpfParams gp[kMaxSweepVariants];
 };
 
+// Geometry sweeps (erasor_process_nodes_tune, DESIGN.md section 8.7): K1's geometry form bins every VoI point of the node batch
+// under n geometries in one scan of the resident map.  Geometry g's polar tables are T, its outputs the arrays of one plain
+// node-mode K1 launch with B bins, and its shared count / min / max tables the k1_smem_bytes(T.R, B) bytes at smem_off in the
+// launch's dynamic shared memory.  Passed as a __grid_constant__ kernel parameter.
+struct K1GeoTables {
+    BinTablesView T;
+    uint16_t*     bin_map;         // per dense VoI-list entry, as the plain launch writes them
+    uint16_t*     bin_qry;
+    uint32_t*     ch_cnt;          // [n_chunks][B + 1]
+    uint32_t*     zmin;            // [2][F][B]
+    uint32_t*     zmax;
+    uint32_t*     cnt;             // [2][F][B + 1]
+    int           B;
+    uint32_t      smem_off;        // 16-byte aligned
+};
+struct K1Geo {
+    K1GeoTables g[kMaxSweepVariants];
+    int         n;                 // geometries of the launch, 1..32
+    int         pad_;
+};
+
 // The multi-GPU fold, done in K4's epilogue: global_keep[index ? index[frame_base + src] : src] = 0 for every rejected point.
 struct K4Fold {
     uint8_t*        keep;      // global keep mask of the map (null: no fold)

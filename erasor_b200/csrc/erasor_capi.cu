@@ -11,6 +11,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -55,6 +56,8 @@ namespace {
 // chunk descriptors (whose changes alloc_epoch and desc_epoch track).  The caller fills in the first part, submit() the rest.  A
 // captured graph replays the step it was captured from, so the graph cache is keyed on it; erasor_wait's class-C fix-up and
 // erasor_profile_k1 read the last one.
+struct TunePlan;
+
 struct Step {
     int           mode = 1;                   // 1: batch of (map_voi, query_voi) pairs, 2: nodes against the resident map
     int           ptr_kind = ERASOR_PTR_HOST; // of the caller's buffers: HOST or DEVICE
@@ -67,6 +70,7 @@ struct Step {
     K4Fold        fold{nullptr, nullptr, 0u, 0u};   // mode 1: onto the caller's global mask (mode 2: submit() sets the map's)
     SrtSweep      ssw{};                      // mode 2, a sweep (ssw.n > 0): the settings' Scan Ratio Test fields, and their
     K4Sweep       ksw{};                      // ground-filter groups with the settings' masks ksw.keep
+    std::shared_ptr<const TunePlan> tune;     // mode 2, a geometry sweep (erasor_process_nodes_tune): its geometries, in place of ssw / ksw
     // set by submit()
     bool          inserts = false;            // node-mode inserts
     bool          with_c = true;              // R-GPF class C launched up front
@@ -78,16 +82,56 @@ struct Step {
     size_t        n_map_global = 0;           // mode 2: map points
 };
 
+bool same_sweep(const SrtSweep& as, const K4Sweep& ak, const SrtSweep& bs, const K4Sweep& bk) {
+    return as.n == bs.n && as.n_flagged == bs.n_flagged && std::memcmp(as.v, bs.v, sizeof(SrtVariant) * (size_t)as.n) == 0 &&
+           ak.keep == bk.keep && ak.rejected == bk.rejected && ak.n == bk.n && ak.n_groups == bk.n_groups &&
+           std::memcmp(ak.bits, bk.bits, sizeof(uint32_t) * (size_t)ak.n_groups) == 0 &&
+           std::memcmp(ak.gp, bk.gp, sizeof(GpfParams) * (size_t)ak.n_groups) == 0;
+}
+
+// A geometry's polar tables, built by build_bin_tables on first use and kept by the handle (erasor_process_nodes_tune)
+struct GeoTables {
+    erasor_geometry_t key{};
+    HostBinTables     host;
+    DeviceBuffer      d_ring, d_pos, d_neg, d_guard;   // written once
+    BinTablesView     view{};
+    int               B = 0;
+};
+
+// A geometry sweep's submission: its distinct geometries in order of first appearance (geo[0] carries setting 0), each with the
+// sweep_ex state of the settings that carry it -- the other settings' Scan Ratio Test is switched off (minimum_num_pts -1) and
+// its groups hold only its settings -- and the K1 launches that bin them (geometries [launch_begin[l], launch_begin[l + 1])).
+// Geometry g's batch tables are the handle's tune_tabs[g].
+struct TuneGeo {
+    const GeoTables* t;
+    int              launch;
+    SrtSweep         ssw;
+    K4Sweep          ksw;
+};
+struct TunePlan {
+    int     n_settings = 0, n_geo = 0, n_launch = 0;
+    int     B_max = 0;
+    TuneGeo geo[kMaxSweepVariants];
+    int     launch_begin[kMaxSweepVariants + 1];
+    size_t  launch_smem[kMaxSweepVariants];
+};
+
+bool same_tune(const TunePlan* a, const TunePlan* b) {
+    if (!a || !b) return a == b;
+    if (a->n_geo != b->n_geo || a->n_launch != b->n_launch) return false;
+    for (int g = 0; g < a->n_geo; ++g)
+        if (a->geo[g].t != b->geo[g].t || a->geo[g].launch != b->geo[g].launch || !same_sweep(a->geo[g].ssw, a->geo[g].ksw, b->geo[g].ssw, b->geo[g].ksw))
+            return false;
+    return true;
+}
+
 bool same_step(const Step& a, const Step& b) {
     return a.mode == b.mode && a.ptr_kind == b.ptr_kind && a.qry_xyz == b.qry_xyz && a.inserts == b.inserts && a.with_c == b.with_c &&
            a.f0 == b.f0 && a.map_xyzi == b.map_xyzi && a.qry_xyzi == b.qry_xyzi && a.cur_map == b.cur_map && a.cur_qry == b.cur_qry &&
            a.user_keep == b.user_keep && a.d_keep == b.d_keep && a.n_keep == b.n_keep && a.keep_out == b.keep_out &&
            a.n_map_global == b.n_map_global && a.map == b.map &&
            a.fold.keep == b.fold.keep && a.fold.index == b.fold.index && a.fold.n == b.fold.n &&
-           a.ssw.n == b.ssw.n && a.ssw.n_flagged == b.ssw.n_flagged && std::memcmp(a.ssw.v, b.ssw.v, sizeof(SrtVariant) * (size_t)a.ssw.n) == 0 &&
-           a.ksw.keep == b.ksw.keep && a.ksw.rejected == b.ksw.rejected && a.ksw.n == b.ksw.n && a.ksw.n_groups == b.ksw.n_groups &&
-           std::memcmp(a.ksw.bits, b.ksw.bits, sizeof(uint32_t) * (size_t)a.ksw.n_groups) == 0 &&
-           std::memcmp(a.ksw.gp, b.ksw.gp, sizeof(GpfParams) * (size_t)a.ksw.n_groups) == 0;
+           same_sweep(a.ssw, a.ksw, b.ssw, b.ksw) && same_tune(a.tune.get(), b.tune.get());
 }
 
 }  // namespace
@@ -164,6 +208,16 @@ struct erasor_ctx {
     uint32_t class_c_count_host = 0;           // queue[kBucketC0] of the submission in flight
     Step     last;                             // the last mask-mode submission
     int      sweep_V = 0;                      // variants of the last node call when it was a sweep (erasor_get_sweep_stats), else 0
+    int      sweep_G = 1;                      // ... and its geometries: d_sweep_flag holds one [stat_F][32] block per geometry
+
+    // geometry sweeps (erasor_process_nodes_tune): the tables of every geometry seen, and per geometry of a call its batch tables
+    std::vector<std::unique_ptr<GeoTables>> geo_tables;
+    struct TuneTabs { HBuf bin_map, bin_qry, chcnt, zmin, zmax, cnt; explicit TuneTabs(uint64_t& e) : bin_map(e), bin_qry(e), chcnt(e), zmin(e), zmax(e), cnt(e) {} };
+    std::vector<std::unique_ptr<TuneTabs>> tune_tabs;
+    HBuf     d_list_idx32{alloc_epoch}, d_list_cnt32{alloc_epoch};   // the VoI lists of a tune call's 32-warp K1 launches (their split
+                                                                      // differs from the 8-warp launches', whose lists are d_list_*)
+    size_t   smem_optin = 0;                   // sharedMemPerBlockOptin of the device
+    bool     tune_unpacked = false;            // ERASOR_B200_TUNE_UNPACKED=1: one geometry per K1 launch (measurement of the packing)
 
     // node mode
     erasor_map_ctx* map = nullptr;
@@ -425,6 +479,33 @@ bool inserts_on(const erasor_ctx* h, int mode) { return mode == 2 && h->node_ins
 
 int run_insert_plan(erasor_ctx* h);
 
+// R-GPF's size classes on their streams (classes: bits 0|1 A and B, bit 2 C), under them the node inserts' plan when on
+int run_k4(erasor_ctx* h, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes, bool only_rgpf, const K4Sweep* k4sweep) {
+    Scope s(h, 4);
+    GpfParams gp{};
+    gp.th_dist = h->p.gf_dist_thr; gp.th_seeds = h->p.gf_th_seeds_height; gp.num_lowest_pts = h->p.num_lowest_pts;
+    gp.num_lpr = h->p.gf_num_lpr; gp.iters = std::min(h->p.gf_iter, kMaxIter); gp.cov_mode = h->p.cov_mode;
+    const bool with_c = (classes & 4) != 0;
+    h->launches += k4_num_launches(with_c);
+    CK(cudaEventRecord(h->ev_fork, h->stream));
+    CK(cudaStreamWaitEvent(h->stream_a, h->ev_fork, 0));
+    CK(cudaStreamWaitEvent(h->stream_b, h->ev_fork, 0));
+    if (with_c) CK(cudaStreamWaitEvent(h->stream_c, h->ev_fork, 0));
+    CK(launch_k4(h->stream_a, h->stream_b, h->stream_c, gp, h->d_recs.as<FlagRec>(), h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->rec_capacity,
+                 h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), h->d_frame_off.as<uint32_t>(),
+                 (mode == 0 || inserts_on(h, mode)) ? h->d_part.as<float4>() : nullptr, keep_mask, ground_mask,
+                 h->d_frame_rej.as<uint32_t>() + h->f0, h->d_scratch.as<unsigned char>(), h->sm_count, h->d_fence.as<unsigned long long>(), fold, classes, k4sweep));
+    CK(cudaEventRecord(h->ev_join_a, h->stream_a));
+    CK(cudaEventRecord(h->ev_join_b, h->stream_b));
+    if (with_c) CK(cudaEventRecord(h->ev_join_c, h->stream_c));
+    // node-mode inserts: the plan and the query scatter need only K1's tables, so they run on the main stream under R-GPF
+    if (inserts_on(h, mode) && !only_rgpf) { int rc = run_insert_plan(h); if (rc) return rc; }
+    CK(cudaStreamWaitEvent(h->stream, h->ev_join_a, 0));
+    CK(cudaStreamWaitEvent(h->stream, h->ev_join_b, 0));
+    if (with_c) CK(cudaStreamWaitEvent(h->stream, h->ev_join_c, 0));
+    return ERASOR_OK;
+}
+
 // sweep / k4sweep: a Scan Ratio Test sweep (node mode): the variants' flags in K2, their masks in K4's epilogue
 int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes = 7, bool only_rgpf = false,
                 const SrtSweep* sweep = nullptr, const K4Sweep* k4sweep = nullptr) {
@@ -467,29 +548,67 @@ int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_
                          k1_big_tables(h->p.num_rings, B) ? 32 : 8));
         }
     }
-    {
-        Scope s(h, 4);
-        GpfParams gp{};
-        gp.th_dist = h->p.gf_dist_thr; gp.th_seeds = h->p.gf_th_seeds_height; gp.num_lowest_pts = h->p.num_lowest_pts;
-        gp.num_lpr = h->p.gf_num_lpr; gp.iters = std::min(h->p.gf_iter, kMaxIter); gp.cov_mode = h->p.cov_mode;
-        const bool with_c = (classes & 4) != 0;
-        h->launches += k4_num_launches(with_c);
-        CK(cudaEventRecord(h->ev_fork, h->stream));
-        CK(cudaStreamWaitEvent(h->stream_a, h->ev_fork, 0));
-        CK(cudaStreamWaitEvent(h->stream_b, h->ev_fork, 0));
-        if (with_c) CK(cudaStreamWaitEvent(h->stream_c, h->ev_fork, 0));
-        CK(launch_k4(h->stream_a, h->stream_b, h->stream_c, gp, h->d_recs.as<FlagRec>(), h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->rec_capacity,
-                     h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), h->d_frame_off.as<uint32_t>(),
-                     (mode == 0 || inserts_on(h, mode)) ? h->d_part.as<float4>() : nullptr, keep_mask, ground_mask,
-                     h->d_frame_rej.as<uint32_t>() + h->f0, h->d_scratch.as<unsigned char>(), h->sm_count, h->d_fence.as<unsigned long long>(), fold, classes, k4sweep));
-        CK(cudaEventRecord(h->ev_join_a, h->stream_a));
-        CK(cudaEventRecord(h->ev_join_b, h->stream_b));
-        if (with_c) CK(cudaEventRecord(h->ev_join_c, h->stream_c));
-        // node-mode inserts: the plan and the query scatter need only K1's tables, so they run on the main stream under R-GPF
-        if (inserts_on(h, mode) && !only_rgpf) { int rc = run_insert_plan(h); if (rc) return rc; }
-        CK(cudaStreamWaitEvent(h->stream, h->ev_join_a, 0));
-        CK(cudaStreamWaitEvent(h->stream, h->ev_join_b, 0));
-        if (with_c) CK(cudaStreamWaitEvent(h->stream, h->ev_join_c, 0));
+    return run_k4(h, mode, keep_mask, ground_mask, fold, classes, only_rgpf, k4sweep);
+}
+
+// A geometry sweep's launches after the query staging: every geometry's table reset, K1's geometry form (one scan of the map per
+// launch of the plan), then per geometry the sweep_ex path on its tables -- the fused Scan Ratio Test + scatter and R-GPF with every
+// class -- over the handle's one set of records and scattered points.  The geometry of setting 0 runs last, so the union counts
+// of the frame tables are its own.
+int run_tune(erasor_ctx* h, const TunePlan& tp, bool qry_xyz) {
+    const int F = h->F;
+    const NodePose* poses = h->d_poses.as<NodePose>();
+    uint32_t* nflag = h->d_nflag.as<uint32_t>() + h->f0;
+    uint32_t* frame_rej = h->d_frame_rej.as<uint32_t>() + h->f0;
+    for (int g = 0; g < tp.n_geo; ++g) {
+        const int B = tp.geo[g].t->B;
+        erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
+        h->launches++;
+        CK(launch_init_tables(h->stream, tt.zmin.as<uint32_t>(), tt.zmax.as<uint32_t>(), 2 * (size_t)F * B, tt.cnt.as<uint32_t>(), 2 * (size_t)F * (B + 1),
+                              h->d_nrecs.as<uint32_t>(), frame_rej, nflag, F, h->d_queue.as<uint32_t>()));
+    }
+    const int n_chunks = (int)(h->n_chunks_map + h->n_chunks_qry);
+    for (int l = 0; l < tp.n_launch; ++l) {
+        Scope s(h, 1);
+        K1Geo G{};
+        for (int g = tp.launch_begin[l]; g < tp.launch_begin[l + 1]; ++g) {
+            erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
+            const GeoTables& t = *tp.geo[g].t;
+            K1GeoTables& o = G.g[G.n];
+            o.T = t.view; o.B = t.B;
+            o.bin_map = tt.bin_map.as<uint16_t>(); o.bin_qry = tt.bin_qry.as<uint16_t>(); o.ch_cnt = tt.chcnt.as<uint32_t>();
+            o.zmin = tt.zmin.as<uint32_t>(); o.zmax = tt.zmax.as<uint32_t>(); o.cnt = tt.cnt.as<uint32_t>();
+            o.smem_off = G.n ? G.g[G.n - 1].smem_off + (uint32_t)k1_geo_smem_bytes(G.g[G.n - 1].T.R, G.g[G.n - 1].B) : 0u;
+            G.n++;
+        }
+        const bool big = tp.launch_smem[l] > 56 * 1024;
+        if (n_chunks) h->launches++;
+        CK(launch_k1_geo(h->stream, G, tp.launch_smem[l], h->cur_map, h->cur_qry, h->d_chunks.as<ChunkDesc>(), n_chunks, F,
+                         h->d_fence.as<unsigned long long>(), poses, (big ? h->d_list_idx32 : h->d_list_idx).as<uint32_t>(),
+                         (big ? h->d_list_cnt32 : h->d_list_cnt).as<uint32_t>(), qry_xyz));
+    }
+    for (int g = tp.n_geo - 1; g >= 0; --g) {
+        const TuneGeo& tg = tp.geo[g];
+        erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
+        if (g != tp.n_geo - 1) {                  // records, queue and frame counters of the geometry before
+            h->launches++;
+            CK(launch_init_tables(h->stream, nullptr, nullptr, 0, nullptr, 0, h->d_nrecs.as<uint32_t>(), frame_rej, nflag, F, h->d_queue.as<uint32_t>()));
+        }
+        SrtParams sp = srt_params(h, h->p.version, 2);
+        sp.R = tg.t->view.R; sp.S = tg.t->view.S; sp.B = tg.t->B;
+        const bool big = tp.launch_smem[tg.launch] > 56 * 1024;      // the K1 launch that wrote g's ids, and its VoI lists
+        {
+            Scope s(h, 2);
+            if (h->n_chunks_map) h->launches++;
+            CK(launch_k2_srt(h->stream, sp, F, h->d_chunks.as<ChunkDesc>(), h->d_chunk_range.as<uint32_t>(), h->n_chunks_map, tt.bin_map.as<uint16_t>(),
+                             h->cur_map, poses, tt.chcnt.as<uint32_t>(), tt.zmin.as<uint32_t>(), tt.zmax.as<uint32_t>(), tt.cnt.as<uint32_t>(),
+                             h->d_frame_off.as<uint32_t>(), nflag, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
+                             h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
+                             (big ? h->d_list_idx32 : h->d_list_idx).as<uint32_t>(), (big ? h->d_list_cnt32 : h->d_list_cnt).as<uint32_t>(),
+                             &tg.ssw, big ? 32 : 8));
+        }
+        int rc = run_k4(h, 2, nullptr, nullptr, K4Fold{nullptr, nullptr, 0u, 0u}, 7, false, &tg.ksw);
+        if (rc) return rc;
     }
     return ERASOR_OK;
 }
@@ -636,6 +755,8 @@ int erasor_create(const erasor_params_t* params, int device, erasor_handle_t* ou
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return fail("cudaGetDeviceProperties", e);
     h->sm_count = prop.multiProcessorCount;
+    h->smem_optin = (size_t)prop.sharedMemPerBlockOptin;
+    if (const char* tu = std::getenv("ERASOR_B200_TUNE_UNPACKED")) h->tune_unpacked = tu[0] == '1';
     const size_t need = std::max(k1_smem_bytes(p.num_rings, h->B), k3_smem_bytes(h->B));
     if (need > (size_t)prop.sharedMemPerBlockOptin) {
         g_create_error = "num_rings*num_sectors too large for the per-CTA shared-memory bin table";
@@ -988,9 +1109,16 @@ int enqueue(erasor_ctx* h, const Step& s) {
         CK(cudaMemsetAsync(s.ssw.n_flagged, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
         CK(cudaMemsetAsync(s.ksw.rejected, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
     }
-    if ((rc = run_k1(h, s.mode))) return rc;
-    if ((rc = run_compare(h, h->p.version, s.mode, s.d_keep, nullptr, s.fold, s.with_c ? 7 : 3, false, s.ssw.n ? &s.ssw : nullptr,
-                          s.ssw.n ? &s.ksw : nullptr))) return rc;
+    if (s.tune) {
+        for (int g = 0; g < s.tune->n_geo; ++g)
+            CK(cudaMemsetAsync(s.tune->geo[g].ssw.n_flagged, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
+        CK(cudaMemsetAsync(s.tune->geo[0].ksw.rejected, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
+        if ((rc = run_tune(h, *s.tune, s.qry_xyz))) return rc;
+    } else {
+        if ((rc = run_k1(h, s.mode))) return rc;
+        if ((rc = run_compare(h, h->p.version, s.mode, s.d_keep, nullptr, s.fold, s.with_c ? 7 : 3, false, s.ssw.n ? &s.ssw : nullptr,
+                              s.ssw.n ? &s.ksw : nullptr))) return rc;
+    }
     if (s.inserts && (rc = run_insert_assemble(h))) return rc;      // (run_compare ran the plan and the query scatter under R-GPF)
     CK(cudaMemcpyAsync(h->h_words.as<uint32_t>() + 1, h->d_queue.as<uint32_t>() + kBucketC0, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
     if ((rc = copy_masks_out(h, s))) return rc;
@@ -1073,6 +1201,43 @@ int submit(erasor_ctx* h, Step st, const uint64_t* map_off, const uint64_t* qry_
         st.ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + (size_t)kMaxSweepVariants * st.f0;
         st.ksw.rejected = h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * st.f0;
         st.ksw.n = (uint32_t)st.n_map_global;
+    } else if (st.tune) {
+        // geometry sweep: every geometry's batch tables, records for the largest geometry, one block of per-setting flag counters
+        // per geometry; class C always runs up front (the records of one geometry are gone once the next one has run)
+        auto plan = std::make_shared<TunePlan>(*st.tune);
+        const size_t n_chunks = (size_t)h->n_chunks_map + h->n_chunks_qry;
+        while (h->tune_tabs.size() < (size_t)plan->n_geo) h->tune_tabs.emplace_back(new erasor_ctx::TuneTabs(h->alloc_epoch));
+        for (int g = 0; g < plan->n_geo; ++g) {
+            const size_t B = (size_t)plan->geo[g].t->B;
+            erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
+            CK(tt.bin_map.ensure(sizeof(uint16_t) * (h->NM + kIdPad)));
+            CK(tt.bin_qry.ensure(sizeof(uint16_t) * (h->NQ + kIdPad)));
+            CK(tt.chcnt.ensure(sizeof(uint32_t) * std::max<size_t>(n_chunks, 1) * (B + 1)));
+            CK(tt.zmin.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
+            CK(tt.zmax.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
+            CK(tt.cnt.ensure(sizeof(uint32_t) * 2 * (size_t)F * (B + 1)));
+        }
+        for (int l = 0; l < plan->n_launch; ++l)
+            if (plan->launch_smem[l] > 56 * 1024) {
+                CK(h->d_list_idx32.ensure(sizeof(uint32_t) * (h->NM + kIdPad)));
+                CK(h->d_list_cnt32.ensure(sizeof(uint32_t) * kListWarps * std::max<size_t>(n_chunks, 1)));
+            }
+        const uint32_t recs = (uint32_t)std::min<size_t>((size_t)F * plan->B_max, kMaxRecords);
+        if (recs > h->rec_capacity) {
+            CK(h->d_recs.ensure(sizeof(FlagRec) * (size_t)recs));
+            CK(h->d_bucket.ensure(sizeof(uint32_t) * (size_t)kNumBuckets * recs));
+            h->rec_capacity = recs;
+        }
+        const size_t rows = (size_t)kMaxSweepVariants * (size_t)h->stat_F;
+        CK(h->d_sweep_flag.ensure(sizeof(uint32_t) * rows * (size_t)plan->n_geo));
+        CK(h->d_sweep_rej.ensure(sizeof(uint32_t) * rows));
+        for (int g = 0; g < plan->n_geo; ++g) {
+            plan->geo[g].ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + rows * (size_t)g + (size_t)kMaxSweepVariants * st.f0;
+            plan->geo[g].ksw.rejected = h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * st.f0;
+            plan->geo[g].ksw.n = (uint32_t)st.n_map_global;
+        }
+        st.tune = plan;
+        st.with_c = true;
     } else if (st.mode == 2) {
         st.fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)st.n_map_global, 0u};   // a sweep leaves the map's mask alone
     }
@@ -1147,10 +1312,12 @@ int process_frames_impl(erasor_handle_t h, const float* map_xyzi, const uint64_t
 }
 
 // |map_voi_| of every node of the last submission = binned + complement counts of the map cloud (K1's tables), into out[0, F)
+// (after a geometry sweep: the tables of any geometry hold them; those of setting 0's are read)
 int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
-    const size_t row = (size_t)h->B + 1;
+    const bool tune = h->last.mode == 2 && h->last.tune;
+    const size_t row = (size_t)(tune ? h->last.tune->geo[0].t->B : h->B) + 1;
     std::vector<uint32_t> c((size_t)h->F * row);
-    CK(cudaMemcpy(c.data(), h->d_cnt.p(), sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(c.data(), (tune ? h->tune_tabs[0]->cnt : h->d_cnt).p(), sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
     for (int f = 0; f < h->F; ++f) {
         uint64_t t = 0;
         for (size_t b = 0; b < row; ++b) t += c[(size_t)f * row + b];
@@ -1161,7 +1328,7 @@ int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
 
 int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                        double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind, bool async,
-                       const SrtSweep* sweep = nullptr, const K4Sweep* groups = nullptr) {
+                       const SrtSweep* sweep = nullptr, const K4Sweep* groups = nullptr, std::shared_ptr<const TunePlan> tune = nullptr) {
     if (!h || !poses7 || !query_offsets) { if (h) h->err = "null argument"; return ERASOR_E_INVALID; }
     if (!h->map) { h->err = "erasor_process_nodes: no map attached (erasor_attach_map)"; return ERASOR_E_STATE; }
     if (n_frames <= 0) { h->err = "n_frames must be positive"; return ERASOR_E_INVALID; }
@@ -1177,15 +1344,20 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
     const size_t N = h->map->n;
     const double range = voi_max_range > 0.0 ? voi_max_range : h->p.max_range;
     h->stat_F = n_frames;
-    h->sweep_V = sweep ? sweep->n : 0;
+    h->sweep_V = sweep ? sweep->n : tune ? tune->n_settings : 0;
+    h->sweep_G = tune ? tune->n_geo : 1;
     h->ins_call_off.assign(h->node_inserts ? 1 : 0, 0);
     // scratch per (frame, map point): bin id 2 + scattered point 16 + source index 4 + class-C scratch 24 bytes; with inserts also
     // R-GPF's partitioned copy 16 + the inserts 16 + K4b's voxels 16 and scratch 36 bytes
     size_t budget = (size_t)16 << 30;
     if (const char* e = std::getenv("ERASOR_B200_NODE_SCRATCH_GB")) budget = (size_t)std::max(1.0, std::atof(e)) << 30;
-    const size_t by_mem = std::max<size_t>(1, budget / ((h->node_inserts ? 130 : 46) * std::max<size_t>(N, 1)));
+    // (a geometry sweep: also per geometry its bin id 2 bytes and its chunk count rows, at most 4 (B + 1) / (5 B) bytes, and the
+    // VoI lists of its 32-warp K1 launches 4 bytes)
+    const size_t per_point = (h->node_inserts ? 130 : 46) + (tune ? 3 * (size_t)tune->n_geo + 4 : 0);
+    const size_t by_mem = std::max<size_t>(1, budget / (per_point * std::max<size_t>(N, 1)));
     const size_t by_idx = std::max<size_t>(1, (size_t)0xFFFFFFF0ull / std::max<size_t>(N, 1) - 1);
-    const int max_frames = (int)std::min<size_t>({by_mem, by_idx, std::max<size_t>(1, kMaxRecords / (size_t)h->B), (size_t)n_frames});
+    const size_t B_max = tune ? (size_t)std::max(h->B, tune->B_max) : (size_t)h->B;
+    const int max_frames = (int)std::min<size_t>({by_mem, by_idx, std::max<size_t>(1, kMaxRecords / B_max), (size_t)n_frames});
     std::vector<uint64_t> mo, qo;
     std::vector<NodePose> poses;
     for (int f0 = 0; f0 < n_frames;) {
@@ -1209,6 +1381,7 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         st.user_keep = frame_keep ? frame_keep + (size_t)f0 * N : nullptr;
         st.keep_out = (f1 == n_frames) ? keep_out : nullptr;
         if (sweep) { st.ssw = *sweep; st.ksw = *groups; }
+        st.tune = tune;
         if ((rc = submit(h, st, mo.data(), qo.data(), F, poses.data(), poses7 + 7 * (size_t)f0))) return rc;
         if (f1 < n_frames) {                                         // the next sub-batch reuses the handle's buffers
             if ((rc = erasor_wait(h))) return rc;
@@ -1404,6 +1577,114 @@ int process_nodes_srt_sweep(erasor_handle_t h, const double* poses7, const float
     return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, ok ? settings : nullptr, n_variants,
                                     variant_keep, ptr_kind, async);
 }
+
+bool same_geometry(const erasor_geometry_t& a, const erasor_geometry_t& b) {
+    return a.max_range == b.max_range && a.min_h == b.min_h && a.max_h == b.max_h && a.num_rings == b.num_rings && a.num_sectors == b.num_sectors;
+}
+
+// The tables of geometry x: the handle's cached ones, or built now with erasor_create's checks and codes
+int geometry_tables(erasor_ctx* h, const erasor_geometry_t& x, const GeoTables** out) {
+    for (const auto& t : h->geo_tables)
+        if (same_geometry(t->key, x)) { *out = t.get(); return ERASOR_OK; }
+    const long long Bll = (long long)x.num_rings * (long long)x.num_sectors;
+    if (x.num_rings < 1 || x.num_sectors < 1 || Bll > 65534) { h->err = "num_rings*num_sectors must be in [1, 65534]"; return ERASOR_E_INVALID; }
+    erasor_params_t p = h->p;
+    p.max_range = x.max_range; p.min_h = x.min_h; p.max_h = x.max_h; p.num_rings = x.num_rings; p.num_sectors = x.num_sectors;
+    std::unique_ptr<GeoTables> t(new GeoTables());
+    t->key = x; t->B = (int)Bll;
+    std::string terr;
+    if (build_bin_tables(p, t->host, terr) != 0) { h->err = terr; return ERASOR_E_INVALID; }
+    if (std::max(k1_smem_bytes(x.num_rings, t->B), k3_smem_bytes(t->B)) > h->smem_optin) {
+        h->err = "num_rings*num_sectors too large for the per-CTA shared-memory bin table";
+        return ERASOR_E_UNSUPPORTED;
+    }
+    const HostBinTables& ht = t->host;
+    const size_t rb = sizeof(double) * ht.ring_thr.size(), sb = sizeof(SectorBoundary) * ht.sec_pos.size(), gb = sizeof(float) * ht.ring_guard.size();
+    CK(t->d_ring.allocate(rb)); CK(t->d_pos.allocate(sb)); CK(t->d_neg.allocate(sb)); CK(t->d_guard.allocate(gb));
+    CK(cudaMemcpy(t->d_ring.p(), ht.ring_thr.data(), rb, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(t->d_pos.p(), ht.sec_pos.data(), sb, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(t->d_neg.p(), ht.sec_neg.data(), sb, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(t->d_guard.p(), ht.ring_guard.data(), gb, cudaMemcpyHostToDevice));
+    t->view = ht.view(t->d_ring.as<double>(), t->d_pos.as<SectorBoundary>(), t->d_neg.as<SectorBoundary>(), t->d_guard.as<float>());
+    h->geo_tables.push_back(std::move(t));
+    *out = h->geo_tables.back().get();
+    return ERASOR_OK;
+}
+
+// erasor_process_nodes_tune: the handle's own geometry alone is sweep_ex; otherwise the settings are split by geometry (first
+// appearance order) and the geometries packed into K1 launches of at most 56 KB of tables, so that every launch keeps the
+// four 8-warp CTAs per SM of the plain kernel (a geometry beyond that runs alone in the 32-warp form, as it would in a plain call).
+int process_nodes_tune_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                            double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind, bool async) {
+    if (!h) return ERASOR_E_INVALID;
+    if (n_settings < 1 || n_settings > kMaxSweepVariants) { h->err = "n_variants must be in [1, 32]"; return ERASOR_E_INVALID; }
+    if (!settings || !variant_keep) { h->err = "null variants or variant_keep"; return ERASOR_E_INVALID; }
+    const erasor_geometry_t own{h->p.max_range, h->p.min_h, h->p.max_h, h->p.num_rings, h->p.num_sectors};
+    erasor_sweep_setting_t ss[kMaxSweepVariants];
+    bool all_own = true;
+    for (int v = 0; v < n_settings; ++v) { ss[v] = settings[v].s; all_own = all_own && same_geometry(settings[v].geometry, own); }
+    if (all_own) return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, ss, n_settings, variant_keep, ptr_kind, async);
+    for (int v = 0; v < n_settings; ++v)
+        if (ss[v].gf_iter > kMaxIter) { h->err = "gf_iter above the tap capacity (8)"; return ERASOR_E_UNSUPPORTED; }
+    if (!h->map) { h->err = "erasor_process_nodes_tune: no map attached (erasor_attach_map)"; return ERASOR_E_INVALID; }
+    if (h->node_inserts) { h->err = "a sweep has no node inserts: erasor_set_node_inserts(h, 0) first"; return ERASOR_E_INVALID; }
+    if (h->pending) { h->err = "erasor_process_nodes_tune while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
+    double range = voi_max_range;
+    if (!(range > 0.0)) {
+        for (int v = 1; v < n_settings; ++v)
+            if (settings[v].geometry.max_range != settings[0].geometry.max_range) {
+                h->err = "voi_max_range <= 0 takes the settings' max_range, and they differ: pass the VoI radius";
+                return ERASOR_E_INVALID;
+            }
+        range = settings[0].geometry.max_range;
+    }
+    CK(cudaSetDevice(h->device));
+    auto plan = std::make_shared<TunePlan>();
+    TunePlan& tp = *plan;
+    tp.n_settings = n_settings;
+    int geo_of[kMaxSweepVariants];
+    for (int v = 0; v < n_settings; ++v) {
+        int g = 0;
+        while (g < tp.n_geo && !same_geometry(tp.geo[g].t->key, settings[v].geometry)) ++g;
+        if (g == tp.n_geo) {
+            const GeoTables* t = nullptr;
+            int rc = geometry_tables(h, settings[v].geometry, &t);
+            if (rc) return rc;
+            tp.geo[tp.n_geo++].t = t;
+            tp.B_max = std::max(tp.B_max, t->B);
+        }
+        geo_of[v] = g;
+    }
+    for (int g = 0; g < tp.n_geo; ++g) {
+        // sweep_ex's state over the settings of geometry g; the others take part with no bin flagged
+        TuneGeo& tg = tp.geo[g];
+        tg.ssw.n = n_settings;
+        tg.ksw.keep = variant_keep;
+        for (int v = 0; v < n_settings; ++v) {
+            const erasor_sweep_setting_t& x = ss[v];
+            tg.ssw.v[v] = SrtVariant{x.scan_ratio_threshold, x.th_bin_max_h, geo_of[v] == g ? x.minimum_num_pts : -1, 0};
+            if (geo_of[v] != g) continue;
+            GpfParams gp{};
+            gp.th_dist = x.gf_dist_thr; gp.th_seeds = x.gf_th_seeds_height; gp.num_lowest_pts = x.num_lowest_pts;
+            gp.num_lpr = x.gf_num_lpr; gp.iters = x.gf_iter; gp.cov_mode = h->p.cov_mode;
+            int k = 0;
+            while (k < tg.ksw.n_groups && std::memcmp(&tg.ksw.gp[k], &gp, sizeof(GpfParams)) != 0) ++k;
+            if (k == tg.ksw.n_groups) tg.ksw.gp[tg.ksw.n_groups++] = gp;
+            tg.ksw.bits[k] |= 1u << v;
+        }
+        // K1 packing
+        const size_t bytes = k1_geo_smem_bytes(tg.t->view.R, tg.t->B);
+        const bool alone = h->tune_unpacked || bytes > 56 * 1024;
+        if (g == 0 || alone || tp.launch_smem[tp.n_launch - 1] + bytes > 56 * 1024 || tp.launch_smem[tp.n_launch - 1] > 56 * 1024) {
+            tp.launch_begin[tp.n_launch] = g;
+            tp.launch_smem[tp.n_launch++] = 0;
+        }
+        tg.launch = tp.n_launch - 1;
+        tp.launch_smem[tg.launch] += bytes;
+        tp.launch_begin[tp.n_launch] = g + 1;
+    }
+    return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, range, nullptr, nullptr, ptr_kind, async, nullptr, nullptr, plan);
+}
 }  // namespace
 
 int erasor_process_nodes_sweep(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
@@ -1423,19 +1704,35 @@ int erasor_process_nodes_sweep_ex_async(erasor_handle_t h, const double* poses7,
     return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, true);
 }
 
+int erasor_process_nodes_tune(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                              double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind) {
+    return process_nodes_tune_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, false);
+}
+int erasor_process_nodes_tune_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                    double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind) {
+    return process_nodes_tune_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, true);
+}
+
 int erasor_get_sweep_stats(erasor_handle_t h, uint32_t* n_flagged_bins, uint32_t* n_rejected_points) {
     if (!h) return ERASOR_E_INVALID;
     if (h->sweep_V <= 0 || h->desc_mode != 2) { h->err = "no erasor_process_nodes_sweep call has run"; return ERASOR_E_STATE; }
     int rc;
     if ((rc = erasor_wait(h))) return rc;
     const size_t F = (size_t)h->stat_F, V = (size_t)h->sweep_V;
-    std::vector<uint32_t> t((size_t)kMaxSweepVariants * F);
+    // a geometry sweep's flag counters: one block per geometry, each setting counted in its own geometry's block only
+    const size_t rows = (size_t)kMaxSweepVariants * F;
+    std::vector<uint32_t> t(rows * (size_t)h->sweep_G);
     for (int k = 0; k < 2; ++k) {
         uint32_t* out = k == 0 ? n_flagged_bins : n_rejected_points;
         if (!out) continue;
-        CK(cudaMemcpy(t.data(), (k == 0 ? h->d_sweep_flag : h->d_sweep_rej).p(), sizeof(uint32_t) * t.size(), cudaMemcpyDeviceToHost));
+        const size_t blocks = k == 0 ? (size_t)h->sweep_G : 1;
+        CK(cudaMemcpy(t.data(), (k == 0 ? h->d_sweep_flag : h->d_sweep_rej).p(), sizeof(uint32_t) * rows * blocks, cudaMemcpyDeviceToHost));
         for (size_t v = 0; v < V; ++v)
-            for (size_t f = 0; f < F; ++f) out[v * F + f] = t[f * kMaxSweepVariants + v];
+            for (size_t f = 0; f < F; ++f) {
+                uint32_t c = 0;
+                for (size_t g = 0; g < blocks; ++g) c += t[g * rows + f * kMaxSweepVariants + v];
+                out[v * F + f] = c;
+            }
     }
     return ERASOR_OK;
 }

@@ -1,4 +1,4 @@
-// kernels.h -- launch wrappers of the path's kernels (definitions in kernels.cu).
+// kernels.h -- launch wrappers of the path's kernels (definitions in kernels.cu; K1's geometry form in k1_geo.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -31,6 +31,12 @@ cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map
                       bool qry_xyz = false /*the query cloud is packed x y z, 12 bytes per point (mask modes)*/,
                       uint32_t* prof = nullptr /*node mode only: run the profiling build, kK1ProfSlots cycle counters per warp*/);
 
+// K1's geometry form (node mode): G's geometries binned in one scan of the map; smem = the sum of their k1_geo_smem_bytes.  The
+// launch runs 32 warps per CTA when smem exceeds k1_big_tables's 56 KB, else 8 (K2 needs that count to walk its lists).
+size_t k1_geo_smem_bytes(int R, int B);
+cudaError_t launch_k1_geo(cudaStream_t st, const K1Geo& G, size_t smem, const float4* map_pts, const float4* qry_pts, const ChunkDesc* chunks,
+                          int n_chunks, int F, unsigned long long* fence, const NodePose* poses, uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz);
+
 cudaError_t launch_k3(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt,
                       const uint32_t* zmin, const uint32_t* zmax, const uint32_t* frame_off, const uint32_t* cnt, uint32_t* dst_start,
                       uint8_t* status, uint8_t* action, uint32_t* flag_slot, uint32_t* n_flagged, uint32_t* frame_rec_base,
@@ -42,7 +48,8 @@ cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const Chun
                           const uint16_t* bin_ids, const float4* pts, const NodePose* poses, const uint32_t* ch_cnt, const uint32_t* zmin,
                           const uint32_t* zmax, const uint32_t* cnt, const uint32_t* frame_off, uint32_t* n_flagged, FlagRec* recs, uint32_t* n_recs,
                           uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list, float4* out_pts, uint32_t* out_src,
-                          const uint32_t* list_idx, const uint32_t* list_cnt, const SrtSweep* sweep = nullptr /*node mode: a Scan Ratio Test sweep*/);
+                          const uint32_t* list_idx, const uint32_t* list_cnt, const SrtSweep* sweep = nullptr /*node mode: a Scan Ratio Test sweep*/,
+                          int k1_warps = 0 /*warps of the K1 launch that wrote the lists; 0: the plain launch's for P.R, P.B*/);
 
 // flag_slot == null: every bin of dst_start's cloud that has an offset is scattered (cloud mode); otherwise the flagged bins only
 cudaError_t launch_k2(cudaStream_t st, const ChunkDesc* chunks, uint32_t chunk_base, uint32_t n_chunks,

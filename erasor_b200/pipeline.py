@@ -106,13 +106,19 @@ def tune_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, e
     """sweep_frame_independent over settings that may also vary R-GPF's fields (1..32 dicts of capi.SRT_SWEEP_FIELDS +
     capi.GF_SWEEP_FIELDS; a missing field comes from ep) in one node-mode pass (erasor_process_nodes_sweep_ex, DESIGN.md section
     8.6): each flagged bin is sorted by z once and fitted once per distinct ground-filter tuple.  Rows as sweep_frame_independent's,
-    with all eight fields.  Needs a CUDA device."""
+    with all eight fields.  When a setting also carries one of capi.GEOMETRY_SWEEP_FIELDS, the pass is erasor_process_nodes_tune
+    (section 8.7): each batch's queries are prepared once, the map is cut to every node's VoI once and binned under every
+    geometry, and the rows carry all thirteen fields.  Needs a CUDA device."""
     from . import capi
-    return _sweep_rows(nodes, initial_map, up, ep, settings, capi.SRT_SWEEP_FIELDS + capi.GF_SWEEP_FIELDS, gt, batch, save_voxel_size)
+    fields = capi.SRT_SWEEP_FIELDS + capi.GF_SWEEP_FIELDS
+    if any(set(dict(s)) & set(capi.GEOMETRY_SWEEP_FIELDS) for s in settings):
+        fields += capi.GEOMETRY_SWEEP_FIELDS
+    return _sweep_rows(nodes, initial_map, up, ep, settings, fields, gt, batch, save_voxel_size)
 
 
 def _sweep_rows(nodes, initial_map, up, ep, variants, fields, gt, batch, save_voxel_size) -> list:
-    """The rows of sweep_frame_independent (fields: the Scan Ratio Test's) and tune_frame_independent (all eight)."""
+    """The rows of sweep_frame_independent (fields: the Scan Ratio Test's) and tune_frame_independent (all eight, or all thirteen
+    with the geometry's)."""
     import torch
 
     from . import capi
@@ -125,12 +131,14 @@ def _sweep_rows(nodes, initial_map, up, ep, variants, fields, gt, batch, save_vo
         if set(v) - set(fields):
             raise ValueError(f"a sweep varies only {fields}, not {sorted(set(v) - set(fields))}")
     ex = len(fields) > len(capi.SRT_SWEEP_FIELDS)
+    geo = len(fields) > len(capi.SRT_SWEEP_FIELDS + capi.GF_SWEEP_FIELDS)
     nodes = list(nodes)
     sel = processed_nodes(nodes, up.removal_interval)
     initial_map = np.ascontiguousarray(initial_map, dtype=np.float32)
     m = capi.Map(initial_map)
     h = capi.Handle(ep.replace(version=up.version))       # /erasor/version as the updater reads it (OfflineMapUpdater.cpp:81)
-    run, settings_of = (h.process_nodes_sweep_ex, h.sweep_settings) if ex else (h.process_nodes_sweep, h.sweep_variants)
+    run, settings_of = ((h.process_nodes_tune, h.tune_settings) if geo else (h.process_nodes_sweep_ex, h.sweep_settings) if ex
+                        else (h.process_nodes_sweep, h.sweep_variants))
     V, n = len(variants), m.size
     leaf = up.map_voxel_size if save_voxel_size is None else save_voxel_size
     rows = []
@@ -160,7 +168,9 @@ def _sweep_rows(nodes, initial_map, up, ep, variants, fields, gt, batch, save_vo
                 capi._memcpy_from_device(static_map, d)
                 q = ev.evaluate(ref, static_map, voxelsize=0.2)
                 arr, _ = settings_of([variants[v]])
-                rows.append(dict(**{f: getattr(arr[0], f) for f in fields}, PR=q["PR"], RR=q["RR"], F1=q["F1"],
+                parts = (arr[0].geometry, arr[0].s) if geo else (arr[0],)
+                value = {f: getattr(part, f) for part in parts for f, _ in type(part)._fields_}
+                rows.append(dict(**{f: value[f] for f in fields}, PR=q["PR"], RR=q["RR"], F1=q["F1"],
                                  kept=int(np.count_nonzero(masks[v])), saved=len(static_map), flagged=int(flagged[v]), rejected=int(rejected[v])))
     finally:
         h.close()

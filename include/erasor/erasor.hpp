@@ -184,6 +184,16 @@ public:
         check(erasor_process_nodes_sweep_ex(h_, poses[0].data(), query_xyzi, query_offsets.data(), static_cast<int>(poses.size()), voi_max_range,
                                             settings.data(), static_cast<int>(settings.size()), d_variant_keep, ptr_kind));
     }
+    // The same sweep over settings that may also differ in the polar geometry and z window (DESIGN.md section 8.7): the map is cut to
+    // each node's VoI once and binned under every geometry; voi_max_range <= 0 takes the settings' common max_range.
+    void process_nodes_tune(const std::vector<std::array<double, 7>>& poses, const float* query_xyzi, const std::vector<uint64_t>& query_offsets,
+                            const std::vector<erasor_tune_setting_t>& settings, uint8_t* d_variant_keep, double voi_max_range = 0.0,
+                            int ptr_kind = ERASOR_PTR_HOST) {
+        if (!map_) throw std::logic_error("ERASOR: load_global_map first");
+        if (poses.empty() || poses.size() + 1 != query_offsets.size()) throw std::invalid_argument("ERASOR: one pose per query VoI");
+        check(erasor_process_nodes_tune(h_, poses[0].data(), query_xyzi, query_offsets.data(), static_cast<int>(poses.size()), voi_max_range,
+                                        settings.data(), static_cast<int>(settings.size()), d_variant_keep, ptr_kind));
+    }
     // Node-mode inserts (DESIGN.md section 8.4): with enable, process_nodes / process_scans also append the query points each node's
     // static estimate puts back into the map to the map's store, and save_static_map voxelises them with the kept map.
     void set_node_inserts(bool enable) { check(erasor_set_node_inserts(h_, enable ? 1 : 0)); inserts_ = enable; }

@@ -262,6 +262,35 @@ int erasor_process_nodes_sweep_ex(erasor_handle_t h, const double* poses7, const
 int erasor_process_nodes_sweep_ex_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                         double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind);
 
+/* ---- geometry and height-window sweep (DESIGN.md section 8.7) ---- */
+/* ERASOR's polar geometry and z window (/erasor/max_range, min_h, max_h, num_rings, num_sectors), as erasor_params_t carries them */
+typedef struct {
+    double max_range;
+    double min_h;
+    double max_h;
+    int    num_rings;
+    int    num_sectors;
+} erasor_geometry_t;
+/* one setting of a tune call: a geometry and the eight fields of erasor_sweep_setting_t */
+typedef struct {
+    erasor_geometry_t      geometry;
+    erasor_sweep_setting_t s;
+} erasor_tune_setting_t;
+/* erasor_process_nodes_sweep_ex over settings that may also differ in geometry (version, cov_mode and skip_voxelize still come
+ * from the handle).  The VoI cut and the origin -> body transform run once per point; K1 bins each VoI point under every
+ * distinct geometry in as few scans of the map as shared memory allows, and each geometry then runs the sweep_ex path on its own
+ * bins.  Mask v equals the map's keep mask after erasor_process_nodes on a fresh map with a handle created with the handle's
+ * parameters and setting v's thirteen fields, the same voi_max_range, queries and ptr_kind; erasor_get_sweep_stats gives that
+ * run's counts.  voi_max_range <= 0 takes the settings' common max_range.  erasor_get_node_stats gives n_voi_points as usual;
+ * its flagged-bin and rejected-point counts are the union counts of the geometry of setting 0.  With every setting carrying the
+ * handle's own geometry the call is erasor_process_nodes_sweep_ex.  Refusals as erasor_process_nodes_sweep_ex, and with
+ * erasor_create's codes a geometry it would refuse (num_rings * num_sectors outside [1, 65534], a table it cannot build, tables
+ * beyond the device's shared memory); ERASOR_E_INVALID for voi_max_range <= 0 when the settings' max_range differ. */
+int erasor_process_nodes_tune(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                              double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind);
+int erasor_process_nodes_tune_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                    double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind);
+
 /* ---- node-mode inserts: the query points each node's static estimate puts back into the map (DESIGN.md section 8.4) ---- */
 /* Opt-in per handle (default off; off changes nothing).  With it on, erasor_process_nodes also builds, per node f, inserted_f:
  * bin by bin in r_pod2pc order, the bins whose selected points hold query points -- R-GPF bins: bin_curr then the R-GPF ground
