@@ -56,7 +56,7 @@ namespace {
 // chunk descriptors (whose changes alloc_epoch and desc_epoch track).  The caller fills in the first part, submit() the rest.  A
 // captured graph replays the step it was captured from, so the graph cache is keyed on it; erasor_wait's class-C fix-up and
 // erasor_profile_k1 read the last one.
-struct TunePlan;
+struct SweepPlan;
 
 struct Step {
     int           mode = 1;                   // 1: batch of (map_voi, query_voi) pairs, 2: nodes against the resident map
@@ -68,9 +68,7 @@ struct Step {
     uint8_t*      user_keep = nullptr;        // mode 1: one byte per VoI point; mode 2: frame_keep [F][n_map] (nullable)
     uint8_t*      keep_out = nullptr;         // mode 2: receives the map's mask (nullable)
     K4Fold        fold{nullptr, nullptr, 0u, 0u};   // mode 1: onto the caller's global mask (mode 2: submit() sets the map's)
-    SrtSweep      ssw{};                      // mode 2, a sweep (ssw.n > 0): the settings' Scan Ratio Test fields, and their
-    K4Sweep       ksw{};                      // ground-filter groups with the settings' masks ksw.keep
-    std::shared_ptr<const TunePlan> tune;     // mode 2, a geometry sweep (erasor_process_nodes_tune): its geometries, in place of ssw / ksw
+    std::shared_ptr<const SweepPlan> sweep;   // mode 2: the sweep of erasor_process_nodes_sweep / _sweep_ex / _tune (null: none)
     // set by submit()
     bool          inserts = false;            // node-mode inserts
     bool          with_c = true;              // R-GPF class C launched up front
@@ -82,14 +80,8 @@ struct Step {
     size_t        n_map_global = 0;           // mode 2: map points
 };
 
-bool same_sweep(const SrtSweep& as, const K4Sweep& ak, const SrtSweep& bs, const K4Sweep& bk) {
-    return as.n == bs.n && as.n_flagged == bs.n_flagged && std::memcmp(as.v, bs.v, sizeof(SrtVariant) * (size_t)as.n) == 0 &&
-           ak.keep == bk.keep && ak.rejected == bk.rejected && ak.n == bk.n && ak.n_groups == bk.n_groups &&
-           std::memcmp(ak.bits, bk.bits, sizeof(uint32_t) * (size_t)ak.n_groups) == 0 &&
-           std::memcmp(ak.gp, bk.gp, sizeof(GpfParams) * (size_t)ak.n_groups) == 0;
-}
-
-// A geometry's polar tables, built by build_bin_tables on first use and kept by the handle (erasor_process_nodes_tune)
+// A geometry's polar tables, built by build_bin_tables and kept by the handle: its own geometry's by erasor_create, a sweep
+// geometry's on first use
 struct GeoTables {
     erasor_geometry_t key{};
     HostBinTables     host;
@@ -98,30 +90,37 @@ struct GeoTables {
     int               B = 0;
 };
 
-// A geometry sweep's submission: its distinct geometries in order of first appearance (geo[0] carries setting 0), each with the
-// sweep_ex state of the settings that carry it -- the other settings' Scan Ratio Test is switched off (minimum_num_pts -1) and
-// its groups hold only its settings -- and the K1 launches that bin them (geometries [launch_begin[l], launch_begin[l + 1])).
-// Geometry g's batch tables are the handle's tune_tabs[g].
-struct TuneGeo {
+// A sweep's submission (erasor_process_nodes_sweep / _sweep_ex / _tune, DESIGN.md sections 8.5-8.7): its distinct geometries in
+// order of first appearance (geo[0] carries setting 0), each with the Scan Ratio Test fields of every setting -- those of the
+// other geometries switched off (minimum_num_pts -1) -- and the ground-filter groups of its own settings.  An own plan's one
+// geometry is the handle's: K1 bins into the handle's per-batch tables, as in a plain call.  Any other plan bins geometry g into
+// the handle's tune_tabs[g], in the K1 launches of launch_begin (geometries [launch_begin[l], launch_begin[l + 1])).
+struct SweepGeo {
     const GeoTables* t;
-    int              launch;
+    int              launch;                   // the K1 launch that bins it (not own)
     SrtSweep         ssw;
     K4Sweep          ksw;
 };
-struct TunePlan {
-    int     n_settings = 0, n_geo = 0, n_launch = 0;
-    int     B_max = 0;
-    TuneGeo geo[kMaxSweepVariants];
-    int     launch_begin[kMaxSweepVariants + 1];
-    size_t  launch_smem[kMaxSweepVariants];
+struct SweepPlan {
+    bool                  own = false;
+    int                   B_max = 0;
+    std::vector<SweepGeo> geo;
+    std::vector<int>      launch_begin;        // not own: K1 launches + 1 entries
+    std::vector<size_t>   launch_smem;         // ... and each launch's shared memory
 };
 
-bool same_tune(const TunePlan* a, const TunePlan* b) {
+bool same_plan(const SweepPlan* a, const SweepPlan* b) {
     if (!a || !b) return a == b;
-    if (a->n_geo != b->n_geo || a->n_launch != b->n_launch) return false;
-    for (int g = 0; g < a->n_geo; ++g)
-        if (a->geo[g].t != b->geo[g].t || a->geo[g].launch != b->geo[g].launch || !same_sweep(a->geo[g].ssw, a->geo[g].ksw, b->geo[g].ssw, b->geo[g].ksw))
+    if (a->geo.size() != b->geo.size() || a->launch_begin != b->launch_begin) return false;
+    for (size_t g = 0; g < a->geo.size(); ++g) {
+        const SrtSweep &as = a->geo[g].ssw, &bs = b->geo[g].ssw;
+        const K4Sweep &ak = a->geo[g].ksw, &bk = b->geo[g].ksw;
+        if (a->geo[g].t != b->geo[g].t || a->geo[g].launch != b->geo[g].launch || as.n != bs.n || as.n_flagged != bs.n_flagged ||
+            std::memcmp(as.v, bs.v, sizeof(SrtVariant) * (size_t)as.n) != 0 || ak.keep != bk.keep || ak.rejected != bk.rejected ||
+            ak.n != bk.n || ak.n_groups != bk.n_groups || std::memcmp(ak.bits, bk.bits, sizeof(uint32_t) * (size_t)ak.n_groups) != 0 ||
+            std::memcmp(ak.gp, bk.gp, sizeof(GpfParams) * (size_t)ak.n_groups) != 0)
             return false;
+    }
     return true;
 }
 
@@ -130,8 +129,7 @@ bool same_step(const Step& a, const Step& b) {
            a.f0 == b.f0 && a.map_xyzi == b.map_xyzi && a.qry_xyzi == b.qry_xyzi && a.cur_map == b.cur_map && a.cur_qry == b.cur_qry &&
            a.user_keep == b.user_keep && a.d_keep == b.d_keep && a.n_keep == b.n_keep && a.keep_out == b.keep_out &&
            a.n_map_global == b.n_map_global && a.map == b.map &&
-           a.fold.keep == b.fold.keep && a.fold.index == b.fold.index && a.fold.n == b.fold.n &&
-           same_sweep(a.ssw, a.ksw, b.ssw, b.ksw) && same_tune(a.tune.get(), b.tune.get());
+           a.fold.keep == b.fold.keep && a.fold.index == b.fold.index && a.fold.n == b.fold.n && same_plan(a.sweep.get(), b.sweep.get());
 }
 
 }  // namespace
@@ -152,14 +150,11 @@ struct erasor_ctx {
     cudaEvent_t     ev_fork = nullptr, ev_join_a = nullptr, ev_join_b = nullptr, ev_join_c = nullptr;
     int             sm_count = 132;
     std::string     err;
-    HostBinTables   tables;
     // Captured graphs hold raw device pointers: every (re)allocation of a device buffer of this handle bumps alloc_epoch, which
     // retires them.  HBuf cannot be built without the epoch, so a buffer added here cannot forget it.
     uint64_t        alloc_epoch = 0;
     struct HBuf : DeviceBuffer { explicit HBuf(uint64_t& e) : DeviceBuffer(&e) {} };
-    HBuf            d_ring{alloc_epoch}, d_pos{alloc_epoch}, d_neg{alloc_epoch}, d_guard{alloc_epoch};
-    BinTablesView   view{};
-    int             B = 0;
+    int             B = 0;                     // bins of the handle's geometry (its polar tables: geo_tables[0])
 
     // per-batch buffers
     HBuf d_map_in{alloc_epoch}, d_qry_in{alloc_epoch};       // staging when the caller's clouds are host memory
@@ -177,7 +172,8 @@ struct erasor_ctx {
     HBuf d_list_idx{alloc_epoch}, d_list_cnt{alloc_epoch};   // node mode: per chunk, the map index of every VoI point (dense, map order) and their number
     HBuf d_k1prof{alloc_epoch};                // erasor_profile_k1: per-warp cycle counters of K1's profiling build
     HBuf d_pack{alloc_epoch}, d_gather{alloc_epoch};         // exchange step: packed keep bits of this rank / of every rank
-    HBuf d_sweep_flag{alloc_epoch}, d_sweep_rej{alloc_epoch};  // Scan Ratio Test sweep: flagged bins / rejected points per (frame, variant), [stat_F][32]
+    HBuf d_sweep_flag{alloc_epoch}, d_sweep_rej{alloc_epoch};  // sweeps: flagged bins per (plan geometry, frame, variant) [G][stat_F][32] /
+                                                               // rejected points per (frame, variant) [stat_F][32]
     PinnedBuffer h_stage, h_pose, h_words;     // h_words: small device -> host read-backs of a submission (pinned: an asynchronous copy into
                                                // pageable memory blocks the launching thread until the whole stream has drained, which
                                                // serialised overlapped handles)
@@ -208,13 +204,12 @@ struct erasor_ctx {
     uint32_t class_c_count_host = 0;           // queue[kBucketC0] of the submission in flight
     Step     last;                             // the last mask-mode submission
     int      sweep_V = 0;                      // variants of the last node call when it was a sweep (erasor_get_sweep_stats), else 0
-    int      sweep_G = 1;                      // ... and its geometries: d_sweep_flag holds one [stat_F][32] block per geometry
 
-    // geometry sweeps (erasor_process_nodes_tune): the tables of every geometry seen, and per geometry of a call its batch tables
+    // the polar tables of every geometry seen, the handle's own first; per geometry of a sweep plan that is not own its batch tables
     std::vector<std::unique_ptr<GeoTables>> geo_tables;
     struct TuneTabs { HBuf bin_map, bin_qry, chcnt, zmin, zmax, cnt; explicit TuneTabs(uint64_t& e) : bin_map(e), bin_qry(e), chcnt(e), zmin(e), zmax(e), cnt(e) {} };
     std::vector<std::unique_ptr<TuneTabs>> tune_tabs;
-    HBuf     d_list_idx32{alloc_epoch}, d_list_cnt32{alloc_epoch};   // the VoI lists of a tune call's 32-warp K1 launches (their split
+    HBuf     d_list_idx32{alloc_epoch}, d_list_cnt32{alloc_epoch};   // the VoI lists of a plan's 32-warp K1 launches (their split
                                                                       // differs from the 8-warp launches', whose lists are d_list_*)
     size_t   smem_optin = 0;                   // sharedMemPerBlockOptin of the device
     bool     tune_unpacked = false;            // ERASOR_B200_TUNE_UNPACKED=1: one geometry per K1 launch (measurement of the packing)
@@ -443,28 +438,87 @@ int stage_host_clouds(erasor_ctx* h, int ptr_kind, const float* map_xyzi, const 
     return ERASOR_OK;
 }
 
-int run_k1(erasor_ctx* h, int mode) {
-    const int B = h->B, F = h->F;
-    {
-        h->launches++;
-        CK(launch_init_tables(h->stream, h->d_zmin.as<uint32_t>(), h->d_zmax.as<uint32_t>(), 2 * (size_t)F * B,
-                              h->d_cnt.as<uint32_t>(), 2 * (size_t)F * (B + 1), h->d_nrecs.as<uint32_t>(), h->d_frame_rej.as<uint32_t>() + h->f0,
-                              h->d_nflag.as<uint32_t>() + h->f0, F, h->d_queue.as<uint32_t>()));
+erasor_geometry_t own_geometry(const erasor_params_t& p) { return erasor_geometry_t{p.max_range, p.min_h, p.max_h, p.num_rings, p.num_sectors}; }
+
+bool same_geometry(const erasor_geometry_t& a, const erasor_geometry_t& b) {
+    return a.max_range == b.max_range && a.min_h == b.min_h && a.max_h == b.max_h && a.num_rings == b.num_rings && a.num_sectors == b.num_sectors;
+}
+
+// The tables of geometry x: the handle's cached ones, or built and uploaded now with erasor_create's checks and codes (erasor_create
+// itself builds the handle's own this way, as the first entry)
+int geometry_tables(erasor_ctx* h, const erasor_geometry_t& x, const GeoTables** out) {
+    for (const auto& t : h->geo_tables)
+        if (same_geometry(t->key, x)) { *out = t.get(); return ERASOR_OK; }
+    const long long Bll = (long long)x.num_rings * (long long)x.num_sectors;
+    if (x.num_rings < 1 || x.num_sectors < 1 || Bll > 65534) { h->err = "num_rings*num_sectors must be in [1, 65534]"; return ERASOR_E_INVALID; }
+    erasor_params_t p = h->p;
+    p.max_range = x.max_range; p.min_h = x.min_h; p.max_h = x.max_h; p.num_rings = x.num_rings; p.num_sectors = x.num_sectors;
+    std::unique_ptr<GeoTables> t(new GeoTables());
+    t->key = x; t->B = (int)Bll;
+    std::string terr;
+    if (build_bin_tables(p, t->host, terr) != 0) { h->err = terr; return ERASOR_E_INVALID; }
+    if (std::max(k1_smem_bytes(x.num_rings, t->B), k3_smem_bytes(t->B)) > h->smem_optin) {
+        h->err = "num_rings*num_sectors too large for the per-CTA shared-memory bin table";
+        return ERASOR_E_UNSUPPORTED;
     }
-    {
-        Scope s(h, 1);
-        if (h->n_chunks_map + h->n_chunks_qry) h->launches++;
-        CK(launch_k1(h->stream, h->view, h->cur_map, h->cur_qry, h->d_chunks.as<ChunkDesc>(), (int)(h->n_chunks_map + h->n_chunks_qry),
-                     h->d_bin_map.as<uint16_t>(), h->d_bin_qry.as<uint16_t>(), h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(),
-                     h->d_zmax.as<uint32_t>(), h->d_cnt.as<uint32_t>(), B, F, h->d_fence.as<unsigned long long>(),
-                     mode == 2 ? h->d_poses.as<NodePose>() : nullptr, mode == 2 ? h->d_list_idx.as<uint32_t>() : nullptr,
-                     mode == 2 ? h->d_list_cnt.as<uint32_t>() : nullptr, mode != 0 && h->last.qry_xyz, mode == 2 ? h->k1_prof : nullptr));
-    }
+    const HostBinTables& ht = t->host;
+    const size_t rb = sizeof(double) * ht.ring_thr.size(), sb = sizeof(SectorBoundary) * ht.sec_pos.size(), gb = sizeof(float) * ht.ring_guard.size();
+    cudaError_t e;
+    auto fail = [&](const char* what) { h->err = std::string(what) + ": " + cudaGetErrorString(e); return ERASOR_E_CUDA; };
+    if ((e = t->d_ring.allocate(rb)) != cudaSuccess || (e = t->d_pos.allocate(sb)) != cudaSuccess || (e = t->d_neg.allocate(sb)) != cudaSuccess ||
+        (e = t->d_guard.allocate(gb)) != cudaSuccess)
+        return fail("cudaMalloc");
+    if ((e = cudaMemcpy(t->d_ring.p(), ht.ring_thr.data(), rb, cudaMemcpyHostToDevice)) != cudaSuccess ||
+        (e = cudaMemcpy(t->d_pos.p(), ht.sec_pos.data(), sb, cudaMemcpyHostToDevice)) != cudaSuccess ||
+        (e = cudaMemcpy(t->d_neg.p(), ht.sec_neg.data(), sb, cudaMemcpyHostToDevice)) != cudaSuccess ||
+        (e = cudaMemcpy(t->d_guard.p(), ht.ring_guard.data(), gb, cudaMemcpyHostToDevice)) != cudaSuccess)
+        return fail("cudaMemcpy");
+    t->view = ht.view(t->d_ring.as<double>(), t->d_pos.as<SectorBoundary>(), t->d_neg.as<SectorBoundary>(), t->d_guard.as<float>());
+    h->geo_tables.push_back(std::move(t));
+    *out = h->geo_tables.back().get();
     return ERASOR_OK;
 }
 
-// K3 -> K2 -> K4 ; mode 0: every bin scattered + partitioned copies (cloud outputs), mode 1 / 2: flagged only + masks
-// classes: which R-GPF size classes to launch (bits 0|1: A and B, bit 2: C); 0x8 alone = R-GPF only, for the class-C fix-up
+// The tables K1 writes for geometry g of a sweep plan: the handle's geometry into the per-batch buffers (no plan, or an own plan),
+// any other into the plan's tune_tabs[g]
+K1GeoTables k1_tables(const erasor_ctx* h, const SweepPlan* plan, int g) {
+    K1GeoTables o{};
+    if (!plan || plan->own) {
+        o.T = h->geo_tables[0]->view; o.B = h->B;
+        o.bin_map = h->d_bin_map.as<uint16_t>(); o.bin_qry = h->d_bin_qry.as<uint16_t>(); o.ch_cnt = h->d_chcnt.as<uint32_t>();
+        o.zmin = h->d_zmin.as<uint32_t>(); o.zmax = h->d_zmax.as<uint32_t>(); o.cnt = h->d_cnt.as<uint32_t>();
+    } else {
+        const erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
+        o.T = plan->geo[g].t->view; o.B = plan->geo[g].t->B;
+        o.bin_map = tt.bin_map.as<uint16_t>(); o.bin_qry = tt.bin_qry.as<uint16_t>(); o.ch_cnt = tt.chcnt.as<uint32_t>();
+        o.zmin = tt.zmin.as<uint32_t>(); o.zmax = tt.zmax.as<uint32_t>(); o.cnt = tt.cnt.as<uint32_t>();
+    }
+    return o;
+}
+
+// the reset of the submission's records, queue and frame counters, and with t the reset of K1's z / count tables t
+int run_init(erasor_ctx* h, const K1GeoTables* t) {
+    const size_t F = (size_t)h->F, B = t ? (size_t)t->B : 0;
+    h->launches++;
+    CK(launch_init_tables(h->stream, t ? t->zmin : nullptr, t ? t->zmax : nullptr, 2 * F * B, t ? t->cnt : nullptr, t ? 2 * F * (B + 1) : 0,
+                          h->d_nrecs.as<uint32_t>(), h->d_frame_rej.as<uint32_t>() + h->f0, h->d_nflag.as<uint32_t>() + h->f0, h->F,
+                          h->d_queue.as<uint32_t>()));
+    return ERASOR_OK;
+}
+
+int run_k1(erasor_ctx* h, int mode) {
+    const K1GeoTables t = k1_tables(h, nullptr, 0);
+    int rc = run_init(h, &t);
+    if (rc) return rc;
+    Scope s(h, 1);
+    if (h->n_chunks_map + h->n_chunks_qry) h->launches++;
+    CK(launch_k1(h->stream, t.T, h->cur_map, h->cur_qry, h->d_chunks.as<ChunkDesc>(), (int)(h->n_chunks_map + h->n_chunks_qry),
+                 t.bin_map, t.bin_qry, t.ch_cnt, t.zmin, t.zmax, t.cnt, t.B, h->F, h->d_fence.as<unsigned long long>(),
+                 mode == 2 ? h->d_poses.as<NodePose>() : nullptr, mode == 2 ? h->d_list_idx.as<uint32_t>() : nullptr,
+                 mode == 2 ? h->d_list_cnt.as<uint32_t>() : nullptr, mode != 0 && h->last.qry_xyz, mode == 2 ? h->k1_prof : nullptr));
+    return ERASOR_OK;
+}
+
 SrtParams srt_params(const erasor_ctx* h, int version, int mode) {
     SrtParams sp{};
     sp.scan_ratio_threshold = h->p.scan_ratio_threshold;
@@ -479,8 +533,9 @@ bool inserts_on(const erasor_ctx* h, int mode) { return mode == 2 && h->node_ins
 
 int run_insert_plan(erasor_ctx* h);
 
-// R-GPF's size classes on their streams (classes: bits 0|1 A and B, bit 2 C), under them the node inserts' plan when on
-int run_k4(erasor_ctx* h, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes, bool only_rgpf, const K4Sweep* k4sweep) {
+// R-GPF's size classes on their streams (classes: bits 0|1 A and B, bit 2 C), under classes A and B the node inserts' plan when on
+// (a late class-C run has no plan to redo); k4sweep: a sweep's ground-filter groups and masks
+int run_k4(erasor_ctx* h, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes, const K4Sweep* k4sweep) {
     Scope s(h, 4);
     GpfParams gp{};
     gp.th_dist = h->p.gf_dist_thr; gp.th_seeds = h->p.gf_th_seeds_height; gp.num_lowest_pts = h->p.num_lowest_pts;
@@ -499,31 +554,49 @@ int run_k4(erasor_ctx* h, int mode, uint8_t* keep_mask, uint8_t* ground_mask, co
     CK(cudaEventRecord(h->ev_join_b, h->stream_b));
     if (with_c) CK(cudaEventRecord(h->ev_join_c, h->stream_c));
     // node-mode inserts: the plan and the query scatter need only K1's tables, so they run on the main stream under R-GPF
-    if (inserts_on(h, mode) && !only_rgpf) { int rc = run_insert_plan(h); if (rc) return rc; }
+    if (inserts_on(h, mode) && (classes & 3)) { int rc = run_insert_plan(h); if (rc) return rc; }
     CK(cudaStreamWaitEvent(h->stream, h->ev_join_a, 0));
     CK(cudaStreamWaitEvent(h->stream, h->ev_join_b, 0));
     if (with_c) CK(cudaStreamWaitEvent(h->stream, h->ev_join_c, 0));
     return ERASOR_OK;
 }
 
-// sweep / k4sweep: a Scan Ratio Test sweep (node mode): the variants' flags in K2, their masks in K4's epilogue
-int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes = 7, bool only_rgpf = false,
-                const SrtSweep* sweep = nullptr, const K4Sweep* k4sweep = nullptr) {
+// The mask modes' K2: the Scan Ratio Test fused into the scatter of the flagged bins, over the tables t that K1 wrote.  Node mode
+// (list_idx non-null) walks the VoI lists of the K1 launch that wrote t, with its k1_warps warps per CTA; sweep: a sweep's settings.
+int run_k2_srt(erasor_ctx* h, const SrtParams& sp, const K1GeoTables& t, const uint32_t* list_idx, const uint32_t* list_cnt, int k1_warps,
+               const SrtSweep* sweep) {
+    Scope s(h, 2);
+    if (h->n_chunks_map) h->launches++;
+    CK(launch_k2_srt(h->stream, sp, h->F, h->d_chunks.as<ChunkDesc>(), h->d_chunk_range.as<uint32_t>(), h->n_chunks_map, t.bin_map, h->cur_map,
+                     list_idx ? h->d_poses.as<NodePose>() : nullptr, t.ch_cnt, t.zmin, t.zmax, t.cnt, h->d_frame_off.as<uint32_t>(),
+                     h->d_nflag.as<uint32_t>() + h->f0, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
+                     h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
+                     list_idx, list_cnt, sweep, k1_warps));
+    return ERASOR_OK;
+}
+
+// K3 -> K2 -> K4 ; mode 0: every bin scattered + partitioned copies (cloud outputs), mode 1 / 2: flagged only + masks
+// classes: which R-GPF size classes to launch (bits 0|1: A and B, bit 2: C)
+int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes = 7) {
     const int B = h->B, F = h->F;
     const NodePose* poses = mode == 2 ? h->d_poses.as<NodePose>() : nullptr;
     uint32_t* nflag = h->d_nflag.as<uint32_t>() + h->f0;
     const SrtParams sp = srt_params(h, version, mode);
-    const bool fused = mode != 0 && (h->fused_srt || sweep);      // mask modes: SRT inside the scatter kernel (a sweep has no K3 form)
-    if (!fused && !only_rgpf) {
-        Scope s(h, 3);
-        h->launches++;
-        CK(launch_k3(h->stream, sp, F, h->d_chunk_range.as<uint32_t>(), h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(),
-                     h->d_zmax.as<uint32_t>(), h->d_frame_off.as<uint32_t>(), h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(),
-                     h->d_status.as<uint8_t>(), h->d_action.as<uint8_t>(), h->d_flag_slot.as<uint32_t>(), nflag,
-                     h->d_frame_rec_base.as<uint32_t>(), h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
-                     h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>()));
-    }
-    if (!only_rgpf) {
+    const int k1_warps = k1_big_tables(h->p.num_rings, B) ? 32 : 8;
+    if (mode != 0 && h->fused_srt) {      // mask modes: SRT inside the scatter kernel
+        const int rc = run_k2_srt(h, sp, k1_tables(h, nullptr, 0), poses ? h->d_list_idx.as<uint32_t>() : nullptr,
+                                  poses ? h->d_list_cnt.as<uint32_t>() : nullptr, k1_warps, nullptr);
+        if (rc) return rc;
+    } else {
+        {
+            Scope s(h, 3);
+            h->launches++;
+            CK(launch_k3(h->stream, sp, F, h->d_chunk_range.as<uint32_t>(), h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(),
+                         h->d_zmax.as<uint32_t>(), h->d_frame_off.as<uint32_t>(), h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(),
+                         h->d_status.as<uint8_t>(), h->d_action.as<uint8_t>(), h->d_flag_slot.as<uint32_t>(), nflag,
+                         h->d_frame_rec_base.as<uint32_t>(), h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
+                         h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>()));
+        }
         Scope s(h, 2);
         if (mode == 0) {
             if (h->n_chunks_map + h->n_chunks_qry) h->launches++;
@@ -531,84 +604,61 @@ int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_
                               h->d_bin_map.as<uint16_t>(), h->cur_map, h->d_dst_start.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
                               h->d_bin_qry.as<uint16_t>(), h->cur_qry, h->d_dst_start.as<uint32_t>() + (size_t)F * (B + 2), h->d_qry_sorted.as<float4>(),
                               h->d_qry_src.as<uint32_t>()));
-        } else if (fused) {
-            if (h->n_chunks_map) h->launches++;
-            CK(launch_k2_srt(h->stream, sp, F, h->d_chunks.as<ChunkDesc>(), h->d_chunk_range.as<uint32_t>(), h->n_chunks_map, h->d_bin_map.as<uint16_t>(),
-                             h->cur_map, poses, h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(), h->d_zmax.as<uint32_t>(), h->d_cnt.as<uint32_t>(),
-                             h->d_frame_off.as<uint32_t>(), nflag, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
-                             h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
-                             poses ? h->d_list_idx.as<uint32_t>() : nullptr, poses ? h->d_list_cnt.as<uint32_t>() : nullptr, sweep));
         } else {
             // mask modes, unfused (ERASOR_B200_UNFUSED_SRT=1): the same stable scatter, restricted to the flagged bins (K3's dense slots)
             if (h->n_chunks_map) h->launches++;
             CK(launch_k2(h->stream, h->d_chunks.as<ChunkDesc>(), 0u, h->n_chunks_map, h->d_bin_map.as<uint16_t>(), h->cur_map, poses,
                          h->d_chcnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(), h->d_flag_slot.as<uint32_t>(), nflag,
                          h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), B,
-                         poses ? h->d_list_idx.as<uint32_t>() : nullptr, poses ? h->d_list_cnt.as<uint32_t>() : nullptr,
-                         k1_big_tables(h->p.num_rings, B) ? 32 : 8));
+                         poses ? h->d_list_idx.as<uint32_t>() : nullptr, poses ? h->d_list_cnt.as<uint32_t>() : nullptr, k1_warps));
         }
     }
-    return run_k4(h, mode, keep_mask, ground_mask, fold, classes, only_rgpf, k4sweep);
+    return run_k4(h, mode, keep_mask, ground_mask, fold, classes, nullptr);
 }
 
-// A geometry sweep's launches after the query staging: every geometry's table reset, K1's geometry form (one scan of the map per
-// launch of the plan), then per geometry the sweep_ex path on its tables -- the fused Scan Ratio Test + scatter and R-GPF with every
-// class -- over the handle's one set of records and scattered points.  The geometry of setting 0 runs last, so the union counts
-// of the frame tables are its own.
-int run_tune(erasor_ctx* h, const TunePlan& tp, bool qry_xyz) {
-    const int F = h->F;
-    const NodePose* poses = h->d_poses.as<NodePose>();
-    uint32_t* nflag = h->d_nflag.as<uint32_t>() + h->f0;
-    uint32_t* frame_rej = h->d_frame_rej.as<uint32_t>() + h->f0;
-    for (int g = 0; g < tp.n_geo; ++g) {
-        const int B = tp.geo[g].t->B;
-        erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
-        h->launches++;
-        CK(launch_init_tables(h->stream, tt.zmin.as<uint32_t>(), tt.zmax.as<uint32_t>(), 2 * (size_t)F * B, tt.cnt.as<uint32_t>(), 2 * (size_t)F * (B + 1),
-                              h->d_nrecs.as<uint32_t>(), frame_rej, nflag, F, h->d_queue.as<uint32_t>()));
-    }
-    const int n_chunks = (int)(h->n_chunks_map + h->n_chunks_qry);
-    for (int l = 0; l < tp.n_launch; ++l) {
-        Scope s(h, 1);
-        K1Geo G{};
-        for (int g = tp.launch_begin[l]; g < tp.launch_begin[l + 1]; ++g) {
-            erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
-            const GeoTables& t = *tp.geo[g].t;
-            K1GeoTables& o = G.g[G.n];
-            o.T = t.view; o.B = t.B;
-            o.bin_map = tt.bin_map.as<uint16_t>(); o.bin_qry = tt.bin_qry.as<uint16_t>(); o.ch_cnt = tt.chcnt.as<uint32_t>();
-            o.zmin = tt.zmin.as<uint32_t>(); o.zmax = tt.zmax.as<uint32_t>(); o.cnt = tt.cnt.as<uint32_t>();
-            o.smem_off = G.n ? G.g[G.n - 1].smem_off + (uint32_t)k1_geo_smem_bytes(G.g[G.n - 1].T.R, G.g[G.n - 1].B) : 0u;
-            G.n++;
+// A sweep's launches after the query staging: K1, then per geometry the fused Scan Ratio Test + scatter and R-GPF with the
+// geometry's settings, over the handle's one set of records and scattered points.  An own plan runs K1 as a plain call does.  Any
+// other plan resets every geometry's tables and bins them with K1's geometry form (one scan of the map per launch of the plan),
+// then runs the geometries in reverse order, resetting the records between them, so that the union counts of the frame tables are
+// those of setting 0's geometry.  classes: R-GPF's size classes (submit() asks for class C up front unless the plan is own).
+int run_sweep(erasor_ctx* h, const SweepPlan& plan, bool qry_xyz, int classes) {
+    const int n_geo = (int)plan.geo.size();
+    int rc;
+    if (plan.own) {
+        if ((rc = run_k1(h, 2))) return rc;
+    } else {
+        for (int g = 0; g < n_geo; ++g) {
+            const K1GeoTables t = k1_tables(h, &plan, g);
+            if ((rc = run_init(h, &t))) return rc;
         }
-        const bool big = tp.launch_smem[l] > 56 * 1024;
-        if (n_chunks) h->launches++;
-        CK(launch_k1_geo(h->stream, G, tp.launch_smem[l], h->cur_map, h->cur_qry, h->d_chunks.as<ChunkDesc>(), n_chunks, F,
-                         h->d_fence.as<unsigned long long>(), poses, (big ? h->d_list_idx32 : h->d_list_idx).as<uint32_t>(),
-                         (big ? h->d_list_cnt32 : h->d_list_cnt).as<uint32_t>(), qry_xyz));
-    }
-    for (int g = tp.n_geo - 1; g >= 0; --g) {
-        const TuneGeo& tg = tp.geo[g];
-        erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
-        if (g != tp.n_geo - 1) {                  // records, queue and frame counters of the geometry before
-            h->launches++;
-            CK(launch_init_tables(h->stream, nullptr, nullptr, 0, nullptr, 0, h->d_nrecs.as<uint32_t>(), frame_rej, nflag, F, h->d_queue.as<uint32_t>()));
+        const int n_chunks = (int)(h->n_chunks_map + h->n_chunks_qry);
+        for (size_t l = 0; l + 1 < plan.launch_begin.size(); ++l) {
+            Scope s(h, 1);
+            K1Geo G{};
+            for (int g = plan.launch_begin[l]; g < plan.launch_begin[l + 1]; ++g, ++G.n) {
+                G.g[G.n] = k1_tables(h, &plan, g);
+                G.g[G.n].smem_off = G.n ? G.g[G.n - 1].smem_off + (uint32_t)k1_geo_smem_bytes(G.g[G.n - 1].T.R, G.g[G.n - 1].B) : 0u;
+            }
+            const bool big = plan.launch_smem[l] > 56 * 1024;
+            if (n_chunks) h->launches++;
+            CK(launch_k1_geo(h->stream, G, plan.launch_smem[l], h->cur_map, h->cur_qry, h->d_chunks.as<ChunkDesc>(), n_chunks, h->F,
+                             h->d_fence.as<unsigned long long>(), h->d_poses.as<NodePose>(), (big ? h->d_list_idx32 : h->d_list_idx).as<uint32_t>(),
+                             (big ? h->d_list_cnt32 : h->d_list_cnt).as<uint32_t>(), qry_xyz));
         }
+    }
+    for (int g = n_geo - 1; g >= 0; --g) {
+        const SweepGeo& sg = plan.geo[g];
+        if (g != n_geo - 1 && (rc = run_init(h, nullptr))) return rc;      // records, queue and frame counters of the geometry before
+        const K1GeoTables t = k1_tables(h, &plan, g);
         SrtParams sp = srt_params(h, h->p.version, 2);
-        sp.R = tg.t->view.R; sp.S = tg.t->view.S; sp.B = tg.t->B;
-        const bool big = tp.launch_smem[tg.launch] > 56 * 1024;      // the K1 launch that wrote g's ids, and its VoI lists
-        {
-            Scope s(h, 2);
-            if (h->n_chunks_map) h->launches++;
-            CK(launch_k2_srt(h->stream, sp, F, h->d_chunks.as<ChunkDesc>(), h->d_chunk_range.as<uint32_t>(), h->n_chunks_map, tt.bin_map.as<uint16_t>(),
-                             h->cur_map, poses, tt.chcnt.as<uint32_t>(), tt.zmin.as<uint32_t>(), tt.zmax.as<uint32_t>(), tt.cnt.as<uint32_t>(),
-                             h->d_frame_off.as<uint32_t>(), nflag, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
-                             h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
-                             (big ? h->d_list_idx32 : h->d_list_idx).as<uint32_t>(), (big ? h->d_list_cnt32 : h->d_list_cnt).as<uint32_t>(),
-                             &tg.ssw, big ? 32 : 8));
-        }
-        int rc = run_k4(h, 2, nullptr, nullptr, K4Fold{nullptr, nullptr, 0u, 0u}, 7, false, &tg.ksw);
-        if (rc) return rc;
+        sp.R = t.T.R; sp.S = t.T.S; sp.B = t.B;
+        // the warps of the K1 launch that wrote g's ids and lists: a plain launch's for an own plan, else those of g's packed launch
+        const bool big = plan.own ? k1_big_tables(t.T.R, t.B) : plan.launch_smem[sg.launch] > 56 * 1024;
+        const bool lists32 = big && !plan.own;
+        if ((rc = run_k2_srt(h, sp, t, (lists32 ? h->d_list_idx32 : h->d_list_idx).as<uint32_t>(), (lists32 ? h->d_list_cnt32 : h->d_list_cnt).as<uint32_t>(),
+                             big ? 32 : 8, &sg.ssw)))
+            return rc;
+        if ((rc = run_k4(h, 2, nullptr, nullptr, K4Fold{nullptr, nullptr, 0u, 0u}, classes, &sg.ksw))) return rc;
     }
     return ERASOR_OK;
 }
@@ -744,8 +794,6 @@ int erasor_create(const erasor_params_t* params, int device, erasor_handle_t* ou
     if (const char* ng = std::getenv("ERASOR_B200_NO_GRAPH")) h->use_graphs = !(ng[0] == '1');
     if (const char* uf = std::getenv("ERASOR_B200_UNFUSED_SRT")) h->fused_srt = !(uf[0] == '1');
     if (const char* cs = std::getenv("ERASOR_B200_CTAS_PER_SM")) h->ctas_per_sm = std::max(1, std::min(8, std::atoi(cs)));
-    std::string terr;
-    if (build_bin_tables(p, h->tables, terr) != 0) { g_create_error = terr; delete h; return ERASOR_E_INVALID; }
     auto fail = [&](const char* what, cudaError_t ce) {
         g_create_error = std::string(what) + ": " + cudaGetErrorString(ce);
         erasor_destroy(h);
@@ -757,11 +805,13 @@ int erasor_create(const erasor_params_t* params, int device, erasor_handle_t* ou
     h->sm_count = prop.multiProcessorCount;
     h->smem_optin = (size_t)prop.sharedMemPerBlockOptin;
     if (const char* tu = std::getenv("ERASOR_B200_TUNE_UNPACKED")) h->tune_unpacked = tu[0] == '1';
-    const size_t need = std::max(k1_smem_bytes(p.num_rings, h->B), k3_smem_bytes(h->B));
-    if (need > (size_t)prop.sharedMemPerBlockOptin) {
-        g_create_error = "num_rings*num_sectors too large for the per-CTA shared-memory bin table";
+    // the handle's polar tables: the first entry of its geometry cache (tables build_bin_tables rejects: ERASOR_E_INVALID; beyond
+    // the device's shared memory: ERASOR_E_UNSUPPORTED)
+    const GeoTables* own = nullptr;
+    if (const int rc = geometry_tables(h, own_geometry(p), &own)) {
+        g_create_error = h->err;
         erasor_destroy(h);
-        return ERASOR_E_UNSUPPORTED;
+        return rc;
     }
     // R-GPF's bins are long serial chains: its CTAs go first whenever SM resources free up (highest stream priority), the
     // bandwidth / issue-bound kernels of this and of overlapped handles fill in around them
@@ -776,20 +826,10 @@ int erasor_create(const erasor_params_t* params, int device, erasor_handle_t* ou
     if ((e = cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
     if ((e = cudaEventCreateWithFlags(&h->ev_join_b, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
     if ((e = cudaEventCreateWithFlags(&h->ev_join_c, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
-    const size_t rb = sizeof(double) * h->tables.ring_thr.size(), sb = sizeof(SectorBoundary) * h->tables.sec_pos.size();
     if ((e = h->h_words.allocate(128)) != cudaSuccess) return fail("cudaMallocHost", e);
     std::memset(h->h_words.p(), 0, 128);
-    const size_t gb = sizeof(float) * h->tables.ring_guard.size();
-    if ((e = h->d_guard.ensure(gb)) != cudaSuccess) return fail("cudaMalloc", e);
-    if ((e = cudaMemcpy(h->d_guard.p(), h->tables.ring_guard.data(), gb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
-    if ((e = h->d_ring.ensure(rb)) != cudaSuccess || (e = h->d_pos.ensure(sb)) != cudaSuccess || (e = h->d_neg.ensure(sb)) != cudaSuccess ||
-        (e = h->d_fence.ensure(sizeof(unsigned long long) * 4)) != cudaSuccess)
-        return fail("cudaMalloc", e);
-    if ((e = cudaMemcpy(h->d_ring.p(), h->tables.ring_thr.data(), rb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
-    if ((e = cudaMemcpy(h->d_pos.p(), h->tables.sec_pos.data(), sb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
-    if ((e = cudaMemcpy(h->d_neg.p(), h->tables.sec_neg.data(), sb, cudaMemcpyHostToDevice)) != cudaSuccess) return fail("cudaMemcpy", e);
+    if ((e = h->d_fence.ensure(sizeof(unsigned long long) * 4)) != cudaSuccess) return fail("cudaMalloc", e);
     if ((e = cudaMemset(h->d_fence.p(), 0, sizeof(unsigned long long) * 4)) != cudaSuccess) return fail("cudaMemset", e);
-    h->view = h->tables.view(h->d_ring.as<double>(), h->d_pos.as<SectorBoundary>(), h->d_neg.as<SectorBoundary>(), h->d_guard.as<float>());
     *out = h;
     return ERASOR_OK;
 }
@@ -908,7 +948,7 @@ int erasor_compare(erasor_handle_t h, int version, int frame) {
     if ((rc = assemble())) return rc;
     const uint32_t n_class_c = h->words()[11];
     if (!with_c && n_class_c > 0) {
-        if ((rc = run_compare(h, version, 0, h->d_keep.as<uint8_t>(), h->d_ground.as<uint8_t>(), K4Fold{nullptr, nullptr, 0u, 0u}, 4, true))) return rc;
+        if ((rc = run_k4(h, 0, h->d_keep.as<uint8_t>(), h->d_ground.as<uint8_t>(), K4Fold{nullptr, nullptr, 0u, 0u}, 4, nullptr))) return rc;
         if ((rc = assemble())) return rc;
     }
     h->class_c_state = (int)std::min<uint32_t>(n_class_c, 0x7FFFFFFFu);
@@ -1105,19 +1145,14 @@ int enqueue(erasor_ctx* h, const Step& s) {
     if ((rc = stage_host_clouds(h, s.ptr_kind, s.mode == 1 ? s.map_xyzi : nullptr, s.qry_xyzi, s.qry_xyz ? 3 * sizeof(float) : sizeof(float4)))) return rc;
     if (s.mode == 2) CK(cudaMemcpyAsync(h->d_poses.p(), h->h_pose.p(), sizeof(NodePose) * (size_t)h->F, cudaMemcpyHostToDevice, h->stream));
     if (s.n_keep) CK(cudaMemsetAsync(s.d_keep, 1, s.n_keep, h->stream));
-    if (s.ssw.n) {
-        CK(cudaMemsetAsync(s.ssw.n_flagged, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
-        CK(cudaMemsetAsync(s.ksw.rejected, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
-    }
-    if (s.tune) {
-        for (int g = 0; g < s.tune->n_geo; ++g)
-            CK(cudaMemsetAsync(s.tune->geo[g].ssw.n_flagged, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
-        CK(cudaMemsetAsync(s.tune->geo[0].ksw.rejected, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
-        if ((rc = run_tune(h, *s.tune, s.qry_xyz))) return rc;
+    if (s.sweep) {
+        for (const SweepGeo& sg : s.sweep->geo)
+            CK(cudaMemsetAsync(sg.ssw.n_flagged, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
+        CK(cudaMemsetAsync(s.sweep->geo[0].ksw.rejected, 0, sizeof(uint32_t) * kMaxSweepVariants * (size_t)h->F, h->stream));
+        if ((rc = run_sweep(h, *s.sweep, s.qry_xyz, s.with_c ? 7 : 3))) return rc;
     } else {
         if ((rc = run_k1(h, s.mode))) return rc;
-        if ((rc = run_compare(h, h->p.version, s.mode, s.d_keep, nullptr, s.fold, s.with_c ? 7 : 3, false, s.ssw.n ? &s.ssw : nullptr,
-                              s.ssw.n ? &s.ksw : nullptr))) return rc;
+        if ((rc = run_compare(h, h->p.version, s.mode, s.d_keep, nullptr, s.fold, s.with_c ? 7 : 3))) return rc;
     }
     if (s.inserts && (rc = run_insert_assemble(h))) return rc;      // (run_compare ran the plan and the query scatter under R-GPF)
     CK(cudaMemcpyAsync(h->h_words.as<uint32_t>() + 1, h->d_queue.as<uint32_t>() + kBucketC0, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
@@ -1194,50 +1229,46 @@ int submit(erasor_ctx* h, Step st, const uint64_t* map_off, const uint64_t* qry_
             std::memcpy(h->h_ins_fwd.as<float>() + 12 * (size_t)f, T.m, sizeof(float) * 12);
         }
     }
-    if (st.ssw.n) {
-        const size_t rows = (size_t)kMaxSweepVariants * (size_t)std::max(h->stat_F, h->f0 + F);
-        CK(h->d_sweep_flag.ensure(sizeof(uint32_t) * rows));
-        CK(h->d_sweep_rej.ensure(sizeof(uint32_t) * rows));
-        st.ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + (size_t)kMaxSweepVariants * st.f0;
-        st.ksw.rejected = h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * st.f0;
-        st.ksw.n = (uint32_t)st.n_map_global;
-    } else if (st.tune) {
-        // geometry sweep: every geometry's batch tables, records for the largest geometry, one block of per-setting flag counters
-        // per geometry; class C always runs up front (the records of one geometry are gone once the next one has run)
-        auto plan = std::make_shared<TunePlan>(*st.tune);
-        const size_t n_chunks = (size_t)h->n_chunks_map + h->n_chunks_qry;
-        while (h->tune_tabs.size() < (size_t)plan->n_geo) h->tune_tabs.emplace_back(new erasor_ctx::TuneTabs(h->alloc_epoch));
-        for (int g = 0; g < plan->n_geo; ++g) {
-            const size_t B = (size_t)plan->geo[g].t->B;
-            erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
-            CK(tt.bin_map.ensure(sizeof(uint16_t) * (h->NM + kIdPad)));
-            CK(tt.bin_qry.ensure(sizeof(uint16_t) * (h->NQ + kIdPad)));
-            CK(tt.chcnt.ensure(sizeof(uint32_t) * std::max<size_t>(n_chunks, 1) * (B + 1)));
-            CK(tt.zmin.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
-            CK(tt.zmax.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
-            CK(tt.cnt.ensure(sizeof(uint32_t) * 2 * (size_t)F * (B + 1)));
-        }
-        for (int l = 0; l < plan->n_launch; ++l)
-            if (plan->launch_smem[l] > 56 * 1024) {
-                CK(h->d_list_idx32.ensure(sizeof(uint32_t) * (h->NM + kIdPad)));
-                CK(h->d_list_cnt32.ensure(sizeof(uint32_t) * kListWarps * std::max<size_t>(n_chunks, 1)));
+    if (st.sweep) {
+        // a sweep: one block of per-setting flag counters per geometry, records for the largest geometry; a plan that is not own
+        // also bins every geometry into its batch tables (and a 32-warp launch into its own VoI lists) and runs class C up front
+        // (the records of one geometry are gone once the next one has run)
+        auto plan = std::make_shared<SweepPlan>(*st.sweep);
+        const size_t n_geo = plan->geo.size(), n_chunks = (size_t)h->n_chunks_map + h->n_chunks_qry;
+        if (!plan->own) {
+            while (h->tune_tabs.size() < n_geo) h->tune_tabs.emplace_back(new erasor_ctx::TuneTabs(h->alloc_epoch));
+            for (size_t g = 0; g < n_geo; ++g) {
+                const size_t B = (size_t)plan->geo[g].t->B;
+                erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
+                CK(tt.bin_map.ensure(sizeof(uint16_t) * (h->NM + kIdPad)));
+                CK(tt.bin_qry.ensure(sizeof(uint16_t) * (h->NQ + kIdPad)));
+                CK(tt.chcnt.ensure(sizeof(uint32_t) * std::max<size_t>(n_chunks, 1) * (B + 1)));
+                CK(tt.zmin.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
+                CK(tt.zmax.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
+                CK(tt.cnt.ensure(sizeof(uint32_t) * 2 * (size_t)F * (B + 1)));
             }
+            for (size_t smem : plan->launch_smem)
+                if (smem > 56 * 1024) {
+                    CK(h->d_list_idx32.ensure(sizeof(uint32_t) * (h->NM + kIdPad)));
+                    CK(h->d_list_cnt32.ensure(sizeof(uint32_t) * kListWarps * std::max<size_t>(n_chunks, 1)));
+                }
+            st.with_c = true;
+        }
         const uint32_t recs = (uint32_t)std::min<size_t>((size_t)F * plan->B_max, kMaxRecords);
         if (recs > h->rec_capacity) {
             CK(h->d_recs.ensure(sizeof(FlagRec) * (size_t)recs));
             CK(h->d_bucket.ensure(sizeof(uint32_t) * (size_t)kNumBuckets * recs));
             h->rec_capacity = recs;
         }
-        const size_t rows = (size_t)kMaxSweepVariants * (size_t)h->stat_F;
-        CK(h->d_sweep_flag.ensure(sizeof(uint32_t) * rows * (size_t)plan->n_geo));
+        const size_t rows = (size_t)kMaxSweepVariants * (size_t)std::max(h->stat_F, h->f0 + F);
+        CK(h->d_sweep_flag.ensure(sizeof(uint32_t) * rows * n_geo));
         CK(h->d_sweep_rej.ensure(sizeof(uint32_t) * rows));
-        for (int g = 0; g < plan->n_geo; ++g) {
-            plan->geo[g].ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + rows * (size_t)g + (size_t)kMaxSweepVariants * st.f0;
+        for (size_t g = 0; g < n_geo; ++g) {
+            plan->geo[g].ssw.n_flagged = h->d_sweep_flag.as<uint32_t>() + rows * g + (size_t)kMaxSweepVariants * st.f0;
             plan->geo[g].ksw.rejected = h->d_sweep_rej.as<uint32_t>() + (size_t)kMaxSweepVariants * st.f0;
             plan->geo[g].ksw.n = (uint32_t)st.n_map_global;
         }
-        st.tune = plan;
-        st.with_c = true;
+        st.sweep = plan;
     } else if (st.mode == 2) {
         st.fold = K4Fold{h->map->d_keep.as<uint8_t>(), nullptr, (uint32_t)st.n_map_global, 0u};   // a sweep leaves the map's mask alone
     }
@@ -1312,12 +1343,12 @@ int process_frames_impl(erasor_handle_t h, const float* map_xyzi, const uint64_t
 }
 
 // |map_voi_| of every node of the last submission = binned + complement counts of the map cloud (K1's tables), into out[0, F)
-// (after a geometry sweep: the tables of any geometry hold them; those of setting 0's are read)
+// (after a sweep: the tables of any of its geometries hold them; those of geometry 0 are read)
 int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
-    const bool tune = h->last.mode == 2 && h->last.tune;
-    const size_t row = (size_t)(tune ? h->last.tune->geo[0].t->B : h->B) + 1;
+    const K1GeoTables t = k1_tables(h, h->last.mode == 2 ? h->last.sweep.get() : nullptr, 0);
+    const size_t row = (size_t)t.B + 1;
     std::vector<uint32_t> c((size_t)h->F * row);
-    CK(cudaMemcpy(c.data(), (tune ? h->tune_tabs[0]->cnt : h->d_cnt).p(), sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(c.data(), t.cnt, sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
     for (int f = 0; f < h->F; ++f) {
         uint64_t t = 0;
         for (size_t b = 0; b < row; ++b) t += c[(size_t)f * row + b];
@@ -1328,7 +1359,7 @@ int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
 
 int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                        double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind, bool async,
-                       const SrtSweep* sweep = nullptr, const K4Sweep* groups = nullptr, std::shared_ptr<const TunePlan> tune = nullptr) {
+                       std::shared_ptr<const SweepPlan> sweep = nullptr) {
     if (!h || !poses7 || !query_offsets) { if (h) h->err = "null argument"; return ERASOR_E_INVALID; }
     if (!h->map) { h->err = "erasor_process_nodes: no map attached (erasor_attach_map)"; return ERASOR_E_STATE; }
     if (n_frames <= 0) { h->err = "n_frames must be positive"; return ERASOR_E_INVALID; }
@@ -1344,19 +1375,18 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
     const size_t N = h->map->n;
     const double range = voi_max_range > 0.0 ? voi_max_range : h->p.max_range;
     h->stat_F = n_frames;
-    h->sweep_V = sweep ? sweep->n : tune ? tune->n_settings : 0;
-    h->sweep_G = tune ? tune->n_geo : 1;
+    h->sweep_V = sweep ? sweep->geo[0].ssw.n : 0;
     h->ins_call_off.assign(h->node_inserts ? 1 : 0, 0);
     // scratch per (frame, map point): bin id 2 + scattered point 16 + source index 4 + class-C scratch 24 bytes; with inserts also
     // R-GPF's partitioned copy 16 + the inserts 16 + K4b's voxels 16 and scratch 36 bytes
     size_t budget = (size_t)16 << 30;
     if (const char* e = std::getenv("ERASOR_B200_NODE_SCRATCH_GB")) budget = (size_t)std::max(1.0, std::atof(e)) << 30;
-    // (a geometry sweep: also per geometry its bin id 2 bytes and its chunk count rows, at most 4 (B + 1) / (5 B) bytes, and the
-    // VoI lists of its 32-warp K1 launches 4 bytes)
-    const size_t per_point = (h->node_inserts ? 130 : 46) + (tune ? 3 * (size_t)tune->n_geo + 4 : 0);
+    // (a sweep plan that is not own: also per geometry its bin id 2 bytes and its chunk count rows, at most 4 (B + 1) / (5 B) bytes,
+    // and the VoI lists of its 32-warp K1 launches 4 bytes)
+    const size_t per_point = (h->node_inserts ? 130 : 46) + (sweep && !sweep->own ? 3 * sweep->geo.size() + 4 : 0);
     const size_t by_mem = std::max<size_t>(1, budget / (per_point * std::max<size_t>(N, 1)));
     const size_t by_idx = std::max<size_t>(1, (size_t)0xFFFFFFF0ull / std::max<size_t>(N, 1) - 1);
-    const size_t B_max = tune ? (size_t)std::max(h->B, tune->B_max) : (size_t)h->B;
+    const size_t B_max = sweep ? (size_t)std::max(h->B, sweep->B_max) : (size_t)h->B;
     const int max_frames = (int)std::min<size_t>({by_mem, by_idx, std::max<size_t>(1, kMaxRecords / B_max), (size_t)n_frames});
     std::vector<uint64_t> mo, qo;
     std::vector<NodePose> poses;
@@ -1380,8 +1410,7 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         st.qry_xyzi = query_xyzi ? query_xyzi + (qxyz ? 3 : 4) * q0 : nullptr;
         st.user_keep = frame_keep ? frame_keep + (size_t)f0 * N : nullptr;
         st.keep_out = (f1 == n_frames) ? keep_out : nullptr;
-        if (sweep) { st.ssw = *sweep; st.ksw = *groups; }
-        st.tune = tune;
+        st.sweep = sweep;
         if ((rc = submit(h, st, mo.data(), qo.data(), F, poses.data(), poses7 + 7 * (size_t)f0))) return rc;
         if (f1 < n_frames) {                                         // the next sub-batch reuses the handle's buffers
             if ((rc = erasor_wait(h))) return rc;
@@ -1408,7 +1437,8 @@ int erasor_wait(erasor_handle_t h) {
         if (!s.with_c && h->class_c_count_host > 0) {
             // bins beyond class B's capacity turned up in a submission that ran without class C: run that class now (R-GPF only; the
             // bins are independent, the masks only gain zeros), then repeat the output copies.  The next submissions launch it up front.
-            int rc = run_compare(h, h->p.version, s.mode, s.d_keep, nullptr, s.fold, 4, true, nullptr, s.ssw.n ? &s.ksw : nullptr);
+            // (A sweep that gets here has an own plan, whose geometry 0 is the handle's: the others launch class C up front.)
+            int rc = run_k4(h, s.mode, s.d_keep, nullptr, s.fold, 4, s.sweep ? &s.sweep->geo[0].ksw : nullptr);
             if (rc) return rc;
             if (s.inserts && (rc = run_insert_assemble(h))) return rc;
             if ((rc = copy_masks_out(h, s))) return rc;
@@ -1535,182 +1565,125 @@ int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const fl
     return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, frame_keep, keep_out, ptr_kind, true);
 }
 
+extern "C++" {   // (a template and overloads: C++ linkage)
 namespace {
-// The sweeps' common path: the settings' Scan Ratio Test fields go to K2, their ground-filter fields are grouped for K4 (one
-// GpfParams per distinct tuple, in order of first appearance, with the settings that carry it).
-int process_nodes_sweep_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
-                             double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind, bool async) {
+// Every sweep entry point's settings as erasor_process_nodes_tune takes them: erasor_process_nodes_sweep's with the handle's
+// geometry and ground-filter fields, erasor_process_nodes_sweep_ex's with the handle's geometry
+erasor_tune_setting_t widen(const erasor_ctx*, const erasor_tune_setting_t& x) { return x; }
+erasor_tune_setting_t widen(const erasor_ctx* h, const erasor_sweep_setting_t& x) { return erasor_tune_setting_t{own_geometry(h->p), x}; }
+erasor_tune_setting_t widen(const erasor_ctx* h, const erasor_srt_variant_t& x) {
+    return widen(h, erasor_sweep_setting_t{x.scan_ratio_threshold, x.th_bin_max_h, h->p.gf_dist_thr, h->p.gf_th_seeds_height, x.minimum_num_pts,
+                                           h->p.num_lowest_pts, h->p.gf_num_lpr, h->p.gf_iter});
+}
+
+// The sweeps' one path (fn: the entry point, for the messages): the settings' checks, then their plan.  The settings are split by
+// geometry (first appearance order); per geometry their Scan Ratio Test fields go to K2 and their ground-filter fields are grouped
+// for K4 (one GpfParams per distinct tuple, in order of first appearance, with the settings that carry it).  The plan is own when
+// every setting carries the handle's geometry.  Otherwise its geometries are packed into K1 launches of at most 56 KB of tables, so
+// that every launch keeps the four 8-warp CTAs per SM of the plain kernel (a geometry beyond that runs alone in the 32-warp form,
+// as it would in a plain call).
+template <class Setting>
+int process_nodes_sweep(erasor_handle_t h, const char* fn, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets,
+                        int n_frames, double voi_max_range, const Setting* settings, int n_settings, uint8_t* variant_keep, int ptr_kind, bool async) {
     if (!h) return ERASOR_E_INVALID;
     if (n_settings < 1 || n_settings > kMaxSweepVariants) { h->err = "n_variants must be in [1, 32]"; return ERASOR_E_INVALID; }
     if (!settings || !variant_keep) { h->err = "null variants or variant_keep"; return ERASOR_E_INVALID; }
+    erasor_tune_setting_t x[kMaxSweepVariants];
+    for (int v = 0; v < n_settings; ++v) x[v] = widen(h, settings[v]);
     for (int v = 0; v < n_settings; ++v)
-        if (settings[v].gf_iter > kMaxIter) { h->err = "gf_iter above the tap capacity (8)"; return ERASOR_E_UNSUPPORTED; }
-    if (!h->map) { h->err = "erasor_process_nodes_sweep: no map attached (erasor_attach_map)"; return ERASOR_E_INVALID; }
+        if (x[v].s.gf_iter > kMaxIter) { h->err = "gf_iter above the tap capacity (8)"; return ERASOR_E_UNSUPPORTED; }
+    if (!h->map) { h->err = std::string(fn) + ": no map attached (erasor_attach_map)"; return ERASOR_E_INVALID; }
     if (h->node_inserts) { h->err = "a sweep has no node inserts: erasor_set_node_inserts(h, 0) first"; return ERASOR_E_INVALID; }
-    if (h->pending) { h->err = "erasor_process_nodes_sweep while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
-    SrtSweep variants{};
-    K4Sweep groups{};
-    variants.n = n_settings;
-    groups.keep = variant_keep;
-    for (int v = 0; v < n_settings; ++v) {
-        const erasor_sweep_setting_t& x = settings[v];
-        variants.v[v] = SrtVariant{x.scan_ratio_threshold, x.th_bin_max_h, x.minimum_num_pts, 0};
-        GpfParams gp{};
-        gp.th_dist = x.gf_dist_thr; gp.th_seeds = x.gf_th_seeds_height; gp.num_lowest_pts = x.num_lowest_pts;
-        gp.num_lpr = x.gf_num_lpr; gp.iters = x.gf_iter; gp.cov_mode = h->p.cov_mode;
-        int g = 0;
-        while (g < groups.n_groups && std::memcmp(&groups.gp[g], &gp, sizeof(GpfParams)) != 0) ++g;
-        if (g == groups.n_groups) groups.gp[groups.n_groups++] = gp;
-        groups.bits[g] |= 1u << v;
-    }
-    return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, nullptr, nullptr, ptr_kind, async, &variants, &groups);
-}
-
-// erasor_process_nodes_sweep: the settings with the handle's ground-filter fields (one group)
-int process_nodes_srt_sweep(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
-                            double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind, bool async) {
-    erasor_sweep_setting_t settings[kMaxSweepVariants];
-    const bool ok = h && variants && n_variants >= 1 && n_variants <= kMaxSweepVariants;     // otherwise the common path refuses
-    for (int v = 0; ok && v < n_variants; ++v)
-        settings[v] = erasor_sweep_setting_t{variants[v].scan_ratio_threshold, variants[v].th_bin_max_h, h->p.gf_dist_thr, h->p.gf_th_seeds_height,
-                                             variants[v].minimum_num_pts, h->p.num_lowest_pts, h->p.gf_num_lpr, h->p.gf_iter};
-    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, ok ? settings : nullptr, n_variants,
-                                    variant_keep, ptr_kind, async);
-}
-
-bool same_geometry(const erasor_geometry_t& a, const erasor_geometry_t& b) {
-    return a.max_range == b.max_range && a.min_h == b.min_h && a.max_h == b.max_h && a.num_rings == b.num_rings && a.num_sectors == b.num_sectors;
-}
-
-// The tables of geometry x: the handle's cached ones, or built now with erasor_create's checks and codes
-int geometry_tables(erasor_ctx* h, const erasor_geometry_t& x, const GeoTables** out) {
-    for (const auto& t : h->geo_tables)
-        if (same_geometry(t->key, x)) { *out = t.get(); return ERASOR_OK; }
-    const long long Bll = (long long)x.num_rings * (long long)x.num_sectors;
-    if (x.num_rings < 1 || x.num_sectors < 1 || Bll > 65534) { h->err = "num_rings*num_sectors must be in [1, 65534]"; return ERASOR_E_INVALID; }
-    erasor_params_t p = h->p;
-    p.max_range = x.max_range; p.min_h = x.min_h; p.max_h = x.max_h; p.num_rings = x.num_rings; p.num_sectors = x.num_sectors;
-    std::unique_ptr<GeoTables> t(new GeoTables());
-    t->key = x; t->B = (int)Bll;
-    std::string terr;
-    if (build_bin_tables(p, t->host, terr) != 0) { h->err = terr; return ERASOR_E_INVALID; }
-    if (std::max(k1_smem_bytes(x.num_rings, t->B), k3_smem_bytes(t->B)) > h->smem_optin) {
-        h->err = "num_rings*num_sectors too large for the per-CTA shared-memory bin table";
-        return ERASOR_E_UNSUPPORTED;
-    }
-    const HostBinTables& ht = t->host;
-    const size_t rb = sizeof(double) * ht.ring_thr.size(), sb = sizeof(SectorBoundary) * ht.sec_pos.size(), gb = sizeof(float) * ht.ring_guard.size();
-    CK(t->d_ring.allocate(rb)); CK(t->d_pos.allocate(sb)); CK(t->d_neg.allocate(sb)); CK(t->d_guard.allocate(gb));
-    CK(cudaMemcpy(t->d_ring.p(), ht.ring_thr.data(), rb, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(t->d_pos.p(), ht.sec_pos.data(), sb, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(t->d_neg.p(), ht.sec_neg.data(), sb, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(t->d_guard.p(), ht.ring_guard.data(), gb, cudaMemcpyHostToDevice));
-    t->view = ht.view(t->d_ring.as<double>(), t->d_pos.as<SectorBoundary>(), t->d_neg.as<SectorBoundary>(), t->d_guard.as<float>());
-    h->geo_tables.push_back(std::move(t));
-    *out = h->geo_tables.back().get();
-    return ERASOR_OK;
-}
-
-// erasor_process_nodes_tune: the handle's own geometry alone is sweep_ex; otherwise the settings are split by geometry (first
-// appearance order) and the geometries packed into K1 launches of at most 56 KB of tables, so that every launch keeps the
-// four 8-warp CTAs per SM of the plain kernel (a geometry beyond that runs alone in the 32-warp form, as it would in a plain call).
-int process_nodes_tune_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
-                            double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind, bool async) {
-    if (!h) return ERASOR_E_INVALID;
-    if (n_settings < 1 || n_settings > kMaxSweepVariants) { h->err = "n_variants must be in [1, 32]"; return ERASOR_E_INVALID; }
-    if (!settings || !variant_keep) { h->err = "null variants or variant_keep"; return ERASOR_E_INVALID; }
-    const erasor_geometry_t own{h->p.max_range, h->p.min_h, h->p.max_h, h->p.num_rings, h->p.num_sectors};
-    erasor_sweep_setting_t ss[kMaxSweepVariants];
-    bool all_own = true;
-    for (int v = 0; v < n_settings; ++v) { ss[v] = settings[v].s; all_own = all_own && same_geometry(settings[v].geometry, own); }
-    if (all_own) return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, ss, n_settings, variant_keep, ptr_kind, async);
-    for (int v = 0; v < n_settings; ++v)
-        if (ss[v].gf_iter > kMaxIter) { h->err = "gf_iter above the tap capacity (8)"; return ERASOR_E_UNSUPPORTED; }
-    if (!h->map) { h->err = "erasor_process_nodes_tune: no map attached (erasor_attach_map)"; return ERASOR_E_INVALID; }
-    if (h->node_inserts) { h->err = "a sweep has no node inserts: erasor_set_node_inserts(h, 0) first"; return ERASOR_E_INVALID; }
-    if (h->pending) { h->err = "erasor_process_nodes_tune while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
+    if (h->pending) { h->err = std::string(fn) + " while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
     double range = voi_max_range;
     if (!(range > 0.0)) {
         for (int v = 1; v < n_settings; ++v)
-            if (settings[v].geometry.max_range != settings[0].geometry.max_range) {
+            if (x[v].geometry.max_range != x[0].geometry.max_range) {
                 h->err = "voi_max_range <= 0 takes the settings' max_range, and they differ: pass the VoI radius";
                 return ERASOR_E_INVALID;
             }
-        range = settings[0].geometry.max_range;
+        range = x[0].geometry.max_range;
     }
     CK(cudaSetDevice(h->device));
-    auto plan = std::make_shared<TunePlan>();
-    TunePlan& tp = *plan;
-    tp.n_settings = n_settings;
+    auto plan = std::make_shared<SweepPlan>();
     int geo_of[kMaxSweepVariants];
     for (int v = 0; v < n_settings; ++v) {
-        int g = 0;
-        while (g < tp.n_geo && !same_geometry(tp.geo[g].t->key, settings[v].geometry)) ++g;
-        if (g == tp.n_geo) {
+        size_t g = 0;
+        while (g < plan->geo.size() && !same_geometry(plan->geo[g].t->key, x[v].geometry)) ++g;
+        if (g == plan->geo.size()) {
             const GeoTables* t = nullptr;
-            int rc = geometry_tables(h, settings[v].geometry, &t);
+            int rc = geometry_tables(h, x[v].geometry, &t);
             if (rc) return rc;
-            tp.geo[tp.n_geo++].t = t;
-            tp.B_max = std::max(tp.B_max, t->B);
+            plan->geo.push_back(SweepGeo{t, 0, {}, {}});
+            plan->B_max = std::max(plan->B_max, t->B);
         }
-        geo_of[v] = g;
+        geo_of[v] = (int)g;
     }
-    for (int g = 0; g < tp.n_geo; ++g) {
-        // sweep_ex's state over the settings of geometry g; the others take part with no bin flagged
-        TuneGeo& tg = tp.geo[g];
-        tg.ssw.n = n_settings;
-        tg.ksw.keep = variant_keep;
+    plan->own = plan->geo.size() == 1 && plan->geo[0].t == h->geo_tables[0].get();
+    for (int g = 0; g < (int)plan->geo.size(); ++g) {
+        // the settings of geometry g; the others take part with no bin flagged
+        SweepGeo& sg = plan->geo[g];
+        sg.ssw.n = n_settings;
+        sg.ksw.keep = variant_keep;
         for (int v = 0; v < n_settings; ++v) {
-            const erasor_sweep_setting_t& x = ss[v];
-            tg.ssw.v[v] = SrtVariant{x.scan_ratio_threshold, x.th_bin_max_h, geo_of[v] == g ? x.minimum_num_pts : -1, 0};
+            const erasor_sweep_setting_t& s = x[v].s;
+            sg.ssw.v[v] = SrtVariant{s.scan_ratio_threshold, s.th_bin_max_h, geo_of[v] == g ? s.minimum_num_pts : -1, 0};
             if (geo_of[v] != g) continue;
             GpfParams gp{};
-            gp.th_dist = x.gf_dist_thr; gp.th_seeds = x.gf_th_seeds_height; gp.num_lowest_pts = x.num_lowest_pts;
-            gp.num_lpr = x.gf_num_lpr; gp.iters = x.gf_iter; gp.cov_mode = h->p.cov_mode;
+            gp.th_dist = s.gf_dist_thr; gp.th_seeds = s.gf_th_seeds_height; gp.num_lowest_pts = s.num_lowest_pts;
+            gp.num_lpr = s.gf_num_lpr; gp.iters = s.gf_iter; gp.cov_mode = h->p.cov_mode;
             int k = 0;
-            while (k < tg.ksw.n_groups && std::memcmp(&tg.ksw.gp[k], &gp, sizeof(GpfParams)) != 0) ++k;
-            if (k == tg.ksw.n_groups) tg.ksw.gp[tg.ksw.n_groups++] = gp;
-            tg.ksw.bits[k] |= 1u << v;
+            while (k < sg.ksw.n_groups && std::memcmp(&sg.ksw.gp[k], &gp, sizeof(GpfParams)) != 0) ++k;
+            if (k == sg.ksw.n_groups) sg.ksw.gp[sg.ksw.n_groups++] = gp;
+            sg.ksw.bits[k] |= 1u << v;
         }
+        if (plan->own) continue;
         // K1 packing
-        const size_t bytes = k1_geo_smem_bytes(tg.t->view.R, tg.t->B);
+        const size_t bytes = k1_geo_smem_bytes(sg.t->view.R, sg.t->B);
         const bool alone = h->tune_unpacked || bytes > 56 * 1024;
-        if (g == 0 || alone || tp.launch_smem[tp.n_launch - 1] + bytes > 56 * 1024 || tp.launch_smem[tp.n_launch - 1] > 56 * 1024) {
-            tp.launch_begin[tp.n_launch] = g;
-            tp.launch_smem[tp.n_launch++] = 0;
+        if (g == 0 || alone || plan->launch_smem.back() + bytes > 56 * 1024 || plan->launch_smem.back() > 56 * 1024) {
+            plan->launch_begin.push_back(g);
+            plan->launch_smem.push_back(0);
         }
-        tg.launch = tp.n_launch - 1;
-        tp.launch_smem[tg.launch] += bytes;
-        tp.launch_begin[tp.n_launch] = g + 1;
+        sg.launch = (int)plan->launch_smem.size() - 1;
+        plan->launch_smem.back() += bytes;
     }
-    return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, range, nullptr, nullptr, ptr_kind, async, nullptr, nullptr, plan);
+    if (!plan->own) plan->launch_begin.push_back((int)plan->geo.size());
+    return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, range, nullptr, nullptr, ptr_kind, async, plan);
 }
 }  // namespace
+}  // extern "C++"
 
 int erasor_process_nodes_sweep(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind) {
-    return process_nodes_srt_sweep(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants, variant_keep, ptr_kind, false);
+    return process_nodes_sweep(h, "erasor_process_nodes_sweep", poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants,
+                               variant_keep, ptr_kind, false);
 }
 int erasor_process_nodes_sweep_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                      double voi_max_range, const erasor_srt_variant_t* variants, int n_variants, uint8_t* variant_keep, int ptr_kind) {
-    return process_nodes_srt_sweep(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants, variant_keep, ptr_kind, true);
+    return process_nodes_sweep(h, "erasor_process_nodes_sweep", poses7, query_xyzi, query_offsets, n_frames, voi_max_range, variants, n_variants,
+                               variant_keep, ptr_kind, true);
 }
 int erasor_process_nodes_sweep_ex(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                   double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind) {
-    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, false);
+    return process_nodes_sweep(h, "erasor_process_nodes_sweep_ex", poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings,
+                               variant_keep, ptr_kind, false);
 }
 int erasor_process_nodes_sweep_ex_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                         double voi_max_range, const erasor_sweep_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind) {
-    return process_nodes_sweep_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, true);
+    return process_nodes_sweep(h, "erasor_process_nodes_sweep_ex", poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings,
+                               variant_keep, ptr_kind, true);
 }
 
 int erasor_process_nodes_tune(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                               double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind) {
-    return process_nodes_tune_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, false);
+    return process_nodes_sweep(h, "erasor_process_nodes_tune", poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings,
+                               variant_keep, ptr_kind, false);
 }
 int erasor_process_nodes_tune_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                     double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind) {
-    return process_nodes_tune_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings, variant_keep, ptr_kind, true);
+    return process_nodes_sweep(h, "erasor_process_nodes_tune", poses7, query_xyzi, query_offsets, n_frames, voi_max_range, settings, n_settings,
+                               variant_keep, ptr_kind, true);
 }
 
 int erasor_get_sweep_stats(erasor_handle_t h, uint32_t* n_flagged_bins, uint32_t* n_rejected_points) {
@@ -1719,13 +1692,13 @@ int erasor_get_sweep_stats(erasor_handle_t h, uint32_t* n_flagged_bins, uint32_t
     int rc;
     if ((rc = erasor_wait(h))) return rc;
     const size_t F = (size_t)h->stat_F, V = (size_t)h->sweep_V;
-    // a geometry sweep's flag counters: one block per geometry, each setting counted in its own geometry's block only
-    const size_t rows = (size_t)kMaxSweepVariants * F;
-    std::vector<uint32_t> t(rows * (size_t)h->sweep_G);
+    // the flag counters: one block per geometry of the plan, each setting counted in its own geometry's block only
+    const size_t rows = (size_t)kMaxSweepVariants * F, G = h->last.sweep ? h->last.sweep->geo.size() : 1;
+    std::vector<uint32_t> t(rows * G);
     for (int k = 0; k < 2; ++k) {
         uint32_t* out = k == 0 ? n_flagged_bins : n_rejected_points;
         if (!out) continue;
-        const size_t blocks = k == 0 ? (size_t)h->sweep_G : 1;
+        const size_t blocks = k == 0 ? G : 1;
         CK(cudaMemcpy(t.data(), (k == 0 ? h->d_sweep_flag : h->d_sweep_rej).p(), sizeof(uint32_t) * rows * blocks, cudaMemcpyDeviceToHost));
         for (size_t v = 0; v < V; ++v)
             for (size_t f = 0; f < F; ++f) {

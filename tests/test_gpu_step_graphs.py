@@ -1,8 +1,9 @@
 """GPU: the captured step graphs of the mask modes (erasor_capi.cu submit()).  A handle that replays cached CUDA graphs must return,
 byte for byte, what a handle that launches every step plainly (ERASOR_B200_NO_GRAPH=1) returns -- masks, node, frame and sweep
 counters, inserts and kernel launch counts -- over one interleaved sequence that replays graphs across changed sweep settings, fold
-on and off, frame_keep null and non-null, inserts toggled, and host and device pointers.  And erasor_profile_k1 after a replayed step
-rebins that step's query, not the query of the step captured last."""
+on and off, geometry sweeps (the handle's geometry alone, two geometries, one geometry changed), frame_keep null and non-null,
+inserts toggled, and host and device pointers.  And erasor_profile_k1 after a replayed step rebins that step's query, not the query
+of the step captured last."""
 import numpy as np
 import pytest
 
@@ -13,6 +14,9 @@ S1 = [dict(scan_ratio_threshold=0.10), dict(scan_ratio_threshold=0.20)]
 S2 = [dict(scan_ratio_threshold=0.15), dict(scan_ratio_threshold=0.25, minimum_num_pts=3)]
 G1 = [dict(gf_dist_thr=0.10), dict(gf_dist_thr=0.20)]
 G2 = [dict(gf_dist_thr=0.10), dict(gf_dist_thr=0.30)]
+T0 = [dict(scan_ratio_threshold=0.10), dict(scan_ratio_threshold=0.20, gf_dist_thr=0.30)]     # the handle's geometry only
+T1 = [dict(scan_ratio_threshold=0.20), dict(num_rings=20, num_sectors=108)]
+T2 = [dict(scan_ratio_threshold=0.20), dict(num_rings=20, num_sectors=90)]                      # T1 with one geometry changed
 
 
 @pytest.fixture(scope="module")
@@ -82,11 +86,12 @@ def test_graph_replay_equals_plain_launches(capi, small_workload, monkeypatch):
             r["ins"], r["ins_off"] = h.node_inserts()
         return r
 
-    def sweep(L, q, settings, ex=False):
+    def sweep(L, q, settings, ex=False, tune=False):
         h = L["h"]
         V = len(settings)
         h.reset_keep_mask(L["vk"].data_ptr(), V * n)
-        (h.process_nodes_sweep_ex if ex else h.process_nodes_sweep)(poses[q], dev[q].data_ptr(), qo, settings, L["vk"].data_ptr())
+        fn = h.process_nodes_tune if tune else h.process_nodes_sweep_ex if ex else h.process_nodes_sweep
+        fn(poses[q], dev[q].data_ptr(), qo, settings, L["vk"].data_ptr())
         return dict(vk=L["vk"][:V * n].cpu().numpy(), sweep=np.stack(h.sweep_stats()), stats=np.stack(h.node_stats()))
 
     def batch(L, kind="device", fold=True):
@@ -107,6 +112,8 @@ def test_graph_replay_equals_plain_launches(capi, small_workload, monkeypatch):
         (node, ("A",), dict(kind="packed")), (node, ("A",), {}), (node, ("B",), dict(fk=False)),
         (sweep, ("A", S1), {}), (sweep, ("B", S1), {}), (sweep, ("A", S2), {}), (sweep, ("A", S1), {}), (sweep, ("B", S2), {}),
         (sweep, ("A", G1), dict(ex=True)), (sweep, ("A", G2), dict(ex=True)), (sweep, ("A", G1), dict(ex=True)),
+        (sweep, ("A", T0), dict(tune=True)), (sweep, ("A", T1), dict(tune=True)), (sweep, ("A", T1), dict(tune=True)),
+        (sweep, ("A", T2), dict(tune=True)), (sweep, ("A", T2), dict(tune=True)), (sweep, ("B", T1), dict(tune=True)),
         (node, ("A",), {}), (inserts, (True,), {}), (node, ("A",), {}), (inserts, (False,), {}), (node, ("A",), {}),
         (inserts, (True,), {}), (node, ("A",), {}), (node, ("B",), dict(fk=False)), (inserts, (False,), {}), (node, ("B",), dict(fk=False)),
         (inserts, (True,), {}), (node, ("B",), dict(fk=False)), (node, ("A",), dict(kind="host")), (inserts, (False,), {}),
