@@ -9,17 +9,20 @@ The reference below is written from the algorithm (DESIGN.md, include/erasor_b20
   binning.h), ring = min(floor(r / ring_size), R - 1), sector = min(floor(theta / sector_size), S - 1); binned iff
   min_h < z < max_h and r <= max_range.  The sign of a zero y is ignored (-0.0 is +0.0), so azimuth is 0 or pi there, never -pi.
 - bin statistics: count, min z, max z per bin.
-- SRT (version 3): LITTLE if the map bin is empty or the query bin has fewer than minimum_num_pts points; else
+- SRT (version 3): LITTLE if the map bin is empty, the query bin has fewer than minimum_num_pts points (the reference compares
+  a size_t with the int, so a negative minimum_num_pts is a huge bound: every bin is LITTLE) or the query bin is empty; else
   ratio = min(dh_map / dh_query, dh_query / dh_map) (C++ std::min: a NaN first argument wins); ratio < threshold gives MAP_HIGH
   (dh_map >= dh_query) or CURR_HIGH, otherwise MERGE.  Second pass: MAP_HIGH with dh_map > 0.5 is handed to R-GPF, else the bin
   is left alone (status 0); MERGE next to a CURR_HIGH bin (ring +-1, sector +-1; a sector index below 0 or past S - 1 is wrapped by
-  num_rings, as the reference does) is BLOCKED.
+  num_rings, as the reference does) is BLOCKED.  Version 2: the same first pass on the bins occupied in both clouds, no second
+  pass, and MAP_HIGH is handed to R-GPF when the map bin's top is above th_bin_max_h (in double).
 - R-GPF on a handed-over bin: z sorted stably; lpr = mean of sorted z[num_lowest_pts : num_lowest_pts + gf_num_lpr] (0 if
   empty); seeds = points with z < lpr + gf_th_seeds_height; gf_iter times: plane through the current ground set (mean, two-pass
   mean-centred covariance, np.linalg.eigh, normal = eigenvector of the smallest eigenvalue; an empty set gives normal (0, 0, 1) and
   d = 0, the fallback the device documents), ground = points with normal . (p - mean) < gf_dist_thr.  The test is one-sided, so
   the sign of the normal decides which side is ground: the reference takes the device's sign (every other property is compared
-  up to sign).  Map points of a handed-over bin that end up non-ground are removed; every other map point is kept.
+  up to sign).  Map points of a handed-over bin that end up non-ground are removed (with gf_iter 0: every point that is not a
+  seed, since only the seeds return to the map); every other map point is kept.
 
 Tolerances (every one of them is stated next to its use):
 - EPS32 = 2^-23 (float32 machine epsilon).
@@ -116,14 +119,21 @@ def _cpp_min(a, b):
 
 
 def srt_status(p, mstat, qstat, eps_dh: float = 0.0):
-    """Version-3 status per bin, and the bins whose decisive quantity lies within the band of its threshold (node mode moves
-    every z by up to eps_dh; in cloud mode eps_dh = 0 and nothing is ambiguous)."""
+    """Status per bin (version 3, or version 2 when p.version == 2), which bins are handed to R-GPF, and the bins whose decisive
+    quantity lies within the band of its threshold (node mode moves every z by up to eps_dh; in cloud mode eps_dh = 0 and nothing
+    is ambiguous).  The query count is compared as the reference's size_t against the int minimum_num_pts, which the int is
+    converted to: a negative minimum_num_pts is a huge bound and sends every bin to LITTLE.  Only a bin occupied in both clouds
+    takes the ratio test (an empty query bin has no heights); version 3 gives the others LITTLE, version 2 leaves them unassigned
+    (0, the value of LITTLE)."""
     R, S = p.num_rings, p.num_sectors
     (mc, mmn, mmx), (qc, qmn, qmx) = mstat, qstat
+    enough = (qc >= p.minimum_num_pts) if p.minimum_num_pts >= 0 else np.zeros(R * S, dtype=bool)
+    if p.version == 2:
+        return _srt_status_v2(p, mstat, qstat, enough, eps_dh)
     pass1 = np.zeros(R * S)
     near = np.zeros(R * S, dtype=bool)
     with np.errstate(divide="ignore", invalid="ignore"):
-        for b in np.nonzero((mc > 0) & (qc >= p.minimum_num_pts))[0]:
+        for b in np.nonzero((mc > 0) & (qc > 0) & enough)[0]:
             mdh, cdh = mmx[b] - mmn[b], qmx[b] - qmn[b]
             ratio = _cpp_min(np.float64(mdh) / np.float64(cdh), np.float64(cdh) / np.float64(mdh))
             if ratio < p.scan_ratio_threshold:
@@ -154,6 +164,28 @@ def srt_status(p, mstat, qstat, eps_dh: float = 0.0):
                 if (rr, tj) != (r, theta) and pass1[tj * R + rr] == CURR_HIGH:
                     close = True
         st[b] = BLOCKED if close else MERGE
+    return st, flagged, near
+
+
+def _srt_status_v2(p, mstat, qstat, enough, eps_dh):
+    """Version 2: one pass, no neighbour test; MAP_HIGH goes to R-GPF when the map bin's top is above th_bin_max_h (in double)."""
+    (mc, mmn, mmx), (qc, qmn, qmx) = mstat, qstat
+    st = np.zeros(len(mc))
+    flagged = np.zeros(len(mc), dtype=bool)
+    near = np.zeros(len(mc), dtype=bool)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        for b in np.nonzero((mc > 0) & (qc > 0) & enough)[0]:
+            mdh, cdh = mmx[b] - mmn[b], qmx[b] - qmn[b]
+            ratio = _cpp_min(np.float64(mdh) / np.float64(cdh), np.float64(cdh) / np.float64(mdh))
+            if ratio < p.scan_ratio_threshold:
+                st[b] = MAP_HIGH if mdh >= cdh else CURR_HIGH
+                flagged[b] = bool(mdh >= cdh and np.float64(mmx[b]) > np.float64(p.th_bin_max_h))
+            else:
+                st[b] = MERGE
+            if eps_dh > 0.0:
+                if mdh > 0 and cdh > 0:
+                    near[b] |= abs(ratio - p.scan_ratio_threshold) <= ratio * 2 * eps_dh * (1 / mdh + 1 / cdh)
+                near[b] |= abs(mdh - cdh) <= 4 * eps_dh or min(mdh, cdh) <= 2 * eps_dh or abs(mmx[b] - p.th_bin_max_h) <= eps_dh
     return st, flagged, near
 
 
@@ -434,6 +466,239 @@ def srt_cases(p):
     return m, q, want
 
 
+# -- the sweep paths' inputs (tests/test_gpu_sweep_float64.py): every frame below is also held to the oracle on the CPU ----------
+SWEEP_THRESHOLDS = (0.10, 0.15, 0.20, 0.25, 0.30)
+nx32 = lambda v, d: float(np.nextafter(F32(v), F32(d)))       # the float32 next to v towards d
+
+
+def _case_cloud(p, ring, sec, zr, cnt, rng, tag):
+    """cnt points of bin (ring, sector) holding both extrema of zr = (lo, hi), the rest within 2 cm of lo (ground under a tall
+    object, so that R-GPF's labels are clear), intensity tag."""
+    x, y = xy_in_bin(p, ring, sec, cnt, rng, lo=0.25, hi=0.75)
+    fill = rng.uniform(zr[0], zr[0] + min(0.02, zr[1] - zr[0]), max(cnt - 2, 0))
+    z = np.concatenate([[zr[0], zr[1]], fill])[:cnt]
+    return np.stack([x, y, z, np.full(cnt, tag)], 1)
+
+
+def _tie_frame(p, cases, seed):
+    """(map, query, [(bin, case)]) of cases = [(map z range or None, map count, query z range or None, query count)], one bin each"""
+    rng = np.random.default_rng(seed)
+    ms, qs, where = [], [], []
+    for k, (mz, mc, qz, qc) in enumerate(cases):
+        ring, sec = 2 + k % 12, 1 + 2 * (k // 12)
+        assert sec < p.num_sectors
+        if mz is not None:
+            ms.append(_case_cloud(p, ring, sec, mz, mc, rng, 3.0))
+        if qz is not None and qc:
+            qs.append(_case_cloud(p, ring, sec, qz, qc, rng, 7.0))
+        where.append((sec * p.num_rings + ring, (mz, mc, qz, qc)))
+    return np.concatenate(ms).astype(F32), np.concatenate(qs).astype(F32), where
+
+
+def srt_tie_frame(p):
+    """Version 3 on seq_05's geometry: every Scan Ratio Test quantity of the sweep grid exactly on its threshold and one float32
+    step off it.  Each bin's lowest point is at z = 0 (inside (-1.3, 3.2)), so dh is exactly the float32 top height and the double
+    ratio of two such heights is exact; asserted below."""
+    cases = []
+    for t in SWEEP_THRESHOLDS:
+        top = F32(t * 2.5)
+        assert np.float64(top) / 2.5 == t and np.float64(nx32(top, 0)) / 2.5 < t     # on the threshold, one step below
+        cases += [((0.0, 2.5), 24, (0.0, float(top)), 45), ((0.0, 2.5), 24, (0.0, nx32(top, 0)), 45)]
+    cases += [((0.0, 0.5), 24, (0.0, 0.02), 45), ((0.0, nx32(0.5, 9)), 24, (0.0, 0.02), 45)]        # map_dh 0.5 and one ulp above
+    for k in (1, 10, 40):                                              # qc == minimum_num_pts and one below
+        cases += [((0.0, 2.5), 24, (0.0, 0.1) if k > 2 else (0.0, 0.0), k), ((0.0, 2.5), 24, (0.0, 0.1) if k > 2 else (0.0, 0.0), k - 1)]
+    cases += [((0.0, 2.5), 24, None, 0),                               # an empty query bin beside an occupied map bin
+              ((0.0, 2.5), 24, (0.0, 0.0), 45),                        # dh_query 0: ratio min(inf, 0) = 0
+              ((0.0, 0.0), 24, (0.0, 0.0), 45),                        # both 0: ratio NaN, not below any threshold
+              ((0.0, 0.0), 24, (0.0, 0.5), 45),                        # dh_map 0: CURR_HIGH
+              (None, 0, (0.0, 0.5), 45)]                               # an empty map bin
+    return _tie_frame(p, cases, seed=31)
+
+
+TIE_SETTINGS = ([dict(scan_ratio_threshold=t, minimum_num_pts=k) for k in (0, 1, 10, 40, -1, -5) for t in SWEEP_THRESHOLDS] +
+                [dict(scan_ratio_threshold=0.3, minimum_num_pts=9), dict(scan_ratio_threshold=0.1, minimum_num_pts=39)])
+V2_MAX_H = (-1.0, 0.0, 0.5, 1.5)
+
+
+def srt_v2_frame(p):
+    """Version 2: the map bin's top exactly on each th_bin_max_h and one float32 step above (for 0.0 the smallest denormal), a
+    low query so that the ratio is far below every threshold."""
+    cases = []
+    for h in V2_MAX_H:
+        assert np.float64(F32(h)) == h
+        lo = max(h - 1.0, -1.25)
+        for top in (h, nx32(h, 9)):
+            cases.append(((lo, top), 24, (lo, lo + 0.005), 45))
+    return _tie_frame(p, cases, seed=37)
+
+
+V2_SETTINGS = ([dict(th_bin_max_h=h, scan_ratio_threshold=t) for h in V2_MAX_H for t in (0.1, 0.3)] +
+               [dict(th_bin_max_h=0.0, minimum_num_pts=k) for k in (0, -1)])
+
+# R-GPF under ground-filter groups: RGPF_KINDS plus the remaining sort switches (256, 1024, 2048) and one point past each
+GROUP_KINDS = RGPF_KINDS + [("flat", n) for n in (256, 257, 1024, 1025, 2048, 2049)]
+
+
+def group_specs():
+    return [(2 + i % 16, 4 * i + 2, k, n, None) for i, (k, n) in enumerate(GROUP_KINDS)] + [FAR_COMPACT]
+
+
+# each list is one sweep_ex call (two or more ground-filter groups); the gf_iter 0 group and a num_lowest_pts >= n group each run
+# first in one of them, because a bin's plane record comes from the first group.  num_lowest_pts 2 and 3 are n and n - 1 of the
+# 'three' bin and n of the 'two' bin; where num_lowest_pts >= n empties the LPR window (lpr 0), a seeds height of -0.5 keeps the
+# objects out of the seeds, so that the fit stays determined
+GROUP_CALLS = [
+    [dict(gf_iter=0), dict(gf_iter=1), dict(gf_iter=3, scan_ratio_threshold=0.3), dict(gf_iter=8)],
+    [dict(num_lowest_pts=600, gf_th_seeds_height=-0.5), dict(num_lowest_pts=0), dict(num_lowest_pts=5), dict(num_lowest_pts=2),
+     dict(num_lowest_pts=3), dict(num_lowest_pts=512, gf_th_seeds_height=-0.5)],
+    [dict(gf_num_lpr=1), dict(gf_num_lpr=20), dict(gf_num_lpr=10000), dict(gf_num_lpr=10000, num_lowest_pts=2560, gf_th_seeds_height=-0.5, gf_iter=1)],
+    [dict(gf_th_seeds_height=s, gf_dist_thr=d) for s in (0.1, 0.3, 0.6) for d in (0.1, 0.3)] + [dict(gf_iter=0, num_lowest_pts=600)],
+]
+
+
+def witness_geometries():
+    """(name, geometry fields) of the geometries the bin-edge witnesses run under"""
+    return [("kitti_60x15x60", dict(max_range=60.0, num_rings=15, num_sectors=60)),
+            ("kitti_60x15x108", dict(max_range=60.0, num_rings=15, num_sectors=108)),
+            ("kitti_80x20x108", dict(max_range=80.0, num_rings=20, num_sectors=108)),
+            ("exact_gates", dict(max_range=64.0, num_rings=16, num_sectors=64, min_h=-1.25, max_h=3.0)),
+            ("40x360", dict(max_range=80.0, num_rings=40, num_sectors=360)),
+            ("4x12", dict(max_range=60.0, num_rings=4, num_sectors=12)),
+            ("26x181", dict(max_range=60.0, num_rings=26, num_sectors=181)),
+            ("26x182", dict(max_range=60.0, num_rings=26, num_sectors=182))]
+
+
+def witness_frame(p, seed=41):
+    """(map, query, witnesses) of one geometry's bin-edge scene.  Each edge lies between a bin X that the Scan Ratio Test always
+    hands to R-GPF (a 'flat' bin with a low query) and a bin Y that it never can (Y's query spans 2.5 m, its map at most 1.02 m with
+    every witness) or no bin at all.  A map witness is a point 1 m above X's ground: non-ground in X (removed), kept in Y.
+    - a ring radius on the -x axis (r exact, azimuth pi) and one ulp either side: X = ring k - 1, Y = ring k;
+    - the range gate r = max_range on the -y axis and one ulp either side: X = the outer ring;
+    - azimuth 0 (y = +-0, +-denormal, +-1 ulp): X = sector S - 1, Y = sector 0; azimuth pi the same way (for an even S, where pi is
+      a sector edge): X = sector S/2 - 1, Y = sector S/2;
+    - z on max_h and one and two ulps under it, and one over it, inside X = (the outer ring, sector 1);
+    - min_h: three bins Z of ground 4 cm above min_h and one point 0.47 m over it, each with one witness on min_h, one ulp over it
+      or one under it; a binned witness widens Z's map dh to 0.51 > 0.5 and hands Z to R-GPF (the query's 0.02 m puts the ratio
+      under every threshold), which removes the top point;
+    - the minimum_num_pts-th query point of a flat bin X = ring k - 1, on the ring radius k (+y axis: it lands in ring k, and X
+      stays below minimum_num_pts) or one ulp inside it (-y axis: X has enough query points and goes to R-GPF).
+    witnesses: list of dict(group, cloud ('map' / 'query'), idx (row in its cloud), alt (float32 x, y, z on the other side of the
+    edge))."""
+    rng = np.random.default_rng(seed)
+    R, S, rs, ss = p.num_rings, p.num_sectors, p.max_range / p.num_rings, 2.0 * PI_CFG / p.num_sectors
+    zg = p.min_h + 0.4
+    zw = float(F32(zg + 1.0))
+    ms, qs, wit = [], [], []
+
+    def x_bin(ring, sec, nq=None):
+        m, q = rgpf_bin(p, ring, sec, "flat", 48, rng)
+        ms.append(m); qs.append(q if nq is None else q[:nq])
+
+    def y_bin(ring, sec):
+        x, y = xy_in_bin(p, ring, sec, 6, rng)
+        ms.append(np.stack([x, y, zg + rng.uniform(0.0, 0.02, 6), np.full(6, 40.0)], 1).astype(F32))
+        x, y = xy_in_bin(p, ring, sec, 45, rng)
+        qz = np.concatenate([[zg, zg + 2.5], zg + rng.uniform(0.0, 2.5, 43)])
+        qs.append(np.stack([x, y, qz, np.full(45, 7.0)], 1).astype(F32))
+
+    def add(group, pts, alts, cloud="map"):
+        dst = ms if cloud == "map" else qs
+        base = sum(len(a) for a in dst)
+        dst.append(np.array([(x, y, z, 9.0) for x, y, z in pts], dtype=F32))
+        for i, a in enumerate(alts):
+            wit.append(dict(group=group, cloud=cloud, idx=base + i, alt=np.array(a, dtype=F32)))
+
+    up, dn = (lambda v: nx32(v, np.inf)), (lambda v: nx32(v, -np.inf))
+    s_pi, k = S // 2, max(1, R // 2)
+    rk = F32(k * rs)
+    x_bin(k - 1, s_pi); y_bin(k, s_pi)                                        # a ring radius
+    add("ring", [(-rk, 0.0, zw), (-dn(rk), 0.0, zw), (-up(rk), 0.0, zw)],
+        [(-dn(rk), 0.0, zw), (-rk, 0.0, zw), (-dn(rk), 0.0, zw)])
+    ug = F32(p.max_range)                                                      # the range gate
+    sec_ny = int(polar(p, np.array([[0.0, -1.0, zg]]))[0][0]) // R
+    x_bin(R - 1, sec_ny)
+    add("range", [(0.0, -ug, zw), (0.0, -dn(ug), zw), (0.0, -up(ug), zw)],
+        [(0.0, -up(ug), zw), (0.0, -up(ug), zw), (0.0, -ug, zw)])
+    ra = F32((R - 0.5) * rs)                                                    # azimuth 0 and pi, in the outer ring
+    ul = float(np.spacing(ra))
+    x_bin(R - 1, S - 1); y_bin(R - 1, 0)
+    ys = (0.0, -0.0, 1e-45, -1e-45, ul, -ul)
+    flip = lambda y: -y if y != 0.0 else -1e-45                               # the other side of the edge
+    add("azimuth 0", [(ra, y, zw) for y in ys], [(ra, flip(y), zw) for y in ys])
+    if S % 2 == 0:
+        x_bin(R - 1, s_pi - 1); y_bin(R - 1, s_pi)
+        ys = (0.0, 1e-45, -1e-45, ul, -ul)
+        add("azimuth pi", [(-ra, y, zw) for y in ys], [(-ra, flip(y), zw) for y in ys])
+    # the height gates, in the outer ring, sectors 1 to 4
+    at = lambda sec: (F32((R - 0.5) * rs * math.cos((sec + 0.5) * ss)), F32((R - 0.5) * rs * math.sin((sec + 0.5) * ss)))
+    x_bin(R - 1, 1)
+    hin = float(F32(p.max_h)) if float(F32(p.max_h)) < p.max_h else dn(p.max_h)      # the largest float32 under max_h
+    zs = (up(hin), hin, dn(hin), dn(dn(hin)))
+    add("max_h", [(*at(1), z) for z in zs], [(*at(1), up(hin) if z < p.max_h else hin) for z in zs])
+    lin = float(F32(p.min_h)) if float(F32(p.min_h)) > p.min_h else up(p.min_h)      # the smallest float32 over min_h
+    for j, z0 in enumerate((dn(lin), lin, up(lin))):
+        sec = 2 + j
+        x, y = xy_in_bin(p, R - 1, sec, 31, rng)
+        mzs = np.concatenate([[lin + 0.04, lin + 0.51], lin + 0.04 + rng.uniform(0.0, 0.005, 29)])
+        ms.append(np.stack([x, y, mzs, np.full(31, 40.0)], 1).astype(F32))
+        x, y = xy_in_bin(p, R - 1, sec, 45, rng)
+        qs.append(np.stack([x, y, lin + 0.1 + rng.uniform(0.0, 0.02, 45), np.full(45, 7.0)], 1).astype(F32))
+        add("min_h", [(*at(sec), z0)], [(*at(sec), dn(lin) if z0 > p.min_h else lin)])
+    # the query witnesses: X = ring k - 1 with minimum_num_pts - 1 query points, on the +y axis (witness on the radius: Y) and on
+    # the -y axis (witness one ulp inside X)
+    need = max(p.minimum_num_pts, 1)
+    sec_y = int(polar(p, np.array([[0.0, 1.0, zg]]))[0][0]) // R
+    for sec in (sec_y, sec_ny):
+        x_bin(k - 1, sec, nq=need - 1); y_bin(k, sec)
+    add("query", [(0.0, rk, zg), (0.0, -dn(rk), zg)], [(0.0, dn(rk), zg), (0.0, -rk, zg)], cloud="query")
+    m, q = np.concatenate(ms).astype(F32), np.concatenate(qs).astype(F32)
+    return m, q, wit
+
+
+def witness_settings():
+    """every witness geometry under two thresholds: 4 x 12 and 26 x 181 first (their K1 tables add up to exactly 56 KB)"""
+    geos = dict(witness_geometries())
+    order = ["4x12", "26x181"] + [g for g in geos if g not in ("4x12", "26x181")]
+    return [dict(geos[g], scan_ratio_threshold=t) for g in order for t in (0.1, 0.3)]
+
+
+WITNESS_VOI = 160.0                  # the VoI radius of the witness calls: beyond every max_range and the range-gate witnesses
+CLASS_C_COARSE = dict(max_range=60.0, num_rings=4, num_sectors=12)     # 15 m x 30 degree bins
+
+
+def class_c_frame(p):
+    """(map, query) of nine flat seq_05 bins (rings 4 to 6 x sectors 11 to 13: 16-28 m, 66-84 degrees) of 1500 to 200 points, all
+    inside one bin (ring 1, sector 2) of CLASS_C_COARSE: 3600 points there, a class-C bin, and class-A/B bins in seq_05's geometry."""
+    sizes = (1500, 400, 300, 300, 250, 250, 200, 200, 200)
+    specs = [(4 + i % 3, 11 + i // 3, "flat", n, None) for i, n in enumerate(sizes)]
+    return frame_of(p, specs, seed=43)
+
+
+CLASS_C_SETTINGS = [dict(scan_ratio_threshold=t) for t in (0.1, 0.3)] + [dict(CLASS_C_COARSE, scan_ratio_threshold=t) for t in (0.1, 0.3)]
+
+
+def clear_witnesses(p, m, q, wit):
+    """The witness frame without the witnesses that lie within the reference's band under p (either neighbour is right for them):
+    (map, query, map rows kept, query rows kept, band witnesses)."""
+    keep_m, keep_q = np.ones(len(m), bool), np.ones(len(q), bool)
+    band = []
+    for w in wit:
+        cloud = m if w["cloud"] == "map" else q
+        _, cand = polar(p, cloud[w["idx"]:w["idx"] + 1])
+        if not (cand == cand[:, :1]).all():
+            band.append(w)
+            (keep_m if w["cloud"] == "map" else keep_q)[w["idx"]] = False
+    rows_m, rows_q = np.nonzero(keep_m)[0], np.nonzero(keep_q)[0]
+    return m[rows_m], q[rows_q], rows_m, rows_q, band
+
+
+def moved(m, q, w):
+    """(map, query) with witness w moved to its other side"""
+    m, q = m.copy(), q.copy()
+    (m if w["cloud"] == "map" else q)[w["idx"], :3] = w["alt"]
+    return m, q
+
+
 # ================================================================================================================================
 # CPU self-tests of the reference
 # ================================================================================================================================
@@ -550,6 +815,186 @@ def test_generated_bins_stay_inside_their_bins():
     qb, _ = polar(p, q)
     st, flagged, _ = srt_status(p, bin_stats(p, mb, m[:, 2]), bin_stats(p, qb, q[:, 2]))
     assert flagged.sum() == len(rgpf_specs()) and set(np.unique(mb)) == set(np.nonzero(flagged)[0])
+
+
+def test_srt_reference_new_rules_by_hand():
+    """Version 2's th_bin_max_h, the both-occupied test and the size_t comparison of the query count, on hand-made bin tables."""
+    p = P.preset("seq_05")
+    B = p.num_bins
+    inf = np.inf
+
+    def tables(rows):      # rows: {bin: (count, min z, max z)}
+        c, mn, mx = np.zeros(B, np.int64), np.full(B, inf), np.full(B, -inf)
+        for b, (n, lo, hi) in rows.items():
+            c[b], mn[b], mx[b] = n, lo, hi
+        return c, mn, mx
+    # bin 0: map dh 2.5, query dh 0.25 (ratio 0.1); bin 1: the same map, no query; bin 2: the same map, one query point (dh 0)
+    mst = tables({0: (20, 0.0, 2.5), 1: (20, 0.0, 2.5), 2: (20, 0.0, 2.5)})
+    qst = tables({0: (12, 0.0, 0.25), 2: (1, 0.0, 0.0)})
+    for k, want in ((13, [False] * 3), (12, [True, False, False]), (1, [True, False, True]), (0, [True, False, True]), (-1, [False] * 3), (-5, [False] * 3)):
+        st, fl, _ = srt_status(p.replace(minimum_num_pts=k, scan_ratio_threshold=0.3), mst, qst)
+        assert fl[:3].tolist() == want, k
+        assert st[1] == LITTLE and (k >= 0 or (st == LITTLE).all()), k
+    # ratio 0.1 is not below 0.1 (MERGE); version 2 has no neighbour test and no dh > 0.5 rule
+    st, fl, _ = srt_status(p.replace(minimum_num_pts=1, scan_ratio_threshold=0.1), mst, qst)
+    assert st[0] == MERGE and not fl[0] and st[2] == MAP_HIGH and fl[2]
+    for top, th, want in ((1.5, 1.5, False), (float(np.nextafter(F32(1.5), F32(9))), 1.5, True), (0.0, 0.0, False), (1e-45, 0.0, True),
+                          (-1.0, -1.0, False), (0.4, 0.05, True)):
+        pv = p.replace(version=2, th_bin_max_h=th, minimum_num_pts=10)
+        m2 = tables({0: (20, top - 0.45, top)})
+        q2 = tables({0: (12, top - 0.45, top - 0.44)})
+        st, fl, _ = srt_status(pv, m2, q2)
+        assert st[0] == MAP_HIGH and fl[0] == want and fl.sum() == want, (top, th)      # map dh 0.45 <= 0.5: flagged all the same
+    st, fl, _ = srt_status(p.replace(version=2, th_bin_max_h=0.0), tables({0: (20, 0.0, 0.5)}), tables({0: (12, -1.0, 1.0)}))
+    assert st[0] == CURR_HIGH and not fl.any()
+    st, fl, _ = srt_status(p.replace(version=2, minimum_num_pts=0), tables({0: (20, 0.0, 2.5)}), tables({}))
+    assert not fl.any() and (st == 0).all()
+    st, fl, _ = srt_status(p.replace(version=2, minimum_num_pts=-1), mst, qst)
+    assert not fl.any() and (st == LITTLE).all()
+
+
+def test_sweep_frames_hold_their_ties():
+    """The tie frames put each case in its own bin, with the intended exact heights and counts, and the reference flags each of
+    them as the hand count says under every setting."""
+    p = P.preset("seq_05").replace(skip_voxelize=1)
+    m, q, where = srt_tie_frame(p)
+    mb, cm = polar(p, m)
+    qb, cq = polar(p, q)
+    assert (mb >= 0).all() and (qb >= 0).all() and (cm == mb[:, None]).all() and (cq == qb[:, None]).all()
+    ms, qs = bin_stats(p, mb, m[:, 2]), bin_stats(p, qb, q[:, 2])
+    f32 = lambda zr: None if zr is None else tuple(float(F32(v)) for v in zr)
+    where = [(b, (f32(mz), mc, f32(qz), qc)) for b, (mz, mc, qz, qc) in where]
+    for b, (mz, mc, qz, qc) in where:
+        assert ms[0][b] == mc and qs[0][b] == qc
+        if mz is not None:
+            assert (ms[1][b], ms[2][b]) == mz
+        if qc:
+            assert (qs[1][b], qs[2][b]) == qz
+    assert sorted(set(np.unique(mb))) == sorted(b for b, c in where if c[0] is not None)
+    for s in TIE_SETTINGS:
+        pv = p.replace(**s)
+        _, fl, near = srt_status(pv, ms, qs)
+        want = 0
+        for b, (mz, mc, qz, qc) in where:
+            if mz is None or qc == 0 or pv.minimum_num_pts < 0 or qc < pv.minimum_num_pts:
+                continue
+            mdh, cdh = mz[1] - mz[0], qz[1] - qz[0]
+            ratio = 0.0 if cdh == 0 and mdh > 0 else (np.nan if mdh == 0 and cdh == 0 else min(mdh / cdh, cdh / mdh) if mdh and cdh else 0.0)
+            want += bool(ratio < pv.scan_ratio_threshold and mdh >= cdh and mdh > 0.5)
+        assert fl.sum() == want and not near.any(), s
+    pv2 = p.replace(version=2)
+    m, q, where = srt_v2_frame(pv2)
+    ms, qs = bin_stats(pv2, polar(pv2, m)[0], m[:, 2]), bin_stats(pv2, polar(pv2, q)[0], q[:, 2])
+    for s in V2_SETTINGS:
+        pv = pv2.replace(**s)
+        _, fl, _ = srt_status(pv, ms, qs)
+        want = 0 if pv.minimum_num_pts < 0 else sum(float(F32(c[0][1])) > pv.th_bin_max_h for _, c in where)
+        assert fl.sum() == want, s
+
+
+def _oracle_against_reference(p, m, q, tag):
+    """The C++ oracle (bit-identical to the device) against the reference on one frame under p: bin tables, statuses, flagged bins
+    and the keep mask outside ambiguous bins.  Returns (reference keep, known, ambiguous bins)."""
+    from oracle import oracle_py
+    o = oracle_py.Oracle(p)
+    try:
+        o.run(m, q)
+        mb, _ = polar(p, m)
+        assert np.array_equal(o.bin_of_point(0), mb), tag
+        mn, mx, cnt, _ = o.bins(0)
+        rc, rmn, rmx = bin_stats(p, mb, m[:, 2])
+        occ = rc > 0
+        assert np.array_equal(cnt, rc) and np.array_equal(mn[occ], rmn[occ]) and np.array_equal(mx[occ], rmx[occ]), tag
+        report, ambiguous = [], []
+        st, keep, known = _reference_keep(p, m, q, {pl["bin"]: pl for pl in o.planes()}, p.cov_mode, tag, report, ambiguous)
+        assert np.array_equal(o.status()[0], st), (tag, np.nonzero(o.status()[0] != st)[0][:10])
+        # the map points the static map keeps: those of the arranged bins and of the complement (a query point's source index
+        # carries the top bit).  Without a plane-fit iteration R-GPF rejects nothing, but only the seeds return to the map.
+        okeep = np.zeros(len(m), np.uint8)
+        for which in (o.ARRANGED, o.COMPLEMENT):
+            _, src = o.cloud(which)
+            okeep[src[src < 0x80000000]] = 1
+        _, rej = o.cloud(o.MAP_REJECTED)
+        assert not okeep[rej].any() and (p.gf_iter == 0 or (okeep == 0).sum() == len(rej)), tag
+        assert np.array_equal(okeep[known], keep[known]), tag
+        return keep, known, ambiguous
+    finally:
+        o.close()
+
+
+def test_sweep_frames_reference_against_the_oracle():
+    """Every frame of the sweep tests under every setting they run: the reference and the oracle agree, so the GPU comparisons
+    rest on a reference pinned on the CPU."""
+    base = P.preset("seq_05").replace(skip_voxelize=1)
+    m, q, _ = srt_tie_frame(base)
+    for s in TIE_SETTINGS:
+        _oracle_against_reference(base.replace(**s), m, q, ("tie", s))
+    pv2 = base.replace(version=2)
+    m, q, _ = srt_v2_frame(pv2)
+    for s in V2_SETTINGS:
+        _oracle_against_reference(pv2.replace(**s), m, q, ("v2", s))
+    m, q = class_c_frame(base)
+    for s in CLASS_C_SETTINGS:
+        _, known, _ = _oracle_against_reference(base.replace(**s), m, q, ("class C", s))
+        assert known.all()
+    for name, g in witness_geometries():
+        m, q, wit = witness_frame(base.replace(**g))
+        for s in witness_settings():
+            pv = base.replace(**s)
+            mc, qc, _, _, _ = clear_witnesses(pv, m, q, wit)
+            _oracle_against_reference(pv, mc, qc, ("witness", name, s))
+    # the oracle's polar binning with the band witnesses in: every point in one of the reference's candidate bins
+    from oracle import oracle_py
+    for name, g in witness_geometries():
+        pv = base.replace(**g)
+        m, q, _ = witness_frame(pv)
+        o = oracle_py.Oracle(pv)
+        o.run(m, q)
+        _, cand = polar(pv, m)
+        assert (o.bin_of_point(0)[:, None] == cand).any(1).all(), name
+        o.close()
+
+
+@pytest.mark.parametrize("cov_mode", [0, 1])
+def test_group_frame_reference_against_the_oracle(cov_mode):
+    p = P.preset(RGPF_PRESET).replace(skip_voxelize=1, cov_mode=cov_mode)
+    m, q = frame_of(p, group_specs(), seed=47)
+    n_amb = []
+    for call in GROUP_CALLS:
+        for s in call:
+            _, _, amb = _oracle_against_reference(p.replace(**s), m, q, ("groups", s))
+            n_amb.append(len(amb))
+    assert max(n_amb) <= 1, n_amb
+
+
+def test_witnesses_are_decisive():
+    """Moving any witness to the other side of its edge changes the reference's keep mask, and both sides are binned exactly as
+    intended (a ring, sector or gate apart): the GPU comparison of the witnesses cannot pass by keeping or removing everything."""
+    base = P.preset("seq_05").replace(skip_voxelize=1)
+    from oracle import oracle_py
+    for name, g in witness_geometries():
+        p = base.replace(**g)
+        m, q, wit = witness_frame(p)
+        groups = {w["group"] for w in wit}
+        assert groups >= {"ring", "range", "azimuth 0", "max_h", "min_h", "query"} and (("azimuth pi" in groups) == (p.num_sectors % 2 == 0))
+
+        def keep_of(mm, qq):
+            o = oracle_py.Oracle(p)
+            o.run(mm, qq)
+            planes = {pl["bin"]: pl for pl in o.planes()}
+            o.close()
+            report, amb = [], []
+            _, keep, known = _reference_keep(p, mm, qq, planes, 0, name, report, amb)
+            assert known.all() and not amb, name
+            return keep
+        k0 = keep_of(m, q)
+        for w in wit:
+            cloud = m if w["cloud"] == "map" else q
+            b0 = polar(p, cloud[w["idx"]:w["idx"] + 1])[0][0]
+            b1 = polar(p, w["alt"][None, :].astype(np.float64))[0][0]
+            assert b0 != b1, (name, w["group"], w["idx"])
+            k1 = keep_of(*moved(m, q, w))
+            assert not np.array_equal(k0, k1), (name, w["group"], cloud[w["idx"]].tolist(), w["alt"].tolist())
 
 
 def _cov_f32(pts, shift: bool):
