@@ -252,18 +252,26 @@ cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map
 // ============================================================================================
 __device__ __forceinline__ double std_min_d(double a, double b) { return (b < a) ? b : a; }   // std::min, NaN-faithful (App. B-4)
 
+// The heights the Scan Ratio Test compares, from a bin's ordered z extremes in the map and the query cloud (erasor.cpp:370-373, 462-465)
+struct SrtHeights { double map_max, map_dh, curr_dh, ratio; };
+__device__ __forceinline__ SrtHeights srt_heights(uint32_t zmx_m, uint32_t zmn_m, uint32_t zmx_q, uint32_t zmn_q) {
+    SrtHeights h;
+    h.map_max = (double)ordered_to_float(zmx_m);
+    h.map_dh  = h.map_max - (double)ordered_to_float(zmn_m);
+    h.curr_dh = (double)ordered_to_float(zmx_q) - (double)ordered_to_float(zmn_q);
+    h.ratio   = std_min_d(h.map_dh / h.curr_dh, h.curr_dh / h.map_dh);
+    return h;
+}
+
 // Does the Scan Ratio Test hand this bin to R-GPF?  The same decisions as k3_srt's status passes, reduced to the one bit
 // the scatter needs: version 3 -- MAP_IS_HIGHER in pass 1 and map_dh > 0.5 in pass 2 (erasor.cpp:448-486, 507-511; the
 // neighbour test of pass 2 only relabels MERGE_BINS as BLOCKED); version 2 -- MAP_IS_HIGHER and map.max_h > th_bin_max_h
 // (erasor.cpp:346-389).
 __device__ __forceinline__ bool srt_is_flagged(const SrtParams& P, uint32_t mc, uint32_t qc, uint32_t zmx_m, uint32_t zmn_m, uint32_t zmx_q, uint32_t zmn_q) {
     if (mc == 0u || qc == 0u || P.minimum_num_pts < 0 || qc < (uint32_t)P.minimum_num_pts) return false;
-    const double map_max = (double)ordered_to_float(zmx_m);
-    const double map_dh  = map_max - (double)ordered_to_float(zmn_m);
-    const double curr_dh = (double)ordered_to_float(zmx_q) - (double)ordered_to_float(zmn_q);
-    const double ratio   = std_min_d(map_dh / curr_dh, curr_dh / map_dh);
-    if (!(ratio < P.scan_ratio_threshold) || !(map_dh >= curr_dh)) return false;
-    return (P.version == 3) ? (map_dh > 0.5) : (map_max > P.th_bin_max_h);
+    const SrtHeights h = srt_heights(zmx_m, zmn_m, zmx_q, zmn_q);
+    if (!(h.ratio < P.scan_ratio_threshold) || !(h.map_dh >= h.curr_dh)) return false;
+    return (P.version == 3) ? (h.map_dh > 0.5) : (h.map_max > P.th_bin_max_h);
 }
 
 // The action k3_srt gives a bin (what r_pod_selected takes from it), without the curr_rejected bit: version 3 -- ACT_FLAG or
@@ -271,13 +279,38 @@ __device__ __forceinline__ bool srt_is_flagged(const SrtParams& P, uint32_t mc, 
 __device__ __forceinline__ uint8_t srt_action(const SrtParams& P, uint32_t mc, uint32_t qc, uint32_t zmx_m, uint32_t zmn_m, uint32_t zmx_q, uint32_t zmn_q) {
     if (srt_is_flagged(P, mc, qc, zmx_m, zmn_m, zmx_q, zmn_q)) return ACT_FLAG;
     if (P.version == 3 || P.minimum_num_pts < 0 || qc < (uint32_t)P.minimum_num_pts) return ACT_MAP;
-    if (qc != 0u && mc != 0u) {
-        const double map_dh  = (double)ordered_to_float(zmx_m) - (double)ordered_to_float(zmn_m);
-        const double curr_dh = (double)ordered_to_float(zmx_q) - (double)ordered_to_float(zmn_q);
-        const double ratio   = std_min_d(map_dh / curr_dh, curr_dh / map_dh);
-        return (ratio < P.scan_ratio_threshold) ? ACT_MAP : ACT_MERGE;
-    }
+    if (qc != 0u && mc != 0u) return (srt_heights(zmx_m, zmn_m, zmx_q, zmn_q).ratio < P.scan_ratio_threshold) ? ACT_MAP : ACT_MERGE;
     return qc != 0u ? ACT_CURR : (mc != 0u ? ACT_MAP : ACT_NONE);
+}
+
+// In-place exclusive prefix of bin b over the per-chunk count rows [c0, c1) (B + 1 counts per row), eight rows per round trip: the
+// loads of a batch are independent, only the running sum is serial
+__device__ __forceinline__ void chunk_rows_excl_prefix(uint32_t* __restrict__ ch_cnt, int B, int b, uint32_t c0, uint32_t c1) {
+    uint32_t run = 0;
+    for (uint32_t k0 = c0; k0 < c1; k0 += 8u) {
+        uint32_t v[8];
+#pragma unroll
+        for (uint32_t u = 0; u < 8u; ++u) v[u] = (k0 + u < c1) ? ch_cnt[(size_t)(k0 + u) * (B + 1) + b] : 0u;
+#pragma unroll
+        for (uint32_t u = 0; u < 8u; ++u) {
+            if (k0 + u < c1) { ch_cnt[(size_t)(k0 + u) * (B + 1) + b] = run; run += v[u]; }
+        }
+    }
+}
+
+// The record of flagged bin `bin` of `frame` (its n points start at src_begin in the scattered map array), handed to its R-GPF size
+// bucket (order inside a bucket is irrelevant: bins are independent).  ri < rec_capacity.
+__device__ __forceinline__ FlagRec& push_flag_rec(FlagRec* __restrict__ recs, uint32_t ri, uint32_t rec_capacity, uint32_t* __restrict__ queue,
+                                                  uint32_t* __restrict__ bucket_list, uint32_t frame, uint32_t bin, uint32_t slot, uint32_t n,
+                                                  uint32_t src_begin) {
+    FlagRec& rc = recs[ri];
+    rc.frame = frame; rc.bin = bin; rc.slot = slot; rc.n_points = n; rc.src_begin = src_begin;
+    rc.n_seeds = 0; rc.n_empty_fits = 0; rc.n_ground_final = 0; rc.lpr_height = 0.0; rc.cursor = 0u; rc.n_rejected = 0u;
+    if (n != 0u) {
+        const int bk = rgpf_bucket_of(n);
+        bucket_list[(size_t)bk * rec_capacity + atomicAdd(&queue[bk], 1u)] = ri;
+    }
+    return rc;
 }
 
 __global__ void __launch_bounds__(1024)
@@ -398,18 +431,7 @@ k3_srt(SrtParams P, int F, const uint32_t* __restrict__ chunk_range /*[2][F+1]*/
         const uint32_t c0 = chunk_range[c * (F + 1) + f], c1 = chunk_range[c * (F + 1) + f + 1];
         for (int b = tid; b <= B; b += nt) {
             const bool take = (P.scatter_mode == 0) || (b < B && (act_out[b] & 0x0F) == ACT_FLAG);
-            if (!take) continue;
-            // eight rows per round trip: the loads of a batch are independent, only the running sum is serial
-            uint32_t run = 0;
-            for (uint32_t k0 = c0; k0 < c1; k0 += 8u) {
-                uint32_t v[8];
-#pragma unroll
-                for (uint32_t u = 0; u < 8u; ++u) v[u] = (k0 + u < c1) ? ch_cnt[(size_t)(k0 + u) * (B + 1) + b] : 0u;
-#pragma unroll
-                for (uint32_t u = 0; u < 8u; ++u) {
-                    if (k0 + u < c1) { ch_cnt[(size_t)(k0 + u) * (B + 1) + b] = run; run += v[u]; }
-                }
-            }
+            if (take) chunk_rows_excl_prefix(ch_cnt, B, b, c0, c1);
         }
     }
     __syncthreads();
@@ -450,16 +472,7 @@ k3_srt(SrtParams P, int F, const uint32_t* __restrict__ chunk_range /*[2][F+1]*/
         if ((act_out[b] & 0x0F) == ACT_FLAG) {
             const uint32_t slot = slot_out[b];
             const uint32_t ri   = rec_base + slot;
-            if (ri < rec_capacity) {
-                FlagRec& rc = recs[ri];
-                rc.frame = f; rc.bin = b; rc.slot = slot; rc.n_points = cm[b];
-                rc.src_begin = frame_off[f] + s_sz[b];
-                rc.n_seeds = 0; rc.n_empty_fits = 0; rc.n_ground_final = 0; rc.lpr_height = 0.0; rc.cursor = 0u; rc.n_rejected = 0u;
-                if (cm[b] != 0u) {   // hand the record to the R-GPF size bucket (order inside a bucket is irrelevant: bins are independent)
-                    const int bk = rgpf_bucket_of(cm[b]);
-                    bucket_list[(size_t)bk * rec_capacity + atomicAdd(&queue[bk], 1u)] = ri;
-                }
-            }
+            if (ri < rec_capacity) push_flag_rec(recs, ri, rec_capacity, queue, bucket_list, f, b, slot, cm[b], frame_off[f] + s_sz[b]);
         }
     }
     __syncthreads();
@@ -598,6 +611,49 @@ __device__ __forceinline__ void k2_scatter_pass(const uint16_t* __restrict__ ids
     }
 }
 
+// One window [win0, win0 + ns) of slots of the CTA's chunk (row `row`): zero the warps' rows, count pass, column scan into absolute
+// destinations from the window's bases, scatter pass.  The caller writes the bases into s_base[0, ns) (the barriers here order them
+// before the column scan) and calls after a barrier behind its last use of the rows s_tab[0, W * ns).  Each warp takes its part of
+// the chunk: a contiguous sub-range of its points -- or, in node mode, the dense VoI lists that k1_warps / W of K1's warps left for
+// their sub-ranges (same split, same order).
+template <int W, bool NODE>
+__device__ __forceinline__ void k2_window(const ChunkDesc& cd, uint32_t row, uint32_t win0, uint32_t ns, uint32_t* s_tab, const uint32_t* s_base,
+                                          const uint16_t* s_slot, const float* s_T, int B, const uint16_t* __restrict__ bin_ids,
+                                          const float4* __restrict__ pts, const uint32_t* __restrict__ list_idx, const uint32_t* __restrict__ list_cnt,
+                                          int k1_warps, float4* __restrict__ out_pts, uint32_t* __restrict__ out_src) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int      nseg = NODE ? k1_warps / W : 1;
+    const uint32_t sub  = (((cd.len + (NODE ? k1_warps : W) - 1) / (NODE ? k1_warps : W)) + 31u) & ~31u;
+    auto seg_range = [&](int g, uint32_t& s0, uint32_t& s1) {
+        const uint32_t kw = (uint32_t)warp * nseg + g;
+        s0 = min(cd.len, kw * sub);
+        s1 = NODE ? s0 + list_cnt[(size_t)row * kListWarps + kw] : min(cd.len, s0 + sub);
+    };
+    const uint16_t* ids = bin_ids + cd.bin_begin;
+    const uint32_t local0 = cd.begin - cd.frame_begin;
+    const float4* src = NODE ? pts : pts + cd.begin;
+    const uint32_t* lidx = NODE ? list_idx + cd.bin_begin : nullptr;
+    uint32_t* mine = s_tab + (size_t)warp * ns;              // row stride of this window: ns
+    for (uint32_t i = tid; i < (uint32_t)W * ns; i += W * 32) s_tab[i] = 0u;
+    __syncthreads();
+    for (int g = 0; g < nseg; ++g) { uint32_t s0, s1; seg_range(g, s0, s1); k2_count_pass(ids, s0, s1, s_slot, win0, ns, mine, B, lane); }
+    __syncthreads();
+    for (uint32_t j = tid; j < ns; j += W * 32) {
+        uint32_t run = s_base[j];
+#pragma unroll
+        for (int w = 0; w < W; ++w) {
+            const uint32_t c = s_tab[(size_t)w * ns + j];
+            s_tab[(size_t)w * ns + j] = run;
+            run += c;
+        }
+    }
+    __syncthreads();
+    for (int g = 0; g < nseg; ++g) {
+        uint32_t s0, s1; seg_range(g, s0, s1);
+        k2_scatter_pass<NODE>(ids, s0, s1, s_slot, win0, ns, mine, B, lane, src, s_T, cd.out_base, local0, out_pts, out_src, lidx);
+    }
+}
+
 // DUAL (cloud mode): one launch scatters both clouds -- CTAs [0, second.first_row) take the map cloud's chunks with the
 // arguments below, the rest the query cloud's with `second` (chunk rows are numbered map first, then query).
 struct K2Second { uint32_t first_row; const uint16_t* bin_ids; const float4* pts; const uint32_t* dst_start; float4* out_pts; uint32_t* out_src; };
@@ -611,7 +667,7 @@ k2_scatter_win(const ChunkDesc* __restrict__ chunks, uint32_t chunk_base, const 
                const uint32_t* __restrict__ list_idx, const uint32_t* __restrict__ list_cnt, int k1_warps, K2Second second) {
     extern __shared__ uint32_t s_tab[];   // [W][ns] per-warp counters / destinations | [SW] bases | u16 slot of every bin [B+1]
     __shared__ float s_T[12];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const uint32_t row = chunk_base + blockIdx.x;
     if (DUAL && row >= second.first_row) {        // CTA-uniform
         bin_ids = second.bin_ids; pts = second.pts; dst_start = second.dst_start; out_pts = second.out_pts; out_src = second.out_src;
@@ -629,47 +685,16 @@ k2_scatter_win(const ChunkDesc* __restrict__ chunks, uint32_t chunk_base, const 
         for (int b = tid; b <= B; b += W * 32) s_slot[b] = (ds[b] == kSkip) ? (uint16_t)0xFFFFu : (uint16_t)b;   // (the query cloud's complement is not scattered)
     }
     if (NODE && tid < 12) s_T[tid] = poses[cd.frame].T[tid];
-    // this warp's part of the chunk: a contiguous sub-range of its points -- or, in node mode, the dense VoI lists that
-    // k1_warps / W of K1's warps left for their sub-ranges (same split, same order)
-    const int      nseg = NODE ? k1_warps / W : 1;
-    const uint32_t sub  = (((cd.len + (NODE ? k1_warps : W) - 1) / (NODE ? k1_warps : W)) + 31u) & ~31u;
-    auto seg_range = [&](int g, uint32_t& s0, uint32_t& s1) {
-        const uint32_t kw = (uint32_t)warp * nseg + g;
-        s0 = min(cd.len, kw * sub);
-        s1 = NODE ? s0 + list_cnt[(size_t)row * kListWarps + kw] : min(cd.len, s0 + sub);
-    };
-    const uint16_t* ids = bin_ids + cd.bin_begin;
-    const uint32_t local0 = cd.begin - cd.frame_begin;
-    const float4* src = NODE ? pts : pts + cd.begin;
-    const uint32_t* lidx = NODE ? list_idx + cd.bin_begin : nullptr;
 
     for (uint32_t win0 = 0; win0 < n_slots; win0 += SW) {
-        const uint32_t ns = min(SW, n_slots - win0);          // row stride of this window
-        uint32_t* mine = s_tab + (size_t)warp * ns;
+        const uint32_t ns = min(SW, n_slots - win0);
         __syncthreads();                                      // slot table ready / previous window's rows consumed
-        for (uint32_t i = tid; i < (uint32_t)W * ns; i += W * 32) s_tab[i] = 0u;
-        __syncthreads();
-        for (int g = 0; g < nseg; ++g) { uint32_t s0, s1; seg_range(g, s0, s1); k2_count_pass(ids, s0, s1, s_slot, win0, ns, mine, B, lane); }
         // bases of the window's slots: dst_start + points of the bin in earlier chunks of the frame
         for (int b = tid; b <= B; b += W * 32) {
             const uint32_t sl = (uint32_t)s_slot[b] - win0;
             if (sl < ns) s_base[sl] = ds[b] + pref[b];
         }
-        __syncthreads();
-        for (uint32_t j = tid; j < ns; j += W * 32) {
-            uint32_t run = s_base[j];
-#pragma unroll
-            for (int w = 0; w < W; ++w) {
-                const uint32_t c = s_tab[(size_t)w * ns + j];
-                s_tab[(size_t)w * ns + j] = run;
-                run += c;
-            }
-        }
-        __syncthreads();
-        for (int g = 0; g < nseg; ++g) {
-            uint32_t s0, s1; seg_range(g, s0, s1);
-            k2_scatter_pass<NODE>(ids, s0, s1, s_slot, win0, ns, mine, B, lane, src, s_T, cd.out_base, local0, out_pts, out_src, lidx);
-        }
+        k2_window<W, NODE>(cd, row, win0, ns, s_tab, s_base, s_slot, s_T, B, bin_ids, pts, list_idx, list_cnt, k1_warps, out_pts, out_src);
     }
 }
 
@@ -684,16 +709,13 @@ k2_scatter_win(const ChunkDesc* __restrict__ chunks, uint32_t chunk_base, const 
 __device__ __forceinline__ uint32_t srt_variant_mask(const SrtSweep& S, int version, uint32_t mc, uint32_t qc, uint32_t zmx_m, uint32_t zmn_m,
                                                      uint32_t zmx_q, uint32_t zmn_q) {
     if (mc == 0u || qc == 0u) return 0u;
-    const double map_max = (double)ordered_to_float(zmx_m);
-    const double map_dh  = map_max - (double)ordered_to_float(zmn_m);
-    const double curr_dh = (double)ordered_to_float(zmx_q) - (double)ordered_to_float(zmn_q);
-    const double ratio   = std_min_d(map_dh / curr_dh, curr_dh / map_dh);
-    if (!(map_dh >= curr_dh)) return 0u;
+    const SrtHeights h = srt_heights(zmx_m, zmn_m, zmx_q, zmn_q);
+    if (!(h.map_dh >= h.curr_dh)) return 0u;
     uint32_t m = 0u;
     for (int v = 0; v < S.n; ++v) {
         const SrtVariant& x = S.v[v];
-        if (x.minimum_num_pts < 0 || qc < (uint32_t)x.minimum_num_pts || !(ratio < x.scan_ratio_threshold)) continue;   // App. B-9: < 0 flags nothing
-        if ((version == 3) ? (map_dh > 0.5) : (map_max > x.th_bin_max_h)) m |= 1u << v;
+        if (x.minimum_num_pts < 0 || qc < (uint32_t)x.minimum_num_pts || !(h.ratio < x.scan_ratio_threshold)) continue;   // App. B-9: < 0 flags nothing
+        if ((version == 3) ? (h.map_dh > 0.5) : (h.map_max > x.th_bin_max_h)) m |= 1u << v;
     }
     return m;
 }
@@ -787,25 +809,11 @@ k2_srt_scatter_body(const SrtParams& P, int F, const ChunkDesc* __restrict__ chu
     __syncthreads();
     const uint32_t rec_base = leader ? s_bcast[0] : 0u;
 
-    // this warp's part of the chunk: a contiguous sub-range of its points -- or, in node mode, the dense VoI lists that
-    // k1_warps / W of K1's warps left for their sub-ranges (same split, same order)
-    const int      nseg = NODE ? k1_warps / W : 1;
-    const uint32_t sub  = (((cd.len + (NODE ? k1_warps : W) - 1) / (NODE ? k1_warps : W)) + 31u) & ~31u;
-    auto seg_range = [&](int g, uint32_t& s0, uint32_t& s1) {
-        const uint32_t kw = (uint32_t)warp * nseg + g;
-        s0 = min(cd.len, kw * sub);
-        s1 = NODE ? s0 + list_cnt[(size_t)row * kListWarps + kw] : min(cd.len, s0 + sub);
-    };
-    const uint16_t* ids = bin_ids + cd.bin_begin;
-    const uint32_t local0 = cd.begin - cd.frame_begin;
-    const float4* src = NODE ? pts : pts + cd.begin;
-    const uint32_t* lidx = NODE ? list_idx + cd.bin_begin : nullptr;
     const uint32_t fbase = frame_off[f];
     uint32_t win_carry = 0u;                                  // points of the flagged bins of earlier windows
 
     for (uint32_t win0 = 0; win0 < n_slots; win0 += SW) {
         const uint32_t ns = min(SW, n_slots - win0);
-        uint32_t* mine = s_tab + (size_t)warp * ns;
         uint32_t* s_bin = s_tab;                              // [ns] bin of every slot of the window   (rows are not in use yet)
         uint32_t* s_pf  = s_tab + ns;                         // [ns] points of the bin in earlier chunks of the frame
         __syncthreads();
@@ -835,15 +843,8 @@ k2_srt_scatter_body(const SrtParams& P, int F, const ChunkDesc* __restrict__ chu
             for (uint32_t j = tid; j < ns; j += NT) {
                 const uint32_t b = s_bin[j], slot = win0 + j, ri = rec_base + slot, sz = cm[b];
                 if (ri < rec_capacity) {
-                    FlagRec& rc = recs[ri];
-                    rc.frame = (uint32_t)f; rc.bin = b; rc.slot = slot; rc.n_points = sz;
-                    rc.src_begin = fbase + win_carry + s_base[j];
-                    rc.n_seeds = 0; rc.n_empty_fits = 0; rc.n_ground_final = 0; rc.lpr_height = 0.0; rc.cursor = 0u; rc.n_rejected = 0u;
+                    FlagRec& rc = push_flag_rec(recs, ri, rec_capacity, queue, bucket_list, (uint32_t)f, b, slot, sz, fbase + win_carry + s_base[j]);
                     if constexpr (SWEEP) rc.cursor = srt_variant_mask(*sweep, P.version, sz, cq[b], mxm[b], mnm[b], mxq[b], mnq[b]);
-                    if (sz != 0u) {
-                        const int bk = rgpf_bucket_of(sz);
-                        bucket_list[(size_t)bk * rec_capacity + atomicAdd(&queue[bk], 1u)] = ri;
-                    }
                 }
             }
         }
@@ -851,24 +852,7 @@ k2_srt_scatter_body(const SrtParams& P, int F, const ChunkDesc* __restrict__ chu
         // absolute base per slot, then the rows can be zeroed (s_bin / s_pf live in them)
         for (uint32_t j = tid; j < ns; j += NT) s_base[j] = win_carry + s_base[j] + s_pf[j];
         __syncthreads();
-        for (uint32_t i = tid; i < (uint32_t)W * ns; i += NT) s_tab[i] = 0u;
-        __syncthreads();
-        for (int g = 0; g < nseg; ++g) { uint32_t s0, s1; seg_range(g, s0, s1); k2_count_pass(ids, s0, s1, s_slot, win0, ns, mine, B, lane); }
-        __syncthreads();
-        for (uint32_t j = tid; j < ns; j += NT) {
-            uint32_t run = s_base[j];
-#pragma unroll
-            for (int w = 0; w < W; ++w) {
-                const uint32_t c = s_tab[(size_t)w * ns + j];
-                s_tab[(size_t)w * ns + j] = run;
-                run += c;
-            }
-        }
-        __syncthreads();
-        for (int g = 0; g < nseg; ++g) {
-            uint32_t s0, s1; seg_range(g, s0, s1);
-            k2_scatter_pass<NODE>(ids, s0, s1, s_slot, win0, ns, mine, B, lane, src, s_T, cd.out_base, local0, out_pts, out_src, lidx);
-        }
+        k2_window<W, NODE>(cd, row, win0, ns, s_tab, s_base, s_slot, s_T, B, bin_ids, pts, list_idx, list_cnt, k1_warps, out_pts, out_src);
         win_carry += win_total;
     }
 }
@@ -2164,11 +2148,8 @@ k_ins_plan(SrtParams P, int F, const uint32_t* __restrict__ chunk_range /*[2][F+
     for (int b = tid; b <= B; b += nt) dsq[b] = (b < B && inserts(b)) ? s_sz[b] : kSkip;
     if (tid == 0) dsq[B + 1] = tot;
     const uint32_t c0 = chunk_range[(F + 1) + f], c1 = chunk_range[(F + 1) + f + 1];
-    for (int b = tid; b < B; b += nt) {
-        if (!inserts(b)) continue;
-        uint32_t run = 0;
-        for (uint32_t k = c0; k < c1; ++k) { const uint32_t v = ch_cnt[(size_t)k * (B + 1) + b]; ch_cnt[(size_t)k * (B + 1) + b] = run; run += v; }
-    }
+    for (int b = tid; b < B; b += nt)
+        if (inserts(b)) chunk_rows_excl_prefix(ch_cnt, B, b, c0, c1);
 }
 
 cudaError_t launch_ins_plan(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt, const uint32_t* zmin,

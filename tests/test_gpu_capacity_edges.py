@@ -166,6 +166,12 @@ def test_k2_windows_frames_and_nodes(capi, oracle_mod):
     gm.close()
 
 
+def test_k2_windows_frames_and_nodes_unfused(capi, oracle_mod, monkeypatch):
+    """The same windows through the unfused mask-mode path: k3_srt, then k2_scatter_win over K3's flagged slots."""
+    monkeypatch.setenv("ERASOR_B200_UNFUSED_SRT", "1")          # read when the handle is created
+    test_k2_windows_frames_and_nodes(capi, oracle_mod)
+
+
 # ---- a dense map end to end ------------------------------------------------------------------------------------------------------
 def dense_frame(small_workload, n_target: int = 6_000_000, seed: int = 5):
     """large_scale_05's geometry on a dense VoI: a frame of the small workload cropped to 30 m, replicated with jitter (the way
