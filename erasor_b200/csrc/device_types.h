@@ -11,6 +11,7 @@ constexpr uint16_t kNoBin16   = 0xFFFFu;       // bin id of a point that failed 
 constexpr uint32_t kIdPad     = 1024;          // slack entries behind the bin-id arrays: K2 prefetches ids without bounds checks
 constexpr uint32_t kMapPad    = 256;           // slack points behind the resident map: node-mode K1 streams it without bounds checks
 constexpr int      kListWarps = 32;            // node mode: per-chunk stride of the per-warp VoI list counters (K1 runs 8 or 32 warps)
+constexpr uint32_t kK2Stage   = 512;           // node mode: per K2 warp and window, taken VoI entries staged for the scatter (beyond: re-walk)
 constexpr int      kMaxIter   = 8;             // gf_iter upper bound for the tap arrays
 
 // K1's profiling build (erasor_profile_k1): per warp, SM cycles spent in each phase of the node-mode map path, the warp's

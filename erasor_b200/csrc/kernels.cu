@@ -521,9 +521,13 @@ cudaError_t launch_k3(cudaStream_t st, const SrtParams& P, int F, const uint32_t
 // (40 x 360 bins in cloud mode) takes several window passes over the chunk's bin ids, so there is no bin-count limit
 // and no slow fallback.  NODE: points are read from the resident map and moved origin -> body on the way (fetch_VoI's
 // transform, OfflineMapUpdater.cpp:436), the source index is the global map index.
-// pass A of one window: per-slot counts of the warp's sub-range [s0, s1) into its own row
-__device__ __forceinline__ void k2_count_pass(const uint16_t* __restrict__ ids, uint32_t s0, uint32_t s1, const uint16_t* __restrict__ s_slot,
-                                              uint32_t win0, uint32_t ns, uint32_t* __restrict__ mine, int B, int lane) {
+// pass A of one window: per-slot counts of the warp's sub-range [s0, s1) into its own row.  STAGE (node mode): the positions of
+// the taken entries also go, in order, to the warp's staging row stage[0, cap) from index n_st on; returns the running number of
+// taken entries, which exceeds cap when they did not all fit.
+template <bool STAGE>
+__device__ __forceinline__ uint32_t k2_count_pass(const uint16_t* __restrict__ ids, uint32_t s0, uint32_t s1, const uint16_t* __restrict__ s_slot,
+                                                  uint32_t win0, uint32_t ns, uint32_t* __restrict__ mine, int B, int lane,
+                                                  uint16_t* __restrict__ stage = nullptr, uint32_t n_st = 0u, uint32_t cap = 0u) {
     // Both passes walk the sub-range 256 points (8 steps of 32) at a time; the bin ids of the next block are loaded while
     // the current one is processed, so that no step waits on global memory.  Only points of the window's slots take part
     // in the match_any ranking.
@@ -545,12 +549,18 @@ __device__ __forceinline__ void k2_count_pass(const uint16_t* __restrict__ ids, 
             if (take) {
                 const unsigned peers = __match_any_sync(tmask, sl);
                 if (lane == __ffs(peers) - 1) mine[sl] += __popc(peers);
+                if constexpr (STAGE) {
+                    const uint32_t at = n_st + __popc(tmask & ((1u << lane) - 1u));
+                    if (at < cap) stage[at] = (uint16_t)i;
+                }
             }
+            if constexpr (STAGE) n_st += __popc(tmask);
             __syncwarp();
         }
 #pragma unroll
         for (int u = 0; u < 8; ++u) cur[u] = nxt[u];
     }
+    return n_st;
 }
 
 // pass B of one window: re-walk the sub-range in order; mine[] holds the absolute destination of the next point per slot
@@ -611,46 +621,134 @@ __device__ __forceinline__ void k2_scatter_pass(const uint16_t* __restrict__ ids
     }
 }
 
-// One window [win0, win0 + ns) of slots of the CTA's chunk (row `row`): zero the warps' rows, count pass, column scan into absolute
+// Node mode, pass B from the staging row: the n (<= kK2Stage) taken entries the count pass kept, in order.  Groups of 4 x 32
+// entries: every list_idx load of a group goes out (with its bin id), then every map-point load, then the ranking against mine[],
+// then the transforms and stores -- no load waits on the ranking.  Lanes past n repeat the last staged entry (n > 0 here: a
+// position K1 wrote in this step, so its list_idx and map point are in bounds) and store nothing.
+__device__ __forceinline__ void k2_scatter_staged(const uint16_t* __restrict__ stage, uint32_t n, const uint16_t* __restrict__ ids,
+                                                  const uint16_t* __restrict__ s_slot, uint32_t win0, uint32_t* __restrict__ mine, int B, int lane,
+                                                  const float4* __restrict__ src, const float* __restrict__ s_T, uint32_t out_base,
+                                                  float4* __restrict__ out_pts, uint32_t* __restrict__ out_src, const uint32_t* __restrict__ lidx) {
+    constexpr int G = 4;
+    for (uint32_t k0 = 0; k0 < n; k0 += 32u * G) {
+        uint32_t key[G], si[G], dst[G];
+        bool take[G];
+        float4 pv[G];
+#pragma unroll
+        for (int u = 0; u < G; ++u) {
+            const uint32_t k = k0 + (uint32_t)u * 32u + lane;
+            take[u] = k < n;                                  // every staged entry belongs to a slot of the window
+            const uint32_t pos = (uint32_t)stage[min(k, n - 1u)];
+            key[u] = ids[pos];
+            si[u]  = lidx[pos];
+        }
+#pragma unroll
+        for (int u = 0; u < G; ++u) pv[u] = src[si[u]];
+#pragma unroll
+        for (int u = 0; u < G; ++u) {
+            const uint32_t sl   = (uint32_t)s_slot[min(key[u], (uint32_t)B)] - win0;
+            const uint32_t base = take[u] ? mine[sl] : 0u;
+            const unsigned tmask = __ballot_sync(FULL_MASK, take[u]);   // also orders the reads of mine[] before the updates below
+            dst[u] = 0u;
+            if (take[u]) {
+                const unsigned peers = __match_any_sync(tmask, sl);
+                if (lane == __ffs(peers) - 1) mine[sl] = base + __popc(peers);
+                dst[u] = base + __popc(peers & ((1u << lane) - 1u));
+            }
+            __syncwarp();
+        }
+#pragma unroll
+        for (int u = 0; u < G; ++u) {
+            if (take[u]) {
+                const size_t o = (size_t)out_base + dst[u];
+                out_pts[o] = pcl_affine(s_T, pv[u]);
+                out_src[o] = si[u];
+            }
+        }
+    }
+}
+
+// Node mode: the exclusive prefix of the chunk's K1 list counts, s_lpre[0, k1_warps] (warp 0; the caller's next barrier publishes it).
+// K1 warp k's list starts at position k * sub of the chunk and holds list_cnt[row * kListWarps + k] entries; in warp order the
+// lists are map order, and s_lpre numbers that concatenation.
+__device__ __forceinline__ void k2_list_prefix(const uint32_t* __restrict__ list_cnt, uint32_t row, int k1_warps, uint32_t* s_lpre) {
+    const int tid = threadIdx.x;
+    if (tid >= 32) return;
+    const uint32_t c = (tid < k1_warps) ? list_cnt[(size_t)row * kListWarps + tid] : 0u;
+    uint32_t incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL_MASK, incl, o); if (tid >= o) incl += v; }
+    s_lpre[tid + 1] = incl;
+    if (tid == 0) s_lpre[0] = 0u;
+}
+
+// bytes of K2's u16 slot table (B + 1 bins, padded); node mode's staging rows follow it
+__host__ __device__ __forceinline__ size_t k2_slot_bytes(int B) { return ((sizeof(uint16_t) * ((size_t)B + 2)) + 15) & ~(size_t)15; }
+
+// One window [win0, win0 + ns) of slots of the CTA's chunk: zero the warps' rows, count pass, column scan into absolute
 // destinations from the window's bases, scatter pass.  The caller writes the bases into s_base[0, ns) (the barriers here order them
 // before the column scan) and calls after a barrier behind its last use of the rows s_tab[0, W * ns).  Each warp takes its part of
-// the chunk: a contiguous sub-range of its points -- or, in node mode, the dense VoI lists that k1_warps / W of K1's warps left for
-// their sub-ranges (same split, same order).
+// the chunk: a contiguous sub-range of its points -- or, in node mode, an even share [w L / W, (w + 1) L / W) of the L entries of the
+// chunk's VoI lists taken in order (s_lpre, k2_list_prefix), which may span several of K1's lists.  Node mode walks the bin ids once:
+// the count pass stages the positions of the warp's taken entries (kK2Stage per warp in s_stage), and the scatter reads only those;
+// a warp whose taken entries do not fit re-walks its share instead.  Either way warp order is list order, so the column scan keeps
+// map order inside every bin.
 template <int W, bool NODE>
-__device__ __forceinline__ void k2_window(const ChunkDesc& cd, uint32_t row, uint32_t win0, uint32_t ns, uint32_t* s_tab, const uint32_t* s_base,
+__device__ __forceinline__ void k2_window(const ChunkDesc& cd, uint32_t win0, uint32_t ns, uint32_t* s_tab, const uint32_t* s_base,
                                           const uint16_t* s_slot, const float* s_T, int B, const uint16_t* __restrict__ bin_ids,
-                                          const float4* __restrict__ pts, const uint32_t* __restrict__ list_idx, const uint32_t* __restrict__ list_cnt,
-                                          int k1_warps, float4* __restrict__ out_pts, uint32_t* __restrict__ out_src) {
+                                          const float4* __restrict__ pts, const uint32_t* __restrict__ list_idx, const uint32_t* s_lpre,
+                                          uint16_t* s_stage, int k1_warps, float4* __restrict__ out_pts, uint32_t* __restrict__ out_src) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int      nseg = NODE ? k1_warps / W : 1;
-    const uint32_t sub  = (((cd.len + (NODE ? k1_warps : W) - 1) / (NODE ? k1_warps : W)) + 31u) & ~31u;
-    auto seg_range = [&](int g, uint32_t& s0, uint32_t& s1) {
-        const uint32_t kw = (uint32_t)warp * nseg + g;
-        s0 = min(cd.len, kw * sub);
-        s1 = NODE ? s0 + list_cnt[(size_t)row * kListWarps + kw] : min(cd.len, s0 + sub);
-    };
     const uint16_t* ids = bin_ids + cd.bin_begin;
-    const uint32_t local0 = cd.begin - cd.frame_begin;
-    const float4* src = NODE ? pts : pts + cd.begin;
-    const uint32_t* lidx = NODE ? list_idx + cd.bin_begin : nullptr;
     uint32_t* mine = s_tab + (size_t)warp * ns;              // row stride of this window: ns
     for (uint32_t i = tid; i < (uint32_t)W * ns; i += W * 32) s_tab[i] = 0u;
     __syncthreads();
-    for (int g = 0; g < nseg; ++g) { uint32_t s0, s1; seg_range(g, s0, s1); k2_count_pass(ids, s0, s1, s_slot, win0, ns, mine, B, lane); }
-    __syncthreads();
-    for (uint32_t j = tid; j < ns; j += W * 32) {
-        uint32_t run = s_base[j];
+    auto column_scan = [&]() {
+        for (uint32_t j = tid; j < ns; j += W * 32) {
+            uint32_t run = s_base[j];
 #pragma unroll
-        for (int w = 0; w < W; ++w) {
-            const uint32_t c = s_tab[(size_t)w * ns + j];
-            s_tab[(size_t)w * ns + j] = run;
-            run += c;
+            for (int w = 0; w < W; ++w) {
+                const uint32_t c = s_tab[(size_t)w * ns + j];
+                s_tab[(size_t)w * ns + j] = run;
+                run += c;
+            }
         }
-    }
-    __syncthreads();
-    for (int g = 0; g < nseg; ++g) {
-        uint32_t s0, s1; seg_range(g, s0, s1);
-        k2_scatter_pass<NODE>(ids, s0, s1, s_slot, win0, ns, mine, B, lane, src, s_T, cd.out_base, local0, out_pts, out_src, lidx);
+    };
+    if constexpr (NODE) {
+        const uint32_t sub = (((cd.len + k1_warps - 1) / k1_warps) + 31u) & ~31u;      // K1's split (k1_rpod_bin, k1_geo)
+        const uint32_t L = s_lpre[k1_warps];
+        const uint32_t lo = (uint32_t)((uint64_t)L * warp / W), hi = (uint32_t)((uint64_t)L * (warp + 1) / W);
+        // the warp's share as contiguous position ranges, in order: [at + a, at + b) of K1 warp k's list for every k it reaches
+        auto for_pieces = [&](auto&& piece) {
+            for (int k = 0; k < k1_warps; ++k) {
+                const uint32_t p0 = s_lpre[k], a = max(lo, p0), b = min(hi, s_lpre[k + 1]);
+                if (a < b) { const uint32_t at = min(cd.len, (uint32_t)k * sub) - p0; piece(at + a, at + b); }
+            }
+        };
+        const uint32_t* lidx = list_idx + cd.bin_begin;
+        uint16_t* stage = s_stage + (size_t)warp * kK2Stage;
+        const uint32_t cap = (cd.len <= 0x10000u) ? kK2Stage : 0u;      // positions are staged as 16-bit offsets in the chunk
+        uint32_t n_st = 0u;
+        for_pieces([&](uint32_t s0, uint32_t s1) { n_st = k2_count_pass<true>(ids, s0, s1, s_slot, win0, ns, mine, B, lane, stage, n_st, cap); });
+        __syncthreads();
+        column_scan();
+        __syncthreads();
+        if (n_st <= cap) {
+            k2_scatter_staged(stage, n_st, ids, s_slot, win0, mine, B, lane, pts, s_T, cd.out_base, out_pts, out_src, lidx);
+        } else {
+            for_pieces([&](uint32_t s0, uint32_t s1) {
+                k2_scatter_pass<true>(ids, s0, s1, s_slot, win0, ns, mine, B, lane, pts, s_T, cd.out_base, 0u, out_pts, out_src, lidx);
+            });
+        }
+    } else {
+        const uint32_t sub = (((cd.len + W - 1) / W) + 31u) & ~31u;
+        const uint32_t s0 = min(cd.len, (uint32_t)warp * sub), s1 = min(cd.len, s0 + sub);
+        k2_count_pass<false>(ids, s0, s1, s_slot, win0, ns, mine, B, lane);
+        __syncthreads();
+        column_scan();
+        __syncthreads();
+        k2_scatter_pass<false>(ids, s0, s1, s_slot, win0, ns, mine, B, lane, pts + cd.begin, s_T, cd.out_base, cd.begin - cd.frame_begin,
+                               out_pts, out_src, nullptr);
     }
 }
 
@@ -665,8 +763,9 @@ k2_scatter_win(const ChunkDesc* __restrict__ chunks, uint32_t chunk_base, const 
                const uint32_t* __restrict__ dst_start /*[F][B+2] of this cloud*/, const uint32_t* __restrict__ flag_slot /*[F][B]; null: every bin + complement*/,
                const uint32_t* __restrict__ n_flagged /*[F]*/, float4* __restrict__ out_pts, uint32_t* __restrict__ out_src, int B, uint32_t SW,
                const uint32_t* __restrict__ list_idx, const uint32_t* __restrict__ list_cnt, int k1_warps, K2Second second) {
-    extern __shared__ uint32_t s_tab[];   // [W][ns] per-warp counters / destinations | [SW] bases | u16 slot of every bin [B+1]
+    extern __shared__ uint32_t s_tab[];   // [W][ns] per-warp counters / destinations | [SW] bases | u16 slot of every bin [B+1] | NODE: u16 staging [W][kK2Stage]
     __shared__ float s_T[12];
+    __shared__ uint32_t s_lpre[NODE ? kListWarps + 1 : 1];
     const int tid = threadIdx.x;
     const uint32_t row = chunk_base + blockIdx.x;
     if (DUAL && row >= second.first_row) {        // CTA-uniform
@@ -677,6 +776,8 @@ k2_scatter_win(const ChunkDesc* __restrict__ chunks, uint32_t chunk_base, const 
     const uint32_t* pref = ch_cnt + (size_t)row * (B + 1);
     uint32_t* s_base = s_tab + (size_t)W * SW;
     uint16_t* s_slot = reinterpret_cast<uint16_t*>(s_base + SW);
+    uint16_t* s_stage = s_slot + k2_slot_bytes(B) / sizeof(uint16_t);
+    if constexpr (NODE) k2_list_prefix(list_cnt, row, k1_warps, s_lpre);
     const uint32_t n_slots = flag_slot ? n_flagged[cd.frame] : (uint32_t)(B + 1);
     if (flag_slot) {
         const uint32_t* fs = flag_slot + (size_t)cd.frame * B;
@@ -694,7 +795,7 @@ k2_scatter_win(const ChunkDesc* __restrict__ chunks, uint32_t chunk_base, const 
             const uint32_t sl = (uint32_t)s_slot[b] - win0;
             if (sl < ns) s_base[sl] = ds[b] + pref[b];
         }
-        k2_window<W, NODE>(cd, row, win0, ns, s_tab, s_base, s_slot, s_T, B, bin_ids, pts, list_idx, list_cnt, k1_warps, out_pts, out_src);
+        k2_window<W, NODE>(cd, win0, ns, s_tab, s_base, s_slot, s_T, B, bin_ids, pts, list_idx, s_lpre, s_stage, k1_warps, out_pts, out_src);
     }
 }
 
@@ -732,10 +833,11 @@ k2_srt_scatter_body(const SrtParams& P, int F, const ChunkDesc* __restrict__ chu
                     uint32_t* __restrict__ queue, uint32_t* __restrict__ bucket_list,
                     float4* __restrict__ out_pts, uint32_t* __restrict__ out_src, uint32_t SW,
                     const uint32_t* __restrict__ list_idx, const uint32_t* __restrict__ list_cnt, int k1_warps, const SrtSweep* sweep) {
-    extern __shared__ uint32_t s_tab[];   // [W][ns] rows | [SW] bases | u16 slot of every bin [B+1]
+    extern __shared__ uint32_t s_tab[];   // [W][ns] rows | [SW] bases | u16 slot of every bin [B+1] | NODE: u16 staging [W][kK2Stage]
     __shared__ float    s_T[12];
     __shared__ uint32_t s_part[34];
     __shared__ uint32_t s_bcast[2];
+    __shared__ uint32_t s_lpre[NODE ? kListWarps + 1 : 1];
     constexpr int NT = W * 32;
     const int B = P.B;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -746,35 +848,50 @@ k2_srt_scatter_body(const SrtParams& P, int F, const ChunkDesc* __restrict__ chu
     const bool leader = row == row0;
     uint32_t* s_base = s_tab + (size_t)W * SW;
     uint16_t* s_slot = reinterpret_cast<uint16_t*>(s_base + SW);
+    uint16_t* s_stage = s_slot + k2_slot_bytes(B) / sizeof(uint16_t);
     const uint32_t* cm = cnt + ((size_t)0 * F + f) * (B + 1);
     const uint32_t* cq = cnt + ((size_t)1 * F + f) * (B + 1);
     const uint32_t* mnm = zmin + ((size_t)0 * F + f) * B; const uint32_t* mxm = zmax + ((size_t)0 * F + f) * B;
     const uint32_t* mnq = zmin + ((size_t)1 * F + f) * B; const uint32_t* mxq = zmax + ((size_t)1 * F + f) * B;
+    if constexpr (NODE) k2_list_prefix(list_cnt, row, k1_warps, s_lpre);
 
     // ---- Scan Ratio Test: flagged bit per bin (coalesced over the tables) ----
+    // Each thread takes its bins kPro at a time: all six table loads of the batch go out before any FP64 work (no branch between
+    // them; a bin with an empty cloud is decided by srt_is_flagged / srt_variant_mask themselves).
+    constexpr int kPro = SWEEP ? 1 : 4;      // the sweep's per-variant loop needs the registers of three more bins (spills at 2 and 4)
+    __shared__ uint32_t s_vcnt[SWEEP ? kMaxSweepVariants : 1];    // sweep: the leader counts the flagged bins of every variant
     if constexpr (SWEEP) {
-        // a bin takes a slot when any variant flags it; the leader counts the flagged bins of every variant
-        __shared__ uint32_t s_vcnt[kMaxSweepVariants];
         if (tid < kMaxSweepVariants) s_vcnt[tid] = 0u;
         __syncthreads();
-        for (int b = tid; b <= B; b += NT) {
-            uint32_t m = 0u;
-            if (b < B) m = srt_variant_mask(*sweep, P.version, cm[b], cq[b], mxm[b], mnm[b], mxq[b], mnq[b]);
-            s_slot[b] = m ? (uint16_t)0u : (uint16_t)0xFFFFu;
-            if (leader)
-                for (uint32_t r = m; r; r &= r - 1u) atomicAdd(&s_vcnt[__ffs(r) - 1], 1u);
+    }
+    for (int bb = tid; bb <= B; bb += NT * kPro) {
+        uint32_t mc[kPro], qc[kPro], zxm[kPro], znm[kPro], zxq[kPro], znq[kPro];
+#pragma unroll
+        for (int u = 0; u < kPro; ++u) {
+            const int b = bb + u * NT;
+            const bool in = b < B;
+            mc[u]  = in ? cm[b]  : 0u; qc[u]  = in ? cq[b]  : 0u;
+            zxm[u] = in ? mxm[b] : 0u; znm[u] = in ? mnm[b] : 0u;
+            zxq[u] = in ? mxq[b] : 0u; znq[u] = in ? mnq[b] : 0u;
         }
+#pragma unroll
+        for (int u = 0; u < kPro; ++u) {
+            const int b = bb + u * NT;
+            if (b > B) break;
+            if constexpr (SWEEP) {
+                // a bin takes a slot when any variant flags it
+                const uint32_t m = srt_variant_mask(*sweep, P.version, mc[u], qc[u], zxm[u], znm[u], zxq[u], znq[u]);
+                s_slot[b] = m ? (uint16_t)0u : (uint16_t)0xFFFFu;
+                if (leader)
+                    for (uint32_t r = m; r; r &= r - 1u) atomicAdd(&s_vcnt[__ffs(r) - 1], 1u);
+            } else {
+                s_slot[b] = srt_is_flagged(P, mc[u], qc[u], zxm[u], znm[u], zxq[u], znq[u]) ? (uint16_t)0u : (uint16_t)0xFFFFu;
+            }
+        }
+    }
+    if constexpr (SWEEP) {
         __syncthreads();
         if (leader && tid < sweep->n) sweep->n_flagged[(size_t)f * kMaxSweepVariants + tid] = s_vcnt[tid];
-    } else {
-        for (int b = tid; b <= B; b += NT) {
-            bool fl = false;
-            if (b < B) {
-                const uint32_t mc = cm[b], qc = cq[b];
-                if (mc != 0u && qc != 0u) fl = srt_is_flagged(P, mc, qc, mxm[b], mnm[b], mxq[b], mnq[b]);
-            }
-            s_slot[b] = fl ? (uint16_t)0u : (uint16_t)0xFFFFu;
-        }
     }
     if (NODE && tid < 12) s_T[tid] = poses[f].T[tid];
     __syncthreads();
@@ -827,12 +944,12 @@ k2_srt_scatter_body(const SrtParams& P, int F, const ChunkDesc* __restrict__ chu
             const uint32_t b = s_bin[j];
             s_base[j] = cm[b];
             uint32_t pf = 0u;
-            for (uint32_t k0 = row0; k0 < row; k0 += 8u) {    // eight rows per round trip
-                uint32_t v[8];
+            for (uint32_t k0 = row0; k0 < row; k0 += 16u) {   // sixteen rows per round trip, all loads before the sum
+                uint32_t v[16];
 #pragma unroll
-                for (uint32_t u = 0; u < 8u; ++u) v[u] = (k0 + u < row) ? ch_cnt[(size_t)(k0 + u) * (B + 1) + b] : 0u;
+                for (uint32_t u = 0; u < 16u; ++u) v[u] = (k0 + u < row) ? ch_cnt[(size_t)(k0 + u) * (B + 1) + b] : 0u;
 #pragma unroll
-                for (uint32_t u = 0; u < 8u; ++u) pf += v[u];
+                for (uint32_t u = 0; u < 16u; ++u) pf += v[u];
             }
             s_pf[j] = pf;
         }
@@ -852,7 +969,7 @@ k2_srt_scatter_body(const SrtParams& P, int F, const ChunkDesc* __restrict__ chu
         // absolute base per slot, then the rows can be zeroed (s_bin / s_pf live in them)
         for (uint32_t j = tid; j < ns; j += NT) s_base[j] = win_carry + s_base[j] + s_pf[j];
         __syncthreads();
-        k2_window<W, NODE>(cd, row, win0, ns, s_tab, s_base, s_slot, s_T, B, bin_ids, pts, list_idx, list_cnt, k1_warps, out_pts, out_src);
+        k2_window<W, NODE>(cd, win0, ns, s_tab, s_base, s_slot, s_T, B, bin_ids, pts, list_idx, s_lpre, s_stage, k1_warps, out_pts, out_src);
         win_carry += win_total;
     }
 }
@@ -876,15 +993,16 @@ template <int W, bool NODE>
 __global__ void __launch_bounds__(W * 32, 4)
 k2_srt_sweep_scatter(K2_SRT_PARAMS, const __grid_constant__ SrtSweep sweep) { k2_srt_scatter_body<W, NODE, true>(K2_SRT_ARGS, &sweep); }
 
-static void k2_smem_plan(int B, bool with_complement, uint32_t& SW, size_t& smem) {
+static void k2_smem_plan(int B, bool with_complement, bool node, uint32_t& SW, size_t& smem) {
     constexpr int W = 8;
-    const size_t fixed  = ((sizeof(uint16_t) * ((size_t)B + 2)) + 15) & ~(size_t)15;
+    // the slot table, and in node mode the warps' staging rows behind it (8 KB: 900 bins keep four CTAs per SM at 42 KB)
+    const size_t fixed  = k2_slot_bytes(B) + (node ? sizeof(uint16_t) * W * (size_t)kK2Stage : 0);
     // one window over all slots while that leaves two CTAs per SM; beyond that (40 x 360 bins) the largest window that does:
     // mask mode rarely has more flagged bins per frame than it holds, cloud mode takes ceil((B + 1) / window) passes
     const uint32_t n_slots_max = with_complement ? (uint32_t)B + 1u : (uint32_t)B;
     const size_t full = sizeof(uint32_t) * (size_t)(W + 1) * n_slots_max + fixed;
     const size_t two_per_sm = 111 * 1024;                 // two CTAs per SM: (227 KB - static shared memory) / 2
-    const size_t budget = full <= two_per_sm ? full : two_per_sm;      // 40 x 360: 2356-slot windows (config 5 flags ~2060 bins per frame)
+    const size_t budget = full <= two_per_sm ? full : two_per_sm;      // 40 x 360: 2356-slot windows (2129 in node mode; config 5 flags ~2060 bins per frame)
     SW   = (uint32_t)std::min<size_t>(std::max<uint32_t>(n_slots_max, 1u), std::max<size_t>(1, (budget - fixed) / (sizeof(uint32_t) * (W + 1))));
     smem = sizeof(uint32_t) * (size_t)(W + 1) * SW + fixed;
 }
@@ -898,7 +1016,7 @@ cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const Chun
     constexpr int W = 8;
     if (k1_warps == 0) k1_warps = k1_big_tables(P.R, P.B) ? 32 : 8;     // the split K1 compacted the chunk's VoI points in
     uint32_t SW; size_t smem;
-    k2_smem_plan(P.B, false, SW, smem);
+    k2_smem_plan(P.B, false, poses != nullptr, SW, smem);
     cudaError_t e;
     if (sweep) {                                                  // node mode only
         auto kern = k2_srt_sweep_scatter<W, true>;
@@ -921,7 +1039,7 @@ cudaError_t launch_k2(cudaStream_t st, const ChunkDesc* chunks, uint32_t chunk_b
     if (n_chunks == 0) return cudaSuccess;
     constexpr int W = 8;
     uint32_t SW; size_t smem;
-    k2_smem_plan(B, flag_slot == nullptr, SW, smem);
+    k2_smem_plan(B, flag_slot == nullptr, poses != nullptr, SW, smem);
     cudaError_t e;
     const K2Second none{0u, nullptr, nullptr, nullptr, nullptr, nullptr};
     if (poses) {
@@ -943,7 +1061,7 @@ cudaError_t launch_k2_both(cudaStream_t st, const ChunkDesc* chunks, uint32_t n_
     if (n_chunks_map + n_chunks_qry == 0) return cudaSuccess;
     constexpr int W = 8;
     uint32_t SW; size_t smem;
-    k2_smem_plan(B, true, SW, smem);
+    k2_smem_plan(B, true, false, SW, smem);
     auto kern = k2_scatter_win<W, false, true>;
     cudaError_t e = ensure_dyn_smem(kern, smem);
     if (e != cudaSuccess) return e;
