@@ -35,6 +35,7 @@ EXPORTS = [
     "erasor_voxelize_batch",
     "erasor_set_node_inserts", "erasor_get_node_inserts", "erasor_map_append_inserts", "erasor_map_inserts", "erasor_map_clear_inserts",
     "erasor_save_node_map",
+    "erasor_map_create_retest", "erasor_map_retest_extents", "erasor_process_nodes_retest", "erasor_process_nodes_retest_async",
     "erasor_comm_unique_id", "erasor_comm_init", "erasor_comm_destroy", "erasor_allgather_and_keep", "erasor_and_keep_masks",
     "erasor_get_kernel_time_ms", "erasor_reset_kernel_times", "erasor_forget_run_history", "erasor_get_rgpf_profile", "erasor_get_srt_profile", "erasor_profile_k1",
     "erasor_updater_create", "erasor_updater_destroy", "erasor_updater_reset", "erasor_updater_last_error", "erasor_updater_process_node", "erasor_updater_prefetch_scan",
@@ -226,6 +227,10 @@ def _load():
     L.erasor_map_inserts.argtypes = [c_void_p, POINTER(c_void_p), POINTER(c_size_t)]
     L.erasor_map_clear_inserts.argtypes = [c_void_p]
     L.erasor_save_node_map.argtypes = [c_void_p, c_void_p, c_float, POINTER(c_void_p), POINTER(c_size_t)]
+    L.erasor_map_create_retest.argtypes = [c_void_p, POINTER(c_void_p)]
+    L.erasor_map_retest_extents.argtypes = [c_void_p, POINTER(c_size_t), POINTER(c_uint64)]
+    L.erasor_process_nodes_retest.argtypes = [c_void_p, POINTER(c_double), c_void_p, POINTER(c_uint64), c_int, c_int, c_double, c_void_p, c_int]
+    L.erasor_process_nodes_retest_async.argtypes = L.erasor_process_nodes_retest.argtypes
     L.erasor_comm_unique_id.argtypes = [c_void_p]
     L.erasor_comm_init.argtypes = [c_void_p, c_void_p, c_int, c_int]
     L.erasor_comm_destroy.argtypes = [c_void_p]
@@ -718,6 +723,55 @@ class Handle(_Native):
         keep = self._map.get_keep()
         return keep, (fk_dev.cpu().numpy() if fk_dev is not None else None)
 
+    # -- node-mode re-test, pass 2 (DESIGN.md section 8.4.1) -----------------------------------------------------------------------
+    def process_nodes_retest(self, poses7, query_xyzi, query_offsets, first_node: int, voi_max_range: float = 0.0, packed_xyz: bool = False):
+        """erasor_process_nodes_retest with host buffers: node f of the batch is store node first_node + f of the attached re-test
+        map (Map.create_retest) and sees only its extent.  Returns the map's keep mask after this batch."""
+        P = np.ascontiguousarray(poses7, dtype=np.float64).reshape(-1, 7)
+        q = _cloud(query_xyzi)
+        if packed_xyz:
+            q = np.ascontiguousarray(q[:, :3])
+        qo = np.ascontiguousarray(query_offsets, dtype=np.uint64)
+        F = len(qo) - 1
+        assert len(P) == F
+        keep = np.empty(max(self._map.size, 1), dtype=np.uint8)
+        self._ck(self.L.erasor_process_nodes_retest(self.h, P.ctypes.data_as(POINTER(c_double)), q.ctypes.data if len(q) else None,
+                                                    qo.ctypes.data_as(POINTER(c_uint64)), F, int(first_node), float(voi_max_range),
+                                                    keep.ctypes.data, PTR_HOST | (PTR_QUERY_XYZ if packed_xyz else 0)))
+        self.n_frames = F
+        return keep[:self._map.size]
+
+    def process_nodes_retest_ptr(self, poses7: np.ndarray, query_ptr: int, query_offsets: np.ndarray, first_node: int, voi_max_range: float,
+                                 keep_out_ptr: int, ptr_kind: int, asynchronous: bool = False):
+        """Raw-pointer form of process_nodes_retest (device tensors or pinned host memory); poses7 and query_offsets must stay alive
+        until an asynchronous submission has been waited for."""
+        assert poses7.dtype == np.float64 and poses7.flags["C_CONTIGUOUS"] and query_offsets.dtype == np.uint64
+        fn = self.L.erasor_process_nodes_retest_async if asynchronous else self.L.erasor_process_nodes_retest
+        F = len(query_offsets) - 1
+        self._ck(fn(self.h, poses7.ctypes.data_as(POINTER(c_double)), c_void_p(query_ptr) if query_ptr else None,
+                    query_offsets.ctypes.data_as(POINTER(c_uint64)), F, int(first_node), float(voi_max_range),
+                    c_void_p(keep_out_ptr) if keep_out_ptr else None, ptr_kind))
+        self.n_frames = F
+
+    def process_scans_retest(self, poses7, raw_xyzi, raw_offsets, query_voxel_size: float, lidar2body7, first_node: int,
+                             voi_max_range: float = 0.0, ptr_kind: int = PTR_HOST):
+        """process_scans for the re-test pass: the raw scans voxelised and moved to the body frame again (erasor_voxelize_batch is
+        deterministic, so these are the queries pass 1 saw), then erasor_process_nodes_retest from store node first_node.  Returns
+        the attached re-test map's keep mask after this batch."""
+        if ptr_kind == PTR_DEVICE:
+            d, qo = self.voxelize_batch_ptr(int(raw_xyzi), raw_offsets, query_voxel_size, 0, lidar2body7, PTR_DEVICE)
+        else:
+            x = _cloud(raw_xyzi)
+            d, qo = self.voxelize_batch_ptr(x.ctypes.data if len(x) else 0, raw_offsets, query_voxel_size, 0, lidar2body7, PTR_HOST)
+        P = np.ascontiguousarray(poses7, dtype=np.float64).reshape(-1, 7)
+        F = len(qo) - 1
+        assert len(P) == F
+        self._ck(self.L.erasor_process_nodes_retest(self.h, P.ctypes.data_as(POINTER(c_double)), c_void_p(d) if d else None,
+                                                    qo.ctypes.data_as(POINTER(c_uint64)), F, int(first_node), float(voi_max_range), None,
+                                                    PTR_DEVICE))
+        self.n_frames = F
+        return self._map.get_keep()
+
     def save_static_map(self, m: "Map", voxel: float) -> np.ndarray:
         """save_static_map of node mode (OfflineMapUpdater.cpp:174-196 without the file): the resident map's points under its keep
         mask, followed by the map's insert store (empty unless inserts were appended), voxelised at `voxel`, in the map frame."""
@@ -869,6 +923,27 @@ class Map(_Native):
         rc = self.L.erasor_map_clear_inserts(self.h)
         if rc != OK:
             raise ErasorError(rc, "erasor_map_clear_inserts")
+
+    # -- node-mode re-test (DESIGN.md section 8.4.1) -------------------------------------------------------------------------------
+    def create_retest(self) -> "Map":
+        """The re-test map of this map (erasor_map_create_retest): the kept points in map order, then the insert store in node
+        order; keep all ones, empty store.  This map is not changed."""
+        r = Map.__new__(Map)
+        r._create("erasor_map_create_retest", self.h)
+        return r
+
+    def retest_extents(self) -> np.ndarray:
+        """uint64 [n_nodes]: store node k sees the prefix [0, extents[k]) of this re-test map"""
+        n = c_size_t(0)
+        rc = self.L.erasor_map_retest_extents(self.h, ctypes.byref(n), None)
+        if rc != OK:
+            raise ErasorError(rc, "erasor_map_retest_extents: not a re-test map")
+        out = np.zeros(n.value, dtype=np.uint64)
+        if n.value:
+            rc = self.L.erasor_map_retest_extents(self.h, ctypes.byref(n), out.ctypes.data_as(POINTER(c_uint64)))
+            if rc != OK:
+                raise ErasorError(rc, "erasor_map_retest_extents")
+        return out
 
 
 class Updater(_Native):

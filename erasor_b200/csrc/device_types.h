@@ -29,9 +29,11 @@ struct ChunkDesc {
     uint32_t len;          // points in this chunk
     uint32_t frame;        // frame index
     uint32_t cloud;        // 0 map, 1 query
-    uint32_t frame_begin;  // source index of the frame's first point (node mode, map cloud: 0 -- every frame scans the whole map)
-    uint32_t bin_begin;    // index of the chunk's first point in the bin-id array (batch mode: == begin; node mode: frame * n_map + begin)
-    uint32_t out_base;     // base of the frame's region in the scattered arrays and the per-frame masks (batch: frame_begin; node: frame * n_map)
+    uint32_t frame_begin;  // source index of the frame's first point (node mode, map cloud: 0 -- every frame scans a prefix of the map)
+    uint32_t bin_begin;    // index of the chunk's first point in the bin-id array (batch mode: == begin; node mode: the frame's map offset
+                           // + begin, the offsets being f * n_map, or a re-test map's cumulative extents)
+    uint32_t out_base;     // base of the frame's region in the scattered arrays and the per-frame masks (batch: frame_begin; node: the
+                           // frame's map offset)
     uint32_t pad_;
 };
 

@@ -46,6 +46,9 @@ struct erasor_map_ctx {
     size_t       n = 0;
     DeviceBuffer d_ins;                        // node-mode inserts appended by the callers (erasor_map_append_inserts), float4 [n_ins]
     size_t       n_ins = 0;
+    std::vector<uint64_t> ins_node_off{0};     // the store offset of every appended node, in append order, then n_ins
+    bool         retest = false;               // made by erasor_map_create_retest ...
+    std::vector<uint64_t> extents;             // ... and then node k of its source's store sees the prefix [0, extents[k])
     cudaStream_t st = nullptr;
     std::string  err;
 };
@@ -317,8 +320,9 @@ uint32_t choose_chunk(const erasor_ctx* h, const uint64_t* map_off, const uint64
 }
 
 // Build chunk descriptors + per-frame chunk ranges + frame offsets, upload them, size every buffer.
-// mode 0: single frame, cloud outputs; 1: batch of (map_voi, query_voi) pairs, masks; 2: node mode -- map_off is
-// {0, n_map, 2 n_map, ...}: every frame scans the whole resident map (fetch_VoI fused into K1), masks on global indices.
+// mode 0: single frame, cloud outputs; 1: batch of (map_voi, query_voi) pairs, masks; 2: node mode -- frame f scans the prefix
+// [0, map_off[f+1] - map_off[f]) of the resident map (fetch_VoI fused into K1): the whole map ({0, n_map, 2 n_map, ...}) or a
+// re-test node's extent; masks on global indices.
 int prepare_batch(erasor_ctx* h, const uint64_t* map_off, const uint64_t* qry_off, int F, int mode) {
     if (F <= 0) { h->err = "n_frames must be positive"; return ERASOR_E_INVALID; }
     const size_t NM = map_off[F], NQ = qry_off[F];
@@ -1357,9 +1361,11 @@ int read_node_voi_counts(erasor_handle_t h, uint32_t* out) {
     return ERASOR_OK;
 }
 
+// extents (nullable, n_frames entries): frame f scans only the prefix [0, extents[f]) of the attached map (a re-test map's nodes,
+// erasor_process_nodes_retest); without them every frame scans the whole map
 int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                        double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind, bool async,
-                       std::shared_ptr<const SweepPlan> sweep = nullptr) {
+                       std::shared_ptr<const SweepPlan> sweep = nullptr, const uint64_t* extents = nullptr) {
     if (!h || !poses7 || !query_offsets) { if (h) h->err = "null argument"; return ERASOR_E_INVALID; }
     if (!h->map) { h->err = "erasor_process_nodes: no map attached (erasor_attach_map)"; return ERASOR_E_STATE; }
     if (n_frames <= 0) { h->err = "n_frames must be positive"; return ERASOR_E_INVALID; }
@@ -1398,8 +1404,9 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         while (f1 < n_frames && f1 - f0 < max_frames && fits(f1)) ++f1;
         if (f1 == f0) { h->err = "a single query exceeds 2^32 points"; return ERASOR_E_INVALID; }
         const int F = f1 - f0;
-        mo.resize((size_t)F + 1);
-        for (int f = 0; f <= F; ++f) mo[f] = (uint64_t)f * N;
+        // each frame's map side is its own range of the bin-id / scatter arrays, the map read from index 0 (prepare_batch, mode 2)
+        mo.assign((size_t)F + 1, 0);
+        for (int f = 0; f < F; ++f) mo[f + 1] = mo[f] + (extents ? extents[f0 + f] : N);
         const uint64_t q0 = query_offsets[f0];
         qo.assign(query_offsets + f0, query_offsets + f1 + 1);
         for (auto& v : qo) v -= q0;
@@ -1563,6 +1570,37 @@ int erasor_process_nodes(erasor_handle_t h, const double* poses7, const float* q
 int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                                double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind) {
     return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, frame_keep, keep_out, ptr_kind, true);
+}
+
+extern "C++" {
+namespace {
+// pass 2 of the node-mode re-test (DESIGN.md section 8.4.1): the plain node path with each frame's map side cut to its node's extent
+int process_nodes_retest(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                         int first_node, double voi_max_range, uint8_t* keep_out, int ptr_kind, bool async) {
+    if (!h) return ERASOR_E_INVALID;
+    if (!poses7 || !query_offsets) { h->err = "null argument"; return ERASOR_E_INVALID; }
+    if (!h->map) { h->err = "erasor_process_nodes_retest: no map attached (erasor_attach_map)"; return ERASOR_E_STATE; }
+    if (h->pending) { h->err = "erasor_process_nodes_retest while a submission is pending (erasor_wait first)"; return ERASOR_E_STATE; }
+    if (!h->map->retest) { h->err = "erasor_process_nodes_retest: the attached map was not made by erasor_map_create_retest"; return ERASOR_E_INVALID; }
+    if (h->node_inserts) { h->err = "the re-test pass has no node inserts: erasor_set_node_inserts(h, 0) first"; return ERASOR_E_INVALID; }
+    const size_t n_nodes = h->map->extents.size();
+    if (n_frames <= 0 || first_node < 0 || (size_t)first_node + (size_t)n_frames > n_nodes) {
+        h->err = "erasor_process_nodes_retest: nodes [first_node, first_node + n_frames) must lie in [0, " + std::to_string(n_nodes) + ")";
+        return ERASOR_E_INVALID;
+    }
+    return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, voi_max_range, nullptr, keep_out, ptr_kind, async, nullptr,
+                              h->map->extents.data() + first_node);
+}
+}  // namespace
+}  // extern "C++"
+
+int erasor_process_nodes_retest(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                int first_node, double voi_max_range, uint8_t* keep_out, int ptr_kind) {
+    return process_nodes_retest(h, poses7, query_xyzi, query_offsets, n_frames, first_node, voi_max_range, keep_out, ptr_kind, false);
+}
+int erasor_process_nodes_retest_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
+                                      int first_node, double voi_max_range, uint8_t* keep_out, int ptr_kind) {
+    return process_nodes_retest(h, poses7, query_xyzi, query_offsets, n_frames, first_node, voi_max_range, keep_out, ptr_kind, true);
 }
 
 extern "C++" {   // (a template and overloads: C++ linkage)
@@ -1792,6 +1830,8 @@ int erasor_map_append_inserts(erasor_map_t m, erasor_handle_t h) {
     CK(grow_points(m->d_ins, m->n_ins, m->n_ins + n, h->stream));
     if (n) CK(cudaMemcpyAsync(m->d_ins.as<float4>() + m->n_ins, h->d_ins_call.p(), sizeof(float4) * n, cudaMemcpyDeviceToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
+    m->ins_node_off.pop_back();                // (the old end: the first appended node's start)
+    for (size_t f = 0; f < h->ins_call_off.size(); ++f) m->ins_node_off.push_back(m->n_ins + h->ins_call_off[f]);
     m->n_ins += n;
     return ERASOR_OK;
 }
@@ -1806,6 +1846,56 @@ int erasor_map_inserts(erasor_map_t m, const float** d_xyzi, size_t* n) {
 int erasor_map_clear_inserts(erasor_map_t m) {
     if (!m) return ERASOR_E_INVALID;
     m->n_ins = 0;
+    m->ins_node_off.assign(1, 0);
+    return ERASOR_OK;
+}
+
+// The re-test map (DESIGN.md section 8.4.1): m's kept points compacted in map order on the device, then m's insert store, with
+// kMapPad zeroed points of slack as erasor_map_create leaves them; one read of the kept count sizes it.  Node k of the store sees the
+// prefix of the map that holds m's kept points and the inserts of the nodes before k.
+int erasor_map_create_retest(erasor_map_t m, erasor_map_t* out) {
+    if (!m || !out) { g_create_error = "null argument"; return ERASOR_E_INVALID; }
+    *out = nullptr;
+    erasor_map_ctx* r = new erasor_map_ctx();
+    r->device = m->device;
+    cudaError_t e;
+    auto fail = [&](const char* what, cudaError_t ce) { g_create_error = std::string(what) + ": " + cudaGetErrorString(ce); erasor_map_destroy(r); return ERASOR_E_CUDA; };
+    if ((e = cudaSetDevice(m->device)) != cudaSuccess) return fail("cudaSetDevice", e);
+    if ((e = cudaStreamCreateWithFlags(&r->st, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
+    if ((e = cudaStreamSynchronize(m->st)) != cudaSuccess) return fail("cudaStreamSynchronize", e);
+    const size_t tiles = compact_tiles(m->n);
+    DeviceBuffer d_tiles;                      // per tile its kept count and its offset, then the kept total
+    if ((e = d_tiles.allocate(sizeof(uint32_t) * (2 * tiles + 1))) != cudaSuccess) return fail("cudaMalloc", e);
+    uint32_t* tile_cnt = d_tiles.as<uint32_t>();
+    uint32_t* tile_off = tile_cnt + tiles;
+    uint32_t* d_total = tile_off + tiles;
+    if ((e = launch_compact_count(r->st, m->d_keep.as<const uint8_t>(), m->n, tile_cnt, tile_off, d_total)) != cudaSuccess) return fail("k_compact_count", e);
+    uint32_t n_kept = 0;
+    if ((e = cudaMemcpyAsync(&n_kept, d_total, sizeof(uint32_t), cudaMemcpyDeviceToHost, r->st)) != cudaSuccess) return fail("cudaMemcpy", e);
+    if ((e = cudaStreamSynchronize(r->st)) != cudaSuccess) return fail("cudaStreamSynchronize", e);
+    const size_t n = (size_t)n_kept + m->n_ins;
+    if (n >= 0xFFFFFFF0ull) { g_create_error = "re-test map beyond 2^32 points"; erasor_map_destroy(r); return ERASOR_E_INVALID; }
+    r->n = n;
+    if ((e = r->d_pts.allocate(sizeof(float4) * (n + kMapPad))) != cudaSuccess) return fail("cudaMalloc", e);
+    if ((e = r->d_keep.allocate(std::max<size_t>(n, 1))) != cudaSuccess) return fail("cudaMalloc", e);
+    if ((e = launch_compact_scatter(r->st, m->d_pts.as<const float4>(), m->d_keep.as<const uint8_t>(), m->n, tile_off, r->d_pts.as<float4>())) != cudaSuccess)
+        return fail("k_compact_scatter", e);
+    if (m->n_ins && (e = cudaMemcpyAsync(r->d_pts.as<float4>() + n_kept, m->d_ins.p(), sizeof(float4) * m->n_ins, cudaMemcpyDeviceToDevice, r->st)) != cudaSuccess)
+        return fail("cudaMemcpy", e);
+    if ((e = cudaMemsetAsync(r->d_pts.as<float4>() + n, 0, sizeof(float4) * kMapPad, r->st)) != cudaSuccess) return fail("cudaMemset", e);
+    if (n && (e = cudaMemsetAsync(r->d_keep.p(), 1, n, r->st)) != cudaSuccess) return fail("cudaMemset", e);
+    if ((e = cudaStreamSynchronize(r->st)) != cudaSuccess) return fail("cudaStreamSynchronize", e);
+    r->retest = true;
+    r->extents.resize(m->ins_node_off.size() - 1);
+    for (size_t k = 0; k < r->extents.size(); ++k) r->extents[k] = n_kept + m->ins_node_off[k];
+    *out = r;
+    return ERASOR_OK;
+}
+
+int erasor_map_retest_extents(erasor_map_t m, size_t* n_nodes, uint64_t* extents) {
+    if (!m || !n_nodes || !m->retest) return ERASOR_E_INVALID;
+    *n_nodes = m->extents.size();
+    if (extents) std::copy(m->extents.begin(), m->extents.end(), extents);
     return ERASOR_OK;
 }
 

@@ -2568,4 +2568,93 @@ cudaError_t launch_fill_u8(cudaStream_t st, uint8_t* p, size_t n, uint8_t v) {
     return cudaGetLastError();
 }
 
+// ---- the re-test map's order-preserving compaction of pts[keep != 0] (DESIGN.md section 8.4.1) ---------------------------------
+// One CTA per tile of kCompactTile points, walked in kCompactTile / 256 rounds of 256 consecutive points: the tiles' kept counts,
+// one exclusive scan over them, then every tile writes its kept points at its offset, round by round in point order.
+constexpr int kCompactThreads = 256;
+
+__global__ void __launch_bounds__(kCompactThreads) k_compact_count(const uint8_t* __restrict__ keep, size_t n, uint32_t* __restrict__ tile_cnt) {
+    __shared__ uint32_t s_w[kCompactThreads / 32];
+    const size_t base = (size_t)blockIdx.x * kCompactTile;
+    uint32_t c = 0;
+    for (uint32_t i = threadIdx.x; i < kCompactTile; i += kCompactThreads)
+        c += (base + i < n && keep[base + i] != 0) ? 1u : 0u;
+    for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(FULL_MASK, c, o);
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = c;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t t = 0;
+        for (int w = 0; w < kCompactThreads / 32; ++w) t += s_w[w];
+        tile_cnt[blockIdx.x] = t;
+    }
+}
+
+// one CTA: exclusive prefix of the tile counts in 1024-entry steps with a running carry; *total = the kept points
+__global__ void __launch_bounds__(1024) k_compact_scan(const uint32_t* __restrict__ tile_cnt, uint32_t n_tiles, uint32_t* __restrict__ tile_off,
+                                                       uint32_t* __restrict__ total) {
+    __shared__ uint32_t s_w[32];
+    __shared__ uint32_t s_carry;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) s_carry = 0u;
+    __syncthreads();
+    for (uint32_t b = 0; b < n_tiles; b += 1024u) {
+        const uint32_t i = b + (uint32_t)tid;
+        const uint32_t c = i < n_tiles ? tile_cnt[i] : 0u;
+        uint32_t incl = c;
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL_MASK, incl, o); if (lane >= o) incl += v; }
+        if (lane == 31) s_w[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            uint32_t w = s_w[lane], wi = w;
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL_MASK, wi, o); if (lane >= o) wi += v; }
+            s_w[lane] = wi - w;                                  // exclusive prefix of the warps' sums
+        }
+        __syncthreads();
+        const uint32_t carry = s_carry;
+        if (i < n_tiles) tile_off[i] = carry + s_w[warp] + incl - c;
+        __syncthreads();                                         // every thread has read s_carry and s_w
+        if (tid == 1023) s_carry = carry + s_w[warp] + incl;
+        __syncthreads();
+    }
+    if (tid == 0) *total = s_carry;
+}
+
+__global__ void __launch_bounds__(kCompactThreads) k_compact_scatter(const float4* __restrict__ pts, const uint8_t* __restrict__ keep, size_t n,
+                                                                     const uint32_t* __restrict__ tile_off, float4* __restrict__ out) {
+    __shared__ uint32_t s_w[kCompactThreads / 32 + 1];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const size_t base = (size_t)blockIdx.x * kCompactTile;
+    uint32_t at = tile_off[blockIdx.x];
+    for (uint32_t r = 0; r < kCompactTile; r += kCompactThreads) {
+        const size_t i = base + r + (uint32_t)tid;
+        const bool in = i < n && keep[i] != 0;
+        const unsigned bal = __ballot_sync(FULL_MASK, in);
+        if (lane == 0) s_w[warp] = __popc(bal);
+        __syncthreads();
+        if (tid == 0) {
+            uint32_t t = 0;
+            for (int w = 0; w < kCompactThreads / 32; ++w) { const uint32_t c = s_w[w]; s_w[w] = t; t += c; }
+            s_w[kCompactThreads / 32] = t;
+        }
+        __syncthreads();
+        if (in) out[at + s_w[warp] + __popc(bal & ((1u << lane) - 1u))] = pts[i];
+        at += s_w[kCompactThreads / 32];
+        __syncthreads();                                         // s_w is rewritten by the next round
+    }
+}
+
+cudaError_t launch_compact_count(cudaStream_t st, const uint8_t* keep, size_t n, uint32_t* tile_cnt, uint32_t* tile_off, uint32_t* total) {
+    const size_t tiles = compact_tiles(n);
+    if (tiles) k_compact_count<<<(unsigned)tiles, kCompactThreads, 0, st>>>(keep, n, tile_cnt);
+    k_compact_scan<<<1, 1024, 0, st>>>(tile_cnt, (uint32_t)tiles, tile_off, total);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_compact_scatter(cudaStream_t st, const float4* pts, const uint8_t* keep, size_t n, const uint32_t* tile_off, float4* out) {
+    const size_t tiles = compact_tiles(n);
+    if (tiles == 0) return cudaSuccess;
+    k_compact_scatter<<<(unsigned)tiles, kCompactThreads, 0, st>>>(pts, keep, n, tile_off, out);
+    return cudaGetLastError();
+}
+
 }  // namespace erasor

@@ -97,6 +97,13 @@ cudaError_t launch_k5(cudaStream_t st, int B, int version, int skip_voxelize, co
 
 cudaError_t launch_fold_keep(cudaStream_t st, const uint8_t* keep, const uint32_t* voi_index, size_t n, uint8_t* global_keep, size_t n_global);
 cudaError_t launch_fill_u8(cudaStream_t st, uint8_t* p, size_t n, uint8_t v);
+// the re-test map (erasor_map_create_retest): order-preserving compaction of pts[keep != 0], n < 2^32, in tiles of kCompactTile
+// points.  launch_compact_count: the tiles' kept counts (tile_cnt), their exclusive prefix (tile_off) and the kept total (*total),
+// compact_tiles(n) entries each; launch_compact_scatter then writes the kept points to out[0, *total) in point order.
+constexpr uint32_t kCompactTile = 4096;
+inline size_t compact_tiles(size_t n) { return (n + kCompactTile - 1) / kCompactTile; }
+cudaError_t launch_compact_count(cudaStream_t st, const uint8_t* keep, size_t n, uint32_t* tile_cnt, uint32_t* tile_off, uint32_t* total);
+cudaError_t launch_compact_scatter(cudaStream_t st, const float4* pts, const uint8_t* keep, size_t n, const uint32_t* tile_off, float4* out);
 // exchange step of the frame-sharded job: pack the keep bytes into bits, AND the all-gathered words of every rank, unpack
 cudaError_t launch_pack_keep_bits(cudaStream_t st, const uint8_t* keep, size_t n, uint32_t* words);
 cudaError_t launch_and_unpack_keep(cudaStream_t st, const uint32_t* gathered, int n_ranks, size_t n, uint8_t* keep);

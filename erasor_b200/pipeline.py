@@ -50,30 +50,40 @@ def processed_nodes(nodes: Iterable[Node], removal_interval: int) -> list:
 
 
 def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep, batch: int = 20, save_voxel_size: Optional[float] = None,
-                          prepare: Optional[Callable] = None, inserts: bool = False) -> dict:
+                          prepare: Optional[Callable] = None, inserts: bool = False, retest: bool = False) -> dict:
     """The frame-independent twin of run_offline: every node callback_node would process is tested against the same initial map
     (node mode, erasor_process_nodes), in batches of `batch` nodes, each batch's raw scans voxelised at query_voxel_size and moved
     to the body frame on the device in one submission (erasor_voxelize_batch); then save_static_map of the kept map.  prepare
     (optional) replaces the device query preparation: prepare(raw_xyzi, raw_offsets) -> (queries, query_offsets).  inserts: also
     put back the query points each node's static estimate holds (node-mode inserts), saved with the kept map in node order.
-    Returns run_offline's dict plus "keep", the map's keep mask.  Needs a CUDA device."""
+    retest (needs inserts): a second pass over the same batches against the re-test map M2 = kept map ++ every node's inserts
+    (DESIGN.md section 8.4.1), node j seeing the kept map and the inserts of the nodes before it; the saved map is then M2 under
+    the second pass's mask.  Returns run_offline's dict plus "keep", the map's keep mask after the first pass, and with retest
+    "retest_keep" (M2's mask) and "retest_size" (M2's points).  Needs a CUDA device."""
     from . import capi
     if up.is_large_scale:
         raise ValueError("node mode has no large-scale windowing: use run_offline")
+    if retest and not inserts:
+        raise ValueError("the re-test pass tests the first pass's inserts: retest needs inserts=True")
     nodes = list(nodes)
     sel = processed_nodes(nodes, up.removal_interval)
     m = capi.Map(np.ascontiguousarray(initial_map, dtype=np.float32))
     h = capi.Handle(ep.replace(version=up.version))       # /erasor/version as the updater reads it (OfflineMapUpdater.cpp:81)
-    try:
-        h.attach_map(m)
-        h.set_node_inserts(inserts)
-        l2b = np.asarray(up.lidar2body, dtype=np.float64)
+    r = None
+    l2b = np.asarray(up.lidar2body, dtype=np.float64)
+    leaf = up.map_voxel_size if save_voxel_size is None else save_voxel_size
+
+    def batches():
         for b0 in range(0, len(sel), int(batch)):
             chunk = sel[b0:b0 + int(batch)]
             poses = np.stack([np.asarray(o, dtype=np.float64).reshape(7) for _, o, _ in chunk])
             scans = [np.ascontiguousarray(c, dtype=np.float32).reshape(-1, 4) for _, _, c in chunk]
-            off = np.cumsum([0] + [len(s) for s in scans]).astype(np.uint64)
-            raw = np.concatenate(scans)
+            yield b0, poses, np.concatenate(scans), np.cumsum([0] + [len(s) for s in scans]).astype(np.uint64)
+
+    try:
+        h.attach_map(m)
+        h.set_node_inserts(inserts)
+        for _, poses, raw, off in batches():
             if prepare is None:
                 h.process_scans(poses, raw, off, up.query_voxel_size, l2b, voi_max_range=up.max_range)
             else:
@@ -82,11 +92,28 @@ def run_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep
             if inserts:
                 m.append_inserts(h)
         keep = m.get_keep()
-        static_map = h.save_static_map(m, up.map_voxel_size if save_voxel_size is None else save_voxel_size)
+        res = {"nodes": len(nodes), "processed_scans": len(sel), "keep": keep}
+        if retest:
+            r = m.create_retest()
+            h.set_node_inserts(False)
+            h.attach_map(r)
+            for b0, poses, raw, off in batches():
+                if prepare is None:
+                    h.process_scans_retest(poses, raw, off, up.query_voxel_size, l2b, b0, voi_max_range=up.max_range)
+                else:
+                    q, qo = prepare(raw, off)
+                    h.process_nodes_retest(poses, q, qo, b0, voi_max_range=up.max_range)
+            res["retest_keep"] = r.get_keep()
+            res["retest_size"] = r.size
+            res["static_map"] = h.save_static_map(r, leaf)
+        else:
+            res["static_map"] = h.save_static_map(m, leaf)
     finally:
         h.close()
+        if r is not None:
+            r.close()
         m.close()
-    return {"static_map": static_map, "nodes": len(nodes), "processed_scans": len(sel), "keep": keep}
+    return res
 
 
 def sweep_frame_independent(nodes: Iterable[Node], initial_map: np.ndarray, up, ep, variants, gt: Optional[np.ndarray] = None, batch: int = 20,
@@ -180,11 +207,12 @@ def _sweep_rows(nodes, initial_map, up, ep, variants, fields, gt, batch, save_vo
 
 def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, make_updater: Optional[Callable] = None,
                  map_leafsize: Optional[float] = None, out_dir: Optional[str] = None, frame_independent: bool = False,
-                 inserts: bool = False, pcd_mode: str = "ascii") -> dict:
+                 inserts: bool = False, pcd_mode: str = "ascii", retest: bool = False) -> dict:
     """mapgen -> updater -> evaluation on one node list.  GT for PR/RR = the naive map itself (it carries the labels), which is
     how the reference scores a run (analysis_runner.py compares <seq>_..._original / voxelised map with the result).
     frame_independent runs node mode (run_frame_independent) on the naive map instead of the sequential updater; inserts (node
-    mode only) puts each node's inserted query points back into its static map.  pcd_mode: the DATA mode of the two files written
+    mode only) puts each node's inserted query points back into its static map, and retest (with inserts) tests them again in a
+    second node-mode pass (run_frame_independent).  pcd_mode: the DATA mode of the two files written
     to out_dir ("ascii", as the reference writes them, "binary" or "binary_compressed"; the binary modes need the device writer,
     so an injected updater takes only "ascii")."""
     from . import capi
@@ -198,10 +226,10 @@ def run_sequence(nodes, up, ep, voxelize: Optional[mapgen.Voxelizer] = None, mak
     if frame_independent:
         if make_updater is not None:
             raise ValueError("node mode runs on the device: make_updater does not apply")
-        res = run_frame_independent(nodes, naive, up, ep, inserts=inserts)
+        res = run_frame_independent(nodes, naive, up, ep, inserts=inserts, retest=retest)
     else:
-        if inserts:
-            raise ValueError("inserts are a node-mode option: the sequential updater always inserts")
+        if inserts or retest:
+            raise ValueError("inserts and retest are node-mode options: the sequential updater always inserts and re-tests")
         res = run_offline(nodes, naive, up, ep, make_updater=make_updater)
     res["naive_map"] = naive
     if make_updater is None:            # the device updater ran: score on the device too (same counts, same dict)
@@ -246,6 +274,7 @@ def read_bag_nodes(bag_path: str, topic: str = "/node/combined/optimized", keep_
 
 def run_bag(bag: str, config_yaml: str, out_dir: Optional[str] = None, frame_independent: bool = False, **kw) -> dict:
     """A reference bag + a reference config/*.yaml -> naive map, static map and PR/RR: run_sequence on the bag's nodes, with the
-    sequential updater or, with frame_independent, node mode (inserts=True in kw: with node-mode inserts)."""
+    sequential updater or, with frame_independent, node mode (inserts=True in kw: with node-mode inserts; retest=True as well:
+    with their re-test pass)."""
     ep, up = params.load_yaml(config_yaml)
     return run_sequence(read_bag_nodes(bag), up, ep, out_dir=out_dir, frame_independent=frame_independent, **kw)

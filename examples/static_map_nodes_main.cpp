@@ -8,6 +8,8 @@
 // With a ROS bag of erasor/node messages instead of <data_dir> (a path ending in .bag), the map is the yaml's initial_map_path, the
 // poses are the bag's doubles, and each batch's clouds are decoded from the bag on the device in one call (NodeBag::load_device).
 // inserts = 1 turns node-mode inserts on: the query points each node's static estimate puts back into the map are saved with it.
+// inserts = 2 also re-tests them (DESIGN.md section 8.4.1): a second pass over the same batches against the kept map followed by
+// every node's inserts, each node seeing the inserts of the nodes before it; the re-test map under that pass's mask is saved.
 //   usage: static_map_nodes_main <config.yaml> <data_dir> [init_idx] [batch] [inserts]
 //          static_map_nodes_main <config.yaml> <file.bag> [init_idx] [batch] [inserts]
 #include <cstdio>
@@ -71,7 +73,9 @@ int main(int argc, char** argv) {
         const std::string data_dir = argv[2];
         const int init_idx = argc > 3 ? std::atoi(argv[3]) : 0;
         const int batch = argc > 4 ? std::max(1, std::atoi(argv[4])) : 20;
-        const bool inserts = argc > 5 && std::atoi(argv[5]) != 0;
+        const int inserts_arg = argc > 5 ? std::atoi(argv[5]) : 0;
+        if (inserts_arg < 0 || inserts_arg > 2) throw std::invalid_argument("inserts must be 0 (off), 1 (on) or 2 (on, with the re-test pass)");
+        const bool inserts = inserts_arg != 0, retest = inserts_arg == 2;
         if (cfg.updater.is_large_scale) throw std::invalid_argument("node mode has no large-scale windowing: use offline_map_updater_main");
         if (cfg.updater.removal_interval < 1) throw std::invalid_argument("removal_interval must be >= 1");
         erasor_params_t ep = cfg.erasor;
@@ -91,12 +95,16 @@ int main(int argc, char** argv) {
             for (size_t i = init_idx > 0 ? (size_t)init_idx : 0; i < bag.size(); ++i)
                 if ((i - init_idx + 1) % cfg.updater.removal_interval == 0) sel.push_back(i);
             DeviceBuffer raw;
-            for (size_t b0 = 0; b0 < sel.size(); b0 += (size_t)batch) {
-                const std::vector<uint64_t> nodes(sel.begin() + b0, sel.begin() + std::min(sel.size(), b0 + (size_t)batch));
-                std::vector<std::array<double, 7>> bp;
-                for (uint64_t i : nodes) bp.push_back(bag.node(i).odom);
-                const std::vector<uint64_t> off = bag.load_device(nodes, [&](size_t m) { return raw.reserve(m); });
-                erasor.process_scans(bp, raw.data(), off, cfg.updater.query_voxel_size, l2b, cfg.updater.max_range, ERASOR_PTR_DEVICE);
+            for (int pass = 0; pass < (retest ? 2 : 1); ++pass) {
+                if (pass == 1) erasor.begin_retest();
+                for (size_t b0 = 0; b0 < sel.size(); b0 += (size_t)batch) {
+                    const std::vector<uint64_t> nodes(sel.begin() + b0, sel.begin() + std::min(sel.size(), b0 + (size_t)batch));
+                    std::vector<std::array<double, 7>> bp;
+                    for (uint64_t i : nodes) bp.push_back(bag.node(i).odom);
+                    const std::vector<uint64_t> off = bag.load_device(nodes, [&](size_t m) { return raw.reserve(m); });
+                    if (pass == 0) erasor.process_scans(bp, raw.data(), off, cfg.updater.query_voxel_size, l2b, cfg.updater.max_range, ERASOR_PTR_DEVICE);
+                    else erasor.process_scans_retest(bp, raw.data(), off, (int)b0, cfg.updater.query_voxel_size, l2b, cfg.updater.max_range, ERASOR_PTR_DEVICE);
+                }
             }
             const ERASOR::DeviceClouds saved = erasor.save_static_map(0.2f);
             const std::string target = cfg.save_path + "/" + cfg.data_name + "_result.pcd";
@@ -111,15 +119,19 @@ int main(int argc, char** argv) {
             if ((i - init_idx + 1) % cfg.updater.removal_interval == 0) sel.push_back(i);
         auto scan_path = [&](int i) { char name[64]; std::snprintf(name, sizeof(name), "/pcds/%06d.pcd", i); return data_dir + name; };
         DeviceBuffer raw;                                               // a batch's raw scans, back to back
-        for (size_t b0 = 0; b0 < sel.size(); b0 += (size_t)batch) {
-            const size_t nb = std::min(sel.size() - b0, (size_t)batch);
-            std::vector<std::array<double, 7>> bp(nb);
-            std::vector<uint64_t> off(nb + 1, 0);
-            for (size_t j = 0; j < nb; ++j) {                           // each scan read on the device behind the previous one
-                bp[j] = poses[sel[b0 + j]];
-                off[j + 1] = off[j] + codec.load_device(scan_path(sel[b0 + j]), [&](size_t m) { return raw.reserve(off[j] + m, off[j]) + 4 * off[j]; });
+        for (int pass = 0; pass < (retest ? 2 : 1); ++pass) {
+            if (pass == 1) erasor.begin_retest();                       // the re-test pass reads the same scans again
+            for (size_t b0 = 0; b0 < sel.size(); b0 += (size_t)batch) {
+                const size_t nb = std::min(sel.size() - b0, (size_t)batch);
+                std::vector<std::array<double, 7>> bp(nb);
+                std::vector<uint64_t> off(nb + 1, 0);
+                for (size_t j = 0; j < nb; ++j) {                       // each scan read on the device behind the previous one
+                    bp[j] = poses[sel[b0 + j]];
+                    off[j + 1] = off[j] + codec.load_device(scan_path(sel[b0 + j]), [&](size_t m) { return raw.reserve(off[j] + m, off[j]) + 4 * off[j]; });
+                }
+                if (pass == 0) erasor.process_scans(bp, raw.data(), off, cfg.updater.query_voxel_size, l2b, cfg.updater.max_range, ERASOR_PTR_DEVICE);
+                else erasor.process_scans_retest(bp, raw.data(), off, (int)b0, cfg.updater.query_voxel_size, l2b, cfg.updater.max_range, ERASOR_PTR_DEVICE);
             }
-            erasor.process_scans(bp, raw.data(), off, cfg.updater.query_voxel_size, l2b, cfg.updater.max_range, ERASOR_PTR_DEVICE);
         }
         const ERASOR::DeviceClouds saved = erasor.save_static_map(0.2f);
         const std::string target = cfg.save_path + "/" + cfg.data_name + "_result.pcd";

@@ -198,6 +198,40 @@ public:
     // static estimate puts back into the map to the map's store, and save_static_map voxelises them with the kept map.
     void set_node_inserts(bool enable) { check(erasor_set_node_inserts(h_, enable ? 1 : 0)); inserts_ = enable; }
     void clear_node_inserts() { if (map_ && erasor_map_clear_inserts(map_) != ERASOR_OK) throw std::runtime_error("ERASOR: erasor_map_clear_inserts"); }
+    // Node-mode re-test (DESIGN.md section 8.4.1), after a first pass with inserts on: the held map becomes its re-test map -- the
+    // kept points, then every node's inserts in node order, keep all ones -- and inserts go off.  process_nodes_retest /
+    // process_scans_retest then run the same nodes again, node k seeing the kept points and the inserts of the nodes before it;
+    // save_static_map saves the re-test map under its keep mask.  Returns the store's node count.
+    size_t begin_retest() {
+        if (!map_) throw std::logic_error("ERASOR: load_global_map first");
+        check(erasor_synchronize(h_));
+        erasor_map_t r = nullptr;
+        if (erasor_map_create_retest(map_, &r) != ERASOR_OK) throw std::runtime_error(std::string("ERASOR: ") + erasor_last_error(nullptr));
+        set_node_inserts(false);
+        erasor_attach_map(h_, nullptr);
+        erasor_map_destroy(map_);
+        map_ = r;
+        check(erasor_attach_map(h_, map_));
+        size_t n = 0;
+        erasor_map_retest_extents(map_, &n, nullptr);
+        return n;
+    }
+    // process_nodes for the re-test pass: node f of the batch is store node first_node + f
+    std::vector<uint8_t> process_nodes_retest(const std::vector<std::array<double, 7>>& poses, const std::vector<PointCloud>& query_vois,
+                                              int first_node, double voi_max_range = 0.0) {
+        if (!map_) throw std::logic_error("ERASOR: load_global_map first");
+        if (poses.size() != query_vois.size() || poses.empty()) throw std::invalid_argument("ERASOR: one pose per query VoI");
+        const size_t F = poses.size();
+        std::vector<uint64_t> qo(F + 1, 0);
+        for (size_t f = 0; f < F; ++f) qo[f + 1] = qo[f] + query_vois[f].size();
+        PointCloud q(qo[F]);
+        for (size_t f = 0; f < F; ++f) std::copy(query_vois[f].begin(), query_vois[f].end(), q.begin() + static_cast<std::ptrdiff_t>(qo[f]));
+        std::vector<uint8_t> keep(std::max<size_t>(erasor_map_size(map_), 1));
+        check(erasor_process_nodes_retest(h_, poses[0].data(), reinterpret_cast<const float*>(q.data()), qo.data(), static_cast<int>(F), first_node,
+                                          voi_max_range, keep.data(), ERASOR_PTR_HOST));
+        keep.resize(erasor_map_size(map_));
+        return keep;
+    }
     // the same, from a map already in device memory (16-byte aligned float4 per point), e.g. read by PcdCodec::load_device
     void load_global_map_device(const float* d_map_xyzi, size_t n) {
         if (map_) { erasor_attach_map(h_, nullptr); erasor_map_destroy(map_); map_ = nullptr; }
@@ -252,6 +286,17 @@ public:
         for (size_t f = 0; f < raw_scans.size(); ++f) std::copy(raw_scans[f].begin(), raw_scans[f].end(), raw.begin() + static_cast<std::ptrdiff_t>(off[f]));
         process_scans(poses, reinterpret_cast<const float*>(raw.data()), off, query_voxel_size, lidar2body, voi_max_range, ERASOR_PTR_HOST);
         return static_mask();
+    }
+    // process_scans for the re-test pass (after begin_retest): the scans are voxelised again -- the same queries as the first pass --
+    // and node f of the batch is store node first_node + f
+    void process_scans_retest(const std::vector<std::array<double, 7>>& poses, const float* raw_xyzi, const std::vector<uint64_t>& raw_offsets,
+                              int first_node, double query_voxel_size, const std::array<double, 7>& lidar2body, double voi_max_range = 0.0,
+                              int ptr_kind = ERASOR_PTR_HOST) {
+        if (!map_) throw std::logic_error("ERASOR: load_global_map first");
+        if (poses.empty() || poses.size() + 1 != raw_offsets.size()) throw std::invalid_argument("ERASOR: one pose per raw scan");
+        const DeviceClouds q = voxelize_batch(raw_xyzi, raw_offsets, static_cast<float>(query_voxel_size), nullptr, lidar2body.data(), ptr_kind);
+        check(erasor_process_nodes_retest(h_, poses[0].data(), q.d_xyzi, q.offsets.data(), static_cast<int>(poses.size()), first_node, voi_max_range,
+                                          nullptr, ERASOR_PTR_DEVICE));
     }
     // save_static_map of node mode (OfflineMapUpdater.cpp:174-196 without the file): the map load_global_map holds, under its
     // current keep mask, followed by the map's insert store (empty unless inserts are on), voxelised at voxel_size -- one cloud,

@@ -304,13 +304,33 @@ int erasor_set_node_inserts(erasor_handle_t h, int enable);
  * device memory valid until the handle's next submission; offsets (HOST, n_frames + 1): node f is [offsets[f], offsets[f+1]) */
 int erasor_get_node_inserts(erasor_handle_t h, const float** d_xyzi, uint64_t* offsets);
 /* The map's insert store: erasor_map_append_inserts appends h's last call (synchronous); callers append in node order -- lanes
- * sharing a map append after their own erasor_wait.  erasor_map_inserts: device pointer and point count; clear empties it. */
+ * sharing a map append after their own erasor_wait.  The store also records where each appended node's inserts start (the
+ * re-test map's extents below).  erasor_map_inserts: device pointer and point count; clear empties it. */
 int erasor_map_append_inserts(erasor_map_t m, erasor_handle_t h);
 int erasor_map_inserts(erasor_map_t m, const float** d_xyzi, size_t* n);
 int erasor_map_clear_inserts(erasor_map_t m);
 /* node mode's save_static_map: voxelize_preserving_labels(map[keep] ++ the map's inserts, leaf) through erasor_voxelize_batch
  * (its output rules and errors); with an empty store, the kept map alone.  Waits for h; *d_out valid until h's next voxelize. */
 int erasor_save_node_map(erasor_handle_t h, erasor_map_t m, float leaf, const float** d_out, size_t* n_out);
+
+/* ---- node-mode re-test: the inserts of every node tested again by the nodes after it (DESIGN.md section 8.4.1) ---- */
+/* The re-test map of a node-mode job (DESIGN.md section 8.4.1): m's kept points in map order, then m's insert store in node
+ * order, on m's device; keep all ones, empty store.  Node k of the store (k = 0 .. n_nodes-1) sees the prefix
+ * [0, extent[k]), extent[k] = n_kept + store offset of node k.  m is not changed.  Synchronous (wait for the handles that write
+ * m first).  Errors as erasor_map_create (erasor_last_error(NULL)); ERASOR_E_INVALID for a result of 2^32 points or more. */
+int erasor_map_create_retest(erasor_map_t m, erasor_map_t* out);
+/* n_nodes of a re-test map, and (nullable, n_nodes entries) the extents; ERASOR_E_INVALID for a map not made by the call above */
+int erasor_map_retest_extents(erasor_map_t m, size_t* n_nodes, uint64_t* extents);
+/* erasor_process_nodes against an attached re-test map: node f of the call is store node first_node + f and sees only its
+ * extent.  Same poses / queries / ptr_kind / voi_max_range / keep_out / sub-batch rules as erasor_process_nodes; no frame_keep.
+ * The map's keep mask &= the verdicts on the points each node sees.  Packed x y z queries (ERASOR_PTR_QUERY_XYZ) are allowed:
+ * the pass has no inserts.  ERASOR_E_INVALID: the attached map is not a re-test map, first_node < 0 or first_node + n_frames >
+ * n_nodes, node inserts on for h; ERASOR_E_STATE: no map attached, a submission pending.  A re-test map attached to
+ * erasor_process_nodes or to the sweeps is a plain map (every point visible to every node). */
+int erasor_process_nodes_retest(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets,
+                                int n_frames, int first_node, double voi_max_range, uint8_t* keep_out, int ptr_kind);
+int erasor_process_nodes_retest_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets,
+                                      int n_frames, int first_node, double voi_max_range, uint8_t* keep_out, int ptr_kind);
 
 /* erasor_utils::voxelize_preserving_labels (erasor_utils.cpp:80-114) of n_clouds clouds in one submission, each on its own
  * pcl::VoxelGrid, optionally followed by one pcl::transformPointCloud.  Cloud c is xyzi[offsets[c] .. offsets[c+1]) (offsets: HOST,

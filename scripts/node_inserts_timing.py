@@ -1,13 +1,16 @@
-"""Cost and quality of node-mode inserts (DESIGN.md section 8.4) on the bench's seq-05 twin (20 nodes, one resident map).
+"""Cost and quality of node-mode inserts (DESIGN.md section 8.4) and of their re-test pass (section 8.4.1) on the bench's seq-05
+twin (20 nodes, one resident map).
 
   check    first, for version 3 with and without skip_voxelize: every node's inserts and offsets of one 20-node call against the
            oracle model (tests/node_inserts_model.py), bit for bit
-  timing   node-mode scans/s with inserts off and on, the same workload (device-resident queries, asynchronous submissions dealt
+  timing   node-mode scans/s with inserts off, on (pass 1) and of the re-test pass (pass 2, erasor_process_nodes_retest over
+           the re-test map of pass 1's 20 nodes), the same workload (device-resident queries, asynchronous submissions dealt
            round-robin over the lanes as bench.py does), one lane and four lanes; the arms alternate within every repetition and
-           each arm has its own handles, so both replay captured graphs
+           each arm has its own handles, so all replay captured graphs; and the re-test map's build time (erasor_map_create_retest)
   quality  NN-matched PR/RR (erasor_b200/evaluate.py, GT = the labelled initial map) of node mode's final map without inserts
            (map[keep], as bench.py scores it) and with them (map[keep] ++ every node's inserts), for the bench preset and the
-           configs.3_seqs_00_01_02_07 presets, next to the sequential updater on the same twin (161 nodes, every 8th processed)
+           configs.3_seqs_00_01_02_07 presets, and of the re-test pass's final map (M2[keep2]: the kept map and every node's
+           inserts under pass 2's mask), next to the sequential updater on the same twin (161 nodes, every 8th processed)
 Prints one JSON object; the card's name and power limit are read in the same run.
   usage: python scripts/node_inserts_timing.py [--reps 7] [--steps 20]"""
 import argparse
@@ -49,38 +52,72 @@ def check(p, map_world, poses, qs, qo, dq):
     return int(ref_off[-1])
 
 
+def pass1_map(p, map_world, poses, qo, dq):
+    """the resident map after pass 1 with inserts on (all nodes in one call), its store filled"""
+    m, h = capi.Map(map_world), capi.Handle(p)
+    h.attach_map(m)
+    h.set_node_inserts(True)
+    h.process_nodes_ptr(poses, dq.data_ptr(), qo, 0.0, 0, 0, capi.PTR_DEVICE)
+    m.append_inserts(h)
+    h.close()
+    return m
+
+
+def retest_build(p, map_world, poses, qo, dq, reps):
+    """erasor_map_create_retest's wall time (synchronous: compaction, the kept-count read, the store copy) on pass 1's map"""
+    m = pass1_map(p, map_world, poses, qo, dq)
+    ms = []
+    for _ in range(reps + 1):
+        t0 = time.perf_counter()
+        r = m.create_retest()
+        ms.append(1e3 * (time.perf_counter() - t0))
+        size = r.size
+        r.close()
+    out = {"median_ms": round(float(np.median(ms[1:])), 3), "all_ms": [round(x, 3) for x in ms[1:]], "map_points": int(m.size),
+           "kept_points": int(np.count_nonzero(m.get_keep())), "retest_map_points": int(size)}
+    m.close()
+    return out
+
+
 def timing(p, map_world, poses, qo, dq, lanes, reps, steps):
     import torch
     m = capi.Map(map_world)
+    src = pass1_map(p, map_world, poses, qo, dq[0])
+    r = src.create_retest()
     arms = {}
-    for name, on in (("off", False), ("on", True)):
+    for name, on in (("off", False), ("on", True), ("retest", False)):
         hs = [capi.Handle(p) for _ in range(lanes)]
         for h in hs:
-            h.attach_map(m)
+            h.attach_map(r if name == "retest" else m)
             h.set_node_inserts(on)
         arms[name] = hs
     F = len(qo) - 1
 
-    def run(hs, n):
+    def run(name, n):
+        hs = arms[name]
         for i in range(n):
-            hs[i % len(hs)].process_nodes_ptr(poses, dq[i % len(dq)].data_ptr(), qo, 0.0, 0, 0, capi.PTR_DEVICE, asynchronous=True)
+            if name == "retest":                              # (refused while pending: wait first, as process_nodes does inside)
+                hs[i % len(hs)].wait()
+                hs[i % len(hs)].process_nodes_retest_ptr(poses, dq[i % len(dq)].data_ptr(), qo, 0, 0.0, 0, capi.PTR_DEVICE, asynchronous=True)
+            else:
+                hs[i % len(hs)].process_nodes_ptr(poses, dq[i % len(dq)].data_ptr(), qo, 0.0, 0, 0, capi.PTR_DEVICE, asynchronous=True)
         for h in hs:
             h.wait()
 
-    for hs in arms.values():
-        run(hs, 2 * lanes)                                     # warm: buffers, captured graphs
+    for name in arms:
+        run(name, 2 * lanes)                                   # warm: buffers, captured graphs
     out = {k: [] for k in arms}
     for _ in range(reps):
-        for name, hs in arms.items():
+        for name in arms:
             torch.cuda.synchronize()
             t0 = time.perf_counter()
-            run(hs, steps * lanes)
+            run(name, steps * lanes)
             torch.cuda.synchronize()
             out[name].append(steps * lanes * F / (time.perf_counter() - t0))
     for hs in arms.values():
         for h in hs:
             h.close()
-    m.close()
+    r.close(); src.close(); m.close()
     return {k: {"median_scans_per_s": round(float(np.median(v))), "all": [round(x) for x in v]} for k, v in out.items()}
 
 
@@ -91,12 +128,24 @@ def node_quality(p, map_world, poses, qo, dq):
     h.process_nodes_ptr(poses, dq.data_ptr(), qo, 0.0, 0, 0, capi.PTR_DEVICE)
     ins, _ = h.node_inserts()
     keep = m.get_keep().astype(bool)
-    h.close(); m.close()
+    # the re-test pass over the same nodes: M2 = map[keep] ++ inserts, node j seeing the inserts of the nodes before it
+    m.append_inserts(h)
+    r = m.create_retest()
+    h.set_node_inserts(False)
+    h.attach_map(r)
+    h.process_nodes_retest_ptr(poses, dq.data_ptr(), qo, 0, 0.0, 0, capi.PTR_DEVICE)
+    M2 = np.empty((r.size, 4), dtype=np.float32)
+    capi._memcpy_from_device(M2, r.points_ptr)
+    keep2 = r.get_keep().astype(bool)
+    h.close(); r.close(); m.close()
     q = {}
-    for name, est in (("without_inserts", map_world[keep]), ("with_inserts", np.concatenate([map_world[keep], ins]))):
-        r = evaluate.evaluate(map_world, est)
-        q[name] = {"PR": round(r["PR"], 3), "RR": round(r["RR"], 3), "F1": round(r["F1"], 4)}
+    for name, est in (("without_inserts", map_world[keep]), ("with_inserts", np.concatenate([map_world[keep], ins])),
+                      ("with_inserts_retest", M2[keep2])):
+        res = evaluate.evaluate(map_world, est)
+        q[name] = {"PR": round(res["PR"], 3), "RR": round(res["RR"], 3), "F1": round(res["F1"], 4)}
     q["inserted_points"] = int(len(ins))
+    q["retest_rejected_inserts"] = int(np.count_nonzero(~keep2[int(keep.sum()):]))
+    q["retest_rejected_kept_points"] = int(np.count_nonzero(~keep2[:int(keep.sum())]))
     return q
 
 
@@ -130,6 +179,7 @@ def main():
         p = p0.replace(version=3, skip_voxelize=skip)
         key = f"v3_skip_voxelize_{skip}"
         res["checked_inserted_points"][key] = check(p, map_world, poses, qs, qo, dq[0])
+        res.setdefault("retest_map_build", {})[key] = retest_build(p, map_world, poses, qo, dq[0], a.reps)
         for lanes in (1, 4):
             res["timing"][f"{key}_lanes_{lanes}"] = timing(p, map_world, poses, qo, dq, lanes, a.reps, a.steps)
     res["quality"] = {"seq_05 (bench)": node_quality(p0, map_world, poses, qo, dq[0])}
