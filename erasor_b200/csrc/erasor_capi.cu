@@ -97,7 +97,7 @@ struct GeoTables {
 // order of first appearance (geo[0] carries setting 0), each with the Scan Ratio Test fields of every setting -- those of the
 // other geometries switched off (minimum_num_pts -1) -- and the ground-filter groups of its own settings.  An own plan's one
 // geometry is the handle's: K1 bins into the handle's per-batch tables, as in a plain call.  Any other plan bins geometry g into
-// the handle's tune_tabs[g], in the K1 launches of launch_begin (geometries [launch_begin[l], launch_begin[l + 1])).
+// the handle's k1_sweep[g], in the K1 launches of launch_begin (geometries [launch_begin[l], launch_begin[l + 1])).
 struct SweepGeo {
     const GeoTables* t;
     int              launch;                   // the K1 launch that bins it (not own)
@@ -158,13 +158,14 @@ struct erasor_ctx {
     uint64_t        alloc_epoch = 0;
     struct HBuf : DeviceBuffer { explicit HBuf(uint64_t& e) : DeviceBuffer(&e) {} };
     int             B = 0;                     // bins of the handle's geometry (its polar tables: geo_tables[0])
+    // one geometry's K1 outputs, the arrays of its K1GeoTables (sized by ensure_k1_bufs, read through k1_tables)
+    struct K1Bufs { HBuf bin_map, bin_qry, ch_cnt, zmin, zmax, cnt; explicit K1Bufs(uint64_t& e) : bin_map(e), bin_qry(e), ch_cnt(e), zmin(e), zmax(e), cnt(e) {} };
 
     // per-batch buffers
     HBuf d_map_in{alloc_epoch}, d_qry_in{alloc_epoch};       // staging when the caller's clouds are host memory
-    HBuf d_bin_map{alloc_epoch}, d_bin_qry{alloc_epoch};     // uint16 bin id per point
+    K1Bufs k1_own{alloc_epoch};                              // the handle's geometry
     HBuf d_chunks{alloc_epoch}, d_chunk_range{alloc_epoch}, d_frame_off{alloc_epoch};
-    HBuf d_chcnt{alloc_epoch}, d_zmin{alloc_epoch}, d_zmax{alloc_epoch}, d_cnt{alloc_epoch}, d_dst_start{alloc_epoch}, d_status{alloc_epoch},
-         d_action{alloc_epoch}, d_flag_slot{alloc_epoch}, d_nflag{alloc_epoch};
+    HBuf d_dst_start{alloc_epoch}, d_status{alloc_epoch}, d_action{alloc_epoch}, d_flag_slot{alloc_epoch}, d_nflag{alloc_epoch};
     HBuf d_recs{alloc_epoch}, d_nrecs{alloc_epoch}, d_frame_rej{alloc_epoch}, d_frame_rec_base{alloc_epoch}, d_queue{alloc_epoch}, d_bucket{alloc_epoch};
     HBuf d_map_sorted{alloc_epoch}, d_map_src{alloc_epoch}, d_qry_sorted{alloc_epoch}, d_qry_src{alloc_epoch}, d_part{alloc_epoch}, d_scratch{alloc_epoch};
     HBuf d_keep{alloc_epoch}, d_ground{alloc_epoch};
@@ -208,12 +209,10 @@ struct erasor_ctx {
     Step     last;                             // the last mask-mode submission
     int      sweep_V = 0;                      // variants of the last node call when it was a sweep (erasor_get_sweep_stats), else 0
 
-    // the polar tables of every geometry seen, the handle's own first; per geometry of a sweep plan that is not own its batch tables
+    // the polar tables of every geometry seen, the handle's own first; per geometry of a sweep plan that is not own its K1 outputs
     std::vector<std::unique_ptr<GeoTables>> geo_tables;
-    struct TuneTabs { HBuf bin_map, bin_qry, chcnt, zmin, zmax, cnt; explicit TuneTabs(uint64_t& e) : bin_map(e), bin_qry(e), chcnt(e), zmin(e), zmax(e), cnt(e) {} };
-    std::vector<std::unique_ptr<TuneTabs>> tune_tabs;
-    HBuf     d_list_idx32{alloc_epoch}, d_list_cnt32{alloc_epoch};   // the VoI lists of a plan's 32-warp K1 launches (their split
-                                                                      // differs from the 8-warp launches', whose lists are d_list_*)
+    std::vector<std::unique_ptr<K1Bufs>> k1_sweep;
+    HBuf     d_list_idx32{alloc_epoch}, d_list_cnt32{alloc_epoch};   // the VoI lists of a plan's 32-warp K1 launches (k1_lists)
     size_t   smem_optin = 0;                   // sharedMemPerBlockOptin of the device
     bool     tune_unpacked = false;            // ERASOR_B200_TUNE_UNPACKED=1: one geometry per K1 launch (measurement of the packing)
 
@@ -302,7 +301,7 @@ uint32_t choose_chunk(const erasor_ctx* h, const uint64_t* map_off, const uint64
     // wave costs a whole CTA latency.  Frames are chunked separately, so the count is taken over the real frame sizes.
     // The dense per-chunk count rows cost 4*(B+1) bytes each: keep the chunk at >= 5*B points (<= 5 % extra traffic).
     const size_t total = (size_t)(map_off[F] + qry_off[F]);
-    const size_t slots = (size_t)h->sm_count * (k1_big_tables(h->p.num_rings, h->B) ? 1 : h->ctas_per_sm);
+    const size_t slots = (size_t)h->sm_count * (k1_warps(k1_smem_bytes(h->p.num_rings, h->B)) == 32 ? 1 : h->ctas_per_sm);
     auto count = [&](size_t ch) {
         size_t n = 0;
         for (int f = 0; f < F; ++f) n += (size_t)((map_off[f + 1] - map_off[f] + ch - 1) / ch) + (size_t)((qry_off[f + 1] - qry_off[f] + ch - 1) / ch);
@@ -317,6 +316,18 @@ uint32_t choose_chunk(const erasor_ctx* h, const uint64_t* map_off, const uint64
         ch = cap;      // several waves anyway
     }
     return (uint32_t)ch;
+}
+
+// k's room for K1's outputs over NM map and NQ query points, n_chunks chunks and F frames of B bins (the bin ids with kIdPad of
+// slack: K2 prefetches ids past a chunk's end unchecked)
+int ensure_k1_bufs(erasor_ctx* h, erasor_ctx::K1Bufs& k, size_t NM, size_t NQ, size_t n_chunks, size_t F, size_t B) {
+    CK(k.bin_map.ensure(sizeof(uint16_t) * (NM + kIdPad)));
+    CK(k.bin_qry.ensure(sizeof(uint16_t) * (NQ + kIdPad)));
+    CK(k.ch_cnt.ensure(sizeof(uint32_t) * std::max<size_t>(n_chunks, 1) * (B + 1)));
+    CK(k.zmin.ensure(sizeof(uint32_t) * 2 * F * B));
+    CK(k.zmax.ensure(sizeof(uint32_t) * 2 * F * B));
+    CK(k.cnt.ensure(sizeof(uint32_t) * 2 * F * (B + 1)));
+    return ERASOR_OK;
 }
 
 // Build chunk descriptors + per-frame chunk ranges + frame offsets, upload them, size every buffer.
@@ -374,13 +385,8 @@ int prepare_batch(erasor_ctx* h, const uint64_t* map_off, const uint64_t* qry_of
     CK(h->d_chunks.ensure(sizeof(ChunkDesc) * std::max<size_t>(n_chunks, 1)));
     CK(h->d_chunk_range.ensure(sizeof(uint32_t) * range.size()));
     CK(h->d_frame_off.ensure(sizeof(uint32_t) * foff.size()));
-    CK(h->d_bin_map.ensure(sizeof(uint16_t) * (NM + kIdPad)));      // + slack: K2 prefetches ids past a chunk's end unchecked
-    CK(h->d_bin_qry.ensure(sizeof(uint16_t) * (NQ + kIdPad)));
-    CK(h->d_chcnt.ensure(sizeof(uint32_t) * std::max<size_t>(n_chunks, 1) * (B + 1)));
+    if (const int rc = ensure_k1_bufs(h, h->k1_own, NM, NQ, n_chunks, (size_t)F, (size_t)B)) return rc;
     CK(h->d_map_sorted.ensure(sizeof(float4) * std::max<size_t>(NM, 1)));
-    CK(h->d_zmin.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
-    CK(h->d_zmax.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
-    CK(h->d_cnt.ensure(sizeof(uint32_t) * 2 * (size_t)F * (B + 1)));
     CK(h->d_dst_start.ensure(sizeof(uint32_t) * 2 * (size_t)F * (B + 2)));
     CK(h->d_status.ensure((size_t)F * B));
     CK(h->d_action.ensure((size_t)F * B));
@@ -483,21 +489,27 @@ int geometry_tables(erasor_ctx* h, const erasor_geometry_t& x, const GeoTables**
     return ERASOR_OK;
 }
 
-// The tables K1 writes for geometry g of a sweep plan: the handle's geometry into the per-batch buffers (no plan, or an own plan),
-// any other into the plan's tune_tabs[g]
+// The tables K1 writes for geometry g of a sweep plan: the handle's geometry into k1_own (no plan, or an own plan), any other into
+// k1_sweep[g]
 K1GeoTables k1_tables(const erasor_ctx* h, const SweepPlan* plan, int g) {
+    const bool own = !plan || plan->own;
+    const GeoTables& geo = own ? *h->geo_tables[0] : *plan->geo[g].t;
+    const erasor_ctx::K1Bufs& k = own ? h->k1_own : *h->k1_sweep[g];
     K1GeoTables o{};
-    if (!plan || plan->own) {
-        o.T = h->geo_tables[0]->view; o.B = h->B;
-        o.bin_map = h->d_bin_map.as<uint16_t>(); o.bin_qry = h->d_bin_qry.as<uint16_t>(); o.ch_cnt = h->d_chcnt.as<uint32_t>();
-        o.zmin = h->d_zmin.as<uint32_t>(); o.zmax = h->d_zmax.as<uint32_t>(); o.cnt = h->d_cnt.as<uint32_t>();
-    } else {
-        const erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
-        o.T = plan->geo[g].t->view; o.B = plan->geo[g].t->B;
-        o.bin_map = tt.bin_map.as<uint16_t>(); o.bin_qry = tt.bin_qry.as<uint16_t>(); o.ch_cnt = tt.chcnt.as<uint32_t>();
-        o.zmin = tt.zmin.as<uint32_t>(); o.zmax = tt.zmax.as<uint32_t>(); o.cnt = tt.cnt.as<uint32_t>();
-    }
+    o.T = geo.view; o.B = geo.B;
+    o.bin_map = k.bin_map.as<uint16_t>(); o.bin_qry = k.bin_qry.as<uint16_t>(); o.ch_cnt = k.ch_cnt.as<uint32_t>();
+    o.zmin = k.zmin.as<uint32_t>(); o.zmax = k.zmax.as<uint32_t>(); o.cnt = k.cnt.as<uint32_t>();
     return o;
+}
+
+// The node-mode K1 launch that bins geometry g of a sweep plan (null: a plain call): its warps per CTA and the VoI lists it writes.
+// A plain call and an own plan run the plain K1 into d_list_*; a plan that is not own gives its 32-warp launches d_list_*32, since
+// their split of a chunk differs from its 8-warp launches'.
+struct K1Lists { int warps; erasor_ctx::HBuf& idx; erasor_ctx::HBuf& cnt; };
+K1Lists k1_lists(erasor_ctx* h, const SweepPlan* plan, int g) {
+    if (!plan || plan->own) return {k1_warps(k1_smem_bytes(h->p.num_rings, h->B)), h->d_list_idx, h->d_list_cnt};
+    const int warps = k1_warps(plan->launch_smem[plan->geo[g].launch]);
+    return warps == 32 ? K1Lists{warps, h->d_list_idx32, h->d_list_cnt32} : K1Lists{warps, h->d_list_idx, h->d_list_cnt};
 }
 
 // the reset of the submission's records, queue and frame counters, and with t the reset of K1's z / count tables t
@@ -516,19 +528,19 @@ int run_k1(erasor_ctx* h, int mode) {
     if (rc) return rc;
     Scope s(h, 1);
     if (h->n_chunks_map + h->n_chunks_qry) h->launches++;
-    CK(launch_k1(h->stream, t.T, h->cur_map, h->cur_qry, h->d_chunks.as<ChunkDesc>(), (int)(h->n_chunks_map + h->n_chunks_qry),
-                 t.bin_map, t.bin_qry, t.ch_cnt, t.zmin, t.zmax, t.cnt, t.B, h->F, h->d_fence.as<unsigned long long>(),
-                 mode == 2 ? h->d_poses.as<NodePose>() : nullptr, mode == 2 ? h->d_list_idx.as<uint32_t>() : nullptr,
+    CK(launch_k1(h->stream, t, h->cur_map, h->cur_qry, h->d_chunks.as<ChunkDesc>(), (int)(h->n_chunks_map + h->n_chunks_qry), h->F,
+                 h->d_fence.as<unsigned long long>(), mode == 2 ? h->d_poses.as<NodePose>() : nullptr, mode == 2 ? h->d_list_idx.as<uint32_t>() : nullptr,
                  mode == 2 ? h->d_list_cnt.as<uint32_t>() : nullptr, mode != 0 && h->last.qry_xyz, mode == 2 ? h->k1_prof : nullptr));
     return ERASOR_OK;
 }
 
-SrtParams srt_params(const erasor_ctx* h, int version, int mode) {
+// the handle's Scan Ratio Test settings over the geometry of K1's tables t
+SrtParams srt_params(const erasor_ctx* h, const K1GeoTables& t, int version, int mode) {
     SrtParams sp{};
     sp.scan_ratio_threshold = h->p.scan_ratio_threshold;
     sp.th_bin_max_h = h->p.th_bin_max_h;
     sp.minimum_num_pts = h->p.minimum_num_pts;
-    sp.version = version; sp.R = h->p.num_rings; sp.S = h->p.num_sectors; sp.B = h->B; sp.scatter_mode = mode == 0 ? 0 : 1;
+    sp.version = version; sp.R = t.T.R; sp.S = t.T.S; sp.B = t.B; sp.scatter_mode = mode == 0 ? 0 : 1;
     return sp;
 }
 
@@ -571,32 +583,32 @@ int run_k2_srt(erasor_ctx* h, const SrtParams& sp, const K1GeoTables& t, const u
                const SrtSweep* sweep) {
     Scope s(h, 2);
     if (h->n_chunks_map) h->launches++;
-    CK(launch_k2_srt(h->stream, sp, h->F, h->d_chunks.as<ChunkDesc>(), h->d_chunk_range.as<uint32_t>(), h->n_chunks_map, t.bin_map, h->cur_map,
-                     list_idx ? h->d_poses.as<NodePose>() : nullptr, t.ch_cnt, t.zmin, t.zmax, t.cnt, h->d_frame_off.as<uint32_t>(),
-                     h->d_nflag.as<uint32_t>() + h->f0, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
-                     h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
-                     list_idx, list_cnt, sweep, k1_warps));
+    CK(launch_k2_srt(h->stream, sp, h->F, t, h->d_chunks.as<ChunkDesc>(), h->d_chunk_range.as<uint32_t>(), h->n_chunks_map, h->cur_map,
+                     list_idx ? h->d_poses.as<NodePose>() : nullptr, h->d_frame_off.as<uint32_t>(), h->d_nflag.as<uint32_t>() + h->f0,
+                     h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity, h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>(),
+                     h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), list_idx, list_cnt, k1_warps, sweep));
     return ERASOR_OK;
 }
 
 // K3 -> K2 -> K4 ; mode 0: every bin scattered + partitioned copies (cloud outputs), mode 1 / 2: flagged only + masks
 // classes: which R-GPF size classes to launch (bits 0|1: A and B, bit 2: C)
 int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_t* ground_mask, const K4Fold& fold, int classes = 7) {
-    const int B = h->B, F = h->F;
+    const int F = h->F;
     const NodePose* poses = mode == 2 ? h->d_poses.as<NodePose>() : nullptr;
     uint32_t* nflag = h->d_nflag.as<uint32_t>() + h->f0;
-    const SrtParams sp = srt_params(h, version, mode);
-    const int k1_warps = k1_big_tables(h->p.num_rings, B) ? 32 : 8;
+    const K1GeoTables t = k1_tables(h, nullptr, 0);
+    const SrtParams sp = srt_params(h, t, version, mode);
+    const K1Lists l = k1_lists(h, nullptr, 0);
+    uint32_t* list_idx = poses ? l.idx.as<uint32_t>() : nullptr;
+    uint32_t* list_cnt = poses ? l.cnt.as<uint32_t>() : nullptr;
     if (mode != 0 && h->fused_srt) {      // mask modes: SRT inside the scatter kernel
-        const int rc = run_k2_srt(h, sp, k1_tables(h, nullptr, 0), poses ? h->d_list_idx.as<uint32_t>() : nullptr,
-                                  poses ? h->d_list_cnt.as<uint32_t>() : nullptr, k1_warps, nullptr);
+        const int rc = run_k2_srt(h, sp, t, list_idx, list_cnt, l.warps, nullptr);
         if (rc) return rc;
     } else {
         {
             Scope s(h, 3);
             h->launches++;
-            CK(launch_k3(h->stream, sp, F, h->d_chunk_range.as<uint32_t>(), h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(),
-                         h->d_zmax.as<uint32_t>(), h->d_frame_off.as<uint32_t>(), h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(),
+            CK(launch_k3(h->stream, sp, F, t, h->d_chunk_range.as<uint32_t>(), h->d_frame_off.as<uint32_t>(), h->d_dst_start.as<uint32_t>(),
                          h->d_status.as<uint8_t>(), h->d_action.as<uint8_t>(), h->d_flag_slot.as<uint32_t>(), nflag,
                          h->d_frame_rec_base.as<uint32_t>(), h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
                          h->d_queue.as<uint32_t>(), h->d_bucket.as<uint32_t>()));
@@ -604,17 +616,14 @@ int run_compare(erasor_ctx* h, int version, int mode, uint8_t* keep_mask, uint8_
         Scope s(h, 2);
         if (mode == 0) {
             if (h->n_chunks_map + h->n_chunks_qry) h->launches++;
-            CK(launch_k2_both(h->stream, h->d_chunks.as<ChunkDesc>(), h->n_chunks_map, h->n_chunks_qry, h->d_chcnt.as<uint32_t>(), B,
-                              h->d_bin_map.as<uint16_t>(), h->cur_map, h->d_dst_start.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
-                              h->d_bin_qry.as<uint16_t>(), h->cur_qry, h->d_dst_start.as<uint32_t>() + (size_t)F * (B + 2), h->d_qry_sorted.as<float4>(),
-                              h->d_qry_src.as<uint32_t>()));
+            CK(launch_k2_both(h->stream, t, h->d_chunks.as<ChunkDesc>(), h->n_chunks_map, h->n_chunks_qry,
+                              h->cur_map, h->d_dst_start.as<uint32_t>(), h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(),
+                              h->cur_qry, h->d_dst_start.as<uint32_t>() + (size_t)F * (t.B + 2), h->d_qry_sorted.as<float4>(), h->d_qry_src.as<uint32_t>()));
         } else {
             // mask modes, unfused (ERASOR_B200_UNFUSED_SRT=1): the same stable scatter, restricted to the flagged bins (K3's dense slots)
             if (h->n_chunks_map) h->launches++;
-            CK(launch_k2(h->stream, h->d_chunks.as<ChunkDesc>(), 0u, h->n_chunks_map, h->d_bin_map.as<uint16_t>(), h->cur_map, poses,
-                         h->d_chcnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(), h->d_flag_slot.as<uint32_t>(), nflag,
-                         h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), B,
-                         poses ? h->d_list_idx.as<uint32_t>() : nullptr, poses ? h->d_list_cnt.as<uint32_t>() : nullptr, k1_warps));
+            CK(launch_k2(h->stream, t, 0, h->d_chunks.as<ChunkDesc>(), 0u, h->n_chunks_map, h->cur_map, poses, h->d_dst_start.as<uint32_t>(),
+                         h->d_flag_slot.as<uint32_t>(), nflag, h->d_map_sorted.as<float4>(), h->d_map_src.as<uint32_t>(), list_idx, list_cnt, l.warps));
         }
     }
     return run_k4(h, mode, keep_mask, ground_mask, fold, classes, nullptr);
@@ -643,24 +652,18 @@ int run_sweep(erasor_ctx* h, const SweepPlan& plan, bool qry_xyz, int classes) {
                 G.g[G.n] = k1_tables(h, &plan, g);
                 G.g[G.n].smem_off = G.n ? G.g[G.n - 1].smem_off + (uint32_t)k1_geo_smem_bytes(G.g[G.n - 1].T.R, G.g[G.n - 1].B) : 0u;
             }
-            const bool big = plan.launch_smem[l] > 56 * 1024;
+            const K1Lists lists = k1_lists(h, &plan, plan.launch_begin[l]);
             if (n_chunks) h->launches++;
             CK(launch_k1_geo(h->stream, G, plan.launch_smem[l], h->cur_map, h->cur_qry, h->d_chunks.as<ChunkDesc>(), n_chunks, h->F,
-                             h->d_fence.as<unsigned long long>(), h->d_poses.as<NodePose>(), (big ? h->d_list_idx32 : h->d_list_idx).as<uint32_t>(),
-                             (big ? h->d_list_cnt32 : h->d_list_cnt).as<uint32_t>(), qry_xyz));
+                             h->d_fence.as<unsigned long long>(), h->d_poses.as<NodePose>(), lists.idx.as<uint32_t>(), lists.cnt.as<uint32_t>(), qry_xyz));
         }
     }
     for (int g = n_geo - 1; g >= 0; --g) {
         const SweepGeo& sg = plan.geo[g];
         if (g != n_geo - 1 && (rc = run_init(h, nullptr))) return rc;      // records, queue and frame counters of the geometry before
         const K1GeoTables t = k1_tables(h, &plan, g);
-        SrtParams sp = srt_params(h, h->p.version, 2);
-        sp.R = t.T.R; sp.S = t.T.S; sp.B = t.B;
-        // the warps of the K1 launch that wrote g's ids and lists: a plain launch's for an own plan, else those of g's packed launch
-        const bool big = plan.own ? k1_big_tables(t.T.R, t.B) : plan.launch_smem[sg.launch] > 56 * 1024;
-        const bool lists32 = big && !plan.own;
-        if ((rc = run_k2_srt(h, sp, t, (lists32 ? h->d_list_idx32 : h->d_list_idx).as<uint32_t>(), (lists32 ? h->d_list_cnt32 : h->d_list_cnt).as<uint32_t>(),
-                             big ? 32 : 8, &sg.ssw)))
+        const K1Lists lists = k1_lists(h, &plan, g);
+        if ((rc = run_k2_srt(h, srt_params(h, t, h->p.version, 2), t, lists.idx.as<uint32_t>(), lists.cnt.as<uint32_t>(), lists.warps, &sg.ssw)))
             return rc;
         if ((rc = run_k4(h, 2, nullptr, nullptr, K4Fold{nullptr, nullptr, 0u, 0u}, classes, &sg.ksw))) return rc;
     }
@@ -694,33 +697,34 @@ int ensure_insert_buffers(erasor_ctx* h) {
 
 // ... after K1: the action of every bin and the stable scatter of the inserting bins' query points ...
 int run_insert_plan(erasor_ctx* h) {
-    const int B = h->B, F = h->F;
+    const int F = h->F;
+    const K1GeoTables t = k1_tables(h, nullptr, 0);
     CK(cudaMemcpyAsync(h->d_ins_fwd.p(), h->h_ins_fwd.p(), sizeof(float) * 12 * (size_t)F, cudaMemcpyHostToDevice, h->stream));
     h->launches += 1 + (h->n_chunks_qry ? 1 : 0);
-    CK(launch_ins_plan(h->stream, srt_params(h, h->p.version, 2), F, h->d_chunk_range.as<uint32_t>(), h->d_chcnt.as<uint32_t>(), h->d_zmin.as<uint32_t>(),
-                       h->d_zmax.as<uint32_t>(), h->d_cnt.as<uint32_t>(), h->d_action.as<uint8_t>(), h->d_flag_slot.as<uint32_t>(),
-                       h->d_ins_slot.as<uint32_t>(), h->d_ins_n.as<uint32_t>(), h->d_dst_start.as<uint32_t>()));
-    CK(launch_k2(h->stream, h->d_chunks.as<ChunkDesc>(), h->n_chunks_map, h->n_chunks_qry, h->d_bin_qry.as<uint16_t>(), h->cur_qry, nullptr,
-                 h->d_chcnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>() + (size_t)F * (B + 2), h->d_ins_slot.as<uint32_t>(), h->d_ins_n.as<uint32_t>(),
-                 h->d_qry_sorted.as<float4>(), h->d_qry_src.as<uint32_t>(), B, nullptr, nullptr, 8));
+    CK(launch_ins_plan(h->stream, srt_params(h, t, h->p.version, 2), F, t, h->d_chunk_range.as<uint32_t>(), h->d_action.as<uint8_t>(),
+                       h->d_flag_slot.as<uint32_t>(), h->d_ins_slot.as<uint32_t>(), h->d_ins_n.as<uint32_t>(), h->d_dst_start.as<uint32_t>()));
+    CK(launch_k2(h->stream, t, 1, h->d_chunks.as<ChunkDesc>(), h->n_chunks_map, h->n_chunks_qry, h->cur_qry, nullptr,
+                 h->d_dst_start.as<uint32_t>() + (size_t)F * (t.B + 2), h->d_ins_slot.as<uint32_t>(), h->d_ins_n.as<uint32_t>(),
+                 h->d_qry_sorted.as<float4>(), h->d_qry_src.as<uint32_t>(), nullptr, nullptr, 8));
     return ERASOR_OK;
 }
 
 // ... after R-GPF: K4b over every frame's flagged bins (v3), then sizes, offsets and the copy; the offsets are read back through
 // pinned memory (again after a late class-C run, which changes the ground of its bins)
 int run_insert_assemble(erasor_ctx* h) {
-    const int B = h->B, F = h->F;
+    const int F = h->F;
+    const K1GeoTables t = k1_tables(h, nullptr, 0);
     const bool vox = h->p.version == 3 && !h->p.skip_voxelize;
     const uint32_t* qoff = h->d_frame_off.as<uint32_t>() + (F + 1);
     if (vox) {
         h->launches++;
-        CK(launch_k4b(h->stream, (float)h->p.map_voxel_size, B, F, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
-                      h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(), qoff, h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(),
+        CK(launch_k4b(h->stream, (float)h->p.map_voxel_size, t.B, F, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
+                      t.cnt, h->d_dst_start.as<uint32_t>(), qoff, h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(),
                       h->d_vox.as<float4>(), h->d_vox_cnt.as<uint32_t>(), h->d_vox_start.as<uint32_t>(), h->d_vox_scratch.as<unsigned char>(), h->sm_count));
     }
     h->launches += kInsAssembleLaunches;
-    CK(launch_ins_assemble(h->stream, B, F, vox ? 1 : 0, h->d_action.as<uint8_t>(), h->d_flag_slot.as<uint32_t>(), h->d_frame_rec_base.as<uint32_t>(),
-                           h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity, h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(),
+    CK(launch_ins_assemble(h->stream, t.B, F, vox ? 1 : 0, h->d_action.as<uint8_t>(), h->d_flag_slot.as<uint32_t>(), h->d_frame_rec_base.as<uint32_t>(),
+                           h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity, t.cnt, h->d_dst_start.as<uint32_t>(),
                            qoff, vox ? h->d_vox_cnt.as<uint32_t>() : nullptr, vox ? h->d_vox_start.as<uint32_t>() : nullptr,
                            h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(), vox ? h->d_vox.as<float4>() : nullptr, h->d_ins_fwd.as<float>(),
                            h->d_ins_bin_off.as<uint32_t>(), h->d_ins_frame_cnt.as<uint32_t>(), h->d_ins_off.as<uint32_t>(), h->d_ins.as<float4>(),
@@ -896,7 +900,8 @@ int erasor_compare(erasor_handle_t h, int version, int frame) {
     if (h->stage > 1) { h->err = "erasor_compare called twice: set_inputs -> exactly one compare (OfflineMapUpdater.cpp:266-272)"; return ERASOR_E_STATE; }
     if (version != 2 && version != 3) { h->err = "Other version is not implemented!"; return ERASOR_E_INVALID; }
     CK(cudaSetDevice(h->device));
-    const int B = h->B;
+    const K1GeoTables t = k1_tables(h, nullptr, 0);
+    const int B = t.B;
     const size_t NM = h->NM, NQ = h->NQ;
     CK(h->d_keep.ensure(std::max<size_t>(NM, 1)));
     CK(h->d_ground.ensure(std::max<size_t>(NM, 1)));
@@ -926,14 +931,14 @@ int erasor_compare(erasor_handle_t h, int version, int frame) {
             Scope s(h, 4);
             h->launches++;
             CK(launch_k4b(h->stream, (float)h->p.map_voxel_size, B, 1, h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(), h->rec_capacity,
-                          h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(), h->d_frame_off.as<uint32_t>() + 2, h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(),
+                          t.cnt, h->d_dst_start.as<uint32_t>(), h->d_frame_off.as<uint32_t>() + 2, h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(),
                           h->d_vox.as<float4>(), h->d_vox_cnt.as<uint32_t>(), h->d_vox_start.as<uint32_t>(),
                           h->d_vox_scratch.as<unsigned char>(), h->sm_count));
         }
         {
             Scope s(h, 5);
             h->launches += 2;
-            CK(launch_k5(h->stream, B, version, h->p.skip_voxelize, h->d_cnt.as<uint32_t>(), h->d_dst_start.as<uint32_t>(), h->d_action.as<uint8_t>(),
+            CK(launch_k5(h->stream, B, version, h->p.skip_voxelize, t.cnt, h->d_dst_start.as<uint32_t>(), h->d_action.as<uint8_t>(),
                          h->d_flag_slot.as<uint32_t>(), h->d_recs.as<FlagRec>(), h->d_nrecs.as<uint32_t>(),
                          vox ? h->d_vox_cnt.as<uint32_t>() : nullptr, vox ? h->d_vox_start.as<uint32_t>() : nullptr,
                          h->d_map_sorted.as<float4>(), h->d_qry_sorted.as<float4>(), h->d_part.as<float4>(),
@@ -1041,20 +1046,21 @@ int erasor_get_bins(erasor_handle_t h, int which_cloud, int32_t* bin_of_point, f
     if (node && bin_of_point) { h->err = "node mode keeps no per-point bins of the map"; return ERASOR_E_STATE; }
     if (which_cloud != 0 && which_cloud != 1) { h->err = "which_cloud"; return ERASOR_E_INVALID; }
     CK(cudaSetDevice(h->device));
-    const int B = h->B;
+    const K1GeoTables t = k1_tables(h, nullptr, 0);
+    const int B = t.B;
     const size_t n = which_cloud == 0 ? h->NM : h->NQ;
     CK(cudaStreamSynchronize(h->stream));
     if (bin_of_point && n) {
         std::vector<uint16_t> tmp(n);
-        CK(cudaMemcpy(tmp.data(), which_cloud == 0 ? h->d_bin_map.p() : h->d_bin_qry.p(), sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(tmp.data(), which_cloud == 0 ? t.bin_map : t.bin_qry, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < n; ++i) bin_of_point[i] = tmp[i] == kNoBin16 ? -1 : (int32_t)tmp[i];
     }
     if (min_h || max_h || count) {
         std::vector<uint32_t> mn(B), mx(B);
-        CK(cudaMemcpy(mn.data(), h->d_zmin.as<uint32_t>() + (size_t)which_cloud * B, sizeof(uint32_t) * B, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(mx.data(), h->d_zmax.as<uint32_t>() + (size_t)which_cloud * B, sizeof(uint32_t) * B, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(mn.data(), t.zmin + (size_t)which_cloud * B, sizeof(uint32_t) * B, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(mx.data(), t.zmax + (size_t)which_cloud * B, sizeof(uint32_t) * B, cudaMemcpyDeviceToHost));
         std::vector<uint32_t> c(B, 0);
-        CK(cudaMemcpy(c.data(), h->d_cnt.as<uint32_t>() + (size_t)which_cloud * (B + 1), sizeof(uint32_t) * B, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(c.data(), t.cnt + (size_t)which_cloud * (B + 1), sizeof(uint32_t) * B, cudaMemcpyDeviceToHost));
         const float nan = std::numeric_limits<float>::quiet_NaN();
         for (int b = 0; b < B; ++b) {
             const bool empty = mn[b] == 0xFFFFFFFFu && mx[b] == 0u;
@@ -1240,22 +1246,13 @@ int submit(erasor_ctx* h, Step st, const uint64_t* map_off, const uint64_t* qry_
         auto plan = std::make_shared<SweepPlan>(*st.sweep);
         const size_t n_geo = plan->geo.size(), n_chunks = (size_t)h->n_chunks_map + h->n_chunks_qry;
         if (!plan->own) {
-            while (h->tune_tabs.size() < n_geo) h->tune_tabs.emplace_back(new erasor_ctx::TuneTabs(h->alloc_epoch));
+            while (h->k1_sweep.size() < n_geo) h->k1_sweep.emplace_back(new erasor_ctx::K1Bufs(h->alloc_epoch));
             for (size_t g = 0; g < n_geo; ++g) {
-                const size_t B = (size_t)plan->geo[g].t->B;
-                erasor_ctx::TuneTabs& tt = *h->tune_tabs[g];
-                CK(tt.bin_map.ensure(sizeof(uint16_t) * (h->NM + kIdPad)));
-                CK(tt.bin_qry.ensure(sizeof(uint16_t) * (h->NQ + kIdPad)));
-                CK(tt.chcnt.ensure(sizeof(uint32_t) * std::max<size_t>(n_chunks, 1) * (B + 1)));
-                CK(tt.zmin.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
-                CK(tt.zmax.ensure(sizeof(uint32_t) * 2 * (size_t)F * B));
-                CK(tt.cnt.ensure(sizeof(uint32_t) * 2 * (size_t)F * (B + 1)));
+                if ((rc = ensure_k1_bufs(h, *h->k1_sweep[g], h->NM, h->NQ, n_chunks, (size_t)F, (size_t)plan->geo[g].t->B))) return rc;
+                const K1Lists lists = k1_lists(h, plan.get(), (int)g);     // (an 8-warp launch's are prepare_batch's, sized already)
+                CK(lists.idx.ensure(sizeof(uint32_t) * (h->NM + kIdPad)));
+                CK(lists.cnt.ensure(sizeof(uint32_t) * kListWarps * std::max<size_t>(n_chunks, 1)));
             }
-            for (size_t smem : plan->launch_smem)
-                if (smem > 56 * 1024) {
-                    CK(h->d_list_idx32.ensure(sizeof(uint32_t) * (h->NM + kIdPad)));
-                    CK(h->d_list_cnt32.ensure(sizeof(uint32_t) * kListWarps * std::max<size_t>(n_chunks, 1)));
-                }
             st.with_c = true;
         }
         const uint32_t recs = (uint32_t)std::min<size_t>((size_t)F * plan->B_max, kMaxRecords);
@@ -1678,8 +1675,7 @@ int process_nodes_sweep(erasor_handle_t h, const char* fn, const double* poses7,
         if (plan->own) continue;
         // K1 packing
         const size_t bytes = k1_geo_smem_bytes(sg.t->view.R, sg.t->B);
-        const bool alone = h->tune_unpacked || bytes > 56 * 1024;
-        if (g == 0 || alone || plan->launch_smem.back() + bytes > 56 * 1024 || plan->launch_smem.back() > 56 * 1024) {
+        if (g == 0 || h->tune_unpacked || k1_warps(plan->launch_smem.back() + bytes) == 32) {
             plan->launch_begin.push_back(g);
             plan->launch_smem.push_back(0);
         }
@@ -2043,7 +2039,7 @@ int erasor_profile_k1(erasor_handle_t h, uint32_t* out, size_t* n, int* warps_pe
     CK(cudaSetDevice(h->device));
     int rc;
     if (h->pending && (rc = erasor_wait(h))) return rc;
-    const int nw = k1_big_tables(h->p.num_rings, h->B) ? 32 : 8;
+    const int nw = k1_lists(h, nullptr, 0).warps;
     const size_t words = (size_t)(h->n_chunks_map + h->n_chunks_qry) * nw * kK1ProfSlots;
     const size_t cap = *n;
     *n = words;

@@ -159,7 +159,7 @@ cudaError_t launch_k1_geo(cudaStream_t st, const K1Geo& G, size_t smem, const fl
                           int n_chunks, int F, unsigned long long* fence, const NodePose* poses, uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz) {
     if (n_chunks == 0) return cudaSuccess;
     constexpr int UNROLL = 4;
-    const bool big = smem > 56 * 1024;            // k1_big_tables's rule, on the launch's packed tables
+    const bool big = k1_warps(smem) == 32;
     auto kern = big ? k1_geo_bin<1024, UNROLL> : k1_geo_bin<256, UNROLL>;
     cudaError_t e = ensure_dyn_smem(kern, smem);
     if (e != cudaSuccess) return e;

@@ -220,30 +220,24 @@ k1_rpod_bin(BinTablesView T, const float4* __restrict__ map_pts, const float4* _
     }
 }
 
-bool k1_big_tables(int R, int B) { return k1_smem_bytes(R, B) > 56 * 1024; }
-
 size_t k1_smem_bytes(int R, int B) {
     return sizeof(float2) * ((R + 2) & ~1) + sizeof(uint32_t) * ((size_t)(B + 1) + 2 * (size_t)B);
 }
 
-cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map_pts, const float4* qry_pts,
-                      const ChunkDesc* chunks, int n_chunks, uint16_t* bin_map, uint16_t* bin_qry, uint32_t* ch_cnt,
-                      uint32_t* zmin, uint32_t* zmax, uint32_t* cnt_tab, int B, int F, unsigned long long* fence, const NodePose* poses,
-                      uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz, uint32_t* prof) {
+cudaError_t launch_k1(cudaStream_t st, const K1GeoTables& t, const float4* map_pts, const float4* qry_pts, const ChunkDesc* chunks, int n_chunks,
+                      int F, unsigned long long* fence, const NodePose* poses, uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz, uint32_t* prof) {
     if (n_chunks == 0) return cudaSuccess;
     if (prof && !poses) return cudaErrorInvalidValue;      // the profiling build covers node mode only
     constexpr int UNROLL = 4;
-    // Bin tables beyond ~56 KB (40 x 360 bins: 173 KB) leave one CTA per SM: give that CTA 32 warps instead of 8, the
-    // kernel needs ~32 resident warps per SM to cover its latencies.
-    const bool big = k1_big_tables(T.R, B);
+    const size_t smem = k1_smem_bytes(t.T.R, t.B);
+    const bool big = k1_warps(smem) == 32;
     auto kern = prof  ? (big ? k1_rpod_bin<1024, UNROLL, true, true> : k1_rpod_bin<256, UNROLL, true, true>)
               : poses ? (big ? k1_rpod_bin<1024, UNROLL, true> : k1_rpod_bin<256, UNROLL, true>)
                       : (big ? k1_rpod_bin<1024, UNROLL, false> : k1_rpod_bin<256, UNROLL, false>);
-    const size_t smem = k1_smem_bytes(T.R, B);
     cudaError_t e = ensure_dyn_smem(kern, smem);
     if (e != cudaSuccess) return e;
-    kern<<<n_chunks, big ? 1024 : 256, smem, st>>>(T, map_pts, qry_pts, chunks, bin_map, bin_qry, ch_cnt, zmin, zmax, cnt_tab, B, F, fence, poses,
-                                                   list_idx, list_cnt, qry_xyz ? 1 : 0, prof);
+    kern<<<n_chunks, big ? 1024 : 256, smem, st>>>(t.T, map_pts, qry_pts, chunks, t.bin_map, t.bin_qry, t.ch_cnt, t.zmin, t.zmax, t.cnt, t.B, F, fence,
+                                                   poses, list_idx, list_cnt, qry_xyz ? 1 : 0, prof);
     return cudaGetLastError();
 }
 
@@ -494,14 +488,13 @@ k3_srt(SrtParams P, int F, const uint32_t* __restrict__ chunk_range /*[2][F+1]*/
 
 size_t k3_smem_bytes(int B) { return sizeof(uint32_t) * ((size_t)B + 2 + 34) + (size_t)B + 16; }
 
-cudaError_t launch_k3(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt,
-                      const uint32_t* zmin, const uint32_t* zmax, const uint32_t* frame_off, const uint32_t* cnt, uint32_t* dst_start,
-                      uint8_t* status, uint8_t* action, uint32_t* flag_slot, uint32_t* n_flagged, uint32_t* frame_rec_base,
+cudaError_t launch_k3(cudaStream_t st, const SrtParams& P, int F, const K1GeoTables& t, const uint32_t* chunk_range, const uint32_t* frame_off,
+                      uint32_t* dst_start, uint8_t* status, uint8_t* action, uint32_t* flag_slot, uint32_t* n_flagged, uint32_t* frame_rec_base,
                       FlagRec* recs, uint32_t* n_recs, uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list) {
     const size_t smem = k3_smem_bytes(P.B);
     cudaError_t e = ensure_dyn_smem(k3_srt, smem);
     if (e != cudaSuccess) return e;
-    k3_srt<<<F, 1024, smem, st>>>(P, F, chunk_range, ch_cnt, zmin, zmax, frame_off, cnt, dst_start, status, action,
+    k3_srt<<<F, 1024, smem, st>>>(P, F, chunk_range, t.ch_cnt, t.zmin, t.zmax, frame_off, t.cnt, dst_start, status, action,
                                   flag_slot, n_flagged, frame_rec_base, recs, n_recs, rec_capacity, queue, bucket_list);
     return cudaGetLastError();
 }
@@ -1007,67 +1000,67 @@ static void k2_smem_plan(int B, bool with_complement, bool node, uint32_t& SW, s
     smem = sizeof(uint32_t) * (size_t)(W + 1) * SW + fixed;
 }
 
-cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const ChunkDesc* chunks, const uint32_t* chunk_range, uint32_t n_chunks_map,
-                          const uint16_t* bin_ids, const float4* pts, const NodePose* poses, const uint32_t* ch_cnt, const uint32_t* zmin,
-                          const uint32_t* zmax, const uint32_t* cnt, const uint32_t* frame_off, uint32_t* n_flagged, FlagRec* recs, uint32_t* n_recs,
-                          uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list, float4* out_pts, uint32_t* out_src,
-                          const uint32_t* list_idx, const uint32_t* list_cnt, const SrtSweep* sweep, int k1_warps) {
+cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const K1GeoTables& t, const ChunkDesc* chunks, const uint32_t* chunk_range,
+                          uint32_t n_chunks_map, const float4* pts, const NodePose* poses, const uint32_t* frame_off, uint32_t* n_flagged, FlagRec* recs,
+                          uint32_t* n_recs, uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list, float4* out_pts, uint32_t* out_src,
+                          const uint32_t* list_idx, const uint32_t* list_cnt, int k1_warps, const SrtSweep* sweep) {
     if (n_chunks_map == 0) return cudaSuccess;
     constexpr int W = 8;
-    if (k1_warps == 0) k1_warps = k1_big_tables(P.R, P.B) ? 32 : 8;     // the split K1 compacted the chunk's VoI points in
     uint32_t SW; size_t smem;
     k2_smem_plan(P.B, false, poses != nullptr, SW, smem);
     cudaError_t e;
     if (sweep) {                                                  // node mode only
         auto kern = k2_srt_sweep_scatter<W, true>;
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, bin_ids, pts, poses, ch_cnt, zmin, zmax, cnt, frame_off, n_flagged, recs, n_recs,
-                                                 rec_capacity, queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps, *sweep);
+        kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, t.bin_map, pts, poses, t.ch_cnt, t.zmin, t.zmax, t.cnt, frame_off, n_flagged,
+                                                 recs, n_recs, rec_capacity, queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps, *sweep);
     } else {
         auto kern = poses ? k2_srt_scatter<W, true> : k2_srt_scatter<W, false>;
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, bin_ids, pts, poses, ch_cnt, zmin, zmax, cnt, frame_off, n_flagged, recs, n_recs,
-                                                 rec_capacity, queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps);
+        kern<<<n_chunks_map, W * 32, smem, st>>>(P, F, chunks, chunk_range, t.bin_map, pts, poses, t.ch_cnt, t.zmin, t.zmax, t.cnt, frame_off, n_flagged,
+                                                 recs, n_recs, rec_capacity, queue, bucket_list, out_pts, out_src, SW, list_idx, list_cnt, k1_warps);
     }
     return cudaGetLastError();
 }
 
-cudaError_t launch_k2(cudaStream_t st, const ChunkDesc* chunks, uint32_t chunk_base, uint32_t n_chunks,
-                      const uint16_t* bin_ids, const float4* pts, const NodePose* poses, const uint32_t* ch_cnt, const uint32_t* dst_start,
-                      const uint32_t* flag_slot, const uint32_t* n_flagged, float4* out_pts, uint32_t* out_src, int B,
-                      const uint32_t* list_idx, const uint32_t* list_cnt, int k1_warps) {
+cudaError_t launch_k2(cudaStream_t st, const K1GeoTables& t, int cloud, const ChunkDesc* chunks, uint32_t chunk_base, uint32_t n_chunks,
+                      const float4* pts, const NodePose* poses, const uint32_t* dst_start, const uint32_t* flag_slot, const uint32_t* n_flagged,
+                      float4* out_pts, uint32_t* out_src, const uint32_t* list_idx, const uint32_t* list_cnt, int k1_warps) {
     if (n_chunks == 0) return cudaSuccess;
     constexpr int W = 8;
     uint32_t SW; size_t smem;
-    k2_smem_plan(B, flag_slot == nullptr, poses != nullptr, SW, smem);
+    k2_smem_plan(t.B, flag_slot == nullptr, poses != nullptr, SW, smem);
+    const uint16_t* bin_ids = cloud == 0 ? t.bin_map : t.bin_qry;
     cudaError_t e;
     const K2Second none{0u, nullptr, nullptr, nullptr, nullptr, nullptr};
     if (poses) {
         auto kern = k2_scatter_win<W, true, false>;
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks, W * 32, smem, st>>>(chunks, chunk_base, bin_ids, pts, poses, ch_cnt, dst_start, flag_slot, n_flagged, out_pts, out_src, B, SW, list_idx, list_cnt, k1_warps, none);
+        kern<<<n_chunks, W * 32, smem, st>>>(chunks, chunk_base, bin_ids, pts, poses, t.ch_cnt, dst_start, flag_slot, n_flagged, out_pts, out_src, t.B, SW,
+                                             list_idx, list_cnt, k1_warps, none);
     } else {
         auto kern = k2_scatter_win<W, false, false>;
         if ((e = ensure_dyn_smem(kern, smem)) != cudaSuccess) return e;
-        kern<<<n_chunks, W * 32, smem, st>>>(chunks, chunk_base, bin_ids, pts, nullptr, ch_cnt, dst_start, flag_slot, n_flagged, out_pts, out_src, B, SW, nullptr, nullptr, W, none);
+        kern<<<n_chunks, W * 32, smem, st>>>(chunks, chunk_base, bin_ids, pts, nullptr, t.ch_cnt, dst_start, flag_slot, n_flagged, out_pts, out_src, t.B, SW,
+                                             nullptr, nullptr, W, none);
     }
     return cudaGetLastError();
 }
 
 // cloud mode: the map cloud's chunks (rows [0, n_chunks_map)) and the query cloud's (the n_chunks_qry rows behind them) in one launch
-cudaError_t launch_k2_both(cudaStream_t st, const ChunkDesc* chunks, uint32_t n_chunks_map, uint32_t n_chunks_qry, const uint32_t* ch_cnt, int B,
-                           const uint16_t* bin_map, const float4* map_pts, const uint32_t* dst_start_map, float4* out_map, uint32_t* src_map,
-                           const uint16_t* bin_qry, const float4* qry_pts, const uint32_t* dst_start_qry, float4* out_qry, uint32_t* src_qry) {
+cudaError_t launch_k2_both(cudaStream_t st, const K1GeoTables& t, const ChunkDesc* chunks, uint32_t n_chunks_map, uint32_t n_chunks_qry,
+                           const float4* map_pts, const uint32_t* dst_start_map, float4* out_map, uint32_t* src_map,
+                           const float4* qry_pts, const uint32_t* dst_start_qry, float4* out_qry, uint32_t* src_qry) {
     if (n_chunks_map + n_chunks_qry == 0) return cudaSuccess;
     constexpr int W = 8;
     uint32_t SW; size_t smem;
-    k2_smem_plan(B, true, false, SW, smem);
+    k2_smem_plan(t.B, true, false, SW, smem);
     auto kern = k2_scatter_win<W, false, true>;
     cudaError_t e = ensure_dyn_smem(kern, smem);
     if (e != cudaSuccess) return e;
-    const K2Second second{n_chunks_map, bin_qry, qry_pts, dst_start_qry, out_qry, src_qry};
-    kern<<<n_chunks_map + n_chunks_qry, W * 32, smem, st>>>(chunks, 0u, bin_map, map_pts, nullptr, ch_cnt, dst_start_map, nullptr, nullptr, out_map, src_map, B, SW,
-                                                             nullptr, nullptr, W, second);
+    const K2Second second{n_chunks_map, t.bin_qry, qry_pts, dst_start_qry, out_qry, src_qry};
+    kern<<<n_chunks_map + n_chunks_qry, W * 32, smem, st>>>(chunks, 0u, t.bin_map, map_pts, nullptr, t.ch_cnt, dst_start_map, nullptr, nullptr, out_map, src_map,
+                                                             t.B, SW, nullptr, nullptr, W, second);
     return cudaGetLastError();
 }
 
@@ -2270,13 +2263,12 @@ k_ins_plan(SrtParams P, int F, const uint32_t* __restrict__ chunk_range /*[2][F+
         if (inserts(b)) chunk_rows_excl_prefix(ch_cnt, B, b, c0, c1);
 }
 
-cudaError_t launch_ins_plan(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt, const uint32_t* zmin,
-                            const uint32_t* zmax, const uint32_t* cnt, uint8_t* action, uint32_t* flag_slot, uint32_t* ins_slot, uint32_t* n_ins,
-                            uint32_t* dst_start) {
+cudaError_t launch_ins_plan(cudaStream_t st, const SrtParams& P, int F, const K1GeoTables& t, const uint32_t* chunk_range, uint8_t* action,
+                            uint32_t* flag_slot, uint32_t* ins_slot, uint32_t* n_ins, uint32_t* dst_start) {
     const size_t smem = sizeof(uint32_t) * ((size_t)P.B + 1);
     cudaError_t e = ensure_dyn_smem(k_ins_plan, smem);
     if (e != cudaSuccess) return e;
-    k_ins_plan<<<F, 1024, smem, st>>>(P, F, chunk_range, ch_cnt, zmin, zmax, cnt, action, flag_slot, ins_slot, n_ins, dst_start);
+    k_ins_plan<<<F, 1024, smem, st>>>(P, F, chunk_range, t.ch_cnt, t.zmin, t.zmax, t.cnt, action, flag_slot, ins_slot, n_ins, dst_start);
     return cudaGetLastError();
 }
 

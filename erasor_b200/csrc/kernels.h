@@ -17,50 +17,50 @@ struct CopyJob {
 };
 
 size_t k1_smem_bytes(int R, int B);
-bool   k1_big_tables(int R, int B);      // one 1024-thread CTA per SM instead of four 256-thread ones
 size_t k3_smem_bytes(int B);
+
+// K1's warps per CTA over shared tables of this many bytes: beyond 56 KB (40 x 360 bins: 173 KB) one CTA fits per SM and needs 32
+// warps to cover K1's latencies, else four 8-warp CTAs do.  K2 walks the VoI lists with the count of the K1 launch that wrote them.
+constexpr size_t kK1SmallTables = 56 * 1024;
+inline int k1_warps(size_t table_smem_bytes) { return table_smem_bytes > kK1SmallTables ? 32 : 8; }
 
 cudaError_t launch_init_tables(cudaStream_t st, uint32_t* zmin, uint32_t* zmax, size_t n, uint32_t* cnt, size_t n_cnt, uint32_t* n_recs,
                                uint32_t* frame_rejected, uint32_t* n_flagged, int F, uint32_t* queue);
 
 // poses != null: node mode (the map cloud is the resident global map; fetch_VoI's cut + transform fused into the binning)
-cudaError_t launch_k1(cudaStream_t st, const BinTablesView& T, const float4* map_pts, const float4* qry_pts,
-                      const ChunkDesc* chunks, int n_chunks, uint16_t* bin_map, uint16_t* bin_qry, uint32_t* ch_cnt,
-                      uint32_t* zmin, uint32_t* zmax, uint32_t* cnt_tab, int B, int F, unsigned long long* fence, const NodePose* poses,
+cudaError_t launch_k1(cudaStream_t st, const K1GeoTables& t, const float4* map_pts, const float4* qry_pts, const ChunkDesc* chunks, int n_chunks, int F,
+                      unsigned long long* fence, const NodePose* poses,
                       uint32_t* list_idx /*node mode: map index of every VoI point, per chunk*/, uint32_t* list_cnt /*node mode: VoI points per chunk*/,
                       bool qry_xyz = false /*the query cloud is packed x y z, 12 bytes per point (mask modes)*/,
                       uint32_t* prof = nullptr /*node mode only: run the profiling build, kK1ProfSlots cycle counters per warp*/);
 
-// K1's geometry form (node mode): G's geometries binned in one scan of the map; smem = the sum of their k1_geo_smem_bytes.  The
-// launch runs 32 warps per CTA when smem exceeds k1_big_tables's 56 KB, else 8 (K2 needs that count to walk its lists).
+// K1's geometry form (node mode): G's geometries binned in one scan of the map; smem = the sum of their k1_geo_smem_bytes.
 size_t k1_geo_smem_bytes(int R, int B);
 cudaError_t launch_k1_geo(cudaStream_t st, const K1Geo& G, size_t smem, const float4* map_pts, const float4* qry_pts, const ChunkDesc* chunks,
                           int n_chunks, int F, unsigned long long* fence, const NodePose* poses, uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz);
 
-cudaError_t launch_k3(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt,
-                      const uint32_t* zmin, const uint32_t* zmax, const uint32_t* frame_off, const uint32_t* cnt, uint32_t* dst_start,
-                      uint8_t* status, uint8_t* action, uint32_t* flag_slot, uint32_t* n_flagged, uint32_t* frame_rec_base,
+cudaError_t launch_k3(cudaStream_t st, const SrtParams& P, int F, const K1GeoTables& t, const uint32_t* chunk_range, const uint32_t* frame_off,
+                      uint32_t* dst_start, uint8_t* status, uint8_t* action, uint32_t* flag_slot, uint32_t* n_flagged, uint32_t* frame_rec_base,
                       FlagRec* recs, uint32_t* n_recs, uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list);
 
 // mask modes: Scan Ratio Test + stable scatter of the flagged bins + R-GPF records / queue in one kernel (no k3_srt launch);
-// ch_cnt holds K1's raw per-chunk counts
-cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const ChunkDesc* chunks, const uint32_t* chunk_range, uint32_t n_chunks_map,
-                          const uint16_t* bin_ids, const float4* pts, const NodePose* poses, const uint32_t* ch_cnt, const uint32_t* zmin,
-                          const uint32_t* zmax, const uint32_t* cnt, const uint32_t* frame_off, uint32_t* n_flagged, FlagRec* recs, uint32_t* n_recs,
-                          uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list, float4* out_pts, uint32_t* out_src,
-                          const uint32_t* list_idx, const uint32_t* list_cnt, const SrtSweep* sweep = nullptr /*node mode: a Scan Ratio Test sweep*/,
-                          int k1_warps = 0 /*warps of the K1 launch that wrote the lists; 0: the plain launch's for P.R, P.B*/);
+// t.ch_cnt holds K1's raw per-chunk counts
+cudaError_t launch_k2_srt(cudaStream_t st, const SrtParams& P, int F, const K1GeoTables& t, const ChunkDesc* chunks, const uint32_t* chunk_range,
+                          uint32_t n_chunks_map, const float4* pts, const NodePose* poses, const uint32_t* frame_off, uint32_t* n_flagged, FlagRec* recs,
+                          uint32_t* n_recs, uint32_t rec_capacity, uint32_t* queue, uint32_t* bucket_list, float4* out_pts, uint32_t* out_src,
+                          const uint32_t* list_idx, const uint32_t* list_cnt, int k1_warps /*warps of the K1 launch that wrote the lists*/,
+                          const SrtSweep* sweep /*node mode: a Scan Ratio Test sweep, or null*/);
 
-// flag_slot == null: every bin of dst_start's cloud that has an offset is scattered (cloud mode); otherwise the flagged bins only
-cudaError_t launch_k2(cudaStream_t st, const ChunkDesc* chunks, uint32_t chunk_base, uint32_t n_chunks,
-                      const uint16_t* bin_ids, const float4* pts, const NodePose* poses, const uint32_t* ch_cnt, const uint32_t* dst_start,
-                      const uint32_t* flag_slot, const uint32_t* n_flagged, float4* out_pts, uint32_t* out_src, int B,
-                      const uint32_t* list_idx, const uint32_t* list_cnt, int k1_warps /*warps of the K1 launch that wrote the lists (8 or 32)*/);
+// the stable scatter of one cloud (0 map, 1 query: whose bin ids it reads); flag_slot == null: every bin of dst_start's cloud that
+// has an offset is scattered (cloud mode); otherwise the flagged bins only
+cudaError_t launch_k2(cudaStream_t st, const K1GeoTables& t, int cloud, const ChunkDesc* chunks, uint32_t chunk_base, uint32_t n_chunks,
+                      const float4* pts, const NodePose* poses, const uint32_t* dst_start, const uint32_t* flag_slot, const uint32_t* n_flagged,
+                      float4* out_pts, uint32_t* out_src, const uint32_t* list_idx, const uint32_t* list_cnt, int k1_warps);
 
 // cloud mode: both clouds' stable scatters in one launch (chunk rows: map first, then query)
-cudaError_t launch_k2_both(cudaStream_t st, const ChunkDesc* chunks, uint32_t n_chunks_map, uint32_t n_chunks_qry, const uint32_t* ch_cnt, int B,
-                           const uint16_t* bin_map, const float4* map_pts, const uint32_t* dst_start_map, float4* out_map, uint32_t* src_map,
-                           const uint16_t* bin_qry, const float4* qry_pts, const uint32_t* dst_start_qry, float4* out_qry, uint32_t* src_qry);
+cudaError_t launch_k2_both(cudaStream_t st, const K1GeoTables& t, const ChunkDesc* chunks, uint32_t n_chunks_map, uint32_t n_chunks_qry,
+                           const float4* map_pts, const uint32_t* dst_start_map, float4* out_map, uint32_t* src_map,
+                           const float4* qry_pts, const uint32_t* dst_start_qry, float4* out_qry, uint32_t* src_qry);
 
 int k4_num_launches(bool with_class_c);
 // sorted_pts / sorted_src: K2's output (bins contiguous in source order + source index of every slot).
@@ -78,9 +78,8 @@ cudaError_t launch_k4b(cudaStream_t st, float leaf, int B, int F, const FlagRec*
                        float4* vox_pts, uint32_t* vox_cnt, uint32_t* vox_start, unsigned char* gscratch, int grid);
 
 // node-mode inserts: after K1, the action / flag slot of every (frame, bin) and the query scatter plan of the inserting bins
-cudaError_t launch_ins_plan(cudaStream_t st, const SrtParams& P, int F, const uint32_t* chunk_range, uint32_t* ch_cnt, const uint32_t* zmin,
-                            const uint32_t* zmax, const uint32_t* cnt, uint8_t* action, uint32_t* flag_slot, uint32_t* ins_slot, uint32_t* n_ins,
-                            uint32_t* dst_start);
+cudaError_t launch_ins_plan(cudaStream_t st, const SrtParams& P, int F, const K1GeoTables& t, const uint32_t* chunk_range, uint8_t* action,
+                            uint32_t* flag_slot, uint32_t* ins_slot, uint32_t* n_ins, uint32_t* dst_start);
 // after R-GPF (and K4b): per-frame sizes and offsets ins_off [F+1], then every frame's inserts into out, body -> origin by fwd [F][12]
 cudaError_t launch_ins_assemble(cudaStream_t st, int B, int F, int vox, const uint8_t* action, const uint32_t* flag_slot, uint32_t* frame_rec_base,
                                 const FlagRec* recs, const uint32_t* n_recs, uint32_t rec_capacity, const uint32_t* cnt, const uint32_t* dst_start,

@@ -21,7 +21,7 @@ sm_count = int(sys.argv[3]) if len(sys.argv) > 3 else 132
 p, map_world, poses, qs = bench.load_workload(config, 0, 1, frames)
 R, S = p.num_rings, p.num_sectors
 B = R * S
-NW = 32 if 4 * ((B + 1) + 2 * B) + 8 * ((R + 2) & ~1) > 56 * 1024 else 8       # kernels.cu k1_big_tables
+NW = 32 if 4 * ((B + 1) + 2 * B) + 8 * ((R + 2) & ~1) > 56 * 1024 else 8       # kernels.h k1_warps
 n_map = len(map_world)
 F = len(poses)
 
