@@ -467,14 +467,17 @@ int geometry_tables(erasor_ctx* h, const erasor_geometry_t& x, const GeoTables**
     t->key = x; t->B = (int)Bll;
     std::string terr;
     if (build_bin_tables(p, t->host, terr) != 0) { h->err = terr; return ERASOR_E_INVALID; }
-    if (std::max(k1_smem_bytes(x.num_rings, t->B), k3_smem_bytes(t->B)) > h->smem_optin) {
+    const size_t k1_bytes = k1_smem_bytes(x.num_rings, t->B);
+    size_t k1_max = 0;
+    cudaError_t e;
+    auto fail = [&](const char* what) { h->err = std::string(what) + ": " + cudaGetErrorString(e); return ERASOR_E_CUDA; };
+    if ((e = k1_table_limit(k1_bytes, false, false, h->smem_optin, &k1_max)) != cudaSuccess) return fail("cudaFuncGetAttributes");
+    if (k1_bytes > k1_max || k3_smem_bytes(t->B) > h->smem_optin) {
         h->err = "num_rings*num_sectors too large for the per-CTA shared-memory bin table";
         return ERASOR_E_UNSUPPORTED;
     }
     const HostBinTables& ht = t->host;
     const size_t rb = sizeof(double) * ht.ring_thr.size(), sb = sizeof(SectorBoundary) * ht.sec_pos.size(), gb = sizeof(float) * ht.ring_guard.size();
-    cudaError_t e;
-    auto fail = [&](const char* what) { h->err = std::string(what) + ": " + cudaGetErrorString(e); return ERASOR_E_CUDA; };
     if ((e = t->d_ring.allocate(rb)) != cudaSuccess || (e = t->d_pos.allocate(sb)) != cudaSuccess || (e = t->d_neg.allocate(sb)) != cudaSuccess ||
         (e = t->d_guard.allocate(gb)) != cudaSuccess)
         return fail("cudaMalloc");
@@ -487,6 +490,21 @@ int geometry_tables(erasor_ctx* h, const erasor_geometry_t& x, const GeoTables**
     h->geo_tables.push_back(std::move(t));
     *out = h->geo_tables.back().get();
     return ERASOR_OK;
+}
+
+// Node mode's K1 over tables of table_bytes for the grid of geometry x (geo_form: K1's geometry form, a tune's launch; prof: the
+// profiling build): ERASOR_E_UNSUPPORTED, before anything is enqueued, when the launch cannot take them.  geometry_tables admits a
+// geometry by the K1 of the mask and cloud modes, whose static shared memory is 32 KB smaller, so a geometry may run there and
+// not here.
+int node_k1_fits(erasor_ctx* h, const char* fn, const erasor_geometry_t& x, size_t table_bytes, bool geo_form, bool prof) {
+    size_t lim = 0;
+    const cudaError_t e = geo_form ? k1_geo_table_limit(table_bytes, h->smem_optin, &lim) : k1_table_limit(table_bytes, true, prof, h->smem_optin, &lim);
+    if (e != cudaSuccess) { h->err = std::string("cudaFuncGetAttributes: ") + cudaGetErrorString(e); return ERASOR_E_CUDA; }
+    if (table_bytes <= lim) return ERASOR_OK;
+    h->err = std::string(fn) + ": a " + std::to_string(x.num_rings) + " x " + std::to_string(x.num_sectors) + " polar grid needs " +
+             std::to_string(table_bytes) + " bytes of K1 tables, node mode's K1 takes at most " + std::to_string(lim) +
+             " on this device (the cloud and batch modes run it)";
+    return ERASOR_E_UNSUPPORTED;
 }
 
 // The tables K1 writes for geometry g of a sweep plan: the handle's geometry into k1_own (no plan, or an own plan), any other into
@@ -1374,6 +1392,10 @@ int process_nodes_impl(erasor_handle_t h, const double* poses7, const float* que
         return ERASOR_E_INVALID;
     }
     int rc;
+    if (!sweep || sweep->own) {                                    // (any other sweep plan: process_nodes_sweep checks its launches)
+        const erasor_geometry_t x = own_geometry(h->p);
+        if ((rc = node_k1_fits(h, "node mode", x, k1_smem_bytes(x.num_rings, h->B), false, false))) return rc;
+    }
     if (h->pending && (rc = erasor_wait(h))) return rc;
     const size_t N = h->map->n;
     const double range = voi_max_range > 0.0 ? voi_max_range : h->p.max_range;
@@ -1683,6 +1705,10 @@ int process_nodes_sweep(erasor_handle_t h, const char* fn, const double* poses7,
         plan->launch_smem.back() += bytes;
     }
     if (!plan->own) plan->launch_begin.push_back((int)plan->geo.size());
+    for (size_t l = 0; l < plan->launch_smem.size(); ++l) {      // (a launch beyond 56 KB holds one geometry)
+        const int rc = node_k1_fits(h, fn, plan->geo[plan->launch_begin[l]].t->key, plan->launch_smem[l], true, false);
+        if (rc) return rc;
+    }
     return process_nodes_impl(h, poses7, query_xyzi, query_offsets, n_frames, range, nullptr, nullptr, ptr_kind, async, plan);
 }
 }  // namespace
@@ -2046,6 +2072,7 @@ int erasor_profile_k1(erasor_handle_t h, uint32_t* out, size_t* n, int* warps_pe
     if (warps_per_cta) *warps_per_cta = nw;
     if (!out) return ERASOR_OK;
     if (cap < words) { h->err = "profile buffer too small"; return ERASOR_E_CAPACITY; }
+    if ((rc = node_k1_fits(h, "erasor_profile_k1", own_geometry(h->p), k1_smem_bytes(h->p.num_rings, h->B), false, true))) return rc;
     CK(h->d_k1prof.ensure(sizeof(uint32_t) * std::max<size_t>(words, 1)));
     h->k1_prof = h->d_k1prof.as<uint32_t>();
     rc = run_k1(h, 2);

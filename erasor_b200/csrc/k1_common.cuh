@@ -13,7 +13,9 @@
 namespace erasor {
 
 // cudaFuncSetAttribute costs a few microseconds per call; the dynamic shared-memory ceiling of a kernel only ever has
-// to grow, so remember the largest value set per kernel and skip the call otherwise.
+// to grow, so remember the largest value set per kernel and skip the call otherwise.  A refused ceiling is returned and
+// cleared: left as the thread's last error, the launch check of the next good launch (cudaGetLastError) would report it,
+// on whichever handle made that launch.
 template <class K>
 static cudaError_t ensure_dyn_smem(K kern, size_t bytes) {
     static std::mutex mu;
@@ -24,7 +26,19 @@ static cudaError_t ensure_dyn_smem(K kern, size_t bytes) {
     if (it != seen.end() && it->second >= bytes) return cudaSuccess;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e == cudaSuccess) seen[key] = bytes;
+    else cudaGetLastError();
     return e;
+}
+
+// The most dynamic shared memory kern can launch with on a device whose blocks opt in to smem_optin bytes: the opt-in less
+// the kernel's static shared memory
+template <class K>
+static cudaError_t max_dyn_smem(K kern, size_t smem_optin, size_t* out) {
+    cudaFuncAttributes a;
+    const cudaError_t e = cudaFuncGetAttributes(&a, kern);
+    if (e != cudaSuccess) { cudaGetLastError(); return e; }
+    *out = smem_optin > a.sharedSizeBytes ? smem_optin - a.sharedSizeBytes : 0;
+    return cudaSuccess;
 }
 
 __device__ __forceinline__ float4 ld_stream_f4(const float4* p) {

@@ -155,12 +155,18 @@ k1_geo_bin(const __grid_constant__ K1Geo G, const float4* __restrict__ map_pts, 
 
 size_t k1_geo_smem_bytes(int R, int B) { return (k1_smem_bytes(R, B) + 15) & ~(size_t)15; }
 
+// the kernel launch_k1_geo runs over tables of smem bytes
+static auto k1_geo_kernel(size_t smem) { return k1_warps(smem) == 32 ? k1_geo_bin<1024, 4> : k1_geo_bin<256, 4>; }
+
+cudaError_t k1_geo_table_limit(size_t table_bytes, size_t smem_optin, size_t* limit) {
+    return max_dyn_smem(k1_geo_kernel(table_bytes), smem_optin, limit);
+}
+
 cudaError_t launch_k1_geo(cudaStream_t st, const K1Geo& G, size_t smem, const float4* map_pts, const float4* qry_pts, const ChunkDesc* chunks,
                           int n_chunks, int F, unsigned long long* fence, const NodePose* poses, uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz) {
     if (n_chunks == 0) return cudaSuccess;
-    constexpr int UNROLL = 4;
     const bool big = k1_warps(smem) == 32;
-    auto kern = big ? k1_geo_bin<1024, UNROLL> : k1_geo_bin<256, UNROLL>;
+    auto kern = k1_geo_kernel(smem);
     cudaError_t e = ensure_dyn_smem(kern, smem);
     if (e != cudaSuccess) return e;
     kern<<<n_chunks, big ? 1024 : 256, smem, st>>>(G, map_pts, qry_pts, chunks, F, fence, poses, list_idx, list_cnt, qry_xyz ? 1 : 0);

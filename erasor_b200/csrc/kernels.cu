@@ -224,16 +224,28 @@ size_t k1_smem_bytes(int R, int B) {
     return sizeof(float2) * ((R + 2) & ~1) + sizeof(uint32_t) * ((size_t)(B + 1) + 2 * (size_t)B);
 }
 
+constexpr int kK1Unroll = 4;
+
+// the K1 kernel launch_k1 runs over tables of smem bytes: node mode (prof: its profiling build) or the other modes
+static auto k1_kernel(size_t smem, bool node, bool prof) {
+    constexpr int U = kK1Unroll;
+    const bool big = k1_warps(smem) == 32;
+    return prof ? (big ? k1_rpod_bin<1024, U, true, true> : k1_rpod_bin<256, U, true, true>)
+         : node ? (big ? k1_rpod_bin<1024, U, true> : k1_rpod_bin<256, U, true>)
+                : (big ? k1_rpod_bin<1024, U, false> : k1_rpod_bin<256, U, false>);
+}
+
+cudaError_t k1_table_limit(size_t table_bytes, bool node, bool prof, size_t smem_optin, size_t* limit) {
+    return max_dyn_smem(k1_kernel(table_bytes, node, prof), smem_optin, limit);
+}
+
 cudaError_t launch_k1(cudaStream_t st, const K1GeoTables& t, const float4* map_pts, const float4* qry_pts, const ChunkDesc* chunks, int n_chunks,
                       int F, unsigned long long* fence, const NodePose* poses, uint32_t* list_idx, uint32_t* list_cnt, bool qry_xyz, uint32_t* prof) {
     if (n_chunks == 0) return cudaSuccess;
     if (prof && !poses) return cudaErrorInvalidValue;      // the profiling build covers node mode only
-    constexpr int UNROLL = 4;
     const size_t smem = k1_smem_bytes(t.T.R, t.B);
     const bool big = k1_warps(smem) == 32;
-    auto kern = prof  ? (big ? k1_rpod_bin<1024, UNROLL, true, true> : k1_rpod_bin<256, UNROLL, true, true>)
-              : poses ? (big ? k1_rpod_bin<1024, UNROLL, true> : k1_rpod_bin<256, UNROLL, true>)
-                      : (big ? k1_rpod_bin<1024, UNROLL, false> : k1_rpod_bin<256, UNROLL, false>);
+    auto kern = k1_kernel(smem, poses != nullptr, prof != nullptr);
     cudaError_t e = ensure_dyn_smem(kern, smem);
     if (e != cudaSuccess) return e;
     kern<<<n_chunks, big ? 1024 : 256, smem, st>>>(t.T, map_pts, qry_pts, chunks, t.bin_map, t.bin_qry, t.ch_cnt, t.zmin, t.zmax, t.cnt, t.B, F, fence,

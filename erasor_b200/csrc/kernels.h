@@ -24,6 +24,14 @@ size_t k3_smem_bytes(int B);
 constexpr size_t kK1SmallTables = 56 * 1024;
 inline int k1_warps(size_t table_smem_bytes) { return table_smem_bytes > kK1SmallTables ? 32 : 8; }
 
+// The most table bytes the K1 launch over tables of table_bytes can take on a device whose blocks opt in to smem_optin bytes of
+// shared memory: the opt-in less the static shared memory of the kernel the launch runs.  launch_k1 (node: node mode, prof: its
+// profiling build; else the mask and cloud modes) and launch_k1_geo (table_bytes: the sum of its geometries' k1_geo_smem_bytes).
+// Node mode's 32-warp kernels keep a 32 KB VoI ring in static shared memory, so they reach fewer bins than the other modes
+// (H100, 227 KB opt-in: about 16 560 bins against 19 300).
+cudaError_t k1_table_limit(size_t table_bytes, bool node, bool prof, size_t smem_optin, size_t* limit);
+cudaError_t k1_geo_table_limit(size_t table_bytes, size_t smem_optin, size_t* limit);
+
 cudaError_t launch_init_tables(cudaStream_t st, uint32_t* zmin, uint32_t* zmax, size_t n, uint32_t* cnt, size_t n_cnt, uint32_t* n_recs,
                                uint32_t* frame_rejected, uint32_t* n_flagged, int F, uint32_t* queue);
 

@@ -203,7 +203,9 @@ int    erasor_attach_map(erasor_handle_t h, erasor_map_t m);
  *     (1 also for points outside the node's VoI);
  *   - keep_out (nullable): copy of the map's keep mask after this batch (n_map bytes).
  * query_xyzi / frame_keep / keep_out: host or device (ptr_kind); host buffers should be pinned.  With ERASOR_PTR_QUERY_XYZ
- * in ptr_kind, query_xyzi holds 3 floats per point. */
+ * in ptr_kind, query_xyzi holds 3 floats per point.  Node mode's K1 keeps a 32 KB VoI ring in shared memory next to its bin
+ * tables, so it reaches fewer bins than erasor_create admits (H100: about 16 560 against 19 300 at 100 rings): a larger geometry
+ * runs in the other modes, and node mode, its sweeps and tune refuse it with ERASOR_E_UNSUPPORTED before enqueuing anything. */
 int erasor_process_nodes(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                          double voi_max_range, uint8_t* frame_keep, uint8_t* keep_out, int ptr_kind);
 int erasor_process_nodes_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
@@ -285,7 +287,7 @@ typedef struct {
  * its flagged-bin and rejected-point counts are the union counts of the geometry of setting 0.  With every setting carrying the
  * handle's own geometry the call is erasor_process_nodes_sweep_ex.  Refusals as erasor_process_nodes_sweep_ex, and with
  * erasor_create's codes a geometry it would refuse (num_rings * num_sectors outside [1, 65534], a table it cannot build, tables
- * beyond the device's shared memory); ERASOR_E_INVALID for voi_max_range <= 0 when the settings' max_range differ. */
+ * beyond the device's shared memory), ERASOR_E_UNSUPPORTED for one beyond node mode's K1 (erasor_process_nodes); ERASOR_E_INVALID for voi_max_range <= 0 when the settings' max_range differ. */
 int erasor_process_nodes_tune(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,
                               double voi_max_range, const erasor_tune_setting_t* settings, int n_settings, uint8_t* variant_keep, int ptr_kind);
 int erasor_process_nodes_tune_async(erasor_handle_t h, const double* poses7, const float* query_xyzi, const uint64_t* query_offsets, int n_frames,

@@ -23,10 +23,11 @@ K4B_CAP = (160 * 1024 - 64) // 36                  # 4549
 RGPF_SWITCHES = (128, 256, 512, 1024, 2048, 2560)
 
 
-def k2_window(B: int, with_complement: bool = False) -> int:
-    """kernels.cu k2_smem_plan: slots per window of the SRT + scatter kernel (W = 8 warps, two CTAs per SM in 111 KB)."""
+def k2_window(B: int, with_complement: bool = False, node: bool = False) -> int:
+    """kernels.cu k2_smem_plan: slots per window of the SRT + scatter kernel (W = 8 warps, two CTAs per SM in 111 KB; node mode
+    also stages kK2Stage = 512 VoI entries of 2 bytes per warp)."""
     W = 8
-    fixed = (2 * (B + 2) + 15) & ~15
+    fixed = ((2 * (B + 2) + 15) & ~15) + (2 * W * 512 if node else 0)
     n_slots_max = B + 1 if with_complement else B
     full = 4 * (W + 1) * n_slots_max + fixed
     budget = min(full, 111 * 1024)

@@ -379,9 +379,27 @@ def rgpf_specs():
     return [(2 + i % 16, 5 * i + 2, k, n, None) for i, (k, n) in enumerate(RGPF_KINDS)] + [FAR_COMPACT]
 
 
-def edge_points(p, seed=3):
-    """float32 [n, 4]: points on every ring radius and sector angle and one ulp either side, azimuth +-pi and +-0, the range
-    gate, the origin, z on the height gates and one ulp either side, and a seeded bulk over the whole disc."""
+def pi_sliver(steps: int = 400):
+    """float32 [n, 2]: the sliver between azimuth pi and the sector boundary at PI_CFG (the truncated pi the sector size is defined
+    with): |y| = (pi - PI_CFG) * |x| and up to `steps` float32 steps either side, both signs of y, x = -1, -7.3, -33, -79.9.  They
+    lie inside EPS_THETA of the boundary, so the float64 reference takes either neighbour; the device must equal the oracle."""
+    pts = []
+    for x in (1.0, 7.3, 33.0, 79.9):
+        y0 = F32((math.pi - PI_CFG) * x)
+        ys = [y0]
+        a = b = y0
+        for _ in range(steps):
+            a, b = np.nextafter(a, F32(np.inf)), np.nextafter(b, F32(0))
+            ys += [a, b]
+        for y in ys:
+            pts += [(-x, y), (-x, -y)]
+    return np.array(pts, dtype=np.float64).astype(F32)
+
+
+def edge_points(p, seed=3, sliver=True):
+    """float32 [n, 4]: points on every ring radius and sector angle and one ulp either side, azimuth +-pi and +-0, the truncated-pi
+    sliver (pi_sliver; all inside the bands, sliver=False leaves it out), the range gate, the origin, z on the height gates and
+    one ulp either side, and a seeded bulk over the whole disc."""
     rng = np.random.default_rng(seed)
     R, S, rmax = p.num_rings, p.num_sectors, p.max_range
     rs, ss = rmax / R, 2.0 * PI_CFG / S
@@ -406,7 +424,7 @@ def edge_points(p, seed=3):
             pts.append((r, y))
     for x, y in ((0.0, 0.0), (-0.0, 0.0), (0.0, -0.0), (-0.0, -0.0), (1e-45, 0.0), (-1e-45, 0.0), (0.0, 1e-45), (0.0, -1e-45)):
         pts.append((x, y))                                     # the lower edge of ring 0: the origin
-    xy = np.array(pts, dtype=np.float64).astype(F32)
+    xy = np.concatenate([np.array(pts, dtype=np.float64).astype(F32)] + ([pi_sliver()] if sliver else []))
     out = [np.stack([xy[:, 0], xy[:, 1], np.full(len(xy), zmid)], 1)]
     # z on the gates: float32 nearest and one ulp either side, at points well inside a bin
     gz = []
@@ -739,7 +757,7 @@ def test_polar_reference_matches_the_numpy_restatement():
     import np_restatement as NR
     for name in ("seq_05", "seq_00", "synthetic_40x360"):
         p = P.preset(name)
-        pts = edge_points(p)
+        pts = edge_points(p, sliver=False)
         b, cand = polar(p, pts)
         nb, _ = NR.bin_of_points(p, pts)
         clear = (cand == cand[:, :1]).all(1)
@@ -1056,7 +1074,7 @@ def _tables_equal(a, b):
 @pytest.mark.gpu
 @needs_gpu
 @pytest.mark.parametrize("preset", ["seq_05", "seq_00", "exact_gates"])
-def test_binning_edges(capi, preset):
+def test_binning_edges(capi, oracle_mod, preset):
     if preset == "exact_gates":   # gates and radii that float32 represents exactly, so that z == max_h and r == max_range are hit
         p = P.preset("seq_05").replace(min_h=-1.25, max_h=3.0, max_range=64.0, num_rings=16, num_sectors=64)
     else:
@@ -1073,6 +1091,11 @@ def test_binning_edges(capi, preset):
     assert np.array_equal(bm, bq), "the map and the query path bin the same point differently"
     amb = ~(cand == cand[:, :1]).all(1)
     assert np.array_equal(bm[~amb], exact[~amb])
+    # inside the bands (the truncated-pi sliver among them) the reference takes either neighbour: the oracle decides
+    o = oracle_mod.Oracle(p)
+    o.run(pts, pts[:0])
+    assert np.array_equal(bm, o.bin_of_point(0)), (preset, int((bm != o.bin_of_point(0)).sum()))
+    o.close()
     print(f"{preset}: {len(pts)} points, {int(amb.sum())} within a band, {int((bm[amb] != exact[amb]).sum())} of them in the other neighbour")
     # the node path (fetch_VoI + K1 at the identity pose) builds the same tables, and the mask mode keeps the same points
     keep_cloud, _ = h.get_static_mask()

@@ -28,16 +28,32 @@ def _host_bins(p, pts):
     return bins, st, qe.value, eps.value
 
 
-@pytest.mark.parametrize("name", list(P.PRESETS))
+# the edges of the legal geometry range (seq_05 otherwise): one ring or sector, 19 000 of either, a grid past node mode's K1
+# limit, a tiny and a huge max_range, a height window with no float32 inside it
+GEOMETRY_EDGES = {
+    "1x1": dict(num_rings=1, num_sectors=1), "1x2": dict(num_rings=1, num_sectors=2), "2x1": dict(num_rings=2, num_sectors=1),
+    "3x3": dict(num_rings=3, num_sectors=3), "7x9": dict(num_rings=7, num_sectors=9), "1x19000": dict(num_rings=1, num_sectors=19000),
+    "19000x1": dict(num_rings=19000, num_sectors=1), "120x160": dict(num_rings=120, num_sectors=160),
+    "range0.5": dict(max_range=0.5), "range5000": dict(max_range=5000.0, num_rings=20),
+    "z_one_ulp": dict(min_h=0.0, max_h=float(np.nextafter(np.float32(0), np.float32(1)))),
+}
+
+
+@pytest.mark.parametrize("name", list(P.PRESETS) + list(GEOMETRY_EDGES))
 def test_exact_thresholds_match_oracle(oracle_mod, name):
-    p = P.preset(name).replace(skip_voxelize=1)
+    from test_erasor_float64_reference import pi_sliver
+    p = (P.preset(name) if name in P.PRESETS else P.preset("seq_05").replace(**GEOMETRY_EDGES[name])).replace(skip_voxelize=1)
     pts = synth.adversarial_points(p, n_random=400000, seed=21)
+    s = pi_sliver()
+    z = np.float32(0.5 * (p.min_h + p.max_h))
+    pts = np.concatenate([pts, np.stack([s[:, 0], s[:, 1], np.full(len(s), z), np.ones(len(s))], 1).astype(np.float32)])
     b, st, qerr, eps = _host_bins(p, pts)
     o = oracle_mod.Oracle(p)
     o.run(pts, pts[:0])
     assert np.array_equal(b, o.bin_of_point(0))
     assert st[1] == 0, "ambiguous sector decisions"
-    assert st[2] > 0, "the adversarial set must exercise the exact sector path"
+    if name in P.PRESETS:
+        assert st[2] > 0, "the adversarial set must exercise the exact sector path"
     assert qerr < 0.5 * eps, f"float sector coordinate error {qerr} too close to the guard band {eps}"
 
 
